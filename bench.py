@@ -1,9 +1,9 @@
-"""bench.py -- images/sec of the PerspectiveFields inference hot path (BASELINE.json metric) on N B200s.
+"""bench.py -- images/sec of the PerspectiveFields inference hot path on N H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--config C2|C3|C4|C5|P360]     # this repo's CUDA path
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--config C2|C3|C4|C5|P360] [--dump-outputs DIR]   # this repo's CUDA path
     python bench.py --impl reference [...]                                              # the reference algorithm on the host CPU cores
 
-A step is one pass of the hot path over one batch of synthetic input.  Configurations (BASELINE.json `configs`, SURVEY.md 8d):
+A step is one pass of the hot path over one batch of synthetic input.  Configurations (SURVEY.md 8d):
   C2 (default, the configuration the metric is quoted on): ``Paramnet-360Cities-edina-centered``, 32 x 640x480 per GPU
   C3: ``Paramnet-360Cities-edina-uncentered`` (principal-point head), 64 x 512x512
   C4: ``PersNet_Paramnet-GSV-uncentered``, 32 x 640x480 per GPU (256 over 8 GPUs) -- the multi-GPU configuration
@@ -21,6 +21,11 @@ Prints ONE JSON line on rank 0:  value = whole-job images/s with inputs resident
 e2e = the same through the public API from host numpy arrays incl. H2D of the inputs and D2H of every returned tensor,
 roofline = achieved algorithmic FLOP/s of the dominant kernel measured with CUDA events vs the measured bf16 peak,
 roofline_post = achieved GB/s of the HBM-bound write-out stage, cpu_baseline = the oracle port of the reference timed on the host.
+
+--dump-outputs DIR: after the timed steps, the arrays the last timed step returned (pred_gravity, pred_latitude, gravity_original,
+latitude_original, params) are written as DIR/<name>.npy in float32.  Inputs and weights are seeded, so two builds run with the
+same arguments can be compared output for output.  The files stay below 64 MB in all: arrays above 1 MiB then keep the same
+fraction of their flattened elements, a fixed seeded sample (sorted positions drawn with numpy's default_rng(0)).
 """
 import argparse
 import ctypes
@@ -35,7 +40,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
-METRIC = "images/sec at 640x480 (Paramnet-360Cities-edina), 1/2/4/8xB200 vs ref CPU"
+METRIC = "images/sec at 640x480 (Paramnet-360Cities-edina), H100 vs ref CPU"
 CONFIGS = {
     "C2": dict(version="Paramnet-360Cities-edina-centered", batch=32, sizes=[(480, 640)],
                workload="C2: Paramnet-360Cities-edina-centered, batch=32 640x480 synthetic uint8 BGR per GPU, seeded synthetic checkpoint"),
@@ -62,11 +67,12 @@ def parse():
     ap.add_argument("--micro-batch", type=int, default=32, help="images per micro-batch of the gather-inclusive multi-GPU leg")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-profile-passes", action="store_true", help="skip the roofline / per-kernel passes (A/B timing runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs to DIR/<name>.npy (float32, <= 64 MB in all)")
     return ap.parse_args()
 
 
 class ClockSampler:
-    """SM clock / throttle-reason samples DURING the timed region (B200_PROFILING.md recipe), read through NVML from the
+    """SM clock / throttle-reason samples DURING the timed region, read through NVML from the
     main thread once all K steps have been enqueued, repeatedly until the end event completes (the GPU is busy with the queued
     steps; sampling between the enqueues starved the GPU on boxes where one NVML call takes ~40 ms).
     A concurrent poller -- an `nvidia-smi -lms` child or an NVML thread -- measurably slowed the launches it was observing."""
@@ -113,7 +119,7 @@ class ClockSampler:
 
 def physical_cores():
     """Threads for the CPU reference: one per physical core (torch's own default when OMP_NUM_THREADS is unset).  Using every
-    hyper-thread (128 on this pool's hosts) makes ATen's CPU kernels ~10x SLOWER, which would only flatter the GPU number."""
+    hyper-thread makes ATen's CPU kernels much SLOWER, which would only flatter the GPU number."""
     try:
         import psutil
         n = psutil.cpu_count(logical=False)
@@ -166,12 +172,12 @@ def cpu_reference_images_per_s(cfg, n_images, repeats):
 def workload_config(args, cfg, B, world):
     return {"workload": cfg["workload"], "global_batch": B * world,
             "parallelism": f"dp{world} (independent images, no data-path collective)",
-            "l2": "256 MiB flush write between timed steps; per-step working set (activations of the batch) >> 126 MB L2"}
+            "l2": "256 MiB flush write between timed steps; per-step working set (activations of the batch) >> 50 MB L2"}
 
 
 def run_reference(args, rank):
     """--impl reference: the reference's CPU implementation of the path (the oracle port: the reference is pure Python
-    and /root/reference does not exist on the GPU box) on all physical host cores; each step = inference_batch of a bounded
+    and needs no checkout of it) on all physical host cores; each step = inference_batch of a bounded
     sample of the workload (`cpu_baseline.sample`); `config` is this repo's arm's."""
     if rank != 0:
         return
@@ -225,7 +231,7 @@ class Bench:
             k, v = kv.split("=")
             self.model.set_option(k, int(v))
         self.L = _native.lib()
-        self.flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > L2 (126 MB)
+        self.flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > L2 (50 MB)
 
     def barrier(self):
         if self.world > 1:
@@ -238,9 +244,9 @@ class Bench:
             self.dist.all_reduce(t, op=self.dist.ReduceOp.MAX)
         return t.item()
 
-    def resident_leg(self, imgs, steps, warmup, sampler=None, trace=False):
+    def resident_leg(self, imgs, steps, warmup, sampler=None, keep_last=False):
         """K steps with the inputs already in HBM: flush L2, pf_forward on the staged blob.  Returns (ms of the timed region on this
-        rank, kernel launches, host enqueue ms per step)."""
+        rank, kernel launches, host enqueue ms per step); keep_last: the last step's outputs stay in self.last_out."""
         torch = self.torch
         B = len(imgs)
         heights, widths = [im.shape[0] for im in imgs], [im.shape[1] for im in imgs]
@@ -268,6 +274,7 @@ class Bench:
             while not e1.query() and len(sampler.rows) < 64:
                 sampler.sample()
         self.barrier()
+        self.last_out = out if keep_last else None
         del out
         return e0.elapsed_time(e1), self.L.pf_kernel_launch_count() - l0, host_ms, (blob, offsets, heights, widths)
 
@@ -359,20 +366,31 @@ class Bench:
         return max(f0.elapsed_time(f1), wall_ms), h2d_bytes, d2h_bytes
 
 
+def dump_outputs(out, d, limit=60 << 20):
+    """The tensors of one forward's result dict as d/<name>.npy (float32).  Arrays of up to 1 MiB are written whole; when the
+    rest exceed what is left of `limit` bytes, each of them keeps the same fraction of its flattened elements, a seeded sample."""
+    import numpy as np
+    import torch
+
+    arrays = {k: v for k, v in out.items() if torch.is_tensor(v)}
+    small = sum(v.numel() * 4 for v in arrays.values() if v.numel() * 4 <= 1 << 20)
+    big = sum(v.numel() * 4 for v in arrays.values() if v.numel() * 4 > 1 << 20)
+    os.makedirs(d, exist_ok=True)
+    rng = np.random.default_rng(0)
+    for k in sorted(arrays):
+        a = arrays[k].float().cpu().numpy()
+        if a.nbytes > 1 << 20 and big > limit - small:
+            a = a.reshape(-1)
+            a = a[np.sort(rng.choice(a.size, a.size * (limit - small) // big, replace=False))]
+        np.save(os.path.join(d, k + ".npy"), np.ascontiguousarray(a, np.float32))
+
+
 def roofline_objects(args, B, prof, prof_ms, ms, per_kernel, heights, widths, peaks, write_peak=None):
-    peak_tf = peaks.get("bf16_tflops_sustained") or 1400.0
-    peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (cuBLAS bf16, kernel timed inside a long step)" if peaks else "fallback 1.4 PFLOP/s sustained (B200_PROFILING.md)"
+    peak_tf = peaks.get("bf16_tflops_sustained") or 989.0
+    peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (cuBLAS bf16, kernel timed inside a long step)" if peaks else "H100 SXM data sheet: 989 TFLOP/s dense bf16 (not measured)"
     traffic, traffic_src = None, None
-    for name in ("r02_ncu_dominant_kernel.json", "r01_ncu_dominant_kernel.json"):
-        try:   # DRAM bytes per launch of the dominant kernel from the committed `ncu --set full` capture (profiles/)
-            with open(os.path.join(ROOT, "profiles", name)) as f:
-                t = json.load(f)
-            traffic, traffic_src = t["dram_bytes_per_launch"], t["source"]
-            break
-        except Exception:
-            pass
-    names = {5: "gemm_tma_kernel<BN,GEMM> (persistent TMA -> tcgen05.mma kind::f16 -> TMEM, bf16x3 split precision, 128 x BN tiles: every Linear / 1x1 / patchified conv)",
-             6: "gemm_tma_kernel<BN,HALO> (persistent TMA halo -> tcgen05.mma kind::f16 -> TMEM, bf16x3 split precision, 3x3 conv, 16x8-pixel x BN tiles)"}
+    names = {5: "gemm_tma_kernel<BN,GEMM> (persistent TMA -> wgmma, bf16x3 split precision, 128 x BN tiles: every Linear / 1x1 / patchified conv)",
+             6: "gemm_tma_kernel<BN,HALO> (persistent TMA halo -> wgmma, bf16x3 split precision, 3x3 conv, 16x8-pixel x BN tiles)"}
     cfgs = [c for c in range(7) if prof[3 * c + 2] > 0]
     gemm_ms = sum(prof[3 * c] for c in cfgs)
     gemm_flops = sum(prof[3 * c + 1] for c in cfgs)
@@ -404,7 +422,7 @@ def post_roofline(per_kernel, heights, widths, peaks, write_peak=None):
     if not pk or pk["ms_per_step"] <= 0:
         return None
     post_bytes = sum(4 * (3 * 320 * 320 + 3 * int(h_) * int(w_)) for h_, w_ in zip(heights, widths))
-    hbm_peak = peaks.get("hbm_gbs") or 6500.0
+    hbm_peak = peaks.get("hbm_gbs") or 3350.0
     gbps = post_bytes / (pk["ms_per_step"] / 1000.0) / 1e9
     r = {"bound": "hbm", "kernel": "postprocess_kernel (bilinear resample to (H,W) + F.normalize / asin, all images of the batch in one launch)",
          "achieved": gbps, "peak": hbm_peak, "unit": "GB/s", "frac": gbps / hbm_peak, "bytes_per_step": post_bytes,
@@ -431,7 +449,7 @@ def load_peaks():
 def measured_write_peak(dev):
     """Pure-WRITE bandwidth of this GPU's HBM (GB/s), measured live the way MEASURED_PEAKS.json measures the copy peak: the better
     of torch ``fill_`` and a 16-byte streaming-store kernel (pf_op_fill_stream) over 1 GiB, best of 4 each, CUDA events.  The copy peak counts read + write bytes; a kernel that only writes (the
-    post-process / camera-field write-out) cannot exceed this number, which on this pool's B200s is well below half the copy peak."""
+    post-process / camera-field write-out) cannot exceed this number."""
     import torch
 
     from perspectivefields_b200 import _native
@@ -489,7 +507,7 @@ def camera_fields_roofline(dev, heights, widths, peaks, steps, write_peak=None):
     torch.cuda.synchronize(dev)
     ms = e0.elapsed_time(e1) / reps
     nbytes = 12 * sum(int(h) * int(w) for h, w in zip(heights, widths))
-    hbm_peak = peaks.get("hbm_gbs") or 6500.0
+    hbm_peak = peaks.get("hbm_gbs") or 3350.0
     r = {"kernel": "camera_fields_kernel", "ms": ms, "bytes": nbytes, "achieved": nbytes / ms / 1e6, "peak": hbm_peak, "unit": "GB/s",
          "frac": nbytes / ms / 1e6 / hbm_peak, "timing": how}
     if write_peak:
@@ -546,7 +564,7 @@ def gather_leg(b, imgs_rank, steps, warmup, micro_batch):
     if rank == 0:
         out.update({"bytes_received_per_step_rank0": moved / steps, "achieved_gbs_into_rank0": moved / (ms / 1000.0) / 1e9,
                     "results_on_rank0": n_back,
-                    "note": "achieved_gbs is bytes / whole step time (the transfers overlap the forward; NVLink 5 peak is 900 GB/s per direction)"})
+                    "note": "achieved_gbs is bytes / whole step time (the transfers overlap the forward; H100 SXM NVLink peak is 450 GB/s per direction)"})
     return out
 
 
@@ -581,8 +599,11 @@ def main():
     gc.disable()
 
     # ---------------- leg 1: inputs resident in HBM ("value") ------------------------------------------------
-    ms, launches, host_ms, staged = b.resident_leg(imgs, args.steps, args.warmup, sampler)
+    ms, launches, host_ms, staged = b.resident_leg(imgs, args.steps, args.warmup, sampler, keep_last=bool(args.dump_outputs))
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(b.last_out, args.dump_outputs)
+    b.last_out = None
     ms_max = b.max_over_ranks(ms)
     value = world * B * args.steps / (ms_max / 1000.0)
     roofline = roofline_post = None

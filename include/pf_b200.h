@@ -1,4 +1,4 @@
-/* pf_b200.h -- C ABI of the B200-native PerspectiveFields inference engine (libpf_b200.so).
+/* pf_b200.h -- C ABI of the H100-native (sm_90a) PerspectiveFields inference engine (libpf_b200.so).
  *
  * The reference (jinlinyi/PerspectiveFields) is pure Python and has no FFI boundary of its own: the boundary it
  * offers is the class perspective2d.PerspectiveFields (perspective2d/perspectivefields.py:121-272).  This header is
@@ -93,7 +93,7 @@ int pf_forward(pf_handle h, const pf_batch* batch, void* workspace, int64_t work
 
 /* Per-launch timing of the GEMM engine with CUDA events on the launch stream (bench.py roofline leg).  pf_profile_read
  * fills out21[cfg*3 + {0,1,2}] = {milliseconds, algorithmic FLOPs (2*M*N*K), launches} per engine configuration (slots 0-4 are
- * unused since ABI 2 -- the earlier HMMA / register-staged engines were removed; 5: TMA+tcgen05 GEMM mode, 6: TMA+tcgen05 halo
+ * unused since ABI 2 -- the earlier HMMA / register-staged engines were removed; 5: TMA+wgmma GEMM mode, 6: TMA+wgmma halo
  * 3x3 mode) accumulated since the previous read; synchronise the stream first. */
 int pf_profile_enable(pf_handle h, int on /* 0 off, 1 on, n > 1: on + pre-create events for n GEMM launches */);
 int pf_profile_read(pf_handle h, double* out21);
@@ -103,20 +103,16 @@ int pf_profile_read(pf_handle h, double* out21);
 int pf_profile_kernels_enable(pf_handle h, int max_launches);
 int pf_profile_kernels_read(pf_handle h, char* buf, int cap);
 
-/* Engine options (all default 1 unless noted; the whole graph runs on the persistent TMA -> tcgen05 -> TMEM engine with pre-split
+/* Engine options (all default 1 unless noted; the whole graph runs on the persistent TMA -> wgmma engine with pre-split
  * bf16 hi/lo activations, gemm_tma.cuh):
- * "attn_tc": attention core on tcgen05 / TMEM (attention_tc.cuh: S = Q K^T into TMEM, softmax one thread per row from TMEM, P V as a
- *   second MMA with V consumed MN-major); 0 = the warp-level mma.sync kernel (attention_mma.cuh).
- * "attn_mma": (with "attn_tc" = 0) mma.sync attention core instead of the exact-softmax CUDA-core kernel.
- * "attn_split": q / kv leave their GEMMs as split planes (0 = fp32, split inside the attention kernel).
+ * "attn_mma": (with "attn_split" = 0) mma.sync attention core instead of the exact-softmax CUDA-core kernel.
+ * "attn_split": q / kv leave their GEMMs as split planes for the mma.sync attention core (attention_mma.cuh); 0 = fp32.
  * "stem_tc": the two 7x7 stems as patch gather + TMA GEMM instead of fp32 direct convolution.
  * "phase_conv1": conv_fuse_conv1 composed with the x2 bilinear upsample in front of it (four output phases on the 160x160 grid
  *   + an exact fp32 border-ring kernel); 0 = materialise the upsampled tensor, conv at 320x320.
- * "pair": GEMM-mode launches with at least one 256 x BN tile per TPC run on CTA pairs (gemm2_tma.cuh, tcgen05.mma.cta_group::2);
- *   0 = every launch on the single-CTA kernel.
  * "pdl": programmatic dependent launch of the graph's kernels (a kernel's prologue overlaps its predecessor's tail).
- * "fork" (default 0): the spatial-reduction branch of a MiT block on a second stream beside the q projection (measured 1 % slower).
- * "dw_ln" (default 0): ConvNeXt depthwise 7x7 fused with the LayerNorm behind it (measured slower: profiles/r02_notes.md).
+ * "fork" (default 0): the spatial-reduction branch of a MiT block on a second stream beside the q projection (slower in the forward graph: the two streams' persistent kernels compete for SMs).
+ * "dw_ln" (default 0): ConvNeXt depthwise 7x7 fused with the LayerNorm behind it (slower than the separate kernels).
  * "decode_only" (default 0; classification heads, SURVEY.md 8f-3): the 73 / 180 logits are never written -- the 1x1 prediction
  *   conv, argmax and bin decode (gravity_head.py:243-244 + utils/utils.py:114-130, latitude_head.py:205-208 + utils.py:148-162)
  *   run in one kernel and pred_gravity / pred_latitude receive the decoded fields [n,2,320,320] / [n,1,320,320] (degrees). */
@@ -172,7 +168,7 @@ int pf_jpeg_decode_batch(pf_jpeg_handle j, int n, const uint8_t* const* data, co
 
 /* ---- single-operator entry points (unit tests; the same kernels pf_forward launches) -------------------- */
 
-/* Conv / linear on NHWC fp32 on the TMA -> tcgen05 engine, bf16x3 split precision (the input is split into hi/lo planes first,
+/* Conv / linear on NHWC fp32 on the TMA -> wgmma engine, bf16x3 split precision (the input is split into hi/lo planes first,
  * as a producer kernel of the forward graph would; 3x3/s1/p1 with Cin % 64 == 0 -> halo mode, 1x1 -> GEMM mode, else patch gather).  x: [B,H,W,Cin]; whi/wlo: bf16 [N][KH*KW*Cin]
  * ordered (ky,kx,ci); bias: [N] or NULL; res: [B,OH,OW,N] or NULL; y: [B,OH,OW,N].
  * y = act(conv(relu_in?(x)) + bias) (+ relu_res?(res));  act: 0 none, 1 ReLU, 2 GELU. */
@@ -182,7 +178,7 @@ int pf_op_conv_gemm(const float* x, int B, int H, int W, int Cin, const void* wh
 int pf_op_layernorm(const float* x, float* y, int64_t rows, int C, const float* w, const float* b, float eps, void* stream);
 int pf_op_attention(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream);      /* CUDA-core fp32 */
 int pf_op_attention_mma(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream);  /* warp-level mma.sync, bf16x3 */
-int pf_op_attention_tc(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream);   /* tcgen05 / TMEM, bf16x3 (default) */
+int pf_op_attention_tc(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream);   /* q / kv split into bf16 hi/lo planes first, then the mma.sync core as the forward graph runs it */
 int pf_op_dwconv3x3_gelu(const float* x, float* y, int B, int H, int W, int C, const float* w9c, const float* bias, void* stream);
 int pf_op_dwconv7x7(const float* x, float* y, int B, int H, int W, int C, const float* w49c, const float* bias, void* stream);
 int pf_op_upsample2x(const float* x, float* y, int B, int H, int W, int C, void* stream);

@@ -2,7 +2,7 @@
 
 This package is a plain PyTorch-CPU / numpy restatement of the reference algorithm
 (``perspective2d.PerspectiveFields.inference{,_batch}``, reference file:line cited per function).
-It exists so that the CUDA product path can be checked on a box where ``/root/reference`` is not
+It exists so that the CUDA product path can be checked on a box where the reference is not
 present.  Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s ``cpu_baseline`` /
 ``--impl reference`` legs may import it; the product package ``perspectivefields_b200`` never does
 and fails loudly when its CUDA library is missing.

@@ -1,4 +1,4 @@
-"""Import-time stubs that let the UNMODIFIED reference (``/root/reference``) be imported
+"""Import-time stubs that let the UNMODIFIED reference (a checkout named by ``PF_REFERENCE_ROOT``) be imported
 in this container.  TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).
 
 The reference needs ``timm``, ``yacs``, ``omegaconf``, ``matplotlib``, ``equilib`` and
@@ -12,19 +12,18 @@ The reference needs ``timm``, ``yacs``, ``omegaconf``, ``matplotlib``, ``equilib
 * ``matplotlib*``, ``equilib`` (``__version__ == "0.3.0"`` is asserted in utils/panocam.py:8),
   ``imageio``                      -> empty modules
 
-Nothing here is imported by the product package.  ``/root/reference`` does not exist on the
-GPU box, so only the golden generator (tests/golden/make_golden.py) and the CPU-side
-"oracle == reference" tests (skipped when the reference is absent) call ``load_reference``.
+Nothing here is imported by the product package, and no test needs the reference: only the golden
+generators (tests/golden/make_golden*.py) call ``load_reference``.
 """
 import os
 import sys
 import types
 
-REFERENCE_ROOT = os.environ.get("PF_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("PF_REFERENCE_ROOT", "")
 
 
 def reference_available():
-    return os.path.isdir(os.path.join(REFERENCE_ROOT, "perspective2d"))
+    return bool(REFERENCE_ROOT) and os.path.isdir(os.path.join(REFERENCE_ROOT, "perspective2d"))
 
 
 def _module(name, **attrs):
@@ -124,7 +123,7 @@ def _install_stubs():
 def load_reference():
     """Return the reference's ``perspective2d`` package (imported unmodified)."""
     if not reference_available():
-        raise RuntimeError(f"reference tree not found at {REFERENCE_ROOT}")
+        raise RuntimeError(f"reference tree not found at {REFERENCE_ROOT!r} (set PF_REFERENCE_ROOT)")
     _install_stubs()
     if REFERENCE_ROOT not in sys.path:
         sys.path.insert(0, REFERENCE_ROOT)

@@ -1,4 +1,4 @@
-"""perspectivefields_b200 -- B200-native (sm_100a CUDA) implementation of the PerspectiveFields inference path.
+"""perspectivefields_b200 -- H100-native (sm_90a CUDA) implementation of the PerspectiveFields inference path.
 
     from perspectivefields_b200 import PerspectiveFields
     model = PerspectiveFields("Paramnet-360Cities-edina-centered").eval().cuda()

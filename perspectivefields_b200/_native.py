@@ -1,7 +1,7 @@
 """ctypes binding of libpf_b200.so (C ABI declared in include/pf_b200.h) and its in-tree build recipe.
 
 There is no CPU fallback: importing this module works without a GPU (so the ABI can be inspected), but every
-compute entry point needs the CUDA library and a B200.
+compute entry point needs the CUDA library and an H100 (sm_90a).
 """
 import ctypes
 import os
@@ -16,7 +16,7 @@ HEADER = os.path.join(ROOT, "include", "pf_b200.h")
 PF_F32, PF_BF16 = 0, 1
 PF_PARAM_NONE, PF_PARAM_CENTERED, PF_PARAM_UNCENTERED = 0, 1, 2
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared", "-ldl"]
 
 
@@ -55,7 +55,7 @@ def needs_build():
 
 
 def build(force=False, verbose=False):
-    """Compile csrc/pf_b200.cu for sm_100a into libpf_b200.so next to this file (nvcc cross-compiles without a GPU)."""
+    """Compile csrc/pf_b200.cu for sm_90a into libpf_b200.so next to this file (nvcc cross-compiles without a GPU)."""
     if not force and not needs_build():
         return LIB_PATH
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")

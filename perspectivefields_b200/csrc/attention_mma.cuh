@@ -207,9 +207,9 @@ inline cudaError_t attention_mma_launch(const float* q, const float* kv, float* 
                                         SplitT qs = SplitT(), SplitT kvs = SplitT()) {
   if ((qs.hi != nullptr) != (kvs.hi != nullptr) || (qs.hi && (qs.ld != C || kvs.ld != 2 * C))) return cudaErrorInvalidValue;
   const int tiles = cdiv(N, kAmQTile);
-  // passes per block: the grid should be about one resident wave (148 SMs x 3 blocks); the K/V staging of a block is
+  // passes per block: the grid should be about one resident wave (132 SMs x 3 blocks); the K/V staging of a block is
   // amortised over tpb * 64 queries
-  int tpb = (tiles * heads * B) / 400;
+  int tpb = (tiles * heads * B) / 396;
   tpb = tpb < 1 ? 1 : (tpb > tiles ? tiles : tpb);
   dim3 grid(cdiv(tiles, tpb), heads, B);
   if (qs.hi) return launch_pdl(attention_mma_kernel<true>, grid, dim3(kAmThreads), kAmSmem, st, nullptr, nullptr, qs.hi, qs.lo, kvs.hi, kvs.lo, out, sp.hi, sp.lo, N, C, tpb);

@@ -1,4 +1,4 @@
-// Common device helpers for the sm_100a kernels of the PerspectiveFields inference path.
+// Common device helpers for the sm_90a kernels of the PerspectiveFields inference path.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -13,7 +13,7 @@ __host__ __device__ inline long long cdivl(long long a, long long b) { return (a
 
 // ---------------------------------------------------------------- programmatic dependent launch (PDL)
 // The forward graph is ~450 dependent launches of 10-60 us kernels.  Kernels launched with
-// cudaLaunchAttributeProgrammaticStreamSerialization may begin (block scheduling, prologue: barrier init, TMEM allocation,
+// cudaLaunchAttributeProgrammaticStreamSerialization may begin (block scheduling, prologue: barrier init,
 // descriptor prefetch) while the previous kernel of the stream is still draining; pdl_wait() (griddepcontrol.wait) then blocks
 // until that kernel has completed and its memory is visible -- every kernel launched that way calls it before its first global
 // access.  It is a no-op for ordinary launches.  pdl_launch() lets the NEXT kernel's launch proceed as early as possible.
@@ -49,7 +49,7 @@ __device__ __forceinline__ void split_bf16x2(float a, float b, uint32_t& hi, uin
 }
 
 // A "split tensor": the two bf16 planes of an fp32 activation tensor, NHWC with `ld` channels per pixel.  GEMM inputs are
-// always stored this way by their producer so that the tcgen05 kernels can TMA-load them without any conversion.
+// always stored this way by their producer so that the wgmma kernels can TMA-load them without any conversion.
 struct SplitT {
   __nv_bfloat16* hi = nullptr;
   __nv_bfloat16* lo = nullptr;

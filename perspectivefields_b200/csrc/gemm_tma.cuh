@@ -1,20 +1,19 @@
-// TMA -> tcgen05 -> TMEM engine: persistent, warp-specialised, epilogue overlapped with the next tile's main loop.
+// TMA -> wgmma engine: persistent, warp-specialised, TMA producer running ahead of the MMA warpgroups through an mbarrier ring.
 //
 // All GEMM operands arrive PRE-SPLIT: activations as two bf16 planes (hi = bf16(x), lo = bf16(x - hi)) written by the
 // producing kernel's epilogue, weights as hi/lo planes split at load time.  Each product costs three bf16 MMAs
-// (lo*hi + hi*lo + hi*hi, fp32 accumulation in TMEM) -- see DESIGN.md "precision".  Nothing is converted here: tiles go
-// HBM/L2 --TMA--> swizzled shared memory --tcgen05.mma--> TMEM --tcgen05.ld--> fused epilogue --> HBM.
+// (lo*hi + hi*lo + hi*hi, fp32 accumulation) -- see DESIGN.md "precision".  Nothing is converted here: tiles go
+// HBM/L2 --TMA--> swizzled shared memory --wgmma--> registers --> fused epilogue --> HBM.
 //
-//   MODE_GEMM : C[M,N] = A[M,K] W[N,K]^T.     A tiles 128 x 32 (SWIZZLE_64B) by 2-D TMA, K step 32, NS-stage ring.
+//   MODE_GEMM : C[M,N] = A[M,K] W[N,K]^T.     A tiles 128 x KB by 2-D TMA, NS-stage ring.
 //   MODE_HALO : 3x3 / stride 1 / pad 1 convolution, 16 x 8 pixel tiles.  One 4-D TMA per 64-channel chunk loads the
 //               18 x 10 input halo (OOB = zero padding) as [180 pixels][128 B] SWIZZLE_128B; the A operand of filter tap
-//               (ky,kx) is a shifted view of it (start + (ky*10+kx)*128 B, SBO = 1280 B; semantics probed by
-//               tools/tc_probe.cu).  Weights stream through an NS-stage ring of 32-wide K steps (2 per tap and chunk).
+//               (ky,kx) is a shifted view of it (start + (ky*10+kx)*128 B, SBO = 1280 B).  Weights stream through an NS-stage
+//               ring of KB-wide K steps.
 //
-//   warp 0 : TMA producer (B ring; in MODE_GEMM also A)      warp 2 : TMEM allocator, MODE_HALO halo (A) producer
-//   warp 1 : MMA issuer (one elected lane)                   warps 4-11: epilogue (TMEM lane quarter = warp % 4, two warps per
-//                                                                        quarter draining alternate 32-column chunks)
-//   two TMEM accumulators (2 x BN columns): the epilogue of tile i runs under the main loop of tile i+1.
+//   warpgroup 0 : warp 0 = TMA producer (B ring; in MODE_GEMM also A), warp 1 = MODE_HALO halo (A) producer
+//   warpgroups 1, 2 : MMA + epilogue, rows 0-63 and 64-127 of the 128 x BN tile (wgmma M = 64 per warpgroup); each
+//                     accumulates its 64 x BN block in registers and runs the fused epilogue on it.
 //
 // Epilogue (fused): + bias | border-class bias, ReLU / GELU, layer scale, + relu?(residual), + second residual; writes the
 // fp32 tensor and/or the bf16 hi/lo planes (optionally rectified) that the next GEMM will TMA-load.
@@ -25,11 +24,8 @@
 
 namespace pf {
 
-#ifndef PF_EPI_PAIR_STORE
-#define PF_EPI_PAIR_STORE 1      // halo-mode epilogue: lane pairs write 32 contiguous bytes per store (0 = 16 bytes per lane and row)
-#endif
 constexpr int MODE_GEMM = 0, MODE_HALO = 1;
-constexpr int kTmaThreads = 384;   // warps 0-3: TMA / MMA / TMEM-alloc+halo / idle;  warps 4-11: epilogue (two per TMEM lane quarter)
+constexpr int kTmaThreads = 384;   // warpgroup 0: producers;  warpgroups 1-2: MMA + epilogue
 constexpr int kHaloBytes = 180 * 128;   // one bf16 plane of an 18 x 10 pixel x 64 channel halo (what one TMA box delivers)
 
 struct TmaGemmParams {
@@ -56,58 +52,28 @@ struct TmaGemmParams {
   // bilinear x2 upsample in front of it (weights.py:_compose_up2_conv3): chunk ph, low-res pixel (y, x) -> pixel
   // (2y + ph/2, 2x + ph%2) of the 2H x 2W output, 32 channels.  C / S / the prediction tail are addressed on that grid.
   int phase4;
-  // timing experiments (tests/diag/gemm_probe.py, env PF_GEMM_DBG; 0 in production): bit 0 = epilogue without global stores,
-  // bit 1 = producer re-arms the stages without loading (operands stay whatever the first pass loaded), bit 2 = no MMAs issued,
-  // bit 3 = epilogue without the TMEM read, bit 4 = no fence.proxy.async, bit 5 = no bulk wait, bit 6 = no bias staging,
-  // bit 7 = the epilogue only waits and releases the accumulator, bit 8 = producer / MMA warps poll their barriers
-  // (test_wait) instead of the suspending try_wait, bit 9 = the epilogue warps too, bit 10 = (halo mode) the halo producer re-arms its
-  // buffers without loading.  Bits 0, 1, 2, 7 act in halo mode as well (env PF_HALO_DBG).  Results are then meaningless; only the kernel duration is of interest.
-  int dbg;
 };
 
-// KB = K elements per pipeline step: 32 (64 B rows, SWIZZLE_64B) for wide tiles, 64 (128 B rows, SWIZZLE_128B) for BN <= 128
+// KB = K elements per pipeline step: 32 (64 B rows, SWIZZLE_64B) for wide tiles, 64 (128 B rows, SWIZZLE_128B) for narrow ones
 // where a 32-wide step would be shorter than the barrier round trip that feeds it.
 template <int BN, int MODE, int KB> struct TmaCfg {
   static_assert(KB == 32 || KB == 64, "KB");
+  static_assert(BN % 32 == 0 && BN <= 256, "BN");
   static constexpr int kBPlane = BN * KB * 2;                   // bf16 plane of one K step of B
   static constexpr int kAPlane = 128 * KB * 2;                  // MODE_GEMM: plane of a 128 x KB A tile
   static constexpr int kStage = (MODE == MODE_GEMM ? 2 * kAPlane : 0) + 2 * kBPlane;
   static constexpr int kABuf = 2 * kHtPlaneBytes;               // MODE_HALO: hi + lo halo planes (1024 B multiples)
-  // MODE_GEMM epilogue staging, 64 KB: warps 4-11 (two per TMEM lane quarter, alternate 32-column chunks), each two 4 KB tiles
-  // (32 rows x 32 columns fp32, or bf16 hi + lo) that receive the residual tile (TMA load) and send the result (TMA store).
-  // Plus bias / layer-scale copies (2 x 256 floats per warp).
-#ifdef PF_PROBE_DEEP_RING   // pipeline-depth experiment (tests/diag/gemm_dbg_probe.py with dbg bit 7): no epilogue staging, all smem to the ring
-  static constexpr int kEpiStage = 0;
-  static constexpr int kEpiVec = 0;
-#else
-  static constexpr int kEpiStage = MODE == MODE_GEMM ? 4 * 16384 : 0;
-  static constexpr int kEpiVec = MODE == MODE_GEMM ? 8 * 2 * 256 * 4 : 0;
-#endif
-  static constexpr int kBudget = 225 * 1024 - kEpiStage - kEpiVec - (MODE == MODE_HALO ? 2 * kABuf : 0);
+  // epilogue staging: each MMA warpgroup moves its accumulators through shared memory 64 columns at a time so that one thread
+  // then holds 32 consecutive columns of one row (row pitch 68 floats: the row-wise float4 reads are free of bank conflicts)
+  static constexpr int kAccPitch = 68;
+  static constexpr int kAccStage = 2 * 64 * kAccPitch * 4;
+  static constexpr int kBudget = 225 * 1024 - kAccStage - (MODE == MODE_HALO ? 2 * kABuf : 0);
   static constexpr int kStagesRaw = kBudget / kStage;
   static constexpr int kStages = kStagesRaw > 16 ? 16 : kStagesRaw;
-  static constexpr int kSmemBytes = (MODE == MODE_HALO ? 2 * kABuf : 0) + kStages * kStage + kEpiStage + kEpiVec + 512 + 1024;
-  // Narrow halo tiles (BN <= 128): a tcgen05.mma costs max(N / 2, 32 + N / 4) clk (tools/mma_rate.cu: below N = 128 it is bound by
-  // fetching its 128 x 16 A slice and B from shared memory), so the three MMAs per product are folded into TWO: a_hi x [b_hi ; b_lo] as ONE MMA of
-  // width 2 BN (the hi and lo weight planes of a pipeline step are adjacent in shared memory) into an accumulator pair
-  // (D1 | D2), and a_lo x b_hi into D1; the epilogue adds D1 + D2.  Same products, one A-slice read less per K step.
-  static constexpr bool kDual = MODE == MODE_HALO && BN <= 128;
-  static constexpr int kAccCols = kDual ? 2 * BN : BN;            // TMEM columns of one accumulator
-  static constexpr int kTmemCols = 2 * kAccCols <= 32 ? 32 : (2 * kAccCols <= 64 ? 64 : (2 * kAccCols <= 128 ? 128 : (2 * kAccCols <= 256 ? 256 : 512)));
-  static constexpr uint32_t kIdesc = umma_idesc_bf16(BN);
-  static constexpr uint32_t kIdesc2 = umma_idesc_bf16(2 * BN <= 256 ? 2 * BN : 256);
+  static constexpr int kSmemBytes = (MODE == MODE_HALO ? 2 * kABuf : 0) + kStages * kStage + kAccStage + 512 + 1024;
   static_assert(kStages >= 2, "ring too shallow");
-  static_assert(2 * kAccCols <= 512, "two accumulators must fit TMEM");
-  static_assert(!kDual || kBPlane % 1024 == 0, "dual-N: the lo plane must continue the hi plane's swizzle pattern");
+  static_assert(kSmemBytes <= 227 * 1024, "shared memory per block");
 };
-
-// K-major operand descriptor for a tile whose rows are KB bf16 wide (KB = 32: SWIZZLE_64B, 8-row groups 512 B apart;
-// KB = 64: SWIZZLE_128B, 1024 B apart)
-template <int KB>
-__device__ __forceinline__ uint64_t tma_tile_desc(uint32_t smem_addr) {
-  constexpr uint64_t sbo = KB == 32 ? 512 : 1024, layout = KB == 32 ? 4 : 2;
-  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | ((uint64_t)1 << 16) | ((sbo >> 4) << 32) | ((uint64_t)1 << 46) | (layout << 61);
-}
 
 // ------------------------------------------------------------------------------------------------ TMA PTX
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
@@ -125,18 +91,8 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];\n" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
 
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];\n"
-               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(src), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;\n" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;\n" ::"n"(N) : "memory"); }
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;\n" ::: "memory"); }
-
 struct TmaMaps {   // passed by value as a __grid_constant__ kernel parameter
   CUtensorMap a_hi, a_lo, a2_hi, a2_lo, b_hi, b_lo;
-  CUtensorMap c, s_hi, s_lo, res;   // MODE_GEMM epilogue: fp32 output, split output planes, fp32 residual (32 x 32 boxes)
 };
 
 template <int BN, int MODE, int KB>
@@ -144,23 +100,19 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
   using Cfg = TmaCfg<BN, MODE, KB>;
   constexpr int NS = Cfg::kStages;
   constexpr int SPC = 9 * (64 / KB);          // MODE_HALO: pipeline steps per 64-channel chunk (9 taps x 64 / KB)
+  constexpr int kConsumerWarps = 8;
   extern __shared__ unsigned char smem_dyn[];
   const uint32_t raw = smem_u32(smem_dyn);
   const uint32_t sbase = (raw + 1023u) & ~1023u;
   unsigned char* sm = smem_dyn + (sbase - raw);
   const uint32_t a_base = sbase;                                                  // MODE_HALO: 2 halo buffers
   const uint32_t ring = sbase + (MODE == MODE_HALO ? 2 * Cfg::kABuf : 0);         // NS stages
-  const uint32_t epi_base = ring + NS * Cfg::kStage;                              // MODE_GEMM: 4 x 16 KB staging (1024 B aligned)
-  const uint32_t vec_base = epi_base + Cfg::kEpiStage;                            // MODE_GEMM: bias / gamma copies
-  const uint32_t bars = vec_base + Cfg::kEpiVec;
+  const uint32_t acc_base = ring + NS * Cfg::kStage;                              // epilogue staging, one half per MMA warpgroup
+  const uint32_t bars = acc_base + Cfg::kAccStage;
   auto full_b = [&](int s) { return bars + 8u * s; };
   auto empty_b = [&](int s) { return bars + 8u * (NS + s); };
   auto full_a = [&](int i) { return bars + 8u * (2 * NS + i); };
   auto empty_a = [&](int i) { return bars + 8u * (2 * NS + 2 + i); };
-  auto tmem_full = [&](int i) { return bars + 8u * (2 * NS + 4 + i); };
-  auto tmem_empty = [&](int i) { return bars + 8u * (2 * NS + 6 + i); };
-  const uint32_t tmem_slot = bars + 8u * (2 * NS + 8);
-  auto res_bar = [&](int w, int i) { return bars + 8u * (2 * NS + 9 + 2 * w + i); };   // MODE_GEMM: residual tile i of epilogue warp w landed
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int n_tiles = cdiv(p.N, BN);
@@ -172,20 +124,15 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
   // resident for all of its tiles instead of being re-streamed from L2 for every tile.
   const bool b_resident = MODE == MODE_HALO && nchunks == 1 && SPC <= NS;
 
-  if (warp == 0 && lane == 0) {
+  if (tid == 0) {
     tma_prefetch_desc(&maps.a_hi); tma_prefetch_desc(&maps.a_lo); tma_prefetch_desc(&maps.b_hi); tma_prefetch_desc(&maps.b_lo);
-    for (int s = 0; s < NS; ++s) { mbar_init(full_b(s), 1); mbar_init(empty_b(s), 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(full_a(i), 1); mbar_init(empty_a(i), 1); mbar_init(tmem_full(i), 1); mbar_init(tmem_empty(i), 256); }
-    for (int i = 0; i < 16; ++i) mbar_init(res_bar(i >> 1, i & 1), 1);
+    for (int s = 0; s < NS; ++s) { mbar_init(full_b(s), 1); mbar_init(empty_b(s), kConsumerWarps); }
+    for (int i = 0; i < 2; ++i) { mbar_init(full_a(i), 1); mbar_init(empty_a(i), kConsumerWarps); }
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, Cfg::kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *reinterpret_cast<volatile uint32_t*>(sm + (tmem_slot - sbase));
-  // everything above (barrier init, TMEM allocation, descriptor prefetch) overlaps the tail of the previous kernel of the stream
-  // when this one was launched with programmatic stream serialisation; from here on its results are read
+  // everything above (barrier init, descriptor prefetch) overlaps the tail of the previous kernel of the stream when this one
+  // was launched with programmatic stream serialisation; from here on its results are read
   pdl_wait();
   pdl_launch();
 
@@ -197,9 +144,10 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
     mt = tile / p.groups;
   };
 
-  if (warp == 0) {
-    // ======================================================================= TMA producer: B ring (+ A tiles in MODE_GEMM)
-    if (lane == 0) {
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n");
+    if (warp == 0 && lane == 0) {
+      // ===================================================================== TMA producer: B ring (+ A tiles in MODE_GEMM)
       int it = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         int mt, g, n0;
@@ -208,8 +156,7 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
         if (b_resident && it > 0) break;     // resident weights: loaded with the first tile only (one group / N tile per launch)
         for (int kc = 0; kc < nk; ++kc, ++it) {
           const int s = it % NS;
-          if (p.dbg & 256) mbar_wait_spin(empty_b(s), ((it / NS) & 1) ^ 1); else mbar_wait(empty_b(s), ((it / NS) & 1) ^ 1);
-          if ((p.dbg & 2) && it >= NS) { mbar_arrive(full_b(s)); continue; }
+          mbar_wait(empty_b(s), ((it / NS) & 1) ^ 1);
           mbar_expect_tx(full_b(s), Cfg::kStage);
           const uint32_t st = ring + s * Cfg::kStage;
           int kcol;
@@ -226,10 +173,8 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
           tma_load_2d(bdst + Cfg::kBPlane, &maps.b_lo, full_b(s), kcol, brow);
         }
       }
-    }
-  } else if (warp == 2) {
-    // ======================================================================= MODE_HALO: halo (A) producer
-    if (MODE == MODE_HALO && lane == 0) {
+    } else if (MODE == MODE_HALO && warp == 1 && lane == 0) {
+      // ===================================================================== MODE_HALO: halo (A) producer
       int ita = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         int mt, g, n0;
@@ -238,7 +183,6 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
         for (int c = 0; c < nchunks; ++c, ++ita) {
           const int buf = ita & 1;
           mbar_wait(empty_a(buf), ((ita >> 1) & 1) ^ 1);
-          if ((p.dbg & 1024) && ita >= 2) { mbar_arrive(full_a(buf)); continue; }
           mbar_expect_tx(full_a(buf), 2 * kHaloBytes);
           const uint32_t dst = a_base + buf * Cfg::kABuf;
           const int ci = c * 64;
@@ -252,393 +196,252 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
         }
       }
     }
-  } else if (warp == 1) {
-    // ======================================================================= MMA issuer
-    int it = 0, ita = 0, tl = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++tl) {
-      const int as = tl & 1;
-      if (p.dbg & 256) mbar_wait_spin(tmem_empty(as), ((tl >> 1) & 1) ^ 1); else mbar_wait(tmem_empty(as), ((tl >> 1) & 1) ^ 1);      // the epilogue has drained this accumulator
-      tc_fence_after();
-      const uint32_t acc = tmem + (uint32_t)(as * Cfg::kAccCols);
-      for (int kc = 0; kc < nk; ++kc, ++it) {
-        const int s = it % NS;
-        uint32_t a_hi, a_lo;
-        int a_kbase = 0;
-        bool chunk_end = false;
-        if (MODE == MODE_HALO) {
-          const int c = kc / SPC, u = kc - c * SPC;
-          const int tap = KB == 32 ? (u >> 1) : u, ky = tap / 3, kx = tap - ky * 3;
-          const int buf = ita & 1;
-          if (u == 0) mbar_wait(full_a(buf), (ita >> 1) & 1);
-          a_hi = a_base + buf * Cfg::kABuf + (ky * kHtHaloW + kx) * 128;
-          a_lo = a_hi + kHtPlaneBytes;
-          a_kbase = KB == 32 ? (u & 1) * 64 : 0;          // KB = 32: second half of the 128 B pixel row
-          chunk_end = u == SPC - 1;
-        } else {
-          a_hi = ring + s * Cfg::kStage;
-          a_lo = a_hi + Cfg::kAPlane;
-        }
-        const int sb = b_resident ? kc : s;                                   // resident weights: step kc lives in slot kc
-        if (!b_resident || tl == 0) { if (p.dbg & 256) mbar_wait_spin(full_b(sb), b_resident ? 0 : ((it / NS) & 1)); else mbar_wait(full_b(sb), b_resident ? 0 : ((it / NS) & 1)); }
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t b_hi = ring + sb * Cfg::kStage + (MODE == MODE_GEMM ? 2 * Cfg::kAPlane : 0);
-          // descriptors of this step's first K=16 slice; the following slices are +32 B, i.e. +2 in the (address >> 4) field
-          // (no carry: shared-memory addresses are < 2^18), so the issuing thread spends two adds per MMA instead of a rebuild
-          uint64_t dah = MODE == MODE_HALO ? ht_a_desc(a_hi + a_kbase) : tma_tile_desc<KB>(a_hi);
-          uint64_t dal = dah + (uint64_t)((a_lo - a_hi) >> 4);
-          uint64_t dbh = tma_tile_desc<KB>(b_hi);
-          uint64_t dbl = dbh + (uint64_t)(Cfg::kBPlane >> 4);
-#pragma unroll
-          for (int kk = 0; kk < KB / 16; ++kk) {
-            if (p.dbg & 4) break;
-            if (Cfg::kDual) {
-              umma_bf16(acc, dah, dbh, Cfg::kIdesc2, (kc | kk) ? 1u : 0u);     // (D1 | D2) (+)= a_hi x [b_hi ; b_lo]
-              umma_bf16(acc, dal, dbh, Cfg::kIdesc, 1u);                       //  D1        += a_lo x b_hi
-            } else {
-              umma_bf16(acc, dal, dbh, Cfg::kIdesc, (kc | kk) ? 1u : 0u);
-              umma_bf16(acc, dah, dbl, Cfg::kIdesc, 1u);
-              umma_bf16(acc, dah, dbh, Cfg::kIdesc, 1u);
-            }
-            dah += 2; dal += 2; dbh += 2; dbl += 2;
-          }
-          if (!b_resident) umma_commit(empty_b(s));
-          if (MODE == MODE_HALO && chunk_end) umma_commit(empty_a(ita & 1));
-          if (kc == nk - 1) umma_commit(tmem_full(as));
-        }
-        __syncwarp();
-        if (MODE == MODE_HALO && chunk_end) ++ita;
-      }
-    }
-  } else if (MODE == MODE_GEMM && warp >= 4) {
-    // ======================================================================= MODE_GEMM epilogue: warps 4-11, TMA loads / stores
-    // Per warp (32 tile rows) and 32-column chunk: TMEM -> registers, + bias, activation, layer scale, + residual tile (TMA-
-    // loaded into swizzled smem one chunk ahead), then the result goes to a swizzled smem tile and ONE thread issues a
-    // bulk-tensor store: global traffic is full 128 B rows written by the copy engine instead of 16 B-per-row thread stores.
-    // Eight warps: TMEM lane quarter q = warp % 4, warps w and w + 4 take alternate 32-column chunks.  Each warp owns two 4 KB
-    // smem tiles used in turn: the residual tile of a chunk is TMA-loaded INTO the tile, the result overwrites it in place (a lane
-    // reads and writes only its own row) and is TMA-stored from it.  The residual of the warp's next chunk is requested as soon
-    // as the store that last used the other tile has been read out.
-    {
-      const bool has_res = p.res != nullptr;
-      const int q = warp & 3;
-      const int ew = warp - 4;                              // 0..7
-      const int ch0 = ew >> 2;                              // this warp's chunks: ch0, ch0 + 2, ...
-      const uint32_t stg = epi_base + ew * 8192;
-      unsigned char* stg_p = sm + (stg - sbase);
-      float* bias_s = reinterpret_cast<float*>(sm + (vec_base - sbase)) + ew * 512;
-      float* gamma_s = bias_s + 256;
-      uint32_t cc = 0;                                      // chunks staged so far by this warp (tile = cc & 1, barrier phase = (cc >> 1) & 1)
-      int tl = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++tl) {
-        int mt, g, n0;
-        decode(tile, mt, g, n0);
-        const int as = tl & 1;
-        const int row0 = mt * 128 + q * 32;
-        const int nch = ((p.N - n0 < BN ? p.N - n0 : BN) + 31) / 32;
-        for (int j = lane; j < BN && !(p.dbg & 64); j += 32) {
-          const bool ok = n0 + j < p.N;
-          bias_s[j] = (p.bias_mode && ok) ? __ldg(p.bias + n0 + j) : 0.f;
-          gamma_s[j] = (p.gamma && ok) ? __ldg(p.gamma + n0 + j) : 1.f;
-        }
-        __syncwarp();
-        const bool warp_active = row0 < p.M && ch0 < nch;    // warp-uniform: this warp's rows / chunks intersect the matrix
-        if (has_res && warp_active && lane == 0) {          // residual of this tile's first chunk
-          bulk_wait_read<0>();                              // (both tiles free: every earlier store has been read out)
-          mbar_expect_tx(res_bar(ew, cc & 1), 4096);
-          tma_load_2d(stg + (cc & 1) * 4096, &maps.res, res_bar(ew, cc & 1), p.r_coff + n0 + ch0 * 32, row0);
-        }
-        if (p.dbg & 512) mbar_wait_spin(tmem_full(as), (tl >> 1) & 1); else mbar_wait(tmem_full(as), (tl >> 1) & 1);
-        tc_fence_after();
-#pragma unroll 1
-        for (int ch = ch0; ch < nch; ch += 2) {
-          if (p.dbg & 128) break;
-          uint32_t v[32];
-          if (p.dbg & 8) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = (uint32_t)(lane + j);
-          } else {
-            tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * Cfg::kAccCols + ch * 32), v);
-          }
-          if (!warp_active) continue;                                  // whole warp beyond the matrix (warp-uniform)
-          const int ob = cc & 1;
-          if (lane == 0) {
-            if (has_res) {
-              bulk_wait_read<0>();                                     // the store of the previous chunk has read tile ob ^ 1
-              if (ch + 2 < nch) {                                      // residual of the next chunk into it
-                mbar_expect_tx(res_bar(ew, ob ^ 1), 4096);
-                tma_load_2d(stg + (ob ^ 1) * 4096, &maps.res, res_bar(ew, ob ^ 1), p.r_coff + n0 + (ch + 2) * 32, row0);
-              }
-            } else if (!(p.dbg & 32)) {
-              bulk_wait_read<1>();                                     // the store that used tile ob two chunks ago has read it
-            }
-          }
-          __syncwarp();
-          float o[32];
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 bv = *reinterpret_cast<const float4*>(bias_s + ch * 32 + j);
-            o[j] = __uint_as_float(v[j]) + bv.x; o[j + 1] = __uint_as_float(v[j + 1]) + bv.y;
-            o[j + 2] = __uint_as_float(v[j + 2]) + bv.z; o[j + 3] = __uint_as_float(v[j + 3]) + bv.w;
-          }
-          if (p.act == 1) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) o[j] = fmaxf(o[j], 0.f);
-          } else if (p.act == 2) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) o[j] = gelu_erf(o[j]);
-          }
-          if (p.gamma) {
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const float4 gv = *reinterpret_cast<const float4*>(gamma_s + ch * 32 + j);
-              o[j] *= gv.x; o[j + 1] *= gv.y; o[j + 2] *= gv.z; o[j + 3] *= gv.w;
-            }
-          }
-          unsigned char* ob_p = stg_p + ob * 4096;
-          if (has_res) {
-            mbar_wait(res_bar(ew, ob), (cc >> 1) & 1);
-            const unsigned char* rb = ob_p + lane * 128;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              float4 rv = *reinterpret_cast<const float4*>(rb + ((j ^ (lane & 7)) << 4));
-              if (p.res_relu) { rv.x = fmaxf(rv.x, 0.f); rv.y = fmaxf(rv.y, 0.f); rv.z = fmaxf(rv.z, 0.f); rv.w = fmaxf(rv.w, 0.f); }
-              o[4 * j] += rv.x; o[4 * j + 1] += rv.y; o[4 * j + 2] += rv.z; o[4 * j + 3] += rv.w;
-            }
-            __syncwarp();      // (split output: a lane's 64 B hi/lo rows overlap other lanes' 128 B residual rows)
-          }
-          ++cc;
-          if (p.C) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              *reinterpret_cast<float4*>(ob_p + lane * 128 + ((j ^ (lane & 7)) << 4)) = make_float4(o[4 * j], o[4 * j + 1], o[4 * j + 2], o[4 * j + 3]);
-          } else {   // split output only: hi plane tile at +0, lo plane tile at +2048, rows of 64 B, SWIZZLE_64B
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              uint4 h, l;
-              float t[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) t[e] = p.split_relu ? fmaxf(o[8 * j + e], 0.f) : o[8 * j + e];
-              split_bf16x2(t[0], t[1], h.x, l.x); split_bf16x2(t[2], t[3], h.y, l.y);
-              split_bf16x2(t[4], t[5], h.z, l.z); split_bf16x2(t[6], t[7], h.w, l.w);
-              const int off = lane * 64 + ((j ^ ((lane >> 1) & 3)) << 4);
-              *reinterpret_cast<uint4*>(ob_p + off) = h;
-              *reinterpret_cast<uint4*>(ob_p + 2048 + off) = l;
-            }
-          }
-          if (!(p.dbg & 16)) fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0 && !(p.dbg & 1)) {
-            const int col = n0 + ch * 32;
-            if (p.C) tma_store_2d(&maps.c, stg + ob * 4096, p.c_coff + col, row0);
-            else { tma_store_2d(&maps.s_hi, stg + ob * 4096, p.s_coff + col, row0); tma_store_2d(&maps.s_lo, stg + ob * 4096 + 2048, p.s_coff + col, row0); }
-            bulk_commit();
-          }
-        }
-        tc_fence_before();
-        mbar_arrive(tmem_empty(as));
-      }
-      if (lane == 0) bulk_wait_all();            // all stores have landed before the CTA exits
-    }
-  } else if (warp >= 4) {
-    // ======================================================================= epilogue warps (MODE_HALO)
-    const int q = warp & 3;                       // TMEM lane quarter (hardware: warp id % 4)
-    const int eh = (warp - 4) >> 2;               // which half of the 32-column chunks this warp drains
-    const int r = q * 32 + lane;                  // row of the tile
-    int tl = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++tl) {
-      int mt, g, n0;
-      decode(tile, mt, g, n0);
-      const int as = tl & 1;
-      long long m;
-      bool valid;
-      int cls_off = 0;
-      int bimg = 0, oy = 0, ox = 0;
-      if (MODE == MODE_GEMM) {
-        m = (long long)mt * 128 + r;
-        valid = m < p.M;
-      } else {
-        const int tx = mt % tiles_x, ty = (mt / tiles_x) % tiles_y;
-        bimg = mt / (tiles_x * tiles_y);
-        oy = ty * kHtTileH + (r >> 3); ox = tx * kHtTileW + (r & 7);
-        valid = oy < p.H && ox < p.W;
-        m = ((long long)bimg * p.H + oy) * p.W + ox;
-        if (p.bias_mode == 2) {
-          const int ry = oy == 0 ? 0 : (oy == p.H - 1 ? 2 : 1);
-          const int rx = ox == 0 ? 0 : (ox == p.W - 1 ? 2 : 1);
-          cls_off = (ry * 3 + rx) * p.N;
-        }
-      }
-      const float* __restrict__ bias = p.bias ? p.bias + (long long)g * p.bias_gstride : nullptr;
-      mbar_wait(tmem_full(as), (tl >> 1) & 1);
-      tc_fence_after();
-#pragma unroll 1
-      for (int ch = eh; ch < BN / 32; ch += 2) {
-        if (p.dbg & 128) break;
-        uint32_t v[32];
-        tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * Cfg::kAccCols + ch * 32), v);
-        if (Cfg::kDual) {       // second half of the accumulator pair: the a_hi x b_lo products
-          uint32_t v2[32];
-          tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * Cfg::kAccCols + BN + ch * 32), v2);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(v2[j]));
-        }
-        const int nb = n0 + ch * 32;
-        const bool ph4 = MODE == MODE_HALO && BN == 128 && p.phase4;
-        // output row / first output column of this chunk (phase mode: hi-res pixel of phase `ch`, channels 0-31)
-        const long long mo = ph4 ? ((long long)bimg * 2 * p.H + 2 * oy + (ch >> 1)) * (2 * p.W) + 2 * ox + (ch & 1) : m;
-        const int nbo = ph4 ? 0 : nb;
-        const bool chunk_ok = nb < p.N && !(p.dbg & 1);      // warp-uniform
-        float o[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) o[j] = __uint_as_float(v[j]);
-        if (valid && chunk_ok) {
-          if (p.bias_mode) {
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const float4 bv = __ldg(reinterpret_cast<const float4*>(bias + cls_off + nb + j));
-              o[j] += bv.x; o[j + 1] += bv.y; o[j + 2] += bv.z; o[j + 3] += bv.w;
-            }
-          }
-          if (p.act == 1) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) o[j] = fmaxf(o[j], 0.f);
-          } else if (p.act == 2) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) o[j] = gelu_erf(o[j]);
-          }
-          if (p.gamma) {
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const float4 gv = __ldg(reinterpret_cast<const float4*>(p.gamma + nb + j));
-              o[j] *= gv.x; o[j + 1] *= gv.y; o[j + 2] *= gv.z; o[j + 3] *= gv.w;
-            }
-          }
-          if (p.res) {
-            const float* rp = p.res + m * p.ldr + p.r_coff + g * p.r_gcoff + nb;
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              float4 rv = *reinterpret_cast<const float4*>(rp + j);
-              if (p.res_relu) { rv.x = fmaxf(rv.x, 0.f); rv.y = fmaxf(rv.y, 0.f); rv.z = fmaxf(rv.z, 0.f); rv.w = fmaxf(rv.w, 0.f); }
-              o[j] += rv.x; o[j + 1] += rv.y; o[j + 2] += rv.z; o[j + 3] += rv.w;
-            }
-          }
-          if (p.res2) {
-            const float* rp = p.res2 + m * p.ldr2 + p.r2_coff + g * p.r2_gcoff + nb;
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const float4 rv = *reinterpret_cast<const float4*>(rp + j);
-              o[j] += rv.x; o[j + 1] += rv.y; o[j + 2] += rv.z; o[j + 3] += rv.w;
-            }
-          }
-          if (MODE == MODE_HALO && (BN == 32 || BN == 128) && p.pred_w) {
-            float v0 = __ldg(p.pred_b), v1 = p.pred_nc > 1 ? __ldg(p.pred_b + 1) : 0.f;
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const float4 w0 = __ldg(reinterpret_cast<const float4*>(p.pred_w + j));
-              v0 = fmaf(o[j], w0.x, v0); v0 = fmaf(o[j + 1], w0.y, v0); v0 = fmaf(o[j + 2], w0.z, v0); v0 = fmaf(o[j + 3], w0.w, v0);
-              if (p.pred_nc > 1) {
-                const float4 w1 = __ldg(reinterpret_cast<const float4*>(p.pred_w + 32 + j));
-                v1 = fmaf(o[j], w1.x, v1); v1 = fmaf(o[j + 1], w1.y, v1); v1 = fmaf(o[j + 2], w1.z, v1); v1 = fmaf(o[j + 3], w1.w, v1);
-              }
-            }
-            const long long HWl = (long long)p.H * p.W * (ph4 ? 4 : 1);
-            const long long bi = mo / HWl, pix = mo - bi * HWl;
-            float* po = p.pred_out + bi * p.pred_nc * HWl + pix;
-            if (p.pred_mode == 1) {
-              const float nrm = fmaxf(sqrtf(v0 * v0 + v1 * v1), 1e-12f);
-              po[0] = v0 / nrm; po[HWl] = v1 / nrm;
-            } else {
-              po[0] = fminf(fmaxf(v0, -1.f), 1.f);
-            }
-          }
-        }
-#if PF_EPI_PAIR_STORE
-        // Stores.  A thread owns one pixel row of the chunk (128 B of fp32, 64 B per bf16 plane); storing it 16 bytes at a time makes
-        // every warp-wide store touch 32 half-filled sectors, and the short-K launches were bound by exactly that (r02 notes:
-        // 494 us against 233 us of main loop).  The two lanes of an x-adjacent pixel pair exchange halves so that each store
-        // instruction writes 32 contiguous bytes per pair: full sectors, half as many per request.
-        if (chunk_ok && (p.C || p.Shi)) {
-          const bool odd = lane & 1;
-          const bool valid_p = __shfl_xor_sync(0xffffffffu, (int)valid, 1) != 0;
-          const long long mo_p = mo + (odd ? -1 : 1) * (ph4 ? 2 : 1);       // the partner's pixel: same image row, x +- 1
-          const long long moA = odd ? mo_p : mo, moB = odd ? mo : mo_p;     // row A = the even lane's pixel, row B = the odd lane's
-          const bool vA = odd ? valid_p : valid, vB = odd ? valid : valid_p;
-          if (p.C) {
-            float* cA = p.C + moA * p.ldc + p.c_coff + g * p.c_gcoff + nbo + (odd ? 4 : 0);
-            float* cB = p.C + moB * p.ldc + p.c_coff + g * p.c_gcoff + nbo + (odd ? 4 : 0);
-#pragma unroll
-            for (int t = 0; t < 4; ++t) {      // float4 slots 2t (even lane) and 2t + 1 (odd lane) of both rows
-              float k[4], r[4];
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                k[e] = odd ? o[8 * t + 4 + e] : o[8 * t + e];
-                r[e] = __shfl_xor_sync(0xffffffffu, odd ? o[8 * t + e] : o[8 * t + 4 + e], 1);
-              }
-              if (vA) *reinterpret_cast<float4*>(cA + 8 * t) = odd ? make_float4(r[0], r[1], r[2], r[3]) : make_float4(k[0], k[1], k[2], k[3]);
-              if (vB) *reinterpret_cast<float4*>(cB + 8 * t) = odd ? make_float4(k[0], k[1], k[2], k[3]) : make_float4(r[0], r[1], r[2], r[3]);
-            }
-          }
-          if (p.Shi) {
-            const long long sA = moA * p.lds + p.s_coff + g * p.s_gcoff + nbo + (odd ? 8 : 0);
-            const long long sB = moB * p.lds + p.s_coff + g * p.s_gcoff + nbo + (odd ? 8 : 0);
-#pragma unroll
-            for (int t = 0; t < 2; ++t) {      // 8-column slots 2t (even lane) and 2t + 1 (odd lane) of both rows
-              float k[8], r[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) {
-                const float mine = odd ? o[16 * t + 8 + e] : o[16 * t + e], give = odd ? o[16 * t + e] : o[16 * t + 8 + e];
-                k[e] = p.split_relu ? fmaxf(mine, 0.f) : mine;
-                r[e] = __shfl_xor_sync(0xffffffffu, p.split_relu ? fmaxf(give, 0.f) : give, 1);
-              }
-              uint4 kh, kl, rh, rl;
-              split_bf16x2(k[0], k[1], kh.x, kl.x); split_bf16x2(k[2], k[3], kh.y, kl.y);
-              split_bf16x2(k[4], k[5], kh.z, kl.z); split_bf16x2(k[6], k[7], kh.w, kl.w);
-              split_bf16x2(r[0], r[1], rh.x, rl.x); split_bf16x2(r[2], r[3], rh.y, rl.y);
-              split_bf16x2(r[4], r[5], rh.z, rl.z); split_bf16x2(r[6], r[7], rh.w, rl.w);
-              if (vA) {
-                *reinterpret_cast<uint4*>(p.Shi + sA + 16 * t) = odd ? rh : kh;
-                *reinterpret_cast<uint4*>(p.Slo + sA + 16 * t) = odd ? rl : kl;
-              }
-              if (vB) {
-                *reinterpret_cast<uint4*>(p.Shi + sB + 16 * t) = odd ? kh : rh;
-                *reinterpret_cast<uint4*>(p.Slo + sB + 16 * t) = odd ? kl : rl;
-              }
-            }
-          }
-        }
-#else
-        if (valid && chunk_ok) {
-          if (p.C) {
-            float* cp = p.C + mo * p.ldc + p.c_coff + g * p.c_gcoff + nbo;
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(cp + j) = make_float4(o[j], o[j + 1], o[j + 2], o[j + 3]);
-          }
-          if (p.Shi) {
-            const long long so = mo * p.lds + p.s_coff + g * p.s_gcoff + nbo;
-#pragma unroll
-            for (int j = 0; j < 32; j += 8) {
-              uint4 h, l;
-              float t[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) t[e] = p.split_relu ? fmaxf(o[j + e], 0.f) : o[j + e];
-              split_bf16x2(t[0], t[1], h.x, l.x); split_bf16x2(t[2], t[3], h.y, l.y);
-              split_bf16x2(t[4], t[5], h.z, l.z); split_bf16x2(t[6], t[7], h.w, l.w);
-              *reinterpret_cast<uint4*>(p.Shi + so + j) = h;
-              *reinterpret_cast<uint4*>(p.Slo + so + j) = l;
-            }
-          }
-        }
-#endif
-      }
-      tc_fence_before();
-      mbar_arrive(tmem_empty(as));
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem, Cfg::kTmemCols);
+  // ======================================================================= MMA + epilogue warpgroups
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n");
+  const int wg = (warp >> 2) - 1;                 // 0: tile rows 0-63, 1: rows 64-127
+  const int wt = tid & 127;                       // thread within the warpgroup
+  float* stage = reinterpret_cast<float*>(sm + (acc_base - sbase)) + wg * 64 * Cfg::kAccPitch;
+  // epilogue ownership: row `erow` of this warpgroup's 64, 32-column half `eh` of each 64-column staging round
+  const int erow = wt & 63, eh = wt >> 6;
+  const int r = wg * 64 + erow;                   // row of the tile
+  float acc[BN / 2];
+  int it = 0, ita = 0;
+  for (int tile = blockIdx.x, tl = 0; tile < total_tiles; tile += gridDim.x, ++tl) {
+    int mt, g, n0;
+    decode(tile, mt, g, n0);
+    // ---------------- main loop: per K step, 3 products x BN / 64 (+ one 32-wide) wgmmas, one commit group; the stage of the
+    // previous step is released once that step's group has completed (one group stays in flight under the next wait)
+    int prev_s = -1, prev_buf = -1;
+    fence_regs(acc);
+    for (int kc = 0; kc < nk; ++kc, ++it) {
+      const int s = it % NS;
+      uint32_t a_hi, a_lo;
+      bool chunk_end = false;
+      int buf = 0;
+      if (MODE == MODE_HALO) {
+        const int c = kc / SPC, u = kc - c * SPC;
+        const int tap = KB == 32 ? (u >> 1) : u, ky = tap / 3, kx = tap - ky * 3;
+        buf = ita & 1;
+        if (u == 0) mbar_wait(full_a(buf), (ita >> 1) & 1);
+        // this warpgroup's 64 pixels are image rows 8 wg .. 8 wg + 7 of the tile
+        a_hi = a_base + buf * Cfg::kABuf + ((ky + 8 * wg) * kHtHaloW + kx) * 128 + (KB == 32 ? (u & 1) * 64 : 0);
+        a_lo = a_hi + kHtPlaneBytes;
+        chunk_end = u == SPC - 1;
+      } else {
+        a_hi = ring + s * Cfg::kStage + wg * 64 * KB * 2;
+        a_lo = a_hi + Cfg::kAPlane;
+      }
+      const int sb = b_resident ? kc : s;                                   // resident weights: step kc lives in slot kc
+      if (!b_resident || tl == 0) mbar_wait(full_b(sb), b_resident ? 0 : ((it / NS) & 1));
+      const uint32_t b_hi = ring + sb * Cfg::kStage + (MODE == MODE_GEMM ? 2 * Cfg::kAPlane : 0);
+      const uint64_t dah = MODE == MODE_HALO ? ht_a_desc(a_hi) : wgmma_tile_desc<KB>(a_hi);
+      const uint64_t dal = MODE == MODE_HALO ? ht_a_desc(a_lo) : wgmma_tile_desc<KB>(a_lo);
+      const uint64_t dbh = wgmma_tile_desc<KB>(b_hi);
+      const uint64_t dbl = wgmma_tile_desc<KB>(b_hi + Cfg::kBPlane);
+      constexpr uint64_t kChunk = (uint64_t)(64 * KB * 2) >> 4;          // 64 weight rows further in the B tile
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < KB / 16; ++kk) {
+        const uint32_t first = (kc | kk) ? 1u : 0u;
+#pragma unroll
+        for (int j = 0; j < BN / 64; ++j) {
+          wgmma_n64(acc + 32 * j, dal + 2 * kk, dbh + 2 * kk + j * kChunk, first);
+          wgmma_n64(acc + 32 * j, dah + 2 * kk, dbl + 2 * kk + j * kChunk, 1u);
+          wgmma_n64(acc + 32 * j, dah + 2 * kk, dbh + 2 * kk + j * kChunk, 1u);
+        }
+        if constexpr (BN % 64 != 0) {
+          constexpr int j = BN / 64;
+          wgmma_n32(acc + 32 * j, dal + 2 * kk, dbh + 2 * kk + j * kChunk, first);
+          wgmma_n32(acc + 32 * j, dah + 2 * kk, dbl + 2 * kk + j * kChunk, 1u);
+          wgmma_n32(acc + 32 * j, dah + 2 * kk, dbh + 2 * kk + j * kChunk, 1u);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (lane == 0 && prev_s >= 0) {
+        if (!b_resident) mbar_arrive(empty_b(prev_s));
+        if (MODE == MODE_HALO && prev_buf >= 0) mbar_arrive(empty_a(prev_buf));
+      }
+      prev_s = s;
+      prev_buf = chunk_end ? buf : -1;
+      if (MODE == MODE_HALO && chunk_end) ++ita;
+    }
+    wgmma_wait<0>();
+    fence_regs(acc);
+    if (lane == 0 && prev_s >= 0) {
+      if (!b_resident) mbar_arrive(empty_b(prev_s));
+      if (MODE == MODE_HALO && prev_buf >= 0) mbar_arrive(empty_a(prev_buf));
+    }
+
+    // ---------------- epilogue
+    long long m;
+    bool valid;
+    int cls_off = 0;
+    int bimg = 0, oy = 0, ox = 0;
+    if (MODE == MODE_GEMM) {
+      m = (long long)mt * 128 + r;
+      valid = m < p.M;
+    } else {
+      const int tx = mt % tiles_x, ty = (mt / tiles_x) % tiles_y;
+      bimg = mt / (tiles_x * tiles_y);
+      oy = ty * kHtTileH + (r >> 3); ox = tx * kHtTileW + (r & 7);
+      valid = oy < p.H && ox < p.W;
+      m = ((long long)bimg * p.H + oy) * p.W + ox;
+      if (p.bias_mode == 2) {
+        const int ry = oy == 0 ? 0 : (oy == p.H - 1 ? 2 : 1);
+        const int rx = ox == 0 ? 0 : (ox == p.W - 1 ? 2 : 1);
+        cls_off = (ry * 3 + rx) * p.N;
+      }
+    }
+    const float* __restrict__ bias = p.bias ? p.bias + (long long)g * p.bias_gstride : nullptr;
+    // accumulator fragment of m64nNk16: register 4 jb + 2 h + e holds row 16 (wt / 32) + lane / 4 + 8 h, column 8 jb + 2 (lane % 4) + e
+    const int frow = (wt >> 5) * 16 + (lane >> 2), fcol = 2 * (lane & 3);
+#pragma unroll
+    for (int rd = 0; rd < (BN + 63) / 64; ++rd) {
+      named_bar_sync(1 + wg, 128);                // the previous round's (or tile's) rows have been read
+#pragma unroll
+      for (int jb = 0; jb < 8; ++jb) {
+        const int cb = rd * 8 + jb;
+        if (cb < BN / 8) {
+          float* d0 = stage + frow * Cfg::kAccPitch + jb * 8 + fcol;
+          *reinterpret_cast<float2*>(d0) = make_float2(acc[4 * cb], acc[4 * cb + 1]);
+          *reinterpret_cast<float2*>(d0 + 8 * Cfg::kAccPitch) = make_float2(acc[4 * cb + 2], acc[4 * cb + 3]);
+        }
+      }
+      named_bar_sync(1 + wg, 128);
+      const int ch = 2 * rd + eh;                 // this thread's 32-column chunk (warp-uniform)
+      if (ch >= BN / 32) continue;
+      const int nb = n0 + ch * 32;
+      const bool ph4 = MODE == MODE_HALO && BN == 128 && p.phase4;
+      // output row / first output column of this chunk (phase mode: hi-res pixel of phase `ch`, channels 0-31)
+      const long long mo = ph4 ? ((long long)bimg * 2 * p.H + 2 * oy + (ch >> 1)) * (2 * p.W) + 2 * ox + (ch & 1) : m;
+      const int nbo = ph4 ? 0 : nb;
+      const bool chunk_ok = nb < p.N;      // warp-uniform
+      float o[32];
+      const float* srow = stage + erow * Cfg::kAccPitch + eh * 32;
+#pragma unroll
+      for (int j = 0; j < 32; j += 4) {
+        const float4 t = *reinterpret_cast<const float4*>(srow + j);
+        o[j] = t.x; o[j + 1] = t.y; o[j + 2] = t.z; o[j + 3] = t.w;
+      }
+      if (valid && chunk_ok) {
+        if (p.bias_mode) {
+#pragma unroll
+          for (int j = 0; j < 32; j += 4) {
+            const float4 bv = __ldg(reinterpret_cast<const float4*>(bias + cls_off + nb + j));
+            o[j] += bv.x; o[j + 1] += bv.y; o[j + 2] += bv.z; o[j + 3] += bv.w;
+          }
+        }
+        if (p.act == 1) {
+#pragma unroll
+          for (int j = 0; j < 32; ++j) o[j] = fmaxf(o[j], 0.f);
+        } else if (p.act == 2) {
+#pragma unroll
+          for (int j = 0; j < 32; ++j) o[j] = gelu_erf(o[j]);
+        }
+        if (p.gamma) {
+#pragma unroll
+          for (int j = 0; j < 32; j += 4) {
+            const float4 gv = __ldg(reinterpret_cast<const float4*>(p.gamma + nb + j));
+            o[j] *= gv.x; o[j + 1] *= gv.y; o[j + 2] *= gv.z; o[j + 3] *= gv.w;
+          }
+        }
+        if (p.res) {
+          const float* rp = p.res + m * p.ldr + p.r_coff + g * p.r_gcoff + nb;
+#pragma unroll
+          for (int j = 0; j < 32; j += 4) {
+            float4 rv = *reinterpret_cast<const float4*>(rp + j);
+            if (p.res_relu) { rv.x = fmaxf(rv.x, 0.f); rv.y = fmaxf(rv.y, 0.f); rv.z = fmaxf(rv.z, 0.f); rv.w = fmaxf(rv.w, 0.f); }
+            o[j] += rv.x; o[j + 1] += rv.y; o[j + 2] += rv.z; o[j + 3] += rv.w;
+          }
+        }
+        if (p.res2) {
+          const float* rp = p.res2 + m * p.ldr2 + p.r2_coff + g * p.r2_gcoff + nb;
+#pragma unroll
+          for (int j = 0; j < 32; j += 4) {
+            const float4 rv = *reinterpret_cast<const float4*>(rp + j);
+            o[j] += rv.x; o[j + 1] += rv.y; o[j + 2] += rv.z; o[j + 3] += rv.w;
+          }
+        }
+        if (MODE == MODE_HALO && (BN == 32 || BN == 128) && p.pred_w) {
+          float v0 = __ldg(p.pred_b), v1 = p.pred_nc > 1 ? __ldg(p.pred_b + 1) : 0.f;
+#pragma unroll
+          for (int j = 0; j < 32; j += 4) {
+            const float4 w0 = __ldg(reinterpret_cast<const float4*>(p.pred_w + j));
+            v0 = fmaf(o[j], w0.x, v0); v0 = fmaf(o[j + 1], w0.y, v0); v0 = fmaf(o[j + 2], w0.z, v0); v0 = fmaf(o[j + 3], w0.w, v0);
+            if (p.pred_nc > 1) {
+              const float4 w1 = __ldg(reinterpret_cast<const float4*>(p.pred_w + 32 + j));
+              v1 = fmaf(o[j], w1.x, v1); v1 = fmaf(o[j + 1], w1.y, v1); v1 = fmaf(o[j + 2], w1.z, v1); v1 = fmaf(o[j + 3], w1.w, v1);
+            }
+          }
+          const long long HWl = (long long)p.H * p.W * (ph4 ? 4 : 1);
+          const long long bi = mo / HWl, pix = mo - bi * HWl;
+          float* po = p.pred_out + bi * p.pred_nc * HWl + pix;
+          if (p.pred_mode == 1) {
+            const float nrm = fmaxf(sqrtf(v0 * v0 + v1 * v1), 1e-12f);
+            po[0] = v0 / nrm; po[HWl] = v1 / nrm;
+          } else {
+            po[0] = fminf(fmaxf(v0, -1.f), 1.f);
+          }
+        }
+      }
+      // Stores.  A thread owns one row of the chunk (128 B of fp32, 64 B per bf16 plane); storing it 16 bytes at a time makes every
+      // warp-wide store touch 32 half-filled sectors.  The two lanes of an adjacent row pair (x-adjacent pixels in halo mode)
+      // exchange halves so that each store instruction writes 32 contiguous bytes per pair: full sectors, half as many per request.
+      if (chunk_ok && (p.C || p.Shi)) {
+        const bool odd = lane & 1;
+        const bool valid_p = __shfl_xor_sync(0xffffffffu, (int)valid, 1) != 0;
+        const long long mo_p = mo + (odd ? -1 : 1) * (ph4 ? 2 : 1);       // the partner's row (pixel: same image row, x +- 1)
+        const long long moA = odd ? mo_p : mo, moB = odd ? mo : mo_p;     // row A = the even lane's, row B = the odd lane's
+        const bool vA = odd ? valid_p : valid, vB = odd ? valid : valid_p;
+        if (p.C) {
+          float* cA = p.C + moA * p.ldc + p.c_coff + g * p.c_gcoff + nbo + (odd ? 4 : 0);
+          float* cB = p.C + moB * p.ldc + p.c_coff + g * p.c_gcoff + nbo + (odd ? 4 : 0);
+#pragma unroll
+          for (int t = 0; t < 4; ++t) {      // float4 slots 2t (even lane) and 2t + 1 (odd lane) of both rows
+            float k[4], rr[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              k[e] = odd ? o[8 * t + 4 + e] : o[8 * t + e];
+              rr[e] = __shfl_xor_sync(0xffffffffu, odd ? o[8 * t + e] : o[8 * t + 4 + e], 1);
+            }
+            if (vA) *reinterpret_cast<float4*>(cA + 8 * t) = odd ? make_float4(rr[0], rr[1], rr[2], rr[3]) : make_float4(k[0], k[1], k[2], k[3]);
+            if (vB) *reinterpret_cast<float4*>(cB + 8 * t) = odd ? make_float4(k[0], k[1], k[2], k[3]) : make_float4(rr[0], rr[1], rr[2], rr[3]);
+          }
+        }
+        if (p.Shi) {
+          const long long sA = moA * p.lds + p.s_coff + g * p.s_gcoff + nbo + (odd ? 8 : 0);
+          const long long sB = moB * p.lds + p.s_coff + g * p.s_gcoff + nbo + (odd ? 8 : 0);
+#pragma unroll
+          for (int t = 0; t < 2; ++t) {      // 8-column slots 2t (even lane) and 2t + 1 (odd lane) of both rows
+            float k[8], rr[8];
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+              const float mine = odd ? o[16 * t + 8 + e] : o[16 * t + e], give = odd ? o[16 * t + e] : o[16 * t + 8 + e];
+              k[e] = p.split_relu ? fmaxf(mine, 0.f) : mine;
+              rr[e] = __shfl_xor_sync(0xffffffffu, p.split_relu ? fmaxf(give, 0.f) : give, 1);
+            }
+            uint4 kh, kl, rh, rl;
+            split_bf16x2(k[0], k[1], kh.x, kl.x); split_bf16x2(k[2], k[3], kh.y, kl.y);
+            split_bf16x2(k[4], k[5], kh.z, kl.z); split_bf16x2(k[6], k[7], kh.w, kl.w);
+            split_bf16x2(rr[0], rr[1], rh.x, rl.x); split_bf16x2(rr[2], rr[3], rh.y, rl.y);
+            split_bf16x2(rr[4], rr[5], rh.z, rl.z); split_bf16x2(rr[6], rr[7], rh.w, rl.w);
+            if (vA) {
+              *reinterpret_cast<uint4*>(p.Shi + sA + 16 * t) = odd ? rh : kh;
+              *reinterpret_cast<uint4*>(p.Slo + sA + 16 * t) = odd ? rl : kl;
+            }
+            if (vB) {
+              *reinterpret_cast<uint4*>(p.Shi + sB + 16 * t) = odd ? kh : rh;
+              *reinterpret_cast<uint4*>(p.Slo + sB + 16 * t) = odd ? kl : rl;
+            }
+          }
+        }
+      }
+    }
+  }
 }
 
 }  // namespace pf

@@ -169,7 +169,7 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict_
 }
 
 #ifndef PF_LN_NR3
-#define PF_LN_NR3 1            // rows in flight per lane group for C > 128 (A/B: 1 row 1.58 ms, 2 rows 1.64 ms, 4 rows 1.65 ms per step; C <= 128: 4 rows)
+#define PF_LN_NR3 1            // rows in flight per lane group for C > 128 (C <= 128: 4 rows)
 #endif
 inline cudaError_t layernorm_launch(const float* in, float* out, long long rows, int C, const float* w, const float* b, float eps,
                                     cudaStream_t st, SplitT sp = SplitT(), SplitT patch = SplitT(), int R = 0, int sr = 0) {
@@ -271,14 +271,14 @@ inline cudaError_t attention_launch(const float* q, const float* kv, float* out,
 #define PF_DW3_PX 4            // output pixels per thread along x (x 2 rows x 4 channels)
 #endif
 #ifndef PF_DW3_HOIST
-#define PF_DW3_HOIST 1          // A/B on one box: 1.40 ms per step hoisted, 1.455 ms row by row
+#define PF_DW3_HOIST 1          // 0: weights loaded row by row
 #endif
 #ifndef PF_DW3_MINBLOCKS
-#define PF_DW3_MINBLOCKS 2     // (3 blocks per SM = 80 registers with spills measured 4 % slower, A/B in profiles/r02_notes.md)
+#define PF_DW3_MINBLOCKS 2     // (3 blocks per SM = 80 registers, with spills)
 #endif
 // Index arithmetic is 32-bit in units of float4 (4 channels): o00 = pixel (y0, x0) of the thread's tile, neighbours at +- W*C/4 and
 // +- C/4 (modular unsigned arithmetic: an index is only dereferenced when its row / column predicate holds).  The 64-bit
-// per-load address chains of the first version were a third of the executed instructions (ncu: profiles/r02_notes.md).
+// per-load address chains of a first version were a third of its executed instructions.
 __global__ void __launch_bounds__(256, PF_DW3_MINBLOCKS) dwconv3x3_gelu_kernel(const float* __restrict__ in, float* __restrict__ out, int B, int H, int W, int C,
                                                              const float* __restrict__ w, const float* __restrict__ bias,
                                                              __nv_bfloat16* __restrict__ shi = nullptr, __nv_bfloat16* __restrict__ slo = nullptr) {
@@ -391,7 +391,6 @@ __global__ void __launch_bounds__(256, PF_DW3_MINBLOCKS) dwconv3x3_gelu_kernel(c
 // Depthwise 7x7 conv (pad 3) + bias on NHWC -- ConvNeXt block head, convnext.py:28-30,48.  w: [49][C].
 // thread = 4 channels x (2 rows x 8 consecutive pixels): per input row 14 activation loads serve both output rows; 98 weight +
 // 112 activation loads (16 B) for 3136 FMAs, which balances the L1 path against the FMA pipe (one row x 4 pixels was L1-bound 2.4x)
-// (two blocks per SM at 128 registers measured no faster: 22.8 vs 22.5 ms per step with 24 B of spills; profiles/r02_notes.md)
 #ifndef PF_DW7_PX
 #define PF_DW7_PX 4            // output pixels per thread along x (x 2 rows x 4 channels); A/B: 4 px at 2 blocks / SM 0.78 ms, 8 px at 1 block 0.84 ms
 #endif
@@ -561,7 +560,7 @@ __global__ void __launch_bounds__(C / 4 * (C <= 192 ? 240 / (C / 4) : (C == 384 
 inline cudaError_t dwconv7x7_ln_launch(const float* in, int B, int H, int W, int C, const float* w, const float* bias, const float* gw, const float* gb,
                                        float eps, SplitT out, cudaStream_t st) {
   const int ngroups = B * ((H + 1) / 2) * ((W + 7) / 8);
-  auto grid = [&](int G) { const int g = cdiv(ngroups, G); return dim3((unsigned)(g < 148 * 8 ? g : 148 * 8)); };
+  auto grid = [&](int G) { const int g = cdiv(ngroups, G); return dim3((unsigned)(g < 132 * 8 ? g : 132 * 8)); };
   switch (C) {
     case 96: return launch_pdl(dwconv7x7_ln_kernel<96>, grid(10), dim3(240), 0, st, in, B, H, W, w, bias, gw, gb, eps, out.hi, out.lo);
     case 192: return launch_pdl(dwconv7x7_ln_kernel<192>, grid(5), dim3(240), 0, st, in, B, H, W, w, bias, gw, gb, eps, out.hi, out.lo);
@@ -573,7 +572,7 @@ inline cudaError_t dwconv7x7_ln_launch(const float* in, int B, int H, int W, int
 
 inline unsigned ew_grid(long long total) {
   long long g = cdivl(total, 256);
-  const long long cap = 148LL * 32;
+  const long long cap = 132LL * 32;
   return (unsigned)(g < cap ? (g > 0 ? g : 1) : cap);
 }
 
@@ -677,7 +676,7 @@ __global__ void __launch_bounds__(256) im2col_split_kernel(const __nv_bfloat16* 
 // x0 [B,320,320,4] fp32 (b,g,r,0): dst[m][(ky*7+kx)*3 + c] split into bf16 hi/lo, K padded 147 -> 160 with zeros, so that the
 // stems run on the TMA GEMM engine too.  One thread = one output pixel x 8 consecutive K columns (16 B per plane).
 // (A one-pixel-per-thread variant -- 49 float4 loads, 40 16-byte stores into the thread's own 320-byte row -- executed a third of
-// the instructions and ran 3x SLOWER: every store instruction of a warp touched 32 different rows.  profiles/r02_notes.md)
+// the instructions but every store instruction of a warp touched 32 different rows.)
 inline long long stem_gather_threads(int B, int OH, int OW) { return (long long)B * OH * OW * 20; }
 __global__ void __launch_bounds__(256) stem_gather_kernel(const float* __restrict__ x0, __nv_bfloat16* __restrict__ dhi, __nv_bfloat16* __restrict__ dlo,
                                                           int B, int OH, int OW, int stride) {

@@ -1,4 +1,4 @@
-// libpf_b200.so -- C ABI (include/pf_b200.h) and forward orchestration of the B200-native PerspectiveFields
+// libpf_b200.so -- C ABI (include/pf_b200.h) and forward orchestration of the H100-native (sm_90a) PerspectiveFields
 // inference engine.  One engine per device; pf_forward enqueues the whole graph of
 // perspective2d/perspectivefields.py:223-272 on the caller's stream.
 #include "../../include/pf_b200.h"
@@ -143,14 +143,12 @@ struct pf_engine {
   GemmW conv0, conv1;
   GemmW conv1p;                       // conv_fuse_conv1 composed with the x2 upsample in front of it: 4 phases x 32 outputs per head
   const float *conv1f_w, *conv1f_b;   // plain fp32 conv_fuse_conv1 [head][tap][ci][o] / bias, for the border-ring kernel
-  bool use_attn_tc = true;            // option "attn_tc": attention core on tcgen05 / TMEM (attention_tc.cuh); 0 = warp-level mma.sync kernel
   bool use_fork = false;              // option "fork": the spatial-reduction branch of a MiT block (sr conv -> LayerNorm -> kv) runs on a second
                                       // stream next to the q projection (both only depend on LayerNorm 1; their grids leave SMs idle: 50-75 tiles).
-                                      // Default OFF: measured 1 % slower (the persistent kernels of the two streams compete for SMs and the
-                                      // event waits break the programmatic-dependent-launch chain; profiles/r02_notes.md)
+                                      // Default OFF: the persistent kernels of the two streams compete for SMs and the event waits break
+                                      // the programmatic-dependent-launch chain
   cudaStream_t side = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-  bool use_pair = true;               // option "pair": GEMM-mode launches with enough tiles run on CTA pairs (gemm2_tma.cuh, cta_group::2)
   bool use_dwln = false;              // option "dw_ln": ConvNeXt depthwise 7x7 fused with the LayerNorm that follows it
   bool use_pdl = true;                // option "pdl": programmatic dependent launch of the graph's kernels (common.cuh)
   bool decode_only = false;           // option "decode_only": classification heads return decoded fields, logits are never written
@@ -188,7 +186,7 @@ struct pf_engine {
   std::unordered_map<MapKey, CUtensorMap, MapKeyHash> map_cache;
   bool use_stem_tc = true;    // 7x7 stems as patch gather + TMA GEMM (option "stem_tc"; 0 = fp32 CUDA-core direct convolution)
   bool use_attn_mma = true;   // tensor-core attention core (option "attn_mma"; 0 = CUDA-core fp32 kernel)
-  int sm_count = 148;
+  int sm_count = 132;
   bool profile = false;
   struct ProfRec { cudaEvent_t a, b; double flops; int cfg; int M, N, K, KH, stride, groups, Cin; };
   std::vector<ProfRec> prof;
@@ -423,9 +421,6 @@ struct Fwd {
   const char* map2d(CUtensorMap* m, const void* base, long long cols, long long rows, long long ld, int box_rows, int kb) {
     return cached_map(m, pf_engine::MapKey{base, cols, rows, ld, 0, box_rows, kb}, [&](CUtensorMap* o) { return tma_map_2d(o, base, cols, rows, ld, box_rows, kb); });
   }
-  const char* map_tile32(CUtensorMap* m, const void* base, long long rows, long long ld, bool f32) {
-    return cached_map(m, pf_engine::MapKey{base, rows, ld, 0, f32 ? 1 : 2, 32, 0}, [&](CUtensorMap* o) { return tma_map_tile32(o, base, rows, ld, f32); });
-  }
   const char* map_halo(CUtensorMap* m, const void* base, int B, int H, int W, int ld) {
     return cached_map(m, pf_engine::MapKey{base, ((long long)B << 32) | (unsigned)H, W, ld, 3, 0, 0}, [&](CUtensorMap* o) { return tma_map_halo(o, base, B, H, W, ld); });
   }
@@ -436,53 +431,18 @@ struct Fwd {
     TmaGemmParams p{};
     p.M = (int)M; p.Cin = K; p.N = N; p.K = K; p.a_c0 = a_c0; p.groups = 1;
     fill_epi(p, w, o, 0);
-    if (const char* d = getenv("PF_GEMM_DBG")) p.dbg = atoi(d);      // timing experiments only (gemm_tma.cuh: TmaGemmParams::dbg)
     TmaMaps maps{};
     const int bn = tma_pick_bn_gemm(M, N, K, e->sm_count);
-    // CTA-pair kernel (256 x BN tiles, tcgen05.mma.cta_group::2: half the weight traffic per SM) when there are enough pair tiles
-    const int pair_clusters = (e->use_pair && !getenv("PF_NO_PAIR")) ? gemm2_plan(e->device, (int)M, N, bn) : 0;
-    const int kb = pair_clusters ? 32 : tma_pick_kb(bn, K, MODE_GEMM);
+    const int kb = tma_pick_kb(bn, K, MODE_GEMM);
     const char* msg = nullptr;
     if (!msg) msg = map2d(&maps.a_hi, A.hi, A.ld, M, A.ld, 128, kb);
     if (!msg) msg = map2d(&maps.a_lo, A.lo, A.ld, M, A.ld, 128, kb);
-    if (!msg) msg = map2d(&maps.b_hi, w.hi, K, N, K, pair_clusters ? bn / 2 : bn, kb);
-    if (!msg) msg = map2d(&maps.b_lo, w.lo, K, N, K, pair_clusters ? bn / 2 : bn, kb);
-    // epilogue tiles go through TMA as well: fp32 output, or (when there is no fp32 output) the split planes; residual
-    if (o.C && o.S.hi) return fail(PF_ERR_ARG, "tgemm: fp32 and split outputs together are not supported in GEMM mode");
+    if (!msg) msg = map2d(&maps.b_hi, w.hi, K, N, K, bn, kb);
+    if (!msg) msg = map2d(&maps.b_lo, w.lo, K, N, K, bn, kb);
     if (o.res2 || o.bias_mode == 2) return fail(PF_ERR_ARG, "tgemm: second residual / border-class bias are halo-mode features");
-    if (!msg && o.C) msg = map_tile32(&maps.c, o.C, M, o.ldc, true);
-    if (!msg && o.S.hi) msg = map_tile32(&maps.s_hi, o.S.hi, M, o.S.ld, false);
-    if (!msg && o.S.hi) msg = map_tile32(&maps.s_lo, o.S.lo, M, o.S.ld, false);
-    if (!msg && o.res) msg = map_tile32(&maps.res, o.res, M, o.ldr, true);
     if (msg) return fail(PF_ERR_CUDA, "%s", msg);
     maps.a2_hi = maps.a_hi; maps.a2_lo = maps.a_lo;
-    if (!o.C) maps.c = maps.a_hi;
-    if (!o.S.hi) { maps.s_hi = maps.a_hi; maps.s_lo = maps.a_hi; }
-    if (!o.res) maps.res = maps.a_hi;
-    if (pair_clusters) return launch_pair(maps, p, bn, pair_clusters);
     return launch_tma(MODE_GEMM, maps, p);
-  }
-  static cudaError_t gemm_tma_pair_mode(const TmaMaps& maps, const TmaGemmParams& p, int bn, int nclusters, cudaStream_t st) {
-    return gemm2_launch(maps, p, bn, nclusters, st);
-  }
-  int launch_pair(const TmaMaps& maps, const TmaGemmParams& p, int bn, int nclusters) {
-    if (e->profile) {
-      pf_engine::ProfRec r{};
-      for (cudaEvent_t* ev : {&r.a, &r.b}) {
-        if (e->ev_pool.empty()) { CU(cudaEventCreate(ev)); }
-        else { *ev = e->ev_pool.back(); e->ev_pool.pop_back(); }
-      }
-      r.flops = 2.0 * (double)p.M * (double)p.N * (double)p.K;
-      r.cfg = 5;
-      r.M = p.M; r.N = p.N; r.K = p.K; r.KH = 1; r.stride = 2; r.groups = 1; r.Cin = p.Cin;   // (stride 2 marks pair launches in the CSV)
-      CU(cudaEventRecord(r.a, st));
-      LAUNCHED(gemm_tma_pair_mode(maps, p, bn, nclusters, st));
-      CU(cudaEventRecord(r.b, st));
-      e->prof.push_back(r);
-      return PF_OK;
-    }
-    LAUNCHED(gemm_tma_pair_mode(maps, p, bn, nclusters, st));
-    return PF_OK;
   }
   // 3x3 / stride 1 / pad 1 convolution on split NHWC planes (optionally a second source for channels >= c_split)
   int thalo(const SplitT& A, int a_c0, int a_gc, const SplitT* A2, int c_split, int a2_c0, int B, int H, int W, int Cin, const GemmW& w, int N,
@@ -493,7 +453,6 @@ struct Fwd {
     p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.N = N; p.K = 9 * Cin; p.a_c0 = a_c0; p.a_gc = a_gc; p.groups = groups;
     p.c_split = A2 ? c_split : 0; p.a2_c0 = a2_c0;
     fill_epi(p, w, o, bias_gstride);
-    if (const char* d = getenv("PF_HALO_DBG")) p.dbg = atoi(d);      // timing experiments only (gemm_tma.cuh: TmaGemmParams::dbg)
     TmaMaps maps{};
     const int bn = tma_pick_bn(N, MODE_HALO), kb = tma_pick_kb(bn, p.K, MODE_HALO);
     const char* msg = nullptr;
@@ -505,7 +464,6 @@ struct Fwd {
     } else { maps.a2_hi = maps.a_hi; maps.a2_lo = maps.a_lo; }
     if (!msg) msg = map2d(&maps.b_hi, w.hi, p.K, (long long)groups * N, p.K, bn, kb);
     if (!msg) msg = map2d(&maps.b_lo, w.lo, p.K, (long long)groups * N, p.K, bn, kb);
-    maps.c = maps.a_hi; maps.s_hi = maps.a_hi; maps.s_lo = maps.a_hi; maps.res = maps.a_hi;   // halo mode: epilogue stores from registers
     if (msg) return fail(PF_ERR_CUDA, "%s", msg);
     return launch_tma(MODE_HALO, maps, p, pred);
   }
@@ -527,20 +485,6 @@ struct Fwd {
   int ln_split(const float* x, const SplitT& y, long long rows, int C, const LnW& w, float eps, float* yf = nullptr) {
     if (dry) return PF_OK;
     LAUNCHED(layernorm_launch(x, yf, rows, C, w.w, w.b, eps, st, y));
-    return PF_OK;
-  }
-  // attention core on tcgen05: q [n*N, C] and kv [n*100, 2C] split planes -> a split planes
-  int attention_tc(const SplitT& q, const SplitT& kv, const SplitT& a, int nimg, int N, int C, int heads) {
-    if (dry) return PF_OK;
-    if (q.ld != C || kv.ld != 2 * C || a.ld != C || C != heads * kAtcD) return fail(PF_ERR_ARG, "attention_tc: layout");
-    AtcMaps maps{};
-    const char* msg = nullptr;
-    if (!msg) msg = map2d(&maps.q_hi, q.hi, C, (long long)nimg * N, C, 128, 64);
-    if (!msg) msg = map2d(&maps.q_lo, q.lo, C, (long long)nimg * N, C, 128, 64);
-    if (!msg) msg = map2d(&maps.kv_hi, kv.hi, 2 * C, (long long)nimg * kAtcKeys, 2 * C, kAtcKeysPad, 64);
-    if (!msg) msg = map2d(&maps.kv_lo, kv.lo, 2 * C, (long long)nimg * kAtcKeys, 2 * C, kAtcKeysPad, 64);
-    if (msg) return fail(PF_ERR_CUDA, "%s", msg);
-    LAUNCHED(attention_tc_launch(maps, a.hi, a.lo, nimg, N, C, heads, e->sm_count, st));
     return PF_OK;
   }
   // LayerNorm whose output is (also) written in patch order for a k = s = sr convolution on the R x R map (y may be empty)
@@ -723,7 +667,7 @@ static int fwd_tails_post(Fwd& F, const pf_batch* bt, const float* conv1_out, Po
 }
 
 // =============================================================================================== TMA forward graph
-// Same network as run_forward, on the TMA -> tcgen05 engine: every GEMM input is a pre-split bf16 hi/lo tensor written by
+// Same network as run_forward, on the TMA -> wgmma engine: every GEMM input is a pre-split bf16 hi/lo tensor written by
 // its producer (LayerNorm, attention, depthwise conv, upsample, stem, or the previous GEMM's epilogue).
 static int run_forward_tma(Fwd& F, const pf_batch* bt) {
   pf_engine* e = F.e;
@@ -803,7 +747,7 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
       Epi oq, okv;
       if (qkv_split) { oq.S = q; okv.S = kv; } else { oq.C = qf; oq.ldc = C; okv.C = kvf; okv.ldc = 2 * C; }
       // q and the spatial-reduction branch both depend on LayerNorm 1 only: fork the branch onto the engine's side stream (its
-      // GEMMs have 50-75 tiles for 148 SMs; q's second, partial wave leaves SMs idle as well) and join before the attention core
+      // GEMMs have 50-75 tiles for 132 SMs; q's second, partial wave leaves SMs idle as well) and join before the attention core
       const bool fork = !dry && sr > 1 && e->use_fork && e->side && !e->kp.on && !e->profile && !sync_debug() && !e->debug;
       if (fork) {
         CU(cudaEventRecord(e->ev_fork, st));
@@ -825,9 +769,7 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
       } else {
         TRY(F.tgemm(t1, rows, C, 0, b.kv, 2 * C, okv));
       }
-      if (qkv_split && e->use_attn_tc) {
-        TRY(F.attention_tc(q, kv, a, n, N, C, heads));
-      } else if (!dry) {
+      if (!dry) {
         if (qkv_split) LAUNCHED(attention_mma_launch(nullptr, nullptr, nullptr, n, N, C, heads, st, a, q, kv));
         else if (e->use_attn_mma) LAUNCHED(attention_mma_launch(qf, kvf, nullptr, n, N, C, heads, st, a));
         else LAUNCHED(attention_launch(qf, kvf, nullptr, n, N, C, heads, st, a));
@@ -998,13 +940,7 @@ static int configure_device(int device) {
   std::lock_guard<std::mutex> lock(mu);
   if (device < (int)done.size() && done[device]) return PF_OK;
   CU(gemm_tma_configure_device());
-  {
-    cudaDeviceProp prop;
-    CU(cudaGetDeviceProperties(&prop, device));
-    CU(gemm2_configure_device(device, prop.multiProcessorCount));
-  }
   CU(attention_mma_configure_device());
-  CU(attention_tc_configure_device());
   CU(cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem));
   CU(cudaFuncSetAttribute(conv1_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kRingSmem));
   CU(cudaFuncSetAttribute(preprocess_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPreMaxSmemRows * kNet * 3));
@@ -1031,7 +967,7 @@ int pf_create(int device, const pf_model_desc* desc, pf_handle* out) {
   CU(cudaSetDevice(device));
   cudaDeviceProp prop;
   CU(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) return fail(PF_ERR_CUDA, "pf_create: device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) return fail(PF_ERR_CUDA, "pf_create: device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major, prop.minor);
   TRY(configure_device(device));
   pf_engine* e = new pf_engine();
   e->device = device;
@@ -1198,9 +1134,7 @@ int pf_set_option(pf_handle h, const char* name, int value) {
   if (!strcmp(name, "decode_only")) { h->decode_only = value != 0; return PF_OK; }
   if (!strcmp(name, "pdl")) { h->use_pdl = value != 0; return PF_OK; }
   if (!strcmp(name, "dw_ln")) { h->use_dwln = value != 0; return PF_OK; }
-  if (!strcmp(name, "pair")) { h->use_pair = value != 0; return PF_OK; }
   if (!strcmp(name, "fork")) { h->use_fork = value != 0; return PF_OK; }
-  if (!strcmp(name, "attn_tc")) { h->use_attn_tc = value != 0; return PF_OK; }
   return fail(PF_ERR_ARG, "pf_set_option: unknown option '%s'", name);
 }
 // out[cfg*3 + {0,1,2}] = {milliseconds, algorithmic FLOPs, launches} per GEMM engine configuration (7 configs),
@@ -1209,7 +1143,7 @@ int pf_profile_read(pf_handle h, double* out9) {
   if (!h || !out9) return fail(PF_ERR_ARG, "pf_profile_read: null argument");
   for (int i = 0; i < 21; ++i) out9[i] = 0.0;
   FILE* csv = nullptr;
-  if (const char* path = getenv("PF_PROFILE_CSV")) {   // optional per-launch dump (profiles/)
+  if (const char* path = getenv("PF_PROFILE_CSV")) {   // optional per-launch dump
     csv = fopen(path, "w");
     if (csv) fprintf(csv, "engine_cfg,M,N,K,Cin,KH,stride,groups,ms,algorithmic_tflops\n");
   }
@@ -1522,7 +1456,7 @@ int pf_op_postprocess(const float* vec, const float* lat, int n, const int32_t* 
 
 int pf_op_fill_stream(float* dst, int64_t numel, float value, void* stream) {
   if (!dst || numel < 4 || (numel & 3) || ((uintptr_t)dst & 15)) return fail(PF_ERR_ARG, "pf_op_fill_stream: bad argument");
-  LAUNCHED((fill_stream_kernel<<<148 * 16, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<float4*>(dst), numel / 4, value), cudaGetLastError()));
+  LAUNCHED((fill_stream_kernel<<<132 * 16, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<float4*>(dst), numel / 4, value), cudaGetLastError()));
   return PF_OK;
 }
 int pf_op_layernorm(const float* x, float* y, int64_t rows, int C, const float* w, const float* b, float eps, void* stream) {
@@ -1542,7 +1476,7 @@ int pf_op_attention_mma(const float* q, const float* kv, float* out, int B, int 
   return PF_OK;
 }
 int pf_op_attention_tc(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream) {
-  if (!q || !kv || !out || C != heads * kAtcD) return fail(PF_ERR_ARG, "pf_op_attention_tc: head_dim must be 64");
+  if (!q || !kv || !out || C != heads * kAmD) return fail(PF_ERR_ARG, "pf_op_attention_tc: head_dim must be 64");
   TRY(configure_current_device());
   cudaStream_t st = (cudaStream_t)stream;
   int dev = 0;
@@ -1552,17 +1486,20 @@ int pf_op_attention_tc(const float* q, const float* kv, float* out, int B, int N
   pf_engine tmp;
   tmp.device = dev;
   tmp.sm_count = prop.multiProcessorCount;
-  const long long nq = (long long)B * N * C, nkv = (long long)B * kAtcKeys * 2 * C;
+  const long long nq = (long long)B * N * C, nkv = (long long)B * kAmKeys * 2 * C;
   char* scratch = nullptr;
   CU(cudaMalloc(&scratch, (2 * nq + nkv) * 4 + 8192));
   Fwd F{&tmp, Arena{}, st, false, B};
   F.ar.base = scratch; F.ar.cap = (2 * nq + nkv) * 4 + 8192;
-  SplitT qs = F.salloc((long long)B * N, C), kvs = F.salloc((long long)B * kAtcKeys, 2 * C), as = F.salloc((long long)B * N, C);
+  SplitT qs = F.salloc((long long)B * N, C), kvs = F.salloc((long long)B * kAmKeys, 2 * C), as = F.salloc((long long)B * N, C);
   int r = PF_OK;
   cudaError_t le = (split_kernel<<<(unsigned)cdivl(nq, 256), 256, 0, st>>>(q, qs.hi, qs.lo, nq, 0), cudaGetLastError());
   if (le == cudaSuccess) le = (split_kernel<<<(unsigned)cdivl(nkv, 256), 256, 0, st>>>(kv, kvs.hi, kvs.lo, nkv, 0), cudaGetLastError());
   if (le != cudaSuccess) r = fail(PF_ERR_CUDA, "split_kernel: %s", cudaGetErrorString(le));
-  if (r == PF_OK) r = F.attention_tc(qs, kvs, as, B, N, C, heads);
+  if (r == PF_OK) {
+    le = attention_mma_launch(nullptr, nullptr, nullptr, B, N, C, heads, st, as, qs, kvs);
+    if (le != cudaSuccess) r = fail(PF_ERR_CUDA, "attention_mma_launch: %s", cudaGetErrorString(le));
+  }
   if (r == PF_OK) {
     le = (merge_split_kernel<<<(unsigned)cdivl(nq, 256), 256, 0, st>>>(as.hi, as.lo, out, nq), cudaGetLastError());
     if (le != cudaSuccess) r = fail(PF_ERR_CUDA, "merge_split_kernel: %s", cudaGetErrorString(le));

@@ -176,8 +176,8 @@ __device__ __forceinline__ float fast_asinf(float x) {
 // rows as ONE float4 in shared memory; then every thread produces 4 consecutive output pixels of one row from two 16-byte
 // shared-memory taps per pixel (per-column index / weight tables, built once per block), normalises the up-vector
 // (v * rsqrt(max(|v|^2, 1e-24)) == v / max(|v|, 1e-12)), applies asin + rad2deg and writes three 16-byte streaming stores.
-// Measured before this version (ncu, profiles/r02_notes.md): 160 instructions per pixel, issue slots 70 % busy, DRAM 15 %:
-// instruction-bound; this version needs ~45 and is bound by its 12 B/pixel of stores.
+// A straightforward version needs ~160 instructions per pixel and is instruction-bound; this one needs ~45 and is bound by
+// its 12 B/pixel of stores.
 // The interpolation is evaluated as hx * (hy v00 + ly v10) + lx * (hy v01 + ly v11): ATen's bilinear kernel nests the two axes the
 // other way round (same weights, same products; the results differ by fp32 rounding only, ~1e-7 relative).
 constexpr int kPostRows = 4, kPostBand = 16, kPostThreads = 256, kPostMaxW = 3072;   // (static 20.6 KB + 8 B per column <= 48 KB)
@@ -314,9 +314,8 @@ __device__ __forceinline__ float fast_atan2_deg(float y, float h) {
 // One thread = 4 consecutive pixels of one row.  The pixel -> ray map is linear: its three world components are evaluated in
 // float64 for the thread's FIRST pixel (x_j = linspace sample: 1e-16 relative, like the numpy reference), rounded to float32
 // and advanced by float32 steps for the other three (the steps are ~1/f: their rounding is 1e-10 absolute); square root,
-// division and arctangent are float32 (fast_atan2_deg).  History (ncu, profiles/r02_notes.md): float64 sqrt / divide / atan2 per
-// pixel: 0.11 of the HBM roofline; float64 linear forms + float32 transcendentals: 0.35, the XU pipe (conversions, MUFU) 68 %
-// busy with ~10 conversions / special-function operations per pixel; this version issues ~4.5.
+// division and arctangent are float32 (fast_atan2_deg): float64 square roots, divisions and arctangents per pixel would make
+// the kernel bound by conversions and special-function operations instead of its stores.
 __global__ void __launch_bounds__(256) camera_fields_kernel(const __grid_constant__ CamBatch batch, float* __restrict__ up, float* __restrict__ lat) {
   const CamImage& c = batch.im[blockIdx.y];
   const int W4 = (c.W + 3) >> 2;

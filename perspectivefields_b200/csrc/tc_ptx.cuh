@@ -1,5 +1,5 @@
-// tcgen05 / TMEM / mbarrier PTX wrappers and the descriptor helpers shared by the sm_100a tensor-core kernels
-// (gemm_tma.cuh: persistent TMA -> tcgen05 -> TMEM engine; fused_mlp.cuh).
+// wgmma / mbarrier PTX wrappers and the shared-memory matrix descriptors of the sm_90a tensor-core kernels
+// (gemm_tma.cuh: persistent TMA -> wgmma engine).
 //
 // Every mbarrier wait is bounded (clock64 watchdog -> __trap) so that a protocol bug aborts the launch instead of
 // hanging the device.
@@ -8,24 +8,19 @@
 
 namespace pf {
 
-// Instruction descriptor of tcgen05.mma.kind::f16: fp32 accumulate (bits 4-5 = 1), A / B = bf16 (bits 7-9, 10-12 = 1), both
-// K-major, N >> 3 at bit 17, M >> 4 at bit 24 (M = 128 rows per CTA).
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-
-// Halo tile of the 3x3 / stride 1 / pad 1 convolutions: a CTA owns a 16 x 8 output-pixel tile (128 = UMMA M) and stages the
-// 18 x 10 input halo of one 64-channel chunk once in shared memory (bf16 hi + lo planes, 128 B per pixel, SWIZZLE_128B applied
-// on absolute address bits).  The A operand of filter tap (ky, kx) is a SHIFTED VIEW of that pixel array:
+// Halo tile of the 3x3 / stride 1 / pad 1 convolutions: a CTA owns a 16 x 8 output-pixel tile (128 rows, two wgmma M = 64
+// halves of 8 image rows each) and stages the 18 x 10 input halo of one 64-channel chunk once in shared memory (bf16 hi + lo
+// planes, 128 B per pixel, SWIZZLE_128B).  The A operand of filter tap (ky, kx) is a SHIFTED VIEW of that pixel array:
 //     start address = plane + (ky*10 + kx) * 128 B,   8-row groups (= 8 pixels of one image row) SBO = 10 * 128 B apart
-// (descriptor semantics verified on hardware with tools/tc_probe.cu: base_offset 0, arbitrary 128 B-aligned start and SBO work
-// because the swizzle is a function of the absolute shared-memory address).
+// The swizzle is a function of the absolute shared-memory address on both sides (TMA writes and wgmma reads), so a view that
+// starts at any 128 B boundary reads the pattern the TMA wrote with base offset 0 (checked on H100: setting the base offset to
+// (start >> 7) & 7 gives wrong halo convolutions).
 constexpr int kHtTileH = 16, kHtTileW = 8;                 // output tile (rows x cols) = 128 pixels
 constexpr int kHtHaloW = kHtTileW + 2, kHtHaloH = kHtTileH + 2;
 constexpr int kHtHaloPix = kHtHaloW * kHtHaloH;            // 180
 constexpr int kHtPlaneBytes = 23 * 1024;                   // 180 x 128 B rounded up to a 1024 B multiple
 
-// ------------------------------------------------------------------------------------------- PTX wrappers
+// ------------------------------------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(bar), "r"(count) : "memory");
 }
@@ -45,54 +40,55 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     if (clock64() - t0 > 4000000000LL) __trap();  // ~2 s: protocol bug, abort instead of hanging the GPU
   }
 }
-// pure polling variant (mbarrier.test_wait never suspends the thread): for the single-lane producer / MMA-issuer loops, where the
-// wake-up latency of a suspended try_wait would sit on the critical path of every pipeline stage
-__device__ __forceinline__ uint32_t mbar_test_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile("{\n\t.reg .pred p;\n\tmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
-               : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-  return ok;
-}
-__device__ __forceinline__ void mbar_wait_spin(uint32_t bar, uint32_t parity) {
-  if (mbar_test_wait(bar, parity)) return;
-  const long long t0 = clock64();
-  while (!mbar_test_wait(bar, parity)) {
-    if (clock64() - t0 > 4000000000LL) __trap();
-  }
-}
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
 __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }
+// named barrier over `count` threads (id 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(count) : "memory"); }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_slot, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_slot), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 x bf16 -> fp32
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-               ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-                 "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-                 "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-                 "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-               : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
+// ------------------------------------------------------------------------------------------- wgmma
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of accumulator registers across the asynchronous MMAs that own them
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// K-major SWIZZLE_128B descriptor for the halo view: 128 B rows, 8-row groups kHtHaloW * 128 B apart.
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, bf16 operands from shared-memory descriptors (both K-major), fp32 accumulators in the
+// registers of the issuing warpgroup.  scale_d = 0 overwrites D.
+#define PF_R8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+__device__ __forceinline__ void wgmma_n64(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
+      "%32, %33, p, 1, 1, 0, 0;\n\t}\n"
+      : PF_R8(0), PF_R8(8), PF_R8(16), PF_R8(24)
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_n32(float* d, uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}\n"
+      : PF_R8(0), PF_R8(8)
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
+}
+#undef PF_R8
+
+// K-major SWIZZLE_128B (kb = 64: 128 B rows, 8-row groups 1024 B apart) or SWIZZLE_64B (kb = 32: 64 B rows, 512 B apart) descriptor
+// of a tile that starts on a swizzle-pattern boundary.  Advancing K by 16 elements is +32 B of start address (+2 in the field).
+template <int KB>
+__device__ __forceinline__ uint64_t wgmma_tile_desc(uint32_t smem_addr) {
+  constexpr uint64_t sbo = KB == 32 ? 512 : 1024, layout = KB == 32 ? 2 : 1;
+  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | ((uint64_t)1 << 16) | ((sbo >> 4) << 32) | (layout << 62);
+}
+// halo view: 128 B rows, SWIZZLE_128B, 8-row groups kHtHaloW * 128 B apart, start anywhere on a 128 B boundary
 __device__ __forceinline__ uint64_t ht_a_desc(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | ((uint64_t)1 << 16) | ((uint64_t)((kHtHaloW * 128) >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
+  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | ((uint64_t)1 << 16) | ((uint64_t)((kHtHaloW * 128) >> 4) << 32) |
+         ((uint64_t)1 << 62);
 }
 
 }  // namespace pf

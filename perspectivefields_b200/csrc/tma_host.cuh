@@ -8,8 +8,6 @@
 #include <string>
 
 #include "gemm_tma.cuh"
-#include "gemm2_tma.cuh"
-#include "attention_tc.cuh"
 
 namespace pf {
 
@@ -44,22 +42,6 @@ inline const char* tma_map_2d(CUtensorMap* m, const void* base, long long cols, 
   return r == CUDA_SUCCESS ? nullptr : "cuTensorMapEncodeTiled (2d) failed";
 }
 
-// 32-row x 32-column epilogue tile of a row-major [rows][ld] tensor: fp32 (128 B rows, SWIZZLE_128B) or bf16 (64 B, SWIZZLE_64B)
-inline const char* tma_map_tile32(CUtensorMap* m, const void* base, long long rows, long long ld, bool is_f32) {
-  PFN_tensorMapEncodeTiled enc = tma_encoder();
-  if (!enc) return "cuTensorMapEncodeTiled entry point not available";
-  const int es_bytes = is_f32 ? 4 : 2;
-  cuuint64_t dims[2] = {(cuuint64_t)ld, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * es_bytes};
-  cuuint32_t box[2] = {32, 32};
-  cuuint32_t es[2] = {1, 1};
-  if (((uintptr_t)base & 15) || (strides[0] & 15)) return "tma_map_tile32: alignment";
-  CUresult r = enc(m, is_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, is_f32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? nullptr : "cuTensorMapEncodeTiled (tile32) failed";
-}
-
 // bf16 NHWC tensor [B][H][W][ld]; box = 1 x 18 x 10 x 64 channels (128 B), SWIZZLE_128B: one halo chunk.
 inline const char* tma_map_halo(CUtensorMap* m, const void* base, int B, int H, int W, int ld) {
   PFN_tensorMapEncodeTiled enc = tma_encoder();
@@ -82,22 +64,22 @@ inline int tma_pick_bn(int N, int mode) {
   return bn;
 }
 
-// GEMM mode with the number of rows known.  The widest tile moves the fewest operand bytes per output column (GEMM mode is bound
-// by L2 -> shared-memory operand traffic: about 1.6 clk per operand row and K step of 16 on a full machine, measured -- a 128 x 256
-// tile costs 614 clk per K step against 384 clk of MMA), so it wins whenever the tiles fill the machine.  A launch that leaves
-// most SMs idle (stage-4 / spatially reduced layers: 25 row tiles) is faster with narrower tiles spread over more SMs: pick the
-// width that minimises waves x time per tile in that model.  Results do not depend on the choice (same K order per output).
+// GEMM mode with the number of rows known.  The widest tile moves the fewest operand bytes per output column, so it wins whenever
+// the tiles fill the machine.  A launch that leaves most SMs idle (stage-4 / spatially reduced layers: 25 row tiles) is faster
+// with narrower tiles spread over more SMs: pick the width that minimises waves x time per tile, with a K step of 16 costing the
+// larger of its MMA time (3 products x 128 x BN x 16 at 4096 bf16 FLOP per clock and SM, the H100 SXM data-sheet peak) and
+// its operand loads (1.6 clk per operand row), plus a fixed ~3000 clk per tile.  Results do not depend on the choice (same K
+// order per output).
 inline int tma_pick_bn_gemm(long long M, int N, int K, int sm_count) {
   const int base = tma_pick_bn(N, MODE_GEMM);
-  static const int policy = getenv("PF_BN_POLICY") ? atoi(getenv("PF_BN_POLICY")) : 1;     // 0: always the widest tile (A/B runs)
   const long long mt = cdivl(M, 128);
-  if (!policy || mt * cdiv(N, base) * 4 > 3LL * sm_count) return base;
+  if (mt * cdiv(N, base) * 4 > 3LL * sm_count) return base;
   int best = base;
   double best_cost = 1e30;
   for (int bn = base; bn >= 32; bn -= 32) {
     const long long tiles = mt * cdiv(N, bn);
     const double waves = (double)cdivl(tiles, sm_count);
-    const double mma = 3.0 * (bn / 2 > 32 + bn / 4 ? bn / 2 : 32 + bn / 4), load = 1.6 * (128 + bn);
+    const double mma = 3.0 * bn, load = 1.6 * (128 + bn);
     const double cost = waves * ((K / 16) * (mma > load ? mma : load) + 3000.0);
     if (cost < best_cost - 1e-9) { best_cost = cost; best = bn; }
   }
@@ -105,10 +87,9 @@ inline int tma_pick_bn_gemm(long long M, int N, int K, int sm_count) {
 }
 
 // K elements per pipeline step: 64 for narrow tiles when K allows it (halo mode: BN <= 128; GEMM mode, whose stages also
-// hold the A tile and whose epilogue staging takes 72 KB: BN <= 64), else 32
+// hold the A tile: BN <= 64), else 32
 inline int tma_pick_kb(int bn, int K, int mode) {
-  static const int wide = getenv("PF_KB64") ? atoi(getenv("PF_KB64")) : 0;     // experiment: 128-byte TMA rows for wider GEMM-mode tiles
-  const int lim = mode == MODE_HALO ? 128 : (wide ? wide : 64);
+  const int lim = mode == MODE_HALO ? 128 : 64;
   return (bn <= lim && K % 64 == 0) ? 64 : 32;
 }
 
@@ -149,7 +130,6 @@ inline cudaError_t gemm_tma_launch_bn(const TmaMaps& maps, const TmaGemmParams& 
 #define PF_TMA_VARIANTS(X)                                                                                                  \
   X(256, MODE_GEMM, 32) X(224, MODE_GEMM, 32) X(192, MODE_GEMM, 32) X(160, MODE_GEMM, 32) X(128, MODE_GEMM, 32) X(96, MODE_GEMM, 32) \
   X(64, MODE_GEMM, 32) X(32, MODE_GEMM, 32) X(64, MODE_GEMM, 64) X(32, MODE_GEMM, 64)                                        \
-  X(96, MODE_GEMM, 64) X(128, MODE_GEMM, 64) X(160, MODE_GEMM, 64)                                                           \
   X(256, MODE_HALO, 32) X(128, MODE_HALO, 64) X(64, MODE_HALO, 64) X(32, MODE_HALO, 64)
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a per-device (per-context) attribute: called once for every device an engine is
@@ -161,78 +141,6 @@ inline cudaError_t gemm_tma_configure_device() {
   PF_TMA_VARIANTS(PF_TMA_CFG)
 #undef PF_TMA_CFG
   return e;
-}
-
-// ---- attention core on tcgen05 (attention_tc.cuh)
-inline cudaError_t attention_tc_configure_device() {
-  return cudaFuncSetAttribute(attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAtcSmemBytes);
-}
-inline cudaError_t attention_tc_launch(const AtcMaps& maps, __nv_bfloat16* ohi, __nv_bfloat16* olo, int B, int N, int C, int heads, int sm_count,
-                                       cudaStream_t st) {
-  const int total = B * heads * cdiv(N, 128);
-  int grid = total < sm_count ? total : sm_count;
-  const int ipc = cdiv(total, grid);          // contiguous items per CTA: K / V of an (image, head) are loaded once per CTA that touches it
-  grid = cdiv(total, ipc);
-  return launch_pdl(attention_tc_kernel, dim3(grid), dim3(kAtcThreads), kAtcSmemBytes, st, maps, ohi, olo, B, N, C, heads, total, ipc);
-}
-
-// ---- CTA-pair GEMM (gemm2_tma.cuh): cluster 2x1x1, one pair per TPC
-#define PF_TMA2_VARIANTS(X) X(256) X(224) X(192) X(160) X(128) X(96) X(64)
-
-struct Gemm2Info { int max_clusters[9]; };   // index BN / 32: concurrently resident pairs on this device (0 = not available)
-inline Gemm2Info& gemm2_info(int device) {
-  static Gemm2Info info[64];
-  return info[device & 63];
-}
-inline cudaError_t gemm2_configure_device(int device, int sm_count) {
-  cudaError_t e = cudaSuccess;
-  Gemm2Info& gi = gemm2_info(device);
-#define PF_TMA2_CFG(BN_)                                                                                                      \
-  if (e == cudaSuccess) {                                                                                                     \
-    e = cudaFuncSetAttribute(gemm2_tma_kernel<BN_>, cudaFuncAttributeMaxDynamicSharedMemorySize, Tma2Cfg<BN_>::kSmemBytes);   \
-    if (e == cudaSuccess) {                                                                                                   \
-      cudaLaunchConfig_t cfg{};                                                                                               \
-      cfg.gridDim = dim3(sm_count & ~1); cfg.blockDim = dim3(kTmaThreads); cfg.dynamicSmemBytes = Tma2Cfg<BN_>::kSmemBytes;   \
-      cudaLaunchAttribute at[1];                                                                                              \
-      at[0].id = cudaLaunchAttributeClusterDimension;                                                                         \
-      at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;                                     \
-      cfg.attrs = at; cfg.numAttrs = 1;                                                                                       \
-      int n = 0;                                                                                                              \
-      if (cudaOccupancyMaxActiveClusters(&n, gemm2_tma_kernel<BN_>, &cfg) != cudaSuccess) { n = 0; (void)cudaGetLastError(); } \
-      gi.max_clusters[BN_ / 32] = n;                                                                                          \
-    }                                                                                                                         \
-  }
-  PF_TMA2_VARIANTS(PF_TMA2_CFG)
-#undef PF_TMA2_CFG
-  return e;
-}
-
-template <int BN>
-inline cudaError_t gemm2_launch_bn(const TmaMaps& maps, const TmaGemmParams& p, int nclusters, cudaStream_t st) {
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(2 * nclusters); cfg.blockDim = dim3(kTmaThreads); cfg.dynamicSmemBytes = Tma2Cfg<BN>::kSmemBytes; cfg.stream = st;
-  cudaLaunchAttribute at[2];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-  at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = pdl_enabled() ? 2 : 1;
-  return cudaLaunchKernelEx(&cfg, gemm2_tma_kernel<BN>, maps, p);
-}
-// pair tiles of this problem and the number of clusters to launch (0: use the single-CTA kernel)
-inline int gemm2_plan(int device, int M, int N, int bn) {
-  const int avail = gemm2_info(device).max_clusters[bn / 32];
-  if (avail < 1 || bn < 64) return 0;
-  const long long tiles = (long long)cdiv(M, 256) * cdiv(N, bn);
-  if (tiles < avail) return 0;              // too few pair tiles to cover the machine once: 128-row tiles spread better
-  return avail;
-}
-inline cudaError_t gemm2_launch(const TmaMaps& maps, const TmaGemmParams& p, int bn, int nclusters, cudaStream_t st) {
-#define PF_TMA2_CASE(BN_) if (bn == BN_) return gemm2_launch_bn<BN_>(maps, p, nclusters, st);
-  PF_TMA2_VARIANTS(PF_TMA2_CASE)
-#undef PF_TMA2_CASE
-  return cudaErrorInvalidValue;
 }
 
 inline cudaError_t gemm_tma_launch(int mode, const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, int sm_count, cudaStream_t st,

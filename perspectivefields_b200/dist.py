@@ -1,5 +1,5 @@
 """Multi-GPU ``inference_batch`` (SURVEY.md section 8e): one process per GPU (``torch.distributed`` for the rendezvous; NCCL over
-NVLink on a B200 box, gloo in the CPU tests).  The path has no cross-image dependency, so the list is sharded in contiguous
+NVLink on a multi-GPU box, gloo in the CPU tests).  The path has no cross-image dependency, so the list is sharded in contiguous
 chunks, every rank runs the ordinary single-GPU path on its shard in micro-batches, and the results are gathered to ONE rank so
 that the caller gets the ``list[dict]`` a single-GPU call would return -- bit-identical per image, tensors on that rank's device
 (where the reference would have put them).
@@ -151,7 +151,7 @@ def inference_batch_sharded(model, img_bgr_list, gather_to=0, group=None, micro_
 
     The receives of a round are posted only after the gathering rank's OWN forward of that round has finished: an NCCL receive
     kernel posted earlier would sit on its SMs spinning for the peers' data while the forward's persistent kernels (one
-    225 KB-shared-memory CTA per SM) need every SM (measured: +30 % on the root's step, profiles/r02_notes.md).
+    225 KB-shared-memory CTA per SM) need every SM.
 
     ``model`` provides ``infer_raw(imgs) -> raw`` (the five output blobs of one micro-batch + host metadata),
     ``assemble_raw(raw) -> list[dict]`` and ``out_classes()`` (``PerspectiveFields`` does)."""

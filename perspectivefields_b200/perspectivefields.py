@@ -1,11 +1,11 @@
 """Drop-in for ``perspective2d.PerspectiveFields`` (reference: perspective2d/perspectivefields.py:121-272) whose
-whole forward runs in libpf_b200.so (hand-written sm_100a CUDA, C ABI in include/pf_b200.h).
+whole forward runs in libpf_b200.so (hand-written sm_90a CUDA, C ABI in include/pf_b200.h).
 
 Kept from the reference surface: ``PerspectiveFields(version)``, ``.eval()``, ``.cuda()/.to()``, ``.device``,
 ``.versions()``, ``.inference(img_bgr)``, ``.inference_batch(list)``, ``.forward(batched_inputs)``,
 ``.state_dict()/.load_state_dict()`` with the reference's key names, attributes ``version``, ``param_on``, ``cfg``,
 ``input_format``; result dictionaries with the same keys, order, shapes and dtypes.  There is no CPU path: the model
-must live on a CUDA device (B200) and libpf_b200.so must be built, otherwise inference raises.
+must live on a CUDA device (H100) and libpf_b200.so must be built, otherwise inference raises.
 """
 import ctypes
 
@@ -294,7 +294,7 @@ class PerspectiveFields(nn.Module):
     def _get_engine(self):
         dev = self.device
         if dev.type != "cuda":
-            raise RuntimeError("perspectivefields_b200 has no CPU path: move the model to a B200 with .cuda() first")
+            raise RuntimeError("perspectivefields_b200 has no CPU path: move the model to an H100 with .cuda() first")
         if dev.index is None:
             dev = torch.device("cuda", torch.cuda.current_device())
         if self._engine is None or self._engine.device != dev:
@@ -460,7 +460,7 @@ class PerspectiveFields(nn.Module):
         return res
 
     def set_option(self, name, value):
-        """Engine options (see pf_set_option in include/pf_b200.h), e.g. ``set_option("tcgen05", 1)``."""
+        """Engine options (see pf_set_option in include/pf_b200.h), e.g. ``set_option("pdl", 0)``."""
         eng = self._get_engine()
         _native.check(eng.L.pf_set_option(eng.handle, name.encode(), int(value)))
         self._options[name] = int(value)

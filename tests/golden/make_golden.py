@@ -7,7 +7,7 @@ TORCH_HOME hub cache, construct ``perspective2d.PerspectiveFields(version).eval(
 own loader (perspectivefields.py:178-192), run ``inference_batch`` on CPU fp32 on two synthetic images
 (480x640 uniform noise, 360x500 smooth), and store a strided sub-sample of every returned tensor together
 with float64 checksums.  The fixtures pin oracle/model.py to the reference (tests/test_oracle_golden.py)
-on machines where /root/reference does not exist.
+on machines without a checkout of the reference (PF_REFERENCE_ROOT names one).
 """
 import json
 import os

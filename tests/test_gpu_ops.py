@@ -1,5 +1,5 @@
 """GPU: every operator of libpf_b200.so, called through the C ABI, against a float64 torch restatement of the same op
-on the same seeded inputs (all GEMM-shaped operators run on the TMA -> tcgen05 engine, the only engine since ABI 2).  Tolerances: 5e-5 relative for the bf16x3 split-precision GEMM engine (per-product error
+on the same seeded inputs (all GEMM-shaped operators run on the TMA -> wgmma engine, the only engine since ABI 2).  Tolerances: 5e-5 relative for the bf16x3 split-precision GEMM engine (per-product error
 ~2^-17; the end-to-end bar is 1e-3), 1e-5 for fp32 CUDA-core ops, bit-exact for the integer resize."""
 import ctypes
 
@@ -132,7 +132,7 @@ def test_preprocess_is_bit_exact_vs_pillow(hw):
     assert np.array_equal(got[..., :3], ref) and not got[..., 3].any()
 
 
-# ---- more GEMM-mode / halo-mode shapes of the TMA -> tcgen05 engine
+# ---- more GEMM-mode / halo-mode shapes of the TMA -> wgmma engine
 TC_CASES = [
     (2, 20, 20, 256, 256, 3, 1, 1, 1, 1, 0, 0),     # RCU conv1
     (1, 23, 17, 256, 256, 3, 1, 1, 0, 0, 1, 1),     # RCU conv2 + relu(residual), ragged M (391 rows)
@@ -148,10 +148,10 @@ TC_CASES = [
     (1, 40, 40, 320, 64, 3, 1, 1, 0, 1, 0, 0),      # N tile 64, K = 2880
     (2, 40, 40, 64, 128, 3, 2, 1, 0, 0, 0, 0),      # N tile 128, stride 2
     (1, 1, 500, 64, 320, 1, 1, 0, 0, 0, 0, 0),      # N = 320 -> five 64-wide tiles
-    # CTA-pair kernel (gemm2_tma.cuh, tcgen05.mma.cta_group::2): taken when there are at least as many 256-row pair tiles as TPCs
-    (1, 1, 12800, 320, 320, 1, 1, 0, 0, 0, 1, 0),   # MiT stage-3 proj: 50 pairs x 2 N tiles of 160, + residual
-    (1, 1, 20000, 96, 384, 1, 1, 0, 0, 2, 0, 0),    # ragged M (78.1 pairs), GELU, 3 K steps
-    (1, 1, 19000, 1280, 320, 1, 1, 0, 0, 0, 1, 1),  # K = 1280 (the ring wraps many times), relu(residual), last pair half empty
+    # large GEMM-mode launches (several tiles per CTA of the persistent grid)
+    (1, 1, 12800, 320, 320, 1, 1, 0, 0, 0, 1, 0),   # MiT stage-3 proj: 100 row tiles x 2 N tiles of 160, + residual
+    (1, 1, 20000, 96, 384, 1, 1, 0, 0, 2, 0, 0),    # ragged M (156.25 row tiles), GELU, 3 K steps
+    (1, 1, 19000, 1280, 320, 1, 1, 0, 0, 0, 1, 1),  # K = 1280 (the ring wraps many times), relu(residual), last row tile partial
     (1, 1, 25000, 64, 640, 1, 1, 0, 0, 1, 0, 0),    # N = 640 -> three N tiles of 224 (last one partial), ReLU
     (1, 1, 40000, 128, 64, 1, 1, 0, 0, 0, 0, 0),    # narrow N = 64 (32 weight rows per CTA)
 ]
