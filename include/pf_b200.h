@@ -175,6 +175,51 @@ int pf_jpeg_decode_batch(pf_jpeg_handle j, int n, const uint8_t* const* data, co
 int pf_op_conv_gemm(const float* x, int B, int H, int W, int Cin, const void* whi, const void* wlo, const float* bias,
                     int N, int KH, int KW, int stride, int pad, int in_relu, int act, const float* res, int res_relu,
                     float* y, void* stream);
+/* One launch of the TMA -> wgmma engine with every epilogue feature the forward graph uses, on operands the caller has already
+ * split into bf16 hi/lo planes (DEVICE pointers).  Runs the forward's own helpers (map construction, tile dispatch, the
+ * per-group launch split), so a test reaches exactly what pf_forward launches.  Enqueued on `stream`, no synchronisation.
+ *   mode 0 (GEMM): C[M, N] = A[M, K] W[N, K]^T, one group; A rows of pitch lda, first column a_c0.
+ *   mode 1 (halo): 3x3 / stride 1 / pad 1 convolution of NHWC [B, H, W, lda] planes, Cin (multiple of 64) channels per group
+ *     starting at a_c0 + g * a_gc; with a2_hi / a2_lo, input channels >= c_split come from A2 (pitch lda2) at a2_c0 + (ci - c_split),
+ *     the same for every group.  W: [groups * N][9 * Cin], K ordered (ky, kx, ci).
+ * Epilogue per output row m and column n of group g:
+ *   v = acc + bias[g * bias_gstride + cls * N + n]  (bias_mode 1: cls = 0; 2: border class (ry * 3 + rx), halo mode, H, W >= 2)
+ *   v = act(v) (0 none, 1 ReLU, 2 GELU);  v *= gamma[n];  v += relu?(res[m * ldr + r_coff + g * r_gcoff + n]);
+ *   v += res2[m * ldr2 + r2_coff + g * r2_gcoff + n]
+ *   C[m * ldc + c_coff + g * c_gcoff + n] = v;  S planes at m * lds + s_coff + g * s_gcoff + n = split(relu?(v)) (split_relu).
+ * phase4 (halo mode, N = 128): column 32 ph + c is channel c of output pixel (2y + ph / 2, 2x + ph % 2) of a 2H x 2W grid.
+ * pred[g] (halo mode, npred = groups): fused 1x1 conv 32 -> nc + normalise (mode 1) / clamp (mode 2), NCHW into pred[g].out.
+ * force_bn / force_kb: run this instantiation instead of the dispatcher's (0 = its choice); a pair the engine does not
+ * instantiate, or cannot run this problem with, is PF_ERR_ARG before anything is launched.  picked_bn / picked_kb: what ran. */
+typedef struct pf_tma_pred { const float* w; const float* b; float* out; int nc, mode; } pf_tma_pred;
+typedef struct pf_tma_op {
+  int mode;
+  int64_t M; int K;
+  int B, H, W, Cin;
+  int N, groups;
+  const void* a_hi; const void* a_lo; int lda, a_c0, a_gc;
+  const void* a2_hi; const void* a2_lo; int lda2, c_split, a2_c0;
+  const void* w_hi; const void* w_lo; const float* bias; int bias_mode, bias_gstride;
+  int act; const float* gamma;
+  const float* res; int ldr, r_coff, r_gcoff, res_relu;
+  const float* res2; int ldr2, r2_coff, r2_gcoff;
+  float* C; int ldc, c_coff, c_gcoff;
+  void* s_hi; void* s_lo; int lds, s_coff, s_gcoff, split_relu;
+  int phase4;
+  int npred; pf_tma_pred pred[2];
+  int force_bn, force_kb;
+  int picked_bn, picked_kb;   /* out */
+} pf_tma_op;
+int pf_op_tma(pf_tma_op* op, void* stream);
+/* The border ring of the phase-composed conv_fuse_conv1 (the two outermost rows / columns of the 2H x 2W output, H, W >= 2),
+ * recomputed in fp32 as pf_forward does after the phase4 launch: c_hi / c_lo: split planes [B, H, W, 128] (head 0 channels
+ * 0-63, head 1 64-127); wf: fp32 [2][9 taps][64 ci][32 o]; bias [2][32]; out: NHWC [B, 2H, 2W, 64] or NULL; with pg_w the
+ * prediction tails of both heads (pg_*: gravity, 2 channels, normalised; pl_*: latitude, 1 channel, clamped; NCHW). */
+int pf_op_conv1_ring(const void* c_hi, const void* c_lo, int B, int H, int W, const float* wf, const float* bias, float* out,
+                     const float* pg_w, const float* pg_b, float* pg_out, const float* pl_w, const float* pl_b, float* pl_out, void* stream);
+/* Host only, no device needed: the (bn, kb) the engine's dispatcher picks for a launch (mode 0 GEMM with M rows; mode 1 halo:
+ * K = 9 * Cin) on a device with sm_count SMs. */
+int pf_tma_pick_tile(int mode, int64_t M, int N, int K, int sm_count, int* bn, int* kb);
 int pf_op_layernorm(const float* x, float* y, int64_t rows, int C, const float* w, const float* b, float eps, void* stream);
 int pf_op_attention(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream);      /* CUDA-core fp32 */
 int pf_op_attention_mma(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream);  /* warp-level mma.sync, bf16x3 */

@@ -43,6 +43,30 @@ class pf_batch(ctypes.Structure):
                 ("params", ctypes.c_void_p)]
 
 
+class pf_tma_pred(ctypes.Structure):
+    """include/pf_b200.h: struct pf_tma_pred (fused prediction tail of one group)."""
+    _fields_ = [("w", ctypes.c_void_p), ("b", ctypes.c_void_p), ("out", ctypes.c_void_p), ("nc", ctypes.c_int), ("mode", ctypes.c_int)]
+
+
+def _fields(spec):
+    """"int a, b; ptr c; i64 d" -> ctypes fields in that order (ptr: any pointer, i64: int64_t)."""
+    types = {"int": ctypes.c_int, "ptr": ctypes.c_void_p, "i64": ctypes.c_int64}
+    out = []
+    for decl in spec.split(";"):
+        t, names = decl.split(None, 1)
+        out += [(n.strip(), types[t]) for n in names.split(",")]
+    return out
+
+
+class pf_tma_op(ctypes.Structure):
+    """include/pf_b200.h: struct pf_tma_op (one launch of the TMA -> wgmma engine, pf_op_tma)."""
+    _fields_ = _fields("int mode; i64 M; int K, B, H, W, Cin, N, groups; ptr a_hi, a_lo; int lda, a_c0, a_gc; ptr a2_hi, a2_lo;"
+                       "int lda2, c_split, a2_c0; ptr w_hi, w_lo, bias; int bias_mode, bias_gstride, act; ptr gamma, res;"
+                       "int ldr, r_coff, r_gcoff, res_relu; ptr res2; int ldr2, r2_coff, r2_gcoff; ptr C; int ldc, c_coff, c_gcoff;"
+                       "ptr s_hi, s_lo; int lds, s_coff, s_gcoff, split_relu, phase4, npred") + \
+        [("pred", pf_tma_pred * 2)] + _fields("int force_bn, force_kb, picked_bn, picked_kb")
+
+
 def _sources():
     return sorted(os.path.join(SRC_DIR, f) for f in os.listdir(SRC_DIR) if f.endswith((".cu", ".cuh"))) + [HEADER]
 
@@ -105,6 +129,9 @@ def lib():
         "pf_debug_numel": (i64, [vp, ctypes.c_char_p]),
         "pf_debug_copy": (i32, [vp, ctypes.c_char_p, vp, i64, vp]),
         "pf_op_conv_gemm": (i32, [vp, i32, i32, i32, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp, i32, vp, vp]),
+        "pf_op_tma": (i32, [ctypes.POINTER(pf_tma_op), vp]),
+        "pf_op_conv1_ring": (i32, [vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+        "pf_tma_pick_tile": (i32, [i32, i64, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32)]),
         "pf_set_option": (i32, [vp, ctypes.c_char_p, i32]),
         "pf_camera_fields": (i32, [i32, ctypes.POINTER(pf_camera), i32, vp, vp, vp]),
         "pf_op_layernorm": (i32, [vp, vp, i64, i32, vp, vp, f32, vp]),
@@ -151,7 +178,7 @@ EXPORTS = ["pf_abi_version", "pf_last_error", "pf_kernel_launch_count", "pf_crea
            "pf_profile_kernels_read", "pf_set_option", "pf_debug_enable", "pf_debug_count", "pf_debug_name", "pf_debug_numel",
            "pf_debug_copy", "pf_camera_fields", "pf_comm_unique_id", "pf_comm_create", "pf_comm_destroy", "pf_gather",
            "pf_jpeg_create", "pf_jpeg_destroy", "pf_jpeg_info", "pf_jpeg_decode_batch",
-           "pf_op_conv_gemm", "pf_op_layernorm", "pf_op_attention", "pf_op_attention_mma", "pf_op_attention_tc", "pf_op_dwconv3x3_gelu", "pf_op_dwconv7x7",
+           "pf_op_conv_gemm", "pf_op_tma", "pf_op_conv1_ring", "pf_tma_pick_tile", "pf_op_layernorm", "pf_op_attention", "pf_op_attention_mma", "pf_op_attention_tc", "pf_op_dwconv3x3_gelu", "pf_op_dwconv7x7",
            "pf_op_upsample2x", "pf_op_preprocess", "pf_op_fill_stream", "pf_op_resize_u8", "pf_op_resize_f32", "pf_op_argmax_decode",
            "pf_op_pred_argmax_decode", "pf_op_postprocess"]
 

@@ -365,8 +365,18 @@ struct Fwd {
   static cudaError_t gemm_tma_halo_mode(const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, int sms, cudaStream_t st, const PredTail* pred) {
     return gemm_tma_launch(MODE_HALO, maps, p, bn, kb, sms, st, pred);
   }
-  int launch_tma(int mode, const TmaMaps& maps, const TmaGemmParams& p, const PredTail* pred = nullptr) {
-    const int bn = mode == MODE_GEMM ? tma_pick_bn_gemm(p.M, p.N, p.K, e->sm_count) : tma_pick_bn(p.N, mode), kb = tma_pick_kb(bn, p.K, mode);
+  int force_bn = 0, force_kb = 0;     // pf_op_tma: tile override (0 = the dispatcher's choice)
+  int picked_bn = 0, picked_kb = 0;   // (bn, kb) of the last TMA launch
+  // the one place a launch's (bn, kb) is chosen: tgemm / thalo build the B maps with it and hand it to launch_tma
+  int pick_tile(int mode, const TmaGemmParams& p, const PredTail* pred, int& bn, int& kb) {
+    tma_pick_tile(mode, p.M, p.N, p.K, e->sm_count, bn, kb);
+    if (force_bn) { bn = force_bn; kb = tma_pick_kb(bn, p.K, mode); }
+    if (force_kb) kb = force_kb;
+    if (const char* msg = gemm_tma_check(mode, p, bn, kb, pred != nullptr)) return fail(PF_ERR_ARG, "TMA engine, %s (bn %d, kb %d): %s", mode == MODE_GEMM ? "GEMM mode" : "halo mode", bn, kb, msg);
+    picked_bn = bn; picked_kb = kb;
+    return PF_OK;
+  }
+  int launch_tma(int mode, const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, const PredTail* pred = nullptr) {
     if (e->profile) {
       pf_engine::ProfRec r{};
       for (cudaEvent_t* ev : {&r.a, &r.b}) {
@@ -428,33 +438,36 @@ struct Fwd {
   int tgemm(const SplitT& A, long long M, int K, int a_c0, const GemmW& w, int N, const Epi& o) {
     if (dry) return PF_OK;
     if (K % 32 || N % 32 || A.ld % 8) return fail(PF_ERR_ARG, "tgemm: K/N must be multiples of 32");
+    if (o.res2 || o.bias_mode == 2) return fail(PF_ERR_ARG, "tgemm: second residual / border-class bias are halo-mode features");
     TmaGemmParams p{};
     p.M = (int)M; p.Cin = K; p.N = N; p.K = K; p.a_c0 = a_c0; p.groups = 1;
     fill_epi(p, w, o, 0);
     TmaMaps maps{};
-    const int bn = tma_pick_bn_gemm(M, N, K, e->sm_count);
-    const int kb = tma_pick_kb(bn, K, MODE_GEMM);
+    int bn, kb;
+    TRY(pick_tile(MODE_GEMM, p, nullptr, bn, kb));
     const char* msg = nullptr;
     if (!msg) msg = map2d(&maps.a_hi, A.hi, A.ld, M, A.ld, 128, kb);
     if (!msg) msg = map2d(&maps.a_lo, A.lo, A.ld, M, A.ld, 128, kb);
     if (!msg) msg = map2d(&maps.b_hi, w.hi, K, N, K, bn, kb);
     if (!msg) msg = map2d(&maps.b_lo, w.lo, K, N, K, bn, kb);
-    if (o.res2 || o.bias_mode == 2) return fail(PF_ERR_ARG, "tgemm: second residual / border-class bias are halo-mode features");
     if (msg) return fail(PF_ERR_CUDA, "%s", msg);
     maps.a2_hi = maps.a_hi; maps.a2_lo = maps.a_lo;
-    return launch_tma(MODE_GEMM, maps, p);
+    return launch_tma(MODE_GEMM, maps, p, bn, kb);
   }
   // 3x3 / stride 1 / pad 1 convolution on split NHWC planes (optionally a second source for channels >= c_split)
   int thalo(const SplitT& A, int a_c0, int a_gc, const SplitT* A2, int c_split, int a2_c0, int B, int H, int W, int Cin, const GemmW& w, int N,
             int groups, int bias_gstride, const Epi& o, const PredTail* pred = nullptr) {
     if (dry) return PF_OK;
     if (Cin % 64 || N % 32 || (A2 && c_split % 64)) return fail(PF_ERR_ARG, "thalo: Cin must be a multiple of 64, N of 32");
+    // the nine border classes (weights.py:_compose_proc) assume a pixel is never both the first and the last of a row / column
+    if (w.b && o.bias_mode == 2 && (H < 2 || W < 2)) return fail(PF_ERR_ARG, "thalo: border-class bias needs H, W >= 2 (got %dx%d)", H, W);
     TmaGemmParams p{};
     p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.N = N; p.K = 9 * Cin; p.a_c0 = a_c0; p.a_gc = a_gc; p.groups = groups;
     p.c_split = A2 ? c_split : 0; p.a2_c0 = a2_c0;
     fill_epi(p, w, o, bias_gstride);
     TmaMaps maps{};
-    const int bn = tma_pick_bn(N, MODE_HALO), kb = tma_pick_kb(bn, p.K, MODE_HALO);
+    int bn, kb;
+    TRY(pick_tile(MODE_HALO, p, pred, bn, kb));
     const char* msg = nullptr;
     if (!msg) msg = map_halo(&maps.a_hi, A.hi, B, H, W, A.ld);
     if (!msg) msg = map_halo(&maps.a_lo, A.lo, B, H, W, A.ld);
@@ -465,7 +478,7 @@ struct Fwd {
     if (!msg) msg = map2d(&maps.b_hi, w.hi, p.K, (long long)groups * N, p.K, bn, kb);
     if (!msg) msg = map2d(&maps.b_lo, w.lo, p.K, (long long)groups * N, p.K, bn, kb);
     if (msg) return fail(PF_ERR_CUDA, "%s", msg);
-    return launch_tma(MODE_HALO, maps, p, pred);
+    return launch_tma(MODE_HALO, maps, p, bn, kb, pred);
   }
   // strided / patchifying convolution = patch gather on split planes + TMA GEMM
   int tconv_gather(const SplitT& A, int B, int H, int W, int Cin, int KH, int stride, int pad, const GemmW& w, int N, const Epi& o) {
@@ -1362,6 +1375,70 @@ int pf_op_conv_gemm(const float* x, int B, int H, int W, int Cin, const void* wh
   cudaFree(scratch);
   if (r != PF_OK) return r;
   if (se != cudaSuccess) return fail(PF_ERR_CUDA, "pf_op_conv_gemm: %s", cudaGetErrorString(se));
+  return PF_OK;
+}
+int pf_op_tma(pf_tma_op* op, void* stream) {
+  if (!op || !op->a_hi || !op->a_lo || !op->w_hi || !op->w_lo) return fail(PF_ERR_ARG, "pf_op_tma: null argument");
+  const pf_tma_op& q = *op;
+  if (q.mode != MODE_GEMM && q.mode != MODE_HALO) return fail(PF_ERR_ARG, "pf_op_tma: mode %d", q.mode);
+  if (!q.C && !q.s_hi) return fail(PF_ERR_ARG, "pf_op_tma: no output (C and S are both NULL)");
+  if (!q.s_hi != !q.s_lo || !q.a2_hi != !q.a2_lo) return fail(PF_ERR_ARG, "pf_op_tma: a split pair needs both planes");
+  if (q.bias_mode < 0 || q.bias_mode > 2 || q.act < 0 || q.act > 2) return fail(PF_ERR_ARG, "pf_op_tma: bias_mode %d / act %d", q.bias_mode, q.act);
+  if (q.groups < 1 || q.groups > 2 || q.N < 1) return fail(PF_ERR_ARG, "pf_op_tma: groups %d, N %d", q.groups, q.N);
+  if (q.npred != 0 && q.npred != q.groups) return fail(PF_ERR_ARG, "pf_op_tma: npred must be 0 or groups");
+  if (q.mode == MODE_GEMM && (q.groups != 1 || q.a2_hi || q.phase4 || q.npred || q.M < 1 || q.M > INT32_MAX))
+    return fail(PF_ERR_ARG, "pf_op_tma: GEMM mode runs one group of 1..2^31-1 rows without A2, phase4 or prediction tail");
+  if (q.mode == MODE_HALO && (q.B < 1 || q.H < 1 || q.W < 1)) return fail(PF_ERR_ARG, "pf_op_tma: image size %dx%dx%d", q.B, q.H, q.W);
+  TRY(configure_current_device());
+  int dev = 0;
+  CU(cudaGetDevice(&dev));
+  cudaDeviceProp prop;
+  CU(cudaGetDeviceProperties(&prop, dev));
+  pf_engine tmp;
+  tmp.device = dev;
+  tmp.sm_count = prop.multiProcessorCount;
+  Fwd F{&tmp, Arena{}, (cudaStream_t)stream, false, q.B};
+  F.force_bn = q.force_bn; F.force_kb = q.force_kb;
+  const SplitT A{(__nv_bfloat16*)q.a_hi, (__nv_bfloat16*)q.a_lo, q.lda};
+  const SplitT A2{(__nv_bfloat16*)q.a2_hi, (__nv_bfloat16*)q.a2_lo, q.lda2};
+  const GemmW w{(const __nv_bfloat16*)q.w_hi, (const __nv_bfloat16*)q.w_lo, q.bias};
+  Fwd::Epi o;
+  o.C = q.C; o.ldc = q.ldc; o.c_coff = q.c_coff; o.c_gcoff = q.c_gcoff;
+  o.S = SplitT{(__nv_bfloat16*)q.s_hi, (__nv_bfloat16*)q.s_lo, q.lds}; o.s_coff = q.s_coff; o.s_gcoff = q.s_gcoff; o.split_relu = q.split_relu;
+  o.act = q.act; o.gamma = q.gamma;
+  o.res = q.res; o.ldr = q.ldr; o.r_coff = q.r_coff; o.r_gcoff = q.r_gcoff; o.res_relu = q.res_relu;
+  o.res2 = q.res2; o.ldr2 = q.ldr2; o.r2_coff = q.r2_coff; o.r2_gcoff = q.r2_gcoff;
+  o.bias_mode = q.bias_mode; o.phase4 = q.phase4;
+  PredTail pt[2];
+  for (int g = 0; g < q.npred; ++g) {
+    const pf_tma_pred& s = q.pred[g];
+    if (!s.w || !s.b || !s.out || !(s.mode == 1 ? s.nc == 2 : (s.mode == 2 && s.nc == 1))) return fail(PF_ERR_ARG, "pf_op_tma: prediction tail %d", g);
+    pt[g] = PredTail{s.w, s.b, s.out, s.nc, s.mode};
+  }
+  op->picked_bn = op->picked_kb = 0;
+  const int r = q.mode == MODE_GEMM ? F.tgemm(A, q.M, q.K, q.a_c0, w, q.N, o)
+                                    : F.thalo(A, q.a_c0, q.a_gc, q.a2_hi ? &A2 : nullptr, q.c_split, q.a2_c0, q.B, q.H, q.W, q.Cin, w, q.N, q.groups,
+                                              q.bias_gstride, o, q.npred ? pt : nullptr);
+  if (r == PF_OK) { op->picked_bn = F.picked_bn; op->picked_kb = F.picked_kb; }
+  return r;
+}
+int pf_op_conv1_ring(const void* c_hi, const void* c_lo, int B, int H, int W, const float* wf, const float* bias, float* out,
+                     const float* pg_w, const float* pg_b, float* pg_out, const float* pl_w, const float* pl_b, float* pl_out, void* stream) {
+  if (!c_hi || !c_lo || !wf || !bias) return fail(PF_ERR_ARG, "pf_op_conv1_ring: null argument");
+  const bool tail = pg_w || pg_b || pg_out || pl_w || pl_b || pl_out;
+  if (tail && !(pg_w && pg_b && pg_out && pl_w && pl_b && pl_out)) return fail(PF_ERR_ARG, "pf_op_conv1_ring: the prediction tail needs all six pointers");
+  if (!out && !tail) return fail(PF_ERR_ARG, "pf_op_conv1_ring: no output");
+  // the ring is the two outermost rows / columns of the 2H x 2W output: it needs two of each
+  if (B < 1 || H < 2 || W < 2) return fail(PF_ERR_ARG, "pf_op_conv1_ring: needs B >= 1 and H, W >= 2 (got %dx%dx%d)", B, H, W);
+  TRY(configure_current_device());
+  const dim3 grid((unsigned)cdiv(conv1_ring_count(2 * H, 2 * W), kRingPx), (unsigned)B);
+  LAUNCHED((conv1_ring_kernel<<<grid, 256, kRingSmem, (cudaStream_t)stream>>>((const __nv_bfloat16*)c_hi, (const __nv_bfloat16*)c_lo, H, W, wf, bias, out,
+                                                                             pg_w, pg_b, pg_out, pl_w, pl_b, pl_out), cudaGetLastError()));
+  return PF_OK;
+}
+int pf_tma_pick_tile(int mode, int64_t M, int N, int K, int sm_count, int* bn, int* kb) {
+  if (!bn || !kb || (mode != MODE_GEMM && mode != MODE_HALO) || N < 1 || K < 1 || sm_count < 1) return fail(PF_ERR_ARG, "pf_tma_pick_tile: bad argument");
+  tma_pick_tile(mode, M, N, K, sm_count, *bn, *kb);
   return PF_OK;
 }
 int pf_camera_fields(int device, const pf_camera* cams, int n, float* up, float* lat, void* stream) {

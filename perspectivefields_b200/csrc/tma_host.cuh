@@ -93,6 +93,13 @@ inline int tma_pick_kb(int bn, int K, int mode) {
   return (bn <= lim && K % 64 == 0) ? 64 : 32;
 }
 
+// (bn, kb) of one launch: GEMM mode with the row count and SM count known (tma_pick_bn_gemm), halo mode from N alone.
+// K = the GEMM's K (halo mode: 9 x Cin).  Chosen once per launch: the B-map boxes and the launched instantiation both follow it.
+inline void tma_pick_tile(int mode, long long M, int N, int K, int sm_count, int& bn, int& kb) {
+  bn = mode == MODE_GEMM ? tma_pick_bn_gemm(M, N, K, sm_count) : tma_pick_bn(N, mode);
+  kb = tma_pick_kb(bn, K, mode);
+}
+
 struct PredTail { const float* w; const float* b; float* out; int nc, mode; };   // per group, see TmaGemmParams::pred_*
 
 template <int BN, int MODE, int KB>
@@ -143,7 +150,29 @@ inline cudaError_t gemm_tma_configure_device() {
   return e;
 }
 
-inline cudaError_t gemm_tma_launch(int mode, const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, int sm_count, cudaStream_t st,
+// ring depth of an instantiation, 0 if PF_TMA_VARIANTS does not list it
+inline int tma_stages(int mode, int bn, int kb) {
+#define PF_TMA_NS(BN_, MODE_, KB_) if (mode == MODE_ && bn == BN_ && kb == KB_) return TmaCfg<BN_, MODE_, KB_>::kStages;
+  PF_TMA_VARIANTS(PF_TMA_NS)
+#undef PF_TMA_NS
+  return 0;
+}
+
+// Why the (bn, kb) instantiation cannot compute p: nullptr when it can.  Every case here would otherwise launch something that
+// computes a different result (a K tail, a prediction tail or phase layout the tile width does not implement) or that
+// gemm_tma_launch_bn refuses after the fact (resident weights over several N tiles).
+inline const char* gemm_tma_check(int mode, const TmaGemmParams& p, int bn, int kb, bool pred) {
+  const int ns = tma_stages(mode, bn, kb);
+  if (!ns) return "no engine instantiation for this (mode, bn, kb)";
+  if (mode == MODE_GEMM) return p.K % kb ? "GEMM mode: K must be a multiple of the K step" : nullptr;
+  if (p.phase4 && (p.N != 128 || bn != 128)) return "phase4 needs N = 128 in one 128-wide tile";
+  if (pred && bn != (p.phase4 ? 128 : 32)) return "the fused prediction tail needs N = 32 (phase4: 128) in one tile";
+  const bool resident = p.Cin == 64 && 9 * (64 / kb) <= ns;
+  if ((resident || pred) && cdiv(p.N, bn) > 1) return "resident weights (Cin = 64) and the prediction tail need one N tile per launch";
+  return nullptr;
+}
+
+inline cudaError_t gemm_tma_launch(int mode,const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, int sm_count, cudaStream_t st,
                                    const PredTail* pred = nullptr) {
 #define PF_TMA_CASE(BN_, MODE_, KB_) if (mode == MODE_ && bn == BN_ && kb == KB_) return gemm_tma_launch_bn<BN_, MODE_, KB_>(maps, p, sm_count, st, pred);
   PF_TMA_VARIANTS(PF_TMA_CASE)

@@ -215,21 +215,32 @@ def test_kernel_launches_are_counted():
     assert _native.lib().pf_kernel_launch_count() - before > 300
 
 
-@pytest.mark.parametrize("opts", [{"attn_mma": 0, "stem_tc": 0}, {"phase_conv1": 0}, {"attn_split": 0}])
+OPTION_DEFAULTS = {"fork": 0, "dw_ln": 0, "decode_only": 0}    # every other option defaults to 1 (include/pf_b200.h)
+
+
+@pytest.mark.parametrize("opts", [{"attn_mma": 0, "stem_tc": 0}, {"phase_conv1": 0}, {"attn_split": 0}, {"dw_ln": 1}, {"pdl": 0}, {"fork": 1}])
 def test_engine_options_end_to_end(opts):
     """The same forward with the alternative kernels the options select: exact-softmax CUDA-core attention and direct fp32 stems,
-    conv_fuse_conv1 at 320x320 on the materialised upsample, fp32 q / kv."""
+    conv_fuse_conv1 at 320x320 on the materialised upsample, fp32 q / kv, the fused depthwise 7x7 + LayerNorm.  "pdl" and "fork"
+    only change how the same kernels are scheduled: their outputs equal the default run's exactly.  Each option is restored to
+    the value it had, so that later tests see the model as it was."""
     version = "Paramnet-360Cities-edina-centered"
     m, sd = model(version)
     imgs = golden_images()
     base = m.inference_batch(imgs)
+    prev = {k: m._options.get(k, OPTION_DEFAULTS.get(k, 1)) for k in opts}
     for k, v in opts.items():
         m.set_option(k, v)
     try:
         out = m.inference_batch(imgs)
     finally:
-        for k in opts:
-            m.set_option(k, 1)
+        for k, v in prev.items():
+            m.set_option(k, v)
+    if set(opts) <= {"pdl", "fork"}:
+        for a, b in zip(out, base):
+            for k, v in a.items():
+                assert torch.equal(v, b[k]) if isinstance(v, torch.Tensor) else v == b[k], k
+        return
     print(opts, _check(out, om.inference_batch(sd, version, imgs), version))
     compare_with_golden(version, out, tol=TOL)
     for a, b in zip(out, base):

@@ -132,28 +132,30 @@ def test_preprocess_is_bit_exact_vs_pillow(hw):
     assert np.array_equal(got[..., :3], ref) and not got[..., 3].any()
 
 
-# ---- more GEMM-mode / halo-mode shapes of the TMA -> wgmma engine
+# ---- more GEMM-mode / halo-mode shapes of the TMA -> wgmma engine.  The comments give the (BN, KB) the dispatcher picks on
+# 132 SMs (test_host_logic.py::test_tile_dispatch_of_the_op_cases checks them); 3x3 convs with Cin % 64 == 0 run in halo mode,
+# everything else in GEMM mode (strided / k > 1 convs after a patch gather)
 TC_CASES = [
-    (2, 20, 20, 256, 256, 3, 1, 1, 1, 1, 0, 0),     # RCU conv1
-    (1, 23, 17, 256, 256, 3, 1, 1, 0, 0, 1, 1),     # RCU conv2 + relu(residual), ragged M (391 rows)
-    (2, 16, 16, 64, 512, 3, 1, 1, 0, 0, 0, 0),      # composed proc conv (two N tiles)
-    (1, 1, 700, 320, 256, 1, 1, 0, 0, 0, 0, 0),     # plain linear, K = 320 (10 k-steps, ring wraps)
-    (1, 1, 64, 32, 256, 1, 1, 0, 0, 0, 0, 0),       # single k-step
-    (3, 40, 40, 256, 256, 3, 1, 1, 1, 0, 0, 0),     # 38 tiles, 72 k-steps
-    (1, 1, 700, 320, 640, 1, 1, 0, 0, 0, 0, 0),     # N tile 128 (kv linear)
-    (1, 1, 300, 96, 384, 1, 1, 0, 0, 2, 0, 0),      # N tile 128 + GELU
-    (1, 1, 130, 384, 96, 1, 1, 0, 0, 0, 1, 0),      # N tile 32 (x3) + residual
-    (2, 80, 80, 64, 64, 8, 8, 0, 0, 0, 0, 0),       # N tile 64, k = s = 8
-    (1, 24, 24, 64, 32, 3, 1, 1, 0, 1, 0, 0),       # N tile 32
-    (1, 40, 40, 320, 64, 3, 1, 1, 0, 1, 0, 0),      # N tile 64, K = 2880
-    (2, 40, 40, 64, 128, 3, 2, 1, 0, 0, 0, 0),      # N tile 128, stride 2
-    (1, 1, 500, 64, 320, 1, 1, 0, 0, 0, 0, 0),      # N = 320 -> five 64-wide tiles
+    (2, 20, 20, 256, 256, 3, 1, 1, 1, 1, 0, 0),     # RCU conv1, halo (256, 32)
+    (1, 23, 17, 256, 256, 3, 1, 1, 0, 0, 1, 1),     # RCU conv2 + relu(residual), ragged tiles, halo (256, 32)
+    (2, 16, 16, 64, 512, 3, 1, 1, 0, 0, 0, 0),      # composed proc conv, halo (256, 32): two N tiles
+    (1, 1, 700, 320, 256, 1, 1, 0, 0, 0, 0, 0),     # plain linear, K = 320: (32, 64), 5 K steps
+    (1, 1, 64, 32, 256, 1, 1, 0, 0, 0, 0, 0),       # single K step: (32, 32)
+    (3, 40, 40, 256, 256, 3, 1, 1, 1, 0, 0, 0),     # halo (256, 32): 45 tiles, 72 K steps
+    (1, 1, 700, 320, 640, 1, 1, 0, 0, 0, 0, 0),     # kv linear: (32, 64), 20 N tiles
+    (1, 1, 300, 96, 384, 1, 1, 0, 0, 2, 0, 0),      # GELU, K = 96: (32, 32)
+    (1, 1, 130, 384, 96, 1, 1, 0, 0, 0, 1, 0),      # + residual: (32, 64), 3 N tiles
+    (2, 80, 80, 64, 64, 8, 8, 0, 0, 0, 0, 0),       # k = s = 8, K = 4096: (32, 64)
+    (1, 24, 24, 64, 32, 3, 1, 1, 0, 1, 0, 0),       # halo (32, 64), resident weights
+    (1, 40, 40, 320, 64, 3, 1, 1, 0, 1, 0, 0),      # halo (64, 64), K = 2880
+    (2, 40, 40, 64, 128, 3, 2, 1, 0, 0, 0, 0),      # stride 2, patch gather: (32, 64)
+    (1, 1, 500, 64, 320, 1, 1, 0, 0, 0, 0, 0),      # N = 320 -> ten 32-wide tiles: (32, 64)
     # large GEMM-mode launches (several tiles per CTA of the persistent grid)
-    (1, 1, 12800, 320, 320, 1, 1, 0, 0, 0, 1, 0),   # MiT stage-3 proj: 100 row tiles x 2 N tiles of 160, + residual
-    (1, 1, 20000, 96, 384, 1, 1, 0, 0, 2, 0, 0),    # ragged M (156.25 row tiles), GELU, 3 K steps
-    (1, 1, 19000, 1280, 320, 1, 1, 0, 0, 0, 1, 1),  # K = 1280 (the ring wraps many times), relu(residual), last row tile partial
-    (1, 1, 25000, 64, 640, 1, 1, 0, 0, 1, 0, 0),    # N = 640 -> three N tiles of 224 (last one partial), ReLU
-    (1, 1, 40000, 128, 64, 1, 1, 0, 0, 0, 0, 0),    # narrow N = 64 (32 weight rows per CTA)
+    (1, 1, 12800, 320, 320, 1, 1, 0, 0, 0, 1, 0),   # MiT stage-3 proj: 100 row tiles x 2 N tiles of 160 (160, 32), + residual
+    (1, 1, 20000, 96, 384, 1, 1, 0, 0, 2, 0, 0),    # ragged M (156.25 row tiles), GELU: (192, 32), 3 K steps
+    (1, 1, 19000, 1280, 320, 1, 1, 0, 0, 0, 1, 1),  # K = 1280 (the ring wraps many times), relu(residual), last row tile partial: (160, 32)
+    (1, 1, 25000, 64, 640, 1, 1, 0, 0, 1, 0, 0),    # N = 640 -> three N tiles of 224 (last one partial), ReLU: (224, 32)
+    (1, 1, 40000, 128, 64, 1, 1, 0, 0, 0, 0, 0),    # narrow N = 64: (64, 64)
 ]
 
 

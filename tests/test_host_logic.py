@@ -194,3 +194,31 @@ def test_fast_asin_and_atan2_polynomials_of_the_kernels():
     deg = np.copysign((pr.astype(np.float64) * np.float64(f(57.29577951308232)) + np.where(hi, 90.0, np.where(mid, 45.0, 0.0))).astype(f), yw)   # fmaf: one rounding
     ref = np.degrees(np.arctan2(yw.astype(np.float64), h.astype(np.float64)))
     assert np.abs(deg.astype(np.float64) - ref).max() < 1e-5
+
+
+# (BN, KB) the dispatcher picks for test_gpu_ops.TC_CASES on a 132-SM H100, in order (halo mode: 3x3 / s1 / p1, Cin % 64 == 0)
+TC_PICKS = [("halo", 256, 32), ("halo", 256, 32), ("halo", 256, 32), ("gemm", 32, 64), ("gemm", 32, 32), ("halo", 256, 32),
+            ("gemm", 32, 64), ("gemm", 32, 32), ("gemm", 32, 64), ("gemm", 32, 64), ("halo", 32, 64), ("halo", 64, 64),
+            ("gemm", 32, 64), ("gemm", 32, 64), ("gemm", 160, 32), ("gemm", 192, 32), ("gemm", 160, 32), ("gemm", 224, 32),
+            ("gemm", 64, 64)]
+
+
+def test_tile_dispatch_of_the_op_cases():
+    """pf_tma_pick_tile (the host-side dispatcher of the TMA engine, no device needed) on the op-test shapes: records which
+    instantiation each of them exercises, so that a change of the cost model shows up here and in the case comments."""
+    import ctypes
+
+    from perspectivefields_b200 import _native
+    from test_gpu_ops import TC_CASES
+
+    _native.build()
+    L = _native.lib()
+    got = []
+    for B, H, W, Cin, N, K, s, p, *_ in TC_CASES:
+        halo = K == 3 and s == 1 and p == 1 and Cin % 64 == 0
+        M = B * ((H + 2 * p - K) // s + 1) * ((W + 2 * p - K) // s + 1)
+        bn, kb = ctypes.c_int(), ctypes.c_int()
+        _native.check(L.pf_tma_pick_tile(int(halo), M, N, K * K * Cin, 132, ctypes.byref(bn), ctypes.byref(kb)))
+        got.append(("halo" if halo else "gemm", bn.value, kb.value))
+    assert got == TC_PICKS
+    assert L.pf_tma_pick_tile(2, 1, 32, 32, 132, ctypes.byref(bn), ctypes.byref(kb)) < 0
