@@ -190,7 +190,10 @@ int pf_op_conv_gemm(const float* x, int B, int H, int W, int Cin, const void* wh
  * phase4 (halo mode, N = 128): column 32 ph + c is channel c of output pixel (2y + ph / 2, 2x + ph % 2) of a 2H x 2W grid.
  * pred[g] (halo mode, npred = groups): fused 1x1 conv 32 -> nc + normalise (mode 1) / clamp (mode 2), NCHW into pred[g].out.
  * force_bn / force_kb: run this instantiation instead of the dispatcher's (0 = its choice); a pair the engine does not
- * instantiate, or cannot run this problem with, is PF_ERR_ARG before anything is launched.  picked_bn / picked_kb: what ran. */
+ * instantiate, or cannot run this problem with, is PF_ERR_ARG before anything is launched.  picked_bn / picked_kb: what ran.
+ * force_sched (GEMM mode): 0 = the dispatcher's schedule, 1 = cooperative (128-row tiles), 2 = ping-pong (64-row tiles, one
+ * MMA warpgroup's epilogue overlapping the other's main loop); picked_sched: what ran (1 / 2; 0 in halo mode).  Every
+ * schedule gives bit-identical results. */
 typedef struct pf_tma_pred { const float* w; const float* b; float* out; int nc, mode; } pf_tma_pred;
 typedef struct pf_tma_op {
   int mode;
@@ -209,6 +212,7 @@ typedef struct pf_tma_op {
   int npred; pf_tma_pred pred[2];
   int force_bn, force_kb;
   int picked_bn, picked_kb;   /* out */
+  int force_sched, picked_sched;
 } pf_tma_op;
 int pf_op_tma(pf_tma_op* op, void* stream);
 /* The border ring of the phase-composed conv_fuse_conv1 (the two outermost rows / columns of the 2H x 2W output, H, W >= 2),

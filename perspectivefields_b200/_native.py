@@ -64,7 +64,7 @@ class pf_tma_op(ctypes.Structure):
                        "int lda2, c_split, a2_c0; ptr w_hi, w_lo, bias; int bias_mode, bias_gstride, act; ptr gamma, res;"
                        "int ldr, r_coff, r_gcoff, res_relu; ptr res2; int ldr2, r2_coff, r2_gcoff; ptr C; int ldc, c_coff, c_gcoff;"
                        "ptr s_hi, s_lo; int lds, s_coff, s_gcoff, split_relu, phase4, npred") + \
-        [("pred", pf_tma_pred * 2)] + _fields("int force_bn, force_kb, picked_bn, picked_kb")
+        [("pred", pf_tma_pred * 2)] + _fields("int force_bn, force_kb, picked_bn, picked_kb, force_sched, picked_sched")
 
 
 def _sources():

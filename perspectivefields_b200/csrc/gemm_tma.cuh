@@ -12,8 +12,13 @@
 //               ring of KB-wide K steps.
 //
 //   warpgroup 0 : warp 0 = TMA producer (B ring; in MODE_GEMM also A), warp 1 = MODE_HALO halo (A) producer
-//   warpgroups 1, 2 : MMA + epilogue, rows 0-63 and 64-127 of the 128 x BN tile (wgmma M = 64 per warpgroup); each
+//   warpgroups 1, 2 : MMA + epilogue.  Two schedules:
+//     cooperative (PP = false): both work on one 128 x BN tile, rows 0-63 and 64-127 (wgmma M = 64 per warpgroup); each
 //                     accumulates its 64 x BN block in registers and runs the fused epilogue on it.
+//     ping-pong (PP = true, MODE_GEMM): tiles are 64 x BN and each warpgroup owns every other tile of the CTA's sequence, so one
+//                     warpgroup's epilogue (HBM traffic) overlaps the other's main loop (tensor cores).  A ring stage belongs to
+//                     the warpgroup whose tile it holds.  B is loaded once per 64 rows instead of 128: this pays on short K,
+//                     where the epilogue is a large share of a tile's time.  Same K order per output as the cooperative schedule.
 //
 // Epilogue (fused): + bias | border-class bias, ReLU / GELU, layer scale, + relu?(residual), + second residual; writes the
 // fp32 tensor and/or the bf16 hi/lo planes (optionally rectified) that the next GEMM will TMA-load.
@@ -56,11 +61,13 @@ struct TmaGemmParams {
 
 // KB = K elements per pipeline step: 32 (64 B rows, SWIZZLE_64B) for wide tiles, 64 (128 B rows, SWIZZLE_128B) for narrow ones
 // where a 32-wide step would be shorter than the barrier round trip that feeds it.
-template <int BN, int MODE, int KB> struct TmaCfg {
+template <int BN, int MODE, int KB, bool PP = false> struct TmaCfg {
   static_assert(KB == 32 || KB == 64, "KB");
   static_assert(BN % 32 == 0 && BN <= 256, "BN");
+  static_assert(!PP || MODE == MODE_GEMM, "the ping-pong schedule is a GEMM-mode schedule");
+  static constexpr int kTileM = PP ? 64 : 128;                  // MODE_GEMM: rows per tile
   static constexpr int kBPlane = BN * KB * 2;                   // bf16 plane of one K step of B
-  static constexpr int kAPlane = 128 * KB * 2;                  // MODE_GEMM: plane of a 128 x KB A tile
+  static constexpr int kAPlane = kTileM * KB * 2;               // MODE_GEMM: plane of a kTileM x KB A tile
   static constexpr int kStage = (MODE == MODE_GEMM ? 2 * kAPlane : 0) + 2 * kBPlane;
   static constexpr int kABuf = 2 * kHtPlaneBytes;               // MODE_HALO: hi + lo halo planes (1024 B multiples)
   // epilogue staging: each MMA warpgroup moves its accumulators through shared memory 64 columns at a time so that one thread
@@ -95,12 +102,12 @@ struct TmaMaps {   // passed by value as a __grid_constant__ kernel parameter
   CUtensorMap a_hi, a_lo, a2_hi, a2_lo, b_hi, b_lo;
 };
 
-template <int BN, int MODE, int KB>
+template <int BN, int MODE, int KB, bool PP = false>
 __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_constant__ TmaMaps maps, const TmaGemmParams p, int tiles_x, int tiles_y) {
-  using Cfg = TmaCfg<BN, MODE, KB>;
+  using Cfg = TmaCfg<BN, MODE, KB, PP>;
   constexpr int NS = Cfg::kStages;
   constexpr int SPC = 9 * (64 / KB);          // MODE_HALO: pipeline steps per 64-channel chunk (9 taps x 64 / KB)
-  constexpr int kConsumerWarps = 8;
+  constexpr int kConsumerWarps = PP ? 4 : 8;   // warps that release a ring stage: its warpgroup (ping-pong) or both
   extern __shared__ unsigned char smem_dyn[];
   const uint32_t raw = smem_u32(smem_dyn);
   const uint32_t sbase = (raw + 1023u) & ~1023u;
@@ -113,10 +120,11 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
   auto empty_b = [&](int s) { return bars + 8u * (NS + s); };
   auto full_a = [&](int i) { return bars + 8u * (2 * NS + i); };
   auto empty_a = [&](int i) { return bars + 8u * (2 * NS + 2 + i); };
+  auto order_b = [&](int w) { return bars + 8u * (2 * NS + 4 + w); };   // ping-pong: warpgroup w has issued a tile's main loop
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int n_tiles = cdiv(p.N, BN);
-  const int m_tiles = MODE == MODE_GEMM ? cdiv(p.M, 128) : p.B * tiles_x * tiles_y;
+  const int m_tiles = MODE == MODE_GEMM ? cdiv(p.M, Cfg::kTileM) : p.B * tiles_x * tiles_y;
   const int total_tiles = m_tiles * n_tiles * p.groups;
   const int nchunks = MODE == MODE_HALO ? p.Cin / 64 : 0;
   const int nk = MODE == MODE_GEMM ? p.K / KB : nchunks * SPC;
@@ -127,7 +135,7 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
   if (tid == 0) {
     tma_prefetch_desc(&maps.a_hi); tma_prefetch_desc(&maps.a_lo); tma_prefetch_desc(&maps.b_hi); tma_prefetch_desc(&maps.b_lo);
     for (int s = 0; s < NS; ++s) { mbar_init(full_b(s), 1); mbar_init(empty_b(s), kConsumerWarps); }
-    for (int i = 0; i < 2; ++i) { mbar_init(full_a(i), 1); mbar_init(empty_a(i), kConsumerWarps); }
+    for (int i = 0; i < 2; ++i) { mbar_init(full_a(i), 1); mbar_init(empty_a(i), kConsumerWarps); mbar_init(order_b(i), 4); }
     fence_mbar_init();
   }
   __syncthreads();
@@ -162,8 +170,8 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
           int kcol;
           if (MODE == MODE_GEMM) {
             kcol = kc * KB;
-            tma_load_2d(st, &maps.a_hi, full_b(s), p.a_c0 + g * p.a_gc + kcol, mt * 128);
-            tma_load_2d(st + Cfg::kAPlane, &maps.a_lo, full_b(s), p.a_c0 + g * p.a_gc + kcol, mt * 128);
+            tma_load_2d(st, &maps.a_hi, full_b(s), p.a_c0 + g * p.a_gc + kcol, mt * Cfg::kTileM);
+            tma_load_2d(st + Cfg::kAPlane, &maps.a_lo, full_b(s), p.a_c0 + g * p.a_gc + kcol, mt * Cfg::kTileM);
           } else {
             const int c = kc / SPC, u = kc - c * SPC;
             kcol = KB == 32 ? (u >> 1) * p.Cin + c * 64 + (u & 1) * 32 : u * p.Cin + c * 64;
@@ -201,19 +209,27 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
 
   // ======================================================================= MMA + epilogue warpgroups
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n");
-  const int wg = (warp >> 2) - 1;                 // 0: tile rows 0-63, 1: rows 64-127
+  const int wg = (warp >> 2) - 1;                 // cooperative: 0 = tile rows 0-63, 1 = rows 64-127;  ping-pong: CTA-local tile parity
   const int wt = tid & 127;                       // thread within the warpgroup
   float* stage = reinterpret_cast<float*>(sm + (acc_base - sbase)) + wg * 64 * Cfg::kAccPitch;
   // epilogue ownership: row `erow` of this warpgroup's 64, 32-column half `eh` of each 64-column staging round
   const int erow = wt & 63, eh = wt >> 6;
-  const int r = wg * 64 + erow;                   // row of the tile
+  const int r = PP ? erow : wg * 64 + erow;       // row of the tile
+  constexpr int kTileStep = PP ? 2 : 1;           // ping-pong: this warpgroup's tiles are CTA-local tiles wg, wg + 2, ...
   float acc[BN / 2];
   int it = 0, ita = 0;
-  for (int tile = blockIdx.x, tl = 0; tile < total_tiles; tile += gridDim.x, ++tl) {
+  for (int tl = PP ? wg : 0, tile = blockIdx.x + tl * gridDim.x; tile < total_tiles; tile += kTileStep * gridDim.x, tl += kTileStep) {
     int mt, g, n0;
     decode(tile, mt, g, n0);
-    // ---------------- main loop: per K step, 3 products x BN / 64 (+ one 32-wide) wgmmas, one commit group; the stage of the
-    // previous step is released once that step's group has completed (one group stays in flight under the next wait)
+    if (PP) {
+      it = tl * nk;                               // the producer fills nk stages per tile in CTA-local tile order
+      // main loops alternate: tile tl starts once the other warpgroup has issued tile tl - 1 (its completion (tl - 1) / 2).  This
+      // also keeps a warpgroup's full-barrier waits within one ring round of the producer, which their parity needs.
+      if (tl > 0) mbar_wait(order_b(wg ^ 1), ((tl - 1) >> 1) & 1);
+    }
+    // ---------------- main loop: per k16 of a K step, one m64nBNk16 wgmma per product (lo*hi, hi*lo, hi*hi), one commit group per
+    // step; the stage of the previous step is released once that step's group has completed (one group stays in flight under the
+    // next wait).  The B plane is contiguous in 8-row groups, so one descriptor spans all BN weight rows.
     int prev_s = -1, prev_buf = -1;
     fence_regs(acc);
     for (int kc = 0; kc < nk; ++kc, ++it) {
@@ -231,7 +247,7 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
         a_lo = a_hi + kHtPlaneBytes;
         chunk_end = u == SPC - 1;
       } else {
-        a_hi = ring + s * Cfg::kStage + wg * 64 * KB * 2;
+        a_hi = ring + s * Cfg::kStage + (PP ? 0 : wg * 64 * KB * 2);
         a_lo = a_hi + Cfg::kAPlane;
       }
       const int sb = b_resident ? kc : s;                                   // resident weights: step kc lives in slot kc
@@ -241,23 +257,13 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
       const uint64_t dal = MODE == MODE_HALO ? ht_a_desc(a_lo) : wgmma_tile_desc<KB>(a_lo);
       const uint64_t dbh = wgmma_tile_desc<KB>(b_hi);
       const uint64_t dbl = wgmma_tile_desc<KB>(b_hi + Cfg::kBPlane);
-      constexpr uint64_t kChunk = (uint64_t)(64 * KB * 2) >> 4;          // 64 weight rows further in the B tile
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < KB / 16; ++kk) {
         const uint32_t first = (kc | kk) ? 1u : 0u;
-#pragma unroll
-        for (int j = 0; j < BN / 64; ++j) {
-          wgmma_n64(acc + 32 * j, dal + 2 * kk, dbh + 2 * kk + j * kChunk, first);
-          wgmma_n64(acc + 32 * j, dah + 2 * kk, dbl + 2 * kk + j * kChunk, 1u);
-          wgmma_n64(acc + 32 * j, dah + 2 * kk, dbh + 2 * kk + j * kChunk, 1u);
-        }
-        if constexpr (BN % 64 != 0) {
-          constexpr int j = BN / 64;
-          wgmma_n32(acc + 32 * j, dal + 2 * kk, dbh + 2 * kk + j * kChunk, first);
-          wgmma_n32(acc + 32 * j, dah + 2 * kk, dbl + 2 * kk + j * kChunk, 1u);
-          wgmma_n32(acc + 32 * j, dah + 2 * kk, dbh + 2 * kk + j * kChunk, 1u);
-        }
+        wgmma_bf16<BN>(acc, dal + 2 * kk, dbh + 2 * kk, first);
+        wgmma_bf16<BN>(acc, dah + 2 * kk, dbl + 2 * kk, 1u);
+        wgmma_bf16<BN>(acc, dah + 2 * kk, dbh + 2 * kk, 1u);
       }
       wgmma_commit();
       wgmma_wait<1>();
@@ -269,6 +275,7 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
       prev_buf = chunk_end ? buf : -1;
       if (MODE == MODE_HALO && chunk_end) ++ita;
     }
+    if (PP && lane == 0) mbar_arrive(order_b(wg));
     wgmma_wait<0>();
     fence_regs(acc);
     if (lane == 0 && prev_s >= 0) {
@@ -282,7 +289,7 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
     int cls_off = 0;
     int bimg = 0, oy = 0, ox = 0;
     if (MODE == MODE_GEMM) {
-      m = (long long)mt * 128 + r;
+      m = (long long)mt * Cfg::kTileM + r;
       valid = m < p.M;
     } else {
       const int tx = mt % tiles_x, ty = (mt / tiles_x) % tiles_y;
@@ -313,131 +320,177 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
       }
       named_bar_sync(1 + wg, 128);
       const int ch = 2 * rd + eh;                 // this thread's 32-column chunk (warp-uniform)
-      if (ch >= BN / 32) continue;
-      const int nb = n0 + ch * 32;
       const bool ph4 = MODE == MODE_HALO && BN == 128 && p.phase4;
-      // output row / first output column of this chunk (phase mode: hi-res pixel of phase `ch`, channels 0-31)
-      const long long mo = ph4 ? ((long long)bimg * 2 * p.H + 2 * oy + (ch >> 1)) * (2 * p.W) + 2 * ox + (ch & 1) : m;
-      const int nbo = ph4 ? 0 : nb;
-      const bool chunk_ok = nb < p.N;      // warp-uniform
+      // split planes outside phase mode go out through shared memory (staged_split below)
+      const bool staged_split = p.Shi && !ph4;
       float o[32];
-      const float* srow = stage + erow * Cfg::kAccPitch + eh * 32;
+      if (ch < BN / 32) {
+        const int nb = n0 + ch * 32;
+        // output row / first output column of this chunk (phase mode: hi-res pixel of phase `ch`, channels 0-31)
+        const long long mo = ph4 ? ((long long)bimg * 2 * p.H + 2 * oy + (ch >> 1)) * (2 * p.W) + 2 * ox + (ch & 1) : m;
+        const int nbo = ph4 ? 0 : nb;
+        const bool chunk_ok = nb < p.N;      // warp-uniform
+        const float* srow = stage + erow * Cfg::kAccPitch + eh * 32;
 #pragma unroll
-      for (int j = 0; j < 32; j += 4) {
-        const float4 t = *reinterpret_cast<const float4*>(srow + j);
-        o[j] = t.x; o[j + 1] = t.y; o[j + 2] = t.z; o[j + 3] = t.w;
-      }
-      if (valid && chunk_ok) {
-        if (p.bias_mode) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 bv = __ldg(reinterpret_cast<const float4*>(bias + cls_off + nb + j));
-            o[j] += bv.x; o[j + 1] += bv.y; o[j + 2] += bv.z; o[j + 3] += bv.w;
-          }
+        for (int j = 0; j < 32; j += 4) {
+          const float4 t = *reinterpret_cast<const float4*>(srow + j);
+          o[j] = t.x; o[j + 1] = t.y; o[j + 2] = t.z; o[j + 3] = t.w;
         }
-        if (p.act == 1) {
+        if (valid && chunk_ok) {
+          if (p.bias_mode) {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) o[j] = fmaxf(o[j], 0.f);
-        } else if (p.act == 2) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) o[j] = gelu_erf(o[j]);
-        }
-        if (p.gamma) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 gv = __ldg(reinterpret_cast<const float4*>(p.gamma + nb + j));
-            o[j] *= gv.x; o[j + 1] *= gv.y; o[j + 2] *= gv.z; o[j + 3] *= gv.w;
-          }
-        }
-        if (p.res) {
-          const float* rp = p.res + m * p.ldr + p.r_coff + g * p.r_gcoff + nb;
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            float4 rv = *reinterpret_cast<const float4*>(rp + j);
-            if (p.res_relu) { rv.x = fmaxf(rv.x, 0.f); rv.y = fmaxf(rv.y, 0.f); rv.z = fmaxf(rv.z, 0.f); rv.w = fmaxf(rv.w, 0.f); }
-            o[j] += rv.x; o[j + 1] += rv.y; o[j + 2] += rv.z; o[j + 3] += rv.w;
-          }
-        }
-        if (p.res2) {
-          const float* rp = p.res2 + m * p.ldr2 + p.r2_coff + g * p.r2_gcoff + nb;
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 rv = *reinterpret_cast<const float4*>(rp + j);
-            o[j] += rv.x; o[j + 1] += rv.y; o[j + 2] += rv.z; o[j + 3] += rv.w;
-          }
-        }
-        if (MODE == MODE_HALO && (BN == 32 || BN == 128) && p.pred_w) {
-          float v0 = __ldg(p.pred_b), v1 = p.pred_nc > 1 ? __ldg(p.pred_b + 1) : 0.f;
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 w0 = __ldg(reinterpret_cast<const float4*>(p.pred_w + j));
-            v0 = fmaf(o[j], w0.x, v0); v0 = fmaf(o[j + 1], w0.y, v0); v0 = fmaf(o[j + 2], w0.z, v0); v0 = fmaf(o[j + 3], w0.w, v0);
-            if (p.pred_nc > 1) {
-              const float4 w1 = __ldg(reinterpret_cast<const float4*>(p.pred_w + 32 + j));
-              v1 = fmaf(o[j], w1.x, v1); v1 = fmaf(o[j + 1], w1.y, v1); v1 = fmaf(o[j + 2], w1.z, v1); v1 = fmaf(o[j + 3], w1.w, v1);
+            for (int j = 0; j < 32; j += 4) {
+              const float4 bv = __ldg(reinterpret_cast<const float4*>(bias + cls_off + nb + j));
+              o[j] += bv.x; o[j + 1] += bv.y; o[j + 2] += bv.z; o[j + 3] += bv.w;
             }
           }
-          const long long HWl = (long long)p.H * p.W * (ph4 ? 4 : 1);
-          const long long bi = mo / HWl, pix = mo - bi * HWl;
-          float* po = p.pred_out + bi * p.pred_nc * HWl + pix;
-          if (p.pred_mode == 1) {
-            const float nrm = fmaxf(sqrtf(v0 * v0 + v1 * v1), 1e-12f);
-            po[0] = v0 / nrm; po[HWl] = v1 / nrm;
+          if (p.act == 1) {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) o[j] = fmaxf(o[j], 0.f);
+          } else if (p.act == 2) {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) o[j] = gelu_erf(o[j]);
+          }
+          if (p.gamma) {
+#pragma unroll
+            for (int j = 0; j < 32; j += 4) {
+              const float4 gv = __ldg(reinterpret_cast<const float4*>(p.gamma + nb + j));
+              o[j] *= gv.x; o[j + 1] *= gv.y; o[j + 2] *= gv.z; o[j + 3] *= gv.w;
+            }
+          }
+          if (p.res) {
+            const float* rp = p.res + m * p.ldr + p.r_coff + g * p.r_gcoff + nb;
+#pragma unroll
+            for (int j = 0; j < 32; j += 4) {
+              float4 rv = *reinterpret_cast<const float4*>(rp + j);
+              if (p.res_relu) { rv.x = fmaxf(rv.x, 0.f); rv.y = fmaxf(rv.y, 0.f); rv.z = fmaxf(rv.z, 0.f); rv.w = fmaxf(rv.w, 0.f); }
+              o[j] += rv.x; o[j + 1] += rv.y; o[j + 2] += rv.z; o[j + 3] += rv.w;
+            }
+          }
+          if (p.res2) {
+            const float* rp = p.res2 + m * p.ldr2 + p.r2_coff + g * p.r2_gcoff + nb;
+#pragma unroll
+            for (int j = 0; j < 32; j += 4) {
+              const float4 rv = *reinterpret_cast<const float4*>(rp + j);
+              o[j] += rv.x; o[j + 1] += rv.y; o[j + 2] += rv.z; o[j + 3] += rv.w;
+            }
+          }
+          if (MODE == MODE_HALO && (BN == 32 || BN == 128) && p.pred_w) {
+            float v0 = __ldg(p.pred_b), v1 = p.pred_nc > 1 ? __ldg(p.pred_b + 1) : 0.f;
+#pragma unroll
+            for (int j = 0; j < 32; j += 4) {
+              const float4 w0 = __ldg(reinterpret_cast<const float4*>(p.pred_w + j));
+              v0 = fmaf(o[j], w0.x, v0); v0 = fmaf(o[j + 1], w0.y, v0); v0 = fmaf(o[j + 2], w0.z, v0); v0 = fmaf(o[j + 3], w0.w, v0);
+              if (p.pred_nc > 1) {
+                const float4 w1 = __ldg(reinterpret_cast<const float4*>(p.pred_w + 32 + j));
+                v1 = fmaf(o[j], w1.x, v1); v1 = fmaf(o[j + 1], w1.y, v1); v1 = fmaf(o[j + 2], w1.z, v1); v1 = fmaf(o[j + 3], w1.w, v1);
+              }
+            }
+            const long long HWl = (long long)p.H * p.W * (ph4 ? 4 : 1);
+            const long long bi = mo / HWl, pix = mo - bi * HWl;
+            float* po = p.pred_out + bi * p.pred_nc * HWl + pix;
+            if (p.pred_mode == 1) {
+              const float nrm = fmaxf(sqrtf(v0 * v0 + v1 * v1), 1e-12f);
+              po[0] = v0 / nrm; po[HWl] = v1 / nrm;
+            } else {
+              po[0] = fminf(fmaxf(v0, -1.f), 1.f);
+            }
+          }
+        }
+        // Stores.  A thread owns one row of the chunk (128 B of fp32, 64 B per bf16 plane); storing it 16 bytes at a time makes every
+        // warp-wide store touch 32 half-filled sectors.  The two lanes of an adjacent row pair (x-adjacent pixels in halo mode)
+        // exchange halves so that each store instruction writes 32 contiguous bytes per pair: full sectors, half as many per request.
+        if (chunk_ok && (p.C || (p.Shi && !staged_split))) {
+          const bool odd = lane & 1;
+          const bool valid_p = __shfl_xor_sync(0xffffffffu, (int)valid, 1) != 0;
+          const long long mo_p = mo + (odd ? -1 : 1) * (ph4 ? 2 : 1);       // the partner's row (pixel: same image row, x +- 1)
+          const long long moA = odd ? mo_p : mo, moB = odd ? mo : mo_p;     // row A = the even lane's, row B = the odd lane's
+          const bool vA = odd ? valid_p : valid, vB = odd ? valid : valid_p;
+          if (p.C) {
+            float* cA = p.C + moA * p.ldc + p.c_coff + g * p.c_gcoff + nbo + (odd ? 4 : 0);
+            float* cB = p.C + moB * p.ldc + p.c_coff + g * p.c_gcoff + nbo + (odd ? 4 : 0);
+#pragma unroll
+            for (int t = 0; t < 4; ++t) {      // float4 slots 2t (even lane) and 2t + 1 (odd lane) of both rows
+              float k[4], rr[4];
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                k[e] = odd ? o[8 * t + 4 + e] : o[8 * t + e];
+                rr[e] = __shfl_xor_sync(0xffffffffu, odd ? o[8 * t + e] : o[8 * t + 4 + e], 1);
+              }
+              if (vA) *reinterpret_cast<float4*>(cA + 8 * t) = odd ? make_float4(rr[0], rr[1], rr[2], rr[3]) : make_float4(k[0], k[1], k[2], k[3]);
+              if (vB) *reinterpret_cast<float4*>(cB + 8 * t) = odd ? make_float4(k[0], k[1], k[2], k[3]) : make_float4(rr[0], rr[1], rr[2], rr[3]);
+            }
+          }
+          if (p.Shi && !staged_split) {
+            const long long sA = moA * p.lds + p.s_coff + g * p.s_gcoff + nbo + (odd ? 8 : 0);
+            const long long sB = moB * p.lds + p.s_coff + g * p.s_gcoff + nbo + (odd ? 8 : 0);
+#pragma unroll
+            for (int t = 0; t < 2; ++t) {      // 8-column slots 2t (even lane) and 2t + 1 (odd lane) of both rows
+              float k[8], rr[8];
+#pragma unroll
+              for (int e = 0; e < 8; ++e) {
+                const float mine = odd ? o[16 * t + 8 + e] : o[16 * t + e], give = odd ? o[16 * t + e] : o[16 * t + 8 + e];
+                k[e] = p.split_relu ? fmaxf(mine, 0.f) : mine;
+                rr[e] = __shfl_xor_sync(0xffffffffu, p.split_relu ? fmaxf(give, 0.f) : give, 1);
+              }
+              uint4 kh, kl, rh, rl;
+              split_bf16x2(k[0], k[1], kh.x, kl.x); split_bf16x2(k[2], k[3], kh.y, kl.y);
+              split_bf16x2(k[4], k[5], kh.z, kl.z); split_bf16x2(k[6], k[7], kh.w, kl.w);
+              split_bf16x2(rr[0], rr[1], rh.x, rl.x); split_bf16x2(rr[2], rr[3], rh.y, rl.y);
+              split_bf16x2(rr[4], rr[5], rh.z, rl.z); split_bf16x2(rr[6], rr[7], rh.w, rl.w);
+              if (vA) {
+                *reinterpret_cast<uint4*>(p.Shi + sA + 16 * t) = odd ? rh : kh;
+                *reinterpret_cast<uint4*>(p.Slo + sA + 16 * t) = odd ? rl : kl;
+              }
+              if (vB) {
+                *reinterpret_cast<uint4*>(p.Shi + sB + 16 * t) = odd ? kh : rh;
+                *reinterpret_cast<uint4*>(p.Slo + sB + 16 * t) = odd ? kl : rl;
+              }
+            }
+          }
+        }
+      }
+      // Split planes: a thread's 32 columns are 64 B per plane, so stores from registers leave every 128 B line half written by
+      // two warps (measured on H100: 3x slower than fp32 stores of the same bytes).  The round's bf16 hi / lo values go to
+      // shared memory instead (the fp32 staging area, free once every thread has read it: 64 rows x 128 B per plane, 16 B
+      // pieces XOR-swizzled by row), and the warpgroup stores whole 128 B row segments: 8 lanes per row, 4 rows per instruction.
+      if (staged_split) {
+        named_bar_sync(1 + wg, 128);              // every thread has read its fp32 chunk of this round
+        unsigned char* sS = reinterpret_cast<unsigned char*>(stage);
+        if (ch < BN / 32) {
+#pragma unroll
+          for (int t = 0; t < 4; ++t) {           // 8-column pieces eh * 4 + t of row erow
+            uint4 h, l;
+            float k[8];
+#pragma unroll
+            for (int e = 0; e < 8; ++e) k[e] = p.split_relu ? fmaxf(o[8 * t + e], 0.f) : o[8 * t + e];
+            split_bf16x2(k[0], k[1], h.x, l.x); split_bf16x2(k[2], k[3], h.y, l.y);
+            split_bf16x2(k[4], k[5], h.z, l.z); split_bf16x2(k[6], k[7], h.w, l.w);
+            const int off = erow * 128 + (((eh * 4 + t) ^ (erow & 7)) << 4);
+            *reinterpret_cast<uint4*>(sS + off) = h;
+            *reinterpret_cast<uint4*>(sS + 64 * 128 + off) = l;
+          }
+        }
+        named_bar_sync(1 + wg, 128);
+#pragma unroll
+        for (int i = wt; i < 2 * 64 * 8; i += 128) {
+          const int lo_plane = i >> 9, rr = (i >> 3) & 63, pc = i & 7;
+          const int col = rd * 64 + pc * 8;       // column within the tile
+          if (col >= BN || n0 + col >= p.N) continue;
+          long long mr;
+          bool vr;
+          if (MODE == MODE_GEMM) {
+            mr = (long long)mt * Cfg::kTileM + (PP ? 0 : wg * 64) + rr;
+            vr = mr < p.M;
           } else {
-            po[0] = fminf(fmaxf(v0, -1.f), 1.f);
+            const int rt = wg * 64 + rr, tx = mt % tiles_x, ty = (mt / tiles_x) % tiles_y;
+            const int py = ty * kHtTileH + (rt >> 3), px = tx * kHtTileW + (rt & 7);
+            vr = py < p.H && px < p.W;
+            mr = ((long long)bimg * p.H + py) * p.W + px;
           }
-        }
-      }
-      // Stores.  A thread owns one row of the chunk (128 B of fp32, 64 B per bf16 plane); storing it 16 bytes at a time makes every
-      // warp-wide store touch 32 half-filled sectors.  The two lanes of an adjacent row pair (x-adjacent pixels in halo mode)
-      // exchange halves so that each store instruction writes 32 contiguous bytes per pair: full sectors, half as many per request.
-      if (chunk_ok && (p.C || p.Shi)) {
-        const bool odd = lane & 1;
-        const bool valid_p = __shfl_xor_sync(0xffffffffu, (int)valid, 1) != 0;
-        const long long mo_p = mo + (odd ? -1 : 1) * (ph4 ? 2 : 1);       // the partner's row (pixel: same image row, x +- 1)
-        const long long moA = odd ? mo_p : mo, moB = odd ? mo : mo_p;     // row A = the even lane's, row B = the odd lane's
-        const bool vA = odd ? valid_p : valid, vB = odd ? valid : valid_p;
-        if (p.C) {
-          float* cA = p.C + moA * p.ldc + p.c_coff + g * p.c_gcoff + nbo + (odd ? 4 : 0);
-          float* cB = p.C + moB * p.ldc + p.c_coff + g * p.c_gcoff + nbo + (odd ? 4 : 0);
-#pragma unroll
-          for (int t = 0; t < 4; ++t) {      // float4 slots 2t (even lane) and 2t + 1 (odd lane) of both rows
-            float k[4], rr[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              k[e] = odd ? o[8 * t + 4 + e] : o[8 * t + e];
-              rr[e] = __shfl_xor_sync(0xffffffffu, odd ? o[8 * t + e] : o[8 * t + 4 + e], 1);
-            }
-            if (vA) *reinterpret_cast<float4*>(cA + 8 * t) = odd ? make_float4(rr[0], rr[1], rr[2], rr[3]) : make_float4(k[0], k[1], k[2], k[3]);
-            if (vB) *reinterpret_cast<float4*>(cB + 8 * t) = odd ? make_float4(k[0], k[1], k[2], k[3]) : make_float4(rr[0], rr[1], rr[2], rr[3]);
-          }
-        }
-        if (p.Shi) {
-          const long long sA = moA * p.lds + p.s_coff + g * p.s_gcoff + nbo + (odd ? 8 : 0);
-          const long long sB = moB * p.lds + p.s_coff + g * p.s_gcoff + nbo + (odd ? 8 : 0);
-#pragma unroll
-          for (int t = 0; t < 2; ++t) {      // 8-column slots 2t (even lane) and 2t + 1 (odd lane) of both rows
-            float k[8], rr[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              const float mine = odd ? o[16 * t + 8 + e] : o[16 * t + e], give = odd ? o[16 * t + e] : o[16 * t + 8 + e];
-              k[e] = p.split_relu ? fmaxf(mine, 0.f) : mine;
-              rr[e] = __shfl_xor_sync(0xffffffffu, p.split_relu ? fmaxf(give, 0.f) : give, 1);
-            }
-            uint4 kh, kl, rh, rl;
-            split_bf16x2(k[0], k[1], kh.x, kl.x); split_bf16x2(k[2], k[3], kh.y, kl.y);
-            split_bf16x2(k[4], k[5], kh.z, kl.z); split_bf16x2(k[6], k[7], kh.w, kl.w);
-            split_bf16x2(rr[0], rr[1], rh.x, rl.x); split_bf16x2(rr[2], rr[3], rh.y, rl.y);
-            split_bf16x2(rr[4], rr[5], rh.z, rl.z); split_bf16x2(rr[6], rr[7], rh.w, rl.w);
-            if (vA) {
-              *reinterpret_cast<uint4*>(p.Shi + sA + 16 * t) = odd ? rh : kh;
-              *reinterpret_cast<uint4*>(p.Slo + sA + 16 * t) = odd ? rl : kl;
-            }
-            if (vB) {
-              *reinterpret_cast<uint4*>(p.Shi + sB + 16 * t) = odd ? kh : rh;
-              *reinterpret_cast<uint4*>(p.Slo + sB + 16 * t) = odd ? kl : rl;
-            }
-          }
+          if (!vr) continue;
+          const uint4 v = *reinterpret_cast<const uint4*>(sS + lo_plane * 64 * 128 + rr * 128 + ((pc ^ (rr & 7)) << 4));
+          *reinterpret_cast<uint4*>((lo_plane ? p.Slo : p.Shi) + mr * p.lds + p.s_coff + g * p.s_gcoff + n0 + col) = v;
         }
       }
     }

@@ -359,24 +359,27 @@ struct Fwd {
     return PF_OK;
   }
   // (two names so that the per-kernel profile separates the GEMM-mode and halo-mode launches)
-  static cudaError_t gemm_tma_gemm_mode(const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, int sms, cudaStream_t st, const PredTail* pred) {
-    return gemm_tma_launch(MODE_GEMM, maps, p, bn, kb, sms, st, pred);
+  static cudaError_t gemm_tma_gemm_mode(const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, bool pp, int sms, cudaStream_t st, const PredTail* pred) {
+    return gemm_tma_launch(MODE_GEMM, maps, p, bn, kb, pp, sms, st, pred);
   }
-  static cudaError_t gemm_tma_halo_mode(const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, int sms, cudaStream_t st, const PredTail* pred) {
-    return gemm_tma_launch(MODE_HALO, maps, p, bn, kb, sms, st, pred);
+  static cudaError_t gemm_tma_halo_mode(const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, bool pp, int sms, cudaStream_t st, const PredTail* pred) {
+    return gemm_tma_launch(MODE_HALO, maps, p, bn, kb, pp, sms, st, pred);
   }
   int force_bn = 0, force_kb = 0;     // pf_op_tma: tile override (0 = the dispatcher's choice)
-  int picked_bn = 0, picked_kb = 0;   // (bn, kb) of the last TMA launch
-  // the one place a launch's (bn, kb) is chosen: tgemm / thalo build the B maps with it and hand it to launch_tma
-  int pick_tile(int mode, const TmaGemmParams& p, const PredTail* pred, int& bn, int& kb) {
+  int force_sched = 0;                // pf_op_tma: GEMM-mode schedule override (0 = the dispatcher's choice, 1 cooperative, 2 ping-pong)
+  int picked_bn = 0, picked_kb = 0, picked_sched = 0;   // (bn, kb, schedule) of the last TMA launch
+  // the one place a launch's (bn, kb) and schedule are chosen: tgemm / thalo build the A and B maps with them and hand them to
+  // launch_tma.  pp: the ping-pong schedule (GEMM mode only).
+  int pick_tile(int mode, const TmaGemmParams& p, const PredTail* pred, int& bn, int& kb, bool& pp) {
     tma_pick_tile(mode, p.M, p.N, p.K, e->sm_count, bn, kb);
     if (force_bn) { bn = force_bn; kb = tma_pick_kb(bn, p.K, mode); }
     if (force_kb) kb = force_kb;
-    if (const char* msg = gemm_tma_check(mode, p, bn, kb, pred != nullptr)) return fail(PF_ERR_ARG, "TMA engine, %s (bn %d, kb %d): %s", mode == MODE_GEMM ? "GEMM mode" : "halo mode", bn, kb, msg);
-    picked_bn = bn; picked_kb = kb;
+    pp = mode == MODE_GEMM && (force_sched ? force_sched == 2 : tma_pick_pingpong(p.M, p.N, p.K, bn, e->sm_count));
+    if (const char* msg = gemm_tma_check(mode, p, bn, kb, pred != nullptr, pp)) return fail(PF_ERR_ARG, "TMA engine, %s (bn %d, kb %d): %s", mode == MODE_GEMM ? "GEMM mode" : "halo mode", bn, kb, msg);
+    picked_bn = bn; picked_kb = kb; picked_sched = mode == MODE_GEMM ? (pp ? 2 : 1) : 0;
     return PF_OK;
   }
-  int launch_tma(int mode, const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, const PredTail* pred = nullptr) {
+  int launch_tma(int mode, const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, bool pp, const PredTail* pred = nullptr) {
     if (e->profile) {
       pf_engine::ProfRec r{};
       for (cudaEvent_t* ev : {&r.a, &r.b}) {
@@ -388,14 +391,14 @@ struct Fwd {
       r.cfg = mode == MODE_GEMM ? 5 : 6;
       r.M = (int)Mrows; r.N = p.N; r.K = p.K; r.KH = mode == MODE_GEMM ? 1 : 3; r.stride = 1; r.groups = p.groups; r.Cin = p.Cin;
       CU(cudaEventRecord(r.a, st));
-      if (mode == MODE_GEMM) LAUNCHED(gemm_tma_gemm_mode(maps, p, bn, kb, e->sm_count, st, pred));
-      else LAUNCHED(gemm_tma_halo_mode(maps, p, bn, kb, e->sm_count, st, pred));
+      if (mode == MODE_GEMM) LAUNCHED(gemm_tma_gemm_mode(maps, p, bn, kb, pp, e->sm_count, st, pred));
+      else LAUNCHED(gemm_tma_halo_mode(maps, p, bn, kb, pp, e->sm_count, st, pred));
       CU(cudaEventRecord(r.b, st));
       e->prof.push_back(r);
       return PF_OK;
     }
-    if (mode == MODE_GEMM) LAUNCHED(gemm_tma_gemm_mode(maps, p, bn, kb, e->sm_count, st, pred));
-    else LAUNCHED(gemm_tma_halo_mode(maps, p, bn, kb, e->sm_count, st, pred));
+    if (mode == MODE_GEMM) LAUNCHED(gemm_tma_gemm_mode(maps, p, bn, kb, pp, e->sm_count, st, pred));
+    else LAUNCHED(gemm_tma_halo_mode(maps, p, bn, kb, pp, e->sm_count, st, pred));
     return PF_OK;
   }
   struct Epi {   // epilogue options of one TMA GEMM / conv
@@ -444,15 +447,17 @@ struct Fwd {
     fill_epi(p, w, o, 0);
     TmaMaps maps{};
     int bn, kb;
-    TRY(pick_tile(MODE_GEMM, p, nullptr, bn, kb));
+    bool pp;
+    TRY(pick_tile(MODE_GEMM, p, nullptr, bn, kb, pp));
     const char* msg = nullptr;
-    if (!msg) msg = map2d(&maps.a_hi, A.hi, A.ld, M, A.ld, 128, kb);
-    if (!msg) msg = map2d(&maps.a_lo, A.lo, A.ld, M, A.ld, 128, kb);
+    const int a_rows = pp ? 64 : 128;     // A box = one tile's rows
+    if (!msg) msg = map2d(&maps.a_hi, A.hi, A.ld, M, A.ld, a_rows, kb);
+    if (!msg) msg = map2d(&maps.a_lo, A.lo, A.ld, M, A.ld, a_rows, kb);
     if (!msg) msg = map2d(&maps.b_hi, w.hi, K, N, K, bn, kb);
     if (!msg) msg = map2d(&maps.b_lo, w.lo, K, N, K, bn, kb);
     if (msg) return fail(PF_ERR_CUDA, "%s", msg);
     maps.a2_hi = maps.a_hi; maps.a2_lo = maps.a_lo;
-    return launch_tma(MODE_GEMM, maps, p, bn, kb);
+    return launch_tma(MODE_GEMM, maps, p, bn, kb, pp);
   }
   // 3x3 / stride 1 / pad 1 convolution on split NHWC planes (optionally a second source for channels >= c_split)
   int thalo(const SplitT& A, int a_c0, int a_gc, const SplitT* A2, int c_split, int a2_c0, int B, int H, int W, int Cin, const GemmW& w, int N,
@@ -467,7 +472,8 @@ struct Fwd {
     fill_epi(p, w, o, bias_gstride);
     TmaMaps maps{};
     int bn, kb;
-    TRY(pick_tile(MODE_HALO, p, pred, bn, kb));
+    bool pp;
+    TRY(pick_tile(MODE_HALO, p, pred, bn, kb, pp));
     const char* msg = nullptr;
     if (!msg) msg = map_halo(&maps.a_hi, A.hi, B, H, W, A.ld);
     if (!msg) msg = map_halo(&maps.a_lo, A.lo, B, H, W, A.ld);
@@ -478,7 +484,7 @@ struct Fwd {
     if (!msg) msg = map2d(&maps.b_hi, w.hi, p.K, (long long)groups * N, p.K, bn, kb);
     if (!msg) msg = map2d(&maps.b_lo, w.lo, p.K, (long long)groups * N, p.K, bn, kb);
     if (msg) return fail(PF_ERR_CUDA, "%s", msg);
-    return launch_tma(MODE_HALO, maps, p, bn, kb, pred);
+    return launch_tma(MODE_HALO, maps, p, bn, kb, pp, pred);
   }
   // strided / patchifying convolution = patch gather on split planes + TMA GEMM
   int tconv_gather(const SplitT& A, int B, int H, int W, int Cin, int KH, int stride, int pad, const GemmW& w, int N, const Epi& o) {
@@ -1398,7 +1404,8 @@ int pf_op_tma(pf_tma_op* op, void* stream) {
   tmp.device = dev;
   tmp.sm_count = prop.multiProcessorCount;
   Fwd F{&tmp, Arena{}, (cudaStream_t)stream, false, q.B};
-  F.force_bn = q.force_bn; F.force_kb = q.force_kb;
+  if (q.force_sched < 0 || q.force_sched > 2 || (q.force_sched && q.mode != MODE_GEMM)) return fail(PF_ERR_ARG, "pf_op_tma: force_sched %d", q.force_sched);
+  F.force_bn = q.force_bn; F.force_kb = q.force_kb; F.force_sched = q.force_sched;
   const SplitT A{(__nv_bfloat16*)q.a_hi, (__nv_bfloat16*)q.a_lo, q.lda};
   const SplitT A2{(__nv_bfloat16*)q.a2_hi, (__nv_bfloat16*)q.a2_lo, q.lda2};
   const GemmW w{(const __nv_bfloat16*)q.w_hi, (const __nv_bfloat16*)q.w_lo, q.bias};
@@ -1415,11 +1422,11 @@ int pf_op_tma(pf_tma_op* op, void* stream) {
     if (!s.w || !s.b || !s.out || !(s.mode == 1 ? s.nc == 2 : (s.mode == 2 && s.nc == 1))) return fail(PF_ERR_ARG, "pf_op_tma: prediction tail %d", g);
     pt[g] = PredTail{s.w, s.b, s.out, s.nc, s.mode};
   }
-  op->picked_bn = op->picked_kb = 0;
+  op->picked_bn = op->picked_kb = op->picked_sched = 0;
   const int r = q.mode == MODE_GEMM ? F.tgemm(A, q.M, q.K, q.a_c0, w, q.N, o)
                                     : F.thalo(A, q.a_c0, q.a_gc, q.a2_hi ? &A2 : nullptr, q.c_split, q.a2_c0, q.B, q.H, q.W, q.Cin, w, q.N, q.groups,
                                               q.bias_gstride, o, q.npred ? pt : nullptr);
-  if (r == PF_OK) { op->picked_bn = F.picked_bn; op->picked_kb = F.picked_kb; }
+  if (r == PF_OK) { op->picked_bn = F.picked_bn; op->picked_kb = F.picked_kb; op->picked_sched = F.picked_sched; }
   return r;
 }
 int pf_op_conv1_ring(const void* c_hi, const void* c_lo, int B, int H, int W, const float* wf, const float* bias, float* out,

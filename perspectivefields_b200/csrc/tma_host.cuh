@@ -100,13 +100,23 @@ inline void tma_pick_tile(int mode, long long M, int N, int K, int sm_count, int
   kb = tma_pick_kb(bn, K, mode);
 }
 
+// GEMM-mode schedule on top of (bn, kb): ping-pong (64-row tiles, one warpgroup's epilogue under the other's main loop) or
+// cooperative (128-row tiles, both warpgroups on one tile).  Ping-pong for K <= 512 when the 64-row tiles fill every CTA with
+// at least two.  Measured per launch on the C2 forward (H100 80GB HBM3, 400 W; tools/launch_floors.py), this rule saved about
+// 1 ms per step against the cooperative schedule.  Ping-pong on every launch was slower on the wide short-K ConvNeXt stage-0
+// pw1 (M = 204800, K = 96).
+constexpr int kPingPongKMax = 512;
+inline bool tma_pick_pingpong(long long M, int N, int K, int bn, int sm_count) {
+  return K <= kPingPongKMax && cdivl(M, 64) * cdiv(N, bn) >= 2LL * sm_count;
+}
+
 struct PredTail { const float* w; const float* b; float* out; int nc, mode; };   // per group, see TmaGemmParams::pred_*
 
-template <int BN, int MODE, int KB>
+template <int BN, int MODE, int KB, bool PP = false>
 inline cudaError_t gemm_tma_launch_bn(const TmaMaps& maps, const TmaGemmParams& p, int sm_count, cudaStream_t st, const PredTail* pred) {
-  using Cfg = TmaCfg<BN, MODE, KB>;   // (the > 48 KB shared-memory opt-in is per device: gemm_tma_configure_device, at pf_create)
+  using Cfg = TmaCfg<BN, MODE, KB, PP>;   // (the > 48 KB shared-memory opt-in is per device: gemm_tma_configure_device, at pf_create)
   const int tiles_x = MODE == MODE_HALO ? cdiv(p.W, kHtTileW) : 0, tiles_y = MODE == MODE_HALO ? cdiv(p.H, kHtTileH) : 0;
-  const long long m_tiles = MODE == MODE_GEMM ? cdiv(p.M, 128) : (long long)p.B * tiles_x * tiles_y;
+  const long long m_tiles = MODE == MODE_GEMM ? cdiv(p.M, Cfg::kTileM) : (long long)p.B * tiles_x * tiles_y;
   const long long total = m_tiles * cdiv(p.N, BN) * p.groups;
   const unsigned grid = (unsigned)(total < sm_count ? total : sm_count);
   // resident-weight mode (single chunk, one N tile) assumes every tile of a CTA uses the same weights: one group per launch
@@ -130,7 +140,7 @@ inline cudaError_t gemm_tma_launch_bn(const TmaMaps& maps, const TmaGemmParams& 
       }
     return last;
   }
-  return launch_pdl(gemm_tma_kernel<BN, MODE, KB>, dim3(grid), dim3(kTmaThreads), Cfg::kSmemBytes, st, maps, p, tiles_x, tiles_y);
+  return launch_pdl(gemm_tma_kernel<BN, MODE, KB, PP>, dim3(grid), dim3(kTmaThreads), Cfg::kSmemBytes, st, maps, p, tiles_x, tiles_y);
 }
 
 // every instantiation the dispatcher below can reach: X(BN, MODE, KB)
@@ -138,6 +148,9 @@ inline cudaError_t gemm_tma_launch_bn(const TmaMaps& maps, const TmaGemmParams& 
   X(256, MODE_GEMM, 32) X(224, MODE_GEMM, 32) X(192, MODE_GEMM, 32) X(160, MODE_GEMM, 32) X(128, MODE_GEMM, 32) X(96, MODE_GEMM, 32) \
   X(64, MODE_GEMM, 32) X(32, MODE_GEMM, 32) X(64, MODE_GEMM, 64) X(32, MODE_GEMM, 64)                                        \
   X(256, MODE_HALO, 32) X(128, MODE_HALO, 64) X(64, MODE_HALO, 64) X(32, MODE_HALO, 64)
+// the GEMM-mode (bn, kb) pairs above, in the ping-pong schedule: X(BN, KB)
+#define PF_TMA_PINGPONG_VARIANTS(X)                                                                                         \
+  X(256, 32) X(224, 32) X(192, 32) X(160, 32) X(128, 32) X(96, 32) X(64, 32) X(32, 32) X(64, 64) X(32, 64)
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a per-device (per-context) attribute: called once for every device an engine is
 // created on (pf_create) -- not behind a process-wide flag.
@@ -147,23 +160,30 @@ inline cudaError_t gemm_tma_configure_device() {
   if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_tma_kernel<BN_, MODE_, KB_>, cudaFuncAttributeMaxDynamicSharedMemorySize, TmaCfg<BN_, MODE_, KB_>::kSmemBytes);
   PF_TMA_VARIANTS(PF_TMA_CFG)
 #undef PF_TMA_CFG
+#define PF_TMA_CFG_PP(BN_, KB_)                                                                                               \
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_tma_kernel<BN_, MODE_GEMM, KB_, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TmaCfg<BN_, MODE_GEMM, KB_, true>::kSmemBytes);
+  PF_TMA_PINGPONG_VARIANTS(PF_TMA_CFG_PP)
+#undef PF_TMA_CFG_PP
   return e;
 }
 
-// ring depth of an instantiation, 0 if PF_TMA_VARIANTS does not list it
-inline int tma_stages(int mode, int bn, int kb) {
-#define PF_TMA_NS(BN_, MODE_, KB_) if (mode == MODE_ && bn == BN_ && kb == KB_) return TmaCfg<BN_, MODE_, KB_>::kStages;
+// ring depth of an instantiation, 0 if PF_TMA_VARIANTS (pp: PF_TMA_PINGPONG_VARIANTS) does not list it
+inline int tma_stages(int mode, int bn, int kb, bool pp = false) {
+#define PF_TMA_NS(BN_, MODE_, KB_) if (!pp && mode == MODE_ && bn == BN_ && kb == KB_) return TmaCfg<BN_, MODE_, KB_>::kStages;
   PF_TMA_VARIANTS(PF_TMA_NS)
 #undef PF_TMA_NS
+#define PF_TMA_NS_PP(BN_, KB_) if (pp && mode == MODE_GEMM && bn == BN_ && kb == KB_) return TmaCfg<BN_, MODE_GEMM, KB_, true>::kStages;
+  PF_TMA_PINGPONG_VARIANTS(PF_TMA_NS_PP)
+#undef PF_TMA_NS_PP
   return 0;
 }
 
 // Why the (bn, kb) instantiation cannot compute p: nullptr when it can.  Every case here would otherwise launch something that
 // computes a different result (a K tail, a prediction tail or phase layout the tile width does not implement) or that
 // gemm_tma_launch_bn refuses after the fact (resident weights over several N tiles).
-inline const char* gemm_tma_check(int mode, const TmaGemmParams& p, int bn, int kb, bool pred) {
-  const int ns = tma_stages(mode, bn, kb);
-  if (!ns) return "no engine instantiation for this (mode, bn, kb)";
+inline const char* gemm_tma_check(int mode, const TmaGemmParams& p, int bn, int kb, bool pred, bool pp = false) {
+  const int ns = tma_stages(mode, bn, kb, pp);
+  if (!ns) return pp ? "no ping-pong engine instantiation for this (mode, bn, kb)" : "no engine instantiation for this (mode, bn, kb)";
   if (mode == MODE_GEMM) return p.K % kb ? "GEMM mode: K must be a multiple of the K step" : nullptr;
   if (p.phase4 && (p.N != 128 || bn != 128)) return "phase4 needs N = 128 in one 128-wide tile";
   if (pred && bn != (p.phase4 ? 128 : 32)) return "the fused prediction tail needs N = 32 (phase4: 128) in one tile";
@@ -172,11 +192,14 @@ inline const char* gemm_tma_check(int mode, const TmaGemmParams& p, int bn, int 
   return nullptr;
 }
 
-inline cudaError_t gemm_tma_launch(int mode,const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, int sm_count, cudaStream_t st,
+inline cudaError_t gemm_tma_launch(int mode, const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, bool pp, int sm_count, cudaStream_t st,
                                    const PredTail* pred = nullptr) {
-#define PF_TMA_CASE(BN_, MODE_, KB_) if (mode == MODE_ && bn == BN_ && kb == KB_) return gemm_tma_launch_bn<BN_, MODE_, KB_>(maps, p, sm_count, st, pred);
+#define PF_TMA_CASE(BN_, MODE_, KB_) if (!pp && mode == MODE_ && bn == BN_ && kb == KB_) return gemm_tma_launch_bn<BN_, MODE_, KB_>(maps, p, sm_count, st, pred);
   PF_TMA_VARIANTS(PF_TMA_CASE)
 #undef PF_TMA_CASE
+#define PF_TMA_CASE_PP(BN_, KB_) if (pp && mode == MODE_GEMM && bn == BN_ && kb == KB_) return gemm_tma_launch_bn<BN_, MODE_GEMM, KB_, true>(maps, p, sm_count, st, pred);
+  PF_TMA_PINGPONG_VARIANTS(PF_TMA_CASE_PP)
+#undef PF_TMA_CASE_PP
   return cudaErrorInvalidValue;
 }
 
