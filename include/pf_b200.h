@@ -115,7 +115,12 @@ int pf_profile_kernels_read(pf_handle h, char* buf, int cap);
  * "dw_ln" (default 0): ConvNeXt depthwise 7x7 fused with the LayerNorm behind it (slower than the separate kernels).
  * "decode_only" (default 0; classification heads, SURVEY.md 8f-3): the 73 / 180 logits are never written -- the 1x1 prediction
  *   conv, argmax and bin decode (gravity_head.py:243-244 + utils/utils.py:114-130, latitude_head.py:205-208 + utils.py:148-162)
- *   run in one kernel and pred_gravity / pred_latitude receive the decoded fields [n,2,320,320] / [n,1,320,320] (degrees). */
+ *   run in one kernel and pred_gravity / pred_latitude receive the decoded fields [n,2,320,320] / [n,1,320,320] (degrees).
+ * "bf16" (default 0; NOT the reference's numerics, DESIGN.md section 3): every tensor-core product -- the TMA -> wgmma engine's
+ *   GEMMs and 3x3 convolutions, the 7x7 stems and both products of the mma.sync attention core -- is one bf16 MMA of the
+ *   operands' hi planes (bf16-rounded operands, fp32 accumulation) instead of the three of the split-precision scheme.  The
+ *   CUDA-core kernels (LayerNorm, depthwise convolutions, resampling, softmax, prediction tails, the conv1 border ring, the
+ *   ParamNet stem and tail) stay fp32.  Read at every launch: it can be switched between pf_forward calls on one handle. */
 int pf_set_option(pf_handle h, const char* name, int value);
 
 /* Debug taps (tests only): when enabled, intermediates of the next pf_forward are kept (never recycled) and can be
@@ -215,6 +220,9 @@ typedef struct pf_tma_op {
   int force_sched, picked_sched;
 } pf_tma_op;
 int pf_op_tma(pf_tma_op* op, void* stream);
+/* pf_op_tma in the bf16 precision mode (option "bf16"): the same struct, semantics and tile override, with one bf16 MMA per
+ * product (A_hi * W_hi^T; a_lo / w_lo must still be valid pointers and are not read).  Split outputs still get both planes. */
+int pf_op_tma_bf16(pf_tma_op* op, void* stream);
 /* The border ring of the phase-composed conv_fuse_conv1 (the two outermost rows / columns of the 2H x 2W output, H, W >= 2),
  * recomputed in fp32 as pf_forward does after the phase4 launch: c_hi / c_lo: split planes [B, H, W, 128] (head 0 channels
  * 0-63, head 1 64-127); wf: fp32 [2][9 taps][64 ci][32 o]; bias [2][32]; out: NHWC [B, 2H, 2W, 64] or NULL; with pg_w the
@@ -228,6 +236,7 @@ int pf_op_layernorm(const float* x, float* y, int64_t rows, int C, const float* 
 int pf_op_attention(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream);      /* CUDA-core fp32 */
 int pf_op_attention_mma(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream);  /* warp-level mma.sync, bf16x3 */
 int pf_op_attention_tc(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream);   /* q / kv split into bf16 hi/lo planes first, then the mma.sync core as the forward graph runs it */
+int pf_op_attention_tc_bf16(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream); /* the same in the bf16 precision mode: one mma.sync per product on bf16(q), bf16(k), bf16(P), bf16(v) */
 int pf_op_dwconv3x3_gelu(const float* x, float* y, int B, int H, int W, int C, const float* w9c, const float* bias, void* stream);
 int pf_op_dwconv7x7(const float* x, float* y, int B, int H, int W, int C, const float* w49c, const float* bias, void* stream);
 int pf_op_upsample2x(const float* x, float* y, int B, int H, int W, int C, void* stream);

@@ -130,6 +130,7 @@ def lib():
         "pf_debug_copy": (i32, [vp, ctypes.c_char_p, vp, i64, vp]),
         "pf_op_conv_gemm": (i32, [vp, i32, i32, i32, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp, i32, vp, vp]),
         "pf_op_tma": (i32, [ctypes.POINTER(pf_tma_op), vp]),
+        "pf_op_tma_bf16": (i32, [ctypes.POINTER(pf_tma_op), vp]),
         "pf_op_conv1_ring": (i32, [vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
         "pf_tma_pick_tile": (i32, [i32, i64, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32)]),
         "pf_set_option": (i32, [vp, ctypes.c_char_p, i32]),
@@ -138,6 +139,7 @@ def lib():
         "pf_op_attention": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
         "pf_op_attention_mma": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
         "pf_op_attention_tc": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
+        "pf_op_attention_tc_bf16": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
         "pf_op_dwconv3x3_gelu": (i32, [vp, vp, i32, i32, i32, i32, vp, vp, vp]),
         "pf_op_dwconv7x7": (i32, [vp, vp, i32, i32, i32, i32, vp, vp, vp]),
         "pf_op_upsample2x": (i32, [vp, vp, i32, i32, i32, i32, vp]),
@@ -178,7 +180,8 @@ EXPORTS = ["pf_abi_version", "pf_last_error", "pf_kernel_launch_count", "pf_crea
            "pf_profile_kernels_read", "pf_set_option", "pf_debug_enable", "pf_debug_count", "pf_debug_name", "pf_debug_numel",
            "pf_debug_copy", "pf_camera_fields", "pf_comm_unique_id", "pf_comm_create", "pf_comm_destroy", "pf_gather",
            "pf_jpeg_create", "pf_jpeg_destroy", "pf_jpeg_info", "pf_jpeg_decode_batch",
-           "pf_op_conv_gemm", "pf_op_tma", "pf_op_conv1_ring", "pf_tma_pick_tile", "pf_op_layernorm", "pf_op_attention", "pf_op_attention_mma", "pf_op_attention_tc", "pf_op_dwconv3x3_gelu", "pf_op_dwconv7x7",
+           "pf_op_conv_gemm", "pf_op_tma", "pf_op_tma_bf16", "pf_op_conv1_ring", "pf_tma_pick_tile", "pf_op_layernorm", "pf_op_attention",
+           "pf_op_attention_mma", "pf_op_attention_tc", "pf_op_attention_tc_bf16", "pf_op_dwconv3x3_gelu", "pf_op_dwconv7x7",
            "pf_op_upsample2x", "pf_op_preprocess", "pf_op_fill_stream", "pf_op_resize_u8", "pf_op_resize_f32", "pf_op_argmax_decode",
            "pf_op_pred_argmax_decode", "pf_op_postprocess"]
 

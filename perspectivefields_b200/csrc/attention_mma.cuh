@@ -8,6 +8,9 @@
 //   passes of 64 queries (16 per warp); passes per block are chosen so that the grid is about one resident wave.  Per warp and tile: S = q k^T (mma.sync.m16n8k16, 4 k-steps x 14 key tiles x 3),
 //   row softmax in registers (quad shuffles), O = P V (7 k-steps x 8 tiles x 3; P re-used from the S accumulators as the A
 //   operand, V through ldmatrix.trans), normalise, store fp32 and/or split planes.
+//
+//   NP = 1 (the opt-in bf16 precision mode): K and V are staged as hi planes only (28 KB per block), Q fragments are hi only,
+//   and each product is one mma.sync (hi*hi) with P rounded to bf16 once.  The softmax stays fp32.
 #pragma once
 #include "common.cuh"
 
@@ -16,6 +19,7 @@ namespace pf {
 constexpr int kAmKeys = 100, kAmKeysPad = 112, kAmD = 64, kAmQTile = 64, kAmThreads = 128;   // 4 warps x 16 queries per pass
 constexpr int kAmPlane = kAmKeysPad * kAmD * 2;      // bytes of one bf16 plane (K or V, hi or lo)
 constexpr int kAmSmem = 4 * kAmPlane;                // K_hi, K_lo, V_hi, V_lo = 57344 B
+template <int NP> constexpr int am_smem() { return NP == 3 ? kAmSmem : 2 * kAmPlane; }   // NP = 1: K_hi, V_hi
 
 __device__ __forceinline__ void ldmatrix_x4_trans(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];\n"
@@ -25,28 +29,32 @@ __device__ __forceinline__ void ldmatrix_x4_trans(uint32_t addr, uint32_t& r0, u
 // SPLIT_IN: q and kv arrive as bf16 hi/lo planes (written by the q / kv GEMM epilogues): K and V are copied into shared memory
 // with cp.async (no conversion work), Q fragments are read as bf16 pairs; the 1/8 scale is applied to S in fp32 (a power of
 // two: identical to scaling q).  Otherwise q, kv are fp32 (operator entry point, legacy graph) and are split on the fly.
-template <bool SPLIT_IN>
+template <bool SPLIT_IN, int NP = 3>
 __global__ void __launch_bounds__(kAmThreads) attention_mma_kernel(const float* __restrict__ q, const float* __restrict__ kv,
                                                                    const __nv_bfloat16* __restrict__ q_hi, const __nv_bfloat16* __restrict__ q_lo,
                                                                    const __nv_bfloat16* __restrict__ kv_hi, const __nv_bfloat16* __restrict__ kv_lo,
                                                                    float* __restrict__ out,
                                                                    __nv_bfloat16* __restrict__ shi, __nv_bfloat16* __restrict__ slo, int N, int C,
                                                                    int tiles_per_block) {
+  static_assert(NP == 1 || NP == 3, "NP");
+  constexpr bool kLo = NP == 3;
+  constexpr int kPl = kLo ? 2 : 1;                    // planes per operand (K, V): hi + lo, or hi
   pdl_wait();
   pdl_launch();
   extern __shared__ __align__(128) unsigned char sm_raw[];
-  const uint32_t sK_hi = smem_u32(sm_raw), sK_lo = sK_hi + kAmPlane, sV_hi = sK_lo + kAmPlane, sV_lo = sV_hi + kAmPlane;
+  const uint32_t sK_hi = smem_u32(sm_raw), sK_lo = sK_hi + kAmPlane, sV_hi = sK_hi + kPl * kAmPlane, sV_lo = sV_hi + kAmPlane;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int b = blockIdx.z, h = blockIdx.y;
   // ---- stage K and V of this (image, head): fp32 -> bf16 hi/lo, [key][64] rows of 128 B, chunk (16 B) index ^= key & 7
   if (SPLIT_IN) {
-    // 4 planes (K_hi, K_lo, V_hi, V_lo) x 112 keys x 8 chunks of 16 B
+    // 2 kPl planes (K_hi, K_lo, V_hi, V_lo; NP = 1: K_hi, V_hi) x 112 keys x 8 chunks of 16 B
     const long long kvo = (long long)b * kAmKeys * 2 * C + h * kAmD;
-    for (int i = tid; i < 4 * kAmKeysPad * 8; i += kAmThreads) {
+    for (int i = tid; i < 2 * kPl * kAmKeysPad * 8; i += kAmThreads) {
       const int plane = i / (kAmKeysPad * 8), j = i % (kAmKeysPad * 8), key = j >> 3, c = j & 7;
       const uint32_t dst = sK_hi + plane * kAmPlane + (uint32_t)key * 128u + (uint32_t)((c ^ (key & 7)) << 4);
       const bool valid = key < kAmKeys;    // keys 100..111: zero fill (src-size 0)
-      const __nv_bfloat16* src = ((plane & 1) ? kv_lo : kv_hi) + kvo + (long long)(valid ? key : 0) * 2 * C + ((plane >> 1) ? C : 0) + c * 8;
+      const int lo = plane % kPl, isv = plane / kPl;
+      const __nv_bfloat16* src = (lo ? kv_lo : kv_hi) + kvo + (long long)(valid ? key : 0) * 2 * C + (isv ? C : 0) + c * 8;
       cp_async16(dst, src, valid);
     }
     cp_async_commit();
@@ -63,9 +71,9 @@ __global__ void __launch_bounds__(kAmThreads) attention_mma_kernel(const float* 
     split_bf16x2(v.x, v.y, hh.x, ll.x);
     split_bf16x2(v.z, v.w, hh.y, ll.y);
     const uint32_t off = (uint32_t)key * 128u + (uint32_t)(((d4 >> 1) ^ (key & 7)) << 4) + (uint32_t)(d4 & 1) * 8u;
-    unsigned char* base = sm_raw + (isv ? 2 * kAmPlane : 0);
+    unsigned char* base = sm_raw + (isv ? kPl * kAmPlane : 0);
     *reinterpret_cast<uint2*>(base + off) = hh;
-    *reinterpret_cast<uint2*>(base + kAmPlane + off) = ll;
+    if (kLo) *reinterpret_cast<uint2*>(base + kAmPlane + off) = ll;
   }
   __syncthreads();
 
@@ -81,10 +89,16 @@ __global__ void __launch_bounds__(kAmThreads) attention_mma_kernel(const float* 
 #pragma unroll
       for (int ks = 0; ks < 4; ++ks) {
         const int c0 = ks * 16 + 2 * t;
-        qh[ks][0] = __ldg(reinterpret_cast<const uint32_t*>(q_hi + o0 + c0));     ql[ks][0] = __ldg(reinterpret_cast<const uint32_t*>(q_lo + o0 + c0));
-        qh[ks][1] = __ldg(reinterpret_cast<const uint32_t*>(q_hi + o1 + c0));     ql[ks][1] = __ldg(reinterpret_cast<const uint32_t*>(q_lo + o1 + c0));
-        qh[ks][2] = __ldg(reinterpret_cast<const uint32_t*>(q_hi + o0 + c0 + 8)); ql[ks][2] = __ldg(reinterpret_cast<const uint32_t*>(q_lo + o0 + c0 + 8));
-        qh[ks][3] = __ldg(reinterpret_cast<const uint32_t*>(q_hi + o1 + c0 + 8)); ql[ks][3] = __ldg(reinterpret_cast<const uint32_t*>(q_lo + o1 + c0 + 8));
+        qh[ks][0] = __ldg(reinterpret_cast<const uint32_t*>(q_hi + o0 + c0));
+        qh[ks][1] = __ldg(reinterpret_cast<const uint32_t*>(q_hi + o1 + c0));
+        qh[ks][2] = __ldg(reinterpret_cast<const uint32_t*>(q_hi + o0 + c0 + 8));
+        qh[ks][3] = __ldg(reinterpret_cast<const uint32_t*>(q_hi + o1 + c0 + 8));
+        if (kLo) {
+          ql[ks][0] = __ldg(reinterpret_cast<const uint32_t*>(q_lo + o0 + c0));
+          ql[ks][1] = __ldg(reinterpret_cast<const uint32_t*>(q_lo + o1 + c0));
+          ql[ks][2] = __ldg(reinterpret_cast<const uint32_t*>(q_lo + o0 + c0 + 8));
+          ql[ks][3] = __ldg(reinterpret_cast<const uint32_t*>(q_lo + o1 + c0 + 8));
+        }
       }
     } else {
       const float* q0p = q + ((long long)b * N + (r0 < N ? r0 : N - 1)) * C + h * kAmD;
@@ -113,15 +127,21 @@ __global__ void __launch_bounds__(kAmThreads) attention_mma_kernel(const float* 
         const int key = np * 16 + (lane & 7) + ((lane >> 4) << 3);
         const int chunk = ks * 2 + ((lane >> 3) & 1);
         const uint32_t off = (uint32_t)key * 128u + (uint32_t)((chunk ^ (key & 7)) << 4);
-        uint32_t bh0, bh1, bh2, bh3, bl0, bl1, bl2, bl3;
+        uint32_t bh0, bh1, bh2, bh3;
         ldmatrix_x4(sK_hi + off, bh0, bh1, bh2, bh3);
-        ldmatrix_x4(sK_lo + off, bl0, bl1, bl2, bl3);
-        mma_bf16_16816(s[2 * np], ql[ks], bh0, bh1);
-        mma_bf16_16816(s[2 * np], qh[ks], bl0, bl1);
-        mma_bf16_16816(s[2 * np], qh[ks], bh0, bh1);
-        mma_bf16_16816(s[2 * np + 1], ql[ks], bh2, bh3);
-        mma_bf16_16816(s[2 * np + 1], qh[ks], bl2, bl3);
-        mma_bf16_16816(s[2 * np + 1], qh[ks], bh2, bh3);
+        if (kLo) {
+          uint32_t bl0, bl1, bl2, bl3;
+          ldmatrix_x4(sK_lo + off, bl0, bl1, bl2, bl3);
+          mma_bf16_16816(s[2 * np], ql[ks], bh0, bh1);
+          mma_bf16_16816(s[2 * np], qh[ks], bl0, bl1);
+          mma_bf16_16816(s[2 * np], qh[ks], bh0, bh1);
+          mma_bf16_16816(s[2 * np + 1], ql[ks], bh2, bh3);
+          mma_bf16_16816(s[2 * np + 1], qh[ks], bl2, bl3);
+          mma_bf16_16816(s[2 * np + 1], qh[ks], bh2, bh3);
+        } else {
+          mma_bf16_16816(s[2 * np], qh[ks], bh0, bh1);
+          mma_bf16_16816(s[2 * np + 1], qh[ks], bh2, bh3);
+        }
       }
     }
     // ---- softmax over the 100 valid keys (rows r0: regs 0,1 ; r1: regs 2,3), fp32
@@ -164,15 +184,21 @@ __global__ void __launch_bounds__(kAmThreads) attention_mma_kernel(const float* 
         const int key = j * 16 + (lane & 7) + (((lane >> 3) & 1) << 3);
         const int chunk = np * 2 + (lane >> 4);
         const uint32_t off = (uint32_t)key * 128u + (uint32_t)((chunk ^ (key & 7)) << 4);
-        uint32_t vh0, vh1, vh2, vh3, vl0, vl1, vl2, vl3;
+        uint32_t vh0, vh1, vh2, vh3;
         ldmatrix_x4_trans(sV_hi + off, vh0, vh1, vh2, vh3);
-        ldmatrix_x4_trans(sV_lo + off, vl0, vl1, vl2, vl3);
-        mma_bf16_16816(o[2 * np], pl, vh0, vh1);
-        mma_bf16_16816(o[2 * np], ph, vl0, vl1);
-        mma_bf16_16816(o[2 * np], ph, vh0, vh1);
-        mma_bf16_16816(o[2 * np + 1], pl, vh2, vh3);
-        mma_bf16_16816(o[2 * np + 1], ph, vl2, vl3);
-        mma_bf16_16816(o[2 * np + 1], ph, vh2, vh3);
+        if (kLo) {
+          uint32_t vl0, vl1, vl2, vl3;
+          ldmatrix_x4_trans(sV_lo + off, vl0, vl1, vl2, vl3);
+          mma_bf16_16816(o[2 * np], pl, vh0, vh1);
+          mma_bf16_16816(o[2 * np], ph, vl0, vl1);
+          mma_bf16_16816(o[2 * np], ph, vh0, vh1);
+          mma_bf16_16816(o[2 * np + 1], pl, vh2, vh3);
+          mma_bf16_16816(o[2 * np + 1], ph, vl2, vl3);
+          mma_bf16_16816(o[2 * np + 1], ph, vh2, vh3);
+        } else {
+          mma_bf16_16816(o[2 * np], ph, vh0, vh1);
+          mma_bf16_16816(o[2 * np + 1], ph, vh2, vh3);
+        }
       }
     }
     // ---- normalise and store (row r0: regs 0,1 ; row r1: regs 2,3 ; columns nt*8 + 2t, +1)
@@ -199,12 +225,20 @@ __global__ void __launch_bounds__(kAmThreads) attention_mma_kernel(const float* 
 inline cudaError_t attention_mma_configure_device() {   // per-device shared-memory opt-in (pf_create)
   cudaError_t e = cudaFuncSetAttribute(attention_mma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAmSmem);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(attention_mma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAmSmem);
-  return e;
+  return e;   // (the NP = 1 instantiations use 28 KB: no opt-in)
 }
 
-// q / kv: fp32 pointers, or (qs / kvs non-empty) split planes with row pitch C / 2C
+template <int NP>
+inline cudaError_t attention_mma_launch_np(const float* q, const float* kv, float* out, dim3 grid, int N, int C, int tpb, cudaStream_t st, SplitT sp,
+                                           SplitT qs, SplitT kvs) {
+  if (qs.hi) return launch_pdl(attention_mma_kernel<true, NP>, grid, dim3(kAmThreads), am_smem<NP>(), st, nullptr, nullptr, qs.hi, qs.lo, kvs.hi, kvs.lo, out, sp.hi, sp.lo, N, C, tpb);
+  return launch_pdl(attention_mma_kernel<false, NP>, grid, dim3(kAmThreads), am_smem<NP>(), st, q, kv, nullptr, nullptr, nullptr, nullptr, out, sp.hi, sp.lo, N, C, tpb);
+}
+
+// q / kv: fp32 pointers, or (qs / kvs non-empty) split planes with row pitch C / 2C.  np = bf16 products per output: 3 (split
+// precision) or 1 (bf16 precision mode: only the hi planes of qs / kvs are read)
 inline cudaError_t attention_mma_launch(const float* q, const float* kv, float* out, int B, int N, int C, int heads, cudaStream_t st, SplitT sp = SplitT(),
-                                        SplitT qs = SplitT(), SplitT kvs = SplitT()) {
+                                        SplitT qs = SplitT(), SplitT kvs = SplitT(), int np = 3) {
   if ((qs.hi != nullptr) != (kvs.hi != nullptr) || (qs.hi && (qs.ld != C || kvs.ld != 2 * C))) return cudaErrorInvalidValue;
   const int tiles = cdiv(N, kAmQTile);
   // passes per block: the grid should be about one resident wave (132 SMs x 3 blocks); the K/V staging of a block is
@@ -212,8 +246,9 @@ inline cudaError_t attention_mma_launch(const float* q, const float* kv, float* 
   int tpb = (tiles * heads * B) / 396;
   tpb = tpb < 1 ? 1 : (tpb > tiles ? tiles : tpb);
   dim3 grid(cdiv(tiles, tpb), heads, B);
-  if (qs.hi) return launch_pdl(attention_mma_kernel<true>, grid, dim3(kAmThreads), kAmSmem, st, nullptr, nullptr, qs.hi, qs.lo, kvs.hi, kvs.lo, out, sp.hi, sp.lo, N, C, tpb);
-  return launch_pdl(attention_mma_kernel<false>, grid, dim3(kAmThreads), kAmSmem, st, q, kv, nullptr, nullptr, nullptr, nullptr, out, sp.hi, sp.lo, N, C, tpb);
+  if (np == 1) return attention_mma_launch_np<1>(q, kv, out, grid, N, C, tpb, st, sp, qs, kvs);
+  if (np == 3) return attention_mma_launch_np<3>(q, kv, out, grid, N, C, tpb, st, sp, qs, kvs);
+  return cudaErrorInvalidValue;
 }
 
 }  // namespace pf

@@ -2,7 +2,8 @@
 //
 // All GEMM operands arrive PRE-SPLIT: activations as two bf16 planes (hi = bf16(x), lo = bf16(x - hi)) written by the
 // producing kernel's epilogue, weights as hi/lo planes split at load time.  Each product costs three bf16 MMAs
-// (lo*hi + hi*lo + hi*hi, fp32 accumulation) -- see DESIGN.md "precision".  Nothing is converted here: tiles go
+// (lo*hi + hi*lo + hi*hi, fp32 accumulation) -- see DESIGN.md "precision"; the opt-in bf16 mode (NP = 1) loads the hi planes
+// only and costs one (hi*hi).  The epilogue writes both split planes in either mode.  Nothing is converted here: tiles go
 // HBM/L2 --TMA--> swizzled shared memory --wgmma--> registers --> fused epilogue --> HBM.
 //
 //   MODE_GEMM : C[M,N] = A[M,K] W[N,K]^T.     A tiles 128 x KB by 2-D TMA, NS-stage ring.
@@ -61,15 +62,19 @@ struct TmaGemmParams {
 
 // KB = K elements per pipeline step: 32 (64 B rows, SWIZZLE_64B) for wide tiles, 64 (128 B rows, SWIZZLE_128B) for narrow ones
 // where a 32-wide step would be shorter than the barrier round trip that feeds it.
-template <int BN, int MODE, int KB, bool PP = false> struct TmaCfg {
+// NP = bf16 products per output: 3 (lo*hi + hi*lo + hi*hi on hi / lo planes, fp32-accurate) or 1 (hi*hi only: the opt-in
+// bf16 precision mode).  With one product only the hi planes are loaded, so a stage holds half the bytes and the ring is deeper.
+template <int BN, int MODE, int KB, bool PP = false, int NP = 3> struct TmaCfg {
   static_assert(KB == 32 || KB == 64, "KB");
   static_assert(BN % 32 == 0 && BN <= 256, "BN");
   static_assert(!PP || MODE == MODE_GEMM, "the ping-pong schedule is a GEMM-mode schedule");
+  static_assert(NP == 1 || NP == 3, "NP");
+  static constexpr int kPlanes = NP == 3 ? 2 : 1;               // bf16 planes loaded per operand: hi + lo, or hi
   static constexpr int kTileM = PP ? 64 : 128;                  // MODE_GEMM: rows per tile
   static constexpr int kBPlane = BN * KB * 2;                   // bf16 plane of one K step of B
   static constexpr int kAPlane = kTileM * KB * 2;               // MODE_GEMM: plane of a kTileM x KB A tile
-  static constexpr int kStage = (MODE == MODE_GEMM ? 2 * kAPlane : 0) + 2 * kBPlane;
-  static constexpr int kABuf = 2 * kHtPlaneBytes;               // MODE_HALO: hi + lo halo planes (1024 B multiples)
+  static constexpr int kStage = (MODE == MODE_GEMM ? kPlanes * kAPlane : 0) + kPlanes * kBPlane;
+  static constexpr int kABuf = kPlanes * kHtPlaneBytes;         // MODE_HALO: the halo planes of one chunk (1024 B multiples)
   // epilogue staging: each MMA warpgroup moves its accumulators through shared memory 64 columns at a time so that one thread
   // then holds 32 consecutive columns of one row (row pitch 68 floats: the row-wise float4 reads are free of bank conflicts)
   static constexpr int kAccPitch = 68;
@@ -102,9 +107,10 @@ struct TmaMaps {   // passed by value as a __grid_constant__ kernel parameter
   CUtensorMap a_hi, a_lo, a2_hi, a2_lo, b_hi, b_lo;
 };
 
-template <int BN, int MODE, int KB, bool PP = false>
+template <int BN, int MODE, int KB, bool PP = false, int NP = 3>
 __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_constant__ TmaMaps maps, const TmaGemmParams p, int tiles_x, int tiles_y) {
-  using Cfg = TmaCfg<BN, MODE, KB, PP>;
+  using Cfg = TmaCfg<BN, MODE, KB, PP, NP>;
+  constexpr bool kLo = NP == 3;               // the lo planes are loaded and multiplied
   constexpr int NS = Cfg::kStages;
   constexpr int SPC = 9 * (64 / KB);          // MODE_HALO: pipeline steps per 64-channel chunk (9 taps x 64 / KB)
   constexpr int kConsumerWarps = PP ? 4 : 8;   // warps that release a ring stage: its warpgroup (ping-pong) or both
@@ -133,7 +139,8 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
   const bool b_resident = MODE == MODE_HALO && nchunks == 1 && SPC <= NS;
 
   if (tid == 0) {
-    tma_prefetch_desc(&maps.a_hi); tma_prefetch_desc(&maps.a_lo); tma_prefetch_desc(&maps.b_hi); tma_prefetch_desc(&maps.b_lo);
+    tma_prefetch_desc(&maps.a_hi); tma_prefetch_desc(&maps.b_hi);
+    if (kLo) { tma_prefetch_desc(&maps.a_lo); tma_prefetch_desc(&maps.b_lo); }
     for (int s = 0; s < NS; ++s) { mbar_init(full_b(s), 1); mbar_init(empty_b(s), kConsumerWarps); }
     for (int i = 0; i < 2; ++i) { mbar_init(full_a(i), 1); mbar_init(empty_a(i), kConsumerWarps); mbar_init(order_b(i), 4); }
     fence_mbar_init();
@@ -171,14 +178,14 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
           if (MODE == MODE_GEMM) {
             kcol = kc * KB;
             tma_load_2d(st, &maps.a_hi, full_b(s), p.a_c0 + g * p.a_gc + kcol, mt * Cfg::kTileM);
-            tma_load_2d(st + Cfg::kAPlane, &maps.a_lo, full_b(s), p.a_c0 + g * p.a_gc + kcol, mt * Cfg::kTileM);
+            if (kLo) tma_load_2d(st + Cfg::kAPlane, &maps.a_lo, full_b(s), p.a_c0 + g * p.a_gc + kcol, mt * Cfg::kTileM);
           } else {
             const int c = kc / SPC, u = kc - c * SPC;
             kcol = KB == 32 ? (u >> 1) * p.Cin + c * 64 + (u & 1) * 32 : u * p.Cin + c * 64;
           }
-          const uint32_t bdst = st + (MODE == MODE_GEMM ? 2 * Cfg::kAPlane : 0);
+          const uint32_t bdst = st + (MODE == MODE_GEMM ? Cfg::kPlanes * Cfg::kAPlane : 0);
           tma_load_2d(bdst, &maps.b_hi, full_b(s), kcol, brow);
-          tma_load_2d(bdst + Cfg::kBPlane, &maps.b_lo, full_b(s), kcol, brow);
+          if (kLo) tma_load_2d(bdst + Cfg::kBPlane, &maps.b_lo, full_b(s), kcol, brow);
         }
       }
     } else if (MODE == MODE_HALO && warp == 1 && lane == 0) {
@@ -191,15 +198,15 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
         for (int c = 0; c < nchunks; ++c, ++ita) {
           const int buf = ita & 1;
           mbar_wait(empty_a(buf), ((ita >> 1) & 1) ^ 1);
-          mbar_expect_tx(full_a(buf), 2 * kHaloBytes);
+          mbar_expect_tx(full_a(buf), Cfg::kPlanes * kHaloBytes);
           const uint32_t dst = a_base + buf * Cfg::kABuf;
           const int ci = c * 64;
           if (p.c_split > 0 && ci >= p.c_split) {
             tma_load_4d(dst, &maps.a2_hi, full_a(buf), p.a2_c0 + ci - p.c_split, tx * kHtTileW - 1, ty * kHtTileH - 1, bimg);
-            tma_load_4d(dst + kHtPlaneBytes, &maps.a2_lo, full_a(buf), p.a2_c0 + ci - p.c_split, tx * kHtTileW - 1, ty * kHtTileH - 1, bimg);
+            if (kLo) tma_load_4d(dst + kHtPlaneBytes, &maps.a2_lo, full_a(buf), p.a2_c0 + ci - p.c_split, tx * kHtTileW - 1, ty * kHtTileH - 1, bimg);
           } else {
             tma_load_4d(dst, &maps.a_hi, full_a(buf), p.a_c0 + g * p.a_gc + ci, tx * kHtTileW - 1, ty * kHtTileH - 1, bimg);
-            tma_load_4d(dst + kHtPlaneBytes, &maps.a_lo, full_a(buf), p.a_c0 + g * p.a_gc + ci, tx * kHtTileW - 1, ty * kHtTileH - 1, bimg);
+            if (kLo) tma_load_4d(dst + kHtPlaneBytes, &maps.a_lo, full_a(buf), p.a_c0 + g * p.a_gc + ci, tx * kHtTileW - 1, ty * kHtTileH - 1, bimg);
           }
         }
       }
@@ -227,7 +234,7 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
       // also keeps a warpgroup's full-barrier waits within one ring round of the producer, which their parity needs.
       if (tl > 0) mbar_wait(order_b(wg ^ 1), ((tl - 1) >> 1) & 1);
     }
-    // ---------------- main loop: per k16 of a K step, one m64nBNk16 wgmma per product (lo*hi, hi*lo, hi*hi), one commit group per
+    // ---------------- main loop: per k16 of a K step, one m64nBNk16 wgmma per product (lo*hi, hi*lo, hi*hi; NP = 1: hi*hi), one commit group per
     // step; the stage of the previous step is released once that step's group has completed (one group stays in flight under the
     // next wait).  The B plane is contiguous in 8-row groups, so one descriptor spans all BN weight rows.
     int prev_s = -1, prev_buf = -1;
@@ -252,18 +259,23 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
       }
       const int sb = b_resident ? kc : s;                                   // resident weights: step kc lives in slot kc
       if (!b_resident || tl == 0) mbar_wait(full_b(sb), b_resident ? 0 : ((it / NS) & 1));
-      const uint32_t b_hi = ring + sb * Cfg::kStage + (MODE == MODE_GEMM ? 2 * Cfg::kAPlane : 0);
+      const uint32_t b_hi = ring + sb * Cfg::kStage + (MODE == MODE_GEMM ? Cfg::kPlanes * Cfg::kAPlane : 0);
       const uint64_t dah = MODE == MODE_HALO ? ht_a_desc(a_hi) : wgmma_tile_desc<KB>(a_hi);
-      const uint64_t dal = MODE == MODE_HALO ? ht_a_desc(a_lo) : wgmma_tile_desc<KB>(a_lo);
       const uint64_t dbh = wgmma_tile_desc<KB>(b_hi);
-      const uint64_t dbl = wgmma_tile_desc<KB>(b_hi + Cfg::kBPlane);
       wgmma_fence();
+      if (kLo) {
+        const uint64_t dal = MODE == MODE_HALO ? ht_a_desc(a_lo) : wgmma_tile_desc<KB>(a_lo);
+        const uint64_t dbl = wgmma_tile_desc<KB>(b_hi + Cfg::kBPlane);
 #pragma unroll
-      for (int kk = 0; kk < KB / 16; ++kk) {
-        const uint32_t first = (kc | kk) ? 1u : 0u;
-        wgmma_bf16<BN>(acc, dal + 2 * kk, dbh + 2 * kk, first);
-        wgmma_bf16<BN>(acc, dah + 2 * kk, dbl + 2 * kk, 1u);
-        wgmma_bf16<BN>(acc, dah + 2 * kk, dbh + 2 * kk, 1u);
+        for (int kk = 0; kk < KB / 16; ++kk) {
+          const uint32_t first = (kc | kk) ? 1u : 0u;
+          wgmma_bf16<BN>(acc, dal + 2 * kk, dbh + 2 * kk, first);
+          wgmma_bf16<BN>(acc, dah + 2 * kk, dbl + 2 * kk, 1u);
+          wgmma_bf16<BN>(acc, dah + 2 * kk, dbh + 2 * kk, 1u);
+        }
+      } else {
+#pragma unroll
+        for (int kk = 0; kk < KB / 16; ++kk) wgmma_bf16<BN>(acc, dah + 2 * kk, dbh + 2 * kk, (kc | kk) ? 1u : 0u);
       }
       wgmma_commit();
       wgmma_wait<1>();

@@ -186,6 +186,7 @@ struct pf_engine {
   std::unordered_map<MapKey, CUtensorMap, MapKeyHash> map_cache;
   bool use_stem_tc = true;    // 7x7 stems as patch gather + TMA GEMM (option "stem_tc"; 0 = fp32 CUDA-core direct convolution)
   bool use_attn_mma = true;   // tensor-core attention core (option "attn_mma"; 0 = CUDA-core fp32 kernel)
+  bool bf16 = false;          // option "bf16": every tensor-core product is one bf16 MMA (hi * hi) instead of three; read per launch
   int sm_count = 132;
   bool profile = false;
   struct ProfRec { cudaEvent_t a, b; double flops; int cfg; int M, N, K, KH, stride, groups, Cin; };
@@ -359,12 +360,14 @@ struct Fwd {
     return PF_OK;
   }
   // (two names so that the per-kernel profile separates the GEMM-mode and halo-mode launches)
-  static cudaError_t gemm_tma_gemm_mode(const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, bool pp, int sms, cudaStream_t st, const PredTail* pred) {
-    return gemm_tma_launch(MODE_GEMM, maps, p, bn, kb, pp, sms, st, pred);
+  static cudaError_t gemm_tma_gemm_mode(const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, bool pp, int np, int sms, cudaStream_t st, const PredTail* pred) {
+    return gemm_tma_launch(MODE_GEMM, maps, p, bn, kb, pp, np, sms, st, pred);
   }
-  static cudaError_t gemm_tma_halo_mode(const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, bool pp, int sms, cudaStream_t st, const PredTail* pred) {
-    return gemm_tma_launch(MODE_HALO, maps, p, bn, kb, pp, sms, st, pred);
+  static cudaError_t gemm_tma_halo_mode(const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, bool pp, int np, int sms, cudaStream_t st, const PredTail* pred) {
+    return gemm_tma_launch(MODE_HALO, maps, p, bn, kb, pp, np, sms, st, pred);
   }
+  // bf16 products per output of the tensor-core launches: 3 (split precision) or 1 (option "bf16")
+  int np() const { return e->bf16 ? 1 : 3; }
   int force_bn = 0, force_kb = 0;     // pf_op_tma: tile override (0 = the dispatcher's choice)
   int force_sched = 0;                // pf_op_tma: GEMM-mode schedule override (0 = the dispatcher's choice, 1 cooperative, 2 ping-pong)
   int picked_bn = 0, picked_kb = 0, picked_sched = 0;   // (bn, kb, schedule) of the last TMA launch
@@ -375,7 +378,7 @@ struct Fwd {
     if (force_bn) { bn = force_bn; kb = tma_pick_kb(bn, p.K, mode); }
     if (force_kb) kb = force_kb;
     pp = mode == MODE_GEMM && (force_sched ? force_sched == 2 : tma_pick_pingpong(p.M, p.N, p.K, bn, e->sm_count));
-    if (const char* msg = gemm_tma_check(mode, p, bn, kb, pred != nullptr, pp)) return fail(PF_ERR_ARG, "TMA engine, %s (bn %d, kb %d): %s", mode == MODE_GEMM ? "GEMM mode" : "halo mode", bn, kb, msg);
+    if (const char* msg = gemm_tma_check(mode, p, bn, kb, pred != nullptr, pp, np())) return fail(PF_ERR_ARG, "TMA engine, %s (bn %d, kb %d): %s", mode == MODE_GEMM ? "GEMM mode" : "halo mode", bn, kb, msg);
     picked_bn = bn; picked_kb = kb; picked_sched = mode == MODE_GEMM ? (pp ? 2 : 1) : 0;
     return PF_OK;
   }
@@ -391,14 +394,14 @@ struct Fwd {
       r.cfg = mode == MODE_GEMM ? 5 : 6;
       r.M = (int)Mrows; r.N = p.N; r.K = p.K; r.KH = mode == MODE_GEMM ? 1 : 3; r.stride = 1; r.groups = p.groups; r.Cin = p.Cin;
       CU(cudaEventRecord(r.a, st));
-      if (mode == MODE_GEMM) LAUNCHED(gemm_tma_gemm_mode(maps, p, bn, kb, pp, e->sm_count, st, pred));
-      else LAUNCHED(gemm_tma_halo_mode(maps, p, bn, kb, pp, e->sm_count, st, pred));
+      if (mode == MODE_GEMM) LAUNCHED(gemm_tma_gemm_mode(maps, p, bn, kb, pp, np(), e->sm_count, st, pred));
+      else LAUNCHED(gemm_tma_halo_mode(maps, p, bn, kb, pp, np(), e->sm_count, st, pred));
       CU(cudaEventRecord(r.b, st));
       e->prof.push_back(r);
       return PF_OK;
     }
-    if (mode == MODE_GEMM) LAUNCHED(gemm_tma_gemm_mode(maps, p, bn, kb, pp, e->sm_count, st, pred));
-    else LAUNCHED(gemm_tma_halo_mode(maps, p, bn, kb, pp, e->sm_count, st, pred));
+    if (mode == MODE_GEMM) LAUNCHED(gemm_tma_gemm_mode(maps, p, bn, kb, pp, np(), e->sm_count, st, pred));
+    else LAUNCHED(gemm_tma_halo_mode(maps, p, bn, kb, pp, np(), e->sm_count, st, pred));
     return PF_OK;
   }
   struct Epi {   // epilogue options of one TMA GEMM / conv
@@ -789,8 +792,8 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
         TRY(F.tgemm(t1, rows, C, 0, b.kv, 2 * C, okv));
       }
       if (!dry) {
-        if (qkv_split) LAUNCHED(attention_mma_launch(nullptr, nullptr, nullptr, n, N, C, heads, st, a, q, kv));
-        else if (e->use_attn_mma) LAUNCHED(attention_mma_launch(qf, kvf, nullptr, n, N, C, heads, st, a));
+        if (qkv_split) LAUNCHED(attention_mma_launch(nullptr, nullptr, nullptr, n, N, C, heads, st, a, q, kv, F.np()));
+        else if (e->use_attn_mma) LAUNCHED(attention_mma_launch(qf, kvf, nullptr, n, N, C, heads, st, a, SplitT(), SplitT(), F.np()));
         else LAUNCHED(attention_launch(qf, kvf, nullptr, n, N, C, heads, st, a));
       }
       { Epi o; o.C = x; o.ldc = C; o.res = x; o.ldr = C; TRY(F.tgemm(a, rows, C, 0, b.proj, C, o)); }
@@ -958,7 +961,8 @@ static int configure_device(int device) {
   static std::vector<char> done;
   std::lock_guard<std::mutex> lock(mu);
   if (device < (int)done.size() && done[device]) return PF_OK;
-  CU(gemm_tma_configure_device());
+  CU(gemm_tma_configure_device(3));
+  CU(gemm_tma_configure_device(1));
   CU(attention_mma_configure_device());
   CU(cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem));
   CU(cudaFuncSetAttribute(conv1_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kRingSmem));
@@ -1154,6 +1158,7 @@ int pf_set_option(pf_handle h, const char* name, int value) {
   if (!strcmp(name, "pdl")) { h->use_pdl = value != 0; return PF_OK; }
   if (!strcmp(name, "dw_ln")) { h->use_dwln = value != 0; return PF_OK; }
   if (!strcmp(name, "fork")) { h->use_fork = value != 0; return PF_OK; }
+  if (!strcmp(name, "bf16")) { h->bf16 = value != 0; return PF_OK; }
   return fail(PF_ERR_ARG, "pf_set_option: unknown option '%s'", name);
 }
 // out[cfg*3 + {0,1,2}] = {milliseconds, algorithmic FLOPs, launches} per GEMM engine configuration (7 configs),
@@ -1383,7 +1388,7 @@ int pf_op_conv_gemm(const float* x, int B, int H, int W, int Cin, const void* wh
   if (se != cudaSuccess) return fail(PF_ERR_CUDA, "pf_op_conv_gemm: %s", cudaGetErrorString(se));
   return PF_OK;
 }
-int pf_op_tma(pf_tma_op* op, void* stream) {
+static int op_tma(pf_tma_op* op, void* stream, bool bf16) {
   if (!op || !op->a_hi || !op->a_lo || !op->w_hi || !op->w_lo) return fail(PF_ERR_ARG, "pf_op_tma: null argument");
   const pf_tma_op& q = *op;
   if (q.mode != MODE_GEMM && q.mode != MODE_HALO) return fail(PF_ERR_ARG, "pf_op_tma: mode %d", q.mode);
@@ -1403,6 +1408,7 @@ int pf_op_tma(pf_tma_op* op, void* stream) {
   pf_engine tmp;
   tmp.device = dev;
   tmp.sm_count = prop.multiProcessorCount;
+  tmp.bf16 = bf16;
   Fwd F{&tmp, Arena{}, (cudaStream_t)stream, false, q.B};
   if (q.force_sched < 0 || q.force_sched > 2 || (q.force_sched && q.mode != MODE_GEMM)) return fail(PF_ERR_ARG, "pf_op_tma: force_sched %d", q.force_sched);
   F.force_bn = q.force_bn; F.force_kb = q.force_kb; F.force_sched = q.force_sched;
@@ -1429,6 +1435,8 @@ int pf_op_tma(pf_tma_op* op, void* stream) {
   if (r == PF_OK) { op->picked_bn = F.picked_bn; op->picked_kb = F.picked_kb; op->picked_sched = F.picked_sched; }
   return r;
 }
+int pf_op_tma(pf_tma_op* op, void* stream) { return op_tma(op, stream, false); }
+int pf_op_tma_bf16(pf_tma_op* op, void* stream) { return op_tma(op, stream, true); }
 int pf_op_conv1_ring(const void* c_hi, const void* c_lo, int B, int H, int W, const float* wf, const float* bias, float* out,
                      const float* pg_w, const float* pg_b, float* pg_out, const float* pl_w, const float* pl_b, float* pl_out, void* stream) {
   if (!c_hi || !c_lo || !wf || !bias) return fail(PF_ERR_ARG, "pf_op_conv1_ring: null argument");
@@ -1559,7 +1567,7 @@ int pf_op_attention_mma(const float* q, const float* kv, float* out, int B, int 
   LAUNCHED(attention_mma_launch(q, kv, out, B, N, C, heads, (cudaStream_t)stream));
   return PF_OK;
 }
-int pf_op_attention_tc(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream) {
+static int op_attention_tc(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream, int np) {
   if (!q || !kv || !out || C != heads * kAmD) return fail(PF_ERR_ARG, "pf_op_attention_tc: head_dim must be 64");
   TRY(configure_current_device());
   cudaStream_t st = (cudaStream_t)stream;
@@ -1581,7 +1589,7 @@ int pf_op_attention_tc(const float* q, const float* kv, float* out, int B, int N
   if (le == cudaSuccess) le = (split_kernel<<<(unsigned)cdivl(nkv, 256), 256, 0, st>>>(kv, kvs.hi, kvs.lo, nkv, 0), cudaGetLastError());
   if (le != cudaSuccess) r = fail(PF_ERR_CUDA, "split_kernel: %s", cudaGetErrorString(le));
   if (r == PF_OK) {
-    le = attention_mma_launch(nullptr, nullptr, nullptr, B, N, C, heads, st, as, qs, kvs);
+    le = attention_mma_launch(nullptr, nullptr, nullptr, B, N, C, heads, st, as, qs, kvs, np);
     if (le != cudaSuccess) r = fail(PF_ERR_CUDA, "attention_mma_launch: %s", cudaGetErrorString(le));
   }
   if (r == PF_OK) {
@@ -1592,6 +1600,12 @@ int pf_op_attention_tc(const float* q, const float* kv, float* out, int B, int N
   cudaFree(scratch);
   if (r == PF_OK && se != cudaSuccess) r = fail(PF_ERR_CUDA, "pf_op_attention_tc: %s", cudaGetErrorString(se));
   return r;
+}
+int pf_op_attention_tc(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream) {
+  return op_attention_tc(q, kv, out, B, N, C, heads, stream, 3);
+}
+int pf_op_attention_tc_bf16(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream) {
+  return op_attention_tc(q, kv, out, B, N, C, heads, stream, 1);
 }
 int pf_op_dwconv3x3_gelu(const float* x, float* y, int B, int H, int W, int C, const float* w, const float* bias, void* stream) {
   if (C % 4) return fail(PF_ERR_ARG, "C %% 4");

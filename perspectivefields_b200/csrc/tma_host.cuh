@@ -112,9 +112,9 @@ inline bool tma_pick_pingpong(long long M, int N, int K, int bn, int sm_count) {
 
 struct PredTail { const float* w; const float* b; float* out; int nc, mode; };   // per group, see TmaGemmParams::pred_*
 
-template <int BN, int MODE, int KB, bool PP = false>
+template <int BN, int MODE, int KB, bool PP = false, int NP = 3>
 inline cudaError_t gemm_tma_launch_bn(const TmaMaps& maps, const TmaGemmParams& p, int sm_count, cudaStream_t st, const PredTail* pred) {
-  using Cfg = TmaCfg<BN, MODE, KB, PP>;   // (the > 48 KB shared-memory opt-in is per device: gemm_tma_configure_device, at pf_create)
+  using Cfg = TmaCfg<BN, MODE, KB, PP, NP>;   // (the > 48 KB shared-memory opt-in is per device: gemm_tma_configure_device, at pf_create)
   const int tiles_x = MODE == MODE_HALO ? cdiv(p.W, kHtTileW) : 0, tiles_y = MODE == MODE_HALO ? cdiv(p.H, kHtTileH) : 0;
   const long long m_tiles = MODE == MODE_GEMM ? cdiv(p.M, Cfg::kTileM) : (long long)p.B * tiles_x * tiles_y;
   const long long total = m_tiles * cdiv(p.N, BN) * p.groups;
@@ -135,15 +135,16 @@ inline cudaError_t gemm_tma_launch_bn(const TmaMaps& maps, const TmaGemmParams& 
         if (pred) { q.pred_w = pred[g].w; q.pred_b = pred[g].b; q.pred_out = pred[g].out; q.pred_nc = pred[g].nc; q.pred_mode = pred[g].mode; }
         if (cdiv(p.N, BN) > 1) return cudaErrorInvalidValue;   // (not needed by the network: conv_fuse_conv1 has one N tile)
         const unsigned gr = (unsigned)(m_tiles < sm_count ? m_tiles : sm_count);
-        last = launch_pdl(gemm_tma_kernel<BN, MODE, KB>, dim3(gr), dim3(kTmaThreads), Cfg::kSmemBytes, st, maps, q, tiles_x, tiles_y);
+        last = launch_pdl(gemm_tma_kernel<BN, MODE, KB, false, NP>, dim3(gr), dim3(kTmaThreads), Cfg::kSmemBytes, st, maps, q, tiles_x, tiles_y);
         if (last != cudaSuccess) return last;
       }
     return last;
   }
-  return launch_pdl(gemm_tma_kernel<BN, MODE, KB, PP>, dim3(grid), dim3(kTmaThreads), Cfg::kSmemBytes, st, maps, p, tiles_x, tiles_y);
+  return launch_pdl(gemm_tma_kernel<BN, MODE, KB, PP, NP>, dim3(grid), dim3(kTmaThreads), Cfg::kSmemBytes, st, maps, p, tiles_x, tiles_y);
 }
 
-// every instantiation the dispatcher below can reach: X(BN, MODE, KB)
+// every instantiation the dispatcher below can reach: X(BN, MODE, KB).  Each one exists with three products and with one (the
+// bf16 precision mode picks the same tiles).
 #define PF_TMA_VARIANTS(X)                                                                                                  \
   X(256, MODE_GEMM, 32) X(224, MODE_GEMM, 32) X(192, MODE_GEMM, 32) X(160, MODE_GEMM, 32) X(128, MODE_GEMM, 32) X(96, MODE_GEMM, 32) \
   X(64, MODE_GEMM, 32) X(32, MODE_GEMM, 32) X(64, MODE_GEMM, 64) X(32, MODE_GEMM, 64)                                        \
@@ -153,36 +154,45 @@ inline cudaError_t gemm_tma_launch_bn(const TmaMaps& maps, const TmaGemmParams& 
   X(256, 32) X(224, 32) X(192, 32) X(160, 32) X(128, 32) X(96, 32) X(64, 32) X(32, 32) X(64, 64) X(32, 64)
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a per-device (per-context) attribute: called once for every device an engine is
-// created on (pf_create) -- not behind a process-wide flag.
-inline cudaError_t gemm_tma_configure_device() {
+// created on (pf_create) and every product count np (3 or 1) -- not behind a process-wide flag.
+template <int NP>
+inline cudaError_t gemm_tma_configure_np() {
   cudaError_t e = cudaSuccess;
 #define PF_TMA_CFG(BN_, MODE_, KB_)                                                                                          \
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_tma_kernel<BN_, MODE_, KB_>, cudaFuncAttributeMaxDynamicSharedMemorySize, TmaCfg<BN_, MODE_, KB_>::kSmemBytes);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_tma_kernel<BN_, MODE_, KB_, false, NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, TmaCfg<BN_, MODE_, KB_, false, NP>::kSmemBytes);
   PF_TMA_VARIANTS(PF_TMA_CFG)
 #undef PF_TMA_CFG
 #define PF_TMA_CFG_PP(BN_, KB_)                                                                                               \
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_tma_kernel<BN_, MODE_GEMM, KB_, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TmaCfg<BN_, MODE_GEMM, KB_, true>::kSmemBytes);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_tma_kernel<BN_, MODE_GEMM, KB_, true, NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, TmaCfg<BN_, MODE_GEMM, KB_, true, NP>::kSmemBytes);
   PF_TMA_PINGPONG_VARIANTS(PF_TMA_CFG_PP)
 #undef PF_TMA_CFG_PP
   return e;
 }
+inline cudaError_t gemm_tma_configure_device(int np) {
+  return np == 1 ? gemm_tma_configure_np<1>() : (np == 3 ? gemm_tma_configure_np<3>() : cudaErrorInvalidValue);
+}
 
-// ring depth of an instantiation, 0 if PF_TMA_VARIANTS (pp: PF_TMA_PINGPONG_VARIANTS) does not list it
-inline int tma_stages(int mode, int bn, int kb, bool pp = false) {
-#define PF_TMA_NS(BN_, MODE_, KB_) if (!pp && mode == MODE_ && bn == BN_ && kb == KB_) return TmaCfg<BN_, MODE_, KB_>::kStages;
+// ring depth of an instantiation, 0 if PF_TMA_VARIANTS (pp: PF_TMA_PINGPONG_VARIANTS) does not list it or np is not 3 or 1
+template <int NP>
+inline int tma_stages_np(int mode, int bn, int kb, bool pp) {
+#define PF_TMA_NS(BN_, MODE_, KB_) if (!pp && mode == MODE_ && bn == BN_ && kb == KB_) return TmaCfg<BN_, MODE_, KB_, false, NP>::kStages;
   PF_TMA_VARIANTS(PF_TMA_NS)
 #undef PF_TMA_NS
-#define PF_TMA_NS_PP(BN_, KB_) if (pp && mode == MODE_GEMM && bn == BN_ && kb == KB_) return TmaCfg<BN_, MODE_GEMM, KB_, true>::kStages;
+#define PF_TMA_NS_PP(BN_, KB_) if (pp && mode == MODE_GEMM && bn == BN_ && kb == KB_) return TmaCfg<BN_, MODE_GEMM, KB_, true, NP>::kStages;
   PF_TMA_PINGPONG_VARIANTS(PF_TMA_NS_PP)
 #undef PF_TMA_NS_PP
   return 0;
 }
+inline int tma_stages(int mode, int bn, int kb, bool pp, int np) {
+  return np == 1 ? tma_stages_np<1>(mode, bn, kb, pp) : (np == 3 ? tma_stages_np<3>(mode, bn, kb, pp) : 0);
+}
 
-// Why the (bn, kb) instantiation cannot compute p: nullptr when it can.  Every case here would otherwise launch something that
-// computes a different result (a K tail, a prediction tail or phase layout the tile width does not implement) or that
-// gemm_tma_launch_bn refuses after the fact (resident weights over several N tiles).
-inline const char* gemm_tma_check(int mode, const TmaGemmParams& p, int bn, int kb, bool pred, bool pp = false) {
-  const int ns = tma_stages(mode, bn, kb, pp);
+// Why the (bn, kb) instantiation with np products cannot compute p: nullptr when it can.  Every case here would otherwise launch
+// something that computes a different result (a K tail, a prediction tail or phase layout the tile width does not implement) or
+// that gemm_tma_launch_bn refuses after the fact (resident weights over several N tiles).  Whether the weights are resident
+// depends on the ring depth, so on np: the one-product ring is deeper.
+inline const char* gemm_tma_check(int mode, const TmaGemmParams& p, int bn, int kb, bool pred, bool pp, int np) {
+  const int ns = tma_stages(mode, bn, kb, pp, np);
   if (!ns) return pp ? "no ping-pong engine instantiation for this (mode, bn, kb)" : "no engine instantiation for this (mode, bn, kb)";
   if (mode == MODE_GEMM) return p.K % kb ? "GEMM mode: K must be a multiple of the K step" : nullptr;
   if (p.phase4 && (p.N != 128 || bn != 128)) return "phase4 needs N = 128 in one 128-wide tile";
@@ -192,14 +202,22 @@ inline const char* gemm_tma_check(int mode, const TmaGemmParams& p, int bn, int 
   return nullptr;
 }
 
-inline cudaError_t gemm_tma_launch(int mode, const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, bool pp, int sm_count, cudaStream_t st,
-                                   const PredTail* pred = nullptr) {
-#define PF_TMA_CASE(BN_, MODE_, KB_) if (!pp && mode == MODE_ && bn == BN_ && kb == KB_) return gemm_tma_launch_bn<BN_, MODE_, KB_>(maps, p, sm_count, st, pred);
+template <int NP>
+inline cudaError_t gemm_tma_launch_np(int mode, const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, bool pp, int sm_count, cudaStream_t st,
+                                      const PredTail* pred) {
+#define PF_TMA_CASE(BN_, MODE_, KB_) if (!pp && mode == MODE_ && bn == BN_ && kb == KB_) return gemm_tma_launch_bn<BN_, MODE_, KB_, false, NP>(maps, p, sm_count, st, pred);
   PF_TMA_VARIANTS(PF_TMA_CASE)
 #undef PF_TMA_CASE
-#define PF_TMA_CASE_PP(BN_, KB_) if (pp && mode == MODE_GEMM && bn == BN_ && kb == KB_) return gemm_tma_launch_bn<BN_, MODE_GEMM, KB_, true>(maps, p, sm_count, st, pred);
+#define PF_TMA_CASE_PP(BN_, KB_) if (pp && mode == MODE_GEMM && bn == BN_ && kb == KB_) return gemm_tma_launch_bn<BN_, MODE_GEMM, KB_, true, NP>(maps, p, sm_count, st, pred);
   PF_TMA_PINGPONG_VARIANTS(PF_TMA_CASE_PP)
 #undef PF_TMA_CASE_PP
+  return cudaErrorInvalidValue;
+}
+// np = bf16 products per output: 3 (split precision) or 1 (bf16 precision mode)
+inline cudaError_t gemm_tma_launch(int mode, const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, bool pp, int np, int sm_count, cudaStream_t st,
+                                   const PredTail* pred = nullptr) {
+  if (np == 1) return gemm_tma_launch_np<1>(mode, maps, p, bn, kb, pp, sm_count, st, pred);
+  if (np == 3) return gemm_tma_launch_np<3>(mode, maps, p, bn, kb, pp, sm_count, st, pred);
   return cudaErrorInvalidValue;
 }
 

@@ -198,10 +198,16 @@ class ResizeTransform:
 
 
 class PerspectiveFields(nn.Module):
-    def __init__(self, version="Paramnet-360Cities-edina-centered", logits=True):
+    def __init__(self, version="Paramnet-360Cities-edina-centered", logits=True, precision="fp32"):
         """``logits=False`` (classification variant only, SURVEY.md 8f-3; NOT the reference's behaviour): ``pred_gravity`` /
         ``pred_latitude`` hold the decoded fields ([2,320,320] up-vectors, [1,320,320] degrees) instead of the 73 / 180 raw logits,
-        which are then never written (engine option "decode_only"); the ``*_original`` entries are unchanged."""
+        which are then never written (engine option "decode_only"); the ``*_original`` entries are unchanged.
+
+        ``precision``: ``"fp32"`` (default) keeps the reference's fp32 numerics within 1e-3 (three bf16 MMAs per product).
+        ``"bf16"`` (opt-in, NOT the reference's numerics) runs every tensor-core product as one bf16 MMA on bf16-rounded operands
+        with fp32 accumulation, as ``torch.autocast(dtype=torch.bfloat16)`` would; normalisation, softmax, depthwise convolutions
+        and the prediction tails stay fp32.  Outputs then differ from fp32 by about 1e-2 relative (DESIGN.md section 3 lists the
+        measured error per output).  It is the engine option "bf16" and survives ``.to()`` / ``load_state_dict``."""
         super().__init__()
         zoo = model_zoo[version]  # KeyError for unknown versions, like the reference (perspectivefields.py:127)
         self.version = version
@@ -224,6 +230,10 @@ class PerspectiveFields(nn.Module):
             if self._variant["gravity"] != "classification":
                 raise ValueError("logits=False only applies to the classification variant (PersNet-360Cities)")
             self._options["decode_only"] = 1
+        if precision not in ("fp32", "bf16"):
+            raise ValueError(f"precision must be 'fp32' or 'bf16', got {precision!r}")
+        if precision == "bf16":
+            self._options["bf16"] = 1
         self.training = False
         self._init_weights()
 
