@@ -78,6 +78,10 @@ int64_t pf_kernel_launch_count(void);
 
 /* Engine lifetime.  `device` is the CUDA ordinal; the engine makes it current for its own calls. */
 int pf_create(int device, const pf_model_desc* desc, pf_handle* out);
+/* The same at working size net_h x net_w (DATALOADER.RESIZE = [net_h, net_w]): multiples of 32 in [64, 640] with
+ * (net_h/32) * (net_w/32) <= 256 (the attention key count of every MiT stage).  pf_forward then expects images_chw as
+ * [n,3,net_h,net_w] and writes pred_gravity / pred_latitude as [n,C,net_h,net_w].  pf_create = pf_create_sized(.., 320, 320, ..). */
+int pf_create_sized(int device, const pf_model_desc* desc, int net_h, int net_w, pf_handle* out);
 int pf_destroy(pf_handle h);
 
 /* Register one repacked weight tensor (DEVICE pointer, stays owned by the caller and must outlive the handle).
@@ -237,11 +241,16 @@ int pf_op_attention(const float* q, const float* kv, float* out, int B, int N, i
 int pf_op_attention_mma(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream);  /* warp-level mma.sync, bf16x3 */
 int pf_op_attention_tc(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream);   /* q / kv split into bf16 hi/lo planes first, then the mma.sync core as the forward graph runs it */
 int pf_op_attention_tc_bf16(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream); /* the same in the bf16 precision mode: one mma.sync per product on bf16(q), bf16(k), bf16(P), bf16(v) */
+/* pf_op_attention_tc / _bf16 (bf16 != 0) with NKV keys per image (kv: [B,NKV,2C]), 1..256: 100 runs the 320 x 320 kernel, other
+ * counts up to 112 the single-block kernel with a run-time count, larger ones the key-block (online-softmax) kernel */
+int pf_op_attention_tc_keys(const float* q, const float* kv, float* out, int B, int N, int NKV, int C, int heads, int bf16, void* stream);
 int pf_op_dwconv3x3_gelu(const float* x, float* y, int B, int H, int W, int C, const float* w9c, const float* bias, void* stream);
 int pf_op_dwconv7x7(const float* x, float* y, int B, int H, int W, int C, const float* w49c, const float* bias, void* stream);
 int pf_op_upsample2x(const float* x, float* y, int B, int H, int W, int C, void* stream);
 /* Pillow-exact resize + normalise of ONE uint8 HWC image -> [320,320,4] fp32 (b,g,r,0). */
 int pf_op_preprocess(const uint8_t* img_dev, int H, int W, const float* mean3, const float* std3, float* y, void* stream);
+/* the same to [net_h,net_w,4] (a working size pf_create_sized accepts) */
+int pf_op_preprocess_sized(const uint8_t* img_dev, int H, int W, int net_h, int net_w, const float* mean3, const float* std3, float* y, void* stream);
 /* ResizeTransform.apply_image (perspectivefields.py:34-67) on the device, HWC in -> HWC out, C channels:
  *   uint8 (PIL branch, :38-46): Pillow-exact antialiased bilinear (the same integer kernel as pf_forward's pre-process);
  *   float32 (:47-66): F.interpolate(mode="bilinear", align_corners=False), no antialias. */
@@ -262,6 +271,11 @@ int pf_op_pred_argmax_decode(const float* feat, int ld, int coff, const float* w
 int pf_op_postprocess(const float* vec, const float* lat, int n, const int32_t* height, const int32_t* width,
                       float* gravity_original, const int64_t* gravity_original_offset, float* latitude_original,
                       const int64_t* latitude_original_offset, int lat_is_sin, void* stream);
+/* the same from fields at the working size net_h x net_w: vec [n,2,net_h,net_w], lat [n,1,net_h,net_w] (crop to and scale by
+ * the net size as gravity_head.py:248-256 does with image_size) */
+int pf_op_postprocess_sized(const float* vec, const float* lat, int n, int net_h, int net_w, const int32_t* height, const int32_t* width,
+                            float* gravity_original, const int64_t* gravity_original_offset, float* latitude_original,
+                            const int64_t* latitude_original_offset, int lat_is_sin, void* stream);
 
 #ifdef __cplusplus
 }

@@ -114,6 +114,7 @@ def lib():
         "pf_last_error": (ctypes.c_char_p, []),
         "pf_kernel_launch_count": (i64, []),
         "pf_create": (i32, [i32, ctypes.POINTER(pf_model_desc), ctypes.POINTER(vp)]),
+        "pf_create_sized": (i32, [i32, ctypes.POINTER(pf_model_desc), i32, i32, ctypes.POINTER(vp)]),
         "pf_destroy": (i32, [vp]),
         "pf_set_weight": (i32, [vp, ctypes.c_char_p, vp, i64, i32]),
         "pf_finalize": (i32, [vp]),
@@ -140,10 +141,12 @@ def lib():
         "pf_op_attention_mma": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
         "pf_op_attention_tc": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
         "pf_op_attention_tc_bf16": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
+        "pf_op_attention_tc_keys": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]),
         "pf_op_dwconv3x3_gelu": (i32, [vp, vp, i32, i32, i32, i32, vp, vp, vp]),
         "pf_op_dwconv7x7": (i32, [vp, vp, i32, i32, i32, i32, vp, vp, vp]),
         "pf_op_upsample2x": (i32, [vp, vp, i32, i32, i32, i32, vp]),
         "pf_op_preprocess": (i32, [vp, i32, i32, ctypes.POINTER(f32), ctypes.POINTER(f32), vp, vp]),
+        "pf_op_preprocess_sized": (i32, [vp, i32, i32, i32, i32, ctypes.POINTER(f32), ctypes.POINTER(f32), vp, vp]),
         "pf_op_resize_u8": (i32, [vp, i32, i32, i32, i32, vp, vp]),
         "pf_op_resize_f32": (i32, [vp, i32, i32, i32, i32, i32, vp, vp]),
         "pf_op_argmax_decode": (i32, [vp, vp, i32, i32, i32, i32, vp]),
@@ -151,6 +154,8 @@ def lib():
         "pf_op_pred_argmax_decode": (i32, [vp, i32, i32, vp, vp, vp, i32, i32, i32, i32, vp]),
         "pf_op_postprocess": (i32, [vp, vp, i32, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32), vp, ctypes.POINTER(i64), vp,
                                     ctypes.POINTER(i64), i32, vp]),
+        "pf_op_postprocess_sized": (i32, [vp, vp, i32, i32, i32, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32), vp,
+                                          ctypes.POINTER(i64), vp, ctypes.POINTER(i64), i32, vp]),
         "pf_comm_unique_id": (i32, [vp]),
         "pf_comm_create": (i32, [i32, i32, i32, vp, ctypes.POINTER(vp)]),
         "pf_comm_destroy": (i32, [vp]),
@@ -175,15 +180,15 @@ def lib():
     return L
 
 
-EXPORTS = ["pf_abi_version", "pf_last_error", "pf_kernel_launch_count", "pf_create", "pf_destroy", "pf_set_weight",
+EXPORTS = ["pf_abi_version", "pf_last_error", "pf_kernel_launch_count", "pf_create", "pf_create_sized", "pf_destroy", "pf_set_weight",
            "pf_finalize", "pf_workspace_bytes", "pf_forward", "pf_profile_enable", "pf_profile_read", "pf_profile_kernels_enable",
            "pf_profile_kernels_read", "pf_set_option", "pf_debug_enable", "pf_debug_count", "pf_debug_name", "pf_debug_numel",
            "pf_debug_copy", "pf_camera_fields", "pf_comm_unique_id", "pf_comm_create", "pf_comm_destroy", "pf_gather",
            "pf_jpeg_create", "pf_jpeg_destroy", "pf_jpeg_info", "pf_jpeg_decode_batch",
            "pf_op_conv_gemm", "pf_op_tma", "pf_op_tma_bf16", "pf_op_conv1_ring", "pf_tma_pick_tile", "pf_op_layernorm", "pf_op_attention",
-           "pf_op_attention_mma", "pf_op_attention_tc", "pf_op_attention_tc_bf16", "pf_op_dwconv3x3_gelu", "pf_op_dwconv7x7",
-           "pf_op_upsample2x", "pf_op_preprocess", "pf_op_fill_stream", "pf_op_resize_u8", "pf_op_resize_f32", "pf_op_argmax_decode",
-           "pf_op_pred_argmax_decode", "pf_op_postprocess"]
+           "pf_op_attention_mma", "pf_op_attention_tc", "pf_op_attention_tc_bf16", "pf_op_attention_tc_keys", "pf_op_dwconv3x3_gelu",
+           "pf_op_dwconv7x7", "pf_op_upsample2x", "pf_op_preprocess", "pf_op_preprocess_sized", "pf_op_fill_stream", "pf_op_resize_u8",
+           "pf_op_resize_f32", "pf_op_argmax_decode", "pf_op_pred_argmax_decode", "pf_op_postprocess", "pf_op_postprocess_sized"]
 
 
 class PfError(RuntimeError):

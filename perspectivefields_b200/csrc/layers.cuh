@@ -85,7 +85,7 @@ template <int MAXQ, int LANES, int NR>   // float4 quads per lane; LANES (32 or 
 __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict__ in, float* __restrict__ out, long long rows_ll, int C,
                                                         const float* __restrict__ gw, const float* __restrict__ gb, float eps,
                                                         __nv_bfloat16* __restrict__ shi, __nv_bfloat16* __restrict__ slo,
-                                                        __nv_bfloat16* __restrict__ phi, __nv_bfloat16* __restrict__ plo, int R, int sr) {
+                                                        __nv_bfloat16* __restrict__ phi, __nv_bfloat16* __restrict__ plo, int RH, int RW, int sr) {
   pdl_wait();
   pdl_launch();
   constexpr int RPW = 32 / LANES;       // lane groups (rows) per warp
@@ -131,7 +131,7 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict_
 #pragma unroll
     for (int j = 0; j < NR; ++j) q[j] += __shfl_xor_sync(0xffffffffu, q[j], o);
   // optional second copy in PATCH order for a k = s = sr convolution that follows (spatial-reduction conv of the attention,
-  // mix_transformers.py:112-117; ConvNeXt downsample 2x2/2, convnext.py:93-99): token (b, y, x) of an R x R map goes to row
+  // mix_transformers.py:112-117; ConvNeXt downsample 2x2/2, convnext.py:93-99): token (b, y, x) of an RH x RW map goes to row
   // (b, y / sr, x / sr), columns ((y % sr) * sr + x % sr) * C + c -- the im2col matrix of that convolution, written by the
   // producer instead of a separate gather kernel
 #pragma unroll
@@ -142,10 +142,10 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict_
     const float rstd = 1.0f / sqrtf(fmaf(q[j], inv_c, eps));
     unsigned pb = 0;
     if (phi) {
-      const unsigned uR = (unsigned)R, usr = (unsigned)sr;
-      const unsigned x = row % uR, t = row / uR, y = t % uR, b = t / uR;
-      const unsigned OR = uR / usr;
-      pb = (((b * OR + y / usr) * OR + x / usr) * (usr * usr) + (y % usr) * usr + x % usr) * Q;
+      const unsigned uRH = (unsigned)RH, uRW = (unsigned)RW, usr = (unsigned)sr;
+      const unsigned x = row % uRW, t = row / uRW, y = t % uRH, b = t / uRH;
+      const unsigned ORH = uRH / usr, ORW = uRW / usr;
+      pb = (((b * ORH + y / usr) * ORW + x / usr) * (usr * usr) + (y % usr) * usr + x % usr) * Q;
     }
     const unsigned ob = row * Q;
 #pragma unroll
@@ -172,14 +172,14 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict_
 #define PF_LN_NR3 1            // rows in flight per lane group for C > 128 (C <= 128: 4 rows)
 #endif
 inline cudaError_t layernorm_launch(const float* in, float* out, long long rows, int C, const float* w, const float* b, float eps,
-                                    cudaStream_t st, SplitT sp = SplitT(), SplitT patch = SplitT(), int R = 0, int sr = 0) {
+                                    cudaStream_t st, SplitT sp = SplitT(), SplitT patch = SplitT(), int RH = 0, int RW = 0, int sr = 0) {
   if (C % 4 || C > 768 || rows * (C / 4) >= (1LL << 32)) return cudaErrorInvalidValue;
-  if (patch.hi && (R < 1 || sr < 1 || R % sr || rows % ((long long)R * R))) return cudaErrorInvalidValue;
+  if (patch.hi && (RH < 1 || RW < 1 || sr < 1 || RH % sr || RW % sr || rows % ((long long)RH * RW))) return cudaErrorInvalidValue;
   // rows per block = 8 warps x (32 / LANES) lane groups x NR rows in flight per group
-  if (C <= 64) return launch_pdl(layernorm_kernel<1, 16, 4>, dim3((unsigned)cdivl(rows, 64)), dim3(256), 0, st, in, out, rows, C, w, b, eps, sp.hi, sp.lo, patch.hi, patch.lo, R, sr);
-  if (C <= 128) return launch_pdl(layernorm_kernel<1, 32, 4>, dim3((unsigned)cdivl(rows, 32)), dim3(256), 0, st, in, out, rows, C, w, b, eps, sp.hi, sp.lo, patch.hi, patch.lo, R, sr);
-  if (C <= 384) return launch_pdl(layernorm_kernel<3, 32, PF_LN_NR3>, dim3((unsigned)cdivl(rows, 8 * PF_LN_NR3)), dim3(256), 0, st, in, out, rows, C, w, b, eps, sp.hi, sp.lo, patch.hi, patch.lo, R, sr);
-  return launch_pdl(layernorm_kernel<6, 32, PF_LN_NR3>, dim3((unsigned)cdivl(rows, 8 * PF_LN_NR3)), dim3(256), 0, st, in, out, rows, C, w, b, eps, sp.hi, sp.lo, patch.hi, patch.lo, R, sr);
+  if (C <= 64) return launch_pdl(layernorm_kernel<1, 16, 4>, dim3((unsigned)cdivl(rows, 64)), dim3(256), 0, st, in, out, rows, C, w, b, eps, sp.hi, sp.lo, patch.hi, patch.lo, RH, RW, sr);
+  if (C <= 128) return launch_pdl(layernorm_kernel<1, 32, 4>, dim3((unsigned)cdivl(rows, 32)), dim3(256), 0, st, in, out, rows, C, w, b, eps, sp.hi, sp.lo, patch.hi, patch.lo, RH, RW, sr);
+  if (C <= 384) return launch_pdl(layernorm_kernel<3, 32, PF_LN_NR3>, dim3((unsigned)cdivl(rows, 8 * PF_LN_NR3)), dim3(256), 0, st, in, out, rows, C, w, b, eps, sp.hi, sp.lo, patch.hi, patch.lo, RH, RW, sr);
+  return launch_pdl(layernorm_kernel<6, 32, PF_LN_NR3>, dim3((unsigned)cdivl(rows, 8 * PF_LN_NR3)), dim3(256), 0, st, in, out, rows, C, w, b, eps, sp.hi, sp.lo, patch.hi, patch.lo, RH, RW, sr);
 }
 
 // =====================================================================================================
@@ -673,13 +673,13 @@ __global__ void __launch_bounds__(256) im2col_split_kernel(const __nv_bfloat16* 
 }
 
 // Patch gather for the 7x7 stems (patch_embed1: stride 4, ll_enc: stride 2; pad 3) straight from the normalised input
-// x0 [B,320,320,4] fp32 (b,g,r,0): dst[m][(ky*7+kx)*3 + c] split into bf16 hi/lo, K padded 147 -> 160 with zeros, so that the
+// x0 [B,IH,IW,4] fp32 (b,g,r,0) (the net size): dst[m][(ky*7+kx)*3 + c] split into bf16 hi/lo, K padded 147 -> 160 with zeros, so that the
 // stems run on the TMA GEMM engine too.  One thread = one output pixel x 8 consecutive K columns (16 B per plane).
 // (A one-pixel-per-thread variant -- 49 float4 loads, 40 16-byte stores into the thread's own 320-byte row -- executed a third of
 // the instructions but every store instruction of a warp touched 32 different rows.)
 inline long long stem_gather_threads(int B, int OH, int OW) { return (long long)B * OH * OW * 20; }
 __global__ void __launch_bounds__(256) stem_gather_kernel(const float* __restrict__ x0, __nv_bfloat16* __restrict__ dhi, __nv_bfloat16* __restrict__ dlo,
-                                                          int B, int OH, int OW, int stride) {
+                                                          int B, int OH, int OW, int stride, int IH, int IW) {
   pdl_wait();
   pdl_launch();
   constexpr int KP = 160, KQ = KP / 8;
@@ -690,7 +690,7 @@ __global__ void __launch_bounds__(256) stem_gather_kernel(const float* __restric
     const int ox = (int)(m % (unsigned)OW); unsigned t = m / (unsigned)OW;
     const int oy = (int)(t % (unsigned)OH); const unsigned b = t / (unsigned)OH;
     const int iy0 = oy * stride - 3, ix0 = ox * stride - 3;
-    const unsigned pb = ((b * kNet + (unsigned)iy0) * kNet + (unsigned)ix0) * 4u;     // float index of pixel (iy0, ix0), dereferenced where valid
+    const unsigned pb = ((b * (unsigned)IH + (unsigned)iy0) * (unsigned)IW + (unsigned)ix0) * 4u;     // float index of pixel (iy0, ix0), dereferenced where valid
     float v[8];
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
@@ -699,7 +699,7 @@ __global__ void __launch_bounds__(256) stem_gather_kernel(const float* __restric
       if (k < 147) {
         const int tap = k / 3, c = k - tap * 3;
         const int ky = tap / 7, kx = tap - ky * 7;
-        if ((unsigned)(iy0 + ky) < (unsigned)kNet && (unsigned)(ix0 + kx) < (unsigned)kNet) val = __ldg(x0 + (pb + (unsigned)((ky * kNet + kx) * 4 + c)));
+        if ((unsigned)(iy0 + ky) < (unsigned)IH && (unsigned)(ix0 + kx) < (unsigned)IW) val = __ldg(x0 + (pb + (unsigned)((ky * IW + kx) * 4 + c)));
       }
       v[e] = val;
     }
@@ -970,17 +970,20 @@ __global__ void __launch_bounds__(256) pred_argmax_decode_kernel(const float* __
 
 // =====================================================================================================
 // ParamNet input: cat(pred_gravity, pred_latitude) (param_network.py:47-49 / 194-197), optionally the nearest
-// 320 -> S sub-sample F.interpolate(images, (S, S)) (src = floor(dst * 320 / S)).  NCHW fields -> NHWC [B,S,S,4].
-__global__ void __launch_bounds__(256) pack_fields_kernel(const float* __restrict__ grav, const float* __restrict__ lat, float* __restrict__ out, int B, int S) {
-  const long long total = (long long)B * S * S;
+// IH x IW -> OH x OW sub-sample F.interpolate(images, (OH, OW)) (ATen nearest: src = floor(dst * (float)in / out), clamped).
+// NCHW fields at the net size IH x IW -> NHWC [B,OH,OW,4].
+__global__ void __launch_bounds__(256) pack_fields_kernel(const float* __restrict__ grav, const float* __restrict__ lat, float* __restrict__ out, int B, int IH,
+                                                          int IW, int OH, int OW) {
+  const long long total = (long long)B * OH * OW;
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total) return;
-  const int x = (int)(i % S), y = (int)((i / S) % S), b = (int)(i / ((long long)S * S));
-  const int sy = (int)floorf((float)y * ((float)kNet / (float)S)), sx = (int)floorf((float)x * ((float)kNet / (float)S));
-  const int sp = min(sy, kNet - 1) * kNet + min(sx, kNet - 1);
-  const float g0 = __ldg(grav + (long long)b * 2 * kNet * kNet + sp);
-  const float g1 = __ldg(grav + (long long)b * 2 * kNet * kNet + kNet * kNet + sp);
-  const float l0 = __ldg(lat + (long long)b * kNet * kNet + sp);
+  const int x = (int)(i % OW), y = (int)((i / OW) % OH), b = (int)(i / ((long long)OH * OW));
+  const int sy = (int)floorf((float)y * ((float)IH / (float)OH)), sx = (int)floorf((float)x * ((float)IW / (float)OW));
+  const long long IHW = (long long)IH * IW;
+  const int sp = min(sy, IH - 1) * IW + min(sx, IW - 1);
+  const float g0 = __ldg(grav + (long long)b * 2 * IHW + sp);
+  const float g1 = __ldg(grav + (long long)b * 2 * IHW + IHW + sp);
+  const float l0 = __ldg(lat + (long long)b * IHW + sp);
   reinterpret_cast<float4*>(out)[i] = make_float4(g0, g1, l0, 0.f);
 }
 

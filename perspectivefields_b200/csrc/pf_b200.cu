@@ -100,7 +100,6 @@ static const int kMitDims[4] = {64, 128, 320, 512};
 static const int kMitHeads[4] = {1, 2, 5, 8};
 static const int kMitDepths[4] = {3, 4, 18, 3};
 static const int kMitSr[4] = {8, 4, 2, 1};
-static const int kMitRes[4] = {80, 40, 20, 10};
 static const int kCnxDims[4] = {96, 192, 384, 768};
 static const int kCnxDepths[4] = {3, 3, 9, 3};
 
@@ -130,6 +129,7 @@ struct Arena {
 struct pf_engine {
   int device = 0;
   pf_model_desc desc{};
+  int net_h = kNet, net_w = kNet;     // working size (DATALOADER.RESIZE = [net_h, net_w]): multiples of 32 in [64, 640] (pf_create_sized)
   bool finalized = false;
   std::unordered_map<std::string, WeightRef> weights;
   // resolved weights
@@ -160,11 +160,11 @@ struct pf_engine {
   GemmW pn_ds[4];
   std::vector<CnxBlockW> pn_blocks[4];
   const float *pn_head_w, *pn_head_b;
-  // Pillow resample tables, cached per input size in one device slab owned by the engine (bump allocation; built on the host
+  // Pillow resample tables, cached per (input size, output size) in one device slab owned by the engine (bump allocation; built on the host
   // into a pinned mirror of the slab and copied with cudaMemcpyAsync on the caller's stream: no allocation and no
   // synchronising copy inside pf_forward)
   struct DevTable { int ksize; int* bounds; int* coeffs; };
-  std::map<int, DevTable> tables;
+  std::map<std::pair<int, int>, DevTable> tables;
   char* table_dev = nullptr;
   char* table_host = nullptr;       // pinned
   long long table_off = 0;
@@ -509,10 +509,10 @@ struct Fwd {
     LAUNCHED(layernorm_launch(x, yf, rows, C, w.w, w.b, eps, st, y));
     return PF_OK;
   }
-  // LayerNorm whose output is (also) written in patch order for a k = s = sr convolution on the R x R map (y may be empty)
-  int ln_split_patch(const float* x, const SplitT& y, const SplitT& patch, long long rows, int C, const LnW& w, float eps, int R, int sr) {
+  // LayerNorm whose output is (also) written in patch order for a k = s = sr convolution on the RH x RW map (y may be empty)
+  int ln_split_patch(const float* x, const SplitT& y, const SplitT& patch, long long rows, int C, const LnW& w, float eps, int RH, int RW, int sr) {
     if (dry) return PF_OK;
-    LAUNCHED(layernorm_launch(x, nullptr, rows, C, w.w, w.b, eps, st, y, patch, R, sr));
+    LAUNCHED(layernorm_launch(x, nullptr, rows, C, w.w, w.b, eps, st, y, patch, RH, RW, sr));
     return PF_OK;
   }
   int ln(const float* x, float* y, long long rows, int C, const LnW& w, float eps) {
@@ -524,10 +524,10 @@ struct Fwd {
 
 // ----------------------------------------------------------------------------------------------- the forward graph
 constexpr long long kTableSlabBytes = 8LL << 20;   // ~370 tables of a 2048-pixel axis; reset (after a stream sync) when full
-static int get_table(pf_engine* e, int in_size, pf_engine::DevTable* out, cudaStream_t st) {
-  auto it = e->tables.find(in_size);
+static int get_table(pf_engine* e, int in_size, int out_size, pf_engine::DevTable* out, cudaStream_t st) {
+  auto it = e->tables.find({in_size, out_size});
   if (it == e->tables.end()) {
-    ResampleTable t = make_resample_table(in_size, kNet);
+    ResampleTable t = make_resample_table(in_size, out_size);
     const long long nb = (long long)t.bounds.size() * sizeof(int), nc = (long long)t.coeffs.size() * sizeof(int);
     const long long need = ((nb + 255) & ~255LL) + ((nc + 255) & ~255LL);
     if (need > kTableSlabBytes) return fail(PF_ERR_ARG, "image axis of %d pixels is too long for the resize tables", in_size);
@@ -547,21 +547,21 @@ static int get_table(pf_engine* e, int in_size, pf_engine::DevTable* out, cudaSt
     d.coeffs = (int*)(e->table_dev + o1);
     CU(cudaMemcpyAsync(e->table_dev + o0, e->table_host + o0, need, cudaMemcpyHostToDevice, st));
     e->table_off += need;
-    it = e->tables.emplace(in_size, d).first;
+    it = e->tables.emplace(std::make_pair(in_size, out_size), d).first;
   }
   *out = it->second;
   return PF_OK;
 }
 
-static int pre_rows_needed(int H) {  // input rows one block of kPreRows output rows may need
-  const double scale = (double)H / kNet;
+static int pre_rows_needed(int H, int OH) {  // input rows one block of kPreRows output rows may need
+  const double scale = (double)H / OH;
   const double support = scale < 1.0 ? 1.0 : scale;
   return (int)(kPreRows * scale) + 2 * (int)ceil(support) + 3;
 }
-constexpr int kPreMaxSmemRows = 200 * 1024 / (kNet * 3);
+static int pre_max_smem_rows(int OW) { return kPreSmemBytes / (OW * 3); }   // resampled rows that fit the shared-memory budget
 
 // ----------------------------------------------------------------------------------------------- shared graph sections
-// uint8 HWC (any size) or pre-resized fp32 CHW -> x0 [n,320,320,4] fp32 normalised
+// uint8 HWC (any size) or pre-resized fp32 CHW -> x0 [n,NH,NW,4] fp32 normalised (NH x NW: the engine's working size)
 static int fwd_preprocess(Fwd& F, const pf_batch* bt, float*& x0, PreImage*& d_pre, PostImage*& d_post) {
   pf_engine* e = F.e;
   const pf_model_desc& D = e->desc;
@@ -569,8 +569,10 @@ static int fwd_preprocess(Fwd& F, const pf_batch* bt, float*& x0, PreImage*& d_p
   const bool dry = F.dry;
   cudaStream_t st = F.st;
   Arena& ar = F.ar;
-  // ---------------- pre-process: uint8 HWC (any size) -> [n,320,320,4] fp32 normalised -------------------
-  x0 = ar.f((long long)n * kNet * kNet * 4);
+  const int NH = e->net_h, NW = e->net_w;
+  const int max_rows = pre_max_smem_rows(NW);
+  // ---------------- pre-process: uint8 HWC (any size) -> [n,NH,NW,4] fp32 normalised -------------------
+  x0 = ar.f((long long)n * NH * NW * 4);
   d_pre = (PreImage*)ar.alloc((long long)n * sizeof(PreImage));
   d_post = (PostImage*)ar.alloc((long long)n * sizeof(PostImage));
   if (!dry) {
@@ -581,22 +583,22 @@ static int fwd_preprocess(Fwd& F, const pf_batch* bt, float*& x0, PreImage*& d_p
         const int H = bt->height[i], W = bt->width[i];
         if (H < 1 || W < 1) return fail(PF_ERR_ARG, "image %d has size %dx%d", i, H, W);
         pf_engine::DevTable tx, ty;
-        TRY(get_table(e, W, &tx, st));
-        TRY(get_table(e, H, &ty, st));
-        if (ty.ksize + 1 > kPreMaxSmemRows) return fail(PF_ERR_ARG, "image %d is too tall (%d rows) for the resize kernel", i, H);
+        TRY(get_table(e, W, NW, &tx, st));
+        TRY(get_table(e, H, NH, &ty, st));
+        if (ty.ksize + 1 > max_rows) return fail(PF_ERR_ARG, "image %d is too tall (%d rows) for the resize kernel", i, H);
         pre[i] = PreImage{bt->image_offset[i], H, W, tx.ksize, ty.ksize, tx.bounds, tx.coeffs, ty.bounds, ty.coeffs};
         if (H > max_h) max_h = H;
       }
       CU(cudaMemcpyAsync(d_pre, pre.data(), n * sizeof(PreImage), cudaMemcpyHostToDevice, st));
-      int rows = pre_rows_needed(max_h);
-      if (rows > kPreMaxSmemRows) rows = kPreMaxSmemRows;
-      const int smem = rows * kNet * 3;
-      LAUNCHED((preprocess_kernel<<<dim3(kNet / kPreRows, n), kNet, smem, st>>>(bt->images_u8, d_pre, x0, D.pixel_mean[0], D.pixel_mean[1],
-                                                                               D.pixel_mean[2], D.pixel_std[0], D.pixel_std[1], D.pixel_std[2], rows),
+      int rows = pre_rows_needed(max_h, NH);
+      if (rows > max_rows) rows = max_rows;
+      const int smem = rows * NW * 3;
+      LAUNCHED((preprocess_kernel<<<dim3(NH / kPreRows, n), NW, smem, st>>>(bt->images_u8, d_pre, x0, D.pixel_mean[0], D.pixel_mean[1],
+                                                                           D.pixel_mean[2], D.pixel_std[0], D.pixel_std[1], D.pixel_std[2], rows, NH, NW),
                 cudaGetLastError()));
     } else {
-      const long long total = (long long)n * kNet * kNet;
-      LAUNCHED((normalize_chw_kernel<<<(unsigned)cdivl(total, 256), 256, 0, st>>>(bt->images_chw, x0, n, D.pixel_mean[0], D.pixel_mean[1],
+      const long long total = (long long)n * NH * NW;
+      LAUNCHED((normalize_chw_kernel<<<(unsigned)cdivl(total, 256), 256, 0, st>>>(bt->images_chw, x0, n, NH, NW, D.pixel_mean[0], D.pixel_mean[1],
                                                                                  D.pixel_mean[2], D.pixel_std[0], D.pixel_std[1], D.pixel_std[2]),
                 cudaGetLastError()));
     }
@@ -604,8 +606,8 @@ static int fwd_preprocess(Fwd& F, const pf_batch* bt, float*& x0, PreImage*& d_p
   return PF_OK;
 }
 
-// resample of the (decoded) 320x320 fields to the original sizes: one launch for all images of the batch
-static int launch_postprocess(const float* vec, const float* lat, int n, const int32_t* height, const int32_t* width, const int64_t* g_off,
+// resample of the (decoded) SH x SW fields (the net size) to the original sizes: one launch for all images of the batch
+static int launch_postprocess(const float* vec, const float* lat, int n, int SH, int SW, const int32_t* height, const int32_t* width, const int64_t* g_off,
                               const int64_t* l_off, float* g_out, float* l_out, int lat_is_sin, PostImage* d_post, cudaStream_t st) {
   std::vector<PostImage> post(n);
   long long total = 0;
@@ -619,14 +621,14 @@ static int launch_postprocess(const float* vec, const float* lat, int n, const i
     if (wp <= kPostMaxW && wp > max_wp) max_wp = wp;    // (wider images take the table-less path of the kernel)
   }
   CU(cudaMemcpyAsync(d_post, post.data(), n * sizeof(PostImage), cudaMemcpyHostToDevice, st));
-  const int smem = max_wp * 8;
-  LAUNCHED((postprocess_kernel<<<dim3((unsigned)cdiv(max_h, kPostBand), (unsigned)n), kPostThreads, smem, st>>>(vec, lat, d_post, g_out, l_out, lat_is_sin),
+  const int smem = post_smem_bytes(SW, max_wp);
+  LAUNCHED((postprocess_kernel<<<dim3((unsigned)cdiv(max_h, kPostBand), (unsigned)n), kPostThreads, smem, st>>>(vec, lat, d_post, g_out, l_out, lat_is_sin, SH, SW),
             cudaGetLastError()));
   return PF_OK;
 }
 
 // prediction 1x1 convs (+ normalise / clamp) -> NCHW outputs, then argmax decode (classification) and resample to the
-// original resolutions.  conv1_out: [n,320,320,64] fp32 (gravity head channels 0-31, latitude head 32-63).
+// original resolutions.  conv1_out: [n,NH,NW,64] fp32 (gravity head channels 0-31, latitude head 32-63).
 static int fwd_tails_post(Fwd& F, const pf_batch* bt, const float* conv1_out, PostImage* d_post, bool pred_done = false) {
   pf_engine* e = F.e;
   const pf_model_desc& D = e->desc;
@@ -634,7 +636,7 @@ static int fwd_tails_post(Fwd& F, const pf_batch* bt, const float* conv1_out, Po
   const bool dry = F.dry;
   cudaStream_t st = F.st;
   Arena& ar = F.ar;
-  const int HW = kNet * kNet;
+  const int HW = e->net_h * e->net_w;
   const bool cls_g = D.gravity_classes != 2, cls_l = D.latitude_classes != 1;
   const bool fused_decode = e->decode_only && (cls_g || cls_l);
   if (e->decode_only && cls_g != cls_l) return fail(PF_ERR_ARG, "decode_only needs both heads to be classification heads");
@@ -683,7 +685,7 @@ static int fwd_tails_post(Fwd& F, const pf_batch* bt, const float* conv1_out, Po
   }
   // ---------------- post-process to the original resolutions ------------------------------------------------
   if (!dry)
-    TRY(launch_postprocess(vec, lat, n, bt->height, bt->width, bt->gravity_original_offset, bt->latitude_original_offset, bt->gravity_original,
+    TRY(launch_postprocess(vec, lat, n, e->net_h, e->net_w, bt->height, bt->width, bt->gravity_original_offset, bt->latitude_original_offset, bt->gravity_original,
                            bt->latitude_original, cls_l ? 0 : 1, d_post, st));
   return PF_OK;
 }
@@ -699,58 +701,68 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
   cudaStream_t st = F.st;
   Arena& ar = F.ar;
   using Epi = Fwd::Epi;
+  // working size NH x NW: the MiT stage grids are NH/4 x NW/4 ... NH/32 x NW/32, the attention key count of every stage is
+  // (NH/32) * (NW/32) (100 at 320 x 320), the head levels run at NH/32 x NW/32 ... NH/2 x NW/2
+  const int NH = e->net_h, NW = e->net_w;
+  int RH[4], RW[4];
+  for (int s = 0; s < 4; ++s) { RH[s] = NH >> (s + 2); RW[s] = NW >> (s + 2); }
+  const int nkv = RH[3] * RW[3];
+  if ((NH != kNet || NW != kNet) && (!e->use_attn_mma || !e->use_attn_split || !e->use_stem_tc || !e->use_phase))
+    return fail(PF_ERR_ARG, "options attn_mma / attn_split / stem_tc / phase_conv1 = 0 (reference paths of the 320 x 320 graph) need a 320 x 320 "
+                            "working size; this engine runs at %d x %d", NH, NW);
 
   float* x0; PreImage* d_pre; PostImage* d_post;
   {
     NvtxRange r_("pf:preprocess");
     TRY(fwd_preprocess(F, bt, x0, d_pre, d_post));
   }
-  TRY(F.tap("pre", x0, (long long)n * kNet * kNet * 4));
+  TRY(F.tap("pre", x0, (long long)n * NH * NW * 4));
 
   NvtxRange* sect = new NvtxRange("pf:ll_enc");
   struct SectGuard { NvtxRange*& p; ~SectGuard() { delete p; } } sect_guard{sect};
   auto section = [&](const char* name) { delete sect; sect = nullptr; sect = new NvtxRange(name); };
   SplitT cfeat[4];
-  for (int s = 0; s < 4; ++s) cfeat[s] = F.salloc((long long)n * kMitRes[s] * kMitRes[s], kMitDims[s]);
-  SplitT ll = F.salloc((long long)n * 160 * 160, 64);
+  for (int s = 0; s < 4; ++s) cfeat[s] = F.salloc((long long)n * RH[s] * RW[s], kMitDims[s]);
+  const int LH = NH / 2, LW = NW / 2;                 // low-level encoder / conv_fuse_conv0 grid
+  SplitT ll = F.salloc((long long)n * LH * LW, 64);
   if (e->use_stem_tc) {   // conv7x7/2 (+ folded BN + ReLU) as patch gather + TMA GEMM (K = 147 padded to 160)
     const long long m = ar.mark();
-    const long long M = (long long)n * 160 * 160;
+    const long long M = (long long)n * LH * LW;
     SplitT col = F.salloc(M, 160);
-    if (!dry) LAUNCHED(launch_pdl(stem_gather_kernel, dim3(ew_grid(stem_gather_threads(n, 160, 160))), dim3(256), 0, st, x0, col.hi, col.lo, n, 160, 160, 2));
+    if (!dry) LAUNCHED(launch_pdl(stem_gather_kernel, dim3(ew_grid(stem_gather_threads(n, LH, LW))), dim3(256), 0, st, x0, col.hi, col.lo, n, LH, LW, 2, NH, NW));
     Epi o; o.S = ll; o.act = 1;
     TRY(F.tgemm(col, M, 160, 0, e->llencg, 64, o));
     ar.release(m);
   } else if (!dry) {
     LAUNCHED((stem_conv_launch<7, 7, 2, 3, 64>(x0, 4, n, kNet, kNet, e->llenc_w, e->llenc_b, nullptr, 1, st, ll)));
   }
-  TRY(F.tap_split("ll", ll, (long long)n * 160 * 160 * 64));
+  TRY(F.tap_split("ll", ll, (long long)n * LH * LW * 64));
 
   // ---------------- MiT-B3 encoder ---------------------------------------------------------------------------
   for (int s = 0; s < 4; ++s) {
     { char nm[32]; snprintf(nm, sizeof nm, "pf:mit.stage%d", s + 1); section(nm); }
-    const int C = kMitDims[s], R = kMitRes[s], N = R * R, heads = kMitHeads[s], sr = kMitSr[s];
+    const int C = kMitDims[s], N = RH[s] * RW[s], heads = kMitHeads[s], sr = kMitSr[s];
     const long long rows = (long long)n * N;
     const long long m = ar.mark();
     float* x = ar.f(rows * C);
     float* tf = ar.f(rows * C);                      // patch-embed conv output (before its LayerNorm)
     SplitT t1 = F.salloc(rows, C);                   // LayerNorm output (GEMM input only)
-    SplitT t1p;                                      // the same in patch order [n*100, sr*sr*C]: A operand of the spatial-reduction conv
-    if (sr > 1) t1p = F.salloc((long long)n * 100, sr * sr * C);
+    SplitT t1p;                                      // the same in patch order [n*nkv, sr*sr*C]: A operand of the spatial-reduction conv
+    if (sr > 1) t1p = F.salloc((long long)n * nkv, sr * sr * C);
     SplitT q = F.salloc(rows, C);                    // q and kv leave their GEMMs as split planes: the attention core's MMA operands
     SplitT a = F.salloc(rows, C);                    // attention output
-    float* t2f = ar.f((long long)n * 100 * C);
-    SplitT t2 = F.salloc((long long)n * 100, C);
-    SplitT kv = F.salloc((long long)n * 100, 2 * C);
+    float* t2f = ar.f((long long)n * nkv * C);
+    SplitT t2 = F.salloc((long long)n * nkv, C);
+    SplitT kv = F.salloc((long long)n * nkv, 2 * C);
     const bool qkv_split = e->use_attn_mma && e->use_attn_split;
     float* qf = qkv_split ? nullptr : ar.f(rows * C);                        // (fp32 q / kv: CUDA-core attention kernel, or
-    float* kvf = qkv_split ? nullptr : ar.f((long long)n * 100 * 2 * C);     //  option attn_split = 0)
+    float* kvf = qkv_split ? nullptr : ar.f((long long)n * nkv * 2 * C);     //  option attn_split = 0)
     float* h1 = ar.f(rows * 4 * C);
     SplitT h2 = F.salloc(rows, 4 * C);
     if (s == 0 && e->use_stem_tc) {
       const long long mm = ar.mark();
       SplitT col = F.salloc(rows, 160);
-      if (!dry) LAUNCHED(launch_pdl(stem_gather_kernel, dim3(ew_grid(stem_gather_threads(n, 80, 80))), dim3(256), 0, st, x0, col.hi, col.lo, n, 80, 80, 4));
+      if (!dry) LAUNCHED(launch_pdl(stem_gather_kernel, dim3(ew_grid(stem_gather_threads(n, RH[0], RW[0]))), dim3(256), 0, st, x0, col.hi, col.lo, n, RH[0], RW[0], 4, NH, NW));
       Epi o; o.C = tf; o.ldc = C;
       TRY(F.tgemm(col, rows, 160, 0, e->embed1g, 64, o));
       ar.release(mm);
@@ -758,13 +770,13 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
       if (!dry) LAUNCHED((stem_conv_launch<7, 7, 4, 3, 64>(x0, 4, n, kNet, kNet, e->embed1_w, e->embed1_b, tf, 0, st)));
     } else {
       Epi o; o.C = tf; o.ldc = C;
-      TRY(F.tconv_gather(cfeat[s - 1], n, kMitRes[s - 1], kMitRes[s - 1], kMitDims[s - 1], 3, 2, 1, e->embed[s], C, o));
+      TRY(F.tconv_gather(cfeat[s - 1], n, RH[s - 1], RW[s - 1], kMitDims[s - 1], 3, 2, 1, e->embed[s], C, o));
     }
     TRY(F.ln(tf, x, rows, C, e->embed_ln[s], 1e-5f));
     TRY(F.tapf(x, rows * C, "mit.s%d.embed", s + 1));
     for (int i = 0; i < kMitDepths[s]; ++i) {
       const MitBlockW& b = e->blocks[s][i];
-      if (sr > 1) TRY(F.ln_split_patch(x, t1, t1p, rows, C, b.ln1, 1e-6f, R, sr));     // + the sr conv's im2col matrix
+      if (sr > 1) TRY(F.ln_split_patch(x, t1, t1p, rows, C, b.ln1, 1e-6f, RH[s], RW[s], sr));     // + the sr conv's im2col matrix
       else TRY(F.ln_split(x, t1, rows, C, b.ln1, 1e-6f));
       Epi oq, okv;
       if (qkv_split) { oq.S = q; okv.S = kv; } else { oq.C = qf; oq.ldc = C; okv.C = kvf; okv.ldc = 2 * C; }
@@ -777,9 +789,9 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
         F.st = e->side;
       }
       if (sr > 1) {
-        { Epi o; o.C = t2f; o.ldc = C; TRY(F.tgemm(t1p, (long long)n * 100, sr * sr * C, 0, b.sr, C, o)); }
-        TRY(F.ln_split(t2f, t2, (long long)n * 100, C, b.srln, 1e-5f));
-        TRY(F.tgemm(t2, (long long)n * 100, C, 0, b.kv, 2 * C, okv));
+        { Epi o; o.C = t2f; o.ldc = C; TRY(F.tgemm(t1p, (long long)n * nkv, sr * sr * C, 0, b.sr, C, o)); }
+        TRY(F.ln_split(t2f, t2, (long long)n * nkv, C, b.srln, 1e-5f));
+        TRY(F.tgemm(t2, (long long)n * nkv, C, 0, b.kv, 2 * C, okv));
       }
       if (fork) {
         CU(cudaEventRecord(e->ev_join, e->side));
@@ -792,7 +804,7 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
         TRY(F.tgemm(t1, rows, C, 0, b.kv, 2 * C, okv));
       }
       if (!dry) {
-        if (qkv_split) LAUNCHED(attention_mma_launch(nullptr, nullptr, nullptr, n, N, C, heads, st, a, q, kv, F.np()));
+        if (qkv_split) LAUNCHED(attention_mma_launch(nullptr, nullptr, nullptr, n, N, C, heads, st, a, q, kv, F.np(), nkv));
         else if (e->use_attn_mma) LAUNCHED(attention_mma_launch(qf, kvf, nullptr, n, N, C, heads, st, a, SplitT(), SplitT(), F.np()));
         else LAUNCHED(attention_launch(qf, kvf, nullptr, n, N, C, heads, st, a));
       }
@@ -800,7 +812,7 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
       TRY(F.tapf(x, rows * C, "mit.s%d.b%d.attn", s + 1, i));
       TRY(F.ln_split(x, t1, rows, C, b.ln2, 1e-6f));
       { Epi o; o.C = h1; o.ldc = 4 * C; TRY(F.tgemm(t1, rows, C, 0, b.fc1, 4 * C, o)); }
-      if (!dry) LAUNCHED(launch_pdl(dwconv3x3_gelu_kernel, dim3(ew_grid((long long)n * ((R + 1) / 2) * ((R + PF_DW3_PX - 1) / PF_DW3_PX) * C)), dim3(256), 0, st, h1, nullptr, n, R, R, 4 * C, b.dw_w, b.dw_b, h2.hi, h2.lo));
+      if (!dry) LAUNCHED(launch_pdl(dwconv3x3_gelu_kernel, dim3(ew_grid((long long)n * ((RH[s] + 1) / 2) * ((RW[s] + PF_DW3_PX - 1) / PF_DW3_PX) * C)), dim3(256), 0, st, h1, nullptr, n, RH[s], RW[s], 4 * C, b.dw_w, b.dw_b, h2.hi, h2.lo));
       { Epi o; o.C = x; o.ldc = C; o.res = x; o.ldr = C; TRY(F.tgemm(h2, rows, 4 * C, 0, b.fc2, C, o)); }
       TRY(F.tapf(x, rows * C, "mit.s%d.b%d", s + 1, i));
     }
@@ -810,16 +822,16 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
   }
 
   // ---------------- decoder heads (group 0 = gravity, group 1 = latitude, side by side in the channel dimension) ----
-  float* conv1_out = ar.f((long long)n * kNet * kNet * 64);
+  float* conv1_out = ar.f((long long)n * NH * NW * 64);
   bool fuse_pred = false;
   {
     const long long m = ar.mark();
     float* fused = nullptr;       // fp32 top-down feature of the previous level, upsampled to this level's resolution
-    SplitT fused_s;               // level 1 only: the final fused feature at 160x160, split (input of conv_fuse_conv0)
+    SplitT fused_s;               // level 1 only: the final fused feature at LH x LW, split (input of conv_fuse_conv0)
     for (int lvl = 4; lvl >= 1; --lvl) {
       { char nm[32]; snprintf(nm, sizeof nm, "pf:heads.level%d", lvl); section(nm); }
-      const int r = kMitRes[lvl - 1], Cin = kMitDims[lvl - 1];
-      const long long px = (long long)n * r * r;
+      const int rh = RH[lvl - 1], rw = RW[lvl - 1], Cin = kMitDims[lvl - 1];
+      const long long px = (long long)n * rh * rw;
       float* t = ar.f(px * 512);
       SplitT rt = F.salloc(px, 512);        // relu(t)
       SplitT u = F.salloc(px, 512);         // rectified conv1 outputs
@@ -828,12 +840,12 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
       float* w2 = ar.f(px * 512);
       {   // composed linear_c{lvl} o linear_c{lvl}_proc (both heads: N = 512), border-class bias
         Epi o; o.C = t; o.ldc = 512; o.S = rt; o.split_relu = 1; o.bias_mode = 2;
-        TRY(F.thalo(cfeat[lvl - 1], 0, 0, nullptr, 0, 0, n, r, r, Cin, e->proc[lvl - 1], 512, 1, 0, o));
+        TRY(F.thalo(cfeat[lvl - 1], 0, 0, nullptr, 0, 0, n, rh, rw, Cin, e->proc[lvl - 1], 512, 1, 0, o));
         TRY(F.tapf(t, px * 512, "head.proc%d", lvl));
       }
       auto rcu = [&](const SplitT& A, const GemmW& w, Epi o) {
         o.c_gcoff = 256; o.s_gcoff = 256; o.r_gcoff = 256; o.r2_gcoff = 256;
-        return F.thalo(A, 0, 256, nullptr, 0, 0, n, r, r, 256, w, 256, 2, 256, o);
+        return F.thalo(A, 0, 256, nullptr, 0, 0, n, rh, rw, 256, w, 256, 2, 256, o);
       };
       const float* of = t;
       const SplitT* os = &rt;
@@ -847,12 +859,12 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
       { Epi o; o.C = w2; o.ldc = 512; o.res = of; o.ldr = 512; o.res_relu = 1; TRY(rcu(u, e->rcu[lvl - 1][1][1], o)); }
       if (lvl > 1) {
         float* up = ar.f(px * 4 * 512);
-        if (!dry) LAUNCHED(launch_pdl(upsample2x_kernel, dim3(ew_grid(upsample2x_threads(n, r, r, 512))), dim3(256), 0, st, w2, 512, 0, up, 512, 0, n, r, r, 512, nullptr, nullptr));
+        if (!dry) LAUNCHED(launch_pdl(upsample2x_kernel, dim3(ew_grid(upsample2x_threads(n, rh, rw, 512))), dim3(256), 0, st, w2, 512, 0, up, 512, 0, n, rh, rw, 512, nullptr, nullptr));
         fused = up;
         TRY(F.tapf(up, px * 4 * 512, "head.fusion%d", lvl));
       } else {
         fused_s = F.salloc(px * 4, 512);
-        if (!dry) LAUNCHED(launch_pdl(upsample2x_kernel, dim3(ew_grid(upsample2x_threads(n, r, r, 512))), dim3(256), 0, st, w2, 512, 0, nullptr, 512, 0, n, r, r, 512, fused_s.hi, fused_s.lo));
+        if (!dry) LAUNCHED(launch_pdl(upsample2x_kernel, dim3(ew_grid(upsample2x_threads(n, rh, rw, 512))), dim3(256), 0, st, w2, 512, 0, nullptr, 512, 0, n, rh, rw, 512, fused_s.hi, fused_s.lo));
         TRY(F.tap_split("head.fusion1", fused_s, px * 4 * 512));
       }
     }
@@ -864,20 +876,20 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
     const bool keep_conv1 = !fuse_pred || e->debug;   // (not `o.C != nullptr`: the sizing dry run has null pointers)
     PredTail pt[2] = {{e->pred_g_w, e->pred_g_b, dry ? nullptr : bt->pred_gravity, 2, 1}, {e->pred_l_w, e->pred_l_b, dry ? nullptr : bt->pred_latitude, 1, 2}};
     if (e->use_phase) {
-      // x2 upsample folded into conv1's weights: conv1 runs on the 160x160 grid with N = 4 output phases x 32 (no upsampled
+      // x2 upsample folded into conv1's weights: conv1 runs on the LH x LW grid with N = 4 output phases x 32 (no upsampled
       // tensor); the two outermost output rows / columns, where the identity does not hold, are recomputed by conv1_ring_kernel
-      SplitT c0s = F.salloc((long long)n * 160 * 160, 128);
+      SplitT c0s = F.salloc((long long)n * LH * LW, 128);
       {
         Epi o; o.S = c0s; o.s_gcoff = 64; o.act = 1;
-        TRY(F.thalo(fused_s, 0, 256, &ll, 256, 0, n, 160, 160, 320, e->conv0, 64, 2, 64, o));
-        TRY(F.tap_split("head.conv0", c0s, (long long)n * 160 * 160 * 128));
+        TRY(F.thalo(fused_s, 0, 256, &ll, 256, 0, n, LH, LW, 320, e->conv0, 64, 2, 64, o));
+        TRY(F.tap_split("head.conv0", c0s, (long long)n * LH * LW * 128));
       }
       Epi o; o.ldc = 64; o.c_gcoff = 32; o.act = 1; o.phase4 = 1;
       if (keep_conv1) o.C = conv1_out;
-      TRY(F.thalo(c0s, 0, 64, nullptr, 0, 0, n, 160, 160, 64, e->conv1p, 128, 2, 128, o, fuse_pred ? pt : nullptr));
+      TRY(F.thalo(c0s, 0, 64, nullptr, 0, 0, n, LH, LW, 64, e->conv1p, 128, 2, 128, o, fuse_pred ? pt : nullptr));
       if (!dry) {
-        const dim3 grid((unsigned)cdiv(conv1_ring_count(kNet, kNet), kRingPx), (unsigned)n);
-        LAUNCHED((conv1_ring_kernel<<<grid, 256, kRingSmem, st>>>(c0s.hi, c0s.lo, 160, 160, e->conv1f_w, e->conv1f_b, keep_conv1 ? conv1_out : nullptr,
+        const dim3 grid((unsigned)cdiv(conv1_ring_count(NH, NW), kRingPx), (unsigned)n);
+        LAUNCHED((conv1_ring_kernel<<<grid, 256, kRingSmem, st>>>(c0s.hi, c0s.lo, LH, LW, e->conv1f_w, e->conv1f_b, keep_conv1 ? conv1_out : nullptr,
                                                                  fuse_pred ? e->pred_g_w : nullptr, e->pred_g_b, bt->pred_gravity,
                                                                  fuse_pred ? e->pred_l_w : nullptr, e->pred_l_b, bt->pred_latitude), cudaGetLastError()));
       }
@@ -894,7 +906,7 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
       if (keep_conv1) o.C = conv1_out;
       TRY(F.thalo(c0u, 0, 64, nullptr, 0, 0, n, kNet, kNet, 64, e->conv1, 32, 2, 32, o, fuse_pred ? pt : nullptr));
     }
-    if (keep_conv1) TRY(F.tap("head.conv1", conv1_out, (long long)n * kNet * kNet * 64));
+    if (keep_conv1) TRY(F.tap("head.conv1", conv1_out, (long long)n * NH * NW * 64));
     ar.release(m);
   }
   section("pf:tails_postprocess");
@@ -904,34 +916,36 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
   if (D.param_net != PF_PARAM_NONE) {
     section("pf:paramnet");
     if (D.gravity_classes != 2 || D.latitude_classes != 1) return fail(PF_ERR_ARG, "ParamNet needs regression heads");
-    const int S = D.param_net == PF_PARAM_CENTERED ? kNet : D.param_input_size;
-    float* pin = ar.f((long long)n * S * S * 4);
-    if (!dry) LAUNCHED((pack_fields_kernel<<<(unsigned)cdivl((long long)n * S * S, 256), 256, 0, st>>>(bt->pred_gravity, bt->pred_latitude, pin, n, S), cudaGetLastError()));
-    int r = S / 4;
-    float* x = ar.f((long long)n * r * r * 96);
-    if (!dry) LAUNCHED((stem_conv_launch<4, 4, 4, 0, 96>(pin, 4, n, S, S, e->pn_stem_w, e->pn_stem_b, x, 0, st)));
-    TRY(F.ln(x, x, (long long)n * r * r, 96, e->pn_stem_ln, 1e-6f));
+    // centered: ConvNeXt on the fields at the net size; uncentered: nearest resample to INPUT_SIZE x INPUT_SIZE first
+    const bool centered = D.param_net == PF_PARAM_CENTERED;
+    const int SH = centered ? NH : D.param_input_size, SW = centered ? NW : D.param_input_size;
+    float* pin = ar.f((long long)n * SH * SW * 4);
+    if (!dry) LAUNCHED((pack_fields_kernel<<<(unsigned)cdivl((long long)n * SH * SW, 256), 256, 0, st>>>(bt->pred_gravity, bt->pred_latitude, pin, n, NH, NW, SH, SW), cudaGetLastError()));
+    int rh = SH / 4, rw = SW / 4;
+    float* x = ar.f((long long)n * rh * rw * 96);
+    if (!dry) LAUNCHED((stem_conv_launch<4, 4, 4, 0, 96>(pin, 4, n, SH, SW, e->pn_stem_w, e->pn_stem_b, x, 0, st)));
+    TRY(F.ln(x, x, (long long)n * rh * rw, 96, e->pn_stem_ln, 1e-6f));
     for (int s = 0; s < 4; ++s) {
       const int C = kCnxDims[s];
       if (s > 0) {
-        const int r2 = r / 2;
-        SplitT y = F.salloc((long long)n * r2 * r2, 4 * kCnxDims[s - 1]);      // LayerNorm output written directly as the 2x2/2 conv's im2col matrix
-        TRY(F.ln_split_patch(x, SplitT(), y, (long long)n * r * r, kCnxDims[s - 1], e->pn_ds_ln[s], 1e-6f, r, 2));
-        float* xn = ar.f((long long)n * r2 * r2 * C);
+        const int r2h = rh / 2, r2w = rw / 2;
+        SplitT y = F.salloc((long long)n * r2h * r2w, 4 * kCnxDims[s - 1]);      // LayerNorm output written directly as the 2x2/2 conv's im2col matrix
+        TRY(F.ln_split_patch(x, SplitT(), y, (long long)n * rh * rw, kCnxDims[s - 1], e->pn_ds_ln[s], 1e-6f, rh, rw, 2));
+        float* xn = ar.f((long long)n * r2h * r2w * C);
         Epi o; o.C = xn; o.ldc = C;
-        TRY(F.tgemm(y, (long long)n * r2 * r2, 4 * kCnxDims[s - 1], 0, e->pn_ds[s], C, o));
-        x = xn; r = r2;
+        TRY(F.tgemm(y, (long long)n * r2h * r2w, 4 * kCnxDims[s - 1], 0, e->pn_ds[s], C, o));
+        x = xn; rh = r2h; rw = r2w;
       }
-      const long long rows = (long long)n * r * r;
+      const long long rows = (long long)n * rh * rw;
       float* yf = ar.f(rows * C);
       SplitT y = F.salloc(rows, C);
       SplitT h = F.salloc(rows, 4 * C);
       for (int j = 0; j < kCnxDepths[s]; ++j) {
         const CnxBlockW& b = e->pn_blocks[s][j];
         if (e->use_dwln) {   // depthwise 7x7 + LayerNorm in one kernel, straight to the split planes pwconv1 loads
-          if (!dry) LAUNCHED(dwconv7x7_ln_launch(x, n, r, r, C, b.dw_w, b.dw_b, b.ln.w, b.ln.b, 1e-6f, y, st));
+          if (!dry) LAUNCHED(dwconv7x7_ln_launch(x, n, rh, rw, C, b.dw_w, b.dw_b, b.ln.w, b.ln.b, 1e-6f, y, st));
         } else {
-          if (!dry) LAUNCHED(launch_pdl(dwconv7x7_kernel, dim3(ew_grid((long long)n * ((r + 1) / 2) * ((r + PF_DW7_PX - 1) / PF_DW7_PX) * (C / 4))), dim3(256), 0, st, x, yf, n, r, r, C, b.dw_w, b.dw_b));
+          if (!dry) LAUNCHED(launch_pdl(dwconv7x7_kernel, dim3(ew_grid((long long)n * ((rh + 1) / 2) * ((rw + PF_DW7_PX - 1) / PF_DW7_PX) * (C / 4))), dim3(256), 0, st, x, yf, n, rh, rw, C, b.dw_w, b.dw_b));
           TRY(F.ln_split(yf, y, rows, C, b.ln, 1e-6f));
         }
         { Epi o; o.S = h; o.act = 2; TRY(F.tgemm(y, rows, C, 0, b.pw1, 4 * C, o)); }
@@ -941,7 +955,7 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
     }
     if (!dry) {
       if (!bt->params) return fail(PF_ERR_ARG, "params output is NULL");
-      LAUNCHED((param_tail_kernel<<<n, 256, 0, st>>>(x, r * r, e->pn_norm.w, e->pn_norm.b, e->pn_head_w, e->pn_head_b, bt->params, D.param_net), cudaGetLastError()));
+      LAUNCHED((param_tail_kernel<<<n, 256, 0, st>>>(x, rh * rw, e->pn_norm.w, e->pn_norm.b, e->pn_head_w, e->pn_head_b, bt->params, D.param_net), cudaGetLastError()));
     }
   }
   return PF_OK;
@@ -966,7 +980,8 @@ static int configure_device(int device) {
   CU(attention_mma_configure_device());
   CU(cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem));
   CU(cudaFuncSetAttribute(conv1_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kRingSmem));
-  CU(cudaFuncSetAttribute(preprocess_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPreMaxSmemRows * kNet * 3));
+  CU(cudaFuncSetAttribute(preprocess_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPreSmemBytes));
+  CU(cudaFuncSetAttribute(postprocess_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPostSmemMax));
   if (device >= (int)done.size()) done.resize(device + 1, 0);
   done[device] = 1;
   return PF_OK;
@@ -977,8 +992,18 @@ static int configure_current_device() {
   return configure_device(dev);
 }
 
-int pf_create(int device, const pf_model_desc* desc, pf_handle* out) {
+// a working size the engine supports: H and W multiples of 32 in [64, 640] (the smallest head level is then at least 2 x 2, which
+// the border-class bias needs) with at most kAmMaxKeys attention keys (H/32) * (W/32)
+static bool net_size_ok(int h, int w) {
+  return h >= 64 && w >= 64 && h <= 640 && w <= 640 && h % 32 == 0 && w % 32 == 0 && (h / 32) * (w / 32) <= kAmMaxKeys;
+}
+
+int pf_create(int device, const pf_model_desc* desc, pf_handle* out) { return pf_create_sized(device, desc, kNet, kNet, out); }
+
+int pf_create_sized(int device, const pf_model_desc* desc, int net_h, int net_w, pf_handle* out) {
   if (!desc || !out) return fail(PF_ERR_ARG, "pf_create: null argument");
+  if (!net_size_ok(net_h, net_w))
+    return fail(PF_ERR_ARG, "pf_create: working size %dx%d: height and width must be multiples of 32 in [64, 640] with (H/32)*(W/32) <= %d", net_h, net_w, kAmMaxKeys);
   if (!((desc->gravity_classes == 2 || desc->gravity_classes == 73) && (desc->latitude_classes == 1 || desc->latitude_classes == 180)))
     return fail(PF_ERR_ARG, "pf_create: unsupported head widths %d/%d", desc->gravity_classes, desc->latitude_classes);
   if (desc->param_net < 0 || desc->param_net > 2) return fail(PF_ERR_ARG, "pf_create: bad param_net");
@@ -996,6 +1021,8 @@ int pf_create(int device, const pf_model_desc* desc, pf_handle* out) {
   e->device = device;
   e->sm_count = prop.multiProcessorCount;
   e->desc = *desc;
+  e->net_h = net_h;
+  e->net_w = net_w;
   if (cudaMalloc(&e->table_dev, kTableSlabBytes) != cudaSuccess || cudaMallocHost(&e->table_host, kTableSlabBytes) != cudaSuccess) {
     const int r = fail(PF_ERR_CUDA, "pf_create: resize-table slab: %s", cudaGetErrorString(cudaGetLastError()));
     cudaFree(e->table_dev);
@@ -1536,9 +1563,19 @@ int pf_op_postprocess(const float* vec, const float* lat, int n, const int32_t* 
                       void* stream) {
   if (!vec || !lat || n < 1 || !height || !width || !gravity_original || !gravity_original_offset || !latitude_original || !latitude_original_offset)
     return fail(PF_ERR_ARG, "pf_op_postprocess: bad argument");
+  return pf_op_postprocess_sized(vec, lat, n, kNet, kNet, height, width, gravity_original, gravity_original_offset, latitude_original, latitude_original_offset,
+                                 lat_is_sin, stream);
+}
+int pf_op_postprocess_sized(const float* vec, const float* lat, int n, int net_h, int net_w, const int32_t* height, const int32_t* width, float* gravity_original,
+                            const int64_t* gravity_original_offset, float* latitude_original, const int64_t* latitude_original_offset, int lat_is_sin,
+                            void* stream) {
+  if (!vec || !lat || n < 1 || !height || !width || !gravity_original || !gravity_original_offset || !latitude_original || !latitude_original_offset)
+    return fail(PF_ERR_ARG, "pf_op_postprocess: bad argument");
+  if (!net_size_ok(net_h, net_w)) return fail(PF_ERR_ARG, "pf_op_postprocess: unsupported working size %dx%d", net_h, net_w);
+  TRY(configure_current_device());
   PostImage* d_post = nullptr;
   CU(cudaMalloc(&d_post, n * sizeof(PostImage)));
-  int r = launch_postprocess(vec, lat, n, height, width, gravity_original_offset, latitude_original_offset, gravity_original, latitude_original,
+  int r = launch_postprocess(vec, lat, n, net_h, net_w, height, width, gravity_original_offset, latitude_original_offset, gravity_original, latitude_original,
                              lat_is_sin, d_post, (cudaStream_t)stream);
   cudaError_t se = cudaStreamSynchronize((cudaStream_t)stream);
   cudaFree(d_post);
@@ -1567,8 +1604,9 @@ int pf_op_attention_mma(const float* q, const float* kv, float* out, int B, int 
   LAUNCHED(attention_mma_launch(q, kv, out, B, N, C, heads, (cudaStream_t)stream));
   return PF_OK;
 }
-static int op_attention_tc(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream, int np) {
+static int op_attention_tc(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream, int np, int nkv = kAmKeys) {
   if (!q || !kv || !out || C != heads * kAmD) return fail(PF_ERR_ARG, "pf_op_attention_tc: head_dim must be 64");
+  if (B < 1 || N < 1 || nkv < 1 || nkv > kAmMaxKeys) return fail(PF_ERR_ARG, "pf_op_attention_tc: B %d, N %d, %d keys (1..%d)", B, N, nkv, kAmMaxKeys);
   TRY(configure_current_device());
   cudaStream_t st = (cudaStream_t)stream;
   int dev = 0;
@@ -1578,18 +1616,18 @@ static int op_attention_tc(const float* q, const float* kv, float* out, int B, i
   pf_engine tmp;
   tmp.device = dev;
   tmp.sm_count = prop.multiProcessorCount;
-  const long long nq = (long long)B * N * C, nkv = (long long)B * kAmKeys * 2 * C;
+  const long long nq = (long long)B * N * C, nkve = (long long)B * nkv * 2 * C;
   char* scratch = nullptr;
-  CU(cudaMalloc(&scratch, (2 * nq + nkv) * 4 + 8192));
+  CU(cudaMalloc(&scratch, (2 * nq + nkve) * 4 + 8192));
   Fwd F{&tmp, Arena{}, st, false, B};
-  F.ar.base = scratch; F.ar.cap = (2 * nq + nkv) * 4 + 8192;
-  SplitT qs = F.salloc((long long)B * N, C), kvs = F.salloc((long long)B * kAmKeys, 2 * C), as = F.salloc((long long)B * N, C);
+  F.ar.base = scratch; F.ar.cap = (2 * nq + nkve) * 4 + 8192;
+  SplitT qs = F.salloc((long long)B * N, C), kvs = F.salloc((long long)B * nkv, 2 * C), as = F.salloc((long long)B * N, C);
   int r = PF_OK;
   cudaError_t le = (split_kernel<<<(unsigned)cdivl(nq, 256), 256, 0, st>>>(q, qs.hi, qs.lo, nq, 0), cudaGetLastError());
-  if (le == cudaSuccess) le = (split_kernel<<<(unsigned)cdivl(nkv, 256), 256, 0, st>>>(kv, kvs.hi, kvs.lo, nkv, 0), cudaGetLastError());
+  if (le == cudaSuccess) le = (split_kernel<<<(unsigned)cdivl(nkve, 256), 256, 0, st>>>(kv, kvs.hi, kvs.lo, nkve, 0), cudaGetLastError());
   if (le != cudaSuccess) r = fail(PF_ERR_CUDA, "split_kernel: %s", cudaGetErrorString(le));
   if (r == PF_OK) {
-    le = attention_mma_launch(nullptr, nullptr, nullptr, B, N, C, heads, st, as, qs, kvs, np);
+    le = attention_mma_launch(nullptr, nullptr, nullptr, B, N, C, heads, st, as, qs, kvs, np, nkv);
     if (le != cudaSuccess) r = fail(PF_ERR_CUDA, "attention_mma_launch: %s", cudaGetErrorString(le));
   }
   if (r == PF_OK) {
@@ -1607,6 +1645,9 @@ int pf_op_attention_tc(const float* q, const float* kv, float* out, int B, int N
 int pf_op_attention_tc_bf16(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream) {
   return op_attention_tc(q, kv, out, B, N, C, heads, stream, 1);
 }
+int pf_op_attention_tc_keys(const float* q, const float* kv, float* out, int B, int N, int NKV, int C, int heads, int bf16, void* stream) {
+  return op_attention_tc(q, kv, out, B, N, C, heads, stream, bf16 ? 1 : 3, NKV);
+}
 int pf_op_dwconv3x3_gelu(const float* x, float* y, int B, int H, int W, int C, const float* w, const float* bias, void* stream) {
   if (C % 4) return fail(PF_ERR_ARG, "C %% 4");
   LAUNCHED(launch_pdl(dwconv3x3_gelu_kernel, dim3(ew_grid((long long)B * ((H + 1) / 2) * ((W + PF_DW3_PX - 1) / PF_DW3_PX) * (C / 4))), dim3(256), 0, (cudaStream_t)stream, x, y, B, H, W, C, w, bias, nullptr, nullptr));
@@ -1623,10 +1664,16 @@ int pf_op_upsample2x(const float* x, float* y, int B, int H, int W, int C, void*
   return PF_OK;
 }
 int pf_op_preprocess(const uint8_t* img, int H, int W, const float* mean3, const float* std3, float* y, void* stream) {
+  return pf_op_preprocess_sized(img, H, W, kNet, kNet, mean3, std3, y, stream);
+}
+int pf_op_preprocess_sized(const uint8_t* img, int H, int W, int net_h, int net_w, const float* mean3, const float* std3, float* y, void* stream) {
+  if (!img || !mean3 || !std3 || !y || H < 1 || W < 1) return fail(PF_ERR_ARG, "pf_op_preprocess: bad argument");
+  if (!net_size_ok(net_h, net_w)) return fail(PF_ERR_ARG, "pf_op_preprocess: unsupported working size %dx%d", net_h, net_w);
   TRY(configure_current_device());
   // standalone tables (not cached): test entry point only
-  ResampleTable tx = make_resample_table(W, kNet), ty = make_resample_table(H, kNet);
-  if (ty.ksize + 1 > kPreMaxSmemRows) return fail(PF_ERR_ARG, "image too tall");
+  ResampleTable tx = make_resample_table(W, net_w), ty = make_resample_table(H, net_h);
+  const int max_rows = pre_max_smem_rows(net_w);
+  if (ty.ksize + 1 > max_rows) return fail(PF_ERR_ARG, "image too tall");
   int *bx, *cx, *by, *cy;
   PreImage* d;
   CU(cudaMalloc(&bx, tx.bounds.size() * 4)); CU(cudaMalloc(&cx, tx.coeffs.size() * 4));
@@ -1638,10 +1685,11 @@ int pf_op_preprocess(const uint8_t* img, int H, int W, const float* mean3, const
   CU(cudaMemcpy(cy, ty.coeffs.data(), ty.coeffs.size() * 4, cudaMemcpyHostToDevice));
   PreImage pi{0, H, W, tx.ksize, ty.ksize, bx, cx, by, cy};
   CU(cudaMemcpy(d, &pi, sizeof pi, cudaMemcpyHostToDevice));
-  int rows = pre_rows_needed(H);
-  if (rows > kPreMaxSmemRows) rows = kPreMaxSmemRows;
-  const int smem = rows * kNet * 3;
-  LAUNCHED((preprocess_kernel<<<dim3(kNet / kPreRows, 1), kNet, smem, (cudaStream_t)stream>>>(img, d, y, mean3[0], mean3[1], mean3[2], std3[0], std3[1], std3[2], rows),
+  int rows = pre_rows_needed(H, net_h);
+  if (rows > max_rows) rows = max_rows;
+  const int smem = rows * net_w * 3;
+  LAUNCHED((preprocess_kernel<<<dim3(net_h / kPreRows, 1), net_w, smem, (cudaStream_t)stream>>>(img, d, y, mean3[0], mean3[1], mean3[2], std3[0], std3[1], std3[2], rows,
+                                                                                                 net_h, net_w),
             cudaGetLastError()));
   CU(cudaStreamSynchronize((cudaStream_t)stream));
   cudaFree(bx); cudaFree(cx); cudaFree(by); cudaFree(cy); cudaFree(d);

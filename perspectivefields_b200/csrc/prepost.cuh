@@ -16,10 +16,10 @@ namespace pf {
 // precompute_coeffs/normalize_coeffs_8bpc do; the kernel is pure integer arithmetic and therefore bit-exact.
 constexpr int kPrecisionBits = 32 - 8 - 2;
 
-struct ResampleTable {  // host-side, for one (in_size -> 320) axis
+struct ResampleTable {  // host-side, for one (in_size -> out_size) axis
   int in_size = 0, ksize = 0;
-  std::vector<int> bounds;  // [320][2] = (xmin, count)
-  std::vector<int> coeffs;  // [320][ksize]
+  std::vector<int> bounds;  // [out_size][2] = (xmin, count)
+  std::vector<int> coeffs;  // [out_size][ksize]
 };
 
 inline ResampleTable make_resample_table(int in_size, int out_size) {
@@ -67,14 +67,16 @@ struct PreImage {          // per image, device-visible
   const int* by; const int* cy;   // vertical tables   (depend on H)
 };
 
-constexpr int kPreRows = 8;  // output rows per block
+constexpr int kPreRows = 8;        // output rows per block
+constexpr int kPreMaxW = 640;      // widest working size (block = one thread per output column)
+constexpr int kPreSmemBytes = 200 * 1024;   // budget of the horizontally resampled rows: 213 rows of 320 columns, 106 of 640
 
-// grid = (320 / kPreRows, n_images), block = 320 threads (one per output column).
-// dyn smem = rows_needed * 320 * 3 bytes for the horizontally resampled input rows of this tile.
-// out: [n, 320, 320, 4] fp32 NHWC, channels (b, g, r, 0), value = (u8 - mean[c]) / std[c].
-__global__ void __launch_bounds__(kNet) preprocess_kernel(const unsigned char* __restrict__ blob, const PreImage* __restrict__ imgs, float* __restrict__ out,
-                                                          float m0, float m1, float m2, float s0, float s1, float s2, int max_rows) {
-  extern __shared__ unsigned char s_h[];  // [rows][320][3]
+// grid = (OH / kPreRows, n_images), block = OW threads (one per output column); OH = net height, OW = net width.
+// dyn smem = rows_needed * OW * 3 bytes for the horizontally resampled input rows of this tile.
+// out: [n, OH, OW, 4] fp32 NHWC, channels (b, g, r, 0), value = (u8 - mean[c]) / std[c].
+__global__ void __launch_bounds__(kPreMaxW) preprocess_kernel(const unsigned char* __restrict__ blob, const PreImage* __restrict__ imgs, float* __restrict__ out,
+                                                              float m0, float m1, float m2, float s0, float s1, float s2, int max_rows, int OH, int OW) {
+  extern __shared__ unsigned char s_h[];  // [rows][OW][3]
   const PreImage im = imgs[blockIdx.y];
   const int oy0 = blockIdx.x * kPreRows;
   const int x = threadIdx.x;
@@ -94,7 +96,7 @@ __global__ void __launch_bounds__(kNet) preprocess_kernel(const unsigned char* _
       ++rcount;
     }
     const int nrows = in_last - in_first;
-    // horizontal pass: input rows [in_first, in_last) -> uint8 [nrows][320][3]
+    // horizontal pass: input rows [in_first, in_last) -> uint8 [nrows][OW][3]
     for (int r = 0; r < nrows; ++r) {
       const unsigned char* row = src + ((long long)(in_first + r) * im.W + xmin) * 3;
       int a0 = 1 << (kPrecisionBits - 1), a1 = a0, a2 = a0;
@@ -102,7 +104,7 @@ __global__ void __launch_bounds__(kNet) preprocess_kernel(const unsigned char* _
         const int k = kx[t];
         a0 += row[3 * t] * k; a1 += row[3 * t + 1] * k; a2 += row[3 * t + 2] * k;
       }
-      unsigned char* d = s_h + (r * kNet + x) * 3;
+      unsigned char* d = s_h + (r * OW + x) * 3;
       d[0] = (unsigned char)min(max(a0 >> kPrecisionBits, 0), 255);
       d[1] = (unsigned char)min(max(a1 >> kPrecisionBits, 0), 255);
       d[2] = (unsigned char)min(max(a2 >> kPrecisionBits, 0), 255);
@@ -116,13 +118,13 @@ __global__ void __launch_bounds__(kNet) preprocess_kernel(const unsigned char* _
       int a0 = 1 << (kPrecisionBits - 1), a1 = a0, a2 = a0;
       for (int t = 0; t < yn; ++t) {
         const int k = ky[t];
-        const unsigned char* d = s_h + ((ymin + t) * kNet + x) * 3;
+        const unsigned char* d = s_h + ((ymin + t) * OW + x) * 3;
         a0 += d[0] * k; a1 += d[1] * k; a2 += d[2] * k;
       }
       const float v0 = (float)min(max(a0 >> kPrecisionBits, 0), 255);
       const float v1 = (float)min(max(a1 >> kPrecisionBits, 0), 255);
       const float v2 = (float)min(max(a2 >> kPrecisionBits, 0), 255);
-      reinterpret_cast<float4*>(out)[((long long)blockIdx.y * kNet + o) * kNet + x] =
+      reinterpret_cast<float4*>(out)[((long long)blockIdx.y * OH + o) * OW + x] =
           make_float4((v0 - m0) / s0, (v1 - m1) / s1, (v2 - m2) / s2, 0.f);
     }
     __syncthreads();
@@ -130,22 +132,23 @@ __global__ void __launch_bounds__(kNet) preprocess_kernel(const unsigned char* _
   }
 }
 
-// Lower entry (perspectivefields.py:223-236 called directly): images already resized, fp32 CHW [n,3,320,320].
-__global__ void __launch_bounds__(256) normalize_chw_kernel(const float* __restrict__ in, float* __restrict__ out, int n,
+// Lower entry (perspectivefields.py:223-236 called directly): images already resized, fp32 CHW [n,3,H,W] (the net size).
+__global__ void __launch_bounds__(256) normalize_chw_kernel(const float* __restrict__ in, float* __restrict__ out, int n, int H, int W,
                                                             float m0, float m1, float m2, float s0, float s1, float s2) {
-  const long long total = (long long)n * kNet * kNet;
+  const long long HW = (long long)H * W, total = (long long)n * HW;
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total) return;
-  const long long b = i / (kNet * kNet), p = i % (kNet * kNet);
-  const float* s = in + b * 3 * kNet * kNet + p;
-  reinterpret_cast<float4*>(out)[i] = make_float4((s[0] - m0) / s0, (s[kNet * kNet] - m1) / s1, (s[2 * kNet * kNet] - m2) / s2, 0.f);
+  const long long b = i / HW, p = i % HW;
+  const float* s = in + b * 3 * HW + p;
+  reinterpret_cast<float4*>(out)[i] = make_float4((s[0] - m0) / s0, (s[HW] - m1) / s1, (s[2 * HW] - m2) / s2, 0.f);
 }
 
 // =====================================================================================================
 // Post-process.  Reference: gravity_head.py:237-261, latitude_head.py:195-219, utils/utils.py:483-507.
-//   gravity : vec * (W/320, H/320) -> bilinear (align_corners=False, no antialias) to (H, W) -> F.normalize(dim=0)
+// The fields arrive at the net size SH x SW (DATALOADER.RESIZE, the heads' image_size; 320 x 320 in every shipped config):
+//   gravity : vec * (W/SW, H/SH) -> bilinear (align_corners=False, no antialias) to (H, W) -> F.normalize(dim=0)
 //   latitude: bilinear to (H, W) -> asin -> rad2deg          (regression)   |  bilinear of decoded degrees (classification)
-// ATen upsample_bilinear2d: scale = (float)320 / out; src = scale*(dst+0.5)-0.5, clamped at 0; i1 = i0 + (i0 < 319).
+// ATen upsample_bilinear2d: scale = (float)SH / out; src = scale*(dst+0.5)-0.5, clamped at 0; i1 = i0 + (i0 < SH - 1).
 struct PostImage {
   int H, W;
   long long g_off;  // float offset of this image's [2,H,W] block in the gravity_original blob
@@ -172,7 +175,7 @@ __device__ __forceinline__ float fast_asinf(float x) {
 }
 
 // Block = (band of kPostBand output rows, image).  Per group of kPostRows output rows the block first interpolates VERTICALLY:
-// for each of the 320 source columns it stores (gravity x * W/320, gravity y * H/320, latitude) blended between the two source
+// for each of the SW source columns it stores (gravity x * W/320, gravity y * H/320, latitude) blended between the two source
 // rows as ONE float4 in shared memory; then every thread produces 4 consecutive output pixels of one row from two 16-byte
 // shared-memory taps per pixel (per-column index / weight tables, built once per block), normalises the up-vector
 // (v * rsqrt(max(|v|^2, 1e-24)) == v / max(|v|, 1e-12)), applies asin + rad2deg and writes three 16-byte streaming stores.
@@ -180,32 +183,37 @@ __device__ __forceinline__ float fast_asinf(float x) {
 // its 12 B/pixel of stores.
 // The interpolation is evaluated as hx * (hy v00 + ly v10) + lx * (hy v01 + ly v11): ATen's bilinear kernel nests the two axes the
 // other way round (same weights, same products; the results differ by fp32 rounding only, ~1e-7 relative).
-constexpr int kPostRows = 4, kPostBand = 16, kPostThreads = 256, kPostMaxW = 3072;   // (static 20.6 KB + 8 B per column <= 48 KB)
+constexpr int kPostRows = 4, kPostBand = 16, kPostThreads = 256, kPostMaxW = 3072;
+// dynamic shared memory: the source-row buffer (kPostRows x (SW + 1) float4; 20.6 KB at SW = 320) + 8 B per output column
+inline int post_smem_bytes(int SW, int max_wp) { return kPostRows * (SW + 1) * 16 + max_wp * 8; }
+constexpr int kPostSmemMax = kPostRows * (kPreMaxW + 1) * 16 + kPostMaxW * 8;   // 65600 B
 __global__ void __launch_bounds__(kPostThreads) postprocess_kernel(const float* __restrict__ vec, const float* __restrict__ lat, const PostImage* __restrict__ imgs,
-                                                                   float* __restrict__ g_out, float* __restrict__ l_out, int lat_is_sin) {
-  __shared__ float4 s_v[kPostRows][kNet + 1];        // vertically interpolated source rows (+1: tap xa + 1 of the last column)
-  extern __shared__ __align__(16) unsigned char s_dyn[];   // per output column: int xa, float lx  (W entries each, W padded to 4)
+                                                                   float* __restrict__ g_out, float* __restrict__ l_out, int lat_is_sin, int SH, int SW) {
+  extern __shared__ __align__(16) unsigned char s_dyn[];
+  float4* s_v = reinterpret_cast<float4*>(s_dyn);    // [kPostRows][SW + 1] vertically interpolated source rows (+1: tap xa + 1 of the last column)
+  const int SW1 = SW + 1;
   const PostImage im = imgs[blockIdx.y];
   const int band0 = blockIdx.x * kPostBand;
   if (band0 >= im.H) return;
   const int W4 = (im.W + 3) >> 2, Wp = W4 * 4;
-  int* s_xa = reinterpret_cast<int*>(s_dyn);
-  float* s_lx = reinterpret_cast<float*>(s_dyn) + Wp;
+  int* s_xa = reinterpret_cast<int*>(s_v + kPostRows * SW1);   // per output column: int xa, float lx  (W entries each, W padded to 4)
+  float* s_lx = reinterpret_cast<float*>(s_xa) + Wp;
   const int tid = threadIdx.x;
-  const float sch = (float)kNet / (float)im.H, scw = (float)kNet / (float)im.W;
+  const float sch = (float)SH / (float)im.H, scw = (float)SW / (float)im.W;
   const bool tab = Wp <= kPostMaxW;       // wider images: indices / weights are recomputed per pixel instead
   for (int x = tid; tab && x < Wp; x += kPostThreads) {
     const int xc = min(x, im.W - 1);
     const float sx = fmaxf(scw * ((float)xc + 0.5f) - 0.5f, 0.f);
-    const int xa = min((int)sx, kNet - 1);
+    const int xa = min((int)sx, SW - 1);
     s_xa[x] = xa;
     s_lx[x] = sx - (float)xa;
   }
-  const float* v0 = vec + (long long)blockIdx.y * 2 * kNet * kNet;
-  const float* v1 = v0 + kNet * kNet;
-  const float* lp = lat + (long long)blockIdx.y * kNet * kNet;
-  // the reference scales the field before resampling: vec * [[W/320],[H/320]] (float32 tensor built from python doubles)
-  const float fx = (float)((double)im.W / (double)kNet), fy = (float)((double)im.H / (double)kNet);
+  const long long SHW = (long long)SH * SW;
+  const float* v0 = vec + (long long)blockIdx.y * 2 * SHW;
+  const float* v1 = v0 + SHW;
+  const float* lp = lat + (long long)blockIdx.y * SHW;
+  // the reference scales the field before resampling: vec * [[W/SW],[H/SH]] (float32 tensor built from python doubles)
+  const float fx = (float)((double)im.W / (double)SW), fy = (float)((double)im.H / (double)SH);
   const long long HW = (long long)im.H * im.W;
   const bool vec_ok = (im.W & 3) == 0 && (im.g_off & 3) == 0 && ((im.g_off + HW) & 3) == 0 && (im.l_off & 3) == 0;
   const int band1 = min(band0 + kPostBand, im.H);
@@ -213,18 +221,18 @@ __global__ void __launch_bounds__(kPostThreads) postprocess_kernel(const float* 
   const int g_start = tid % W4, r_start = tid / W4, g_step = kPostThreads % W4, r_step = kPostThreads / W4;
   for (int r0 = band0; r0 < band1; r0 += kPostRows) {
     __syncthreads();     // (the previous group's readers are done; the column tables are complete)
-    for (int i = tid; i < kPostRows * kNet; i += kPostThreads) {
-      const int rr = i / kNet, x = i - rr * kNet;
+    for (int i = tid; i < kPostRows * SW; i += kPostThreads) {
+      const int rr = i / SW, x = i - rr * SW;
       const int y = min(r0 + rr, im.H - 1);
       const float sy = fmaxf(sch * ((float)y + 0.5f) - 0.5f, 0.f);
-      const int y0 = min((int)sy, kNet - 1);
-      const int y1 = y0 + (y0 < kNet - 1);
+      const int y0 = min((int)sy, SH - 1);
+      const int y1 = y0 + (y0 < SH - 1);
       const float ly = sy - (float)y0, hy = 1.f - ly;
-      const int i0 = y0 * kNet + x, i1 = y1 * kNet + x;
+      const int i0 = y0 * SW + x, i1 = y1 * SW + x;
       const float4 t = make_float4(hy * (__ldg(v0 + i0) * fx) + ly * (__ldg(v0 + i1) * fx), hy * (__ldg(v1 + i0) * fy) + ly * (__ldg(v1 + i1) * fy),
                                    hy * __ldg(lp + i0) + ly * __ldg(lp + i1), 0.f);
-      s_v[rr][x] = t;
-      if (x == kNet - 1) s_v[rr][kNet] = t;      // tap xa + 1 of column 319 (its weight lx is 0 there)
+      s_v[rr * SW1 + x] = t;
+      if (x == SW - 1) s_v[rr * SW1 + SW] = t;      // tap xa + 1 of the last column (its weight lx is 0 there)
     }
     __syncthreads();
     const int rows = min(kPostRows, band1 - r0);
@@ -241,14 +249,14 @@ __global__ void __launch_bounds__(kPostThreads) postprocess_kernel(const float* 
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           const float sx = fmaxf(scw * ((float)min(x0 + j, im.W - 1) + 0.5f) - 0.5f, 0.f);
-          xa[j] = min((int)sx, kNet - 1);
+          xa[j] = min((int)sx, SW - 1);
           lx[j] = sx - (float)xa[j];
         }
       }
       float ogx[4], ogy[4], ol[4];
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        const float4 a = s_v[rr][xa[j]], b = s_v[rr][xa[j] + 1];
+        const float4 a = s_v[rr * SW1 + xa[j]], b = s_v[rr * SW1 + xa[j] + 1];
         const float hx = 1.f - lx[j];
         const float gx = hx * a.x + lx[j] * b.x;
         const float gy = hx * a.y + lx[j] * b.y;

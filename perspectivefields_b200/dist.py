@@ -19,7 +19,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-_NET = 320
+_NET = 320          # default working size (DATALOADER.RESIZE); a model built with ``resize`` passes its own net_hw
 _BLOBS = ("pred_gravity", "pred_latitude", "gravity_original", "latitude_original", "params")
 
 
@@ -34,10 +34,11 @@ def micro_batches(lo, hi, mb):
     return [(a, min(a + mb, hi)) for a in range(lo, hi, mb)] if hi > lo else []
 
 
-def _result_spec(variant, h, w):
+def _result_spec(variant, h, w, net_hw=(_NET, _NET)):
     """(key, shape) of every tensor in one image's result dict, in order (SURVEY.md section 8a)."""
     g, l = variant["gravity_classes"], variant["latitude_classes"]
-    spec = [("pred_gravity", (g, _NET, _NET)), ("pred_gravity_original", (2, h, w)), ("pred_latitude", (l, _NET, _NET)),
+    nh, nw = net_hw
+    spec = [("pred_gravity", (g, nh, nw)), ("pred_gravity_original", (2, h, w)), ("pred_latitude", (l, nh, nw)),
             ("pred_latitude_original", (h, w))]
     if variant["param_net"] == "ParamNet":
         spec += [(k, ()) for k in ("pred_roll", "pred_pitch", "pred_vfov", "pred_rel_focal", "pred_general_vfov", "pred_rel_cx", "pred_rel_cy")]
@@ -46,18 +47,21 @@ def _result_spec(variant, h, w):
     return spec
 
 
-def blob_numels(out_classes, sizes):
-    """Element counts of the five output blobs of a micro-batch whose images have the given (h, w) sizes."""
+def blob_numels(out_classes, sizes, net_hw=(_NET, _NET)):
+    """Element counts of the five output blobs of a micro-batch whose images have the given (h, w) sizes, for a model whose
+    working size is ``net_hw`` (``PerspectiveFields.net_size()``)."""
     g, l = out_classes
     m = len(sizes)
     hw = sum(h * w for h, w in sizes)
-    return {"pred_gravity": m * g * _NET * _NET, "pred_latitude": m * l * _NET * _NET, "gravity_original": 2 * hw, "latitude_original": hw,
+    nhw = net_hw[0] * net_hw[1]
+    return {"pred_gravity": m * g * nhw, "pred_latitude": m * l * nhw, "gravity_original": 2 * hw, "latitude_original": hw,
             "params": m * 8}
 
 
-def empty_raw(out_classes, sizes, device):
+def empty_raw(out_classes, sizes, device, net_hw=(_NET, _NET)):
     """Receive buffers with the layout ``PerspectiveFields.infer_raw`` produces for these image sizes."""
     g, l = out_classes
+    nh, nw = net_hw
     m = len(sizes)
     h = np.asarray([s[0] for s in sizes], np.int32)
     w = np.asarray([s[1] for s in sizes], np.int32)
@@ -65,8 +69,8 @@ def empty_raw(out_classes, sizes, device):
     g_off, l_off = np.zeros(m, np.int64), np.zeros(m, np.int64)
     np.cumsum(2 * hw[:-1], out=g_off[1:])
     np.cumsum(hw[:-1], out=l_off[1:])
-    return {"pred_gravity": torch.empty((m, g, _NET, _NET), dtype=torch.float32, device=device),
-            "pred_latitude": torch.empty((m, l, _NET, _NET), dtype=torch.float32, device=device),
+    return {"pred_gravity": torch.empty((m, g, nh, nw), dtype=torch.float32, device=device),
+            "pred_latitude": torch.empty((m, l, nh, nw), dtype=torch.float32, device=device),
             "gravity_original": torch.empty(int(2 * hw.sum()), dtype=torch.float32, device=device),
             "latitude_original": torch.empty(int(hw.sum()), dtype=torch.float32, device=device),
             "params": torch.empty((m, 8), dtype=torch.float32, device=device),
@@ -154,7 +158,8 @@ def inference_batch_sharded(model, img_bgr_list, gather_to=0, group=None, micro_
     225 KB-shared-memory CTA per SM) need every SM.
 
     ``model`` provides ``infer_raw(imgs) -> raw`` (the five output blobs of one micro-batch + host metadata),
-    ``assemble_raw(raw) -> list[dict]`` and ``out_classes()`` (``PerspectiveFields`` does)."""
+    ``assemble_raw(raw) -> list[dict]`` and ``out_classes()`` (``PerspectiveFields`` does), optionally ``net_size()`` (the working
+    size of ``pred_gravity`` / ``pred_latitude``; 320 x 320 when absent)."""
     if not dist.is_available() or not dist.is_initialized():
         return model.inference_batch(img_bgr_list)
     rank, world = dist.get_rank(group), dist.get_world_size(group)
@@ -172,6 +177,7 @@ def inference_batch_sharded(model, img_bgr_list, gather_to=0, group=None, micro_
         side.wait_stream(cur)
     sizes = _sizes(img_bgr_list)
     classes = model.out_classes()
+    net_hw = tuple(model.net_size()) if hasattr(model, "net_size") else (_NET, _NET)   # the blobs follow the model's working size
     my_mbs = micro_batches(lo, hi, micro_batch)
     rounds = max(len(micro_batches(a, b, micro_batch)) for a, b in bounds)
     results = [None] * n
@@ -211,7 +217,7 @@ def inference_batch_sharded(model, img_bgr_list, gather_to=0, group=None, micro_
                     if r == rank or k >= len(mbs):
                         continue
                     a, b = mbs[k]
-                    recv = empty_raw(classes, sizes[a:b], device)
+                    recv = empty_raw(classes, sizes[a:b], device, net_hw)
                     for key in _BLOBS:
                         bufs.append(recv[key])
                         peers.append(r)

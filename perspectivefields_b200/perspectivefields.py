@@ -18,13 +18,31 @@ from .checkpoint import checkpoint_schema, default_state, load_zoo_checkpoint
 from .variants import PIXEL_MEAN, PIXEL_STD, RESIZE, VARIANTS, make_cfg, model_zoo
 from .weights import repack
 
-_NET = RESIZE[0]
+
+def check_resize(resize):
+    """``PerspectiveFields(resize=...)`` -> the working size (H, W).  ``None``: the yaml's DATALOADER.RESIZE ([320, 320]).  H and W
+    (the reference's [Height, Width] order) must be multiples of 32 in [64, 640] with (H/32) * (W/32) <= 256: the attention key
+    count of every MiT stage (100 at 320 x 320); 64 keeps the smallest head level at 2 x 2 or more."""
+    if resize is None:
+        return tuple(int(x) for x in RESIZE)
+    try:
+        h, w = resize
+    except (TypeError, ValueError):
+        raise ValueError(f"resize must be None or (height, width), got {resize!r}") from None
+    if not all(isinstance(x, (int, np.integer)) and not isinstance(x, bool) for x in (h, w)):
+        raise ValueError(f"resize must hold two integers, got {resize!r}")
+    h, w = int(h), int(w)
+    if h % 32 or w % 32 or not (64 <= h <= 640 and 64 <= w <= 640):
+        raise ValueError(f"resize {(h, w)}: height and width must be multiples of 32 in [64, 640]")
+    if (h // 32) * (w // 32) > 256:
+        raise ValueError(f"resize {(h, w)}: (H/32) * (W/32) = {(h // 32) * (w // 32)} attention keys, at most 256 are supported")
+    return h, w
 
 
 class _Engine:
     """One libpf_b200 handle + its device-resident repacked weights and scratch, for one CUDA device."""
 
-    def __init__(self, device, version, ref_state):
+    def __init__(self, device, version, ref_state, net_hw=RESIZE):
         self.L = _native.lib()
         self.device = device
         cfg = VARIANTS[version]
@@ -35,8 +53,12 @@ class _Engine:
         desc.param_input_size = cfg["input_size"]
         desc.pixel_mean[:] = PIXEL_MEAN
         desc.pixel_std[:] = PIXEL_STD
+        self.net_h, self.net_w = int(net_hw[0]), int(net_hw[1])
         self.handle = ctypes.c_void_p()
-        _native.check(self.L.pf_create(device.index, ctypes.byref(desc), ctypes.byref(self.handle)))
+        if (self.net_h, self.net_w) == tuple(RESIZE):
+            _native.check(self.L.pf_create(device.index, ctypes.byref(desc), ctypes.byref(self.handle)))
+        else:
+            _native.check(self.L.pf_create_sized(device.index, ctypes.byref(desc), self.net_h, self.net_w, ctypes.byref(self.handle)))
         self.tensors = {}
         for name, t in repack(ref_state, cfg).items():
             d = t.to(device)
@@ -128,8 +150,8 @@ class _Engine:
         cur = torch.cuda.current_stream(dev)
         gc_, lc_ = (2, 1) if self.decode_only else (self.gravity_classes, self.latitude_classes)
         out = {
-            "pred_gravity": torch.empty((n, gc_, _NET, _NET), dtype=torch.float32, device=dev),
-            "pred_latitude": torch.empty((n, lc_, _NET, _NET), dtype=torch.float32, device=dev),
+            "pred_gravity": torch.empty((n, gc_, self.net_h, self.net_w), dtype=torch.float32, device=dev),
+            "pred_latitude": torch.empty((n, lc_, self.net_h, self.net_w), dtype=torch.float32, device=dev),
             "gravity_original": torch.empty(int(2 * hw.sum()), dtype=torch.float32, device=dev),
             "latitude_original": torch.empty(int(hw.sum()), dtype=torch.float32, device=dev),
             "params": torch.empty((n, 8), dtype=torch.float32, device=dev),
@@ -198,7 +220,7 @@ class ResizeTransform:
 
 
 class PerspectiveFields(nn.Module):
-    def __init__(self, version="Paramnet-360Cities-edina-centered", logits=True, precision="fp32"):
+    def __init__(self, version="Paramnet-360Cities-edina-centered", logits=True, precision="fp32", resize=None):
         """``logits=False`` (classification variant only, SURVEY.md 8f-3; NOT the reference's behaviour): ``pred_gravity`` /
         ``pred_latitude`` hold the decoded fields ([2,320,320] up-vectors, [1,320,320] degrees) instead of the 73 / 180 raw logits,
         which are then never written (engine option "decode_only"); the ``*_original`` entries are unchanged.
@@ -207,12 +229,20 @@ class PerspectiveFields(nn.Module):
         ``"bf16"`` (opt-in, NOT the reference's numerics) runs every tensor-core product as one bf16 MMA on bf16-rounded operands
         with fp32 accumulation, as ``torch.autocast(dtype=torch.bfloat16)`` would; normalisation, softmax, depthwise convolutions
         and the prediction tails stay fp32.  Outputs then differ from fp32 by about 1e-2 relative (DESIGN.md section 3 lists the
-        measured error per output).  It is the engine option "bf16" and survives ``.to()`` / ``load_state_dict``."""
+        measured error per output).  It is the engine option "bf16" and survives ``.to()`` / ``load_state_dict``.
+
+        ``resize``: the working size ``(H, W)`` the network runs at, in the reference's ``DATALOADER.RESIZE = [Height, Width]``
+        order; ``None`` keeps the yaml's ``[320, 320]``.  H and W must be multiples of 32 in [64, 640] with (H/32) * (W/32) <= 256
+        (``ValueError`` otherwise, before any GPU work).  ``cfg.DATALOADER.RESIZE``, ``aug`` and the ``[C, H, W]`` fields
+        ``pred_gravity`` / ``pred_latitude`` follow it; ``forward`` expects ``[3, H, W]`` images.  Like ``precision`` it survives
+        ``.to()`` / ``load_state_dict``."""
         super().__init__()
         zoo = model_zoo[version]  # KeyError for unknown versions, like the reference (perspectivefields.py:127)
         self.version = version
         self.param_on = zoo["param"]
+        self._net_hw = check_resize(resize)
         self.cfg = make_cfg(version)
+        self.cfg.DATALOADER["RESIZE"] = list(self._net_hw)
         self._variant = VARIANTS[version]
         self.register_buffer("pixel_mean", torch.tensor(PIXEL_MEAN).view(-1, 1, 1), False)
         self.register_buffer("pixel_std", torch.tensor(PIXEL_STD).view(-1, 1, 1), False)
@@ -220,7 +250,7 @@ class PerspectiveFields(nn.Module):
         self.freeze = self.cfg.MODEL.FREEZE
         self.debug_on = self.cfg.DEBUG_ON
         self.input_format = self.cfg.INPUT.FORMAT
-        self.aug = ResizeTransform(RESIZE[0], RESIZE[1])
+        self.aug = ResizeTransform(self._net_hw[0], self._net_hw[1])
         self._schema = dict(checkpoint_schema(version))
         self._ref_state = default_state(version)   # reference-layout weights, host side
         self._engine = None
@@ -310,7 +340,7 @@ class PerspectiveFields(nn.Module):
         if self._engine is None or self._engine.device != dev:
             self._drop_engine()
             with torch.cuda.device(dev):
-                eng = _Engine(dev, self.version, self._ref_state)
+                eng = _Engine(dev, self.version, self._ref_state, self._net_hw)
             eng.gravity_classes = self._variant["gravity_classes"]
             eng.latitude_classes = self._variant["latitude_classes"]
             for k, v in self._options.items():
@@ -358,7 +388,7 @@ class PerspectiveFields(nn.Module):
     @torch.no_grad()
     def infer_raw(self, img_bgr_list):
         """``inference_batch`` up to (not including) the per-image views: returns the engine's batch outputs
-        (``pred_gravity [n,Cg,320,320]``, ``pred_latitude``, flat ``gravity_original`` / ``latitude_original`` blobs, ``params [n,8]``)
+        (``pred_gravity [n,Cg,H,W]`` at the working size, ``pred_latitude``, flat ``gravity_original`` / ``latitude_original`` blobs, ``params [n,8]``)
         plus the host-side offsets / sizes ``assemble_raw`` needs.  uint8 images only."""
         imgs = []
         for im in img_bgr_list:
@@ -375,6 +405,10 @@ class PerspectiveFields(nn.Module):
 
     def assemble_raw(self, raw):
         return self._assemble(raw)
+
+    def net_size(self):
+        """The working size (H, W): ``cfg.DATALOADER.RESIZE``, the spatial shape of ``pred_gravity`` / ``pred_latitude``."""
+        return self._net_hw
 
     def out_classes(self):
         """Channel counts of ``pred_gravity`` / ``pred_latitude`` as returned (2 / 1 in "decode_only" mode)."""
@@ -427,14 +461,14 @@ class PerspectiveFields(nn.Module):
 
     @torch.no_grad()
     def forward(self, batched_inputs):
-        """perspectivefields.py:223-272: ``[{"image": float32 [3,320,320] (resized, un-normalised), "height", "width"}]``."""
+        """perspectivefields.py:223-272: ``[{"image": float32 [3,H,W] (resized to the working size, un-normalised), "height", "width"}]``."""
         if any(k in batched_inputs[0] for k in ("gt_gravity", "gt_latitude")) and self.training:
             raise RuntimeError("training is not supported")
         eng = self._get_engine()
         with torch.cuda.device(eng.device):
             chw = torch.stack([x["image"].to(eng.device, torch.float32) for x in batched_inputs]).contiguous()
-            if tuple(chw.shape[1:]) != (3, _NET, _NET):
-                raise ValueError("forward expects images already resized to [3, 320, 320]")
+            if tuple(chw.shape[1:]) != (3,) + self._net_hw:
+                raise ValueError("forward expects images already resized to [3, %d, %d]" % self._net_hw)
             out = eng.forward(len(batched_inputs), [int(x["height"]) for x in batched_inputs],
                               [int(x["width"]) for x in batched_inputs], chw=chw)
         return self._assemble(out)
