@@ -150,6 +150,32 @@ typedef struct pf_camera {
 /* cams: HOST array of n descriptors; up / lat: DEVICE blobs (either may be NULL to skip that field). */
 int pf_camera_fields(int device, const pf_camera* cams, int n, float* up, float* lat, void* stream);
 
+/* ---- views of a panorama and their ground-truth fields -------------------------------------------------------------------
+ * Replaces PanoCam.crop_distortion (perspective2d/utils/panocam.py:559-752) for a batch of views of ONE equirectangular panorama:
+ * each view is a perspective (xi = 0) or Unified Spherical Model (xi > 0) camera of size H x W, focal length f (pixels) and
+ * rotation rot_az * rot_roll^T * rot_el (degrees).  Geometry in float64 in the reference's order of operations, float32 fields.
+ * The crop is a bilinear sample of the panorama (columns wrap, rows clamp, float64 weights, truncated to uint8; DESIGN.md
+ * section 5), 0 outside the catadioptric disk when xi > 1 and f < fmin.  One launch per 12 views; no engine handle, no
+ * synchronisation: offset / status are written on the device. */
+typedef struct pf_pano_view {
+  int32_t height, width;        /* H, W of the view */
+  double f, xi;                 /* focal length in pixels (> 0), mirror parameter */
+  double az, el, roll;          /* degrees */
+  int64_t im_offset;            /* byte offset of this view's [H,W,3] crop in `im` (the layout of pf_batch.images_u8) */
+  int64_t field_offset;         /* float offset of this view's [H,W] blocks in ntheta / nphi / lat; its [H,W,2] blocks in up / xy
+                                   start at 2 * field_offset */
+} pf_pano_view;
+/* pano: DEVICE uint8 [pano_h, pano_w, 3] HWC (pano_h, pano_w >= 2); views: HOST array of n descriptors.  Outputs, DEVICE, each
+ * may be NULL to skip it (at least one must be given):
+ *   im uint8 crops (RGB order of the panorama);  ntheta, nphi, lat float32 [H,W] radians (lat == nphi);
+ *   up float32 [H,W,2] normalised up-vector field;  xy float32 [H,W,2] (x, y) panorama pixel of every view pixel;
+ *   offset double [n]: horizon row at column W / 2 (nan when nphi does not change sign there);
+ *   status int32 [n]: 0 one zero crossing or none, 1 several (the reference prints a WARNING and uses the first), 2 one of the
+ *   reference's assertions fails (e.g. an upside-down camera; offset is nan).
+ * Every argument is checked before anything is launched (PF_ERR_ARG). */
+int pf_pano_views(int device, const uint8_t* pano, int pano_h, int pano_w, const pf_pano_view* views, int n, uint8_t* im, float* ntheta,
+                  float* nphi, float* up, float* lat, float* xy, double* offset, int32_t* status, void* stream);
+
 /* ---- multi-GPU gather of results (SURVEY.md 8e: one process per GPU; NCCL point-to-point over NVLink) ---------------------
  * inference_batch shards its list over the ranks; the per-image results live on each rank's device and are gathered to ONE
  * rank with grouped ncclSend / ncclRecv enqueued on the caller's stream (so that the gather of micro-batch k overlaps the

@@ -25,6 +25,7 @@
 #include "attention_mma.cuh"
 #include "layers.cuh"
 #include "prepost.cuh"
+#include "pano.cuh"
 #include "comm.cuh"
 #include "jpeg.cuh"
 
@@ -1506,6 +1507,62 @@ int pf_camera_fields(int device, const pf_camera* cams, int n, float* up, float*
     }
     const dim3 grid((unsigned)cdivl(max_q, 256), (unsigned)m);
     LAUNCHED((camera_fields_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(b, up, lat), cudaGetLastError()));
+  }
+  return PF_OK;
+}
+
+// PanoCam.crop_distortion (utils/panocam.py:559-752) for n views of one panorama: the host builds each view's rotation matrices
+// (:617-655), minimal focal length and disk (:592-594, :696-705) in float64 once; one launch per kPanoChunk views.
+int pf_pano_views(int device, const uint8_t* pano, int pano_h, int pano_w, const pf_pano_view* views, int n, uint8_t* im, float* ntheta,
+                  float* nphi, float* up, float* lat, float* xy, double* offset, int32_t* status, void* stream) {
+  if (!pano || !views || n < 1) return fail(PF_ERR_ARG, "pf_pano_views: null panorama / views or n < 1");
+  if (pano_h < 2 || pano_w < 2) return fail(PF_ERR_ARG, "pf_pano_views: panorama of %dx%d (needs at least 2x2)", pano_h, pano_w);
+  if (!im && !ntheta && !nphi && !up && !lat && !xy && !offset && !status) return fail(PF_ERR_ARG, "pf_pano_views: no output");
+  for (int i = 0; i < n; ++i) {
+    const pf_pano_view& c = views[i];
+    if (c.height < 1 || c.width < 1) return fail(PF_ERR_ARG, "pf_pano_views: view %d has size %dx%d", i, c.height, c.width);
+    if (!std::isfinite(c.f) || !(c.f > 0.0) || !std::isfinite(c.xi) || !std::isfinite(c.az) || !std::isfinite(c.el) || !std::isfinite(c.roll))
+      return fail(PF_ERR_ARG, "pf_pano_views: view %d: f must be finite and > 0, xi and the angles finite (f %g, xi %g)", i, c.f, c.xi);
+    if (c.im_offset < 0 || c.field_offset < 0) return fail(PF_ERR_ARG, "pf_pano_views: view %d has a negative offset", i);
+  }
+  CU(cudaSetDevice(device));
+  PanoMap m{};
+  m.Hp = pano_h; m.Wp = pano_w;
+  m.ax = (M_PI - -M_PI) / ((pano_w - 1.0) - 0);   // :680-687, python's own expressions
+  m.bx = M_PI - m.ax * (pano_w - 1.0);
+  m.iax = 1.0 / m.ax;
+  m.ay = (-M_PI / 2.0 - M_PI / 2.0) / ((pano_h - 1.0) - 0);
+  m.by = M_PI / 2.0 - m.ay * 0;
+  m.iay = 1.0 / m.ay;
+  auto rad = [](double deg) { return deg * M_PI / 180; };
+  for (int i0 = 0; i0 < n; i0 += kPanoChunk) {
+    const int cnt = n - i0 < kPanoChunk ? n - i0 : kPanoChunk;
+    PanoBatch b{};
+    long long max_px = 1;
+    for (int i = 0; i < cnt; ++i) {
+      const pf_pano_view& c = views[i0 + i];
+      PanoView& o = b.v[i];
+      o.H = c.height; o.W = c.width;
+      o.f = c.f; o.xi = c.xi; o.one_m_xi2 = 1 - c.xi * c.xi;
+      o.u0 = c.width / 2.0; o.v0 = c.height / 2.0;
+      const double ce = cos(rad(c.el)), se = sin(rad(c.el)), ca = cos(rad(c.az)), sa = sin(rad(c.az)), cr = cos(rad(c.roll)), sr = sin(rad(c.roll));
+      const double rel[9] = {1.0, 0.0, 0.0, 0.0, ce, -se, 0.0, se, ce};
+      const double raz[9] = {ca, 0.0, sa, 0.0, 1.0, 0.0, -sa, 0.0, ca};
+      const double rroll[9] = {cr, -sr, 0.0, sr, cr, 0.0, 0.0, 0.0, 1.0};
+      memcpy(o.rel, rel, sizeof rel); memcpy(o.raz, raz, sizeof raz); memcpy(o.rroll, rroll, sizeof rroll);
+      // minfocal(u0, v0, xi, 1, 1) (:64-70): NaN unless xi > 1, and f < NaN is false
+      const double fmin = sqrt(-(1 - c.xi * c.xi) * ((1 - o.u0) * (1 - o.u0) + (1 - o.v0) * (1 - o.v0))) * 1.0001;
+      o.masked = c.f < fmin;
+      const double r = sqrt(-(c.f * c.f) / (1 - c.xi * c.xi));   // diskradius (:18-19)
+      o.r2 = r * r;
+      o.ci0 = nearbyint(c.height / 2.0); o.ci1 = nearbyint(c.width / 2.0);   // np.round: half to even (the default rounding mode)
+      o.im_off = c.im_offset; o.fld_off = c.field_offset;
+      const long long px = (long long)c.height * c.width;
+      if (px > max_px) max_px = px;
+    }
+    const dim3 grid((unsigned)cdivl(max_px, (long long)kPanoThreads * kPanoPix) + 1, (unsigned)cnt);
+    LAUNCHED((pano_views_kernel<<<grid, kPanoThreads, 0, (cudaStream_t)stream>>>(b, m, pano, im, ntheta, nphi, up, lat, xy, offset, status, i0),
+              cudaGetLastError()));
   }
   return PF_OK;
 }

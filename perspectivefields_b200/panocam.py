@@ -3,12 +3,17 @@ inference path): drop-in for the two static methods of the reference's ``perspec
 ParamNet's output into an up-vector field and a latitude map (utils/panocam.py:451-556; called from
 utils/utils.py:367-385 and demo/demo.py:69-78).
 
+Also ``PanoCam.crop_distortion`` (utils/panocam.py:559-752, the reference's notebooks/camera2perspective.ipynb workflow): a
+perspective or Unified Spherical Model view cropped from an equirectangular panorama with its ground-truth fields, and its batched
+form ``crop_distortion_views``, whose crops can go straight into ``PerspectiveFields.inference_batch`` on the device.
+
 Same names, argument order and meaning as the reference.  Differences: results are float32 CUDA tensors (the reference returns
 float64 numpy arrays), and ``camera_fields`` evaluates a whole batch (images may differ in size) in one launch per 24 images.
 There is no CPU path: the functions raise when the CUDA library or a CUDA device is missing.
 """
 import ctypes
 import math
+import os
 
 import numpy as np
 import torch
@@ -71,8 +76,136 @@ def camera_fields(focal_rel, heights, widths, elevation, roll, cx_rel, cy_rel, d
     return ups, lats
 
 
+PANO_OUTPUTS = ("ntheta", "nphi", "up", "lat", "xy_map")
+
+
+def _real(x, name):
+    if isinstance(x, (bool, np.bool_)) or not isinstance(x, (int, float, np.integer, np.floating)) or not math.isfinite(float(x)):
+        raise ValueError(f"{name} must be a finite real number, got {x!r}")
+    return float(x)
+
+
+def _size(x, name):
+    if isinstance(x, (bool, np.bool_)) or not isinstance(x, (int, np.integer)) or int(x) < 1:
+        raise ValueError(f"{name} must be a positive integer, got {x!r}")
+    return int(x)
+
+
+def _check_view(view, i):
+    """(f, xi, H, W, az, el, roll) -- crop_distortion's argument order -- or a dict with those keys -> checked tuple."""
+    keys = ("f", "xi", "H", "W", "az", "el", "roll")
+    if isinstance(view, dict):
+        missing = [k for k in keys if k not in view]
+        if missing:
+            raise ValueError(f"view {i}: missing {missing}")
+        view = [view[k] for k in keys]
+    view = tuple(view)
+    if len(view) != 7:
+        raise ValueError(f"view {i}: expected (f, xi, H, W, az, el, roll), got {len(view)} values")
+    f, xi, h, w, az, el, roll = view
+    f = _real(f, f"view {i}: f")
+    if f <= 0:
+        raise ValueError(f"view {i}: f must be > 0, got {f}")
+    return (f, _real(xi, f"view {i}: xi"), _size(h, f"view {i}: H"), _size(w, f"view {i}: W"), _real(az, f"view {i}: az"),
+            _real(el, f"view {i}: el"), _real(roll, f"view {i}: roll"))
+
+
+def _check_panorama(image360):
+    """numpy / torch uint8 [Hp, Wp, 3] or a path (read with Pillow as RGB, what imageio.imread returns for an 8-bit file) ->
+    the array or tensor, checked; no GPU work."""
+    if isinstance(image360, (str, os.PathLike)):
+        from PIL import Image
+        with Image.open(image360) as im:
+            image360 = np.array(im.convert("RGB"))
+    if isinstance(image360, torch.Tensor):
+        if image360.dtype != torch.uint8:
+            raise TypeError(f"the panorama must be uint8, got {image360.dtype}")
+        shape = tuple(image360.shape)
+    else:
+        image360 = np.asarray(image360)
+        if image360.dtype != np.uint8:
+            raise TypeError(f"the panorama must be uint8, got {image360.dtype}")
+        shape = image360.shape
+    if len(shape) != 3 or shape[2] != 3:
+        raise TypeError(f"the panorama must be [H, W, 3], got {list(shape)}")
+    if shape[0] < 2 or shape[1] < 2:
+        raise ValueError(f"the panorama must be at least 2 x 2, got {shape[0]} x {shape[1]}")
+    return image360
+
+
+def crop_distortion_views(image360, views, outputs=("up", "lat"), device=None):
+    """Batched ``PanoCam.crop_distortion`` (utils/panocam.py:559-752): many views of ONE panorama, one upload, one launch per 12 views,
+    no synchronisation.  ``views``: sequence of ``(f, xi, H, W, az, el, roll)`` (or dicts with those keys; sizes may differ);
+    ``outputs``: any of ``ntheta, nphi, up, lat, xy_map``.  Returns a dict: ``im`` (list of uint8 [H, W, 3] views into one device
+    blob, the panorama's channel order), one list of float32 tensors per selected output ([H, W] radians or [H, W, 2]), ``offset``
+    (float64 [n], the horizon row at column W // 2, nan without a zero crossing) and ``status`` (int32 [n]: 0 fine, 1 several zero
+    crossings (the reference warns), 2 the reference's assertions fail) as device tensors."""
+    outputs = tuple(outputs)
+    bad = [o for o in outputs if o not in PANO_OUTPUTS]
+    if bad:
+        raise ValueError(f"unknown outputs {bad}; choose from {PANO_OUTPUTS}")
+    vs = [_check_view(v, i) for i, v in enumerate(views)]
+    if not vs:
+        raise ValueError("no views")
+    pano = _check_panorama(image360)
+    if not torch.cuda.is_available():
+        raise RuntimeError("perspectivefields_b200.panocam needs a CUDA device (there is no CPU path)")
+    L = _native.lib()
+    if isinstance(pano, torch.Tensor) and pano.is_cuda:
+        if device is not None and torch.device(device) != pano.device:
+            raise ValueError(f"the panorama is on {pano.device}, not on {device}")
+        dev = pano.device
+    else:
+        dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        if dev.type != "cuda":
+            raise RuntimeError("perspectivefields_b200.panocam needs a CUDA device (there is no CPU path)")
+        if dev.index is None:
+            dev = torch.device("cuda", torch.cuda.current_device())
+    n = len(vs)
+    descs = (_native.pf_pano_view * n)()
+    im_off = fld_off = 0
+    for i, (f, xi, h, w, az, el, roll) in enumerate(vs):
+        descs[i] = _native.pf_pano_view(h, w, f, xi, az, el, roll, im_off, fld_off)
+        im_off += (3 * h * w + 15) // 16 * 16          # 16-byte aligned crops and 4-float aligned fields: full-width vector stores
+        fld_off += (h * w + 3) // 4 * 4
+    with torch.cuda.device(dev):
+        src = torch.as_tensor(pano).to(dev).contiguous()
+        im = torch.empty(im_off, dtype=torch.uint8, device=dev)
+        blobs = {o: torch.empty((2 if o in ("up", "xy_map") else 1) * fld_off, dtype=torch.float32, device=dev) for o in outputs}
+        offset = torch.empty(n, dtype=torch.float64, device=dev)
+        status = torch.empty(n, dtype=torch.int32, device=dev)
+        ptr = lambda o: blobs[o].data_ptr() if o in blobs else None
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        _native.check(L.pf_pano_views(dev.index, src.data_ptr(), src.shape[0], src.shape[1], descs, n, im.data_ptr(), ptr("ntheta"),
+                                      ptr("nphi"), ptr("up"), ptr("lat"), ptr("xy_map"), offset.data_ptr(), status.data_ptr(), stream))
+    out = {"im": [im[d.im_offset:d.im_offset + 3 * d.height * d.width].view(d.height, d.width, 3) for d in descs]}
+    for o in outputs:
+        c = 2 if o in ("up", "xy_map") else 1
+        out[o] = [blobs[o][c * d.field_offset:c * (d.field_offset + d.height * d.width)].view((d.height, d.width, 2) if c == 2 else (d.height, d.width))
+                  for d in descs]
+    out["offset"], out["status"] = offset, status
+    return out
+
+
 class PanoCam:
-    """The two field-synthesis static methods of ``perspective2d.utils.panocam.PanoCam`` (same signatures)."""
+    """The field-synthesis static methods of ``perspective2d.utils.panocam.PanoCam`` (same signatures)."""
+
+    @staticmethod
+    def crop_distortion(image360, f, xi, H, W, az, el, roll, device=None):
+        """utils/panocam.py:559-752 -> (im, ntheta, nphi, offset, up, lat, xy_map): CUDA tensors (uint8 [H, W, 3]; float32 [H, W]
+        radians; float32 [H, W, 2]) and ``offset`` as a Python float (nan when the horizon does not cross column W // 2).
+        ``image360``: numpy / CUDA uint8 [Hp, Wp, 3] or a path.  Prints the reference's WARNING when the horizon column crosses zero
+        several times and raises AssertionError where the reference's assertions fail (e.g. an upside-down camera).  This call
+        synchronises (for the offset); ``crop_distortion_views`` does not."""
+        out = crop_distortion_views(image360, [(f, xi, H, W, az, el, roll)], PANO_OUTPUTS, device)
+        status = int(out["status"][0].item())
+        if status == 2:
+            raise AssertionError("crop_distortion: the horizon column crosses zero from below (e.g. an upside-down camera)")
+        nphi = out["nphi"][0]
+        if status == 1:
+            s = torch.sign(nphi[:, int(W) // 2])
+            print("WARNING | Number of zero crossings:", int((s[1:] != s[:-1]).sum().item()))
+        return (out["im"][0], out["ntheta"][0], nphi, float(out["offset"][0].item()), out["up"][0], out["lat"][0], out["xy_map"][0])
 
     @staticmethod
     def get_up_general(focal_rel, im_w, im_h, elevation, roll, cx_rel, cy_rel, device=None):

@@ -359,7 +359,16 @@ class PerspectiveFields(nn.Module):
         """perspectivefields.py:207-221.  uint8 (H, W, 3) images take the fused path (one packed upload, Pillow-exact resize +
         normalise in one kernel); a list containing any other dtype takes the reference's float branch for ALL its members
         (``ResizeTransform.apply_image`` -> non-antialiased ``F.interpolate``, perspectivefields.py:47-66, on the GPU) and then
-        the ``forward`` entry."""
+        the ``forward`` entry.
+
+        CUDA uint8 [H, W, 3] tensors on the model's device (e.g. ``panocam.crop_distortion_views`` crops) take the same fused path
+        without leaving the device: one device-to-device pack into a blob, then the same engine call; the results are identical
+        to those of the same images passed as numpy arrays.  A list must not mix CUDA tensors with host images (TypeError)."""
+        on_dev = [isinstance(im, torch.Tensor) and im.is_cuda for im in img_bgr_list]
+        if any(on_dev):
+            if not all(on_dev):
+                raise TypeError("inference_batch: the list mixes CUDA tensors and host images; pass one kind per call")
+            return self._inference_batch_device(img_bgr_list)
         imgs = []
         all_u8 = True
         for im in img_bgr_list:
@@ -381,6 +390,27 @@ class PerspectiveFields(nn.Module):
                     inputs.append({"image": torch.as_tensor(r.astype("float32").transpose(2, 0, 1)), "height": im.shape[0], "width": im.shape[1]})
                 return self.forward(inputs)
             blob, offsets = eng.stage_images(imgs)
+            out = eng.forward(len(imgs), [im.shape[0] for im in imgs], [im.shape[1] for im in imgs], blob=blob, offsets=offsets)
+        return self._assemble(out)
+
+    def _inference_batch_device(self, imgs):
+        dev = self.device
+        if dev.type != "cuda":
+            raise RuntimeError("perspectivefields_b200 has no CPU path: move the model to an H100 with .cuda() first")
+        if dev.index is None:
+            dev = torch.device("cuda", torch.cuda.current_device())
+        for im in imgs:
+            if im.dtype != torch.uint8 or im.ndim != 3 or im.shape[2] != 3:
+                raise TypeError("inference on CUDA tensors expects uint8 (H, W, 3) images; got %s %s" % (im.dtype, tuple(im.shape)))
+            if im.device != dev:
+                raise ValueError(f"image on {im.device}, the model is on {dev}")
+        eng = self._get_engine()
+        with torch.cuda.device(eng.device):
+            if self.input_format == "RGB":
+                imgs = [im.flip(2) for im in imgs]
+            blob = torch.cat([im.reshape(-1) for im in imgs])      # one device-to-device pack, on the current stream
+            offsets = np.zeros(len(imgs), np.int64)
+            np.cumsum(np.array([im.numel() for im in imgs[:-1]], np.int64), out=offsets[1:])
             out = eng.forward(len(imgs), [im.shape[0] for im in imgs], [im.shape[1] for im in imgs], blob=blob, offsets=offsets)
         return self._assemble(out)
 
