@@ -149,6 +149,11 @@ typedef struct pf_camera {
 } pf_camera;
 /* cams: HOST array of n descriptors; up / lat: DEVICE blobs (either may be NULL to skip that field). */
 int pf_camera_fields(int device, const pf_camera* cams, int n, float* up, float* lat, void* stream);
+/* The same, where vp (HOST [n][2] or NULL) may give image i a point (vp[2i], vp[2i+1]) in pixel-centre coordinates (pixel
+ * (i, j) at (j + .5, i + .5)) that its up field points to instead of the one its elevation and roll imply: PanoCam.get_up
+ * (panocam.py:385-448) at elevation 0, whose vanishing point lies 1e8 px away (:293-300).  NaN pairs keep the camera's own.
+ * pf_camera_fields(..) = pf_camera_fields_vp(.., NULL, ..). */
+int pf_camera_fields_vp(int device, const pf_camera* cams, const double* vp, int n, float* up, float* lat, void* stream);
 
 /* ---- views of a panorama and their ground-truth fields -------------------------------------------------------------------
  * Replaces PanoCam.crop_distortion (perspective2d/utils/panocam.py:559-752) for a batch of views of ONE equirectangular panorama:
@@ -175,6 +180,29 @@ typedef struct pf_pano_view {
  * Every argument is checked before anything is launched (PF_ERR_ARG). */
 int pf_pano_views(int device, const uint8_t* pano, int pano_h, int pano_w, const pf_pano_view* views, int n, uint8_t* im, float* ntheta,
                   float* nphi, float* up, float* lat, float* xy, double* offset, int32_t* status, void* stream);
+
+/* ---- perspective-field overlays (draw_perspective_fields / draw_up_field / draw_latitude_field, utils/utils.py:165-430) -----
+ * Draws the latitude contours (18 filled bands and 19 lines of linspace(-pi/2, pi/2, 19), seismic colours) and the up-vector
+ * arrows (quiver on the lattice arange(0, W, W // density) x arange(0, H, H // density), length up * (sqrt(W^2 + H^2) //
+ * arrow_inv_len)) over an RGB image, 4 x 4 samples per pixel, by the rule of DESIGN.md section 1 (parity with matplotlib
+ * unpinned).  Order: fill, arrows, lines.  One launch per 24 canvases; no engine handle, no synchronisation. */
+typedef struct pf_draw_canvas {
+  int32_t height, width;        /* H, W of the canvas (H * W < 2^31) */
+  int64_t img_offset;           /* byte offset of the input uint8 [H,W,3] RGB canvas in `img` */
+  int64_t out_offset;           /* byte offset of the output [H,W,3] in `out` (may be the input itself; no partial overlap) */
+  int64_t lat_offset;           /* float offset of the [H,W] latitude map (radians, row-major) in `lat`; -1 when draw_lat is 0 */
+  int64_t up_offset;            /* float offset of the up field's element (0, 0, x) in `up`; -1 when draw_up is 0 */
+  int64_t up_stride[3];         /* element strides (>= 0) of the up field: row, column, component ([2,H,W]: W, 1, H*W;  [H,W,2]: 2W, 2, 1) */
+  int32_t density;              /* arrows every W // density columns and H // density rows (both >= 1) */
+  int32_t arrow_inv_len;        /* arrow length = up * (sqrt(W^2 + H^2) // arrow_inv_len), >= 1 */
+  float arrow_rgb[3];           /* arrow colour, [0, 1] */
+  float alpha_fill, alpha_line; /* contourf / contour alpha, [0, 1] */
+  int32_t draw_lat, draw_up;    /* 0 / 1: draw the latitude fill and lines / the arrows */
+} pf_draw_canvas;
+/* canvases: HOST array of n descriptors; img / out: DEVICE uint8 blobs; lat / up: DEVICE float blobs (NULL when no canvas
+ * draws them).  Every argument is checked before anything is launched (PF_ERR_ARG). */
+int pf_draw_fields(int device, const pf_draw_canvas* canvases, int n, const uint8_t* img, uint8_t* out, const float* lat, const float* up,
+                   void* stream);
 
 /* ---- multi-GPU gather of results (SURVEY.md 8e: one process per GPU; NCCL point-to-point over NVLink) ---------------------
  * inference_batch shards its list over the ranks; the per-image results live on each rank's device and are gathered to ONE

@@ -39,6 +39,14 @@ class pf_pano_view(ctypes.Structure):
                 ("im_offset", ctypes.c_int64), ("field_offset", ctypes.c_int64)]
 
 
+class pf_draw_canvas(ctypes.Structure):
+    """include/pf_b200.h: struct pf_draw_canvas (one canvas of pf_draw_fields)."""
+    _fields_ = [("height", ctypes.c_int32), ("width", ctypes.c_int32), ("img_offset", ctypes.c_int64), ("out_offset", ctypes.c_int64),
+                ("lat_offset", ctypes.c_int64), ("up_offset", ctypes.c_int64), ("up_stride", ctypes.c_int64 * 3),
+                ("density", ctypes.c_int32), ("arrow_inv_len", ctypes.c_int32), ("arrow_rgb", ctypes.c_float * 3),
+                ("alpha_fill", ctypes.c_float), ("alpha_line", ctypes.c_float), ("draw_lat", ctypes.c_int32), ("draw_up", ctypes.c_int32)]
+
+
 class pf_batch(ctypes.Structure):
     _fields_ = [("n", ctypes.c_int),
                 ("images_u8", ctypes.c_void_p), ("image_offset", ctypes.POINTER(ctypes.c_int64)),
@@ -143,6 +151,8 @@ def lib():
         "pf_tma_pick_tile": (i32, [i32, i64, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32)]),
         "pf_set_option": (i32, [vp, ctypes.c_char_p, i32]),
         "pf_camera_fields": (i32, [i32, ctypes.POINTER(pf_camera), i32, vp, vp, vp]),
+        "pf_camera_fields_vp": (i32, [i32, ctypes.POINTER(pf_camera), ctypes.POINTER(ctypes.c_double), i32, vp, vp, vp]),
+        "pf_draw_fields": (i32, [i32, ctypes.POINTER(pf_draw_canvas), i32, vp, vp, vp, vp, vp]),
         "pf_pano_views": (i32, [i32, vp, i32, i32, ctypes.POINTER(pf_pano_view), i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
         "pf_op_layernorm": (i32, [vp, vp, i64, i32, vp, vp, f32, vp]),
         "pf_op_attention": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
@@ -191,7 +201,7 @@ def lib():
 EXPORTS = ["pf_abi_version", "pf_last_error", "pf_kernel_launch_count", "pf_create", "pf_create_sized", "pf_destroy", "pf_set_weight",
            "pf_finalize", "pf_workspace_bytes", "pf_forward", "pf_profile_enable", "pf_profile_read", "pf_profile_kernels_enable",
            "pf_profile_kernels_read", "pf_set_option", "pf_debug_enable", "pf_debug_count", "pf_debug_name", "pf_debug_numel",
-           "pf_debug_copy", "pf_camera_fields", "pf_pano_views", "pf_comm_unique_id", "pf_comm_create", "pf_comm_destroy", "pf_gather",
+           "pf_debug_copy", "pf_camera_fields", "pf_camera_fields_vp", "pf_pano_views", "pf_draw_fields", "pf_comm_unique_id", "pf_comm_create", "pf_comm_destroy", "pf_gather",
            "pf_jpeg_create", "pf_jpeg_destroy", "pf_jpeg_info", "pf_jpeg_decode_batch",
            "pf_op_conv_gemm", "pf_op_tma", "pf_op_tma_bf16", "pf_op_conv1_ring", "pf_tma_pick_tile", "pf_op_layernorm", "pf_op_attention",
            "pf_op_attention_mma", "pf_op_attention_tc", "pf_op_attention_tc_bf16", "pf_op_attention_tc_keys", "pf_op_dwconv3x3_gelu",

@@ -26,6 +26,7 @@
 #include "layers.cuh"
 #include "prepost.cuh"
 #include "pano.cuh"
+#include "draw.cuh"
 #include "comm.cuh"
 #include "jpeg.cuh"
 
@@ -1485,7 +1486,15 @@ int pf_tma_pick_tile(int mode, int64_t M, int N, int K, int sm_count, int* bn, i
   return PF_OK;
 }
 int pf_camera_fields(int device, const pf_camera* cams, int n, float* up, float* lat, void* stream) {
+  return pf_camera_fields_vp(device, cams, nullptr, n, up, lat, stream);
+}
+int pf_camera_fields_vp(int device, const pf_camera* cams, const double* vp, int n, float* up, float* lat, void* stream) {
   if (!cams || n < 1 || (!up && !lat)) return fail(PF_ERR_ARG, "pf_camera_fields: bad argument");
+  if (vp) {
+    for (int i = 0; i < n; ++i)
+      if (std::isfinite(vp[2 * i]) != std::isfinite(vp[2 * i + 1]))
+        return fail(PF_ERR_ARG, "pf_camera_fields_vp: image %d: a vanishing point needs two finite coordinates (or two NaN)", i);
+  }
   CU(cudaSetDevice(device));
   for (int i0 = 0; i0 < n; i0 += kCamChunk) {
     const int m = n - i0 < kCamChunk ? n - i0 : kCamChunk;
@@ -1501,6 +1510,8 @@ int pf_camera_fields(int device, const pf_camera* cams, int n, float* up, float*
       o.cx = (c.cx_rel + 0.5) * c.width; o.cy = (c.cy_rel + 0.5) * c.height;
       o.sr = sin(c.roll); o.cr = cos(c.roll); o.se = sin(c.elevation); o.ce = cos(c.elevation);
       o.sgn = c.elevation > 0 ? 1.0 : (c.elevation < 0 ? -1.0 : 0.0);
+      o.vp = vp && std::isfinite(vp[2 * (i0 + i)]);
+      if (o.vp) { o.vpx = vp[2 * (i0 + i)]; o.vpy = vp[2 * (i0 + i) + 1]; o.sgn = 1.0; }
       o.up_off = c.up_offset; o.lat_off = c.lat_offset;
       const long long qd = (long long)c.height * ((c.width + 3) / 4);
       if (qd > max_q) max_q = qd;
@@ -1563,6 +1574,85 @@ int pf_pano_views(int device, const uint8_t* pano, int pano_h, int pano_w, const
     const dim3 grid((unsigned)cdivl(max_px, (long long)kPanoThreads * kPanoPix) + 1, (unsigned)cnt);
     LAUNCHED((pano_views_kernel<<<grid, kPanoThreads, 0, (cudaStream_t)stream>>>(b, m, pano, im, ntheta, nphi, up, lat, xy, offset, status, i0),
               cudaGetLastError()));
+  }
+  return PF_OK;
+}
+
+// matplotlib's "seismic" map as the 256-entry table it samples (LinearSegmentedColormap.from_list: anchors at 0, 1/4, 1/2, 3/4, 1,
+// linear interpolation at i / 255), and t -> entry min(floor(256 t), 255); levels linspace(-pi/2, pi/2, 19).
+static DrawStyle draw_style() {
+  static const double anchors[5][3] = {{0.0, 0.0, 0.3}, {0.0, 0.0, 1.0}, {1.0, 1.0, 1.0}, {1.0, 0.0, 0.0}, {0.5, 0.0, 0.0}};
+  auto seismic = [&](double t, int ch) {
+    const int e = std::min((int)std::floor(256.0 * t), 255);
+    const double x = e / 255.0;
+    const int s = std::min((int)(x * 4.0), 3);
+    const double dist = (x - s / 4.0) / 0.25;
+    return 255.0 * (dist * (anchors[s + 1][ch] - anchors[s][ch]) + anchors[s][ch]);
+  };
+  DrawStyle st{};
+  const int nb = kDrawLevels - 1;
+  for (int k = 0; k < kDrawLevels; ++k) {
+    st.lev[k] = (float)(k == nb ? M_PI / 2 : -M_PI / 2 + k * (M_PI / nb));
+    for (int ch = 0; ch < 3; ++ch) {
+      st.line[k][ch] = (float)seismic((double)k / nb, ch);
+      if (k < nb) st.band[k][ch] = (float)seismic((k + 0.5) / nb, ch);
+    }
+  }
+  return st;
+}
+
+int pf_draw_fields(int device, const pf_draw_canvas* cs, int n, const uint8_t* img, uint8_t* out, const float* lat, const float* up, void* stream) {
+  if (!cs || n < 1 || !img || !out) return fail(PF_ERR_ARG, "pf_draw_fields: null canvases / img / out or n < 1");
+  auto unit = [](float x) { return std::isfinite(x) && x >= 0.f && x <= 1.f; };
+  for (int i = 0; i < n; ++i) {
+    const pf_draw_canvas& c = cs[i];
+    if (c.height < 1 || c.width < 1 || (long long)c.height * c.width >= (1LL << 31))
+      return fail(PF_ERR_ARG, "pf_draw_fields: canvas %d has size %dx%d", i, c.height, c.width);
+    if (c.img_offset < 0 || c.out_offset < 0) return fail(PF_ERR_ARG, "pf_draw_fields: canvas %d has a negative image offset", i);
+    if (!unit(c.alpha_fill) || !unit(c.alpha_line)) return fail(PF_ERR_ARG, "pf_draw_fields: canvas %d: alphas must lie in [0, 1]", i);
+    if (c.draw_lat && (!lat || c.lat_offset < 0)) return fail(PF_ERR_ARG, "pf_draw_fields: canvas %d draws the latitude without a latitude map", i);
+    if (c.draw_up) {
+      if (!up || c.up_offset < 0 || c.up_stride[0] < 0 || c.up_stride[1] < 0 || c.up_stride[2] < 0)
+        return fail(PF_ERR_ARG, "pf_draw_fields: canvas %d draws arrows without an up field, or with a negative offset / stride", i);
+      if (c.density < 1 || c.arrow_inv_len < 1 || c.width / c.density < 1 || c.height / c.density < 1)
+        return fail(PF_ERR_ARG, "pf_draw_fields: canvas %d (%dx%d): density %d and arrow_inv_len %d must be >= 1 and leave W // density, "
+                    "H // density >= 1", i, c.height, c.width, c.density, c.arrow_inv_len);
+      if (!unit(c.arrow_rgb[0]) || !unit(c.arrow_rgb[1]) || !unit(c.arrow_rgb[2])) return fail(PF_ERR_ARG, "pf_draw_fields: canvas %d: arrow colour outside [0, 1]", i);
+    }
+  }
+  CU(cudaSetDevice(device));
+  const DrawStyle st = draw_style();
+  for (int i0 = 0; i0 < n; i0 += kDrawChunk) {
+    const int cnt = n - i0 < kDrawChunk ? n - i0 : kDrawChunk;
+    DrawBatch b{};
+    long long max_tiles = 1;
+    for (int i = 0; i < cnt; ++i) {
+      const pf_draw_canvas& c = cs[i0 + i];
+      DrawCanvas& o = b.c[i];
+      o.H = c.height; o.W = c.width;
+      o.tiles_x = cdiv(c.width, kDrawTW);
+      o.draw_lat = c.draw_lat != 0; o.draw_up = c.draw_up != 0;
+      o.alpha_fill = c.alpha_fill; o.alpha_line = c.alpha_line;
+      o.img_off = c.img_offset; o.out_off = c.out_offset; o.lat_off = c.lat_offset; o.up_off = c.up_offset;
+      o.us_row = c.up_stride[0]; o.us_col = c.up_stride[1]; o.us_comp = c.up_stride[2];
+      if (o.draw_up) {
+        o.sx = c.width / c.density; o.sy = c.height / c.density;
+        o.nx = cdiv(c.width, o.sx); o.ny = cdiv(c.height, o.sy);
+        // np.sqrt(W^2 + H^2) // arrow_inv_len with Python's float floor division
+        const double diag = std::sqrt((double)c.width * c.width + (double)c.height * c.height), q = c.arrow_inv_len;
+        const double mod = std::fmod(diag, q), div = (diag - mod) / q;
+        double fl = std::floor(div);
+        if (div - fl > 0.5) fl += 1.0;
+        o.len = (float)fl;
+        const double sq = std::sqrt((double)o.nx * o.ny);                        // quiver's default width: 0.06 span / clip(sqrt(N), 8, 25)
+        o.w = (float)(0.06 * c.width / std::min(std::max(sq, 8.0), 25.0));
+        for (int ch = 0; ch < 3; ++ch) o.rgb[ch] = 255.f * c.arrow_rgb[ch];
+      }
+      const long long tiles = (long long)o.tiles_x * cdiv(c.height, kDrawTH);
+      if (tiles > max_tiles) max_tiles = tiles;
+    }
+    const dim3 grid((unsigned)max_tiles, (unsigned)cnt);
+    LAUNCHED((draw_fields_kernel<<<grid, kDrawThreads, 0, (cudaStream_t)stream>>>(b, st, img, out, lat, up), cudaGetLastError()));
   }
   return PF_OK;
 }

@@ -295,6 +295,8 @@ struct CamImage {
   double f, cx, cy;           // focal length in pixels, principal point in pixels
   double sr, cr, se, ce;      // sin / cos of roll and elevation (computed on the host in float64)
   double sgn;                 // sign(elevation): +1, -1 or 0 (0 selects the constant field)
+  int vp;                     // 1: the up field points to (vpx, vpy) instead (PanoCam.get_up's far point at elevation 0)
+  double vpx, vpy;
   long long up_off, lat_off;  // float offsets of this image's blocks in the output blobs
 };
 constexpr int kCamChunk = 24;   // images per launch (the descriptors travel as a kernel parameter)
@@ -338,7 +340,7 @@ __global__ void __launch_bounds__(256) camera_fields_kernel(const __grid_constan
 #pragma unroll
       for (int k = 0; k < 4; ++k) { o[2 * k] = (float)(-c.sr); o[2 * k + 1] = (float)(-c.cr); }
     } else {
-      const double vvp_x = (c.sr * c.ce * c.f) / -c.se + c.cx, vvp_y = (c.cr * c.ce * c.f) / -c.se + c.cy;
+      const double vvp_x = c.vp ? c.vpx : (c.sr * c.ce * c.f) / -c.se + c.cx, vvp_y = c.vp ? c.vpy : (c.cr * c.ce * c.f) / -c.se + c.cy;
       const float vy = (float)((vvp_y - ((double)i + 0.5)) * c.sgn);
       const float vx0 = (float)((vvp_x - ((double)j0 + 0.5)) * c.sgn), dvx = (float)(-c.sgn);    // pixel k: vx0 + k * dvx
 #pragma unroll

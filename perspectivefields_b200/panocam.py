@@ -47,8 +47,10 @@ def general_vfov_to_focal(rel_cx, rel_cy, h, gvfov, degree):
         return np.sqrt(f2)
 
 
-def camera_fields(focal_rel, heights, widths, elevation, roll, cx_rel, cy_rel, device=None, up=True, lat=True):
+def camera_fields(focal_rel, heights, widths, elevation, roll, cx_rel, cy_rel, device=None, up=True, lat=True, vp=None):
     """Batched ``get_up_general`` / ``get_lat_general``: every argument is a sequence of length n (radians for the angles).
+    ``vp``: None or a sequence of n (x, y) points in pixel-centre coordinates (pixel (i, j) at (j + .5, i + .5)) that the up
+    fields point to instead, (nan, nan) keeping the camera's own (``PanoCam.get_up`` at elevation 0).
     Returns (list of [H_i, W_i, 2] float32 tensors or None, list of [H_i, W_i] float32 tensors in degrees or None)."""
     L = _native.lib()
     if not torch.cuda.is_available():
@@ -69,8 +71,13 @@ def camera_fields(focal_rel, heights, widths, elevation, roll, cx_rel, cy_rel, d
         up_blob = torch.empty(up_off, dtype=torch.float32, device=dev) if up else None
         lat_blob = torch.empty(lat_off, dtype=torch.float32, device=dev) if lat else None
         stream = torch.cuda.current_stream(dev).cuda_stream
-        _native.check(L.pf_camera_fields(dev.index if dev.index is not None else torch.cuda.current_device(), cams, n,
-                                         up_blob.data_ptr() if up else None, lat_blob.data_ptr() if lat else None, stream))
+        index = dev.index if dev.index is not None else torch.cuda.current_device()
+        up_ptr, lat_ptr = up_blob.data_ptr() if up else None, lat_blob.data_ptr() if lat else None
+        if vp is None:
+            _native.check(L.pf_camera_fields(index, cams, n, up_ptr, lat_ptr, stream))
+        else:
+            vps = (ctypes.c_double * (2 * n))(*[float(c) for p in vp for c in p])
+            _native.check(L.pf_camera_fields_vp(index, cams, vps, n, up_ptr, lat_ptr, stream))
     ups = [up_blob[c.up_offset:c.up_offset + 2 * c.height * c.width].view(c.height, c.width, 2) for c in cams] if up else None
     lats = [lat_blob[c.lat_offset:c.lat_offset + c.height * c.width].view(c.height, c.width) for c in cams] if lat else None
     return ups, lats
@@ -208,6 +215,16 @@ class PanoCam:
         return (out["im"][0], out["ntheta"][0], nphi, float(out["offset"][0].item()), out["up"][0], out["lat"][0], out["xy_map"][0])
 
     @staticmethod
+    def get_up(vfov, im_w, im_h, elevation, roll, device=None):
+        """utils/panocam.py:422-448 (pinhole camera, centred principal point) -> float32 CUDA tensor [im_h, im_w, 2]."""
+        return pinhole_fields([vfov], [im_h], [im_w], [elevation], [roll], device, up=True, lat=False)[0][0]
+
+    @staticmethod
+    def get_lat(vfov, im_w, im_h, elevation, roll, device=None):
+        """utils/panocam.py:384-420 -> float32 CUDA tensor [im_h, im_w], degrees."""
+        return pinhole_fields([vfov], [im_h], [im_w], [elevation], [roll], device, up=False, lat=True)[1][0]
+
+    @staticmethod
     def get_up_general(focal_rel, im_w, im_h, elevation, roll, cx_rel, cy_rel, device=None):
         """utils/panocam.py:451-513 -> float32 CUDA tensor [im_h, im_w, 2]."""
         return camera_fields([focal_rel], [im_h], [im_w], [elevation], [roll], [cx_rel], [cy_rel], device, up=True, lat=False)[0][0]
@@ -216,6 +233,28 @@ class PanoCam:
     def get_lat_general(focal_rel, im_w, im_h, elevation, roll, cx_rel, cy_rel, device=None):
         """utils/panocam.py:515-556 -> float32 CUDA tensor [im_h, im_w], degrees."""
         return camera_fields([focal_rel], [im_h], [im_w], [elevation], [roll], [cx_rel], [cy_rel], device, up=False, lat=True)[1][0]
+
+
+def far_vanishing_point(im_w, im_h, roll):
+    """utils/panocam.py:288-300, :336-382 at elevation 0 (getRelativeVVP returns inf there): the point 1e8 px away along the
+    horizon's normal, in pixel-centre coordinates (the reference's pixel-index point + 0.5).  float64."""
+    dh = math.inf * np.sign(roll) if roll in (math.pi / 2, -math.pi / 2) else -im_w / im_h * np.tan(roll) / 2
+    d = np.array([im_h * ((0.5 + dh) - (0.5 - dh)), -im_w], np.float64)
+    norm = np.sqrt(d @ d)
+    if norm >= 10 * np.finfo(np.float64).eps:                # sklearn's normalize leaves (near-)zero rows unscaled
+        d = d / norm
+    return 1e8 * d[0] + 0.5 * im_w, 1e8 * d[1] + 0.5 * im_h
+
+
+def pinhole_fields(vfov, heights, widths, elevation, roll, device=None, up=True, lat=True):
+    """Batched ``PanoCam.get_up`` / ``get_lat`` (utils/panocam.py:384-448), radians: the ``_general`` fields with focal_rel =
+    1 / (2 tan(vfov / 2)) and a centred principal point, except that at elevation == 0 the up field points to the reference's
+    far vanishing point (``far_vanishing_point``) rather than being constant."""
+    n = len(heights)
+    focal = [1.0 / (2.0 * math.tan(float(v) / 2.0)) for v in vfov]
+    nan = (math.nan, math.nan)
+    vp = [far_vanishing_point(int(widths[i]), int(heights[i]), float(roll[i])) if float(elevation[i]) == 0 else nan for i in range(n)]
+    return camera_fields(focal, heights, widths, elevation, roll, [0.0] * n, [0.0] * n, device, up=up, lat=lat, vp=vp)
 
 
 def fields_from_predictions(preds, sizes, mode="deg", device=None):
