@@ -181,6 +181,32 @@ typedef struct pf_pano_view {
 int pf_pano_views(int device, const uint8_t* pano, int pano_h, int pano_w, const pf_pano_view* views, int n, uint8_t* im, float* ntheta,
                   float* nphi, float* up, float* lat, float* xy, double* offset, int32_t* status, void* stream);
 
+/* ---- pinhole views of a panorama ----------------------------------------------------------------------------------------------
+ * Replaces PanoCam.crop_equi and the crop of PanoCam(path).get_image (perspective2d/utils/panocam.py:121-249; equilib's equi2pers
+ * there) for a batch of views of ONE equirectangular panorama.  A view of width W has fov_x = 2 atan(tan(vfov / 2) ar) and focal
+ * length W / (2 tan(fov_x / 2)); it is rotated by roll, then elevation, then azimuth, and sampled by the rule of DESIGN.md
+ * section 1 (float64 geometry; bilinear: columns wrap, rows clamp, float64 weights).  One launch per 24 views; no engine handle, no
+ * synchronisation. */
+typedef struct pf_equi_view {
+  int32_t height, width;        /* im_h, im_w of the view */
+  double vfov;                  /* vertical field of view, degrees, in (0, 180) */
+  double azimuth, elevation, roll;   /* degrees */
+  double ar;                    /* aspect ratio the field of view is widened by (> 0; fov_x must stay below 180 degrees) */
+  int64_t offset;               /* byte offset of this view's [H,W,C] crop in `im` (a multiple of the element size) */
+} pf_equi_view;
+enum pf_equi_dtype { PF_EQUI_U8 = 0, PF_EQUI_F32 = 1 };
+enum pf_equi_mode { PF_EQUI_BILINEAR = 0, PF_EQUI_NEAREST = 1 };
+/* PF_EQUI_CAST: the sample rounded to float32, then cast to the panorama's dtype (uint8: truncated), crop_equi's
+ * np.asarray(.., dtype=equi_img.dtype).  PF_EQUI_UNIT (uint8 panoramas only): get_image's path, the sample of p / 255 in float32
+ * (ToTensor), rounded to float32, times 255 in float32 and truncated to uint8 (ToPILImage). */
+enum pf_equi_out { PF_EQUI_CAST = 0, PF_EQUI_UNIT = 1 };
+/* pano: DEVICE [pano_h, pano_w, channels] HWC (channels 1 or 3) of dtype enum pf_equi_dtype; views: HOST array of n descriptors;
+ * mode: enum pf_equi_mode; out_kind: enum pf_equi_out; swap_rb: 1 writes channels in the order 2, 1, 0 (BGR from an RGB panorama,
+ * 3 channels only); im: DEVICE blob of crops in the output dtype (float32 for a float32 panorama, uint8 otherwise).  Every
+ * argument is checked before anything is launched (PF_ERR_ARG). */
+int pf_equi_views(int device, const void* pano, int pano_h, int pano_w, int channels, int dtype, const pf_equi_view* views, int n, int mode,
+                  int out_kind, int swap_rb, void* im, void* stream);
+
 /* ---- perspective-field overlays (draw_perspective_fields / draw_up_field / draw_latitude_field, utils/utils.py:165-430) -----
  * Draws the latitude contours (18 filled bands and 19 lines of linspace(-pi/2, pi/2, 19), seismic colours) and the up-vector
  * arrows (quiver on the lattice arange(0, W, W // density) x arange(0, H, H // density), length up * (sqrt(W^2 + H^2) //

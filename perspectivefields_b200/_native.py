@@ -39,6 +39,17 @@ class pf_pano_view(ctypes.Structure):
                 ("im_offset", ctypes.c_int64), ("field_offset", ctypes.c_int64)]
 
 
+class pf_equi_view(ctypes.Structure):
+    """include/pf_b200.h: struct pf_equi_view (one view of pf_equi_views)."""
+    _fields_ = [("height", ctypes.c_int32), ("width", ctypes.c_int32), ("vfov", ctypes.c_double), ("azimuth", ctypes.c_double),
+                ("elevation", ctypes.c_double), ("roll", ctypes.c_double), ("ar", ctypes.c_double), ("offset", ctypes.c_int64)]
+
+
+PF_EQUI_U8, PF_EQUI_F32 = 0, 1
+PF_EQUI_BILINEAR, PF_EQUI_NEAREST = 0, 1
+PF_EQUI_CAST, PF_EQUI_UNIT = 0, 1
+
+
 class pf_draw_canvas(ctypes.Structure):
     """include/pf_b200.h: struct pf_draw_canvas (one canvas of pf_draw_fields)."""
     _fields_ = [("height", ctypes.c_int32), ("width", ctypes.c_int32), ("img_offset", ctypes.c_int64), ("out_offset", ctypes.c_int64),
@@ -154,6 +165,7 @@ def lib():
         "pf_camera_fields_vp": (i32, [i32, ctypes.POINTER(pf_camera), ctypes.POINTER(ctypes.c_double), i32, vp, vp, vp]),
         "pf_draw_fields": (i32, [i32, ctypes.POINTER(pf_draw_canvas), i32, vp, vp, vp, vp, vp]),
         "pf_pano_views": (i32, [i32, vp, i32, i32, ctypes.POINTER(pf_pano_view), i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+        "pf_equi_views": (i32, [i32, vp, i32, i32, i32, i32, ctypes.POINTER(pf_equi_view), i32, i32, i32, i32, vp, vp]),
         "pf_op_layernorm": (i32, [vp, vp, i64, i32, vp, vp, f32, vp]),
         "pf_op_attention": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
         "pf_op_attention_mma": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
@@ -201,7 +213,7 @@ def lib():
 EXPORTS = ["pf_abi_version", "pf_last_error", "pf_kernel_launch_count", "pf_create", "pf_create_sized", "pf_destroy", "pf_set_weight",
            "pf_finalize", "pf_workspace_bytes", "pf_forward", "pf_profile_enable", "pf_profile_read", "pf_profile_kernels_enable",
            "pf_profile_kernels_read", "pf_set_option", "pf_debug_enable", "pf_debug_count", "pf_debug_name", "pf_debug_numel",
-           "pf_debug_copy", "pf_camera_fields", "pf_camera_fields_vp", "pf_pano_views", "pf_draw_fields", "pf_comm_unique_id", "pf_comm_create", "pf_comm_destroy", "pf_gather",
+           "pf_debug_copy", "pf_camera_fields", "pf_camera_fields_vp", "pf_pano_views", "pf_equi_views", "pf_draw_fields", "pf_comm_unique_id", "pf_comm_create", "pf_comm_destroy", "pf_gather",
            "pf_jpeg_create", "pf_jpeg_destroy", "pf_jpeg_info", "pf_jpeg_decode_batch",
            "pf_op_conv_gemm", "pf_op_tma", "pf_op_tma_bf16", "pf_op_conv1_ring", "pf_tma_pick_tile", "pf_op_layernorm", "pf_op_attention",
            "pf_op_attention_mma", "pf_op_attention_tc", "pf_op_attention_tc_bf16", "pf_op_attention_tc_keys", "pf_op_dwconv3x3_gelu",

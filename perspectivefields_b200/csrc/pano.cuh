@@ -41,6 +41,31 @@ __device__ __forceinline__ double pa(double a, double b) { return __dadd_rn(a, b
 __device__ __forceinline__ double ps(double a, double b) { return __dsub_rn(a, b); }
 __device__ __forceinline__ double pd(double a, double b) { return __ddiv_rn(a, b); }
 
+// The project's panorama sampler (DESIGN.md section 1), shared with equi_views_kernel: taps and weights of a bilinear sample at
+// panorama pixel (nx, ny) in pixel-index units; columns wrap (x1 = (x0 + 1) mod Wp), rows clamp (ny to [0, Hp - 1], y1 <= Hp - 1).
+struct PanoTaps {
+  long long x0, x1, y0, y1;
+  double wx, hx, wy, hy;
+};
+__device__ __forceinline__ PanoTaps pano_taps(double nx, double ny, int Hp, int Wp) {
+  PanoTaps t;
+  const double xf = floor(nx);
+  t.wx = ps(nx, xf); t.hx = ps(1.0, t.wx);
+  t.x0 = (long long)xf % Wp;
+  if (t.x0 < 0) t.x0 += Wp;
+  t.x1 = t.x0 + 1 == Wp ? 0 : t.x0 + 1;
+  const double nyc = fmin(fmax(ny, 0.0), (double)(Hp - 1));
+  const double yf = floor(nyc);
+  t.wy = ps(nyc, yf); t.hy = ps(1.0, t.wy);
+  t.y0 = (long long)yf;
+  t.y1 = t.y0 + 1 < Hp ? t.y0 + 1 : t.y0;
+  return t;
+}
+// (1 - wy) ((1 - wx) p00 + wx p01) + wy ((1 - wx) p10 + wx p11), float64, in that order
+__device__ __forceinline__ double pano_lerp(const PanoTaps& t, double p00, double p01, double p10, double p11) {
+  return pa(pm(t.hy, pa(pm(t.hx, p00), pm(t.wx, p01))), pm(t.wy, pa(pm(t.hx, p10), pm(t.wx, p11))));
+}
+
 // out = M p (transpose: M^T p); each row summed left to right, (m0 x + m1 y) + m2 z
 __device__ __forceinline__ void pano_rot(const double* M, bool transpose, double& x, double& y, double& z) {
   double o[3];
@@ -138,19 +163,12 @@ __global__ void __launch_bounds__(kPanoThreads) pano_views_kernel(const __grid_c
       if (im) {
         const bool inside = !v.masked || pa(pm(ps((double)i, v.ci0), ps((double)i, v.ci0)), pm(ps((double)j, v.ci1), ps((double)j, v.ci1))) < v.r2;
         if (inside) {
-          const double xf = floor(nx), wx = ps(nx, xf), hx = ps(1.0, wx);
-          long long x0 = (long long)xf % m.Wp;
-          if (x0 < 0) x0 += m.Wp;
-          const long long x1 = x0 + 1 == m.Wp ? 0 : x0 + 1;
-          const double nyc = fmin(fmax(ny, 0.0), (double)(m.Hp - 1));
-          const double yf = floor(nyc), wy = ps(nyc, yf), hy = ps(1.0, wy);
-          const long long y0 = (long long)yf, y1 = y0 + 1 < m.Hp ? y0 + 1 : y0;
-          const unsigned char* r0 = pano + y0 * m.Wp * 3;
-          const unsigned char* r1 = pano + y1 * m.Wp * 3;
+          const PanoTaps t = pano_taps(nx, ny, m.Hp, m.Wp);
+          const unsigned char* r0 = pano + t.y0 * m.Wp * 3;
+          const unsigned char* r1 = pano + t.y1 * m.Wp * 3;
 #pragma unroll
           for (int c = 0; c < 3; ++c) {
-            const double p00 = __ldg(r0 + x0 * 3 + c), p01 = __ldg(r0 + x1 * 3 + c), p10 = __ldg(r1 + x0 * 3 + c), p11 = __ldg(r1 + x1 * 3 + c);
-            const double s = pa(pm(hy, pa(pm(hx, p00), pm(wx, p01))), pm(wy, pa(pm(hx, p10), pm(wx, p11))));
+            const double s = pano_lerp(t, __ldg(r0 + t.x0 * 3 + c), __ldg(r0 + t.x1 * 3 + c), __ldg(r1 + t.x0 * 3 + c), __ldg(r1 + t.x1 * 3 + c));
             px[3 * k + c] = (unsigned char)(int)fmin(fmax(s, 0.0), 255.0);
           }
         }

@@ -26,6 +26,7 @@
 #include "layers.cuh"
 #include "prepost.cuh"
 #include "pano.cuh"
+#include "equi.cuh"
 #include "draw.cuh"
 #include "comm.cuh"
 #include "jpeg.cuh"
@@ -1574,6 +1575,66 @@ int pf_pano_views(int device, const uint8_t* pano, int pano_h, int pano_w, const
     const dim3 grid((unsigned)cdivl(max_px, (long long)kPanoThreads * kPanoPix) + 1, (unsigned)cnt);
     LAUNCHED((pano_views_kernel<<<grid, kPanoThreads, 0, (cudaStream_t)stream>>>(b, m, pano, im, ntheta, nphi, up, lat, xy, offset, status, i0),
               cudaGetLastError()));
+  }
+  return PF_OK;
+}
+
+// PanoCam.crop_equi / get_image (utils/panocam.py:121-249) for n views of one panorama: the host computes each view's fov_x
+// (:216-218, the wrapper's own expression), focal length and the sines and cosines of its angles once; one launch per kEquiChunk views.
+int pf_equi_views(int device, const void* pano, int pano_h, int pano_w, int channels, int dtype, const pf_equi_view* views, int n, int mode,
+                  int out_kind, int swap_rb, void* im, void* stream) {
+  if (!pano || !views || !im || n < 1) return fail(PF_ERR_ARG, "pf_equi_views: null panorama / views / im or n < 1");
+  if (pano_h < 1 || pano_w < 1) return fail(PF_ERR_ARG, "pf_equi_views: panorama of %dx%d", pano_h, pano_w);
+  if (channels != 1 && channels != 3) return fail(PF_ERR_ARG, "pf_equi_views: %d channels (1 or 3)", channels);
+  if (dtype != PF_EQUI_U8 && dtype != PF_EQUI_F32) return fail(PF_ERR_ARG, "pf_equi_views: unknown dtype %d", dtype);
+  if (mode != PF_EQUI_BILINEAR && mode != PF_EQUI_NEAREST) return fail(PF_ERR_ARG, "pf_equi_views: unknown mode %d", mode);
+  if (out_kind != PF_EQUI_CAST && out_kind != PF_EQUI_UNIT) return fail(PF_ERR_ARG, "pf_equi_views: unknown out_kind %d", out_kind);
+  if (out_kind == PF_EQUI_UNIT && dtype != PF_EQUI_U8) return fail(PF_ERR_ARG, "pf_equi_views: the unit path needs a uint8 panorama");
+  if (swap_rb != 0 && (swap_rb != 1 || channels != 3)) return fail(PF_ERR_ARG, "pf_equi_views: swap_rb must be 0, or 1 with 3 channels");
+  const int esize = dtype == PF_EQUI_F32 ? 4 : 1;
+  std::vector<double> fov_x(n);
+  for (int i = 0; i < n; ++i) {
+    const pf_equi_view& c = views[i];
+    if (c.height < 1 || c.width < 1) return fail(PF_ERR_ARG, "pf_equi_views: view %d has size %dx%d", i, c.height, c.width);
+    if (!std::isfinite(c.azimuth) || !std::isfinite(c.elevation) || !std::isfinite(c.roll))
+      return fail(PF_ERR_ARG, "pf_equi_views: view %d: non-finite angle", i);
+    if (!std::isfinite(c.vfov) || !(c.vfov > 0.0 && c.vfov < 180.0) || !std::isfinite(c.ar) || !(c.ar > 0.0))
+      return fail(PF_ERR_ARG, "pf_equi_views: view %d: vfov %g must lie in (0, 180) and ar %g be finite and > 0", i, c.vfov, c.ar);
+    fov_x[i] = 2 * atan(tan(c.vfov * M_PI / 180.0 / 2) * c.ar) * 180 / M_PI;
+    if (!(fov_x[i] > 0.0 && fov_x[i] < 180.0)) return fail(PF_ERR_ARG, "pf_equi_views: view %d: fov_x %g must lie in (0, 180)", i, fov_x[i]);
+    if (c.offset < 0 || c.offset % esize != 0) return fail(PF_ERR_ARG, "pf_equi_views: view %d: offset %lld (>= 0, a multiple of %d)", i,
+                                                          (long long)c.offset, esize);
+  }
+  CU(cudaSetDevice(device));
+  EquiMap m{};
+  m.Hp = pano_h; m.Wp = pano_w; m.C = channels;
+  m.nearest = mode == PF_EQUI_NEAREST; m.swap_rb = swap_rb;
+  m.su = pano_w / (2 * M_PI); m.sv = pano_h / M_PI;
+  for (int i0 = 0; i0 < n; i0 += kEquiChunk) {
+    const int cnt = n - i0 < kEquiChunk ? n - i0 : kEquiChunk;
+    EquiBatch b{};
+    long long max_px = 1;
+    for (int i = 0; i < cnt; ++i) {
+      const pf_equi_view& c = views[i0 + i];
+      EquiView& o = b.v[i];
+      o.H = c.height; o.W = c.width;
+      o.f = c.width / (2 * tan(fov_x[i0 + i] * M_PI / 180 / 2));
+      o.u0 = c.width / 2.0; o.v0 = c.height / 2.0;
+      const double roll = c.roll / 180 * M_PI, el = c.elevation / 180 * M_PI, az = c.azimuth / 180 * M_PI;   // the wrapper's rot dict
+      o.cr = cos(roll); o.sr = sin(roll); o.ce = cos(el); o.se = sin(el); o.ca = cos(az); o.sa = sin(az);
+      o.off = c.offset;
+      const long long px = (long long)c.height * c.width;
+      if (px > max_px) max_px = px;
+    }
+    const dim3 grid((unsigned)cdivl(max_px, (long long)kEquiThreads * kEquiPix), (unsigned)cnt);
+    cudaStream_t st = (cudaStream_t)stream;
+    unsigned char* out = (unsigned char*)im;
+    if (dtype == PF_EQUI_F32)
+      LAUNCHED((equi_views_kernel<float, false><<<grid, kEquiThreads, 0, st>>>(b, m, (const float*)pano, out), cudaGetLastError()));
+    else if (out_kind == PF_EQUI_UNIT)
+      LAUNCHED((equi_views_kernel<unsigned char, true><<<grid, kEquiThreads, 0, st>>>(b, m, (const unsigned char*)pano, out), cudaGetLastError()));
+    else
+      LAUNCHED((equi_views_kernel<unsigned char, false><<<grid, kEquiThreads, 0, st>>>(b, m, (const unsigned char*)pano, out), cudaGetLastError()));
   }
   return PF_OK;
 }

@@ -7,6 +7,9 @@ Also ``PanoCam.crop_distortion`` (utils/panocam.py:559-752, the reference's note
 perspective or Unified Spherical Model view cropped from an equirectangular panorama with its ground-truth fields, and its batched
 form ``crop_distortion_views``, whose crops can go straight into ``PerspectiveFields.inference_batch`` on the device.
 
+And the pinhole crop of that workflow: ``PanoCam.crop_equi``, ``PanoCam(pano_path).get_image`` with its horizon line and vertical
+vanishing point (utils/panocam.py:121-382), and the batched ``crop_equi_views``, under the crop rule of DESIGN.md section 1.
+
 Same names, argument order and meaning as the reference.  Differences: results are float32 CUDA tensors (the reference returns
 float64 numpy arrays), and ``camera_fields`` evaluates a whole batch (images may differ in size) in one launch per 24 images.
 There is no CPU path: the functions raise when the CUDA library or a CUDA device is missing.
@@ -194,8 +197,193 @@ def crop_distortion_views(image360, views, outputs=("up", "lat"), device=None):
     return out
 
 
+EQUI_MODES = {"bilinear": _native.PF_EQUI_BILINEAR, "nearest": _native.PF_EQUI_NEAREST}
+
+
+def _rad(deg):
+    return deg / 180 * math.pi          # the reference's expression (utils/panocam.py:171-173, :188-193)
+
+
+def _check_equi_view(view, i):
+    """(vfov, im_w, im_h, azimuth, elevation, roll, ar) -- crop_equi's argument order -- or a dict with those keys -> checked tuple."""
+    keys = ("vfov", "im_w", "im_h", "azimuth", "elevation", "roll", "ar")
+    if isinstance(view, dict):
+        missing = [k for k in keys if k not in view]
+        if missing:
+            raise ValueError(f"view {i}: missing {missing}")
+        view = [view[k] for k in keys]
+    view = tuple(view)
+    if len(view) != 7:
+        raise ValueError(f"view {i}: expected (vfov, im_w, im_h, azimuth, elevation, roll, ar), got {len(view)} values")
+    vfov, w, h, az, el, roll, ar = view
+    vfov, ar = _real(vfov, f"view {i}: vfov"), _real(ar, f"view {i}: ar")
+    if not 0.0 < vfov < 180.0:
+        raise ValueError(f"view {i}: vfov must lie in (0, 180) degrees, got {vfov}")
+    if ar <= 0.0:
+        raise ValueError(f"view {i}: ar must be > 0, got {ar}")
+    fov_x = 2 * math.atan(math.tan(vfov * math.pi / 180.0 / 2) * ar) * 180 / math.pi
+    if not fov_x < 180.0:
+        raise ValueError(f"view {i}: the horizontal field of view 2 atan(tan(vfov / 2) ar) = {fov_x} degrees must be < 180")
+    return (vfov, _size(w, f"view {i}: im_w"), _size(h, f"view {i}: im_h"), _real(az, f"view {i}: azimuth"),
+            _real(el, f"view {i}: elevation"), _real(roll, f"view {i}: roll"), ar)
+
+
+def _check_equi_panorama(equi_img):
+    """numpy / torch uint8 or float32 [Hp, Wp] or [Hp, Wp, 3] -> (array or tensor, dtype code, channels); no GPU work."""
+    if isinstance(equi_img, torch.Tensor):
+        codes = {torch.uint8: _native.PF_EQUI_U8, torch.float32: _native.PF_EQUI_F32}
+    else:
+        equi_img = np.asarray(equi_img)
+        codes = {np.dtype(np.uint8): _native.PF_EQUI_U8, np.dtype(np.float32): _native.PF_EQUI_F32}
+    if equi_img.dtype not in codes:
+        raise TypeError(f"the panorama must be uint8 or float32, got {equi_img.dtype}")
+    shape = tuple(equi_img.shape)
+    if len(shape) not in (2, 3) or (len(shape) == 3 and shape[2] != 3):
+        raise TypeError(f"the panorama must be [H, W] or [H, W, 3], got {list(shape)}")
+    if shape[0] < 1 or shape[1] < 1:
+        raise ValueError(f"the panorama must be at least 1 x 1, got {shape[0]} x {shape[1]}")
+    return equi_img, codes[equi_img.dtype], 1 if len(shape) == 2 else 3
+
+
+def _pano_device(pano, device):
+    """The CUDA device a call runs on: the panorama's own when it is a CUDA tensor (``device`` must agree), else ``device`` or the
+    current one."""
+    if not torch.cuda.is_available():
+        raise RuntimeError("perspectivefields_b200.panocam needs a CUDA device (there is no CPU path)")
+    if isinstance(pano, torch.Tensor) and pano.is_cuda:
+        if device is not None and torch.device(device) != pano.device:
+            raise ValueError(f"the panorama is on {pano.device}, not on {device}")
+        return pano.device
+    dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    if dev.type != "cuda":
+        raise RuntimeError("perspectivefields_b200.panocam needs a CUDA device (there is no CPU path)")
+    return torch.device("cuda", torch.cuda.current_device()) if dev.index is None else dev
+
+
+def horizon_vvp(vfov, im_w, im_h, elevation, roll):
+    """get_image's horizon line and relative vertical vanishing point (utils/panocam.py:188-193), degrees in; the reference's tuples."""
+    args = (_rad(elevation), _rad(roll), _rad(vfov), im_h, im_w)
+    return PanoCam.getRelativeHorizonLineFromAngles(*args), PanoCam.getRelativeVVP(*args)
+
+
+def _equi_views(equi_img, views, outputs, mode, img_format, unit, device):
+    outputs = tuple(outputs)
+    bad = [o for o in outputs if o not in ("up", "lat")]
+    if bad:
+        raise ValueError(f"unknown outputs {bad}; choose from ('up', 'lat')")
+    if mode not in EQUI_MODES:
+        raise ValueError(f"unknown mode {mode!r}; choose from {tuple(EQUI_MODES)}")
+    if img_format not in ("RGB", "BGR"):
+        raise ValueError(f"unknown img_format {img_format!r}; choose 'RGB' or 'BGR'")
+    vs = [_check_equi_view(v, i) for i, v in enumerate(views)]
+    if not vs:
+        raise ValueError("no views")
+    pano, dtype, channels = _check_equi_panorama(equi_img)
+    swap = img_format == "BGR"
+    if swap and channels != 3:
+        raise ValueError("img_format='BGR' needs a 3-channel panorama")
+    if unit and dtype != _native.PF_EQUI_U8:
+        raise TypeError("get_image's crop needs a uint8 panorama")
+    dev = _pano_device(pano, device)
+    L = _native.lib()
+    n = len(vs)
+    esize = 4 if dtype == _native.PF_EQUI_F32 else 1
+    descs = (_native.pf_equi_view * n)()
+    off = 0
+    for i, (vfov, w, h, az, el, roll, ar) in enumerate(vs):
+        descs[i] = _native.pf_equi_view(h, w, vfov, az, el, roll, ar, off)
+        off += (channels * h * w * esize + 15) // 16 * 16        # 16-byte aligned crops: full-width vector stores
+    with torch.cuda.device(dev):
+        src = torch.as_tensor(pano).to(dev).contiguous()
+        blob = torch.empty(off, dtype=torch.uint8, device=dev)
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        _native.check(L.pf_equi_views(dev.index, src.data_ptr(), src.shape[0], src.shape[1], channels, dtype, descs, n, EQUI_MODES[mode],
+                                      _native.PF_EQUI_UNIT if unit else _native.PF_EQUI_CAST, int(swap), blob.data_ptr(), stream))
+    tdt = torch.float32 if dtype == _native.PF_EQUI_F32 else torch.uint8
+    shape = (lambda d: (d.height, d.width, 3)) if channels == 3 else (lambda d: (d.height, d.width))
+    out = {"im": [blob[d.offset:d.offset + channels * d.height * d.width * esize].view(tdt).view(shape(d)) for d in descs]}
+    if outputs:
+        ups, lats = pinhole_fields([_rad(v[0]) for v in vs], [v[2] for v in vs], [v[1] for v in vs], [_rad(v[4]) for v in vs],
+                                   [_rad(v[5]) for v in vs], dev, up="up" in outputs, lat="lat" in outputs)
+        out.update({k: f for k, f in (("up", ups), ("lat", lats)) if k in outputs})
+    hv = [horizon_vvp(v[0], v[1], v[2], v[4], v[5]) for v in vs]
+    out["horizon"] = np.array([h for h, _ in hv], np.float64).reshape(n, 2)
+    out["vvp"] = np.array([tuple(p) + (math.nan,) * (3 - len(p)) for _, p in hv], np.float64).reshape(n, 3)
+    return out
+
+
+def crop_equi_views(equi_img, views, outputs=("up", "lat"), mode="bilinear", img_format="RGB", device=None):
+    """Batched ``PanoCam.crop_equi`` (utils/panocam.py:196-249): pinhole views of ONE equirectangular panorama, one upload, one
+    launch per 24 views, no synchronisation.  ``equi_img``: numpy / torch uint8 or float32 [Hp, Wp] or [Hp, Wp, 3]; ``views``:
+    sequence of ``(vfov, im_w, im_h, azimuth, elevation, roll, ar)`` in degrees (or dicts with those keys; sizes may differ);
+    ``outputs``: any of ``up, lat``; ``mode``: ``bilinear`` or ``nearest``; ``img_format="BGR"`` writes the channels in the order
+    2, 1, 0.  Returns a dict: ``im`` (list of CUDA views into one 16-byte-aligned blob, in the panorama's dtype, [H, W, 3] or
+    [H, W]; the uint8 [H, W, 3] crops are valid ``PerspectiveFields.inference_batch`` input), ``up`` / ``lat`` (lists of float32
+    CUDA tensors: the reference's ``get_up`` / ``get_lat`` of each camera, ``lat`` in degrees), ``horizon`` (float64 [n, 2]) and
+    ``vvp`` (float64 [n, 3]; ``(inf, inf, nan)`` for a view at elevation 0, where the reference returns ``(inf, inf)``) as host
+    arrays."""
+    return _equi_views(equi_img, views, outputs, mode, img_format, False, device)
+
+
 class PanoCam:
-    """The field-synthesis static methods of ``perspective2d.utils.panocam.PanoCam`` (same signatures)."""
+    """``perspective2d.utils.panocam.PanoCam``: the panorama given as a path (``get_image``) and the static methods (same
+    signatures), except ``getGravityField`` / ``getAbsVVP``."""
+
+    def __init__(self, pano_path, device=None):
+        """Reads the panorama once (Pillow, converted to RGB as the reference's ``preprocess`` does) and keeps it on the CUDA
+        ``device`` (the reference re-reads the file on every ``get_image``)."""
+        from PIL import Image
+        self.pano_path = pano_path
+        with Image.open(pano_path) as im:
+            pano = np.array(im.convert("RGB"))
+        self.device = _pano_device(None, device)
+        self.pano = torch.from_numpy(pano).to(self.device)
+
+    def get_image(self, vfov=85, im_w=640, im_h=480, azimuth=0, elevation=30, roll=0, ar=4.0 / 3.0, img_format="RGB"):
+        """utils/panocam.py:132-194 -> (crop, horizon, vvp): the crop as a CUDA uint8 [im_h, im_w, 3] tensor in ``img_format``
+        order (the reference returns a PIL image for RGB and a numpy array for BGR), computed as the reference's ToTensor ->
+        sampler -> ToPILImage chain does; horizon and vvp are the reference's tuples."""
+        crop = _equi_views(self.pano, [(vfov, im_w, im_h, azimuth, elevation, roll, ar)], (), "bilinear", img_format, True, self.device)["im"][0]
+        horizon, vvp = horizon_vvp(vfov, im_w, im_h, elevation, roll)
+        return crop, horizon, vvp
+
+    @staticmethod
+    def crop_equi(equi_img, vfov, im_w, im_h, azimuth, elevation, roll, ar, mode):
+        """utils/panocam.py:196-249 -> CUDA tensor in the panorama's dtype, [im_h, im_w, 3] or [im_h, im_w] (degrees in)."""
+        return crop_equi_views(equi_img, [(vfov, im_w, im_h, azimuth, elevation, roll, ar)], (), mode)["im"][0]
+
+    @staticmethod
+    def getRelativeVVP(elevation, roll, vfov, im_h, im_w):
+        """utils/panocam.py:302-333 (radians): the vertical vanishing point over the image size and whether the up vectors point
+        to it (+1) or away (-1); the 2-tuple (inf, inf) at elevation 0."""
+        if elevation == 0:
+            return np.inf, np.inf
+        te, tv = np.tan(elevation), np.tan(vfov / 2)
+        vx = 0.5 - 0.5 / im_w - 0.5 * np.sin(roll) / te / tv * im_h / im_w
+        vy = 0.5 - 0.5 / im_h - 0.5 * np.cos(roll) / te / tv
+        return vx, vy, np.sign(elevation)
+
+    @staticmethod
+    def getRelativeHorizonLineFromAngles(elevation, roll, vfov, im_h, im_w):
+        """utils/panocam.py:335-351 (radians): the horizon's heights at the left and right image borders over the image height."""
+        mid = PanoCam.getMidpointFromAngle(elevation, roll, vfov)
+        dh = PanoCam.getDeltaHeightFromRoll(roll, im_h, im_w)
+        return mid - dh, mid + dh
+
+    @staticmethod
+    def getMidpointFromAngle(elevation, roll, vfov):
+        """utils/panocam.py:353-367 (radians): the horizon's height at the image centre over the image height; inf * sign at ±pi/2."""
+        if elevation in (np.pi / 2, -np.pi / 2):
+            return np.inf * np.sign(elevation)
+        return 0.5 + 0.5 * np.tan(elevation) / np.cos(roll) / np.tan(vfov / 2)
+
+    @staticmethod
+    def getDeltaHeightFromRoll(roll, im_h, im_w):
+        """utils/panocam.py:369-382 (radians): half the horizon's height change across the image over the image height; inf * sign
+        at ±pi/2."""
+        if roll in (np.pi / 2, -np.pi / 2):
+            return np.inf * np.sign(roll)
+        return -im_w / im_h * np.tan(roll) / 2
 
     @staticmethod
     def crop_distortion(image360, f, xi, H, W, az, el, roll, device=None):
@@ -238,7 +426,7 @@ class PanoCam:
 def far_vanishing_point(im_w, im_h, roll):
     """utils/panocam.py:288-300, :336-382 at elevation 0 (getRelativeVVP returns inf there): the point 1e8 px away along the
     horizon's normal, in pixel-centre coordinates (the reference's pixel-index point + 0.5).  float64."""
-    dh = math.inf * np.sign(roll) if roll in (math.pi / 2, -math.pi / 2) else -im_w / im_h * np.tan(roll) / 2
+    dh = PanoCam.getDeltaHeightFromRoll(roll, im_h, im_w)
     d = np.array([im_h * ((0.5 + dh) - (0.5 - dh)), -im_w], np.float64)
     norm = np.sqrt(d @ d)
     if norm >= 10 * np.finfo(np.float64).eps:                # sklearn's normalize leaves (near-)zero rows unscaled
