@@ -230,6 +230,48 @@ typedef struct pf_draw_canvas {
 int pf_draw_fields(int device, const pf_draw_canvas* canvases, int n, const uint8_t* img, uint8_t* out, const float* lat, const float* up,
                    void* stream);
 
+/* ---- scoring against ground-truth perspective fields (csrc/metrics.cuh) -------------------------------------------------
+ * Targets of the heads' losses from ground-truth fields at one size H x W, for n images.  up: DEVICE float32 (x, y) vectors
+ * at up + b*s[0] + y*s[1] + x*s[2] (+ s[3] for y), up_stride = s (elements); lat: DEVICE float32 at lat + b*t[0] + y*t[1] + x*t[2],
+ * degrees (lat_rad 0) or radians (1).  Either may be NULL (that output is skipped).
+ *   gravity_classes 2: gt_gravity = float32 [n, 2, H, W] copy of the up field; >= 3: int64 [n, H, W] labels of
+ *     encode_bin(up, gravity_classes) (utils/utils.py:94-111).
+ *   latitude_classes 1: gt_latitude = float32 [n, 1, H, W] sin(latitude); >= 2: int64 [n, H, W] labels of
+ *     encode_bin_latitude(latitude in degrees, latitude_classes) (utils/utils.py:133-146). */
+int pf_encode_fields(int device, int n, int H, int W, const float* up, const int64_t* up_stride, const float* lat, const int64_t* lat_stride,
+                     int lat_rad, int gravity_classes, int latitude_classes, void* gt_gravity, void* gt_latitude, void* stream);
+/* The heads' losses dicts (persformer_heads.py:60-70) over a batch of n predictions at H x W, into DEVICE float32 losses:
+ *   regression (2 / 1): pred_gravity / gt_gravity float32 [n, 2, H, W], pred_latitude / gt_latitude [n, 1, H, W] ->
+ *     losses[4] = gravity-msg-normal-loss, gravity-l2-loss, latitude-msg-normal-loss, latitude-l2-loss (gravity_head.py:204-218,
+ *     latitude_head.py:225-237);
+ *   classification (>= 3 / >= 2): logits float32 [n, C, H, W] (16-byte aligned, H * W % 4 == 0), labels int64 [n, H, W] ->
+ *     losses[2] = loss_gravity, loss_latitude (cross-entropy, mean over the labels that are not the head's ignore value).
+ * Every value is multiplied by its head's weight.  A mean over no pixel is NaN, and so is a cross-entropy with a label outside
+ * [0, C) that is not the ignore value.  workspace: DEVICE, 256-byte aligned, pf_head_losses_workspace bytes. */
+int64_t pf_head_losses_workspace(int n, int H, int W, int gravity_classes, int latitude_classes);
+int pf_head_losses(int device, int n, int H, int W, int gravity_classes, const float* pred_gravity, const void* gt_gravity, int latitude_classes,
+                   const float* pred_latitude, const void* gt_latitude, int gravity_ignore, int latitude_ignore, float gravity_weight,
+                   float latitude_weight, float* losses, void* workspace, int64_t workspace_bytes, void* stream);
+/* Per-image errors of predicted fields at the original sizes (DESIGN.md section 1).  Offsets and strides are in elements
+ * relative to the base pointers (mask: bytes; -1 = no mask); latitudes are [H, W] row-major, the mask uint8 [H, W]. */
+typedef struct pf_field_image {
+  int32_t height, width;
+  int64_t pred_up_offset, pred_up_stride[3];   /* row, column, component */
+  int64_t pred_lat_offset;                     /* degrees */
+  int64_t gt_up_offset, gt_up_stride[3];
+  int64_t gt_lat_offset;                       /* degrees or radians (lat_rad) */
+  int64_t mask_offset;
+} pf_field_image;
+/* Outputs (DEVICE), field f = 0 (up, degrees between vectors) or 1 (latitude, absolute difference in degrees) of image i at
+ * f * n + i: count int64, mean and median float64 (NaN for count 0), fraction float64 [2, n, n_thresholds] of valid pixels with
+ * an error below each threshold (at most 8).  up_maps / lat_maps: DEVICE float32 blobs of the per-pixel errors (images one
+ * after the other, NaN at invalid pixels), or both NULL.  workspace: DEVICE, 256-byte aligned, pf_field_errors_workspace bytes. */
+int64_t pf_field_errors_workspace(const pf_field_image* images, int n, int with_maps);
+int pf_field_errors(int device, const pf_field_image* images, int n, const float* pred_up, const float* pred_lat, const float* gt_up,
+                    const float* gt_lat, const uint8_t* mask, int lat_rad, const double* thresholds, int n_thresholds, float* up_maps,
+                    float* lat_maps, int64_t* count, double* mean, double* median, double* fraction, void* workspace,
+                    int64_t workspace_bytes, void* stream);
+
 /* ---- multi-GPU gather of results (SURVEY.md 8e: one process per GPU; NCCL point-to-point over NVLink) ---------------------
  * inference_batch shards its list over the ranks; the per-image results live on each rank's device and are gathered to ONE
  * rank with grouped ncclSend / ncclRecv enqueued on the caller's stream (so that the gather of micro-batch k overlaps the

@@ -45,6 +45,13 @@ class pf_equi_view(ctypes.Structure):
                 ("elevation", ctypes.c_double), ("roll", ctypes.c_double), ("ar", ctypes.c_double), ("offset", ctypes.c_int64)]
 
 
+class pf_field_image(ctypes.Structure):
+    """include/pf_b200.h: struct pf_field_image (one image of pf_field_errors)."""
+    _fields_ = [("height", ctypes.c_int32), ("width", ctypes.c_int32), ("pred_up_offset", ctypes.c_int64), ("pred_up_stride", ctypes.c_int64 * 3),
+                ("pred_lat_offset", ctypes.c_int64), ("gt_up_offset", ctypes.c_int64), ("gt_up_stride", ctypes.c_int64 * 3),
+                ("gt_lat_offset", ctypes.c_int64), ("mask_offset", ctypes.c_int64)]
+
+
 PF_EQUI_U8, PF_EQUI_F32 = 0, 1
 PF_EQUI_BILINEAR, PF_EQUI_NEAREST = 0, 1
 PF_EQUI_CAST, PF_EQUI_UNIT = 0, 1
@@ -166,6 +173,12 @@ def lib():
         "pf_draw_fields": (i32, [i32, ctypes.POINTER(pf_draw_canvas), i32, vp, vp, vp, vp, vp]),
         "pf_pano_views": (i32, [i32, vp, i32, i32, ctypes.POINTER(pf_pano_view), i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
         "pf_equi_views": (i32, [i32, vp, i32, i32, i32, i32, ctypes.POINTER(pf_equi_view), i32, i32, i32, i32, vp, vp]),
+        "pf_encode_fields": (i32, [i32, i32, i32, i32, vp, ctypes.POINTER(i64), vp, ctypes.POINTER(i64), i32, i32, i32, vp, vp, vp]),
+        "pf_head_losses_workspace": (i64, [i32, i32, i32, i32, i32]),
+        "pf_head_losses": (i32, [i32, i32, i32, i32, i32, vp, vp, i32, vp, vp, i32, i32, f32, f32, vp, vp, i64, vp]),
+        "pf_field_errors_workspace": (i64, [ctypes.POINTER(pf_field_image), i32, i32]),
+        "pf_field_errors": (i32, [i32, ctypes.POINTER(pf_field_image), i32, vp, vp, vp, vp, vp, i32, ctypes.POINTER(ctypes.c_double), i32,
+                                  vp, vp, vp, vp, vp, vp, vp, i64, vp]),
         "pf_op_layernorm": (i32, [vp, vp, i64, i32, vp, vp, f32, vp]),
         "pf_op_attention": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
         "pf_op_attention_mma": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
@@ -213,7 +226,8 @@ def lib():
 EXPORTS = ["pf_abi_version", "pf_last_error", "pf_kernel_launch_count", "pf_create", "pf_create_sized", "pf_destroy", "pf_set_weight",
            "pf_finalize", "pf_workspace_bytes", "pf_forward", "pf_profile_enable", "pf_profile_read", "pf_profile_kernels_enable",
            "pf_profile_kernels_read", "pf_set_option", "pf_debug_enable", "pf_debug_count", "pf_debug_name", "pf_debug_numel",
-           "pf_debug_copy", "pf_camera_fields", "pf_camera_fields_vp", "pf_pano_views", "pf_equi_views", "pf_draw_fields", "pf_comm_unique_id", "pf_comm_create", "pf_comm_destroy", "pf_gather",
+           "pf_debug_copy", "pf_camera_fields", "pf_camera_fields_vp", "pf_pano_views", "pf_equi_views", "pf_draw_fields",
+           "pf_encode_fields", "pf_head_losses_workspace", "pf_head_losses", "pf_field_errors_workspace", "pf_field_errors", "pf_comm_unique_id", "pf_comm_create", "pf_comm_destroy", "pf_gather",
            "pf_jpeg_create", "pf_jpeg_destroy", "pf_jpeg_info", "pf_jpeg_decode_batch",
            "pf_op_conv_gemm", "pf_op_tma", "pf_op_tma_bf16", "pf_op_conv1_ring", "pf_tma_pick_tile", "pf_op_layernorm", "pf_op_attention",
            "pf_op_attention_mma", "pf_op_attention_tc", "pf_op_attention_tc_bf16", "pf_op_attention_tc_keys", "pf_op_dwconv3x3_gelu",

@@ -880,6 +880,11 @@ __global__ void __launch_bounds__(256) conv1_ring_kernel(const __nv_bfloat16* __
 }
 constexpr int kRingSmem = (128 * kRingPx + 2 * 64 * 32) * 4;
 
+// Bin widths in degrees of the gravity (NC - 1 angle bins plus the "no direction" bin NC - 1) and latitude classes, shared by
+// the decoders below and the encoders of metrics.cuh (utils/utils.py:94-162).
+__host__ __device__ __forceinline__ float gravity_bin_deg(int NC) { return 360.0f / (float)(NC - 1); }
+__host__ __device__ __forceinline__ float latitude_bin_deg(int NC) { return 180.0f / (float)NC; }
+
 // Bin decode shared by the two classification kernels (utils/utils.py:114-130 and :148-162).
 __device__ __forceinline__ void decode_bin_store(float* __restrict__ field, int b, int r, int HW, int NC, int bi, int is_gravity) {
   if (is_gravity) {
@@ -888,11 +893,11 @@ __device__ __forceinline__ void decode_bin_store(float* __restrict__ field, int 
     float* o = field + (long long)b * 2 * HW + r;
     if (bi == NC - 1) { o[0] = 0.f; o[HW] = 0.f; }
     else {
-      const float ang = ((float)bi * (360.0f / (float)(NC - 1)) - 180.0f) / 180.0f * 3.14159265358979323846f;
+      const float ang = ((float)bi * gravity_bin_deg(NC) - 180.0f) / 180.0f * 3.14159265358979323846f;
       o[0] = cosf(ang); o[HW] = sinf(ang);
     }
   } else {
-    const float bin = 180.0f / (float)NC;
+    const float bin = latitude_bin_deg(NC);
     field[(long long)b * HW + r] = (-90.0f + (float)bi * bin) + bin * 0.5f;
   }
 }

@@ -28,6 +28,7 @@
 #include "pano.cuh"
 #include "equi.cuh"
 #include "draw.cuh"
+#include "metrics.cuh"
 #include "comm.cuh"
 #include "jpeg.cuh"
 
@@ -1715,6 +1716,162 @@ int pf_draw_fields(int device, const pf_draw_canvas* cs, int n, const uint8_t* i
     const dim3 grid((unsigned)max_tiles, (unsigned)cnt);
     LAUNCHED((draw_fields_kernel<<<grid, kDrawThreads, 0, (cudaStream_t)stream>>>(b, st, img, out, lat, up), cudaGetLastError()));
   }
+  return PF_OK;
+}
+
+// ----------------------------------------------------------------------------------------------- scoring (metrics.cuh)
+static bool gravity_classes_ok(int c) { return c == 2 || c >= 3; }
+static bool latitude_classes_ok(int c) { return c >= 1; }
+static long long align256(long long b) { return (b + 255) / 256 * 256; }
+
+int pf_encode_fields(int device, int n, int H, int W, const float* up, const int64_t* up_stride, const float* lat, const int64_t* lat_stride,
+                     int lat_rad, int gravity_classes, int latitude_classes, void* gt_gravity, void* gt_latitude, void* stream) {
+  if (n < 1 || H < 1 || W < 1 || (long long)n * H * W >= (1LL << 40)) return fail(PF_ERR_ARG, "pf_encode_fields: bad batch %d x %d x %d", n, H, W);
+  if (!up && !lat) return fail(PF_ERR_ARG, "pf_encode_fields: neither an up nor a latitude field");
+  if (up && (!up_stride || !gt_gravity || !gravity_classes_ok(gravity_classes)))
+    return fail(PF_ERR_ARG, "pf_encode_fields: the up field needs strides, an output and gravity_classes 2 or >= 3 (got %d)", gravity_classes);
+  if (lat && (!lat_stride || !gt_latitude || !latitude_classes_ok(latitude_classes)))
+    return fail(PF_ERR_ARG, "pf_encode_fields: the latitude field needs strides, an output and latitude_classes >= 1 (got %d)", latitude_classes);
+  if (lat_rad != 0 && lat_rad != 1) return fail(PF_ERR_ARG, "pf_encode_fields: lat_rad must be 0 or 1");
+  EncodeArgs a{};
+  a.n = n; a.H = H; a.W = W; a.up = up; a.lat = lat; a.lat_rad = lat_rad; a.gc = gravity_classes; a.lc = latitude_classes;
+  a.gt_g = gt_gravity; a.gt_l = gt_latitude;
+  if (up) { a.us_img = up_stride[0]; a.us_row = up_stride[1]; a.us_col = up_stride[2]; a.us_comp = up_stride[3]; }
+  if (lat) { a.ls_img = lat_stride[0]; a.ls_row = lat_stride[1]; a.ls_col = lat_stride[2]; }
+  CU(cudaSetDevice(device));
+  const long long px = (long long)n * H * W;
+  LAUNCHED((encode_fields_kernel<<<(unsigned)cdivl(px, kMetThreads), kMetThreads, 0, (cudaStream_t)stream>>>(a), cudaGetLastError()));
+  return PF_OK;
+}
+
+// Blocks of the loss passes: classification (gravity, latitude) or regression (one pass over both heads)
+static void loss_blocks(int n, int H, int W, int gc, long long* bg, long long* bl) {
+  const long long px = (long long)n * H * W;
+  if (gc == 2) { *bg = cdivl(px, (long long)kMetThreads * kRegPix); *bl = 0; }
+  else { *bg = cdivl(px / kCePix, kMetThreads); *bl = *bg; }
+}
+int64_t pf_head_losses_workspace(int n, int H, int W, int gravity_classes, int latitude_classes) {
+  if (n < 1 || H < 1 || W < 1) return fail(PF_ERR_ARG, "pf_head_losses_workspace: bad batch %d x %d x %d", n, H, W);
+  if (!((gravity_classes == 2 && latitude_classes == 1) || (gravity_classes >= 3 && latitude_classes >= 2)))
+    return fail(PF_ERR_ARG, "pf_head_losses_workspace: heads %d / %d: both regression (2 / 1) or both classification", gravity_classes, latitude_classes);
+  long long bg, bl;
+  loss_blocks(n, H, W, gravity_classes, &bg, &bl);
+  return gravity_classes == 2 ? align256(bg * kRegSums * 8) + align256(bg * kRegCounts * 8) : align256((bg + bl) * 8) * 2;
+}
+
+int pf_head_losses(int device, int n, int H, int W, int gravity_classes, const float* pred_gravity, const void* gt_gravity, int latitude_classes,
+                   const float* pred_latitude, const void* gt_latitude, int gravity_ignore, int latitude_ignore, float gravity_weight,
+                   float latitude_weight, float* losses, void* workspace, int64_t workspace_bytes, void* stream) {
+  const int64_t need = pf_head_losses_workspace(n, H, W, gravity_classes, latitude_classes);
+  if (need < 0) return (int)need;
+  if (!pred_gravity || !gt_gravity || !pred_latitude || !gt_latitude || !losses || !workspace)
+    return fail(PF_ERR_ARG, "pf_head_losses: null prediction / target / losses / workspace");
+  if (workspace_bytes < need) return fail(PF_ERR_WORKSPACE, "pf_head_losses: workspace %lld B < required %lld B", (long long)workspace_bytes, (long long)need);
+  if (((uintptr_t)workspace & 255) != 0) return fail(PF_ERR_ARG, "pf_head_losses: workspace must be 256-byte aligned");
+  const bool cls = gravity_classes != 2;
+  if (cls && (((long long)H * W) % kCePix != 0 || ((uintptr_t)pred_gravity & 15) || ((uintptr_t)pred_latitude & 15)))
+    return fail(PF_ERR_ARG, "pf_head_losses: classification logits need H * W %% 4 == 0 and 16-byte aligned planes");
+  if (cls && ((long long)latitude_classes * H * W >= (1LL << 40))) return fail(PF_ERR_ARG, "pf_head_losses: logits too large");
+  CU(cudaSetDevice(device));
+  cudaStream_t st = (cudaStream_t)stream;
+  long long bg, bl;
+  loss_blocks(n, H, W, gravity_classes, &bg, &bl);
+  double* psum = (double*)workspace;
+  const int HW = H * W;
+  if (cls) {
+    long long* pcnt = (long long*)((char*)workspace + align256((bg + bl) * 8));
+    const CeHead g{pred_gravity, (const long long*)gt_gravity, gravity_classes, gravity_ignore, (int)bg};
+    const CeHead l{pred_latitude, (const long long*)gt_latitude, latitude_classes, latitude_ignore, (int)bl};
+    LAUNCHED((cross_entropy_kernel<<<(unsigned)(bg + bl), kMetThreads, 0, st>>>(g, l, n, HW, psum, pcnt), cudaGetLastError()));
+    LAUNCHED((loss_finish_kernel<<<1, kMetThreads, 0, st>>>(0, (int)bg, (int)(bg + bl), psum, pcnt, 0, gravity_weight, latitude_weight, losses),
+              cudaGetLastError()));
+  } else {
+    long long* pcnt = (long long*)((char*)workspace + align256(bg * kRegSums * 8));
+    const RegArgs a{pred_gravity, (const float*)gt_gravity, pred_latitude, (const float*)gt_latitude, n, H, W};
+    LAUNCHED((regression_loss_kernel<<<(unsigned)bg, kMetThreads, 0, st>>>(a, (int)bg, psum, pcnt), cudaGetLastError()));
+    LAUNCHED((loss_finish_kernel<<<1, kMetThreads, 0, st>>>(1, (int)bg, (int)bg, psum, pcnt, (long long)n * HW, gravity_weight, latitude_weight, losses),
+              cudaGetLastError()));
+  }
+  return PF_OK;
+}
+
+// Workspace layout of pf_field_errors: device descriptors | fp64 sums [2][blocks] | counts [2][1 + 8][blocks] | maps if not given
+struct FeLayout { long long blocks, pixels, desc, psum, pcnt, maps, total; };
+static int field_errors_layout(const pf_field_image* im, int n, int with_maps, FeLayout* lay) {
+  if (!im || n < 1) return fail(PF_ERR_ARG, "pf_field_errors: null images or n < 1");
+  long long blocks = 0, pixels = 0;
+  for (int i = 0; i < n; ++i) {
+    if (im[i].height < 1 || im[i].width < 1 || (long long)im[i].height * im[i].width >= (1LL << 31))
+      return fail(PF_ERR_ARG, "pf_field_errors: image %d has size %dx%d", i, im[i].height, im[i].width);
+    const long long hw = (long long)im[i].height * im[i].width;
+    blocks += cdivl(hw, kFeTile);
+    pixels += hw;
+  }
+  if (blocks >= (1LL << 31)) return fail(PF_ERR_ARG, "pf_field_errors: too many pixels");
+  lay->blocks = blocks; lay->pixels = pixels;
+  lay->desc = 0;
+  lay->psum = align256((long long)n * sizeof(FeImage));
+  lay->pcnt = lay->psum + align256(2 * blocks * 8);
+  lay->maps = lay->pcnt + align256(2LL * (1 + kFeMaxThr) * blocks * 4);
+  lay->total = lay->maps + (with_maps ? 0 : align256(2 * pixels * 4));
+  return PF_OK;
+}
+int64_t pf_field_errors_workspace(const pf_field_image* images, int n, int with_maps) {
+  FeLayout lay;
+  TRY(field_errors_layout(images, n, with_maps, &lay));
+  return lay.total;
+}
+
+int pf_field_errors(int device, const pf_field_image* images, int n, const float* pred_up, const float* pred_lat, const float* gt_up,
+                    const float* gt_lat, const uint8_t* mask, int lat_rad, const double* thresholds, int n_thresholds, float* up_maps,
+                    float* lat_maps, int64_t* count, double* mean, double* median, double* fraction, void* workspace,
+                    int64_t workspace_bytes, void* stream) {
+  if ((up_maps == nullptr) != (lat_maps == nullptr)) return fail(PF_ERR_ARG, "pf_field_errors: give both maps or neither");
+  FeLayout lay;
+  TRY(field_errors_layout(images, n, up_maps != nullptr, &lay));
+  if (!pred_up || !pred_lat || !gt_up || !gt_lat || !count || !mean || !median || !workspace)
+    return fail(PF_ERR_ARG, "pf_field_errors: null field / output / workspace");
+  if (n_thresholds < 0 || n_thresholds > kFeMaxThr || (n_thresholds > 0 && (!thresholds || !fraction)))
+    return fail(PF_ERR_ARG, "pf_field_errors: %d thresholds (0 to %d, with a fraction output)", n_thresholds, kFeMaxThr);
+  for (int k = 0; k < n_thresholds; ++k)
+    if (std::isnan(thresholds[k])) return fail(PF_ERR_ARG, "pf_field_errors: threshold %d is NaN", k);
+  if (lat_rad != 0 && lat_rad != 1) return fail(PF_ERR_ARG, "pf_field_errors: lat_rad must be 0 or 1");
+  if (workspace_bytes < lay.total) return fail(PF_ERR_WORKSPACE, "pf_field_errors: workspace %lld B < required %lld B", (long long)workspace_bytes, lay.total);
+  if (((uintptr_t)workspace & 255) != 0) return fail(PF_ERR_ARG, "pf_field_errors: workspace must be 256-byte aligned");
+  std::vector<FeImage> d(n);
+  long long block0 = 0, map_off = 0;
+  for (int i = 0; i < n; ++i) {
+    const pf_field_image& c = images[i];
+    if (c.pred_up_offset < 0 || c.pred_lat_offset < 0 || c.gt_up_offset < 0 || c.gt_lat_offset < 0 || c.mask_offset < -1)
+      return fail(PF_ERR_ARG, "pf_field_errors: image %d has a negative offset", i);
+    if (c.mask_offset >= 0 && !mask) return fail(PF_ERR_ARG, "pf_field_errors: image %d has a mask offset but mask is NULL", i);
+    FeImage& o = d[i];
+    o.H = c.height; o.W = c.width;
+    o.pu_off = c.pred_up_offset; o.pu_sr = c.pred_up_stride[0]; o.pu_sc = c.pred_up_stride[1]; o.pu_sk = c.pred_up_stride[2];
+    o.pl_off = c.pred_lat_offset;
+    o.gu_off = c.gt_up_offset; o.gu_sr = c.gt_up_stride[0]; o.gu_sc = c.gt_up_stride[1]; o.gu_sk = c.gt_up_stride[2];
+    o.gl_off = c.gt_lat_offset;
+    o.mask_off = c.mask_offset;
+    o.map_off = map_off;
+    const long long hw = (long long)c.height * c.width;
+    o.block0 = (int)block0; o.nblk = (int)cdivl(hw, kFeTile);
+    block0 += o.nblk; map_off += hw;
+  }
+  CU(cudaSetDevice(device));
+  cudaStream_t st = (cudaStream_t)stream;
+  char* ws = (char*)workspace;
+  FeArgs a{};
+  a.im = (const FeImage*)(ws + lay.desc); a.n = n; a.nblocks = (int)lay.blocks;
+  a.pu = pred_up; a.pl = pred_lat; a.gu = gt_up; a.gl = gt_lat; a.mask = mask;
+  a.lat_rad = lat_rad; a.T = n_thresholds;
+  for (int k = 0; k < n_thresholds; ++k) a.thr[k] = thresholds[k];
+  a.map_up = up_maps ? up_maps : (float*)(ws + lay.maps);
+  a.map_lat = lat_maps ? lat_maps : (float*)(ws + lay.maps) + lay.pixels;
+  a.psum = (double*)(ws + lay.psum); a.pcnt = (int*)(ws + lay.pcnt);
+  CU(cudaMemcpyAsync(ws + lay.desc, d.data(), n * sizeof(FeImage), cudaMemcpyHostToDevice, st));
+  LAUNCHED((field_errors_kernel<<<(unsigned)lay.blocks, kMetThreads, 0, st>>>(a), cudaGetLastError()));
+  const FeOut o{(long long*)count, mean, median, fraction};
+  LAUNCHED((field_stats_kernel<<<dim3((unsigned)n, 2), kFeSelThreads, 0, st>>>(a, o), cudaGetLastError()));
   return PF_OK;
 }
 

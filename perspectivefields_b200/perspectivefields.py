@@ -533,6 +533,91 @@ class PerspectiveFields(nn.Module):
             res.append(d)
         return res
 
+    # ------------------------------------------------------------------------------------------ scoring API
+    def _scoring_device(self):
+        dev = self.device
+        if dev.type != "cuda":
+            raise RuntimeError("perspectivefields_b200 has no CPU path: move the model to an H100 with .cuda() first")
+        return torch.device("cuda", torch.cuda.current_device()) if dev.index is None else dev
+
+    def targets_from_fields(self, up, lat, lat_mode="deg"):
+        """Ground-truth fields -> the reference's targets dict ``{"gt_gravity", "gt_latitude"}`` (persformer_heads.py:60-70) for
+        ``losses``.  ``up``: list of float32 CUDA [H, W, 2] up fields, ``lat``: list of [H, W] latitude maps (``lat_mode`` "deg"
+        as ``camera_fields`` / ``crop_equi_views`` return them, or "rad" as ``crop_distortion_views`` does), all at the working
+        size.  One launch for the whole list; the rule (this project's, the inverse of the inference decode, DESIGN.md section 1):
+        regression gravity ``[n, 2, H, W]`` (the (x, y) components), regression latitude ``sin(lat)`` ``[n, 1, H, W]``;
+        classification ``metrics.encode_bin`` / ``metrics.encode_bin_latitude`` labels, int64 ``[n, H, W]``."""
+        from . import metrics
+
+        lat_rad = metrics._lat_rad(lat_mode)
+        n = len(up)
+        if n == 0 or len(lat) != n:
+            raise ValueError(f"targets_from_fields needs as many latitude maps as up fields (>= 1), got {len(up)} and {len(lat)}")
+        dev = self._scoring_device()
+        h, w = self._net_hw
+        for i in range(n):
+            metrics._cuda_f32(up[i], f"up[{i}]", dev)
+            metrics._cuda_f32(lat[i], f"lat[{i}]", dev)
+            if tuple(up[i].shape) != (h, w, 2) or tuple(lat[i].shape) != (h, w):
+                raise ValueError(f"field {i}: up {list(up[i].shape)} / lat {list(lat[i].shape)}; the working size needs [{h}, {w}, 2] / [{h}, {w}]")
+        u, la = metrics.batch_view(list(up)), metrics.batch_view(list(lat))
+        s = u.stride()
+        gc, lc = self._variant["gravity_classes"], self._variant["latitude_classes"]
+        gg, gl = metrics.encode_fields((u, s, h, w), (la, la.stride(), h, w), gc, lc, lat_rad)
+        return {"gt_gravity": gg, "gt_latitude": gl}
+
+    def losses(self, results, targets):
+        """What ``StandardPersformerHeads`` puts into its losses dict (persformer_heads.py:60-70, gravity_head.py:199-235,
+        latitude_head.py:221-254) for ``inference_batch`` results and ``targets_from_fields`` targets, over the whole list:
+        regression ``gravity-msg-normal-loss``, ``gravity-l2-loss``, ``latitude-msg-normal-loss``, ``latitude-l2-loss``;
+        classification ``loss_gravity``, ``loss_latitude``; weights and ignore values from ``cfg``.  Values are 0-dim float32 CUDA
+        tensors and nothing synchronises.  Where the reference would stop in ``pdb`` (a mean over no pixel) the value is NaN, as
+        it is for a class label outside [0, C) that is not the ignore value.  The ``pred_*`` tensors of one ``inference_batch``
+        call are rows of one buffer and are read in place; other lists are stacked once."""
+        from . import metrics
+
+        if self._options.get("decode_only", 0):
+            raise ValueError("losses needs the logits, which a model built with logits=False does not return")
+        n = len(results)
+        if n == 0:
+            raise ValueError("no results")
+        dev = self._scoring_device()
+        h, w = self._net_hw
+        gc, lc = self._variant["gravity_classes"], self._variant["latitude_classes"]
+        preds = []
+        for key, c in (("pred_gravity", gc), ("pred_latitude", lc)):
+            ts = [metrics._cuda_f32(r[key], f"results[{i}][{key!r}]", dev) for i, r in enumerate(results)]
+            for i, t in enumerate(ts):
+                if tuple(t.shape) != (c, h, w):
+                    raise ValueError(f"results[{i}][{key!r}] is {list(t.shape)}, the model's is [{c}, {h}, {w}]")
+            p = metrics.batch_view(ts)
+            if not p.is_contiguous() or p.data_ptr() % 16:
+                p = torch.stack(ts)
+            preds.append(p)
+        tg = []
+        for key, c in (("gt_gravity", gc), ("gt_latitude", lc)):
+            t = targets[key]
+            reg = c <= 2
+            shape, dtype = ((n, c, h, w), torch.float32) if reg else ((n, h, w), torch.int64)
+            if not isinstance(t, torch.Tensor) or t.dtype != dtype or tuple(t.shape) != shape or t.device != dev:
+                got = f"{t.dtype} {list(t.shape)} on {t.device}" if isinstance(t, torch.Tensor) else type(t).__name__
+                raise ValueError(f"targets[{key!r}] must be {dtype} {list(shape)} on {dev}, got {got}")
+            tg.append(t.contiguous())
+        mc = self.cfg.MODEL
+        wg, wl = float(mc.GRAVITY_DECODER.LOSS_WEIGHT), float(mc.LATITUDE_DECODER.LOSS_WEIGHT)
+        ig, il = int(mc.GRAVITY_DECODER.IGNORE_VALUE), int(mc.LATITUDE_DECODER.IGNORE_VALUE)
+        L = _native.lib()
+        with torch.cuda.device(dev):
+            need = _native.check(L.pf_head_losses_workspace(n, h, w, gc, lc))
+            ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            keys = (("gravity-msg-normal-loss", "gravity-l2-loss", "latitude-msg-normal-loss", "latitude-l2-loss") if gc == 2
+                    else ("loss_gravity", "loss_latitude"))
+            out = torch.empty(len(keys), dtype=torch.float32, device=dev)
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            _native.check(L.pf_head_losses(dev.index, n, h, w, gc, preds[0].data_ptr(), tg[0].data_ptr(), lc, preds[1].data_ptr(),
+                                           tg[1].data_ptr(), ig, il, wg, wl, out.data_ptr(), ws.data_ptr(), ws.numel(), stream))
+        return dict(zip(keys, out.unbind(0)))
+
     def set_option(self, name, value):
         """Engine options (see pf_set_option in include/pf_b200.h), e.g. ``set_option("pdl", 0)``."""
         eng = self._get_engine()
