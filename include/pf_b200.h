@@ -272,6 +272,30 @@ int pf_field_errors(int device, const pf_field_image* images, int n, const float
                     float* lat_maps, int64_t* count, double* mean, double* median, double* fraction, void* workspace,
                     int64_t workspace_bytes, void* stream);
 
+/* ---- camera parameters from perspective fields (csrc/calib.cuh) ------------------------------------------------------------
+ * A Levenberg-Marquardt fit of roll, pitch, f_rel and (principal_point != 0) cx_rel, cy_rel to predicted fields, one camera
+ * per image (DESIGN.md section 1, "Camera fit").  Offsets and strides are in elements relative to the base pointers (mask:
+ * bytes; -1 = no mask).  up: float32 (x, y) vectors at up_base + up_offset + y*s[0] + x*s[1] (+ s[2] for y), so [2, H, W]
+ * predictions and [H, W, 2] camera fields are read in place; lat: float32 [H, W] row-major, degrees; mask: uint8 [H, W].
+ * init: the start (roll, pitch in radians, f_rel > 0, cx_rel, cy_rel; the last two are ignored without principal_point), or a
+ * NaN roll for the closed-form start from the fields. */
+typedef struct pf_fit_image {
+  int32_t height, width;                       /* >= 3 each */
+  int64_t up_offset, up_stride[3];             /* row, column, component */
+  int64_t lat_offset;
+  int64_t mask_offset;
+  double init[5];
+} pf_fit_image;
+/* Outputs (DEVICE), image i: params[5i .. 5i + 4] = roll (degrees, (-180, 180]), pitch (degrees, |pitch| <= 90), f_rel, cx_rel,
+ * cy_rel (0 without principal_point); cost[i] = 1/2 sum delta^2 rho((r / delta)^2) at them (huber = delta > 0: Huber's rho;
+ * huber = 0: least squares, rho(z) = z), with residuals in radians; iterations[i] = cost evaluations; status[i] = 0 converged,
+ * 1 stopped at max_iterations (1 .. 1000) evaluations, 2 fewer valid residuals than parameters (params and cost NaN).
+ * Enqueued on `stream` without synchronisation.  workspace: DEVICE, 256-byte aligned, pf_fit_camera_workspace bytes. */
+int64_t pf_fit_camera_workspace(const pf_fit_image* images, int n);
+int pf_fit_camera(int device, const pf_fit_image* images, int n, const float* up_base, const float* lat_base, const uint8_t* mask_base,
+                  int principal_point, double huber, int max_iterations, double* params, double* cost, int32_t* iterations,
+                  int32_t* status, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ---- multi-GPU gather of results (SURVEY.md 8e: one process per GPU; NCCL point-to-point over NVLink) ---------------------
  * inference_batch shards its list over the ranks; the per-image results live on each rank's device and are gathered to ONE
  * rank with grouped ncclSend / ncclRecv enqueued on the caller's stream (so that the gather of micro-batch k overlaps the

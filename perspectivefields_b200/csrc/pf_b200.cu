@@ -29,6 +29,7 @@
 #include "equi.cuh"
 #include "draw.cuh"
 #include "metrics.cuh"
+#include "calib.cuh"
 #include "comm.cuh"
 #include "jpeg.cuh"
 
@@ -1872,6 +1873,99 @@ int pf_field_errors(int device, const pf_field_image* images, int n, const float
   LAUNCHED((field_errors_kernel<<<(unsigned)lay.blocks, kMetThreads, 0, st>>>(a), cudaGetLastError()));
   const FeOut o{(long long*)count, mean, median, fraction};
   LAUNCHED((field_stats_kernel<<<dim3((unsigned)n, 2), kFeSelThreads, 0, st>>>(a, o), cudaGetLastError()));
+  return PF_OK;
+}
+
+// ----------------------------------------------------------------------------------------------- camera fit (calib.cuh)
+// Workspace layout of pf_fit_camera: device descriptors | per-image state | fp64 partials [kFitQ][pass blocks]
+constexpr int kFitMaxIterations = 1000;
+struct FitLayout { long long blocks, desc, state, part, total; };
+static int fit_layout(const pf_fit_image* im, int n, FitLayout* lay) {
+  if (!im || n < 1) return fail(PF_ERR_ARG, "pf_fit_camera: null images or n < 1");
+  long long blocks = 0;
+  for (int i = 0; i < n; ++i) {
+    if (im[i].height < 3 || im[i].width < 3 || (long long)im[i].height * im[i].width >= (1LL << 31))
+      return fail(PF_ERR_ARG, "pf_fit_camera: image %d has size %dx%d (3x3 at least)", i, im[i].height, im[i].width);
+    blocks += cdivl((long long)im[i].height * im[i].width, kFitTile);
+  }
+  if (blocks >= (1LL << 31)) return fail(PF_ERR_ARG, "pf_fit_camera: too many pixels");
+  lay->blocks = blocks;
+  lay->desc = 0;
+  lay->state = align256((long long)n * sizeof(FitImage));
+  lay->part = lay->state + align256((long long)n * sizeof(FitState));
+  lay->total = lay->part + align256((long long)kFitQ * blocks * 8);
+  return PF_OK;
+}
+int64_t pf_fit_camera_workspace(const pf_fit_image* images, int n) {
+  FitLayout lay;
+  TRY(fit_layout(images, n, &lay));
+  return lay.total;
+}
+
+// Enables programmatic dependent launch for the calling thread while alive (the fit's kernels wait on their predecessor with
+// griddepcontrol.wait before their first global access)
+struct PdlScope {
+  explicit PdlScope(bool on) { pdl_enabled() = on; }
+  ~PdlScope() { pdl_enabled() = false; }
+};
+
+int pf_fit_camera(int device, const pf_fit_image* images, int n, const float* up_base, const float* lat_base, const uint8_t* mask_base,
+                  int principal_point, double huber, int max_iterations, double* params, double* cost, int32_t* iterations,
+                  int32_t* status, void* workspace, int64_t workspace_bytes, void* stream) {
+  FitLayout lay;
+  TRY(fit_layout(images, n, &lay));
+  if (!up_base || !lat_base || !params || !cost || !iterations || !status || !workspace)
+    return fail(PF_ERR_ARG, "pf_fit_camera: null field / output / workspace");
+  if (principal_point != 0 && principal_point != 1) return fail(PF_ERR_ARG, "pf_fit_camera: principal_point must be 0 or 1");
+  if (!(huber == 0.0 || (std::isfinite(huber) && huber > 0.0)))
+    return fail(PF_ERR_ARG, "pf_fit_camera: huber must be 0 (least squares) or finite and > 0, got %g", huber);
+  if (max_iterations < 1 || max_iterations > kFitMaxIterations)
+    return fail(PF_ERR_ARG, "pf_fit_camera: max_iterations %d outside 1 .. %d", max_iterations, kFitMaxIterations);
+  if (workspace_bytes < lay.total) return fail(PF_ERR_WORKSPACE, "pf_fit_camera: workspace %lld B < required %lld B", (long long)workspace_bytes, lay.total);
+  if (((uintptr_t)workspace & 255) != 0) return fail(PF_ERR_ARG, "pf_fit_camera: workspace must be 256-byte aligned");
+  std::vector<FitImage> d(n);
+  long long block0 = 0;
+  for (int i = 0; i < n; ++i) {
+    const pf_fit_image& c = images[i];
+    if (c.up_offset < 0 || c.lat_offset < 0 || c.mask_offset < -1 || c.up_stride[0] < 0 || c.up_stride[1] < 0 || c.up_stride[2] < 0)
+      return fail(PF_ERR_ARG, "pf_fit_camera: image %d has a negative offset or stride", i);
+    if (c.mask_offset >= 0 && !mask_base) return fail(PF_ERR_ARG, "pf_fit_camera: image %d has a mask offset but mask_base is NULL", i);
+    if (!std::isnan(c.init[0])) {
+      bool fin = true;
+      for (int k = 0; k < 5; ++k) fin = fin && std::isfinite(c.init[k]);
+      if (!fin || !(c.init[2] > 0.0)) return fail(PF_ERR_ARG, "pf_fit_camera: image %d: init must be finite with f_rel > 0 (or a NaN roll)", i);
+    }
+    FitImage& o = d[i];
+    o.H = c.height; o.W = c.width;
+    o.up_off = c.up_offset; o.up_sr = c.up_stride[0]; o.up_sc = c.up_stride[1]; o.up_sk = c.up_stride[2];
+    o.lat_off = c.lat_offset;
+    o.mask_off = c.mask_offset;
+    for (int k = 0; k < 5; ++k) o.init[k] = c.init[k];
+    o.block0 = (int)block0; o.nblk = (int)cdivl((long long)c.height * c.width, kFitTile);
+    block0 += o.nblk;
+  }
+  CU(cudaSetDevice(device));
+  cudaStream_t st = (cudaStream_t)stream;
+  char* ws = (char*)workspace;
+  FitArgs a{};
+  a.im = (const FitImage*)(ws + lay.desc); a.st = (FitState*)(ws + lay.state); a.n = n; a.nblocks = (int)lay.blocks;
+  a.up = up_base; a.lat = lat_base; a.mask = mask_base;
+  a.huber = huber; a.max_iter = max_iterations;
+  a.part = (double*)(ws + lay.part);
+  a.params = params; a.cost = cost; a.iters = iterations; a.status = status;
+  CU(cudaMemcpyAsync(ws + lay.desc, d.data(), n * sizeof(FitImage), cudaMemcpyHostToDevice, st));
+  const PdlScope pdl(!sync_debug());
+  const dim3 pass_grid((unsigned)lay.blocks), step_grid((unsigned)cdiv(n, kFitStepWarps));
+  LAUNCHED(launch_pdl(fit_init_kernel, dim3(n), dim3(64), 0, st, a, principal_point));
+  for (int it = 0; it < max_iterations; ++it) {
+    if (principal_point) {
+      LAUNCHED(launch_pdl(fit_pass_kernel<5>, pass_grid, dim3(kFitThreads), 0, st, a));
+      LAUNCHED(launch_pdl(fit_step_kernel<5>, step_grid, dim3(32 * kFitStepWarps), 0, st, a));
+    } else {
+      LAUNCHED(launch_pdl(fit_pass_kernel<3>, pass_grid, dim3(kFitThreads), 0, st, a));
+      LAUNCHED(launch_pdl(fit_step_kernel<3>, step_grid, dim3(32 * kFitStepWarps), 0, st, a));
+    }
+  }
   return PF_OK;
 }
 

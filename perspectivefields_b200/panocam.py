@@ -24,6 +24,19 @@ import torch
 from . import _native
 
 
+def general_vfov(d_cx, d_cy, h, focal, degree):
+    """utils/utils.py:13-44: the general vertical field of view, the angle at the pinhole between the rays through the
+    midpoints of the image's top and bottom edges, for a principal point offset (d_cx, d_cy) from the centre.  Lengths relative
+    to the image height (h = 1) or in pixels (h = the height).  The inverse of ``general_vfov_to_focal``.  Scalars or numpy
+    arrays (float64), or torch tensors (computed with torch ops on their device, without synchronising)."""
+    xp = torch if any(isinstance(v, torch.Tensor) for v in (d_cx, d_cy, focal)) else np
+    p_sqr = focal ** 2 + d_cx ** 2 + (d_cy + 0.5 * h) ** 2
+    q_sqr = focal ** 2 + d_cx ** 2 + (d_cy - 0.5 * h) ** 2
+    cos_fov = (p_sqr + q_sqr - h ** 2) / 2 / xp.sqrt(p_sqr) / xp.sqrt(q_sqr)
+    fov = xp.arccos(cos_fov)
+    return xp.rad2deg(fov) if degree else fov
+
+
 def general_vfov_to_focal(rel_cx, rel_cy, h, gvfov, degree):
     """utils/utils.py:47-91 (SciPy ``fsolve`` there): relative focal length from the general vertical field of view, the
     angle between the rays through the top-centre and bottom-centre pixels, for an off-centre principal point.  Closed form
