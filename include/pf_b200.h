@@ -296,6 +296,33 @@ int pf_fit_camera(int device, const pf_fit_image* images, int n, const float* up
                   int principal_point, double huber, int max_iterations, double* params, double* cost, int32_t* iterations,
                   int32_t* status, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- upright warp: straightened images from camera parameters (csrc/rectify.cuh) --------------------------------------------
+ * Warps each uint8 image (1 or 3 channels, HWC) to a camera with roll 0, pitch 0 (or the input pitch with keep_pitch), a centred
+ * principal point and the focal length of enum pf_rectify_focal, by the rule of DESIGN.md section 1 ("Upright warp").  Offsets are
+ * relative to the base pointers: bytes for the images and the mask, floats for the map; -1 skips that image's mask / map. */
+typedef struct pf_rectify_image {
+  int32_t height, width;            /* input size */
+  int32_t out_height, out_width;    /* output size */
+  int64_t in_offset;                /* bytes of the [height, width, channels] input in in_base */
+  int64_t out_offset;               /* bytes of the [out_height, out_width, channels] output in out_base */
+  int64_t mask_offset;              /* bytes of the uint8 [out_height, out_width] mask (1: sampled, 0: fill) in mask_base, or -1 */
+  int64_t map_offset;               /* floats of the float32 [out_height, out_width, 2] input positions in map_base, or -1 */
+} pf_rectify_image;
+/* PF_RECTIFY_SAME: f_rel * out_height; PF_RECTIFY_VFOV: out_height / (2 tan(vfov / 2)); PF_RECTIFY_FILL: the smallest focal length
+ * >= the SAME one that keeps the four canvas corners inside the input (status 1 and the SAME focal length when none can). */
+enum pf_rectify_focal { PF_RECTIFY_SAME = 0, PF_RECTIFY_VFOV = 1, PF_RECTIFY_FILL = 2 };
+enum pf_rectify_sampler { PF_RECTIFY_BILINEAR = 0, PF_RECTIFY_NEAREST = 1 };
+/* images: HOST array of n (1 .. 65535) descriptors.  params: DEVICE float64 [n, 5] = roll, pitch, general vfov (degrees),
+ * cx_rel, cy_rel per image, read on the device (no synchronisation).  fill: HOST int32 [channels] in 0 .. 255, or NULL for 0.
+ * Outputs (DEVICE): the images, the optional masks and maps (input pixel-centre positions (x, y), NaN where not sampled),
+ * camera float64 [n, 5] (the output camera in the form of params) and status int32 [n] (0 ok, 1 PF_RECTIFY_FILL impossible, 2
+ * unusable parameters: the image is all fill, mask 0, map and camera NaN).  workspace: DEVICE, 256-byte aligned,
+ * pf_rectify_workspace bytes.  Every argument is checked before anything is launched (PF_ERR_ARG). */
+int64_t pf_rectify_workspace(const pf_rectify_image* images, int n);
+int pf_rectify_views(int device, const pf_rectify_image* images, int n, const uint8_t* in_base, uint8_t* out_base, uint8_t* mask_base,
+                     float* map_base, int channels, const double* params, int keep_pitch, int focal_mode, double vfov, int sampler,
+                     const int32_t* fill, double* camera, int32_t* status, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ---- multi-GPU gather of results (SURVEY.md 8e: one process per GPU; NCCL point-to-point over NVLink) ---------------------
  * inference_batch shards its list over the ranks; the per-image results live on each rank's device and are gathered to ONE
  * rank with grouped ncclSend / ncclRecv enqueued on the caller's stream (so that the gather of micro-batch k overlaps the

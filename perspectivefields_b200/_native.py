@@ -58,6 +58,15 @@ class pf_fit_image(ctypes.Structure):
                 ("lat_offset", ctypes.c_int64), ("mask_offset", ctypes.c_int64), ("init", ctypes.c_double * 5)]
 
 
+class pf_rectify_image(ctypes.Structure):
+    """include/pf_b200.h: struct pf_rectify_image (one image of pf_rectify_views)."""
+    _fields_ = [("height", ctypes.c_int32), ("width", ctypes.c_int32), ("out_height", ctypes.c_int32), ("out_width", ctypes.c_int32),
+                ("in_offset", ctypes.c_int64), ("out_offset", ctypes.c_int64), ("mask_offset", ctypes.c_int64), ("map_offset", ctypes.c_int64)]
+
+
+PF_RECTIFY_SAME, PF_RECTIFY_VFOV, PF_RECTIFY_FILL = 0, 1, 2
+PF_RECTIFY_BILINEAR, PF_RECTIFY_NEAREST = 0, 1
+
 PF_EQUI_U8, PF_EQUI_F32 = 0, 1
 PF_EQUI_BILINEAR, PF_EQUI_NEAREST = 0, 1
 PF_EQUI_CAST, PF_EQUI_UNIT = 0, 1
@@ -187,6 +196,9 @@ def lib():
                                   vp, vp, vp, vp, vp, vp, vp, i64, vp]),
         "pf_fit_camera_workspace": (i64, [ctypes.POINTER(pf_fit_image), i32]),
         "pf_fit_camera": (i32, [i32, ctypes.POINTER(pf_fit_image), i32, vp, vp, vp, i32, ctypes.c_double, i32, vp, vp, vp, vp, vp, i64, vp]),
+        "pf_rectify_workspace": (i64, [ctypes.POINTER(pf_rectify_image), i32]),
+        "pf_rectify_views": (i32, [i32, ctypes.POINTER(pf_rectify_image), i32, vp, vp, vp, vp, i32, vp, i32, i32, ctypes.c_double, i32,
+                                   ctypes.POINTER(ctypes.c_int32), vp, vp, vp, i64, vp]),
         "pf_op_layernorm": (i32, [vp, vp, i64, i32, vp, vp, f32, vp]),
         "pf_op_attention": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
         "pf_op_attention_mma": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
@@ -236,7 +248,7 @@ EXPORTS = ["pf_abi_version", "pf_last_error", "pf_kernel_launch_count", "pf_crea
            "pf_profile_kernels_read", "pf_set_option", "pf_debug_enable", "pf_debug_count", "pf_debug_name", "pf_debug_numel",
            "pf_debug_copy", "pf_camera_fields", "pf_camera_fields_vp", "pf_pano_views", "pf_equi_views", "pf_draw_fields",
            "pf_encode_fields", "pf_head_losses_workspace", "pf_head_losses", "pf_field_errors_workspace", "pf_field_errors",
-           "pf_fit_camera_workspace", "pf_fit_camera", "pf_comm_unique_id", "pf_comm_create", "pf_comm_destroy", "pf_gather",
+           "pf_fit_camera_workspace", "pf_fit_camera", "pf_rectify_workspace", "pf_rectify_views", "pf_comm_unique_id", "pf_comm_create", "pf_comm_destroy", "pf_gather",
            "pf_jpeg_create", "pf_jpeg_destroy", "pf_jpeg_info", "pf_jpeg_decode_batch",
            "pf_op_conv_gemm", "pf_op_tma", "pf_op_tma_bf16", "pf_op_conv1_ring", "pf_tma_pick_tile", "pf_op_layernorm", "pf_op_attention",
            "pf_op_attention_mma", "pf_op_attention_tc", "pf_op_attention_tc_bf16", "pf_op_attention_tc_keys", "pf_op_dwconv3x3_gelu",

@@ -30,6 +30,7 @@
 #include "draw.cuh"
 #include "metrics.cuh"
 #include "calib.cuh"
+#include "rectify.cuh"
 #include "comm.cuh"
 #include "jpeg.cuh"
 
@@ -1966,6 +1967,88 @@ int pf_fit_camera(int device, const pf_fit_image* images, int n, const float* up
       LAUNCHED(launch_pdl(fit_step_kernel<3>, step_grid, dim3(32 * kFitStepWarps), 0, st, a));
     }
   }
+  return PF_OK;
+}
+
+// ----------------------------------------------------------------------------------------------- upright warp (rectify.cuh)
+// Workspace layout of pf_rectify_views: device descriptors | per-image maps
+struct RectLayout { long long desc, map, total; };
+static int rectify_layout(const pf_rectify_image* im, int n, RectLayout* lay) {
+  if (!im || n < 1) return fail(PF_ERR_ARG, "pf_rectify_views: null images or n < 1");
+  if (n > 65535) return fail(PF_ERR_ARG, "pf_rectify_views: %d images (at most 65535 per call)", n);
+  for (int i = 0; i < n; ++i) {
+    const pf_rectify_image& c = im[i];
+    if (c.height < 1 || c.width < 1 || (long long)c.height * c.width >= (1LL << 31))
+      return fail(PF_ERR_ARG, "pf_rectify_views: image %d has input size %dx%d", i, c.height, c.width);
+    if (c.out_height < 1 || c.out_width < 1 || (long long)c.out_height * c.out_width >= (1LL << 31))
+      return fail(PF_ERR_ARG, "pf_rectify_views: image %d has output size %dx%d", i, c.out_height, c.out_width);
+  }
+  lay->desc = 0;
+  lay->map = align256((long long)n * sizeof(RectImage));
+  lay->total = lay->map + align256((long long)n * sizeof(RectMap));
+  return PF_OK;
+}
+int64_t pf_rectify_workspace(const pf_rectify_image* images, int n) {
+  RectLayout lay;
+  TRY(rectify_layout(images, n, &lay));
+  return lay.total;
+}
+
+int pf_rectify_views(int device, const pf_rectify_image* images, int n, const uint8_t* in_base, uint8_t* out_base, uint8_t* mask_base,
+                     float* map_base, int channels, const double* params, int keep_pitch, int focal_mode, double vfov, int sampler,
+                     const int32_t* fill, double* camera, int32_t* status, void* workspace, int64_t workspace_bytes, void* stream) {
+  RectLayout lay;
+  TRY(rectify_layout(images, n, &lay));
+  if (!in_base || !out_base || !params || !camera || !status || !workspace)
+    return fail(PF_ERR_ARG, "pf_rectify_views: null input / output / params / camera / status / workspace");
+  if (channels != 1 && channels != 3) return fail(PF_ERR_ARG, "pf_rectify_views: %d channels (1 or 3)", channels);
+  if (keep_pitch != 0 && keep_pitch != 1) return fail(PF_ERR_ARG, "pf_rectify_views: keep_pitch must be 0 or 1");
+  if (focal_mode != PF_RECTIFY_SAME && focal_mode != PF_RECTIFY_VFOV && focal_mode != PF_RECTIFY_FILL)
+    return fail(PF_ERR_ARG, "pf_rectify_views: unknown focal mode %d", focal_mode);
+  if (focal_mode == PF_RECTIFY_VFOV && !(std::isfinite(vfov) && vfov > 0.0 && vfov < 180.0))
+    return fail(PF_ERR_ARG, "pf_rectify_views: vfov %g must lie in (0, 180) degrees", vfov);
+  if (sampler != PF_RECTIFY_BILINEAR && sampler != PF_RECTIFY_NEAREST) return fail(PF_ERR_ARG, "pf_rectify_views: unknown sampler %d", sampler);
+  unsigned char fv[3] = {0, 0, 0};
+  for (int c = 0; fill && c < channels; ++c) {
+    if (fill[c] < 0 || fill[c] > 255) return fail(PF_ERR_ARG, "pf_rectify_views: fill[%d] = %d outside 0 .. 255", c, fill[c]);
+    fv[c] = (unsigned char)fill[c];
+  }
+  if (workspace_bytes < lay.total) return fail(PF_ERR_WORKSPACE, "pf_rectify_views: workspace %lld B < required %lld B", (long long)workspace_bytes, lay.total);
+  if (((uintptr_t)workspace & 255) != 0) return fail(PF_ERR_ARG, "pf_rectify_views: workspace must be 256-byte aligned");
+  std::vector<RectImage> d(n);
+  long long max_px = 1;
+  for (int i = 0; i < n; ++i) {
+    const pf_rectify_image& c = images[i];
+    if (c.in_offset < 0 || c.out_offset < 0 || c.mask_offset < -1 || c.map_offset < -1)
+      return fail(PF_ERR_ARG, "pf_rectify_views: image %d has a negative offset", i);
+    if (c.mask_offset >= 0 && !mask_base) return fail(PF_ERR_ARG, "pf_rectify_views: image %d has a mask offset but mask_base is NULL", i);
+    if (c.map_offset >= 0 && !map_base) return fail(PF_ERR_ARG, "pf_rectify_views: image %d has a map offset but map_base is NULL", i);
+    RectImage& o = d[i];
+    o.H = c.height; o.W = c.width; o.Ho = c.out_height; o.Wo = c.out_width;
+    o.in_off = c.in_offset; o.out_off = c.out_offset; o.mask_off = c.mask_offset; o.map_off = c.map_offset;
+    max_px = std::max(max_px, (long long)c.out_height * c.out_width);
+  }
+  if (cdivl(max_px, (long long)kRectThreads * kRectPix) >= (1LL << 31)) return fail(PF_ERR_ARG, "pf_rectify_views: output too large");
+  CU(cudaSetDevice(device));
+  cudaStream_t st = (cudaStream_t)stream;
+  char* ws = (char*)workspace;
+  RectArgs a{};
+  a.im = (const RectImage*)(ws + lay.desc); a.map = (RectMap*)(ws + lay.map); a.n = n;
+  a.params = params; a.camera = camera; a.status = status;
+  a.keep_pitch = keep_pitch; a.focal_mode = focal_mode; a.vfov = vfov;
+  a.in = in_base; a.out = out_base; a.mask = mask_base; a.xy = map_base;
+  for (int c = 0; c < 3; ++c) a.fill[c] = fv[c];
+  CU(cudaMemcpyAsync(ws + lay.desc, d.data(), n * sizeof(RectImage), cudaMemcpyHostToDevice, st));
+  const PdlScope pdl(!sync_debug());
+  LAUNCHED(launch_pdl(rectify_setup_kernel, dim3((unsigned)cdiv(n, 128)), dim3(128), 0, st, a));
+  const dim3 grid((unsigned)cdivl(max_px, (long long)kRectThreads * kRectPix), (unsigned)n);
+  const bool nearest = sampler == PF_RECTIFY_NEAREST;
+  if (channels == 3)
+    LAUNCHED(nearest ? launch_pdl(rectify_warp_kernel<3, true>, grid, dim3(kRectThreads), 0, st, a)
+                     : launch_pdl(rectify_warp_kernel<3, false>, grid, dim3(kRectThreads), 0, st, a));
+  else
+    LAUNCHED(nearest ? launch_pdl(rectify_warp_kernel<1, true>, grid, dim3(kRectThreads), 0, st, a)
+                     : launch_pdl(rectify_warp_kernel<1, false>, grid, dim3(kRectThreads), 0, st, a));
   return PF_OK;
 }
 
