@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define PF_ABI_VERSION 2
+#define PF_ABI_VERSION 3
 
 typedef struct pf_engine* pf_handle;
 
@@ -107,16 +107,9 @@ int pf_profile_read(pf_handle h, double* out21);
 int pf_profile_kernels_enable(pf_handle h, int max_launches);
 int pf_profile_kernels_read(pf_handle h, char* buf, int cap);
 
-/* Engine options (all default 1 unless noted; the whole graph runs on the persistent TMA -> wgmma engine with pre-split
- * bf16 hi/lo activations, gemm_tma.cuh):
- * "attn_mma": (with "attn_split" = 0) mma.sync attention core instead of the exact-softmax CUDA-core kernel.
- * "attn_split": q / kv leave their GEMMs as split planes for the mma.sync attention core (attention_mma.cuh); 0 = fp32.
- * "stem_tc": the two 7x7 stems as patch gather + TMA GEMM instead of fp32 direct convolution.
- * "phase_conv1": conv_fuse_conv1 composed with the x2 bilinear upsample in front of it (four output phases on the 160x160 grid
- *   + an exact fp32 border-ring kernel); 0 = materialise the upsampled tensor, conv at 320x320.
- * "pdl": programmatic dependent launch of the graph's kernels (a kernel's prologue overlaps its predecessor's tail).
- * "fork" (default 0): the spatial-reduction branch of a MiT block on a second stream beside the q projection (slower in the forward graph: the two streams' persistent kernels compete for SMs).
- * "dw_ln" (default 0): ConvNeXt depthwise 7x7 fused with the LayerNorm behind it (slower than the separate kernels).
+/* Engine options (the whole graph runs on the persistent TMA -> wgmma engine with pre-split bf16 hi/lo activations,
+ * gemm_tma.cuh); any other name is an error:
+ * "pdl" (default 1): programmatic dependent launch of the graph's kernels (a kernel's prologue overlaps its predecessor's tail).
  * "decode_only" (default 0; classification heads, SURVEY.md 8f-3): the 73 / 180 logits are never written -- the 1x1 prediction
  *   conv, argmax and bin decode (gravity_head.py:243-244 + utils/utils.py:114-130, latitude_head.py:205-208 + utils.py:148-162)
  *   run in one kernel and pred_gravity / pred_latitude receive the decoded fields [n,2,320,320] / [n,1,320,320] (degrees).
@@ -410,8 +403,6 @@ int pf_op_conv1_ring(const void* c_hi, const void* c_lo, int B, int H, int W, co
  * K = 9 * Cin) on a device with sm_count SMs. */
 int pf_tma_pick_tile(int mode, int64_t M, int N, int K, int sm_count, int* bn, int* kb);
 int pf_op_layernorm(const float* x, float* y, int64_t rows, int C, const float* w, const float* b, float eps, void* stream);
-int pf_op_attention(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream);      /* CUDA-core fp32 */
-int pf_op_attention_mma(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream);  /* warp-level mma.sync, bf16x3 */
 int pf_op_attention_tc(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream);   /* q / kv split into bf16 hi/lo planes first, then the mma.sync core as the forward graph runs it */
 int pf_op_attention_tc_bf16(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream); /* the same in the bf16 precision mode: one mma.sync per product on bf16(q), bf16(k), bf16(P), bf16(v) */
 /* pf_op_attention_tc / _bf16 (bf16 != 0) with NKV keys per image (kv: [B,NKV,2C]), 1..256: 100 runs the 320 x 320 kernel, other

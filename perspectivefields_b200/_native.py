@@ -200,8 +200,6 @@ def lib():
         "pf_rectify_views": (i32, [i32, ctypes.POINTER(pf_rectify_image), i32, vp, vp, vp, vp, i32, vp, i32, i32, ctypes.c_double, i32,
                                    ctypes.POINTER(ctypes.c_int32), vp, vp, vp, i64, vp]),
         "pf_op_layernorm": (i32, [vp, vp, i64, i32, vp, vp, f32, vp]),
-        "pf_op_attention": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
-        "pf_op_attention_mma": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
         "pf_op_attention_tc": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
         "pf_op_attention_tc_bf16": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
         "pf_op_attention_tc_keys": (i32, [vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]),
@@ -237,7 +235,7 @@ def lib():
                 continue
             raise
         fn.restype, fn.argtypes = res, args
-    if L.pf_abi_version() != 2:
+    if L.pf_abi_version() != 3:
         raise RuntimeError("libpf_b200.so ABI version mismatch")
     _lib = L
     return L
@@ -250,8 +248,8 @@ EXPORTS = ["pf_abi_version", "pf_last_error", "pf_kernel_launch_count", "pf_crea
            "pf_encode_fields", "pf_head_losses_workspace", "pf_head_losses", "pf_field_errors_workspace", "pf_field_errors",
            "pf_fit_camera_workspace", "pf_fit_camera", "pf_rectify_workspace", "pf_rectify_views", "pf_comm_unique_id", "pf_comm_create", "pf_comm_destroy", "pf_gather",
            "pf_jpeg_create", "pf_jpeg_destroy", "pf_jpeg_info", "pf_jpeg_decode_batch",
-           "pf_op_conv_gemm", "pf_op_tma", "pf_op_tma_bf16", "pf_op_conv1_ring", "pf_tma_pick_tile", "pf_op_layernorm", "pf_op_attention",
-           "pf_op_attention_mma", "pf_op_attention_tc", "pf_op_attention_tc_bf16", "pf_op_attention_tc_keys", "pf_op_dwconv3x3_gelu",
+           "pf_op_conv_gemm", "pf_op_tma", "pf_op_tma_bf16", "pf_op_conv1_ring", "pf_tma_pick_tile", "pf_op_layernorm",
+           "pf_op_attention_tc", "pf_op_attention_tc_bf16", "pf_op_attention_tc_keys", "pf_op_dwconv3x3_gelu",
            "pf_op_dwconv7x7", "pf_op_upsample2x", "pf_op_preprocess", "pf_op_preprocess_sized", "pf_op_fill_stream", "pf_op_resize_u8",
            "pf_op_resize_f32", "pf_op_argmax_decode", "pf_op_pred_argmax_decode", "pf_op_postprocess", "pf_op_postprocess_sized"]
 

@@ -1,9 +1,8 @@
 // Spatial-reduction attention core on the tensor cores: softmax(q k^T / 8) v, 100 keys, head_dim 64
 // (mix_transformers.py:127-131), split-precision bf16x3 products (lo*hi + hi*lo + hi*hi, fp32 accumulate) for both
-// q k^T and p v, fp32 softmax.  Replaces the CUDA-core attention_kernel (layers.cuh) on the forward path; ~12 % of the
-// step there.
+// q k^T and p v, fp32 softmax.
 //
-//   block = 4 warps (3 blocks per SM), one (image, head); K and V of the head are split once into bf16 hi/lo planes in shared memory
+//   block = 4 warps (3 blocks per SM), one (image, head); the bf16 hi/lo planes of the head's K and V are staged once in shared memory
 //   (keys padded 100 -> 112, rows of 128 B, 16 B chunks XOR-swizzled for conflict-free ldmatrix); the block then loops over
 //   passes of 64 queries (16 per warp); passes per block are chosen so that the grid is about one resident wave.  Per warp and tile: S = q k^T (mma.sync.m16n8k16, 4 k-steps x 14 key tiles x 3),
 //   row softmax in registers (quad shuffles), O = P V (7 k-steps x 8 tiles x 3; P re-used from the S accumulators as the A
@@ -26,13 +25,12 @@ __device__ __forceinline__ void ldmatrix_x4_trans(uint32_t addr, uint32_t& r0, u
                : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
 }
 
-// SPLIT_IN: q and kv arrive as bf16 hi/lo planes (written by the q / kv GEMM epilogues): K and V are copied into shared memory
+// q and kv arrive as bf16 hi/lo planes (written by the q / kv GEMM epilogues): K and V are copied into shared memory
 // with cp.async (no conversion work), Q fragments are read as bf16 pairs; the 1/8 scale is applied to S in fp32 (a power of
-// two: identical to scaling q).  Otherwise q, kv are fp32 (operator entry point, legacy graph) and are split on the fly.
+// two: identical to scaling q).
 // KEYS: the key count (100: every stage at a 320 x 320 working size); 0 = the run-time count `nkv_rt` (at most kAmKeysPad).
-template <bool SPLIT_IN, int NP = 3, int KEYS = kAmKeys>
-__global__ void __launch_bounds__(kAmThreads) attention_mma_kernel(const float* __restrict__ q, const float* __restrict__ kv,
-                                                                   const __nv_bfloat16* __restrict__ q_hi, const __nv_bfloat16* __restrict__ q_lo,
+template <int NP = 3, int KEYS = kAmKeys>
+__global__ void __launch_bounds__(kAmThreads) attention_mma_kernel(const __nv_bfloat16* __restrict__ q_hi, const __nv_bfloat16* __restrict__ q_lo,
                                                                    const __nv_bfloat16* __restrict__ kv_hi, const __nv_bfloat16* __restrict__ kv_lo,
                                                                    float* __restrict__ out,
                                                                    __nv_bfloat16* __restrict__ shi, __nv_bfloat16* __restrict__ slo, int N, int C,
@@ -48,8 +46,8 @@ __global__ void __launch_bounds__(kAmThreads) attention_mma_kernel(const float* 
   const uint32_t sK_hi = smem_u32(sm_raw), sK_lo = sK_hi + kAmPlane, sV_hi = sK_hi + kPl * kAmPlane, sV_lo = sV_hi + kAmPlane;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int b = blockIdx.z, h = blockIdx.y;
-  // ---- stage K and V of this (image, head): fp32 -> bf16 hi/lo, [key][64] rows of 128 B, chunk (16 B) index ^= key & 7
-  if (SPLIT_IN) {
+  // ---- stage K and V of this (image, head): [key][64] rows of 128 B, chunk (16 B) index ^= key & 7
+  {
     // 2 kPl planes (K_hi, K_lo, V_hi, V_lo; NP = 1: K_hi, V_hi) x 112 keys x 8 chunks of 16 B
     const long long kvo = (long long)b * nkv * 2 * C + h * kAmD;
     for (int i = tid; i < 2 * kPl * kAmKeysPad * 8; i += kAmThreads) {
@@ -63,21 +61,6 @@ __global__ void __launch_bounds__(kAmThreads) attention_mma_kernel(const float* 
     cp_async_commit();
     cp_async_wait<0>();
   }
-  const float* kvb = SPLIT_IN ? nullptr : kv + (long long)b * nkv * 2 * C + h * kAmD;
-  for (int i = tid; !SPLIT_IN && i < kAmKeysPad * (kAmD / 4) * 2; i += kAmThreads) {
-    const int isv = i >= kAmKeysPad * (kAmD / 4);
-    const int j = isv ? i - kAmKeysPad * (kAmD / 4) : i;
-    const int key = j / (kAmD / 4), d4 = j % (kAmD / 4);
-    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (key < nkv) v = __ldg(reinterpret_cast<const float4*>(kvb + (long long)key * 2 * C + (isv ? C : 0) + d4 * 4));
-    uint2 hh, ll;
-    split_bf16x2(v.x, v.y, hh.x, ll.x);
-    split_bf16x2(v.z, v.w, hh.y, ll.y);
-    const uint32_t off = (uint32_t)key * 128u + (uint32_t)(((d4 >> 1) ^ (key & 7)) << 4) + (uint32_t)(d4 & 1) * 8u;
-    unsigned char* base = sm_raw + (isv ? kPl * kAmPlane : 0);
-    *reinterpret_cast<uint2*>(base + off) = hh;
-    if (kLo) *reinterpret_cast<uint2*>(base + kAmPlane + off) = ll;
-  }
   __syncthreads();
 
   const int g = lane >> 2, t = lane & 3;
@@ -85,37 +68,21 @@ __global__ void __launch_bounds__(kAmThreads) attention_mma_kernel(const float* 
     const int q0 = (blockIdx.x * tiles_per_block + it) * kAmQTile + warp * 16;   // first query row of this warp
     if (q0 >= N) break;                                                         // warp-uniform
     const int r0 = q0 + g, r1 = q0 + g + 8;
-    // ---- Q fragments (pre-scaled by 1/8, an exact power of two), split into hi / lo
+    // ---- Q fragments, hi / lo
     uint32_t qh[4][4], ql[4][4];
-    if (SPLIT_IN) {
-      const long long o0 = ((long long)b * N + (r0 < N ? r0 : N - 1)) * C + h * kAmD, o1 = ((long long)b * N + (r1 < N ? r1 : N - 1)) * C + h * kAmD;
+    const long long o0 = ((long long)b * N + (r0 < N ? r0 : N - 1)) * C + h * kAmD, o1 = ((long long)b * N + (r1 < N ? r1 : N - 1)) * C + h * kAmD;
 #pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
-        const int c0 = ks * 16 + 2 * t;
-        qh[ks][0] = __ldg(reinterpret_cast<const uint32_t*>(q_hi + o0 + c0));
-        qh[ks][1] = __ldg(reinterpret_cast<const uint32_t*>(q_hi + o1 + c0));
-        qh[ks][2] = __ldg(reinterpret_cast<const uint32_t*>(q_hi + o0 + c0 + 8));
-        qh[ks][3] = __ldg(reinterpret_cast<const uint32_t*>(q_hi + o1 + c0 + 8));
-        if (kLo) {
-          ql[ks][0] = __ldg(reinterpret_cast<const uint32_t*>(q_lo + o0 + c0));
-          ql[ks][1] = __ldg(reinterpret_cast<const uint32_t*>(q_lo + o1 + c0));
-          ql[ks][2] = __ldg(reinterpret_cast<const uint32_t*>(q_lo + o0 + c0 + 8));
-          ql[ks][3] = __ldg(reinterpret_cast<const uint32_t*>(q_lo + o1 + c0 + 8));
-        }
-      }
-    } else {
-      const float* q0p = q + ((long long)b * N + (r0 < N ? r0 : N - 1)) * C + h * kAmD;
-      const float* q1p = q + ((long long)b * N + (r1 < N ? r1 : N - 1)) * C + h * kAmD;
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
-        const float2 a0 = __ldg(reinterpret_cast<const float2*>(q0p + ks * 16 + 2 * t));
-        const float2 a1 = __ldg(reinterpret_cast<const float2*>(q1p + ks * 16 + 2 * t));
-        const float2 a2 = __ldg(reinterpret_cast<const float2*>(q0p + ks * 16 + 8 + 2 * t));
-        const float2 a3 = __ldg(reinterpret_cast<const float2*>(q1p + ks * 16 + 8 + 2 * t));
-        split_bf16x2(a0.x * 0.125f, a0.y * 0.125f, qh[ks][0], ql[ks][0]);
-        split_bf16x2(a1.x * 0.125f, a1.y * 0.125f, qh[ks][1], ql[ks][1]);
-        split_bf16x2(a2.x * 0.125f, a2.y * 0.125f, qh[ks][2], ql[ks][2]);
-        split_bf16x2(a3.x * 0.125f, a3.y * 0.125f, qh[ks][3], ql[ks][3]);
+    for (int ks = 0; ks < 4; ++ks) {
+      const int c0 = ks * 16 + 2 * t;
+      qh[ks][0] = __ldg(reinterpret_cast<const uint32_t*>(q_hi + o0 + c0));
+      qh[ks][1] = __ldg(reinterpret_cast<const uint32_t*>(q_hi + o1 + c0));
+      qh[ks][2] = __ldg(reinterpret_cast<const uint32_t*>(q_hi + o0 + c0 + 8));
+      qh[ks][3] = __ldg(reinterpret_cast<const uint32_t*>(q_hi + o1 + c0 + 8));
+      if (kLo) {
+        ql[ks][0] = __ldg(reinterpret_cast<const uint32_t*>(q_lo + o0 + c0));
+        ql[ks][1] = __ldg(reinterpret_cast<const uint32_t*>(q_lo + o1 + c0));
+        ql[ks][2] = __ldg(reinterpret_cast<const uint32_t*>(q_lo + o0 + c0 + 8));
+        ql[ks][3] = __ldg(reinterpret_cast<const uint32_t*>(q_lo + o1 + c0 + 8));
       }
     }
     // ---- S = Q K^T : 16 x 112
@@ -152,7 +119,7 @@ __global__ void __launch_bounds__(kAmThreads) attention_mma_kernel(const float* 
 #pragma unroll
     for (int nt = 0; nt < 14; ++nt) {
       const int k0 = nt * 8 + 2 * t;
-      if (SPLIT_IN) { s[nt][0] *= 0.125f; s[nt][1] *= 0.125f; s[nt][2] *= 0.125f; s[nt][3] *= 0.125f; }
+      s[nt][0] *= 0.125f; s[nt][1] *= 0.125f; s[nt][2] *= 0.125f; s[nt][3] *= 0.125f;
       if (k0 >= nkv) { s[nt][0] = -INFINITY; s[nt][2] = -INFINITY; }
       if (k0 + 1 >= nkv) { s[nt][1] = -INFINITY; s[nt][3] = -INFINITY; }
       m0 = fmaxf(m0, fmaxf(s[nt][0], s[nt][1]));
@@ -227,7 +194,7 @@ __global__ void __launch_bounds__(kAmThreads) attention_mma_kernel(const float* 
 
 // ---------------------------------------------------------------------------------------------------------------------------
 // Key-block path: more than kAmKeysPad keys (working sizes other than 320 x 320: (H/32) * (W/32) keys, up to kAmMaxKeys).
-// Same block (4 warps, one (image, head), 16 queries per warp and pass) and the same staging (split-plane input only), with
+// Same block (4 warps, one (image, head), 16 queries per warp and pass) and the same staging, with
 // K and V resident in shared memory for all keys (padded to 16): 4 planes x 256 keys x 128 B = 128 KB at NP = 3, half at NP = 1.
 // The warp loops over blocks of 64 keys with an online (running-max) fp32 softmax: S of one key block is 8 tiles (32 registers
 // per thread instead of 4 * keys / 8), the running output O is rescaled by exp(m_old - m_new) before each block's P V.
@@ -402,23 +369,18 @@ __global__ void __launch_bounds__(kAmThreads) attention_mma_kb_kernel(const __nv
 }
 
 inline cudaError_t attention_mma_configure_device() {   // per-device shared-memory opt-in (pf_create)
-  cudaError_t e = cudaFuncSetAttribute(attention_mma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAmSmem);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(attention_mma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAmSmem);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(attention_mma_kernel<true, 3, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAmSmem);
+  cudaError_t e = cudaFuncSetAttribute(attention_mma_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAmSmem);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(attention_mma_kernel<3, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAmSmem);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(attention_mma_kb_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAmKbSmemMax);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(attention_mma_kb_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, am_kb_smem<1>(kAmMaxKeys));
   return e;   // (the single-block NP = 1 instantiations use 28 KB: no opt-in)
 }
 
 template <int NP>
-inline cudaError_t attention_mma_launch_np(const float* q, const float* kv, float* out, dim3 grid, int N, int C, int tpb, cudaStream_t st, SplitT sp,
-                                           SplitT qs, SplitT kvs, int nkv) {
-  if (nkv != kAmKeys) {   // run-time key count (<= kAmKeysPad; split-plane input only)
-    if (!qs.hi) return cudaErrorInvalidValue;
-    return launch_pdl(attention_mma_kernel<true, NP, 0>, grid, dim3(kAmThreads), am_smem<NP>(), st, nullptr, nullptr, qs.hi, qs.lo, kvs.hi, kvs.lo, out, sp.hi, sp.lo, N, C, tpb, nkv);
-  }
-  if (qs.hi) return launch_pdl(attention_mma_kernel<true, NP>, grid, dim3(kAmThreads), am_smem<NP>(), st, nullptr, nullptr, qs.hi, qs.lo, kvs.hi, kvs.lo, out, sp.hi, sp.lo, N, C, tpb, nkv);
-  return launch_pdl(attention_mma_kernel<false, NP>, grid, dim3(kAmThreads), am_smem<NP>(), st, q, kv, nullptr, nullptr, nullptr, nullptr, out, sp.hi, sp.lo, N, C, tpb, nkv);
+inline cudaError_t attention_mma_launch_np(float* out, dim3 grid, int N, int C, int tpb, cudaStream_t st, SplitT sp, SplitT qs, SplitT kvs, int nkv) {
+  if (nkv != kAmKeys)   // run-time key count (<= kAmKeysPad)
+    return launch_pdl(attention_mma_kernel<NP, 0>, grid, dim3(kAmThreads), am_smem<NP>(), st, qs.hi, qs.lo, kvs.hi, kvs.lo, out, sp.hi, sp.lo, N, C, tpb, nkv);
+  return launch_pdl(attention_mma_kernel<NP>, grid, dim3(kAmThreads), am_smem<NP>(), st, qs.hi, qs.lo, kvs.hi, kvs.lo, out, sp.hi, sp.lo, N, C, tpb, nkv);
 }
 
 // resident blocks per SM of the key-block kernel (228 KB of shared memory per SM, 1 KB of it reserved per block; at most 4)
@@ -428,17 +390,16 @@ inline int attention_kb_blocks_per_sm(int nkv, int np) {
   return b < 1 ? 1 : (b > 4 ? 4 : b);
 }
 
-// q / kv: fp32 pointers, or (qs / kvs non-empty) split planes with row pitch C / 2C.  np = bf16 products per output: 3 (split
-// precision) or 1 (bf16 precision mode: only the hi planes of qs / kvs are read).  nkv: keys per image (kv holds nkv rows per
-// image): 100 = the 320 x 320 kernel; other counts up to kAmKeysPad run the single-block kernel with a run-time count, larger
-// ones (up to kAmMaxKeys) the key-block kernel; both of these read split-plane input only.
-inline cudaError_t attention_mma_launch(const float* q, const float* kv, float* out, int B, int N, int C, int heads, cudaStream_t st, SplitT sp = SplitT(),
-                                        SplitT qs = SplitT(), SplitT kvs = SplitT(), int np = 3, int nkv = kAmKeys) {
-  if ((qs.hi != nullptr) != (kvs.hi != nullptr) || (qs.hi && (qs.ld != C || kvs.ld != 2 * C))) return cudaErrorInvalidValue;
+// qs / kvs: q and kv as split planes with row pitch C / 2C; the result goes to the split planes sp and / or the fp32 tensor out
+// (either may be empty).  np = bf16 products per output: 3 (split precision) or 1 (bf16 precision mode: only the hi planes of
+// qs / kvs are read).  nkv: keys per image (kv holds nkv rows per image): 100 = the 320 x 320 kernel; other counts up to
+// kAmKeysPad run the single-block kernel with a run-time count, larger ones (up to kAmMaxKeys) the key-block kernel.
+inline cudaError_t attention_mma_launch(float* out, int B, int N, int C, int heads, cudaStream_t st, SplitT sp, SplitT qs, SplitT kvs, int np = 3,
+                                        int nkv = kAmKeys) {
+  if (!qs.hi || !kvs.hi || qs.ld != C || kvs.ld != 2 * C) return cudaErrorInvalidValue;
   if (nkv < 1 || nkv > kAmMaxKeys || (np != 1 && np != 3)) return cudaErrorInvalidValue;
   const int tiles = cdiv(N, kAmQTile);
   if (nkv > kAmKeysPad) {
-    if (!qs.hi) return cudaErrorInvalidValue;
     // one resident wave of 132 SMs x the blocks per SM the key-block kernel's shared memory allows
     int tpb = (tiles * heads * B) / (132 * attention_kb_blocks_per_sm(nkv, np));
     tpb = tpb < 1 ? 1 : (tpb > tiles ? tiles : tpb);
@@ -452,8 +413,8 @@ inline cudaError_t attention_mma_launch(const float* q, const float* kv, float* 
   int tpb = (tiles * heads * B) / 396;
   tpb = tpb < 1 ? 1 : (tpb > tiles ? tiles : tpb);
   dim3 grid(cdiv(tiles, tpb), heads, B);
-  if (np == 1) return attention_mma_launch_np<1>(q, kv, out, grid, N, C, tpb, st, sp, qs, kvs, nkv);
-  return attention_mma_launch_np<3>(q, kv, out, grid, N, C, tpb, st, sp, qs, kvs, nkv);
+  if (np == 1) return attention_mma_launch_np<1>(out, grid, N, C, tpb, st, sp, qs, kvs, nkv);
+  return attention_mma_launch_np<3>(out, grid, N, C, tpb, st, sp, qs, kvs, nkv);
 }
 
 }  // namespace pf

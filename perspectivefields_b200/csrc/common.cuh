@@ -55,13 +55,6 @@ struct SplitT {
   __nv_bfloat16* lo = nullptr;
   int ld = 0;
 };
-__device__ __forceinline__ void store_split4(__nv_bfloat16* hi, __nv_bfloat16* lo, long long idx, float4 v) {
-  uint2 h, l;
-  split_bf16x2(v.x, v.y, h.x, l.x);
-  split_bf16x2(v.z, v.w, h.y, l.y);
-  *reinterpret_cast<uint2*>(hi + idx) = h;
-  *reinterpret_cast<uint2*>(lo + idx) = l;
-}
 __device__ __forceinline__ void store_split1(__nv_bfloat16* hi, __nv_bfloat16* lo, long long idx, float v) {
   const __nv_bfloat16 h = __float2bfloat16_rn(v);
   hi[idx] = h;

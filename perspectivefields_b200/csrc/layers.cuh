@@ -1,4 +1,4 @@
-// CUDA-core kernels of the inference path: stems, LayerNorm, spatial-reduction attention, depthwise convs,
+// CUDA-core kernels of the inference path: the ParamNet stem, LayerNorm, depthwise convs,
 // x2 bilinear upsample, prediction tails and the ParamNet pooling/regression tail.  All activations NHWC fp32.
 #pragma once
 #include "common.cuh"
@@ -6,17 +6,14 @@
 namespace pf {
 
 // =====================================================================================================
-// Direct fp32 convolution for the 3-channel stems (K = KH*KW*3 is too small/unaligned for the MMA tile):
-//   patch_embed1.proj  conv7x7/4 p3 3->64 (+bias)            mix_transformers.py:276-282,243-245
-//   ll_enc.conv1+bn1+relu  conv7x7/2 p3 3->64, BN folded      perspectivefields.py:79-83
-//   ConvNeXt stem      conv4x4/4 p0 3->96 (+bias)             convnext.py:88-91
+// Direct fp32 convolution for the ParamNet (ConvNeXt) stem, conv4x4/4 p0 3->96 (+bias), convnext.py:88-91
+// (K = KH*KW*3 = 48 is too small for the MMA tile).
 // in : [B, H, W, ldin] (first 3 channels used); w: [(ky,kx,ci)][COUT]; out: [B, OH, OW, COUT].
 // Block = PIX_PER_BLOCK output pixels of one row x COUT channels; thread = 1 channel x PPT pixels.
 template <int KH, int KW, int STRIDE, int PAD, int COUT, int PPT, int PGROUPS>
 __global__ void __launch_bounds__(COUT* PGROUPS) stem_conv_kernel(const float* __restrict__ in, int ldin, int B, int H, int W,
                                                                   const float* __restrict__ w, const float* __restrict__ bias,
-                                                                  float* __restrict__ out, int OH, int OW, int relu,
-                                                                  __nv_bfloat16* __restrict__ shi, __nv_bfloat16* __restrict__ slo) {
+                                                                  float* __restrict__ out, int OH, int OW) {
   constexpr int PIX = PPT * PGROUPS;                   // output pixels per block (along x)
   constexpr int IN_W = (PIX - 1) * STRIDE + KW;        // input columns needed
   __shared__ float s_in[KH][IN_W][3];
@@ -54,23 +51,17 @@ __global__ void __launch_bounds__(COUT* PGROUPS) stem_conv_kernel(const float* _
 #pragma unroll
   for (int j = 0; j < PPT; ++j) {
     const int ox = ox0 + pg * PPT + j;
-    if (ox < OW) {
-      float v = acc[j];
-      if (relu) v = fmaxf(v, 0.f);
-      const long long oi = ((long long)(b * OH + oy) * OW + ox) * COUT + co;
-      if (out) out[oi] = v;
-      if (shi) store_split1(shi, slo, oi, v);
-    }
+    if (ox < OW) out[((long long)(b * OH + oy) * OW + ox) * COUT + co] = acc[j];
   }
 }
 
 template <int KH, int KW, int STRIDE, int PAD, int COUT>
 inline cudaError_t stem_conv_launch(const float* in, int ldin, int B, int H, int W, const float* w, const float* bias,
-                                    float* out, int relu, cudaStream_t st, SplitT sp = SplitT()) {
+                                    float* out, cudaStream_t st) {
   constexpr int PPT = 4, PGROUPS = (COUT == 64) ? 4 : 2;
   const int OH = (H + 2 * PAD - KH) / STRIDE + 1, OW = (W + 2 * PAD - KW) / STRIDE + 1;
   const int tiles_x = cdiv(OW, PPT * PGROUPS);
-  stem_conv_kernel<KH, KW, STRIDE, PAD, COUT, PPT, PGROUPS><<<B * OH * tiles_x, COUT * PGROUPS, 0, st>>>(in, ldin, B, H, W, w, bias, out, OH, OW, relu, sp.hi, sp.lo);
+  stem_conv_kernel<KH, KW, STRIDE, PAD, COUT, PPT, PGROUPS><<<B * OH * tiles_x, COUT * PGROUPS, 0, st>>>(in, ldin, B, H, W, w, bias, out, OH, OW);
   return cudaGetLastError();
 }
 
@@ -180,88 +171,6 @@ inline cudaError_t layernorm_launch(const float* in, float* out, long long rows,
   if (C <= 128) return launch_pdl(layernorm_kernel<1, 32, 4>, dim3((unsigned)cdivl(rows, 32)), dim3(256), 0, st, in, out, rows, C, w, b, eps, sp.hi, sp.lo, patch.hi, patch.lo, RH, RW, sr);
   if (C <= 384) return launch_pdl(layernorm_kernel<3, 32, PF_LN_NR3>, dim3((unsigned)cdivl(rows, 8 * PF_LN_NR3)), dim3(256), 0, st, in, out, rows, C, w, b, eps, sp.hi, sp.lo, patch.hi, patch.lo, RH, RW, sr);
   return launch_pdl(layernorm_kernel<6, 32, PF_LN_NR3>, dim3((unsigned)cdivl(rows, 8 * PF_LN_NR3)), dim3(256), 0, st, in, out, rows, C, w, b, eps, sp.hi, sp.lo, patch.hi, patch.lo, RH, RW, sr);
-}
-
-// =====================================================================================================
-// Spatial-reduction attention core: softmax(q k^T * 0.125) v with NKV = 100 keys, head_dim 64
-// (mix_transformers.py:127-131; NKV is 100 at every stage for 320x320 inputs, SURVEY.md section 5).
-// q: [B, N, C] (head h = channels h*64..), kv: [B, NKV, 2C] (k | v), out: [B, N, C].
-// Block = 128 queries of one (batch, head); K and V staged in shared memory (fp32); one thread per query,
-// two passes over the keys (max, then exp/accumulate) -- fp32 CUDA-core math, exact softmax.
-constexpr int kAttnNkv = 100, kAttnD = 64, kAttnQ = 128;
-constexpr int kAttnSmem = 2 * kAttnNkv * kAttnD * 4;
-__global__ void __launch_bounds__(kAttnQ) attention_kernel(const float* __restrict__ q, const float* __restrict__ kv, float* __restrict__ out,
-                                                           int N, int C, float scale, __nv_bfloat16* __restrict__ shi, __nv_bfloat16* __restrict__ slo) {
-  extern __shared__ __align__(16) float s_kv[];  // K[100][64], V[100][64]
-  float* sK = s_kv;
-  float* sV = s_kv + kAttnNkv * kAttnD;
-  const int b = blockIdx.z, h = blockIdx.y;
-  const float* kvb = kv + (long long)b * kAttnNkv * 2 * C;
-  for (int i = threadIdx.x; i < kAttnNkv * (kAttnD / 4); i += blockDim.x) {
-    const int j = i / (kAttnD / 4), d4 = i % (kAttnD / 4);
-    const float4 kk = __ldg(reinterpret_cast<const float4*>(kvb + (long long)j * 2 * C + h * kAttnD + d4 * 4));
-    const float4 vv = __ldg(reinterpret_cast<const float4*>(kvb + (long long)j * 2 * C + C + h * kAttnD + d4 * 4));
-    reinterpret_cast<float4*>(sK)[i] = kk;
-    reinterpret_cast<float4*>(sV)[i] = vv;
-  }
-  __syncthreads();
-  const int n = blockIdx.x * kAttnQ + threadIdx.x;
-  if (n >= N) return;
-  float qr[kAttnD];
-  const float* qp = q + ((long long)b * N + n) * C + h * kAttnD;
-#pragma unroll
-  for (int d = 0; d < kAttnD; d += 4) {
-    const float4 t = __ldg(reinterpret_cast<const float4*>(qp + d));
-    qr[d] = t.x * scale; qr[d + 1] = t.y * scale; qr[d + 2] = t.z * scale; qr[d + 3] = t.w * scale;
-  }
-  float mx = -INFINITY;
-  for (int j = 0; j < kAttnNkv; ++j) {
-    const float4* kj = reinterpret_cast<const float4*>(sK + j * kAttnD);
-    float s = 0.f;
-#pragma unroll
-    for (int d4 = 0; d4 < kAttnD / 4; ++d4) {
-      const float4 t = kj[d4];
-      s = fmaf(qr[4 * d4], t.x, s); s = fmaf(qr[4 * d4 + 1], t.y, s); s = fmaf(qr[4 * d4 + 2], t.z, s); s = fmaf(qr[4 * d4 + 3], t.w, s);
-    }
-    mx = fmaxf(mx, s);
-  }
-  float o[kAttnD];
-#pragma unroll
-  for (int d = 0; d < kAttnD; ++d) o[d] = 0.f;
-  float l = 0.f;
-  for (int j = 0; j < kAttnNkv; ++j) {
-    const float4* kj = reinterpret_cast<const float4*>(sK + j * kAttnD);
-    float s = 0.f;
-#pragma unroll
-    for (int d4 = 0; d4 < kAttnD / 4; ++d4) {
-      const float4 t = kj[d4];
-      s = fmaf(qr[4 * d4], t.x, s); s = fmaf(qr[4 * d4 + 1], t.y, s); s = fmaf(qr[4 * d4 + 2], t.z, s); s = fmaf(qr[4 * d4 + 3], t.w, s);
-    }
-    const float pj = expf(s - mx);
-    l += pj;
-    const float4* vj = reinterpret_cast<const float4*>(sV + j * kAttnD);
-#pragma unroll
-    for (int d4 = 0; d4 < kAttnD / 4; ++d4) {
-      const float4 t = vj[d4];
-      o[4 * d4] = fmaf(pj, t.x, o[4 * d4]); o[4 * d4 + 1] = fmaf(pj, t.y, o[4 * d4 + 1]);
-      o[4 * d4 + 2] = fmaf(pj, t.z, o[4 * d4 + 2]); o[4 * d4 + 3] = fmaf(pj, t.w, o[4 * d4 + 3]);
-    }
-  }
-  const float inv = 1.0f / l;
-  const long long oi = ((long long)b * N + n) * C + h * kAttnD;
-#pragma unroll
-  for (int d = 0; d < kAttnD; d += 4) {
-    const float4 r = make_float4(o[d] * inv, o[d + 1] * inv, o[d + 2] * inv, o[d + 3] * inv);
-    if (out) *reinterpret_cast<float4*>(out + oi + d) = r;
-    if (shi) store_split4(shi, slo, oi + d, r);
-  }
-}
-
-inline cudaError_t attention_launch(const float* q, const float* kv, float* out, int B, int N, int C, int heads, cudaStream_t st, SplitT sp = SplitT()) {
-  constexpr int smem = kAttnSmem;   // (> 48 KB: opted in per device by pf_create)
-  dim3 grid(cdiv(N, kAttnQ), heads, B);
-  attention_kernel<<<grid, kAttnQ, smem, st>>>(q, kv, out, N, C, 0.125f, sp.hi, sp.lo);
-  return cudaGetLastError();
 }
 
 // =====================================================================================================
@@ -459,115 +368,6 @@ __global__ void __launch_bounds__(256, PF_DW7_MINBLOCKS) dwconv7x7_kernel(const 
       }
     }
   }
-}
-
-// ConvNeXt block head fused: depthwise 7x7 + bias, then LayerNorm over the C channels of each pixel (eps 1e-6), written as the
-// bf16 hi/lo planes pwconv1 loads (convnext.py:48-50: dwconv -> permute -> norm).  The separate LayerNorm launch and the fp32
-// round trip of the depthwise output disappear.  Block = G pixel groups (2 rows x 8 pixels) x C/4 threads (4 channels each);
-// per pixel the C/4 partial sums meet in shared memory (two passes: mean, then centred variance -- as layernorm_kernel).
-template <int C>
-__global__ void __launch_bounds__(C / 4 * (C <= 192 ? 240 / (C / 4) : (C == 384 ? 2 : 1))) dwconv7x7_ln_kernel(
-    const float* __restrict__ in, int B, int H, int W, const float* __restrict__ w, const float* __restrict__ bias, const float* __restrict__ gw,
-    const float* __restrict__ gb, float eps, __nv_bfloat16* __restrict__ shi, __nv_bfloat16* __restrict__ slo) {
-  constexpr int C4 = C / 4, G = C <= 192 ? 240 / C4 : (C == 384 ? 2 : 1);
-  __shared__ float s_sum[G][16], s_sq[G][16];
-  pdl_wait();
-  pdl_launch();
-  const int XG = (W + 7) >> 3, YG = (H + 1) >> 1;
-  const int ngroups = B * YG * XG;
-  const int g = threadIdx.x / C4, c4 = threadIdx.x - g * C4;
-  for (int base = blockIdx.x * G; base < ngroups; base += gridDim.x * G) {   // block-uniform trip count
-    const int grp = base + g;
-    const bool live = grp < ngroups;
-    if (threadIdx.x < G * 16) { s_sum[threadIdx.x / 16][threadIdx.x % 16] = 0.f; s_sq[threadIdx.x / 16][threadIdx.x % 16] = 0.f; }
-    __syncthreads();
-    int r = live ? grp : 0;
-    const int xg = r % XG; r /= XG;
-    const int y0 = (r % YG) * 2; const int b = r / YG;
-    const int x0 = xg * 8;
-    const float4 bv = __ldg(reinterpret_cast<const float4*>(bias) + c4);
-    float4 acc[2][8];
-#pragma unroll
-    for (int oy = 0; oy < 2; ++oy)
-#pragma unroll
-      for (int p = 0; p < 8; ++p) acc[oy][p] = bv;
-    if (live) {
-#pragma unroll
-      for (int ry = 0; ry < 8; ++ry) {          // input rows y0-3 .. y0+4
-        const int iy = y0 + ry - 3;
-        if ((unsigned)iy >= (unsigned)H) continue;
-        float4 a[14];
-#pragma unroll
-        for (int j = 0; j < 14; ++j) {
-          const int ix = x0 - 3 + j;
-          a[j] = (unsigned)ix < (unsigned)W ? __ldg(reinterpret_cast<const float4*>(in + ((long long)(b * H + iy) * W + ix) * C) + c4) : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-#pragma unroll
-        for (int oy = 0; oy < 2; ++oy) {
-          const int ky = ry - oy;
-          if (ky < 0 || ky > 6) continue;
-#pragma unroll
-          for (int kx = 0; kx < 7; ++kx) {
-            const float4 k = __ldg(reinterpret_cast<const float4*>(w + (ky * 7 + kx) * C) + c4);
-#pragma unroll
-            for (int p = 0; p < 8; ++p) {
-              acc[oy][p].x = fmaf(a[p + kx].x, k.x, acc[oy][p].x); acc[oy][p].y = fmaf(a[p + kx].y, k.y, acc[oy][p].y);
-              acc[oy][p].z = fmaf(a[p + kx].z, k.z, acc[oy][p].z); acc[oy][p].w = fmaf(a[p + kx].w, k.w, acc[oy][p].w);
-            }
-          }
-        }
-      }
-#pragma unroll
-      for (int oy = 0; oy < 2; ++oy)
-#pragma unroll
-        for (int p = 0; p < 8; ++p) atomicAdd(&s_sum[g][oy * 8 + p], (acc[oy][p].x + acc[oy][p].y) + (acc[oy][p].z + acc[oy][p].w));
-    }
-    __syncthreads();
-    float mean[2][8];
-#pragma unroll
-    for (int oy = 0; oy < 2; ++oy)
-#pragma unroll
-      for (int p = 0; p < 8; ++p) mean[oy][p] = s_sum[g][oy * 8 + p] / (float)C;
-    if (live) {
-#pragma unroll
-      for (int oy = 0; oy < 2; ++oy)
-#pragma unroll
-        for (int p = 0; p < 8; ++p) {
-          const float a0 = acc[oy][p].x - mean[oy][p], a1 = acc[oy][p].y - mean[oy][p], a2 = acc[oy][p].z - mean[oy][p], a3 = acc[oy][p].w - mean[oy][p];
-          atomicAdd(&s_sq[g][oy * 8 + p], fmaf(a0, a0, a1 * a1) + fmaf(a2, a2, a3 * a3));
-        }
-    }
-    __syncthreads();
-    if (live) {
-      const float4 lw = __ldg(reinterpret_cast<const float4*>(gw) + c4), lb = __ldg(reinterpret_cast<const float4*>(gb) + c4);
-#pragma unroll
-      for (int oy = 0; oy < 2; ++oy) {
-        if (y0 + oy >= H) break;
-#pragma unroll
-        for (int p = 0; p < 8; ++p) {
-          if (x0 + p >= W) break;
-          const float rstd = 1.0f / sqrtf(s_sq[g][oy * 8 + p] / (float)C + eps), m = mean[oy][p];
-          const float4 y = make_float4((acc[oy][p].x - m) * rstd * lw.x + lb.x, (acc[oy][p].y - m) * rstd * lw.y + lb.y,
-                                       (acc[oy][p].z - m) * rstd * lw.z + lb.z, (acc[oy][p].w - m) * rstd * lw.w + lb.w);
-          store_split4(shi, slo, ((long long)(b * H + y0 + oy) * W + x0 + p) * C + c4 * 4, y);
-        }
-      }
-    }
-    __syncthreads();    // the sums are cleared at the top of the next trip
-  }
-}
-
-inline cudaError_t dwconv7x7_ln_launch(const float* in, int B, int H, int W, int C, const float* w, const float* bias, const float* gw, const float* gb,
-                                       float eps, SplitT out, cudaStream_t st) {
-  const int ngroups = B * ((H + 1) / 2) * ((W + 7) / 8);
-  auto grid = [&](int G) { const int g = cdiv(ngroups, G); return dim3((unsigned)(g < 132 * 8 ? g : 132 * 8)); };
-  switch (C) {
-    case 96: return launch_pdl(dwconv7x7_ln_kernel<96>, grid(10), dim3(240), 0, st, in, B, H, W, w, bias, gw, gb, eps, out.hi, out.lo);
-    case 192: return launch_pdl(dwconv7x7_ln_kernel<192>, grid(5), dim3(240), 0, st, in, B, H, W, w, bias, gw, gb, eps, out.hi, out.lo);
-    case 384: return launch_pdl(dwconv7x7_ln_kernel<384>, grid(2), dim3(192), 0, st, in, B, H, W, w, bias, gw, gb, eps, out.hi, out.lo);
-    case 768: return launch_pdl(dwconv7x7_ln_kernel<768>, grid(1), dim3(192), 0, st, in, B, H, W, w, bias, gw, gb, eps, out.hi, out.lo);
-  }
-  return cudaErrorInvalidValue;
 }
 
 inline unsigned ew_grid(long long total) {

@@ -139,27 +139,17 @@ struct pf_engine {
   bool finalized = false;
   std::unordered_map<std::string, WeightRef> weights;
   // resolved weights
-  const float *embed1_w, *embed1_b, *llenc_w, *llenc_b;
   LnW embed_ln[4], stage_norm[4];
   GemmW embed[4];  // [1..3] used
-  GemmW embed1g, llencg;  // 7x7 stems as [64][160] GEMMs (tensor-core path)
+  GemmW embed1g, llencg;  // 7x7 stems as [64][160] GEMMs
   std::vector<MitBlockW> blocks[4];
   GemmW proc[4];   // composed linear_c{l} o linear_c{l}_proc, both heads side by side (N = 512), index lvl-1
   GemmW rcu[4][2][2];  // [fusion-1][unit-1][conv-1], grouped over the two heads
-  GemmW conv0, conv1;
+  GemmW conv0;
   GemmW conv1p;                       // conv_fuse_conv1 composed with the x2 upsample in front of it: 4 phases x 32 outputs per head
   const float *conv1f_w, *conv1f_b;   // plain fp32 conv_fuse_conv1 [head][tap][ci][o] / bias, for the border-ring kernel
-  bool use_fork = false;              // option "fork": the spatial-reduction branch of a MiT block (sr conv -> LayerNorm -> kv) runs on a second
-                                      // stream next to the q projection (both only depend on LayerNorm 1; their grids leave SMs idle: 50-75 tiles).
-                                      // Default OFF: the persistent kernels of the two streams compete for SMs and the event waits break
-                                      // the programmatic-dependent-launch chain
-  cudaStream_t side = nullptr;
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-  bool use_dwln = false;              // option "dw_ln": ConvNeXt depthwise 7x7 fused with the LayerNorm that follows it
   bool use_pdl = true;                // option "pdl": programmatic dependent launch of the graph's kernels (common.cuh)
   bool decode_only = false;           // option "decode_only": classification heads return decoded fields, logits are never written
-  bool use_attn_split = true;         // option "attn_split": q / kv leave their GEMMs as split planes (0 = fp32, split inside the attention kernel)
-  bool use_phase = true;              // option "phase_conv1": 0 = materialise the upsampled tensor and run conv1 at 320x320
   const float *pred_g_w, *pred_g_b, *pred_l_w, *pred_l_b;
   const float *pn_stem_w, *pn_stem_b;
   LnW pn_stem_ln, pn_ds_ln[4], pn_norm;
@@ -190,8 +180,6 @@ struct pf_engine {
     }
   };
   std::unordered_map<MapKey, CUtensorMap, MapKeyHash> map_cache;
-  bool use_stem_tc = true;    // 7x7 stems as patch gather + TMA GEMM (option "stem_tc"; 0 = fp32 CUDA-core direct convolution)
-  bool use_attn_mma = true;   // tensor-core attention core (option "attn_mma"; 0 = CUDA-core fp32 kernel)
   bool bf16 = false;          // option "bf16": every tensor-core product is one bf16 MMA (hi * hi) instead of three; read per launch
   int sm_count = 132;
   bool profile = false;
@@ -227,10 +215,6 @@ static int get_ln(pf_engine* e, const std::string& n, int C, LnW* l) {
 
 static int resolve_weights(pf_engine* e) {
   char nm[128];
-  TRY(get_f(e, "embed1.w", 147 * 64, &e->embed1_w));
-  TRY(get_f(e, "embed1.b", 64, &e->embed1_b));
-  TRY(get_f(e, "llenc.w", 147 * 64, &e->llenc_w));
-  TRY(get_f(e, "llenc.b", 64, &e->llenc_b));
   TRY(get_gemm(e, "embed1g", 64, 160, 64, &e->embed1g));
   TRY(get_gemm(e, "llencg", 64, 160, 64, &e->llencg));
   for (int s = 0; s < 4; ++s) {
@@ -277,7 +261,6 @@ static int resolve_weights(pf_engine* e) {
       }
     }
   TRY(get_gemm(e, "head.conv0", 64, 9 * 320, 64, &e->conv0, 2));
-  TRY(get_gemm(e, "head.conv1", 32, 9 * 64, 32, &e->conv1, 2));
   TRY(get_gemm(e, "head.conv1p", 128, 9 * 64, 128, &e->conv1p, 2));
   TRY(get_f(e, "head.conv1f.w", 2LL * 9 * 64 * 32, &e->conv1f_w));
   TRY(get_f(e, "head.conv1f.b", 64, &e->conv1f_b));
@@ -696,10 +679,10 @@ static int fwd_tails_post(Fwd& F, const pf_batch* bt, const float* conv1_out, Po
   return PF_OK;
 }
 
-// =============================================================================================== TMA forward graph
-// Same network as run_forward, on the TMA -> wgmma engine: every GEMM input is a pre-split bf16 hi/lo tensor written by
-// its producer (LayerNorm, attention, depthwise conv, upsample, stem, or the previous GEMM's epilogue).
-static int run_forward_tma(Fwd& F, const pf_batch* bt) {
+// =============================================================================================== the forward graph
+// The whole network on the TMA -> wgmma engine: every GEMM input is a pre-split bf16 hi/lo tensor written by its producer
+// (LayerNorm, attention, depthwise conv, upsample, stem gather, or the previous GEMM's epilogue).
+static int run_forward(Fwd& F, const pf_batch* bt) {
   pf_engine* e = F.e;
   const pf_model_desc& D = e->desc;
   const int n = F.n;
@@ -713,9 +696,6 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
   int RH[4], RW[4];
   for (int s = 0; s < 4; ++s) { RH[s] = NH >> (s + 2); RW[s] = NW >> (s + 2); }
   const int nkv = RH[3] * RW[3];
-  if ((NH != kNet || NW != kNet) && (!e->use_attn_mma || !e->use_attn_split || !e->use_stem_tc || !e->use_phase))
-    return fail(PF_ERR_ARG, "options attn_mma / attn_split / stem_tc / phase_conv1 = 0 (reference paths of the 320 x 320 graph) need a 320 x 320 "
-                            "working size; this engine runs at %d x %d", NH, NW);
 
   float* x0; PreImage* d_pre; PostImage* d_post;
   {
@@ -731,7 +711,7 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
   for (int s = 0; s < 4; ++s) cfeat[s] = F.salloc((long long)n * RH[s] * RW[s], kMitDims[s]);
   const int LH = NH / 2, LW = NW / 2;                 // low-level encoder / conv_fuse_conv0 grid
   SplitT ll = F.salloc((long long)n * LH * LW, 64);
-  if (e->use_stem_tc) {   // conv7x7/2 (+ folded BN + ReLU) as patch gather + TMA GEMM (K = 147 padded to 160)
+  {   // conv7x7/2 (+ folded BN + ReLU) as patch gather + TMA GEMM (K = 147 padded to 160)
     const long long m = ar.mark();
     const long long M = (long long)n * LH * LW;
     SplitT col = F.salloc(M, 160);
@@ -739,8 +719,6 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
     Epi o; o.S = ll; o.act = 1;
     TRY(F.tgemm(col, M, 160, 0, e->llencg, 64, o));
     ar.release(m);
-  } else if (!dry) {
-    LAUNCHED((stem_conv_launch<7, 7, 2, 3, 64>(x0, 4, n, kNet, kNet, e->llenc_w, e->llenc_b, nullptr, 1, st, ll)));
   }
   TRY(F.tap_split("ll", ll, (long long)n * LH * LW * 64));
 
@@ -760,20 +738,15 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
     float* t2f = ar.f((long long)n * nkv * C);
     SplitT t2 = F.salloc((long long)n * nkv, C);
     SplitT kv = F.salloc((long long)n * nkv, 2 * C);
-    const bool qkv_split = e->use_attn_mma && e->use_attn_split;
-    float* qf = qkv_split ? nullptr : ar.f(rows * C);                        // (fp32 q / kv: CUDA-core attention kernel, or
-    float* kvf = qkv_split ? nullptr : ar.f((long long)n * nkv * 2 * C);     //  option attn_split = 0)
     float* h1 = ar.f(rows * 4 * C);
     SplitT h2 = F.salloc(rows, 4 * C);
-    if (s == 0 && e->use_stem_tc) {
+    if (s == 0) {
       const long long mm = ar.mark();
       SplitT col = F.salloc(rows, 160);
       if (!dry) LAUNCHED(launch_pdl(stem_gather_kernel, dim3(ew_grid(stem_gather_threads(n, RH[0], RW[0]))), dim3(256), 0, st, x0, col.hi, col.lo, n, RH[0], RW[0], 4, NH, NW));
       Epi o; o.C = tf; o.ldc = C;
       TRY(F.tgemm(col, rows, 160, 0, e->embed1g, 64, o));
       ar.release(mm);
-    } else if (s == 0) {
-      if (!dry) LAUNCHED((stem_conv_launch<7, 7, 4, 3, 64>(x0, 4, n, kNet, kNet, e->embed1_w, e->embed1_b, tf, 0, st)));
     } else {
       Epi o; o.C = tf; o.ldc = C;
       TRY(F.tconv_gather(cfeat[s - 1], n, RH[s - 1], RW[s - 1], kMitDims[s - 1], 3, 2, 1, e->embed[s], C, o));
@@ -784,36 +757,15 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
       const MitBlockW& b = e->blocks[s][i];
       if (sr > 1) TRY(F.ln_split_patch(x, t1, t1p, rows, C, b.ln1, 1e-6f, RH[s], RW[s], sr));     // + the sr conv's im2col matrix
       else TRY(F.ln_split(x, t1, rows, C, b.ln1, 1e-6f));
-      Epi oq, okv;
-      if (qkv_split) { oq.S = q; okv.S = kv; } else { oq.C = qf; oq.ldc = C; okv.C = kvf; okv.ldc = 2 * C; }
-      // q and the spatial-reduction branch both depend on LayerNorm 1 only: fork the branch onto the engine's side stream (its
-      // GEMMs have 50-75 tiles for 132 SMs; q's second, partial wave leaves SMs idle as well) and join before the attention core
-      const bool fork = !dry && sr > 1 && e->use_fork && e->side && !e->kp.on && !e->profile && !sync_debug() && !e->debug;
-      if (fork) {
-        CU(cudaEventRecord(e->ev_fork, st));
-        CU(cudaStreamWaitEvent(e->side, e->ev_fork, 0));
-        F.st = e->side;
-      }
+      Epi oq, okv; oq.S = q; okv.S = kv;
       if (sr > 1) {
         { Epi o; o.C = t2f; o.ldc = C; TRY(F.tgemm(t1p, (long long)n * nkv, sr * sr * C, 0, b.sr, C, o)); }
         TRY(F.ln_split(t2f, t2, (long long)n * nkv, C, b.srln, 1e-5f));
         TRY(F.tgemm(t2, (long long)n * nkv, C, 0, b.kv, 2 * C, okv));
       }
-      if (fork) {
-        CU(cudaEventRecord(e->ev_join, e->side));
-        F.st = st;
-      }
       TRY(F.tgemm(t1, rows, C, 0, b.q, C, oq));
-      if (fork) CU(cudaStreamWaitEvent(st, e->ev_join, 0));
-      if (sr > 1) {
-      } else {
-        TRY(F.tgemm(t1, rows, C, 0, b.kv, 2 * C, okv));
-      }
-      if (!dry) {
-        if (qkv_split) LAUNCHED(attention_mma_launch(nullptr, nullptr, nullptr, n, N, C, heads, st, a, q, kv, F.np(), nkv));
-        else if (e->use_attn_mma) LAUNCHED(attention_mma_launch(qf, kvf, nullptr, n, N, C, heads, st, a, SplitT(), SplitT(), F.np()));
-        else LAUNCHED(attention_launch(qf, kvf, nullptr, n, N, C, heads, st, a));
-      }
+      if (sr == 1) TRY(F.tgemm(t1, rows, C, 0, b.kv, 2 * C, okv));
+      if (!dry) LAUNCHED(attention_mma_launch(nullptr, n, N, C, heads, st, a, q, kv, F.np(), nkv));
       { Epi o; o.C = x; o.ldc = C; o.res = x; o.ldr = C; TRY(F.tgemm(a, rows, C, 0, b.proj, C, o)); }
       TRY(F.tapf(x, rows * C, "mit.s%d.b%d.attn", s + 1, i));
       TRY(F.ln_split(x, t1, rows, C, b.ln2, 1e-6f));
@@ -881,36 +833,22 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
     fuse_pred = D.gravity_classes == 2 && D.latitude_classes == 1;
     const bool keep_conv1 = !fuse_pred || e->debug;   // (not `o.C != nullptr`: the sizing dry run has null pointers)
     PredTail pt[2] = {{e->pred_g_w, e->pred_g_b, dry ? nullptr : bt->pred_gravity, 2, 1}, {e->pred_l_w, e->pred_l_b, dry ? nullptr : bt->pred_latitude, 1, 2}};
-    if (e->use_phase) {
-      // x2 upsample folded into conv1's weights: conv1 runs on the LH x LW grid with N = 4 output phases x 32 (no upsampled
-      // tensor); the two outermost output rows / columns, where the identity does not hold, are recomputed by conv1_ring_kernel
-      SplitT c0s = F.salloc((long long)n * LH * LW, 128);
-      {
-        Epi o; o.S = c0s; o.s_gcoff = 64; o.act = 1;
-        TRY(F.thalo(fused_s, 0, 256, &ll, 256, 0, n, LH, LW, 320, e->conv0, 64, 2, 64, o));
-        TRY(F.tap_split("head.conv0", c0s, (long long)n * LH * LW * 128));
-      }
-      Epi o; o.ldc = 64; o.c_gcoff = 32; o.act = 1; o.phase4 = 1;
-      if (keep_conv1) o.C = conv1_out;
-      TRY(F.thalo(c0s, 0, 64, nullptr, 0, 0, n, LH, LW, 64, e->conv1p, 128, 2, 128, o, fuse_pred ? pt : nullptr));
-      if (!dry) {
-        const dim3 grid((unsigned)cdiv(conv1_ring_count(NH, NW), kRingPx), (unsigned)n);
-        LAUNCHED((conv1_ring_kernel<<<grid, 256, kRingSmem, st>>>(c0s.hi, c0s.lo, LH, LW, e->conv1f_w, e->conv1f_b, keep_conv1 ? conv1_out : nullptr,
-                                                                 fuse_pred ? e->pred_g_w : nullptr, e->pred_g_b, bt->pred_gravity,
-                                                                 fuse_pred ? e->pred_l_w : nullptr, e->pred_l_b, bt->pred_latitude), cudaGetLastError()));
-      }
-    } else {
-      float* c0 = ar.f((long long)n * 160 * 160 * 128);
-      {
-        Epi o; o.C = c0; o.ldc = 128; o.c_gcoff = 64; o.act = 1;
-        TRY(F.thalo(fused_s, 0, 256, &ll, 256, 0, n, 160, 160, 320, e->conv0, 64, 2, 64, o));
-        TRY(F.tap("head.conv0", c0, (long long)n * 160 * 160 * 128));
-      }
-      SplitT c0u = F.salloc((long long)n * kNet * kNet, 128);
-      if (!dry) LAUNCHED(launch_pdl(upsample2x_kernel, dim3(ew_grid(upsample2x_threads(n, 160, 160, 128))), dim3(256), 0, st, c0, 128, 0, nullptr, 128, 0, n, 160, 160, 128, c0u.hi, c0u.lo));
-      Epi o; o.ldc = 64; o.c_gcoff = 32; o.act = 1;
-      if (keep_conv1) o.C = conv1_out;
-      TRY(F.thalo(c0u, 0, 64, nullptr, 0, 0, n, kNet, kNet, 64, e->conv1, 32, 2, 32, o, fuse_pred ? pt : nullptr));
+    // x2 upsample folded into conv1's weights: conv1 runs on the LH x LW grid with N = 4 output phases x 32 (no upsampled
+    // tensor); the two outermost output rows / columns, where the identity does not hold, are recomputed by conv1_ring_kernel
+    SplitT c0s = F.salloc((long long)n * LH * LW, 128);
+    {
+      Epi o; o.S = c0s; o.s_gcoff = 64; o.act = 1;
+      TRY(F.thalo(fused_s, 0, 256, &ll, 256, 0, n, LH, LW, 320, e->conv0, 64, 2, 64, o));
+      TRY(F.tap_split("head.conv0", c0s, (long long)n * LH * LW * 128));
+    }
+    Epi o; o.ldc = 64; o.c_gcoff = 32; o.act = 1; o.phase4 = 1;
+    if (keep_conv1) o.C = conv1_out;
+    TRY(F.thalo(c0s, 0, 64, nullptr, 0, 0, n, LH, LW, 64, e->conv1p, 128, 2, 128, o, fuse_pred ? pt : nullptr));
+    if (!dry) {
+      const dim3 grid((unsigned)cdiv(conv1_ring_count(NH, NW), kRingPx), (unsigned)n);
+      LAUNCHED((conv1_ring_kernel<<<grid, 256, kRingSmem, st>>>(c0s.hi, c0s.lo, LH, LW, e->conv1f_w, e->conv1f_b, keep_conv1 ? conv1_out : nullptr,
+                                                               fuse_pred ? e->pred_g_w : nullptr, e->pred_g_b, bt->pred_gravity,
+                                                               fuse_pred ? e->pred_l_w : nullptr, e->pred_l_b, bt->pred_latitude), cudaGetLastError()));
     }
     if (keep_conv1) TRY(F.tap("head.conv1", conv1_out, (long long)n * NH * NW * 64));
     ar.release(m);
@@ -929,7 +867,7 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
     if (!dry) LAUNCHED((pack_fields_kernel<<<(unsigned)cdivl((long long)n * SH * SW, 256), 256, 0, st>>>(bt->pred_gravity, bt->pred_latitude, pin, n, NH, NW, SH, SW), cudaGetLastError()));
     int rh = SH / 4, rw = SW / 4;
     float* x = ar.f((long long)n * rh * rw * 96);
-    if (!dry) LAUNCHED((stem_conv_launch<4, 4, 4, 0, 96>(pin, 4, n, SH, SW, e->pn_stem_w, e->pn_stem_b, x, 0, st)));
+    if (!dry) LAUNCHED((stem_conv_launch<4, 4, 4, 0, 96>(pin, 4, n, SH, SW, e->pn_stem_w, e->pn_stem_b, x, st)));
     TRY(F.ln(x, x, (long long)n * rh * rw, 96, e->pn_stem_ln, 1e-6f));
     for (int s = 0; s < 4; ++s) {
       const int C = kCnxDims[s];
@@ -948,12 +886,8 @@ static int run_forward_tma(Fwd& F, const pf_batch* bt) {
       SplitT h = F.salloc(rows, 4 * C);
       for (int j = 0; j < kCnxDepths[s]; ++j) {
         const CnxBlockW& b = e->pn_blocks[s][j];
-        if (e->use_dwln) {   // depthwise 7x7 + LayerNorm in one kernel, straight to the split planes pwconv1 loads
-          if (!dry) LAUNCHED(dwconv7x7_ln_launch(x, n, rh, rw, C, b.dw_w, b.dw_b, b.ln.w, b.ln.b, 1e-6f, y, st));
-        } else {
-          if (!dry) LAUNCHED(launch_pdl(dwconv7x7_kernel, dim3(ew_grid((long long)n * ((rh + 1) / 2) * ((rw + PF_DW7_PX - 1) / PF_DW7_PX) * (C / 4))), dim3(256), 0, st, x, yf, n, rh, rw, C, b.dw_w, b.dw_b));
-          TRY(F.ln_split(yf, y, rows, C, b.ln, 1e-6f));
-        }
+        if (!dry) LAUNCHED(launch_pdl(dwconv7x7_kernel, dim3(ew_grid((long long)n * ((rh + 1) / 2) * ((rw + PF_DW7_PX - 1) / PF_DW7_PX) * (C / 4))), dim3(256), 0, st, x, yf, n, rh, rw, C, b.dw_w, b.dw_b));
+        TRY(F.ln_split(yf, y, rows, C, b.ln, 1e-6f));
         { Epi o; o.S = h; o.act = 2; TRY(F.tgemm(y, rows, C, 0, b.pw1, 4 * C, o)); }
         { Epi o; o.C = x; o.ldc = C; o.res = x; o.ldr = C; o.gamma = b.gamma; TRY(F.tgemm(h, rows, 4 * C, 0, b.pw2, C, o)); }
       }
@@ -984,7 +918,6 @@ static int configure_device(int device) {
   CU(gemm_tma_configure_device(3));
   CU(gemm_tma_configure_device(1));
   CU(attention_mma_configure_device());
-  CU(cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem));
   CU(cudaFuncSetAttribute(conv1_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kRingSmem));
   CU(cudaFuncSetAttribute(preprocess_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPreSmemBytes));
   CU(cudaFuncSetAttribute(postprocess_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPostSmemMax));
@@ -1035,12 +968,6 @@ int pf_create_sized(int device, const pf_model_desc* desc, int net_h, int net_w,
     delete e;
     return r;
   }
-  if (cudaStreamCreateWithFlags(&e->side, cudaStreamNonBlocking) != cudaSuccess || cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming) != cudaSuccess) {
-    const int r = fail(PF_ERR_CUDA, "pf_create: side stream / events: %s", cudaGetErrorString(cudaGetLastError()));
-    pf_destroy(e);
-    return r;
-  }
   *out = e;
   return PF_OK;
 }
@@ -1048,9 +975,6 @@ int pf_create_sized(int device, const pf_model_desc* desc, int net_h, int net_w,
 int pf_destroy(pf_handle h) {
   if (!h) return PF_OK;
   cudaSetDevice(h->device);
-  if (h->side) { cudaStreamSynchronize(h->side); cudaStreamDestroy(h->side); }
-  if (h->ev_fork) cudaEventDestroy(h->ev_fork);
-  if (h->ev_join) cudaEventDestroy(h->ev_join);
   cudaFree(h->table_dev);
   cudaFreeHost(h->table_host);
   for (auto& r : h->prof) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
@@ -1081,7 +1005,7 @@ int64_t pf_workspace_bytes(pf_handle h, int n, int max_h) {
   F.ar.dry = true;
   F.ar.keep = h->debug;
   (void)max_h;
-  int r = run_forward_tma(F, nullptr);
+  int r = run_forward(F, nullptr);
   if (r != PF_OK) return r;
   return F.ar.peak + 4096;
 }
@@ -1103,7 +1027,7 @@ int pf_forward(pf_handle h, const pf_batch* bt, void* workspace, int64_t workspa
   {  // capacity check with a dry run (cheap: no launches)
     Fwd T{h, Arena{}, nullptr, true, bt->n};
     T.ar.dry = true; T.ar.keep = h->debug;
-    TRY(run_forward_tma(T, nullptr));
+    TRY(run_forward(T, nullptr));
     if (T.ar.peak > workspace_bytes) return fail(PF_ERR_WORKSPACE, "pf_forward: workspace %lld B < required %lld B", (long long)workspace_bytes, T.ar.peak);
   }
   if (((uintptr_t)workspace & 255) != 0) return fail(PF_ERR_ARG, "pf_forward: workspace must be 256-byte aligned");
@@ -1111,7 +1035,7 @@ int pf_forward(pf_handle h, const pf_batch* bt, void* workspace, int64_t workspa
   h->kp.st = (cudaStream_t)stream;
   tl_kp = &h->kp;
   pdl_enabled() = h->use_pdl && !h->kp.on && !h->profile && !sync_debug();   // (event records between launches defeat it anyway)
-  const int r = run_forward_tma(F, bt);
+  const int r = run_forward(F, bt);
   pdl_enabled() = false;
   tl_kp = nullptr;
   return r;
@@ -1162,7 +1086,7 @@ int pf_profile_kernels_read(pf_handle h, char* buf, int cap) {
       while (*e && (isalnum((unsigned char)*e) || *e == '_')) ++e;
       name.assign(c, e);
     }
-    // template arguments of direct kernel launches distinguish the variants (e.g. stem_conv_launch<7, 7, 2, 3, 64>)
+    // template arguments of direct kernel launches distinguish the variants (e.g. stem_conv_launch<4, 4, 4, 0, 96>)
     if (*e == '<' && e[1] != '<') { const char* t = strchr(e, '>'); if (t) name.append(e, t + 1); }
     auto it = agg.find(name);
     if (it == agg.end()) { order.push_back(name); it = agg.emplace(name, std::make_pair(0, 0.0)).first; }
@@ -1183,14 +1107,8 @@ int pf_profile_kernels_read(pf_handle h, char* buf, int cap) {
 }
 int pf_set_option(pf_handle h, const char* name, int value) {
   if (!h || !name) return fail(PF_ERR_ARG, "pf_set_option: null argument");
-  if (!strcmp(name, "attn_mma")) { h->use_attn_mma = value != 0; return PF_OK; }
-  if (!strcmp(name, "stem_tc")) { h->use_stem_tc = value != 0; return PF_OK; }
-  if (!strcmp(name, "phase_conv1")) { h->use_phase = value != 0; return PF_OK; }
-  if (!strcmp(name, "attn_split")) { h->use_attn_split = value != 0; return PF_OK; }
   if (!strcmp(name, "decode_only")) { h->decode_only = value != 0; return PF_OK; }
   if (!strcmp(name, "pdl")) { h->use_pdl = value != 0; return PF_OK; }
-  if (!strcmp(name, "dw_ln")) { h->use_dwln = value != 0; return PF_OK; }
-  if (!strcmp(name, "fork")) { h->use_fork = value != 0; return PF_OK; }
   if (!strcmp(name, "bf16")) { h->bf16 = value != 0; return PF_OK; }
   return fail(PF_ERR_ARG, "pf_set_option: unknown option '%s'", name);
 }
@@ -2134,18 +2052,6 @@ int pf_op_layernorm(const float* x, float* y, int64_t rows, int C, const float* 
   LAUNCHED(layernorm_launch(x, y, rows, C, w, b, eps, (cudaStream_t)stream));
   return PF_OK;
 }
-int pf_op_attention(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream) {
-  TRY(configure_current_device());
-  if (C != heads * kAttnD) return fail(PF_ERR_ARG, "pf_op_attention: head_dim must be 64");
-  LAUNCHED(attention_launch(q, kv, out, B, N, C, heads, (cudaStream_t)stream));
-  return PF_OK;
-}
-int pf_op_attention_mma(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream) {
-  TRY(configure_current_device());
-  if (C != heads * kAmD) return fail(PF_ERR_ARG, "pf_op_attention_mma: head_dim must be 64");
-  LAUNCHED(attention_mma_launch(q, kv, out, B, N, C, heads, (cudaStream_t)stream));
-  return PF_OK;
-}
 static int op_attention_tc(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream, int np, int nkv = kAmKeys) {
   if (!q || !kv || !out || C != heads * kAmD) return fail(PF_ERR_ARG, "pf_op_attention_tc: head_dim must be 64");
   if (B < 1 || N < 1 || nkv < 1 || nkv > kAmMaxKeys) return fail(PF_ERR_ARG, "pf_op_attention_tc: B %d, N %d, %d keys (1..%d)", B, N, nkv, kAmMaxKeys);
@@ -2169,7 +2075,7 @@ static int op_attention_tc(const float* q, const float* kv, float* out, int B, i
   if (le == cudaSuccess) le = (split_kernel<<<(unsigned)cdivl(nkve, 256), 256, 0, st>>>(kv, kvs.hi, kvs.lo, nkve, 0), cudaGetLastError());
   if (le != cudaSuccess) r = fail(PF_ERR_CUDA, "split_kernel: %s", cudaGetErrorString(le));
   if (r == PF_OK) {
-    le = attention_mma_launch(nullptr, nullptr, nullptr, B, N, C, heads, st, as, qs, kvs, np, nkv);
+    le = attention_mma_launch(nullptr, B, N, C, heads, st, as, qs, kvs, np, nkv);
     if (le != cudaSuccess) r = fail(PF_ERR_CUDA, "attention_mma_launch: %s", cudaGetErrorString(le));
   }
   if (r == PF_OK) {

@@ -3,7 +3,7 @@
 Input: the reference's ``{"model": state_dict}`` layout (perspective2d/perspectivefields.py:178-192; key schema in
 SURVEY.md appendix A).  Output: ``{name: tensor}`` with the names ``csrc/pf_b200.cu:resolve_weights`` looks up.
 
-* GEMM layers (every nn.Linear / groups=1 nn.Conv2d except the 3-channel stems): ``<n>.whi`` / ``<n>.wlo`` = bf16
+* GEMM layers (every nn.Linear / groups=1 nn.Conv2d except the ParamNet stem): ``<n>.whi`` / ``<n>.wlo`` = bf16
   hi / lo planes of the [N][K] weight, K ordered (ky, kx, ci); ``<n>.b`` fp32 bias.
 * Decoder-head ``linear_c{l}`` (1x1, C->768) followed by ``linear_c{l}_proc`` (3x3, 768->256) has no non-linearity in
   between (gravity_head.py:146-149): composed exactly, in fp64, into one 3x3 conv C->256.  The Linear's bias goes
@@ -12,7 +12,7 @@ SURVEY.md appendix A).  Output: ``{name: tensor}`` with the names ``csrc/pf_b200
   concatenated along N (512 outputs).
 * The two heads' RefineNet convs are stored as two weight groups of one grouped launch.
 * Eval-mode BatchNorm of ``ll_enc`` is folded into its conv (perspectivefields.py:73-83).
-* Stems / depthwise / prediction layers stay fp32 in the layouts the CUDA-core kernels read.
+* The ParamNet stem, depthwise and prediction layers stay fp32 in the layouts the CUDA-core kernels read.
 """
 import torch
 
@@ -83,15 +83,11 @@ def repack(sd, cfg):
     """sd: reference-layout state dict (CPU tensors).  cfg: entry of variants.VARIANTS."""
     out = {}
     bb = "backbone."
-    # ---- stems
-    out["embed1.w"] = _stem(sd[bb + "patch_embed1.proj.weight"])
-    out["embed1.b"] = sd[bb + "patch_embed1.proj.bias"].float().contiguous()
+    # ---- the two 7x7 stems as [64][160] GEMM weights (K = (ky,kx,c) padded 147 -> 160 with zeros); ll_enc with its BatchNorm folded in
     scale = sd["ll_enc.bn1.weight"].double() / torch.sqrt(sd["ll_enc.bn1.running_var"].double() + 1e-5)
-    out["llenc.w"] = _stem((sd["ll_enc.conv1.weight"].double() * scale[:, None, None, None]).float())
-    out["llenc.b"] = (sd["ll_enc.bn1.bias"].double() - sd["ll_enc.bn1.running_mean"].double() * scale).float().contiguous()
-    # the same two 7x7 stems as [64][160] GEMM weights (K = (ky,kx,c) padded 147 -> 160 with zeros) for the tensor-core path
-    for name, w, b in (("embed1g", sd[bb + "patch_embed1.proj.weight"].double(), out["embed1.b"]),
-                       ("llencg", sd["ll_enc.conv1.weight"].double() * scale[:, None, None, None], out["llenc.b"])):
+    llenc_b = sd["ll_enc.bn1.bias"].double() - sd["ll_enc.bn1.running_mean"].double() * scale
+    for name, w, b in (("embed1g", sd[bb + "patch_embed1.proj.weight"].double(), sd[bb + "patch_embed1.proj.bias"]),
+                       ("llencg", sd["ll_enc.conv1.weight"].double() * scale[:, None, None, None], llenc_b)):
         wk = torch.zeros(64, 160, dtype=torch.float64)
         wk[:, :147] = w.permute(0, 2, 3, 1).reshape(64, 147)
         _put_gemm(out, name, wk, b)
@@ -130,9 +126,8 @@ def repack(sd, cfg):
                 ks = [f"persformer_heads.{h}.fusion{f}.resConfUnit{u}.conv{c}" for h in heads]
                 _put_gemm(out, f"head.f{f}.u{u}.c{c}", torch.stack([_conv_to_nk(sd[k + ".weight"]) for k in ks]),
                           torch.stack([sd[k + ".bias"] for k in ks]).reshape(-1))
-    for name, key in (("head.conv0", "conv_fuse_conv0.conv"), ("head.conv1", "conv_fuse_conv1.conv")):
-        ks = [f"persformer_heads.{h}.{key}" for h in heads]
-        _put_gemm(out, name, torch.stack([_conv_to_nk(sd[k + ".weight"]) for k in ks]), torch.stack([sd[k + ".bias"] for k in ks]).reshape(-1))
+    ks = [f"persformer_heads.{h}.conv_fuse_conv0.conv" for h in heads]
+    _put_gemm(out, "head.conv0", torch.stack([_conv_to_nk(sd[k + ".weight"]) for k in ks]), torch.stack([sd[k + ".bias"] for k in ks]).reshape(-1))
     # conv_fuse_conv1 composed with the x2 upsample in front of it: N = 4 phases x 32 per head on the 160x160 grid; plus the
     # plain fp32 weights as [head][tap][ci][o] for the border-ring kernel
     ks = [f"persformer_heads.{h}.conv_fuse_conv1.conv" for h in heads]

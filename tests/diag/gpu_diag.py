@@ -67,7 +67,7 @@ def ops():
     for (B, N, heads) in ((2, 6400, 1), (2, 1600, 2), (1, 400, 5), (1, 100, 8), (1, 77, 2)):
         C = heads * 64
         q = rn(B, N, C).cuda(); kv = rn(B, 100, 2 * C).cuda(); o = torch.empty_like(q)
-        _native.check(L.pf_op_attention(q.data_ptr(), kv.data_ptr(), o.data_ptr(), B, N, C, heads, U.stream_ptr()))
+        _native.check(L.pf_op_attention_tc(q.data_ptr(), kv.data_ptr(), o.data_ptr(), B, N, C, heads, U.stream_ptr()))
         qh = q.double().reshape(B, N, heads, 64).permute(0, 2, 1, 3)
         kvh = kv.double().reshape(B, 100, 2, heads, 64).permute(2, 0, 3, 1, 4)
         ref = ((qh @ kvh[0].transpose(-2, -1)) * 0.125).softmax(-1) @ kvh[1]

@@ -33,7 +33,7 @@ def test_library_exports_every_declared_symbol(built):
 
 def test_abi_version_and_error_channel(built):
     L = _native.lib()
-    assert L.pf_abi_version() == 2
+    assert L.pf_abi_version() == 3
     assert L.pf_kernel_launch_count() >= 0
     # argument validation happens before any CUDA call
     assert L.pf_create(0, None, None) < 0

@@ -73,9 +73,8 @@ def test_layernorm(C):
     assert U.rel_err(y, F.layer_norm(x.double(), (C,), w.double(), b.double(), 1e-6)) < 1e-5
 
 
-@pytest.mark.parametrize("engine", ["fp32", "mma", "tc"])
 @pytest.mark.parametrize("shape", [(2, 6400, 1), (2, 1600, 2), (1, 400, 5), (1, 100, 8), (1, 77, 2), (1, 1000, 1)])
-def test_attention(shape, engine):
+def test_attention(shape):
     from perspectivefields_b200 import _native
 
     B, N, heads = shape
@@ -83,13 +82,11 @@ def test_attention(shape, engine):
     g = torch.Generator().manual_seed(N)
     q, kv = (_rn(g, B, N, C) * 2).cuda(), (_rn(g, B, 100, 2 * C) * 2).cuda()
     o = torch.empty_like(q)
-    L = _native.lib()
-    fn = {"fp32": L.pf_op_attention, "mma": L.pf_op_attention_mma, "tc": L.pf_op_attention_tc}[engine]
-    _native.check(fn(q.data_ptr(), kv.data_ptr(), o.data_ptr(), B, N, C, heads, U.stream_ptr()))
+    _native.check(_native.lib().pf_op_attention_tc(q.data_ptr(), kv.data_ptr(), o.data_ptr(), B, N, C, heads, U.stream_ptr()))
     qh = q.double().reshape(B, N, heads, 64).permute(0, 2, 1, 3)
     kvh = kv.double().reshape(B, 100, 2, heads, 64).permute(2, 0, 3, 1, 4)
     ref = ((qh @ kvh[0].transpose(-2, -1)) * 0.125).softmax(-1) @ kvh[1]
-    assert U.rel_err(o, ref.transpose(1, 2).reshape(B, N, C)) < (1e-5 if engine == "fp32" else 5e-5)
+    assert U.rel_err(o, ref.transpose(1, 2).reshape(B, N, C)) < 5e-5
 
 
 def test_depthwise_and_upsample():

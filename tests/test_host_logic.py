@@ -53,8 +53,10 @@ def test_repack_composition_and_bn_fold():
     img = torch.randn(1, 3, 32, 32) * 50
     ref = F.relu(F.batch_norm(F.conv2d(img, sd["ll_enc.conv1.weight"], None, stride=2, padding=3), sd["ll_enc.bn1.running_mean"],
                               sd["ll_enc.bn1.running_var"], sd["ll_enc.bn1.weight"], sd["ll_enc.bn1.bias"], False, 0.1, 1e-5))
-    wf = rp["llenc.w"].reshape(7, 7, 3, 64).permute(3, 2, 0, 1)
-    got = F.relu(F.conv2d(img, wf, rp["llenc.b"], stride=2, padding=3))
+    wk = rp["llencg.whi"].double() + rp["llencg.wlo"].double()      # [64][160]: K = (ky, kx, c), 147 columns + 13 of padding
+    assert wk.shape == (64, 160) and not wk[:, 147:].any()
+    wf = wk[:, :147].reshape(64, 7, 7, 3).permute(0, 3, 1, 2)
+    got = F.relu(F.conv2d(img.double(), wf, rp["llencg.b"].double(), stride=2, padding=3))
     assert U.rel_err(got, ref) < 1e-5
     # every GEMM layer has hi/lo/bias, K multiple of 32
     for k in rp:

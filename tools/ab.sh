@@ -1,7 +1,7 @@
 #!/bin/bash
 # A/B timing on ONE box: bench.py with several builds / option sets, alternating.
 #   usage (on the GPU machine): bash tools/ab.sh <rounds> <steps> <variant>...     variant = <lib-suffix or "new">[:<PF_BENCH_OPTS>]
-#   e.g. bash tools/ab.sh 2 10 base new new:attn_split=0      (perspectivefields_b200/libpf_b200_<suffix>.so; "new" = the working-tree build)
+#   e.g. bash tools/ab.sh 2 10 base new new:pdl=0      (perspectivefields_b200/libpf_b200_<suffix>.so; "new" = the working-tree build)
 R=${1:-2}; K=${2:-10}; shift 2
 for i in $(seq $R); do
   for v in "$@"; do
