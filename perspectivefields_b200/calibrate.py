@@ -10,8 +10,7 @@ import math
 
 import torch
 
-from . import _native
-from .metrics import _base, _cuda_f32
+from . import _batch, _native
 from .panocam import general_vfov, general_vfov_to_focal
 
 MAX_ITERATIONS = 1000
@@ -68,40 +67,20 @@ def fit_camera(results, principal_point=False, init="fields", mask=None, huber=N
         raise ValueError(f"{n} results but {len(mask)} masks")
     if n == 0:
         return []
-    pu = [_cuda_f32(r["pred_gravity_original"], f"results[{i}]['pred_gravity_original']") for i, r in enumerate(results)]
-    dev = pu[0].device
-    pl = [_cuda_f32(r["pred_latitude_original"], f"results[{i}]['pred_latitude_original']", dev) for i, r in enumerate(results)]
-    ms = [None] * n if mask is None else list(mask)
-    for i in range(n):
-        if pu[i].dim() != 3 or pu[i].shape[0] != 2:
-            raise ValueError(f"results[{i}]['pred_gravity_original'] must be [2, H, W], got {list(pu[i].shape)}")
-        h, w = int(pu[i].shape[1]), int(pu[i].shape[2])
-        if h < 3 or w < 3:
-            raise ValueError(f"image {i} has size {h}x{w}: the fit needs 3x3 at least")
-        if tuple(pl[i].shape) != (h, w):
-            raise ValueError(f"results[{i}]['pred_latitude_original'] must be [{h}, {w}], got {list(pl[i].shape)}")
-        if ms[i] is not None:
-            m = ms[i]
-            if not isinstance(m, torch.Tensor) or m.dtype != torch.bool or tuple(m.shape) != (h, w) or m.device != dev:
-                raise ValueError(f"mask[{i}] must be a bool [{h}, {w}] tensor on {dev}")
-            ms[i] = m.contiguous().view(torch.uint8)
-        pl[i] = pl[i].contiguous()
+    pu, pl, ms, dev = _batch.prediction_fields(results, mask, 3)
     starts = _init_from_results(results) if init == "results" else [_NAN_INIT] * n
     L = _native.lib()
-    bu, bl, bm = _base(pu), _base(pl), _base(ms)
+    bu, bl, bm = _batch.base(pu), _batch.base(pl), _batch.base(ms)
     descs = (_native.pf_fit_image * n)()
     for i in range(n):
         d = descs[i]
-        d.height, d.width = int(pu[i].shape[1]), int(pu[i].shape[2])
-        d.up_offset = (pu[i].data_ptr() - bu) // 4
-        d.up_stride[0], d.up_stride[1], d.up_stride[2] = pu[i].stride(1), pu[i].stride(2), pu[i].stride(0)
-        d.lat_offset = (pl[i].data_ptr() - bl) // 4
-        d.mask_offset = -1 if ms[i] is None else ms[i].data_ptr() - bm
-        for k in range(5):
-            d.init[k] = starts[i][k]
+        d.height, d.width = int(pu[i].shape[0]), int(pu[i].shape[1])
+        d.up_offset, d.up_stride[:] = _batch.offset(pu[i], bu), pu[i].stride()
+        d.lat_offset = _batch.offset(pl[i], bl)
+        d.mask_offset = _batch.offset(ms[i], bm)
+        d.init[:] = starts[i]
     with torch.cuda.device(dev):
-        need = _native.check(L.pf_fit_camera_workspace(descs, n))
-        ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        ws = _batch.workspace(L.pf_fit_camera_workspace(descs, n), dev)
         params = torch.empty((n, 5), dtype=torch.float64, device=dev)
         cost = torch.empty(n, dtype=torch.float64, device=dev)
         its = torch.empty(n, dtype=torch.int32, device=dev)

@@ -1560,6 +1560,41 @@ int pf_equi_views(int device, const void* pano, int pano_h, int pano_w, int chan
   return PF_OK;
 }
 
+// ----------------------------------------------------------------------------------------------- batched feature calls
+static long long align256(long long b) { return (b + 255) / 256 * 256; }
+
+// A caller-provided workspace carved into 256-byte-aligned sections, in the order they are added: at[k] is the byte offset of
+// section k; the first holds the per-image descriptors (upload_descriptors)
+struct WsLayout {
+  long long at[4] = {}, total = 0;
+  int count = 0;
+  WsLayout& add(long long bytes) { at[count++] = total; total += align256(bytes); return *this; }
+};
+
+static int check_workspace(const char* fn, const void* ws, int64_t bytes, long long need) {
+  if (bytes < need) return fail(PF_ERR_WORKSPACE, "%s: workspace %lld B < required %lld B", fn, (long long)bytes, need);
+  if (((uintptr_t)ws & 255) != 0) return fail(PF_ERR_ARG, "%s: workspace must be 256-byte aligned", fn);
+  return PF_OK;
+}
+
+static int upload_descriptors(const void* d, size_t bytes, void* ws, cudaStream_t st) {
+  CU(cudaMemcpyAsync(ws, d, bytes, cudaMemcpyHostToDevice, st));
+  return PF_OK;
+}
+
+// The per-image offset rule of the batched calls: a required offset is >= 0; an optional one is -1 (absent) or >= 0, and then
+// the buffer it points into must be given
+static int check_offsets(const char* fn, int i, std::initializer_list<long long> required,
+                         std::initializer_list<std::pair<long long, const void*>> optional = {}) {
+  for (const long long o : required)
+    if (o < 0) return fail(PF_ERR_ARG, "%s: image %d has a negative offset", fn, i);
+  for (const auto& [o, buf] : optional) {
+    if (o < -1) return fail(PF_ERR_ARG, "%s: image %d has a negative offset", fn, i);
+    if (o >= 0 && !buf) return fail(PF_ERR_ARG, "%s: image %d has an offset into a NULL buffer", fn, i);
+  }
+  return PF_OK;
+}
+
 // matplotlib's "seismic" map as the 256-entry table it samples (LinearSegmentedColormap.from_list: anchors at 0, 1/4, 1/2, 3/4, 1,
 // linear interpolation at i / 255), and t -> entry min(floor(256 t), 255); levels linspace(-pi/2, pi/2, 19).
 static DrawStyle draw_style() {
@@ -1590,7 +1625,7 @@ int pf_draw_fields(int device, const pf_draw_canvas* cs, int n, const uint8_t* i
     const pf_draw_canvas& c = cs[i];
     if (c.height < 1 || c.width < 1 || (long long)c.height * c.width >= (1LL << 31))
       return fail(PF_ERR_ARG, "pf_draw_fields: canvas %d has size %dx%d", i, c.height, c.width);
-    if (c.img_offset < 0 || c.out_offset < 0) return fail(PF_ERR_ARG, "pf_draw_fields: canvas %d has a negative image offset", i);
+    TRY(check_offsets("pf_draw_fields", i, {c.img_offset, c.out_offset}));
     if (!unit(c.alpha_fill) || !unit(c.alpha_line)) return fail(PF_ERR_ARG, "pf_draw_fields: canvas %d: alphas must lie in [0, 1]", i);
     if (c.draw_lat && (!lat || c.lat_offset < 0)) return fail(PF_ERR_ARG, "pf_draw_fields: canvas %d draws the latitude without a latitude map", i);
     if (c.draw_up) {
@@ -1642,7 +1677,6 @@ int pf_draw_fields(int device, const pf_draw_canvas* cs, int n, const uint8_t* i
 // ----------------------------------------------------------------------------------------------- scoring (metrics.cuh)
 static bool gravity_classes_ok(int c) { return c == 2 || c >= 3; }
 static bool latitude_classes_ok(int c) { return c >= 1; }
-static long long align256(long long b) { return (b + 255) / 256 * 256; }
 
 int pf_encode_fields(int device, int n, int H, int W, const float* up, const int64_t* up_stride, const float* lat, const int64_t* lat_stride,
                      int lat_rad, int gravity_classes, int latitude_classes, void* gt_gravity, void* gt_latitude, void* stream) {
@@ -1686,8 +1720,7 @@ int pf_head_losses(int device, int n, int H, int W, int gravity_classes, const f
   if (need < 0) return (int)need;
   if (!pred_gravity || !gt_gravity || !pred_latitude || !gt_latitude || !losses || !workspace)
     return fail(PF_ERR_ARG, "pf_head_losses: null prediction / target / losses / workspace");
-  if (workspace_bytes < need) return fail(PF_ERR_WORKSPACE, "pf_head_losses: workspace %lld B < required %lld B", (long long)workspace_bytes, (long long)need);
-  if (((uintptr_t)workspace & 255) != 0) return fail(PF_ERR_ARG, "pf_head_losses: workspace must be 256-byte aligned");
+  TRY(check_workspace("pf_head_losses", workspace, workspace_bytes, need));
   const bool cls = gravity_classes != 2;
   if (cls && (((long long)H * W) % kCePix != 0 || ((uintptr_t)pred_gravity & 15) || ((uintptr_t)pred_latitude & 15)))
     return fail(PF_ERR_ARG, "pf_head_losses: classification logits need H * W %% 4 == 0 and 16-byte aligned planes");
@@ -1716,8 +1749,8 @@ int pf_head_losses(int device, int n, int H, int W, int gravity_classes, const f
 }
 
 // Workspace layout of pf_field_errors: device descriptors | fp64 sums [2][blocks] | counts [2][1 + 8][blocks] | maps if not given
-struct FeLayout { long long blocks, pixels, desc, psum, pcnt, maps, total; };
-static int field_errors_layout(const pf_field_image* im, int n, int with_maps, FeLayout* lay) {
+static int field_errors_layout(const pf_field_image* im, int n, int with_maps, WsLayout* lay, long long* blocks_out = nullptr,
+                               long long* pixels_out = nullptr) {
   if (!im || n < 1) return fail(PF_ERR_ARG, "pf_field_errors: null images or n < 1");
   long long blocks = 0, pixels = 0;
   for (int i = 0; i < n; ++i) {
@@ -1728,16 +1761,13 @@ static int field_errors_layout(const pf_field_image* im, int n, int with_maps, F
     pixels += hw;
   }
   if (blocks >= (1LL << 31)) return fail(PF_ERR_ARG, "pf_field_errors: too many pixels");
-  lay->blocks = blocks; lay->pixels = pixels;
-  lay->desc = 0;
-  lay->psum = align256((long long)n * sizeof(FeImage));
-  lay->pcnt = lay->psum + align256(2 * blocks * 8);
-  lay->maps = lay->pcnt + align256(2LL * (1 + kFeMaxThr) * blocks * 4);
-  lay->total = lay->maps + (with_maps ? 0 : align256(2 * pixels * 4));
+  lay->add((long long)n * sizeof(FeImage)).add(2 * blocks * 8).add(2LL * (1 + kFeMaxThr) * blocks * 4).add(with_maps ? 0 : 2 * pixels * 4);
+  if (blocks_out) *blocks_out = blocks;
+  if (pixels_out) *pixels_out = pixels;
   return PF_OK;
 }
 int64_t pf_field_errors_workspace(const pf_field_image* images, int n, int with_maps) {
-  FeLayout lay;
+  WsLayout lay;
   TRY(field_errors_layout(images, n, with_maps, &lay));
   return lay.total;
 }
@@ -1747,8 +1777,9 @@ int pf_field_errors(int device, const pf_field_image* images, int n, const float
                     float* lat_maps, int64_t* count, double* mean, double* median, double* fraction, void* workspace,
                     int64_t workspace_bytes, void* stream) {
   if ((up_maps == nullptr) != (lat_maps == nullptr)) return fail(PF_ERR_ARG, "pf_field_errors: give both maps or neither");
-  FeLayout lay;
-  TRY(field_errors_layout(images, n, up_maps != nullptr, &lay));
+  WsLayout lay;
+  long long blocks, pixels;
+  TRY(field_errors_layout(images, n, up_maps != nullptr, &lay, &blocks, &pixels));
   if (!pred_up || !pred_lat || !gt_up || !gt_lat || !count || !mean || !median || !workspace)
     return fail(PF_ERR_ARG, "pf_field_errors: null field / output / workspace");
   if (n_thresholds < 0 || n_thresholds > kFeMaxThr || (n_thresholds > 0 && (!thresholds || !fraction)))
@@ -1756,15 +1787,12 @@ int pf_field_errors(int device, const pf_field_image* images, int n, const float
   for (int k = 0; k < n_thresholds; ++k)
     if (std::isnan(thresholds[k])) return fail(PF_ERR_ARG, "pf_field_errors: threshold %d is NaN", k);
   if (lat_rad != 0 && lat_rad != 1) return fail(PF_ERR_ARG, "pf_field_errors: lat_rad must be 0 or 1");
-  if (workspace_bytes < lay.total) return fail(PF_ERR_WORKSPACE, "pf_field_errors: workspace %lld B < required %lld B", (long long)workspace_bytes, lay.total);
-  if (((uintptr_t)workspace & 255) != 0) return fail(PF_ERR_ARG, "pf_field_errors: workspace must be 256-byte aligned");
+  TRY(check_workspace("pf_field_errors", workspace, workspace_bytes, lay.total));
   std::vector<FeImage> d(n);
   long long block0 = 0, map_off = 0;
   for (int i = 0; i < n; ++i) {
     const pf_field_image& c = images[i];
-    if (c.pred_up_offset < 0 || c.pred_lat_offset < 0 || c.gt_up_offset < 0 || c.gt_lat_offset < 0 || c.mask_offset < -1)
-      return fail(PF_ERR_ARG, "pf_field_errors: image %d has a negative offset", i);
-    if (c.mask_offset >= 0 && !mask) return fail(PF_ERR_ARG, "pf_field_errors: image %d has a mask offset but mask is NULL", i);
+    TRY(check_offsets("pf_field_errors", i, {c.pred_up_offset, c.pred_lat_offset, c.gt_up_offset, c.gt_lat_offset}, {{c.mask_offset, mask}}));
     FeImage& o = d[i];
     o.H = c.height; o.W = c.width;
     o.pu_off = c.pred_up_offset; o.pu_sr = c.pred_up_stride[0]; o.pu_sc = c.pred_up_stride[1]; o.pu_sk = c.pred_up_stride[2];
@@ -1781,15 +1809,15 @@ int pf_field_errors(int device, const pf_field_image* images, int n, const float
   cudaStream_t st = (cudaStream_t)stream;
   char* ws = (char*)workspace;
   FeArgs a{};
-  a.im = (const FeImage*)(ws + lay.desc); a.n = n; a.nblocks = (int)lay.blocks;
+  a.im = (const FeImage*)ws; a.n = n; a.nblocks = (int)blocks;
   a.pu = pred_up; a.pl = pred_lat; a.gu = gt_up; a.gl = gt_lat; a.mask = mask;
   a.lat_rad = lat_rad; a.T = n_thresholds;
   for (int k = 0; k < n_thresholds; ++k) a.thr[k] = thresholds[k];
-  a.map_up = up_maps ? up_maps : (float*)(ws + lay.maps);
-  a.map_lat = lat_maps ? lat_maps : (float*)(ws + lay.maps) + lay.pixels;
-  a.psum = (double*)(ws + lay.psum); a.pcnt = (int*)(ws + lay.pcnt);
-  CU(cudaMemcpyAsync(ws + lay.desc, d.data(), n * sizeof(FeImage), cudaMemcpyHostToDevice, st));
-  LAUNCHED((field_errors_kernel<<<(unsigned)lay.blocks, kMetThreads, 0, st>>>(a), cudaGetLastError()));
+  a.map_up = up_maps ? up_maps : (float*)(ws + lay.at[3]);
+  a.map_lat = lat_maps ? lat_maps : (float*)(ws + lay.at[3]) + pixels;
+  a.psum = (double*)(ws + lay.at[1]); a.pcnt = (int*)(ws + lay.at[2]);
+  TRY(upload_descriptors(d.data(), d.size() * sizeof(d[0]), ws, st));
+  LAUNCHED((field_errors_kernel<<<(unsigned)blocks, kMetThreads, 0, st>>>(a), cudaGetLastError()));
   const FeOut o{(long long*)count, mean, median, fraction};
   LAUNCHED((field_stats_kernel<<<dim3((unsigned)n, 2), kFeSelThreads, 0, st>>>(a, o), cudaGetLastError()));
   return PF_OK;
@@ -1798,8 +1826,7 @@ int pf_field_errors(int device, const pf_field_image* images, int n, const float
 // ----------------------------------------------------------------------------------------------- camera fit (calib.cuh)
 // Workspace layout of pf_fit_camera: device descriptors | per-image state | fp64 partials [kFitQ][pass blocks]
 constexpr int kFitMaxIterations = 1000;
-struct FitLayout { long long blocks, desc, state, part, total; };
-static int fit_layout(const pf_fit_image* im, int n, FitLayout* lay) {
+static int fit_layout(const pf_fit_image* im, int n, WsLayout* lay, long long* blocks_out = nullptr) {
   if (!im || n < 1) return fail(PF_ERR_ARG, "pf_fit_camera: null images or n < 1");
   long long blocks = 0;
   for (int i = 0; i < n; ++i) {
@@ -1808,15 +1835,12 @@ static int fit_layout(const pf_fit_image* im, int n, FitLayout* lay) {
     blocks += cdivl((long long)im[i].height * im[i].width, kFitTile);
   }
   if (blocks >= (1LL << 31)) return fail(PF_ERR_ARG, "pf_fit_camera: too many pixels");
-  lay->blocks = blocks;
-  lay->desc = 0;
-  lay->state = align256((long long)n * sizeof(FitImage));
-  lay->part = lay->state + align256((long long)n * sizeof(FitState));
-  lay->total = lay->part + align256((long long)kFitQ * blocks * 8);
+  lay->add((long long)n * sizeof(FitImage)).add((long long)n * sizeof(FitState)).add((long long)kFitQ * blocks * 8);
+  if (blocks_out) *blocks_out = blocks;
   return PF_OK;
 }
 int64_t pf_fit_camera_workspace(const pf_fit_image* images, int n) {
-  FitLayout lay;
+  WsLayout lay;
   TRY(fit_layout(images, n, &lay));
   return lay.total;
 }
@@ -1831,8 +1855,9 @@ struct PdlScope {
 int pf_fit_camera(int device, const pf_fit_image* images, int n, const float* up_base, const float* lat_base, const uint8_t* mask_base,
                   int principal_point, double huber, int max_iterations, double* params, double* cost, int32_t* iterations,
                   int32_t* status, void* workspace, int64_t workspace_bytes, void* stream) {
-  FitLayout lay;
-  TRY(fit_layout(images, n, &lay));
+  WsLayout lay;
+  long long blocks;
+  TRY(fit_layout(images, n, &lay, &blocks));
   if (!up_base || !lat_base || !params || !cost || !iterations || !status || !workspace)
     return fail(PF_ERR_ARG, "pf_fit_camera: null field / output / workspace");
   if (principal_point != 0 && principal_point != 1) return fail(PF_ERR_ARG, "pf_fit_camera: principal_point must be 0 or 1");
@@ -1840,15 +1865,13 @@ int pf_fit_camera(int device, const pf_fit_image* images, int n, const float* up
     return fail(PF_ERR_ARG, "pf_fit_camera: huber must be 0 (least squares) or finite and > 0, got %g", huber);
   if (max_iterations < 1 || max_iterations > kFitMaxIterations)
     return fail(PF_ERR_ARG, "pf_fit_camera: max_iterations %d outside 1 .. %d", max_iterations, kFitMaxIterations);
-  if (workspace_bytes < lay.total) return fail(PF_ERR_WORKSPACE, "pf_fit_camera: workspace %lld B < required %lld B", (long long)workspace_bytes, lay.total);
-  if (((uintptr_t)workspace & 255) != 0) return fail(PF_ERR_ARG, "pf_fit_camera: workspace must be 256-byte aligned");
+  TRY(check_workspace("pf_fit_camera", workspace, workspace_bytes, lay.total));
   std::vector<FitImage> d(n);
   long long block0 = 0;
   for (int i = 0; i < n; ++i) {
     const pf_fit_image& c = images[i];
-    if (c.up_offset < 0 || c.lat_offset < 0 || c.mask_offset < -1 || c.up_stride[0] < 0 || c.up_stride[1] < 0 || c.up_stride[2] < 0)
-      return fail(PF_ERR_ARG, "pf_fit_camera: image %d has a negative offset or stride", i);
-    if (c.mask_offset >= 0 && !mask_base) return fail(PF_ERR_ARG, "pf_fit_camera: image %d has a mask offset but mask_base is NULL", i);
+    TRY(check_offsets("pf_fit_camera", i, {c.up_offset, c.lat_offset}, {{c.mask_offset, mask_base}}));
+    if (c.up_stride[0] < 0 || c.up_stride[1] < 0 || c.up_stride[2] < 0) return fail(PF_ERR_ARG, "pf_fit_camera: image %d has a negative stride", i);
     if (!std::isnan(c.init[0])) {
       bool fin = true;
       for (int k = 0; k < 5; ++k) fin = fin && std::isfinite(c.init[k]);
@@ -1867,14 +1890,14 @@ int pf_fit_camera(int device, const pf_fit_image* images, int n, const float* up
   cudaStream_t st = (cudaStream_t)stream;
   char* ws = (char*)workspace;
   FitArgs a{};
-  a.im = (const FitImage*)(ws + lay.desc); a.st = (FitState*)(ws + lay.state); a.n = n; a.nblocks = (int)lay.blocks;
+  a.im = (const FitImage*)ws; a.st = (FitState*)(ws + lay.at[1]); a.n = n; a.nblocks = (int)blocks;
   a.up = up_base; a.lat = lat_base; a.mask = mask_base;
   a.huber = huber; a.max_iter = max_iterations;
-  a.part = (double*)(ws + lay.part);
+  a.part = (double*)(ws + lay.at[2]);
   a.params = params; a.cost = cost; a.iters = iterations; a.status = status;
-  CU(cudaMemcpyAsync(ws + lay.desc, d.data(), n * sizeof(FitImage), cudaMemcpyHostToDevice, st));
+  TRY(upload_descriptors(d.data(), d.size() * sizeof(d[0]), ws, st));
   const PdlScope pdl(!sync_debug());
-  const dim3 pass_grid((unsigned)lay.blocks), step_grid((unsigned)cdiv(n, kFitStepWarps));
+  const dim3 pass_grid((unsigned)blocks), step_grid((unsigned)cdiv(n, kFitStepWarps));
   LAUNCHED(launch_pdl(fit_init_kernel, dim3(n), dim3(64), 0, st, a, principal_point));
   for (int it = 0; it < max_iterations; ++it) {
     if (principal_point) {
@@ -1890,8 +1913,7 @@ int pf_fit_camera(int device, const pf_fit_image* images, int n, const float* up
 
 // ----------------------------------------------------------------------------------------------- upright warp (rectify.cuh)
 // Workspace layout of pf_rectify_views: device descriptors | per-image maps
-struct RectLayout { long long desc, map, total; };
-static int rectify_layout(const pf_rectify_image* im, int n, RectLayout* lay) {
+static int rectify_layout(const pf_rectify_image* im, int n, WsLayout* lay) {
   if (!im || n < 1) return fail(PF_ERR_ARG, "pf_rectify_views: null images or n < 1");
   if (n > 65535) return fail(PF_ERR_ARG, "pf_rectify_views: %d images (at most 65535 per call)", n);
   for (int i = 0; i < n; ++i) {
@@ -1901,13 +1923,11 @@ static int rectify_layout(const pf_rectify_image* im, int n, RectLayout* lay) {
     if (c.out_height < 1 || c.out_width < 1 || (long long)c.out_height * c.out_width >= (1LL << 31))
       return fail(PF_ERR_ARG, "pf_rectify_views: image %d has output size %dx%d", i, c.out_height, c.out_width);
   }
-  lay->desc = 0;
-  lay->map = align256((long long)n * sizeof(RectImage));
-  lay->total = lay->map + align256((long long)n * sizeof(RectMap));
+  lay->add((long long)n * sizeof(RectImage)).add((long long)n * sizeof(RectMap));
   return PF_OK;
 }
 int64_t pf_rectify_workspace(const pf_rectify_image* images, int n) {
-  RectLayout lay;
+  WsLayout lay;
   TRY(rectify_layout(images, n, &lay));
   return lay.total;
 }
@@ -1915,7 +1935,7 @@ int64_t pf_rectify_workspace(const pf_rectify_image* images, int n) {
 int pf_rectify_views(int device, const pf_rectify_image* images, int n, const uint8_t* in_base, uint8_t* out_base, uint8_t* mask_base,
                      float* map_base, int channels, const double* params, int keep_pitch, int focal_mode, double vfov, int sampler,
                      const int32_t* fill, double* camera, int32_t* status, void* workspace, int64_t workspace_bytes, void* stream) {
-  RectLayout lay;
+  WsLayout lay;
   TRY(rectify_layout(images, n, &lay));
   if (!in_base || !out_base || !params || !camera || !status || !workspace)
     return fail(PF_ERR_ARG, "pf_rectify_views: null input / output / params / camera / status / workspace");
@@ -1931,16 +1951,12 @@ int pf_rectify_views(int device, const pf_rectify_image* images, int n, const ui
     if (fill[c] < 0 || fill[c] > 255) return fail(PF_ERR_ARG, "pf_rectify_views: fill[%d] = %d outside 0 .. 255", c, fill[c]);
     fv[c] = (unsigned char)fill[c];
   }
-  if (workspace_bytes < lay.total) return fail(PF_ERR_WORKSPACE, "pf_rectify_views: workspace %lld B < required %lld B", (long long)workspace_bytes, lay.total);
-  if (((uintptr_t)workspace & 255) != 0) return fail(PF_ERR_ARG, "pf_rectify_views: workspace must be 256-byte aligned");
+  TRY(check_workspace("pf_rectify_views", workspace, workspace_bytes, lay.total));
   std::vector<RectImage> d(n);
   long long max_px = 1;
   for (int i = 0; i < n; ++i) {
     const pf_rectify_image& c = images[i];
-    if (c.in_offset < 0 || c.out_offset < 0 || c.mask_offset < -1 || c.map_offset < -1)
-      return fail(PF_ERR_ARG, "pf_rectify_views: image %d has a negative offset", i);
-    if (c.mask_offset >= 0 && !mask_base) return fail(PF_ERR_ARG, "pf_rectify_views: image %d has a mask offset but mask_base is NULL", i);
-    if (c.map_offset >= 0 && !map_base) return fail(PF_ERR_ARG, "pf_rectify_views: image %d has a map offset but map_base is NULL", i);
+    TRY(check_offsets("pf_rectify_views", i, {c.in_offset, c.out_offset}, {{c.mask_offset, mask_base}, {c.map_offset, map_base}}));
     RectImage& o = d[i];
     o.H = c.height; o.W = c.width; o.Ho = c.out_height; o.Wo = c.out_width;
     o.in_off = c.in_offset; o.out_off = c.out_offset; o.mask_off = c.mask_offset; o.map_off = c.map_offset;
@@ -1951,12 +1967,12 @@ int pf_rectify_views(int device, const pf_rectify_image* images, int n, const ui
   cudaStream_t st = (cudaStream_t)stream;
   char* ws = (char*)workspace;
   RectArgs a{};
-  a.im = (const RectImage*)(ws + lay.desc); a.map = (RectMap*)(ws + lay.map); a.n = n;
+  a.im = (const RectImage*)ws; a.map = (RectMap*)(ws + lay.at[1]); a.n = n;
   a.params = params; a.camera = camera; a.status = status;
   a.keep_pitch = keep_pitch; a.focal_mode = focal_mode; a.vfov = vfov;
   a.in = in_base; a.out = out_base; a.mask = mask_base; a.xy = map_base;
   for (int c = 0; c < 3; ++c) a.fill[c] = fv[c];
-  CU(cudaMemcpyAsync(ws + lay.desc, d.data(), n * sizeof(RectImage), cudaMemcpyHostToDevice, st));
+  TRY(upload_descriptors(d.data(), d.size() * sizeof(d[0]), ws, st));
   const PdlScope pdl(!sync_debug());
   LAUNCHED(launch_pdl(rectify_setup_kernel, dim3((unsigned)cdiv(n, 128)), dim3(128), 0, st, a));
   const dim3 grid((unsigned)cdivl(max_px, (long long)kRectThreads * kRectPix), (unsigned)n);

@@ -10,10 +10,9 @@ use the helpers here.  Nothing here synchronises with the device.
 """
 import ctypes
 
-import numpy as np
 import torch
 
-from . import _native
+from . import _batch, _native
 
 MAX_THRESHOLDS = 8
 _LAT_MODES = {"deg": 0, "rad": 1}
@@ -23,19 +22,6 @@ def _lat_rad(lat_mode):
     if lat_mode not in _LAT_MODES:
         raise ValueError(f"lat_mode must be 'deg' or 'rad', got {lat_mode!r}")
     return _LAT_MODES[lat_mode]
-
-
-def _cuda_f32(t, what, device=None):
-    """A float32 CUDA tensor (on ``device`` when given), else TypeError / ValueError: there is no CPU path."""
-    if not isinstance(t, torch.Tensor):
-        raise TypeError(f"{what} must be a torch tensor, got {type(t).__name__}")
-    if t.dtype != torch.float32:
-        raise TypeError(f"{what} must be float32, got {t.dtype}")
-    if not t.is_cuda:
-        raise ValueError(f"{what} is on {t.device}: perspectivefields_b200 scores on a CUDA device only (there is no CPU path)")
-    if device is not None and t.device != device:
-        raise ValueError(f"{what} is on {t.device}, expected {device}")
-    return t
 
 
 def batch_view(ts):
@@ -79,10 +65,10 @@ def encode_fields(up, lat, gravity_classes, latitude_classes, lat_rad=0):
 def encode_bin(vector_field, num_bin):
     """utils/utils.py:94-111 on the GPU: up field(s) ``[2, H, W]`` or ``[n, 2, H, W]`` (float32 CUDA, channels (x, y)) -> int64
     bin labels ``[H, W]`` / ``[n, H, W]`` on the input's device (the reference returns them on the CPU)."""
-    v = _cuda_f32(vector_field, "vector_field")
+    v = _batch.cuda_f32(vector_field, "vector_field")
     if v.dim() not in (3, 4) or v.shape[-3] != 2:
         raise ValueError(f"vector_field must be [2, H, W] or [n, 2, H, W], got {list(v.shape)}")
-    if isinstance(num_bin, bool) or not isinstance(num_bin, (int, np.integer)) or num_bin < 3:
+    if _batch.positive_int(num_bin, "num_bin") < 3:
         raise ValueError(f"num_bin must be an integer >= 3, got {num_bin!r}")
     b = v if v.dim() == 4 else v.unsqueeze(0)
     if b.numel() == 0:
@@ -95,23 +81,16 @@ def encode_bin(vector_field, num_bin):
 def encode_bin_latitude(latimap, num_classes):
     """utils/utils.py:133-146 on the GPU: latitude map(s) in degrees ``[H, W]`` or ``[n, H, W]`` (float32 CUDA) -> int64 class
     labels of the same shape on the input's device (the reference returns them on the CPU)."""
-    v = _cuda_f32(latimap, "latimap")
+    v = _batch.cuda_f32(latimap, "latimap")
     if v.dim() not in (2, 3):
         raise ValueError(f"latimap must be [H, W] or [n, H, W], got {list(v.shape)}")
-    if isinstance(num_classes, bool) or not isinstance(num_classes, (int, np.integer)) or num_classes < 2:
+    if _batch.positive_int(num_classes, "num_classes") < 2:
         raise ValueError(f"num_classes must be an integer >= 2, got {num_classes!r}")
     b = v if v.dim() == 3 else v.unsqueeze(0)
     if b.numel() == 0:
         return torch.empty(v.shape, dtype=torch.int64, device=v.device)
     _, gl = encode_fields(None, (b, b.stride(), b.shape[1], b.shape[2]), 2, int(num_classes))
     return gl if v.dim() == 3 else gl[0]
-
-
-def _base(tensors):
-    """Common base address of device tensors: descriptors address them by (data_ptr - base) / element size, so one library call
-    reads them in place (one flat device address space)."""
-    ptrs = [t.data_ptr() for t in tensors if t is not None]
-    return min(ptrs) if ptrs else 0
 
 
 def field_errors(results, up, lat, lat_mode="deg", mask=None, thresholds=(1.0, 5.0, 10.0), return_maps=False):
@@ -139,53 +118,36 @@ def field_errors(results, up, lat, lat_mode="deg", mask=None, thresholds=(1.0, 5
         raise ValueError(f"{n} results but {len(up)} up fields, {len(lat)} latitude maps" + ("" if mask is None else f", {len(mask)} masks"))
     T = len(thr)
     if n == 0:
-        dev = torch.device("cuda", torch.cuda.current_device())
+        dev = _batch.device(__name__)
         empty = lambda: {"count": torch.empty(0, dtype=torch.int64, device=dev), "mean": torch.empty(0, dtype=torch.float64, device=dev),
                          "median": torch.empty(0, dtype=torch.float64, device=dev), "fraction": torch.empty((0, T), dtype=torch.float64, device=dev)}
         out = {"up": empty(), "latitude": empty()}
         if return_maps:
             out["up"]["map"], out["latitude"]["map"] = [], []
         return out
-    pu = [_cuda_f32(r["pred_gravity_original"], f"results[{i}]['pred_gravity_original']") for i, r in enumerate(results)]
-    dev = pu[0].device
-    pl = [_cuda_f32(r["pred_latitude_original"], f"results[{i}]['pred_latitude_original']", dev) for i, r in enumerate(results)]
-    gu = [_cuda_f32(u, f"up[{i}]", dev) for i, u in enumerate(up)]
-    gl = [_cuda_f32(v, f"lat[{i}]", dev) for i, v in enumerate(lat)]
-    ms = [None] * n if mask is None else list(mask)
+    pu, pl, ms, dev = _batch.prediction_fields(results, mask, 1)
+    gu = [_batch.cuda_f32(u, f"up[{i}]", dev) for i, u in enumerate(up)]
+    gl = [_batch.cuda_f32(v, f"lat[{i}]", dev) for i, v in enumerate(lat)]
     for i in range(n):
-        if pu[i].dim() != 3 or pu[i].shape[0] != 2:
-            raise ValueError(f"results[{i}]['pred_gravity_original'] must be [2, H, W], got {list(pu[i].shape)}")
-        h, w = int(pu[i].shape[1]), int(pu[i].shape[2])
-        if h < 1 or w < 1:
-            raise ValueError(f"image {i} has size {h}x{w}")
-        if tuple(pl[i].shape) != (h, w):
-            raise ValueError(f"results[{i}]['pred_latitude_original'] must be [{h}, {w}], got {list(pl[i].shape)}")
+        h, w = int(pu[i].shape[0]), int(pu[i].shape[1])
         if tuple(gu[i].shape) != (h, w, 2):
             raise ValueError(f"up[{i}] must be [{h}, {w}, 2], got {list(gu[i].shape)}")
         if tuple(gl[i].shape) != (h, w):
             raise ValueError(f"lat[{i}] must be [{h}, {w}], got {list(gl[i].shape)}")
-        if ms[i] is not None:
-            m = ms[i]
-            if not isinstance(m, torch.Tensor) or m.dtype != torch.bool or tuple(m.shape) != (h, w) or m.device != dev:
-                raise ValueError(f"mask[{i}] must be a bool [{h}, {w}] tensor on {dev}")
-            ms[i] = m.contiguous().view(torch.uint8)
-        pl[i], gl[i] = pl[i].contiguous(), gl[i].contiguous()
+        gl[i] = gl[i].contiguous()
     L = _native.lib()
-    bpu, bpl, bgu, bgl, bm = _base(pu), _base(pl), _base(gu), _base(gl), _base(ms)
+    bpu, bpl, bgu, bgl, bm = _batch.base(pu), _batch.base(pl), _batch.base(gu), _batch.base(gl), _batch.base(ms)
     descs = (_native.pf_field_image * n)()
     for i in range(n):
         d = descs[i]
-        d.height, d.width = int(pu[i].shape[1]), int(pu[i].shape[2])
-        d.pred_up_offset = (pu[i].data_ptr() - bpu) // 4
-        d.pred_up_stride[0], d.pred_up_stride[1], d.pred_up_stride[2] = pu[i].stride(1), pu[i].stride(2), pu[i].stride(0)
-        d.pred_lat_offset = (pl[i].data_ptr() - bpl) // 4
-        d.gt_up_offset = (gu[i].data_ptr() - bgu) // 4
-        d.gt_up_stride[0], d.gt_up_stride[1], d.gt_up_stride[2] = gu[i].stride(0), gu[i].stride(1), gu[i].stride(2)
-        d.gt_lat_offset = (gl[i].data_ptr() - bgl) // 4
-        d.mask_offset = -1 if ms[i] is None else ms[i].data_ptr() - bm
+        d.height, d.width = int(pu[i].shape[0]), int(pu[i].shape[1])
+        d.pred_up_offset, d.pred_up_stride[:] = _batch.offset(pu[i], bpu), pu[i].stride()
+        d.pred_lat_offset = _batch.offset(pl[i], bpl)
+        d.gt_up_offset, d.gt_up_stride[:] = _batch.offset(gu[i], bgu), gu[i].stride()
+        d.gt_lat_offset = _batch.offset(gl[i], bgl)
+        d.mask_offset = _batch.offset(ms[i], bm)
     with torch.cuda.device(dev):
-        need = _native.check(L.pf_field_errors_workspace(descs, n, int(bool(return_maps))))
-        ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        ws = _batch.workspace(L.pf_field_errors_workspace(descs, n, int(bool(return_maps))), dev)
         total = sum(d.height * d.width for d in descs)
         maps = torch.empty((2, total), dtype=torch.float32, device=dev) if return_maps else None
         count = torch.empty((2, n), dtype=torch.int64, device=dev)

@@ -21,7 +21,7 @@ import os
 import numpy as np
 import torch
 
-from . import _native
+from . import _batch, _native
 
 
 def general_vfov(d_cx, d_cy, h, focal, degree):
@@ -69,49 +69,31 @@ def camera_fields(focal_rel, heights, widths, elevation, roll, cx_rel, cy_rel, d
     fields point to instead, (nan, nan) keeping the camera's own (``PanoCam.get_up`` at elevation 0).
     Returns (list of [H_i, W_i, 2] float32 tensors or None, list of [H_i, W_i] float32 tensors in degrees or None)."""
     L = _native.lib()
-    if not torch.cuda.is_available():
-        raise RuntimeError("perspectivefields_b200.panocam needs a CUDA device (there is no CPU path)")
-    dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-    if dev.type != "cuda":
-        raise RuntimeError("perspectivefields_b200.panocam needs a CUDA device (there is no CPU path)")
+    dev = _batch.device(__name__, (), device)
     n = len(heights)
+    sizes = [(int(h), int(w)) for h, w in zip(heights, widths)]
+    up_offs, up_total = _batch.layout([2 * h * w for h, w in sizes])
+    lat_offs, lat_total = _batch.layout([h * w for h, w in sizes])
     cams = (_native.pf_camera * n)()
-    up_off = lat_off = 0
-    for i in range(n):
-        h, w = int(heights[i]), int(widths[i])
+    for i, (h, w) in enumerate(sizes):
         cams[i] = _native.pf_camera(h, w, float(focal_rel[i]), float(elevation[i]), float(roll[i]), float(cx_rel[i]), float(cy_rel[i]),
-                                    up_off, lat_off)
-        up_off += 2 * h * w
-        lat_off += h * w
+                                    up_offs[i], lat_offs[i])
     with torch.cuda.device(dev):
-        up_blob = torch.empty(up_off, dtype=torch.float32, device=dev) if up else None
-        lat_blob = torch.empty(lat_off, dtype=torch.float32, device=dev) if lat else None
+        up_blob = torch.empty(up_total, dtype=torch.float32, device=dev) if up else None
+        lat_blob = torch.empty(lat_total, dtype=torch.float32, device=dev) if lat else None
         stream = torch.cuda.current_stream(dev).cuda_stream
-        index = dev.index if dev.index is not None else torch.cuda.current_device()
         up_ptr, lat_ptr = up_blob.data_ptr() if up else None, lat_blob.data_ptr() if lat else None
         if vp is None:
-            _native.check(L.pf_camera_fields(index, cams, n, up_ptr, lat_ptr, stream))
+            _native.check(L.pf_camera_fields(dev.index, cams, n, up_ptr, lat_ptr, stream))
         else:
             vps = (ctypes.c_double * (2 * n))(*[float(c) for p in vp for c in p])
-            _native.check(L.pf_camera_fields_vp(index, cams, vps, n, up_ptr, lat_ptr, stream))
-    ups = [up_blob[c.up_offset:c.up_offset + 2 * c.height * c.width].view(c.height, c.width, 2) for c in cams] if up else None
-    lats = [lat_blob[c.lat_offset:c.lat_offset + c.height * c.width].view(c.height, c.width) for c in cams] if lat else None
+            _native.check(L.pf_camera_fields_vp(dev.index, cams, vps, n, up_ptr, lat_ptr, stream))
+    ups = _batch.views(up_blob, up_offs, [(h, w, 2) for h, w in sizes]) if up else None
+    lats = _batch.views(lat_blob, lat_offs, sizes) if lat else None
     return ups, lats
 
 
 PANO_OUTPUTS = ("ntheta", "nphi", "up", "lat", "xy_map")
-
-
-def _real(x, name):
-    if isinstance(x, (bool, np.bool_)) or not isinstance(x, (int, float, np.integer, np.floating)) or not math.isfinite(float(x)):
-        raise ValueError(f"{name} must be a finite real number, got {x!r}")
-    return float(x)
-
-
-def _size(x, name):
-    if isinstance(x, (bool, np.bool_)) or not isinstance(x, (int, np.integer)) or int(x) < 1:
-        raise ValueError(f"{name} must be a positive integer, got {x!r}")
-    return int(x)
 
 
 def _check_view(view, i):
@@ -126,11 +108,11 @@ def _check_view(view, i):
     if len(view) != 7:
         raise ValueError(f"view {i}: expected (f, xi, H, W, az, el, roll), got {len(view)} values")
     f, xi, h, w, az, el, roll = view
-    f = _real(f, f"view {i}: f")
+    f = _batch.real(f, f"view {i}: f")
     if f <= 0:
         raise ValueError(f"view {i}: f must be > 0, got {f}")
-    return (f, _real(xi, f"view {i}: xi"), _size(h, f"view {i}: H"), _size(w, f"view {i}: W"), _real(az, f"view {i}: az"),
-            _real(el, f"view {i}: el"), _real(roll, f"view {i}: roll"))
+    return (f, _batch.real(xi, f"view {i}: xi"), _batch.positive_int(h, f"view {i}: H"), _batch.positive_int(w, f"view {i}: W"), _batch.real(az, f"view {i}: az"),
+            _batch.real(el, f"view {i}: el"), _batch.real(roll, f"view {i}: roll"))
 
 
 def _check_panorama(image360):
@@ -171,41 +153,30 @@ def crop_distortion_views(image360, views, outputs=("up", "lat"), device=None):
     if not vs:
         raise ValueError("no views")
     pano = _check_panorama(image360)
-    if not torch.cuda.is_available():
-        raise RuntimeError("perspectivefields_b200.panocam needs a CUDA device (there is no CPU path)")
+    dev = _pano_device(pano, device)
     L = _native.lib()
-    if isinstance(pano, torch.Tensor) and pano.is_cuda:
-        if device is not None and torch.device(device) != pano.device:
-            raise ValueError(f"the panorama is on {pano.device}, not on {device}")
-        dev = pano.device
-    else:
-        dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        if dev.type != "cuda":
-            raise RuntimeError("perspectivefields_b200.panocam needs a CUDA device (there is no CPU path)")
-        if dev.index is None:
-            dev = torch.device("cuda", torch.cuda.current_device())
     n = len(vs)
+    # 16-byte aligned crops and 4-float aligned fields: full-width vector stores
+    im_offs, im_total = _batch.layout([3 * v[2] * v[3] for v in vs], 16)
+    fld_offs, fld_total = _batch.layout([v[2] * v[3] for v in vs], 4)
     descs = (_native.pf_pano_view * n)()
-    im_off = fld_off = 0
     for i, (f, xi, h, w, az, el, roll) in enumerate(vs):
-        descs[i] = _native.pf_pano_view(h, w, f, xi, az, el, roll, im_off, fld_off)
-        im_off += (3 * h * w + 15) // 16 * 16          # 16-byte aligned crops and 4-float aligned fields: full-width vector stores
-        fld_off += (h * w + 3) // 4 * 4
+        descs[i] = _native.pf_pano_view(h, w, f, xi, az, el, roll, im_offs[i], fld_offs[i])
     with torch.cuda.device(dev):
         src = torch.as_tensor(pano).to(dev).contiguous()
-        im = torch.empty(im_off, dtype=torch.uint8, device=dev)
-        blobs = {o: torch.empty((2 if o in ("up", "xy_map") else 1) * fld_off, dtype=torch.float32, device=dev) for o in outputs}
+        im = torch.empty(im_total, dtype=torch.uint8, device=dev)
+        blobs = {o: torch.empty((2 if o in ("up", "xy_map") else 1) * fld_total, dtype=torch.float32, device=dev) for o in outputs}
         offset = torch.empty(n, dtype=torch.float64, device=dev)
         status = torch.empty(n, dtype=torch.int32, device=dev)
         ptr = lambda o: blobs[o].data_ptr() if o in blobs else None
         stream = torch.cuda.current_stream(dev).cuda_stream
         _native.check(L.pf_pano_views(dev.index, src.data_ptr(), src.shape[0], src.shape[1], descs, n, im.data_ptr(), ptr("ntheta"),
                                       ptr("nphi"), ptr("up"), ptr("lat"), ptr("xy_map"), offset.data_ptr(), status.data_ptr(), stream))
-    out = {"im": [im[d.im_offset:d.im_offset + 3 * d.height * d.width].view(d.height, d.width, 3) for d in descs]}
+    hw = [(v[2], v[3]) for v in vs]
+    out = {"im": _batch.views(im, im_offs, [(h, w, 3) for h, w in hw])}
     for o in outputs:
-        c = 2 if o in ("up", "xy_map") else 1
-        out[o] = [blobs[o][c * d.field_offset:c * (d.field_offset + d.height * d.width)].view((d.height, d.width, 2) if c == 2 else (d.height, d.width))
-                  for d in descs]
+        two = o in ("up", "xy_map")
+        out[o] = _batch.views(blobs[o], [2 * f for f in fld_offs] if two else fld_offs, [(h, w, 2) if two else (h, w) for h, w in hw])
     out["offset"], out["status"] = offset, status
     return out
 
@@ -229,7 +200,7 @@ def _check_equi_view(view, i):
     if len(view) != 7:
         raise ValueError(f"view {i}: expected (vfov, im_w, im_h, azimuth, elevation, roll, ar), got {len(view)} values")
     vfov, w, h, az, el, roll, ar = view
-    vfov, ar = _real(vfov, f"view {i}: vfov"), _real(ar, f"view {i}: ar")
+    vfov, ar = _batch.real(vfov, f"view {i}: vfov"), _batch.real(ar, f"view {i}: ar")
     if not 0.0 < vfov < 180.0:
         raise ValueError(f"view {i}: vfov must lie in (0, 180) degrees, got {vfov}")
     if ar <= 0.0:
@@ -237,8 +208,8 @@ def _check_equi_view(view, i):
     fov_x = 2 * math.atan(math.tan(vfov * math.pi / 180.0 / 2) * ar) * 180 / math.pi
     if not fov_x < 180.0:
         raise ValueError(f"view {i}: the horizontal field of view 2 atan(tan(vfov / 2) ar) = {fov_x} degrees must be < 180")
-    return (vfov, _size(w, f"view {i}: im_w"), _size(h, f"view {i}: im_h"), _real(az, f"view {i}: azimuth"),
-            _real(el, f"view {i}: elevation"), _real(roll, f"view {i}: roll"), ar)
+    return (vfov, _batch.positive_int(w, f"view {i}: im_w"), _batch.positive_int(h, f"view {i}: im_h"), _batch.real(az, f"view {i}: azimuth"),
+            _batch.real(el, f"view {i}: elevation"), _batch.real(roll, f"view {i}: roll"), ar)
 
 
 def _check_equi_panorama(equi_img):
@@ -261,16 +232,9 @@ def _check_equi_panorama(equi_img):
 def _pano_device(pano, device):
     """The CUDA device a call runs on: the panorama's own when it is a CUDA tensor (``device`` must agree), else ``device`` or the
     current one."""
-    if not torch.cuda.is_available():
-        raise RuntimeError("perspectivefields_b200.panocam needs a CUDA device (there is no CPU path)")
-    if isinstance(pano, torch.Tensor) and pano.is_cuda:
-        if device is not None and torch.device(device) != pano.device:
-            raise ValueError(f"the panorama is on {pano.device}, not on {device}")
-        return pano.device
-    dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-    if dev.type != "cuda":
-        raise RuntimeError("perspectivefields_b200.panocam needs a CUDA device (there is no CPU path)")
-    return torch.device("cuda", torch.cuda.current_device()) if dev.index is None else dev
+    if isinstance(pano, torch.Tensor) and pano.is_cuda and device is not None and torch.device(device) != pano.device:
+        raise ValueError(f"the panorama is on {pano.device}, not on {device}")
+    return _batch.device(__name__, [pano], device)
 
 
 def horizon_vvp(vfov, im_w, im_h, elevation, roll):
@@ -300,21 +264,20 @@ def _equi_views(equi_img, views, outputs, mode, img_format, unit, device):
     dev = _pano_device(pano, device)
     L = _native.lib()
     n = len(vs)
+    tdt = torch.float32 if dtype == _native.PF_EQUI_F32 else torch.uint8
     esize = 4 if dtype == _native.PF_EQUI_F32 else 1
+    shapes = [(v[2], v[1], 3) if channels == 3 else (v[2], v[1]) for v in vs]
+    offs, total = _batch.layout([math.prod(s) * esize for s in shapes], 16)     # 16-byte aligned crops: full-width vector stores
     descs = (_native.pf_equi_view * n)()
-    off = 0
     for i, (vfov, w, h, az, el, roll, ar) in enumerate(vs):
-        descs[i] = _native.pf_equi_view(h, w, vfov, az, el, roll, ar, off)
-        off += (channels * h * w * esize + 15) // 16 * 16        # 16-byte aligned crops: full-width vector stores
+        descs[i] = _native.pf_equi_view(h, w, vfov, az, el, roll, ar, offs[i])
     with torch.cuda.device(dev):
         src = torch.as_tensor(pano).to(dev).contiguous()
-        blob = torch.empty(off, dtype=torch.uint8, device=dev)
+        blob = torch.empty(total, dtype=torch.uint8, device=dev)
         stream = torch.cuda.current_stream(dev).cuda_stream
         _native.check(L.pf_equi_views(dev.index, src.data_ptr(), src.shape[0], src.shape[1], channels, dtype, descs, n, EQUI_MODES[mode],
                                       _native.PF_EQUI_UNIT if unit else _native.PF_EQUI_CAST, int(swap), blob.data_ptr(), stream))
-    tdt = torch.float32 if dtype == _native.PF_EQUI_F32 else torch.uint8
-    shape = (lambda d: (d.height, d.width, 3)) if channels == 3 else (lambda d: (d.height, d.width))
-    out = {"im": [blob[d.offset:d.offset + channels * d.height * d.width * esize].view(tdt).view(shape(d)) for d in descs]}
+    out = {"im": _batch.views(blob.view(tdt), [o // esize for o in offs], shapes)}
     if outputs:
         ups, lats = pinhole_fields([_rad(v[0]) for v in vs], [v[2] for v in vs], [v[1] for v in vs], [_rad(v[4]) for v in vs],
                                    [_rad(v[5]) for v in vs], dev, up="up" in outputs, lat="lat" in outputs)

@@ -13,7 +13,7 @@ import numpy as np
 import torch
 from torch import nn
 
-from . import _native
+from . import _batch, _native
 from .checkpoint import checkpoint_schema, default_state, load_zoo_checkpoint
 from .variants import PIXEL_MEAN, PIXEL_STD, RESIZE, VARIANTS, make_cfg, model_zoo
 from .weights import repack
@@ -534,12 +534,6 @@ class PerspectiveFields(nn.Module):
         return res
 
     # ------------------------------------------------------------------------------------------ scoring API
-    def _scoring_device(self):
-        dev = self.device
-        if dev.type != "cuda":
-            raise RuntimeError("perspectivefields_b200 has no CPU path: move the model to an H100 with .cuda() first")
-        return torch.device("cuda", torch.cuda.current_device()) if dev.index is None else dev
-
     def targets_from_fields(self, up, lat, lat_mode="deg"):
         """Ground-truth fields -> the reference's targets dict ``{"gt_gravity", "gt_latitude"}`` (persformer_heads.py:60-70) for
         ``losses``.  ``up``: list of float32 CUDA [H, W, 2] up fields, ``lat``: list of [H, W] latitude maps (``lat_mode`` "deg"
@@ -553,11 +547,11 @@ class PerspectiveFields(nn.Module):
         n = len(up)
         if n == 0 or len(lat) != n:
             raise ValueError(f"targets_from_fields needs as many latitude maps as up fields (>= 1), got {len(up)} and {len(lat)}")
-        dev = self._scoring_device()
+        dev = _batch.device(__name__, (), self.device)
         h, w = self._net_hw
         for i in range(n):
-            metrics._cuda_f32(up[i], f"up[{i}]", dev)
-            metrics._cuda_f32(lat[i], f"lat[{i}]", dev)
+            _batch.cuda_f32(up[i], f"up[{i}]", dev)
+            _batch.cuda_f32(lat[i], f"lat[{i}]", dev)
             if tuple(up[i].shape) != (h, w, 2) or tuple(lat[i].shape) != (h, w):
                 raise ValueError(f"field {i}: up {list(up[i].shape)} / lat {list(lat[i].shape)}; the working size needs [{h}, {w}, 2] / [{h}, {w}]")
         u, la = metrics.batch_view(list(up)), metrics.batch_view(list(lat))
@@ -581,12 +575,12 @@ class PerspectiveFields(nn.Module):
         n = len(results)
         if n == 0:
             raise ValueError("no results")
-        dev = self._scoring_device()
+        dev = _batch.device(__name__, (), self.device)
         h, w = self._net_hw
         gc, lc = self._variant["gravity_classes"], self._variant["latitude_classes"]
         preds = []
         for key, c in (("pred_gravity", gc), ("pred_latitude", lc)):
-            ts = [metrics._cuda_f32(r[key], f"results[{i}][{key!r}]", dev) for i, r in enumerate(results)]
+            ts = [_batch.cuda_f32(r[key], f"results[{i}][{key!r}]", dev) for i, r in enumerate(results)]
             for i, t in enumerate(ts):
                 if tuple(t.shape) != (c, h, w):
                     raise ValueError(f"results[{i}][{key!r}] is {list(t.shape)}, the model's is [{c}, {h}, {w}]")
@@ -608,8 +602,7 @@ class PerspectiveFields(nn.Module):
         ig, il = int(mc.GRAVITY_DECODER.IGNORE_VALUE), int(mc.LATITUDE_DECODER.IGNORE_VALUE)
         L = _native.lib()
         with torch.cuda.device(dev):
-            need = _native.check(L.pf_head_losses_workspace(n, h, w, gc, lc))
-            ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            ws = _batch.workspace(L.pf_head_losses_workspace(n, h, w, gc, lc), dev)
             keys = (("gravity-msg-normal-loss", "gravity-l2-loss", "latitude-msg-normal-loss", "latitude-l2-loss") if gc == 2
                     else ("loss_gravity", "loss_latitude"))
             out = torch.empty(len(keys), dtype=torch.float32, device=dev)

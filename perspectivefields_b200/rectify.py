@@ -12,17 +12,13 @@ import numbers
 import numpy as np
 import torch
 
-from . import _native
+from . import _batch, _native
 
 CAMERA_KEYS = ("pred_roll", "pred_pitch", "pred_general_vfov", "pred_rel_cx", "pred_rel_cy")
 OUTPUT_KEYS = ("pred_roll", "pred_pitch", "pred_vfov", "pred_rel_focal", "pred_general_vfov", "pred_rel_cx", "pred_rel_cy")
 MODES = {"bilinear": _native.PF_RECTIFY_BILINEAR, "nearest": _native.PF_RECTIFY_NEAREST}
 OUTPUTS = ("mask", "map")
 _REAL_DTYPES = (torch.float64, torch.float32, torch.float16, torch.bfloat16, torch.int32, torch.int64)
-
-
-def _align16(nbytes):
-    return (nbytes + 15) // 16 * 16
 
 
 def _real_number(x):
@@ -108,9 +104,12 @@ def _check_size(size, images):
             out.append((int(images[i].shape[0]), int(images[i].shape[1])))
             continue
         s = tuple(s)
-        if len(s) != 2 or any(isinstance(x, bool) or not isinstance(x, (int, np.integer)) or x < 1 for x in s) or s[0] * s[1] >= 1 << 31:
+        if len(s) != 2:
             raise ValueError(f"size[{i}] must be two positive integers, got {s!r}")
-        out.append((int(s[0]), int(s[1])))
+        h, w = _batch.positive_int(s[0], f"size[{i}][0]"), _batch.positive_int(s[1], f"size[{i}][1]")
+        if h * w >= 1 << 31:
+            raise ValueError(f"size[{i}] is {h} x {w}: too large")
+        out.append((h, w))
     return out
 
 
@@ -123,9 +122,7 @@ def _params(cols, n, dev):
             if not isinstance(v, torch.Tensor):
                 host[i, j] = v
                 any_host = True
-    up = None
-    if any_host:
-        up = torch.from_numpy(host).pin_memory().to(dev, non_blocking=True)
+    up = _batch.upload([host], torch.float64, dev)[0] if any_host else None
     out = []
     for j, k in enumerate(CAMERA_KEYS):
         col = cols[k]
@@ -187,50 +184,27 @@ def upright(images, cameras, keep_pitch=False, focal="same", size=None, mode="bi
         raise ValueError(f"fill must be an integer in 0 .. 255 or one per channel ({channels}), got {fill!r}")
     sizes = _check_size(size, imgs)
     cols = _check_cameras(cameras, n, dev)
-    if dev is None:
-        devs = {v.device for k in CAMERA_KEYS for v in cols[k] if isinstance(v, torch.Tensor)}
-        if len(devs) > 1:
-            raise ValueError("the cameras are on more than one CUDA device")
-        if not torch.cuda.is_available():
-            raise RuntimeError("perspectivefields_b200.rectify needs a CUDA device (there is no CPU path)")
-        dev = devs.pop() if devs else torch.device("cuda", torch.cuda.current_device())
-    if dev.index is None:
-        dev = torch.device("cuda", torch.cuda.current_device())
+    cam_tensors = [v for k in CAMERA_KEYS for v in cols[k] if isinstance(v, torch.Tensor)]
+    if dev is None and len({v.device for v in cam_tensors}) > 1:
+        raise ValueError("the cameras are on more than one CUDA device")
+    dev = _batch.device(__name__, imgs[:1] + cam_tensors[:1])
     L = _native.lib()
+    out_offs, out_total = _batch.layout([channels * ho * wo for ho, wo in sizes], 16)
+    mask_offs, mask_total = _batch.layout([ho * wo for ho, wo in sizes], 16) if "mask" in outputs else ([-1] * n, 0)
+    map_offs, map_total = _batch.layout([2 * ho * wo for ho, wo in sizes], 4) if "map" in outputs else ([-1] * n, 0)
     descs = (_native.pf_rectify_image * n)()
-    out_off = mask_off = map_off = 0
     for i, (im, (ho, wo)) in enumerate(zip(imgs, sizes)):
-        d = descs[i]
-        d.height, d.width, d.out_height, d.out_width = int(im.shape[0]), int(im.shape[1]), ho, wo
-        d.out_offset = out_off
-        out_off += _align16(channels * ho * wo)
-        d.mask_offset = mask_off if "mask" in outputs else -1
-        mask_off += _align16(ho * wo)
-        d.map_offset = map_off if "map" in outputs else -1
-        map_off += _align16(8 * ho * wo) // 4
+        descs[i] = _native.pf_rectify_image(int(im.shape[0]), int(im.shape[1]), ho, wo, 0, out_offs[i], mask_offs[i], map_offs[i])
     with torch.cuda.device(dev):
-        if isinstance(imgs[0], torch.Tensor):
-            src = [im.contiguous() for im in imgs]
-            base = min(t.data_ptr() for t in src)
-            for i, t in enumerate(src):
-                descs[i].in_offset = t.data_ptr() - base
-        else:
-            offs = np.zeros(n, np.int64)
-            np.cumsum([im.size for im in imgs[:-1]], out=offs[1:])
-            host = torch.empty(int(offs[-1]) + imgs[-1].size, dtype=torch.uint8).pin_memory()
-            hn = host.numpy()
-            for im, o in zip(imgs, offs):
-                hn[o:o + im.size] = np.ascontiguousarray(im).reshape(-1)
-            for i in range(n):
-                descs[i].in_offset = int(offs[i])
-            src = [host.to(dev, non_blocking=True)]
-            base = src[0].data_ptr()
+        src = [im.contiguous() for im in imgs] if isinstance(imgs[0], torch.Tensor) else _batch.upload(imgs, torch.uint8, dev)
+        base = _batch.base(src)
+        for d, t in zip(descs, src):
+            d.in_offset = t.data_ptr() - base
         params = _params(cols, n, dev)
-        need = _native.check(L.pf_rectify_workspace(descs, n))
-        ws = torch.empty(need, dtype=torch.uint8, device=dev)
-        blob = torch.empty(out_off, dtype=torch.uint8, device=dev)
-        mblob = torch.empty(mask_off, dtype=torch.uint8, device=dev) if "mask" in outputs else None
-        xblob = torch.empty(map_off, dtype=torch.float32, device=dev) if "map" in outputs else None
+        ws = _batch.workspace(L.pf_rectify_workspace(descs, n), dev)
+        blob = torch.empty(out_total, dtype=torch.uint8, device=dev)
+        mblob = torch.empty(mask_total, dtype=torch.uint8, device=dev) if "mask" in outputs else None
+        xblob = torch.empty(map_total, dtype=torch.float32, device=dev) if "map" in outputs else None
         cam = torch.empty((n, 5), dtype=torch.float64, device=dev)
         status = torch.empty(n, dtype=torch.int32, device=dev)
         fv = (ctypes.c_int32 * 3)(*[int(v) for v in fills] + [0] * (3 - channels))
@@ -242,13 +216,11 @@ def upright(images, cameras, keep_pitch=False, focal="same", size=None, mode="bi
         roll, pitch, gv, cx, cy = cam.t()
         f = 0.5 / torch.tan(torch.deg2rad(gv) / 2.0)
         cols_out = torch.stack([roll, pitch, gv, f, gv, cx, cy]).t().unbind(0)
-    shape = (lambda d: (d.out_height, d.out_width, 3)) if channels == 3 else (lambda d: (d.out_height, d.out_width))
-    res = {"im": [blob[d.out_offset:d.out_offset + channels * d.out_height * d.out_width].view(shape(d)) for d in descs]}
+    res = {"im": _batch.views(blob, out_offs, [(ho, wo, 3) if channels == 3 else (ho, wo) for ho, wo in sizes])}
     if mblob is not None:
-        res["mask"] = [mblob[d.mask_offset:d.mask_offset + d.out_height * d.out_width].view(torch.bool).view(d.out_height, d.out_width)
-                       for d in descs]
+        res["mask"] = _batch.views(mblob.view(torch.bool), mask_offs, sizes)
     if xblob is not None:
-        res["map"] = [xblob[d.map_offset:d.map_offset + 2 * d.out_height * d.out_width].view(d.out_height, d.out_width, 2) for d in descs]
+        res["map"] = _batch.views(xblob, map_offs, [(ho, wo, 2) for ho, wo in sizes])
     res["camera"] = [dict(zip(OUTPUT_KEYS, c.unbind(0))) for c in cols_out]
     res["status"] = status
     return res

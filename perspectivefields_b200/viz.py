@@ -21,7 +21,7 @@ import os
 import numpy as np
 import torch
 
-from . import _native
+from . import _batch, _native
 from . import panocam
 
 
@@ -131,15 +131,11 @@ def _check_image(img, i):
 
 def _check_up(up, h, w, i):
     """[2, H, W] torch tensor (the reference's torch branch) or [H, W, 2] (numpy, or a tensor such as PanoCam.get_up's) ->
-    (float32 tensor or numpy array, (row, column, component) element strides of the [H, W, 2] view)."""
+    float32 tensor ([H, W, 2] view) or numpy array."""
     if isinstance(up, torch.Tensor):
-        shape = tuple(up.shape)
-        if shape == (2, h, w):
-            t = up.permute(1, 2, 0)
-        elif shape == (h, w, 2):
-            t = up
-        else:
-            raise ValueError(f"up field {i}: expected [2, {h}, {w}] or [{h}, {w}, 2], got {list(shape)}")
+        t = _batch.up_view(up, h, w)
+        if t is None:
+            raise ValueError(f"up field {i}: expected [2, {h}, {w}] or [{h}, {w}, 2], got {list(up.shape)}")
         if not t.is_floating_point():
             raise ValueError(f"up field {i}: expected a float tensor, got {t.dtype}")
         return t
@@ -156,34 +152,18 @@ def _check_lat(lat, h, w, i):
     return lat
 
 
-def _check_unit(x, name):
-    if isinstance(x, (bool, np.bool_)) or not isinstance(x, (int, float, np.integer, np.floating)) or not 0.0 <= float(x) <= 1.0:
-        raise ValueError(f"{name} must be a number in [0, 1], got {x!r}")
-    return float(x)
-
-
 def _check_color(color, default):
     color = default if color is None else tuple(color)
     if len(color) != 3:
         raise ValueError(f"color must be an (r, g, b) triple in [0, 1], got {color!r}")
-    return tuple(_check_unit(c, "color component") for c in color)
+    return tuple(_batch.unit(c, "color component") for c in color)
 
 
 def _check_lattice(density, arrow_inv_len, h, w, i):
-    for v, name in ((density, "density"), (arrow_inv_len, "arrow_inv_len")):
-        if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or v < 1:
-            raise ValueError(f"{name} must be a positive integer, got {v!r}")
+    _batch.positive_int(density, "density")
+    _batch.positive_int(arrow_inv_len, "arrow_inv_len")
     if w // density == 0 or h // density == 0:
         raise ValueError(f"canvas {i} ({h} x {w}): density {density} leaves no arrow step (W // density or H // density is 0)")
-
-
-def _device_of(tensors):
-    for t in tensors:
-        if isinstance(t, torch.Tensor) and t.is_cuda:
-            return t.device
-    if not torch.cuda.is_available():
-        raise RuntimeError("perspectivefields_b200.viz needs a CUDA device (there is no CPU path)")
-    return torch.device("cuda", torch.cuda.current_device())
 
 
 def _on_device(items, dtype, dev):
@@ -200,28 +180,17 @@ def _on_device(items, dtype, dev):
         else:
             host.append(k)
     if host:
-        arrs = [np.ascontiguousarray(items[k].cpu().numpy() if isinstance(items[k], torch.Tensor) else items[k],
-                                     dtype=torch.empty(0, dtype=dtype).numpy().dtype) for k in host]
-        blob = torch.from_numpy(np.concatenate([a.reshape(-1) for a in arrs])).to(dev)
-        off = 0
-        for k, a in zip(host, arrs):
-            out[k] = blob[off:off + a.size].view(a.shape)
-            off += a.size
+        arrs = [items[k].cpu().numpy() if isinstance(items[k], torch.Tensor) else items[k] for k in host]
+        for k, t in zip(host, _batch.upload(arrs, dtype, dev)):
+            out[k] = t
     return out
-
-
-def _base(tensors):
-    """Common base address of a list of device tensors: descriptors address them by (data_ptr - base) / element size, so one
-    library call reads them in place (one flat device address space)."""
-    ptrs = [t.data_ptr() for t in tensors if t is not None]
-    return min(ptrs) if ptrs else 0
 
 
 def _draw(imgs, ups, lats, colors, density, arrow_inv_len, alpha_fill, alpha_line, in_place=False):
     """Checked inputs -> list of CUDA uint8 [H, W, 3] canvases drawn by one pf_draw_fields call.  ``in_place``: the images are
     CUDA tensors that receive the drawing."""
     n = len(imgs)
-    dev = _device_of(list(imgs) + [u for u in ups if u is not None] + [l for l in lats if l is not None])
+    dev = _batch.device(__name__, list(imgs) + [u for u in ups if u is not None] + [l for l in lats if l is not None])
     L = _native.lib()
     with torch.cuda.device(dev):
         imgs_d = _on_device(imgs, torch.uint8, dev)
@@ -232,29 +201,22 @@ def _draw(imgs, ups, lats, colors, density, arrow_inv_len, alpha_fill, alpha_lin
         if in_place:
             outs = imgs_d
         else:
-            sizes = [t.numel() for t in imgs_d]
-            blob = torch.empty(sum(sizes), dtype=torch.uint8, device=dev)
-            outs, off = [], 0
-            for t, s in zip(imgs_d, sizes):
-                outs.append(blob[off:off + s].view(t.shape))
-                off += s
-        ib, ob, lb, ub = _base(imgs_d), _base(outs), _base(lats_d), _base(ups_d)
+            offs, total = _batch.layout([t.numel() for t in imgs_d])
+            outs = _batch.views(torch.empty(total, dtype=torch.uint8, device=dev), offs, [t.shape for t in imgs_d])
+        ib, ob, lb, ub = _batch.base(imgs_d), _batch.base(outs), _batch.base(lats_d), _batch.base(ups_d)
         descs = (_native.pf_draw_canvas * n)()
         for k in range(n):
             h, w = imgs_d[k].shape[:2]
             d = descs[k]
             d.height, d.width = h, w
-            d.img_offset, d.out_offset = imgs_d[k].data_ptr() - ib, outs[k].data_ptr() - ob
+            d.img_offset, d.out_offset = _batch.offset(imgs_d[k], ib), _batch.offset(outs[k], ob)
             d.alpha_fill, d.alpha_line = alpha_fill, alpha_line
-            d.lat_offset, d.up_offset = -1, -1
-            if lats_d[k] is not None:
-                d.draw_lat, d.lat_offset = 1, (lats_d[k].data_ptr() - lb) // 4
+            d.lat_offset, d.up_offset = _batch.offset(lats_d[k], lb), _batch.offset(ups_d[k], ub)
+            d.draw_lat = int(lats_d[k] is not None)
             if ups_d[k] is not None:
-                u = ups_d[k]
-                d.draw_up, d.up_offset = 1, (u.data_ptr() - ub) // 4
-                d.up_stride[0], d.up_stride[1], d.up_stride[2] = u.stride(0), u.stride(1), u.stride(2)
+                d.draw_up, d.up_stride[:] = 1, ups_d[k].stride()
                 d.density, d.arrow_inv_len = int(density), int(arrow_inv_len)
-                d.arrow_rgb[0], d.arrow_rgb[1], d.arrow_rgb[2] = colors[k]
+                d.arrow_rgb[:] = colors[k]
         ptr = lambda b: b if b else None
         stream = torch.cuda.current_stream(dev).cuda_stream
         _native.check(L.pf_draw_fields(dev.index, descs, n, ib, ob, ptr(lb), ptr(ub), stream))
@@ -289,7 +251,7 @@ def draw_fields_batch(imgs, ups=None, lats=None, color=None, density=10, arrow_i
         raise ValueError(f"{n} images but {len(ups)} up fields and {len(lats)} latitude maps")
     imgs = [_check_image(im, k) for k, im in enumerate(imgs)]
     col = _check_color(color, GREEN)
-    af, al = _check_unit(alpha_contourf, "alpha_contourf"), _check_unit(alpha_contour, "alpha_contour")
+    af, al = _batch.unit(alpha_contourf, "alpha_contourf"), _batch.unit(alpha_contour, "alpha_contour")
     for k, im in enumerate(imgs):
         h, w = im.shape[:2]
         if ups[k] is not None:
@@ -328,7 +290,7 @@ def draw_latitude_field(img_rgb, latimap=None, binmap=None, alpha_contourf=0.4, 
     if latimap is None:
         raise ValueError("latimap is required")
     lat = _check_lat(latimap, img.shape[0], img.shape[1], 0)
-    af, al = _check_unit(alpha_contourf, "alpha_contourf"), _check_unit(alpha_contour, "alpha_contour")
+    af, al = _batch.unit(alpha_contourf, "alpha_contourf"), _batch.unit(alpha_contour, "alpha_contour")
     return _finish(_draw([img], [None], [lat], [None], 10, 20, af, al), [img], return_img)[0]
 
 
@@ -343,7 +305,7 @@ def _radians(mode, *angles):
 def _draw_lat_then_up(imgs, ups, lats_deg, up_color, alpha_contourf, alpha_contour, draw_up, draw_lat):
     """draw_from_r_p_f*'s two steps on device fields: draw_latitude_field, then draw_up_field over ITS result (the arrows go over
     the contour lines here, utils.py:312-320), the second call drawing in place."""
-    af, al = _check_unit(alpha_contourf, "alpha_contourf"), _check_unit(alpha_contour, "alpha_contour")
+    af, al = _batch.unit(alpha_contourf, "alpha_contourf"), _batch.unit(alpha_contour, "alpha_contour")
     col = _check_color(up_color, C0)
     n = len(imgs)
     cur = list(imgs)
@@ -365,7 +327,7 @@ def draw_from_r_p_f(img, roll, pitch, vfov, mode, up_color=None, alpha_contourf=
     h, w = img.shape[:2]
     if draw_up:
         _check_lattice(10, 20, h, w, 0)
-    dev = _device_of([img])
+    dev = _batch.device(__name__, [img])
     ups, lats = panocam.pinhole_fields([vfov], [h], [w], [pitch], [roll], dev, up=True, lat=True)
     return _draw_lat_then_up([img], ups, lats, up_color, alpha_contourf, alpha_contour, draw_up, draw_lat)[0]
 
@@ -379,7 +341,7 @@ def draw_from_r_p_f_cx_cy(img, roll, pitch, vfov, rel_cx, rel_cy, mode, up_color
     h, w = img.shape[:2]
     if draw_up:
         _check_lattice(10, 20, h, w, 0)
-    dev = _device_of([img])
+    dev = _batch.device(__name__, [img])
     focal = panocam.general_vfov_to_focal(rel_cx, rel_cy, 1, vfov, False)
     ups, lats = panocam.camera_fields([float(focal)], [h], [w], [pitch], [roll], [float(rel_cx)], [float(rel_cy)], dev)
     return _draw_lat_then_up([img], ups, lats, up_color, alpha_contourf, alpha_contour, draw_up, draw_lat)[0]
@@ -399,6 +361,6 @@ def draw_predictions(imgs, preds, up_color=GREEN, alpha_contourf=0.4, alpha_cont
     if draw_up:
         for k, im in enumerate(imgs):
             _check_lattice(10, 20, im.shape[0], im.shape[1], k)
-    dev = _device_of(imgs)
+    dev = _batch.device(__name__, imgs)
     ups, lats = panocam.fields_from_predictions(preds, [im.shape[:2] for im in imgs], "deg", dev)
     return _draw_lat_then_up(imgs, ups, lats, up_color, alpha_contourf, alpha_contour, draw_up, draw_lat)

@@ -18,7 +18,7 @@ sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
-from perspectivefields_b200 import panocam, viz  # noqa: E402
+from perspectivefields_b200 import _batch, panocam, viz  # noqa: E402
 
 
 def card(index):
@@ -62,7 +62,7 @@ def main():
     ups, lats = panocam.camera_fields(focal, [H] * n, [W] * n, el, roll, [0.0] * n, [0.0] * n, dev)
     lats = [torch.deg2rad(l) for l in lats]
     imgs = [t for t in torch.randint(0, 256, (n, H, W, 3), dtype=torch.uint8, device=dev)]
-    ups_c = [viz._check_up(u, H, W, k) for k, u in enumerate(ups)]
+    ups_c = [_batch.up_view(u, H, W) for u in ups]
 
     def call():
         return viz._draw(imgs, ups_c, lats, [viz.GREEN] * n, a.density, 20, 0.4, 0.9)
