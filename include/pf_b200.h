@@ -95,6 +95,19 @@ int64_t pf_workspace_bytes(pf_handle h, int n, int max_h);
 /* Whole forward of perspectivefields.py:223-272 for one batch, enqueued on `stream` (a cudaStream_t). */
 int pf_forward(pf_handle h, const pf_batch* batch, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- ParamNet on the caller's fields (param_network.py:46-69 ParamNet.forward, :193-221 ParamNetConvNextRegress.forward) -----
+ * The ParamNet section of pf_forward (same kernels, same order, same results on the same fields) run on any fields at the
+ * engine's working size net_h x net_w: gravity DEVICE float32 [n,2,net_h,net_w] up vectors, latitude [n,1,net_h,net_w]
+ * sin(latitude), contiguous, used as given (no normalisation or clamp).  Outputs (DEVICE): params float32 [n,8] in the
+ * pf_batch.params layout; raw float32 [n,5] (or NULL) = the ConvNeXt head's five outputs before any scaling, the prediction of
+ * the reference's training branch (param_network.py:71-128, :223-241).  The option "bf16" applies as in pf_forward.  An engine
+ * without a ParamNet, n < 1, NULL gravity / latitude / params / workspace, or a workspace smaller than
+ * pf_param_workspace_bytes(h, n) is PF_ERR_ARG before anything is launched.  workspace: DEVICE, 256-byte aligned.  Enqueued on
+ * `stream` without synchronisation. */
+int64_t pf_param_workspace_bytes(pf_handle h, int n);
+int pf_param_forward(pf_handle h, int n, const float* gravity, const float* latitude, float* params, float* raw, void* workspace,
+                     int64_t workspace_bytes, void* stream);
+
 /* Per-launch timing of the GEMM engine with CUDA events on the launch stream (bench.py roofline leg).  pf_profile_read
  * fills out21[cfg*3 + {0,1,2}] = {milliseconds, algorithmic FLOPs (2*M*N*K), launches} per engine configuration (slots 0-4 are
  * unused since ABI 2 -- the earlier HMMA / register-staged engines were removed; 5: TMA+wgmma GEMM mode, 6: TMA+wgmma halo
@@ -120,7 +133,7 @@ int pf_profile_kernels_read(pf_handle h, char* buf, int cap);
  *   ParamNet stem and tail) stay fp32.  Read at every launch: it can be switched between pf_forward calls on one handle. */
 int pf_set_option(pf_handle h, const char* name, int value);
 
-/* Debug taps (tests only): when enabled, intermediates of the next pf_forward are kept (never recycled) and can be
+/* Debug taps (tests only): when enabled, intermediates of the next pf_forward (or pf_param_forward) are kept (never recycled) and can be
  * copied out by name (device-to-device, enqueued on `stream`).  Names are listed by pf_debug_name(i). */
 int pf_debug_enable(pf_handle h, int on);
 int pf_debug_count(pf_handle h);

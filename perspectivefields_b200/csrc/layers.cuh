@@ -799,8 +799,10 @@ __global__ void __launch_bounds__(256) pack_fields_kernel(const float* __restric
 // kind 2 (ParamNetConvNextRegress): general_vfov = x2*90, cx = x3, cy = x4, rel_focal = closed-form root of
 //   cos(gvfov) = (p^2+q^2-1)/(2pq), p^2 = f^2+cx^2+(cy+.5)^2, q^2 = f^2+cx^2+(cy-.5)^2 (utils.py:47-91 solves the
 //   same equation with scipy fsolve from f=1.5 and takes abs()).
+// raw (optional, NULL to skip): [B][5] = x0..x4, the head's outputs before the scaling (the training branch's prediction).
 __global__ void __launch_bounds__(256) param_tail_kernel(const float* __restrict__ feat, int HW, const float* __restrict__ nw, const float* __restrict__ nb,
-                                                         const float* __restrict__ hw, const float* __restrict__ hb, float* __restrict__ params, int kind) {
+                                                         const float* __restrict__ hw, const float* __restrict__ hb, float* __restrict__ params,
+                                                         float* __restrict__ raw, int kind) {
   constexpr int C = 768;
   __shared__ float s_x[C];
   __shared__ float s_red[8];
@@ -844,6 +846,7 @@ __global__ void __launch_bounds__(256) param_tail_kernel(const float* __restrict
   if (tid == 0) {
     float* o = params + b * 8;
     const float x0 = s_out[0], x1 = s_out[1], x2 = s_out[2], x3 = s_out[3], x4 = s_out[4];
+    if (raw) { float* r = raw + b * 5; r[0] = x0; r[1] = x1; r[2] = x2; r[3] = x3; r[4] = x4; }
     o[0] = x0 * 90.0f; o[1] = x1 * 90.0f; o[2] = x2 * 90.0f; o[6] = x2; o[7] = 0.f;
     if (kind == 1) {
       o[3] = 0.f; o[4] = 0.f;

@@ -682,6 +682,7 @@ static int fwd_tails_post(Fwd& F, const pf_batch* bt, const float* conv1_out, Po
 // =============================================================================================== the forward graph
 // The whole network on the TMA -> wgmma engine: every GEMM input is a pre-split bf16 hi/lo tensor written by its producer
 // (LayerNorm, attention, depthwise conv, upsample, stem gather, or the previous GEMM's epilogue).
+static int fwd_paramnet(Fwd& F, const float* grav, const float* lat, float* params, float* raw);
 static int run_forward(Fwd& F, const pf_batch* bt) {
   pf_engine* e = F.e;
   const pf_model_desc& D = e->desc;
@@ -859,12 +860,30 @@ static int run_forward(Fwd& F, const pf_batch* bt) {
   // ---------------- ParamNet (ConvNeXt-T on the predicted fields) -------------------------------------------
   if (D.param_net != PF_PARAM_NONE) {
     section("pf:paramnet");
+    TRY(fwd_paramnet(F, dry ? nullptr : bt->pred_gravity, dry ? nullptr : bt->pred_latitude, dry ? nullptr : bt->params, nullptr));
+  }
+  return PF_OK;
+}
+
+// ParamNet (ConvNeXt-T) on fields at the working size, the last section of pf_forward (on the heads' outputs) and all of
+// pf_param_forward (on the caller's fields): grav [n,2,NH,NW] up vectors, lat [n,1,NH,NW] sin(latitude) -> params [n,8]
+// (pf_batch.params layout) and, when raw is non-NULL, the head's five outputs before any scaling as [n,5].
+static int fwd_paramnet(Fwd& F, const float* grav, const float* lat, float* params, float* raw) {
+  pf_engine* e = F.e;
+  const pf_model_desc& D = e->desc;
+  const int n = F.n;
+  const bool dry = F.dry;
+  cudaStream_t st = F.st;
+  Arena& ar = F.ar;
+  using Epi = Fwd::Epi;
+  const int NH = e->net_h, NW = e->net_w;
+  {
     if (D.gravity_classes != 2 || D.latitude_classes != 1) return fail(PF_ERR_ARG, "ParamNet needs regression heads");
     // centered: ConvNeXt on the fields at the net size; uncentered: nearest resample to INPUT_SIZE x INPUT_SIZE first
     const bool centered = D.param_net == PF_PARAM_CENTERED;
     const int SH = centered ? NH : D.param_input_size, SW = centered ? NW : D.param_input_size;
     float* pin = ar.f((long long)n * SH * SW * 4);
-    if (!dry) LAUNCHED((pack_fields_kernel<<<(unsigned)cdivl((long long)n * SH * SW, 256), 256, 0, st>>>(bt->pred_gravity, bt->pred_latitude, pin, n, NH, NW, SH, SW), cudaGetLastError()));
+    if (!dry) LAUNCHED((pack_fields_kernel<<<(unsigned)cdivl((long long)n * SH * SW, 256), 256, 0, st>>>(grav, lat, pin, n, NH, NW, SH, SW), cudaGetLastError()));
     int rh = SH / 4, rw = SW / 4;
     float* x = ar.f((long long)n * rh * rw * 96);
     if (!dry) LAUNCHED((stem_conv_launch<4, 4, 4, 0, 96>(pin, 4, n, SH, SW, e->pn_stem_w, e->pn_stem_b, x, st)));
@@ -894,8 +913,8 @@ static int run_forward(Fwd& F, const pf_batch* bt) {
       TRY(F.tapf(x, rows * C, "cnx.s%d", s));
     }
     if (!dry) {
-      if (!bt->params) return fail(PF_ERR_ARG, "params output is NULL");
-      LAUNCHED((param_tail_kernel<<<n, 256, 0, st>>>(x, rh * rw, e->pn_norm.w, e->pn_norm.b, e->pn_head_w, e->pn_head_b, bt->params, D.param_net), cudaGetLastError()));
+      if (!params) return fail(PF_ERR_ARG, "params output is NULL");
+      LAUNCHED((param_tail_kernel<<<n, 256, 0, st>>>(x, rh * rw, e->pn_norm.w, e->pn_norm.b, e->pn_head_w, e->pn_head_b, params, raw, D.param_net), cudaGetLastError()));
     }
   }
   return PF_OK;
@@ -1036,6 +1055,54 @@ int pf_forward(pf_handle h, const pf_batch* bt, void* workspace, int64_t workspa
   tl_kp = &h->kp;
   pdl_enabled() = h->use_pdl && !h->kp.on && !h->profile && !sync_debug();   // (event records between launches defeat it anyway)
   const int r = run_forward(F, bt);
+  pdl_enabled() = false;
+  tl_kp = nullptr;
+  return r;
+}
+
+// ParamNet alone on the caller's fields: the sizing dry run of fwd_paramnet (no launches)
+static int param_peak(pf_handle h, int n, long long* peak) {
+  Fwd T{h, Arena{}, nullptr, true, n};
+  T.ar.dry = true;
+  T.ar.keep = h->debug;
+  TRY(fwd_paramnet(T, nullptr, nullptr, nullptr, nullptr));
+  *peak = T.ar.peak;
+  return PF_OK;
+}
+
+int64_t pf_param_workspace_bytes(pf_handle h, int n) {
+  if (!h || n < 1) return fail(PF_ERR_ARG, "pf_param_workspace_bytes: bad argument");
+  if (h->desc.param_net == PF_PARAM_NONE) return fail(PF_ERR_ARG, "pf_param_workspace_bytes: this model has no ParamNet");
+  long long peak = 0;
+  TRY(param_peak(h, n, &peak));
+  return peak + 4096;
+}
+
+int pf_param_forward(pf_handle h, int n, const float* gravity, const float* latitude, float* params, float* raw, void* workspace,
+                     int64_t workspace_bytes, void* stream) {
+  if (!h) return fail(PF_ERR_ARG, "pf_param_forward: null handle");
+  if (!h->finalized) return fail(PF_ERR_WEIGHT, "pf_param_forward: pf_finalize has not succeeded");
+  if (h->desc.param_net == PF_PARAM_NONE) return fail(PF_ERR_ARG, "pf_param_forward: this model has no ParamNet");
+  if (n < 1) return fail(PF_ERR_ARG, "pf_param_forward: n = %d, at least 1 pair of fields is needed", n);
+  if (!gravity || !latitude || !params || !workspace) return fail(PF_ERR_ARG, "pf_param_forward: null gravity / latitude / params / workspace");
+  long long peak = 0;
+  TRY(param_peak(h, n, &peak));
+  if (peak > workspace_bytes) return fail(PF_ERR_ARG, "pf_param_forward: workspace %lld B < required %lld B", (long long)workspace_bytes, peak);
+  if (((uintptr_t)workspace & 255) != 0) return fail(PF_ERR_ARG, "pf_param_forward: workspace must be 256-byte aligned");
+  CU(cudaSetDevice(h->device));
+  Fwd F{h, Arena{}, (cudaStream_t)stream, false, n};
+  F.ar.base = (char*)workspace;
+  F.ar.cap = workspace_bytes;
+  F.ar.keep = h->debug;
+  h->taps.clear();
+  h->kp.st = (cudaStream_t)stream;
+  tl_kp = &h->kp;
+  pdl_enabled() = h->use_pdl && !h->kp.on && !h->profile && !sync_debug();
+  int r;
+  {
+    NvtxRange r_("pf:paramnet");
+    r = fwd_paramnet(F, gravity, latitude, params, raw);
+  }
   pdl_enabled() = false;
   tl_kp = nullptr;
   return r;

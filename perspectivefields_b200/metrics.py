@@ -4,13 +4,16 @@
 - ``field_errors``: per-image errors of ``pred_gravity_original`` / ``pred_latitude_original`` against ground-truth fields at
   each image's own size (this project's rule, DESIGN.md section 1), with mixed sizes in one call.
 - ``param_errors``: absolute differences of the ParamNet's camera parameters.
+- ``param_targets`` / ``param_net_losses``: the targets and the loss rule of ParamNet's training branch.
 
-The heads' training losses are ``PerspectiveFields.losses`` and their targets ``PerspectiveFields.targets_from_fields``, which
-use the helpers here.  Nothing here synchronises with the device.
+The heads' training losses are ``PerspectiveFields.losses`` and their targets ``PerspectiveFields.targets_from_fields``, and
+ParamNet's are ``PerspectiveFields.param_losses``, which use the helpers here.  Nothing here synchronises with the device.
 """
 import ctypes
 
+import numpy as np
 import torch
+import torch.nn.functional as F
 
 from . import _batch, _native
 
@@ -193,3 +196,43 @@ def param_errors(results, gt):
             raise ValueError(f"gt[{k!r}] must have shape [{len(results)}], got {list(g.shape)}")
         out[k] = (pred - g).abs()
     return out
+
+
+# ParamNetConvNextRegress.factors (param_network.py:183-191)
+_PARAM_FACTORS = {"roll": 90.0, "pitch": 90.0, "vfov": 90.0, "rel_focal": 1.0, "rel_cx": 1.0, "rel_cy": 1.0, "general_vfov": 90.0}
+
+
+def param_targets(batched_inputs, n, param_net, predict_params):
+    """Host float32 targets of ParamNet's training branch (param_network.py:72-98, :223-229) from ``batched_inputs[i][key]``
+    (host numbers, degrees): ``ParamNet`` [n, 5] = (roll / 90, pitch / 90, vfov / 90, 0, 0); ``ParamNetConvNextRegress``
+    [n, len(predict_params)] = value / factor per key.  Each quotient is taken in float64 and then rounded to float32."""
+    if len(batched_inputs) != n:
+        raise ValueError(f"{n} pairs of fields but {len(batched_inputs)} batched_inputs")
+    keys = _PARAMS_CENTERED if param_net == "ParamNet" else tuple(predict_params)
+    gt = np.zeros((n, 5 if param_net == "ParamNet" else len(keys)), np.float64)
+    for i, x in enumerate(batched_inputs):
+        for j, k in enumerate(keys):
+            if k not in x:
+                raise KeyError(f"batched_inputs[{i}] has no {k!r} (the targets need {keys})")
+            v = x[k]
+            if isinstance(v, torch.Tensor) or not isinstance(v, (int, float, np.integer, np.floating)) or isinstance(v, (bool, np.bool_)):
+                raise TypeError(f"batched_inputs[{i}][{k!r}] must be a host number, got {type(v).__name__}")
+            gt[i, j] = float(v) / _PARAM_FACTORS[k]
+    return gt.astype(np.float32)
+
+
+def param_net_losses(raw, gt, param_net, predict_params, loss_weight):
+    """ParamNet's losses (param_network.py:102-128 ``ParamNet.losses`` with RECOVER_RPF and without RECOVER_PP, :233-241
+    ``ParamNetConvNextRegress.losses``) from its raw head outputs ``raw`` float32 [n, 5] and ``param_targets``' ``gt`` on the
+    same device, in float32 and in the reference's order of operations:
+
+    - ``ParamNet``: ``{"param-l1-loss": mean(|raw - gt| * [1, 1, 1, 0, 0]) * loss_weight}``, the mean over all 5n entries;
+    - ``ParamNetConvNextRegress``: ``{"param/<key>-loss": mean_i((raw - gt)^2 * loss_weight)}`` per key of ``predict_params``.
+
+    Device-agnostic torch operations; returns 0-dim float32 tensors on ``raw``'s device."""
+    if param_net == "ParamNet":
+        mask = torch.ones_like(raw)
+        mask[:, 3:] = 0.0
+        return {"param-l1-loss": (F.l1_loss(raw, gt, reduction="none") * mask).mean() * loss_weight}
+    itemized = F.mse_loss(raw, gt, reduction="none") * loss_weight
+    return {f"param/{k}-loss": itemized[:, j].mean() for j, k in enumerate(predict_params)}

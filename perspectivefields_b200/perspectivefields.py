@@ -2,7 +2,7 @@
 whole forward runs in libpf_b200.so (hand-written sm_90a CUDA, C ABI in include/pf_b200.h).
 
 Kept from the reference surface: ``PerspectiveFields(version)``, ``.eval()``, ``.cuda()/.to()``, ``.device``,
-``.versions()``, ``.inference(img_bgr)``, ``.inference_batch(list)``, ``.forward(batched_inputs)``,
+``.versions()``, ``.inference(img_bgr)``, ``.inference_batch(list)``, ``.forward(batched_inputs)``, ``.param_net(predictions)``,
 ``.state_dict()/.load_state_dict()`` with the reference's key names, attributes ``version``, ``param_on``, ``cfg``,
 ``input_format``; result dictionaries with the same keys, order, shapes and dtypes.  There is no CPU path: the model
 must live on a CUDA device (H100) and libpf_b200.so must be built, otherwise inference raises.
@@ -86,12 +86,11 @@ class _Engine:
         except Exception:
             pass
 
-    def _workspace(self, n, max_h, cur):
-        """Scratch for pf_forward.  The buffer is allocated from torch's caching allocator on the stream of its first use; a
-        caller that switches streams between calls is kept safe by stream-ordering the hand-over: the new stream waits for the
-        last forward that used the workspace (``ws_event``), and a workspace that is replaced is marked as used by that stream
-        (``record_stream``) so that its block is not recycled under a forward still running there."""
-        need = _native.check(self.L.pf_workspace_bytes(self.handle, n, max_h))
+    def _workspace(self, need, cur):
+        """Scratch of ``need`` bytes for pf_forward / pf_param_forward.  The buffer is allocated from torch's caching allocator on
+        the stream of its first use; a caller that switches streams between calls is kept safe by stream-ordering the hand-over:
+        the new stream waits for the last call that used the workspace (``ws_event``), and a workspace that is replaced is marked
+        as used by that stream (``record_stream``) so that its block is not recycled under a call still running there."""
         if self.ws_event is not None and self.ws_stream is not None and self.ws_stream != cur:
             cur.wait_event(self.ws_event)
         if self.workspace is None or self.workspace.numel() < need:
@@ -157,7 +156,7 @@ class _Engine:
             "params": torch.empty((n, 8), dtype=torch.float32, device=dev),
             "g_off": g_off, "l_off": l_off, "h": h, "w": w,
         }
-        ws = self._workspace(n, int(h.max()), cur)
+        ws = self._workspace(_native.check(self.L.pf_workspace_bytes(self.handle, n, int(h.max()))), cur)
         bt = _native.pf_batch()
         bt.n = n
         i64p, i32p = ctypes.POINTER(ctypes.c_int64), ctypes.POINTER(ctypes.c_int32)
@@ -179,6 +178,21 @@ class _Engine:
         if blob is not None and self.staged_slot is not None and self.dev_blob is not None and blob is self.dev_blob[self.staged_slot]:
             self.blob_free[self.staged_slot] = ev   # stage_images may overwrite this device blob once the forward has read it
         return out
+
+    def param_forward(self, gravity, latitude, with_raw):
+        """pf_param_forward on contiguous float32 [n, 2, H, W] / [n, 1, H, W] fields at the working size -> (params [n, 8], raw
+        [n, 5] or None), enqueued on the current stream."""
+        n = int(gravity.shape[0])
+        cur = torch.cuda.current_stream(self.device)
+        params = torch.empty((n, 8), dtype=torch.float32, device=self.device)
+        raw = torch.empty((n, 5), dtype=torch.float32, device=self.device) if with_raw else None
+        ws = self._workspace(_native.check(self.L.pf_param_workspace_bytes(self.handle, n)), cur)
+        _native.check(self.L.pf_param_forward(self.handle, n, gravity.data_ptr(), latitude.data_ptr(), params.data_ptr(),
+                                              raw.data_ptr() if with_raw else None, ws.data_ptr(), ws.numel(), cur.cuda_stream))
+        ev = torch.cuda.Event()
+        ev.record(cur)
+        self.ws_event = ev
+        return params, raw
 
 
 class ResizeTransform:
@@ -610,6 +624,73 @@ class PerspectiveFields(nn.Module):
             _native.check(L.pf_head_losses(dev.index, n, h, w, gc, preds[0].data_ptr(), tg[0].data_ptr(), lc, preds[1].data_ptr(),
                                            tg[1].data_ptr(), ig, il, wg, wl, out.data_ptr(), ws.data_ptr(), ws.numel(), stream))
         return dict(zip(keys, out.unbind(0)))
+
+    # ------------------------------------------------------------------------------------------ ParamNet on given fields
+    def _param_inputs(self, predictions):
+        """Checks of ``param_net`` / ``param_losses`` (all before any GPU work) -> (n, pred_gravity, pred_latitude)."""
+        if self._variant["param_net"] is None:
+            raise ValueError(f"{self.version} has no ParamNet")
+        dev = self.device
+        if dev.type != "cuda":
+            raise RuntimeError("perspectivefields_b200 has no CPU path: move the model to an H100 with .cuda() first")
+        if dev.index is None:
+            dev = torch.device("cuda", torch.cuda.current_device())
+        h, w = self._net_hw
+        ts = []
+        for key, c in (("pred_gravity", 2), ("pred_latitude", 1)):
+            if key not in predictions:
+                raise KeyError(f"predictions has no {key!r}")
+            t = _batch.cuda_f32(predictions[key], f"predictions[{key!r}]", dev)
+            if t.dim() != 4 or tuple(t.shape[1:]) != (c, h, w):
+                raise ValueError(f"predictions[{key!r}] is {list(t.shape)}, the working size needs [n, {c}, {h}, {w}]")
+            ts.append(t)
+        n = int(ts[0].shape[0])
+        if n == 0:
+            raise ValueError("predictions hold no fields (n = 0)")
+        if int(ts[1].shape[0]) != n:
+            raise ValueError(f"{n} gravity fields but {int(ts[1].shape[0])} latitude fields")
+        return n, ts[0], ts[1]
+
+    def _param_run(self, gravity, latitude, with_raw):
+        eng = self._get_engine()
+        with torch.cuda.device(eng.device):
+            return eng.param_forward(gravity.contiguous(), latitude.contiguous(), with_raw)
+
+    @torch.no_grad()
+    def param_net(self, predictions, batched_inputs=None):
+        """The reference's ``param_net(predictions)`` in eval mode (param_network.py:46-69 ``ParamNet``, :193-221
+        ``ParamNetConvNextRegress``) on any fields: ``predictions["pred_gravity"]`` float32 [n, 2, H, W] up vectors and
+        ``["pred_latitude"]`` [n, 1, H, W] sin(latitude) on the model's device at the working size (what the regression heads
+        return, or the ``gt_gravity`` / ``gt_latitude`` of ``targets_from_fields``).  The fields are used as given (no
+        renormalisation or clamp; NaN propagates); the run is the ParamNet section of the forward, so the forward's own fields
+        give its parameters bit for bit.  Returns the keys of the variant's class, in its order: ``pred_roll, pred_pitch,
+        pred_vfov, pred_rel_focal`` (centred) or ``pred_roll, pred_pitch, pred_general_vfov, pred_rel_cx, pred_rel_cy,
+        pred_rel_focal`` (uncentred), each a float32 [n] view of one device tensor (``pred_rel_focal`` too, unlike the
+        reference's host tensor of the uncentred class).  ``batched_inputs`` is ignored, as in the reference's eval branch."""
+        n, g, l = self._param_inputs(predictions)
+        params, _ = self._param_run(g, l, False)
+        if self._variant["param_net"] == "ParamNet":
+            cols = (("pred_roll", 0), ("pred_pitch", 1), ("pred_vfov", 2), ("pred_rel_focal", 5))
+        else:
+            cols = (("pred_roll", 0), ("pred_pitch", 1), ("pred_general_vfov", 2), ("pred_rel_cx", 3), ("pred_rel_cy", 4), ("pred_rel_focal", 5))
+        return {k: params[:, j] for k, j in cols}
+
+    @torch.no_grad()
+    def param_losses(self, predictions, batched_inputs):
+        """The losses of the reference's ``param_net(predictions, batched_inputs)`` in training mode (param_network.py:71-128,
+        :223-241) for fields as ``param_net`` takes them and targets ``batched_inputs[i]`` holding host numbers in degrees:
+        ``roll``, ``pitch``, ``vfov`` (centred; ``{"param-l1-loss"}``) or the keys of ``cfg.MODEL.PARAM_DECODER.PREDICT_PARAMS``
+        (uncentred; ``{"param/<key>-loss"}`` per key), weighted by ``cfg.MODEL.PARAM_DECODER.LOSS_WEIGHT``
+        (``metrics.param_net_losses`` states the rule).  Values are 0-dim float32 device tensors and nothing synchronises."""
+        from . import metrics
+
+        n, g, l = self._param_inputs(predictions)
+        v = self._variant
+        gt = metrics.param_targets(batched_inputs, n, v["param_net"], v["predict_params"])
+        _, raw = self._param_run(g, l, True)
+        with torch.cuda.device(raw.device):
+            gt = _batch.upload([gt], torch.float32, raw.device)[0]
+        return metrics.param_net_losses(raw, gt, v["param_net"], v["predict_params"], float(self.cfg.MODEL.PARAM_DECODER.LOSS_WEIGHT))
 
     def set_option(self, name, value):
         """Engine options (see pf_set_option in include/pf_b200.h), e.g. ``set_option("pdl", 0)``."""
