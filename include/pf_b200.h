@@ -108,6 +108,28 @@ int64_t pf_param_workspace_bytes(pf_handle h, int n);
 int pf_param_forward(pf_handle h, int n, const float* gravity, const float* latitude, float* params, float* raw, void* workspace,
                      int64_t workspace_bytes, void* stream);
 
+/* ---- ParamNet training: gradients of a loss of the raw head outputs with respect to every ParamNet parameter --------------------
+ * pf_param_train_forward is pf_param_forward's raw output (bit for bit) that also keeps, at the start of `workspace`, what the
+ * backward needs: the packed input, the stem's output and the residual stream around every block (the rest is recomputed).
+ * pf_param_backward then takes draw DEVICE float32 [n,5] = d loss / d raw and writes grads DEVICE float32 [pf_param_grad_numel()]
+ * (overwritten, not accumulated): one tensor per parameter in the engine's weight layout, at the offsets pf_param_grad_entry
+ * lists.  With grad_gravity [n,2,net_h,net_w] and grad_latitude [n,1,net_h,net_w] (both or neither) it also writes d loss / d
+ * fields.  It must follow a pf_param_train_forward of the same engine, n and workspace on the same stream, with the workspace
+ * untouched in between, and it needs the training weights registered with pf_set_weight (names "pn.ds<k>.t.whi/.wlo",
+ * "pn.s<s>.b<j>.pw1t.whi/.wlo", ".pw2t.whi/.wlo" = the transposed weights, ".dw.wr" = the depthwise kernel rotated by 180 degrees,
+ * "pn.zero" = 768 zeros), else PF_ERR_WEIGHT.  Parameter gradients are sums in a fixed order without atomics: repeated calls
+ * are bit-identical.  The option "bf16" applies to every GEMM.  Bad arguments as for pf_param_forward (workspace: at least
+ * pf_param_train_workspace_bytes(h, n)) are PF_ERR_ARG before anything is launched.  Enqueued on `stream` without
+ * synchronisation. */
+int64_t pf_param_train_workspace_bytes(pf_handle h, int n);
+int pf_param_train_forward(pf_handle h, int n, const float* gravity, const float* latitude, float* raw, void* workspace,
+                           int64_t workspace_bytes, void* stream);
+int pf_param_backward(pf_handle h, int n, const float* draw, float* grads, float* grad_gravity, float* grad_latitude, void* workspace,
+                      int64_t workspace_bytes, void* stream);
+int64_t pf_param_grad_numel(void);
+/* entry i of the gradient buffer: engine weight name ("pn.stem.w", "pn.s0.b0.pw1.w", ...), offset and length in floats */
+int pf_param_grad_entry(int i, const char** name, int64_t* offset, int64_t* numel);
+
 /* Per-launch timing of the GEMM engine with CUDA events on the launch stream (bench.py roofline leg).  pf_profile_read
  * fills out21[cfg*3 + {0,1,2}] = {milliseconds, algorithmic FLOPs (2*M*N*K), launches} per engine configuration (slots 0-4 are
  * unused since ABI 2 -- the earlier HMMA / register-staged engines were removed; 5: TMA+wgmma GEMM mode, 6: TMA+wgmma halo

@@ -170,6 +170,11 @@ def lib():
         "pf_forward": (i32, [vp, ctypes.POINTER(pf_batch), vp, i64, vp]),
         "pf_param_workspace_bytes": (i64, [vp, i32]),
         "pf_param_forward": (i32, [vp, i32, vp, vp, vp, vp, vp, i64, vp]),
+        "pf_param_train_workspace_bytes": (i64, [vp, i32]),
+        "pf_param_train_forward": (i32, [vp, i32, vp, vp, vp, vp, i64, vp]),
+        "pf_param_backward": (i32, [vp, i32, vp, vp, vp, vp, vp, i64, vp]),
+        "pf_param_grad_numel": (i64, []),
+        "pf_param_grad_entry": (i32, [i32, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(i64), ctypes.POINTER(i64)]),
         "pf_profile_enable": (i32, [vp, i32]),
         "pf_profile_read": (i32, [vp, ctypes.POINTER(ctypes.c_double)]),
         "pf_profile_kernels_enable": (i32, [vp, i32]),
@@ -244,7 +249,8 @@ def lib():
 
 
 EXPORTS = ["pf_abi_version", "pf_last_error", "pf_kernel_launch_count", "pf_create", "pf_create_sized", "pf_destroy", "pf_set_weight",
-           "pf_finalize", "pf_workspace_bytes", "pf_forward", "pf_param_workspace_bytes", "pf_param_forward", "pf_profile_enable", "pf_profile_read", "pf_profile_kernels_enable",
+           "pf_finalize", "pf_workspace_bytes", "pf_forward", "pf_param_workspace_bytes", "pf_param_forward", "pf_param_train_workspace_bytes",
+           "pf_param_train_forward", "pf_param_backward", "pf_param_grad_numel", "pf_param_grad_entry", "pf_profile_enable", "pf_profile_read", "pf_profile_kernels_enable",
            "pf_profile_kernels_read", "pf_set_option", "pf_debug_enable", "pf_debug_count", "pf_debug_name", "pf_debug_numel",
            "pf_debug_copy", "pf_camera_fields", "pf_camera_fields_vp", "pf_pano_views", "pf_equi_views", "pf_draw_fields",
            "pf_encode_fields", "pf_head_losses_workspace", "pf_head_losses", "pf_field_errors_workspace", "pf_field_errors",

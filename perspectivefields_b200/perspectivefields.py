@@ -7,7 +7,9 @@ Kept from the reference surface: ``PerspectiveFields(version)``, ``.eval()``, ``
 ``input_format``; result dictionaries with the same keys, order, shapes and dtypes.  There is no CPU path: the model
 must live on a CUDA device (H100) and libpf_b200.so must be built, otherwise inference raises.
 """
+import collections
 import ctypes
+import itertools
 
 import numpy as np
 import torch
@@ -16,7 +18,9 @@ from torch import nn
 from . import _batch, _native
 from .checkpoint import checkpoint_schema, default_state, load_zoo_checkpoint
 from .variants import PIXEL_MEAN, PIXEL_STD, RESIZE, VARIANTS, make_cfg, model_zoo
-from .weights import repack
+from .weights import PN, param_net_grad_to_ref, param_net_train_weights, repack, repack_param_net
+
+_ENGINE_SERIAL = itertools.count()
 
 
 def check_resize(resize):
@@ -74,6 +78,30 @@ class _Engine:
         self.pinned_event = None
         self.dev_blob = None
         self.staged_slot = None
+        self.serial = next(_ENGINE_SERIAL)
+        self.train_ready = False     # the backward's extra ParamNet tensors are registered (register_train_weights)
+        self._grad_layout = None
+
+    def register_train_weights(self, tensors):
+        """Registers ParamNet's backward-only tensors (weights.param_net_train_weights, already on the device) with the engine."""
+        for name, d in tensors.items():
+            self.tensors[name] = d
+            dt = _native.PF_BF16 if d.dtype == torch.bfloat16 else _native.PF_F32
+            _native.check(self.L.pf_set_weight(self.handle, name.encode(), d.data_ptr(), d.numel(), dt))
+        _native.check(self.L.pf_finalize(self.handle))
+        self.train_ready = True
+
+    def grad_layout(self):
+        """[(engine weight name, offset, numel)] of pf_param_backward's gradient buffer."""
+        if self._grad_layout is None:
+            out, total, i = [], int(self.L.pf_param_grad_numel()), 0
+            name, off, num = ctypes.c_char_p(), ctypes.c_int64(), ctypes.c_int64()
+            while not out or out[-1][1] + out[-1][2] < total:
+                _native.check(self.L.pf_param_grad_entry(i, ctypes.byref(name), ctypes.byref(off), ctypes.byref(num)))
+                out.append((name.value.decode(), off.value, num.value))
+                i += 1
+            self._grad_layout = out
+        return self._grad_layout
 
     def close(self):
         if self.handle:
@@ -194,6 +222,32 @@ class _Engine:
         self.ws_event = ev
         return params, raw
 
+    def param_train_forward(self, gravity, latitude):
+        """pf_param_train_forward on contiguous fields -> raw [n, 5]; the workspace then holds what param_backward reads."""
+        n = int(gravity.shape[0])
+        cur = torch.cuda.current_stream(self.device)
+        raw = torch.empty((n, 5), dtype=torch.float32, device=self.device)
+        ws = self._workspace(_native.check(self.L.pf_param_train_workspace_bytes(self.handle, n)), cur)
+        _native.check(self.L.pf_param_train_forward(self.handle, n, gravity.data_ptr(), latitude.data_ptr(), raw.data_ptr(), ws.data_ptr(),
+                                                    ws.numel(), cur.cuda_stream))
+        return raw
+
+    def param_backward(self, n, draw, input_grads):
+        """pf_param_backward after param_train_forward(n pairs) -> (gradient buffer, d gravity or None, d latitude or None)."""
+        cur = torch.cuda.current_stream(self.device)
+        grads = torch.empty(int(self.L.pf_param_grad_numel()), dtype=torch.float32, device=self.device)
+        dg = dl = None
+        if input_grads:
+            dg = torch.empty((n, 2, self.net_h, self.net_w), dtype=torch.float32, device=self.device)
+            dl = torch.empty((n, 1, self.net_h, self.net_w), dtype=torch.float32, device=self.device)
+        ws = self._workspace(_native.check(self.L.pf_param_train_workspace_bytes(self.handle, n)), cur)
+        _native.check(self.L.pf_param_backward(self.handle, n, draw.data_ptr(), grads.data_ptr(), dg.data_ptr() if input_grads else None,
+                                               dl.data_ptr() if input_grads else None, ws.data_ptr(), ws.numel(), cur.cuda_stream))
+        ev = torch.cuda.Event()
+        ev.record(cur)
+        self.ws_event = ev
+        return grads, dg, dl
+
 
 class ResizeTransform:
     """The ``aug`` attribute of the reference class (perspectivefields.py:16-67, built at :155).  ``apply_image`` keeps the
@@ -279,6 +333,8 @@ class PerspectiveFields(nn.Module):
         if precision == "bf16":
             self._options["bf16"] = 1
         self.training = False
+        self._pn_params = None      # param_net_parameters(): trainable ParamNet weights, the source of truth once created
+        self._pn_synced = None      # (engine serial, training tensors registered, parameter versions) of the last derivation
         self._init_weights()
 
     # ------------------------------------------------------------------------------------------ module plumbing
@@ -308,7 +364,9 @@ class PerspectiveFields(nn.Module):
         if destination is None:
             import collections
             destination = collections.OrderedDict()
+        pn = self._pn_params or {}
         for k, v in self._ref_state.items():
+            v = pn.get(k, v)
             destination[prefix + k] = v if keep_vars else v.detach().clone()
         return destination
 
@@ -327,6 +385,9 @@ class PerspectiveFields(nn.Module):
         for k, v in state_dict.items():
             if k in self._schema:
                 self._ref_state[k] = v.detach().to("cpu", self._ref_state[k].dtype).clone()
+                if self._pn_params is not None and k in self._pn_params:
+                    with torch.no_grad():
+                        self._pn_params[k].copy_(v.detach())     # in place: an optimizer holding the parameters keeps working
         self._drop_engine()
         return torch.nn.modules.module._IncompatibleKeys(missing, unexpected)
 
@@ -336,6 +397,18 @@ class PerspectiveFields(nn.Module):
         self.load_state_dict(state_dict, strict=False)  # a no-op on the {"model": ...} wrapper, as in the reference
         if state_dict:
             self.load_state_dict(state_dict["model"], strict=False)
+
+    def _apply(self, fn, *args, **kwargs):
+        """``.to()`` / ``.cuda()`` / ``.cpu()``: a move to another device writes the ParamNet parameters back into the host state and
+        detaches them from the model (``param_net_parameters()`` then creates a new set on the new device)."""
+        old = self.device
+        out = super()._apply(fn, *args, **kwargs)
+        if getattr(self, "_pn_params", None) is not None and self.device != old:
+            for k, p in self._pn_params.items():
+                self._ref_state[k] = p.detach().to("cpu", self._ref_state[k].dtype).clone()
+            self._pn_params = None
+            self._pn_synced = None
+        return out
 
     def _drop_engine(self):
         if self._jpeg is not None and self._engine is not None:
@@ -361,7 +434,85 @@ class PerspectiveFields(nn.Module):
                 _native.check(eng.L.pf_set_option(eng.handle, k.encode(), v))
             eng.decode_only = bool(self._options.get("decode_only", 0))
             self._engine = eng
+        self._pn_sync(self._engine)
         return self._engine
+
+    def _pn_sync(self, eng):
+        """Re-derives the engine's ParamNet tensors from ``param_net_parameters()`` when a parameter changed (its ``_version``) since
+        the last derivation, or the engine is new: ``weights.repack_param_net`` (+ ``param_net_train_weights`` once the backward
+        has run) as torch operations on the device, copied in place into the registered tensors (their pointers and the engine's
+        cached TMA maps stay valid), enqueued on the current stream."""
+        if self._pn_params is None:
+            return
+        key = (eng.serial, eng.train_ready, tuple(p._version for p in self._pn_params.values()))
+        if key == self._pn_synced:
+            return
+        with torch.no_grad(), torch.cuda.device(eng.device):
+            sd = {k: p.detach() for k, p in self._pn_params.items()}
+            out = repack_param_net(sd, {})
+            if eng.train_ready:
+                param_net_train_weights(sd, out)
+            for name, t in out.items():
+                eng.tensors[name].copy_(t)
+        self._pn_synced = key
+
+    # ------------------------------------------------------------------------------------------ ParamNet training
+    def param_net_parameters(self):
+        """ParamNet's weights as trainable float32 parameters on the model's device: an ordered ``{name: nn.Parameter}`` with every
+        ``param_net.backbone.*`` key of the checkpoint (the reference's names and shapes), for any ``torch.optim`` optimizer.
+        Created on the first call from the current weights; from then on they are ParamNet's weights: every run that uses
+        ParamNet (``inference_batch``, ``forward``, ``param_net``, ``param_losses``, ``param_net_backward``) first re-derives the
+        engine's copies if a parameter changed, ``state_dict()`` returns their values and ``load_state_dict`` writes into them in
+        place.  They are not registered on the module (``parameters()`` and ``.to()`` behave as before); a move to another device
+        writes them back and detaches them.  ``ValueError`` for a variant without ParamNet."""
+        if self._variant["param_net"] is None:
+            raise ValueError(f"{self.version} has no ParamNet")
+        if self._pn_params is None:
+            dev = self.device
+            self._pn_params = collections.OrderedDict(
+                (k, nn.Parameter(self._ref_state[k].detach().to(dev, torch.float32).clone())) for k in self._schema if k.startswith(PN))
+            self._pn_synced = None
+        return collections.OrderedDict(self._pn_params)
+
+    def param_net_backward(self, predictions, batched_inputs, input_grads=False):
+        """``param_losses`` (same inputs, same values bit for bit) plus the gradient of the sum of its losses (detectron2 sums the
+        loss dict) with respect to every ``param_net_parameters()`` entry, accumulated into ``.grad`` as ``loss.backward()`` would
+        (created if None, else added to).  d loss / d raw head outputs comes from torch autograd through
+        ``metrics.param_net_losses``; the ConvNeXt-T backward runs in the engine (pf_param_backward).  With ``input_grads=True`` it
+        returns ``(losses, {"pred_gravity": [n, 2, H, W], "pred_latitude": [n, 1, H, W]})``, the gradient with respect to the
+        fields (uncentred: the nearest sub-sample's gradient, zero at pixels it does not read).  Does not need train mode and
+        nothing synchronises with the host."""
+        from . import metrics
+
+        n, g, l = self._param_inputs(predictions)
+        v = self._variant
+        gt = metrics.param_targets(batched_inputs, n, v["param_net"], v["predict_params"])
+        params = self.param_net_parameters()
+        eng = self._get_engine()
+        with torch.cuda.device(eng.device):
+            if not eng.train_ready:
+                with torch.no_grad():
+                    eng.register_train_weights(param_net_train_weights({k: p.detach() for k, p in params.items()}, {}))
+                self._pn_sync(eng)
+            raw = eng.param_train_forward(g.contiguous(), l.contiguous())
+            gt = _batch.upload([gt], torch.float32, raw.device)[0]
+            with torch.enable_grad():
+                r = raw.detach().requires_grad_(True)
+                losses = metrics.param_net_losses(r, gt, v["param_net"], v["predict_params"], float(self.cfg.MODEL.PARAM_DECODER.LOSS_WEIGHT))
+                draw, = torch.autograd.grad(sum(losses.values()), r)
+            grads, dg, dl = eng.param_backward(n, draw.contiguous(), input_grads)
+            with torch.no_grad():
+                for name, off, numel in eng.grad_layout():
+                    key, t = param_net_grad_to_ref(name, grads[off:off + numel])
+                    p = params[key]
+                    if p.grad is None:
+                        p.grad = t.clone(memory_format=torch.contiguous_format)
+                    else:
+                        p.grad.add_(t)
+        losses = {k: x.detach() for k, x in losses.items()}
+        if input_grads:
+            return losses, {"pred_gravity": dg, "pred_latitude": dl}
+        return losses
 
     # ------------------------------------------------------------------------------------------ inference API
     @torch.no_grad()

@@ -141,25 +141,97 @@ def repack(sd, cfg):
         out[f"head.pred_{short}.b"] = sd[f"persformer_heads.{h}.{pred}.bias"].float().contiguous()
     # ---- ParamNet (ConvNeXt-T)
     if cfg["param_net"] is not None:
-        pn = "param_net.backbone."
-        out["pn.stem.w"] = _stem(sd[pn + "downsample_layers.0.0.weight"])
-        out["pn.stem.b"] = sd[pn + "downsample_layers.0.0.bias"].float().contiguous()
-        _put_ln(out, "pn.stem.ln", sd, pn + "downsample_layers.0.1")
-        for k in (1, 2, 3):
-            _put_ln(out, f"pn.ds{k}.ln", sd, f"{pn}downsample_layers.{k}.0")
-            _put_gemm(out, f"pn.ds{k}", _conv_to_nk(sd[f"{pn}downsample_layers.{k}.1.weight"]), sd[f"{pn}downsample_layers.{k}.1.bias"])
-        for s, C in enumerate(CNX_DIMS):
-            for j in range(CNX_DEPTHS[s]):
-                k = f"{pn}stages.{s}.{j}."
-                n = f"pn.s{s}.b{j}."
-                dw = sd[k + "dwconv.weight"]
-                out[n + "dw.w"] = dw.reshape(C, 49).t().float().contiguous()
-                out[n + "dw.b"] = sd[k + "dwconv.bias"].float().contiguous()
-                _put_ln(out, n + "ln", sd, k + "norm")
-                _put_gemm(out, n + "pw1", sd[k + "pwconv1.weight"], sd[k + "pwconv1.bias"])
-                _put_gemm(out, n + "pw2", sd[k + "pwconv2.weight"], sd[k + "pwconv2.bias"])
-                out[n + "gamma"] = sd[k + "gamma"].float().contiguous()
-        _put_ln(out, "pn.norm", sd, pn + "norm")
-        out["pn.head.w"] = sd[pn + "head.weight"].float().contiguous()
-        out["pn.head.b"] = sd[pn + "head.bias"].float().contiguous()
+        repack_param_net(sd, out)
     return out
+
+
+PN = "param_net.backbone."
+
+
+def repack_param_net(sd, out):
+    """The ParamNet part of ``repack``: ``sd``'s ``param_net.backbone.*`` tensors (any device) -> ``out[name]`` on the same device.
+    ``PerspectiveFields`` also runs it on the device, on its trainable ParamNet parameters."""
+    pn = PN
+    out["pn.stem.w"] = _stem(sd[pn + "downsample_layers.0.0.weight"])
+    out["pn.stem.b"] = sd[pn + "downsample_layers.0.0.bias"].float().contiguous()
+    _put_ln(out, "pn.stem.ln", sd, pn + "downsample_layers.0.1")
+    for k in (1, 2, 3):
+        _put_ln(out, f"pn.ds{k}.ln", sd, f"{pn}downsample_layers.{k}.0")
+        _put_gemm(out, f"pn.ds{k}", _conv_to_nk(sd[f"{pn}downsample_layers.{k}.1.weight"]), sd[f"{pn}downsample_layers.{k}.1.bias"])
+    for s, C in enumerate(CNX_DIMS):
+        for j in range(CNX_DEPTHS[s]):
+            k = f"{pn}stages.{s}.{j}."
+            n = f"pn.s{s}.b{j}."
+            dw = sd[k + "dwconv.weight"]
+            out[n + "dw.w"] = dw.reshape(C, 49).t().float().contiguous()
+            out[n + "dw.b"] = sd[k + "dwconv.bias"].float().contiguous()
+            _put_ln(out, n + "ln", sd, k + "norm")
+            _put_gemm(out, n + "pw1", sd[k + "pwconv1.weight"], sd[k + "pwconv1.bias"])
+            _put_gemm(out, n + "pw2", sd[k + "pwconv2.weight"], sd[k + "pwconv2.bias"])
+            out[n + "gamma"] = sd[k + "gamma"].float().contiguous()
+    _put_ln(out, "pn.norm", sd, pn + "norm")
+    out["pn.head.w"] = sd[pn + "head.weight"].float().contiguous()
+    out["pn.head.b"] = sd[pn + "head.bias"].float().contiguous()
+    return out
+
+
+def param_net_train_weights(sd, out):
+    """The extra engine tensors of ParamNet's backward (pf_param_backward): the transposed hi / lo planes of every GEMM weight
+    (data gradients dX = dY W run on the GEMM engine as dY (W^T)^T), the depthwise kernels rotated by 180 degrees (their data
+    gradient is the forward kernel with the rotated weights) and a zero bias for that launch."""
+    pn = PN
+    for k in (1, 2, 3):
+        hi, lo = split_hi_lo(_conv_to_nk(sd[f"{pn}downsample_layers.{k}.1.weight"]).t())
+        out[f"pn.ds{k}.t.whi"], out[f"pn.ds{k}.t.wlo"] = hi, lo
+    for s, C in enumerate(CNX_DIMS):
+        for j in range(CNX_DEPTHS[s]):
+            k = f"{pn}stages.{s}.{j}."
+            n = f"pn.s{s}.b{j}."
+            for short, key in (("pw1t", "pwconv1"), ("pw2t", "pwconv2")):
+                out[n + short + ".whi"], out[n + short + ".wlo"] = split_hi_lo(sd[k + key + ".weight"].t())
+            out[n + "dw.wr"] = sd[k + "dwconv.weight"].reshape(C, 49).flip(1).t().float().contiguous()
+    ref = sd[pn + "norm.weight"]
+    out["pn.zero"] = torch.zeros(768, dtype=torch.float32, device=ref.device)
+    return out
+
+
+def param_net_grad_to_ref(name, g):
+    """A gradient in the engine layout of ``name`` (pf_param_grad_entry) -> (reference key, tensor in the reference's shape):
+    the inverse of the permutes of ``repack_param_net``."""
+    pn = PN
+    parts = name.split(".")
+    if name.startswith("pn.stem."):
+        if name == "pn.stem.w":
+            return pn + "downsample_layers.0.0.weight", g.view(4, 4, 3, 96).permute(3, 2, 0, 1)
+        if name == "pn.stem.b":
+            return pn + "downsample_layers.0.0.bias", g
+        return pn + "downsample_layers.0.1." + {"w": "weight", "b": "bias"}[parts[-1]], g
+    if name.startswith("pn.ds"):
+        k = int(parts[1][2:])
+        if parts[2] == "ln":
+            return f"{pn}downsample_layers.{k}.0." + {"w": "weight", "b": "bias"}[parts[3]], g
+        cout, cin = CNX_DIMS[k], CNX_DIMS[k - 1]
+        if parts[2] == "w":
+            return f"{pn}downsample_layers.{k}.1.weight", g.view(cout, 2, 2, cin).permute(0, 3, 1, 2)
+        return f"{pn}downsample_layers.{k}.1.bias", g
+    if name.startswith("pn.norm."):
+        return pn + "norm." + {"w": "weight", "b": "bias"}[parts[-1]], g
+    if name.startswith("pn.head."):
+        return pn + "head." + {"w": "weight", "b": "bias"}[parts[-1]], g.view(5, 768) if parts[-1] == "w" else g
+    s, j = int(parts[1][1:]), int(parts[2][1:])
+    C = CNX_DIMS[s]
+    k = f"{pn}stages.{s}.{j}."
+    leaf = ".".join(parts[3:])
+    if leaf == "dw.w":
+        return k + "dwconv.weight", g.view(49, C).t().reshape(C, 1, 7, 7)
+    if leaf == "dw.b":
+        return k + "dwconv.bias", g
+    if leaf == "gamma":
+        return k + "gamma", g
+    layer, wb = parts[3], parts[4]
+    if layer == "ln":
+        return k + "norm." + {"w": "weight", "b": "bias"}[wb], g
+    key = {"pw1": "pwconv1", "pw2": "pwconv2"}[layer]
+    if wb == "w":
+        return k + key + ".weight", g.view(4 * C, C) if layer == "pw1" else g.view(C, 4 * C)
+    return k + key + ".bias", g
