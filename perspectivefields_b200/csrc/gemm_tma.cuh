@@ -22,7 +22,8 @@
 //                     where the epilogue is a large share of a tile's time.  Same K order per output as the cooperative schedule.
 //
 // Epilogue (fused): + bias | border-class bias, ReLU / GELU, layer scale, + relu?(residual), + second residual; writes the
-// fp32 tensor and/or the bf16 hi/lo planes (optionally rectified) that the next GEMM will TMA-load.
+// fp32 tensor and/or the bf16 hi/lo planes (optionally rectified) that the next GEMM will TMA-load.  Residual loads and both kinds
+// of store move through the warpgroup's shared-memory staging rows as whole row segments.
 #pragma once
 #include <cuda.h>
 
@@ -299,14 +300,15 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
     long long m;
     bool valid;
     int cls_off = 0;
-    int bimg = 0, oy = 0, ox = 0;
+    int bimg = 0, oy = 0, ox = 0, oy0 = 0, ox0 = 0;
     if (MODE == MODE_GEMM) {
       m = (long long)mt * Cfg::kTileM + r;
       valid = m < p.M;
     } else {
       const int tx = mt % tiles_x, ty = (mt / tiles_x) % tiles_y;
       bimg = mt / (tiles_x * tiles_y);
-      oy = ty * kHtTileH + (r >> 3); ox = tx * kHtTileW + (r & 7);
+      oy0 = ty * kHtTileH; ox0 = tx * kHtTileW;
+      oy = oy0 + (r >> 3); ox = ox0 + (r & 7);
       valid = oy < p.H && ox < p.W;
       m = ((long long)bimg * p.H + oy) * p.W + ox;
       if (p.bias_mode == 2) {
@@ -316,6 +318,16 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
       }
     }
     const float* __restrict__ bias = p.bias ? p.bias + (long long)g * p.bias_gstride : nullptr;
+    // global row of staging row rr of this warpgroup (MODE_HALO: its pixel), and whether it exists
+    auto stage_row = [&](int rr, long long& mr) -> bool {
+      if (MODE == MODE_GEMM) {
+        mr = (long long)mt * Cfg::kTileM + (PP ? 0 : wg * 64) + rr;
+        return mr < p.M;
+      }
+      const int rt = wg * 64 + rr, py = oy0 + (rt >> 3), px = ox0 + (rt & 7);
+      mr = ((long long)bimg * p.H + py) * p.W + px;
+      return py < p.H && px < p.W;
+    };
     // accumulator fragment of m64nNk16: register 4 jb + 2 h + e holds row 16 (wt / 32) + lane / 4 + 8 h, column 8 jb + 2 (lane % 4) + e
     const int frow = (wt >> 5) * 16 + (lane >> 2), fcol = 2 * (lane & 3);
 #pragma unroll
@@ -332,134 +344,179 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
       }
       named_bar_sync(1 + wg, 128);
       const int ch = 2 * rd + eh;                 // this thread's 32-column chunk (warp-uniform)
+      const bool own = ch < BN / 32;              // (the last round of a BN % 64 == 32 tile has one chunk)
       const bool ph4 = MODE == MODE_HALO && BN == 128 && p.phase4;
-      // split planes outside phase mode go out through shared memory (staged_split below)
+      // fp32 output and split planes outside phase mode go out through shared memory (staged stores below)
       const bool staged_split = p.Shi && !ph4;
+      const int nb = n0 + ch * 32;
+      const bool chunk_ok = own && nb < p.N;     // warp-uniform
+      const bool live = valid && chunk_ok;
+      const float* srow = stage + erow * Cfg::kAccPitch + eh * 32;   // this thread's 32 columns of the staging rows
       float o[32];
-      if (ch < BN / 32) {
-        const int nb = n0 + ch * 32;
-        // output row / first output column of this chunk (phase mode: hi-res pixel of phase `ch`, channels 0-31)
-        const long long mo = ph4 ? ((long long)bimg * 2 * p.H + 2 * oy + (ch >> 1)) * (2 * p.W) + 2 * ox + (ch & 1) : m;
-        const int nbo = ph4 ? 0 : nb;
-        const bool chunk_ok = nb < p.N;      // warp-uniform
-        const float* srow = stage + erow * Cfg::kAccPitch + eh * 32;
+      if (own) {
 #pragma unroll
         for (int j = 0; j < 32; j += 4) {
           const float4 t = *reinterpret_cast<const float4*>(srow + j);
           o[j] = t.x; o[j + 1] = t.y; o[j + 2] = t.z; o[j + 3] = t.w;
         }
-        if (valid && chunk_ok) {
-          if (p.bias_mode) {
+      }
+      if (live) {
+        if (p.bias_mode) {
 #pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const float4 bv = __ldg(reinterpret_cast<const float4*>(bias + cls_off + nb + j));
-              o[j] += bv.x; o[j + 1] += bv.y; o[j + 2] += bv.z; o[j + 3] += bv.w;
-            }
+          for (int j = 0; j < 32; j += 4) {
+            const float4 bv = __ldg(reinterpret_cast<const float4*>(bias + cls_off + nb + j));
+            o[j] += bv.x; o[j + 1] += bv.y; o[j + 2] += bv.z; o[j + 3] += bv.w;
           }
-          if (p.act == 1) {
+        }
+        if (p.act == 1) {
 #pragma unroll
-            for (int j = 0; j < 32; ++j) o[j] = fmaxf(o[j], 0.f);
-          } else if (p.act == 2) {
+          for (int j = 0; j < 32; ++j) o[j] = fmaxf(o[j], 0.f);
+        } else if (p.act == 2) {
 #pragma unroll
-            for (int j = 0; j < 32; ++j) o[j] = gelu_erf(o[j]);
+          for (int j = 0; j < 32; ++j) o[j] = gelu_erf(o[j]);
+        }
+        if (p.gamma) {
+#pragma unroll
+          for (int j = 0; j < 32; j += 4) {
+            const float4 gv = __ldg(reinterpret_cast<const float4*>(p.gamma + nb + j));
+            o[j] *= gv.x; o[j + 1] *= gv.y; o[j + 2] *= gv.z; o[j + 3] *= gv.w;
           }
-          if (p.gamma) {
+        }
+      }
+      // Residuals.  A thread's 32 columns are 128 B of one row, so reading them from registers makes every warp-wide load touch
+      // 32 lines for 16 B each.  The warpgroup reads the round's 64 rows x 64 columns into the staging area instead (free once
+      // every thread has read its accumulators), as whole 256 B row segments: 16 lanes per row, 2 rows per instruction.  The
+      // rows a tile stores are its own, so in-place launches (res == C) still read every residual before it is overwritten.
+      auto stage_in = [&](const float* src, int ld, int coff) {
+        named_bar_sync(1 + wg, 128);              // every thread has read what the staging area holds
+        float4 v[8];
 #pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const float4 gv = __ldg(reinterpret_cast<const float4*>(p.gamma + nb + j));
-              o[j] *= gv.x; o[j + 1] *= gv.y; o[j + 2] *= gv.z; o[j + 3] *= gv.w;
-            }
+        for (int t = 0; t < 8; ++t) {
+          const int i = wt + 128 * t, col = rd * 64 + (i & 15) * 4;
+          long long mr;
+          v[t] = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (col < BN && n0 + col < p.N && stage_row(i >> 4, mr)) v[t] = *reinterpret_cast<const float4*>(src + mr * ld + coff + n0 + col);
+        }
+#pragma unroll
+        for (int t = 0; t < 8; ++t) {
+          const int i = wt + 128 * t;
+          *reinterpret_cast<float4*>(stage + (i >> 4) * Cfg::kAccPitch + (i & 15) * 4) = v[t];
+        }
+        named_bar_sync(1 + wg, 128);
+      };
+      if (p.res) {
+        stage_in(p.res, p.ldr, p.r_coff + g * p.r_gcoff);
+        if (live) {
+#pragma unroll
+          for (int j = 0; j < 32; j += 4) {
+            float4 rv = *reinterpret_cast<const float4*>(srow + j);
+            if (p.res_relu) { rv.x = fmaxf(rv.x, 0.f); rv.y = fmaxf(rv.y, 0.f); rv.z = fmaxf(rv.z, 0.f); rv.w = fmaxf(rv.w, 0.f); }
+            o[j] += rv.x; o[j + 1] += rv.y; o[j + 2] += rv.z; o[j + 3] += rv.w;
           }
-          if (p.res) {
-            const float* rp = p.res + m * p.ldr + p.r_coff + g * p.r_gcoff + nb;
+        }
+      }
+      if (p.res2) {
+        stage_in(p.res2, p.ldr2, p.r2_coff + g * p.r2_gcoff);
+        if (live) {
 #pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              float4 rv = *reinterpret_cast<const float4*>(rp + j);
-              if (p.res_relu) { rv.x = fmaxf(rv.x, 0.f); rv.y = fmaxf(rv.y, 0.f); rv.z = fmaxf(rv.z, 0.f); rv.w = fmaxf(rv.w, 0.f); }
-              o[j] += rv.x; o[j + 1] += rv.y; o[j + 2] += rv.z; o[j + 3] += rv.w;
-            }
+          for (int j = 0; j < 32; j += 4) {
+            const float4 rv = *reinterpret_cast<const float4*>(srow + j);
+            o[j] += rv.x; o[j + 1] += rv.y; o[j + 2] += rv.z; o[j + 3] += rv.w;
           }
-          if (p.res2) {
-            const float* rp = p.res2 + m * p.ldr2 + p.r2_coff + g * p.r2_gcoff + nb;
+        }
+      }
+      // output row / first output column of this chunk (phase mode: hi-res pixel of phase `ch`, channels 0-31)
+      const long long mo = ph4 ? ((long long)bimg * 2 * p.H + 2 * oy + (ch >> 1)) * (2 * p.W) + 2 * ox + (ch & 1) : m;
+      if (MODE == MODE_HALO && (BN == 32 || BN == 128) && p.pred_w && live) {
+        float v0 = __ldg(p.pred_b), v1 = p.pred_nc > 1 ? __ldg(p.pred_b + 1) : 0.f;
 #pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const float4 rv = *reinterpret_cast<const float4*>(rp + j);
-              o[j] += rv.x; o[j + 1] += rv.y; o[j + 2] += rv.z; o[j + 3] += rv.w;
-            }
+        for (int j = 0; j < 32; j += 4) {
+          const float4 w0 = __ldg(reinterpret_cast<const float4*>(p.pred_w + j));
+          v0 = fmaf(o[j], w0.x, v0); v0 = fmaf(o[j + 1], w0.y, v0); v0 = fmaf(o[j + 2], w0.z, v0); v0 = fmaf(o[j + 3], w0.w, v0);
+          if (p.pred_nc > 1) {
+            const float4 w1 = __ldg(reinterpret_cast<const float4*>(p.pred_w + 32 + j));
+            v1 = fmaf(o[j], w1.x, v1); v1 = fmaf(o[j + 1], w1.y, v1); v1 = fmaf(o[j + 2], w1.z, v1); v1 = fmaf(o[j + 3], w1.w, v1);
           }
-          if (MODE == MODE_HALO && (BN == 32 || BN == 128) && p.pred_w) {
-            float v0 = __ldg(p.pred_b), v1 = p.pred_nc > 1 ? __ldg(p.pred_b + 1) : 0.f;
+        }
+        const long long HWl = (long long)p.H * p.W * (ph4 ? 4 : 1);
+        const long long bi = mo / HWl, pix = mo - bi * HWl;
+        float* po = p.pred_out + bi * p.pred_nc * HWl + pix;
+        if (p.pred_mode == 1) {
+          const float nrm = fmaxf(sqrtf(v0 * v0 + v1 * v1), 1e-12f);
+          po[0] = v0 / nrm; po[HWl] = v1 / nrm;
+        } else {
+          po[0] = fminf(fmaxf(v0, -1.f), 1.f);
+        }
+      }
+      // Phase-mode stores (conv1's four output phases: rows are not one dense box).  A thread owns one row of the chunk (128 B of
+      // fp32, 64 B per bf16 plane); storing it 16 bytes at a time makes every warp-wide store touch 32 half-filled sectors.  The
+      // two lanes of an x-adjacent pixel pair exchange halves so that each store instruction writes 32 contiguous bytes per pair.
+      if (ph4 && chunk_ok && (p.C || p.Shi)) {
+        const bool odd = lane & 1;
+        const bool valid_p = __shfl_xor_sync(0xffffffffu, (int)valid, 1) != 0;
+        const long long mo_p = mo + (odd ? -2 : 2);                       // the partner's hi-res pixel (same image row, x +- 1)
+        const long long moA = odd ? mo_p : mo, moB = odd ? mo : mo_p;     // row A = the even lane's, row B = the odd lane's
+        const bool vA = odd ? valid_p : valid, vB = odd ? valid : valid_p;
+        if (p.C) {
+          float* cA = p.C + moA * p.ldc + p.c_coff + g * p.c_gcoff + (odd ? 4 : 0);
+          float* cB = p.C + moB * p.ldc + p.c_coff + g * p.c_gcoff + (odd ? 4 : 0);
 #pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const float4 w0 = __ldg(reinterpret_cast<const float4*>(p.pred_w + j));
-              v0 = fmaf(o[j], w0.x, v0); v0 = fmaf(o[j + 1], w0.y, v0); v0 = fmaf(o[j + 2], w0.z, v0); v0 = fmaf(o[j + 3], w0.w, v0);
-              if (p.pred_nc > 1) {
-                const float4 w1 = __ldg(reinterpret_cast<const float4*>(p.pred_w + 32 + j));
-                v1 = fmaf(o[j], w1.x, v1); v1 = fmaf(o[j + 1], w1.y, v1); v1 = fmaf(o[j + 2], w1.z, v1); v1 = fmaf(o[j + 3], w1.w, v1);
-              }
+          for (int t = 0; t < 4; ++t) {      // float4 slots 2t (even lane) and 2t + 1 (odd lane) of both rows
+            float k[4], rr[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              k[e] = odd ? o[8 * t + 4 + e] : o[8 * t + e];
+              rr[e] = __shfl_xor_sync(0xffffffffu, odd ? o[8 * t + e] : o[8 * t + 4 + e], 1);
             }
-            const long long HWl = (long long)p.H * p.W * (ph4 ? 4 : 1);
-            const long long bi = mo / HWl, pix = mo - bi * HWl;
-            float* po = p.pred_out + bi * p.pred_nc * HWl + pix;
-            if (p.pred_mode == 1) {
-              const float nrm = fmaxf(sqrtf(v0 * v0 + v1 * v1), 1e-12f);
-              po[0] = v0 / nrm; po[HWl] = v1 / nrm;
-            } else {
-              po[0] = fminf(fmaxf(v0, -1.f), 1.f);
+            if (vA) *reinterpret_cast<float4*>(cA + 8 * t) = odd ? make_float4(rr[0], rr[1], rr[2], rr[3]) : make_float4(k[0], k[1], k[2], k[3]);
+            if (vB) *reinterpret_cast<float4*>(cB + 8 * t) = odd ? make_float4(k[0], k[1], k[2], k[3]) : make_float4(rr[0], rr[1], rr[2], rr[3]);
+          }
+        }
+        if (p.Shi) {
+          const long long sA = moA * p.lds + p.s_coff + g * p.s_gcoff + (odd ? 8 : 0);
+          const long long sB = moB * p.lds + p.s_coff + g * p.s_gcoff + (odd ? 8 : 0);
+#pragma unroll
+          for (int t = 0; t < 2; ++t) {      // 8-column slots 2t (even lane) and 2t + 1 (odd lane) of both rows
+            float k[8], rr[8];
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+              const float mine = odd ? o[16 * t + 8 + e] : o[16 * t + e], give = odd ? o[16 * t + e] : o[16 * t + 8 + e];
+              k[e] = p.split_relu ? fmaxf(mine, 0.f) : mine;
+              rr[e] = __shfl_xor_sync(0xffffffffu, p.split_relu ? fmaxf(give, 0.f) : give, 1);
+            }
+            uint4 kh, kl, rh, rl;
+            split_bf16x2(k[0], k[1], kh.x, kl.x); split_bf16x2(k[2], k[3], kh.y, kl.y);
+            split_bf16x2(k[4], k[5], kh.z, kl.z); split_bf16x2(k[6], k[7], kh.w, kl.w);
+            split_bf16x2(rr[0], rr[1], rh.x, rl.x); split_bf16x2(rr[2], rr[3], rh.y, rl.y);
+            split_bf16x2(rr[4], rr[5], rh.z, rl.z); split_bf16x2(rr[6], rr[7], rh.w, rl.w);
+            if (vA) {
+              *reinterpret_cast<uint4*>(p.Shi + sA + 16 * t) = odd ? rh : kh;
+              *reinterpret_cast<uint4*>(p.Slo + sA + 16 * t) = odd ? rl : kl;
+            }
+            if (vB) {
+              *reinterpret_cast<uint4*>(p.Shi + sB + 16 * t) = odd ? kh : rh;
+              *reinterpret_cast<uint4*>(p.Slo + sB + 16 * t) = odd ? kl : rl;
             }
           }
         }
-        // Stores.  A thread owns one row of the chunk (128 B of fp32, 64 B per bf16 plane); storing it 16 bytes at a time makes every
-        // warp-wide store touch 32 half-filled sectors.  The two lanes of an adjacent row pair (x-adjacent pixels in halo mode)
-        // exchange halves so that each store instruction writes 32 contiguous bytes per pair: full sectors, half as many per request.
-        if (chunk_ok && (p.C || (p.Shi && !staged_split))) {
-          const bool odd = lane & 1;
-          const bool valid_p = __shfl_xor_sync(0xffffffffu, (int)valid, 1) != 0;
-          const long long mo_p = mo + (odd ? -1 : 1) * (ph4 ? 2 : 1);       // the partner's row (pixel: same image row, x +- 1)
-          const long long moA = odd ? mo_p : mo, moB = odd ? mo : mo_p;     // row A = the even lane's, row B = the odd lane's
-          const bool vA = odd ? valid_p : valid, vB = odd ? valid : valid_p;
-          if (p.C) {
-            float* cA = p.C + moA * p.ldc + p.c_coff + g * p.c_gcoff + nbo + (odd ? 4 : 0);
-            float* cB = p.C + moB * p.ldc + p.c_coff + g * p.c_gcoff + nbo + (odd ? 4 : 0);
+      }
+      // fp32 output: the round's results go back to the staging rows (free once every thread has read them), and the warpgroup
+      // stores whole 256 B row segments: 16 lanes per row, 2 rows per instruction, instead of 16 B pieces of 32 rows.
+      if (p.C && !ph4) {
+        named_bar_sync(1 + wg, 128);              // every thread has read what the staging area holds
+        if (own) {
+          float* drow = stage + erow * Cfg::kAccPitch + eh * 32;
 #pragma unroll
-            for (int t = 0; t < 4; ++t) {      // float4 slots 2t (even lane) and 2t + 1 (odd lane) of both rows
-              float k[4], rr[4];
+          for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(drow + j) = make_float4(o[j], o[j + 1], o[j + 2], o[j + 3]);
+        }
+        named_bar_sync(1 + wg, 128);
+        float* cbase = p.C + p.c_coff + g * p.c_gcoff + n0;
 #pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                k[e] = odd ? o[8 * t + 4 + e] : o[8 * t + e];
-                rr[e] = __shfl_xor_sync(0xffffffffu, odd ? o[8 * t + e] : o[8 * t + 4 + e], 1);
-              }
-              if (vA) *reinterpret_cast<float4*>(cA + 8 * t) = odd ? make_float4(rr[0], rr[1], rr[2], rr[3]) : make_float4(k[0], k[1], k[2], k[3]);
-              if (vB) *reinterpret_cast<float4*>(cB + 8 * t) = odd ? make_float4(k[0], k[1], k[2], k[3]) : make_float4(rr[0], rr[1], rr[2], rr[3]);
-            }
-          }
-          if (p.Shi && !staged_split) {
-            const long long sA = moA * p.lds + p.s_coff + g * p.s_gcoff + nbo + (odd ? 8 : 0);
-            const long long sB = moB * p.lds + p.s_coff + g * p.s_gcoff + nbo + (odd ? 8 : 0);
-#pragma unroll
-            for (int t = 0; t < 2; ++t) {      // 8-column slots 2t (even lane) and 2t + 1 (odd lane) of both rows
-              float k[8], rr[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) {
-                const float mine = odd ? o[16 * t + 8 + e] : o[16 * t + e], give = odd ? o[16 * t + e] : o[16 * t + 8 + e];
-                k[e] = p.split_relu ? fmaxf(mine, 0.f) : mine;
-                rr[e] = __shfl_xor_sync(0xffffffffu, p.split_relu ? fmaxf(give, 0.f) : give, 1);
-              }
-              uint4 kh, kl, rh, rl;
-              split_bf16x2(k[0], k[1], kh.x, kl.x); split_bf16x2(k[2], k[3], kh.y, kl.y);
-              split_bf16x2(k[4], k[5], kh.z, kl.z); split_bf16x2(k[6], k[7], kh.w, kl.w);
-              split_bf16x2(rr[0], rr[1], rh.x, rl.x); split_bf16x2(rr[2], rr[3], rh.y, rl.y);
-              split_bf16x2(rr[4], rr[5], rh.z, rl.z); split_bf16x2(rr[6], rr[7], rh.w, rl.w);
-              if (vA) {
-                *reinterpret_cast<uint4*>(p.Shi + sA + 16 * t) = odd ? rh : kh;
-                *reinterpret_cast<uint4*>(p.Slo + sA + 16 * t) = odd ? rl : kl;
-              }
-              if (vB) {
-                *reinterpret_cast<uint4*>(p.Shi + sB + 16 * t) = odd ? kh : rh;
-                *reinterpret_cast<uint4*>(p.Slo + sB + 16 * t) = odd ? kl : rl;
-              }
-            }
-          }
+        for (int t = 0; t < 8; ++t) {
+          const int i = wt + 128 * t, col = rd * 64 + (i & 15) * 4;
+          long long mr;
+          if (col < BN && n0 + col < p.N && stage_row(i >> 4, mr))
+            *reinterpret_cast<float4*>(cbase + mr * p.ldc + col) = *reinterpret_cast<const float4*>(stage + (i >> 4) * Cfg::kAccPitch + (i & 15) * 4);
         }
       }
       // Split planes: a thread's 32 columns are 64 B per plane, so stores from registers leave every 128 B line half written by
@@ -467,9 +524,9 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
       // shared memory instead (the fp32 staging area, free once every thread has read it: 64 rows x 128 B per plane, 16 B
       // pieces XOR-swizzled by row), and the warpgroup stores whole 128 B row segments: 8 lanes per row, 4 rows per instruction.
       if (staged_split) {
-        named_bar_sync(1 + wg, 128);              // every thread has read its fp32 chunk of this round
+        named_bar_sync(1 + wg, 128);              // every thread has read what the staging area holds
         unsigned char* sS = reinterpret_cast<unsigned char*>(stage);
-        if (ch < BN / 32) {
+        if (own) {
 #pragma unroll
           for (int t = 0; t < 4; ++t) {           // 8-column pieces eh * 4 + t of row erow
             uint4 h, l;
@@ -488,19 +545,8 @@ __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_c
         for (int i = wt; i < 2 * 64 * 8; i += 128) {
           const int lo_plane = i >> 9, rr = (i >> 3) & 63, pc = i & 7;
           const int col = rd * 64 + pc * 8;       // column within the tile
-          if (col >= BN || n0 + col >= p.N) continue;
           long long mr;
-          bool vr;
-          if (MODE == MODE_GEMM) {
-            mr = (long long)mt * Cfg::kTileM + (PP ? 0 : wg * 64) + rr;
-            vr = mr < p.M;
-          } else {
-            const int rt = wg * 64 + rr, tx = mt % tiles_x, ty = (mt / tiles_x) % tiles_y;
-            const int py = ty * kHtTileH + (rt >> 3), px = tx * kHtTileW + (rt & 7);
-            vr = py < p.H && px < p.W;
-            mr = ((long long)bimg * p.H + py) * p.W + px;
-          }
-          if (!vr) continue;
+          if (col >= BN || n0 + col >= p.N || !stage_row(rr, mr)) continue;
           const uint4 v = *reinterpret_cast<const uint4*>(sS + lo_plane * 64 * 128 + rr * 128 + ((pc ^ (rr & 7)) << 4));
           *reinterpret_cast<uint4*>((lo_plane ? p.Slo : p.Shi) + mr * p.lds + p.s_coff + g * p.s_gcoff + n0 + col) = v;
         }
