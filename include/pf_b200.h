@@ -437,6 +437,43 @@ int pf_op_conv1_ring(const void* c_hi, const void* c_lo, int B, int H, int W, co
 /* Host only, no device needed: the (bn, kb) the engine's dispatcher picks for a launch (mode 0 GEMM with M rows; mode 1 halo:
  * K = 9 * Cin) on a device with sm_count SMs. */
 int pf_tma_pick_tile(int mode, int64_t M, int N, int K, int sm_count, int* bn, int* kb);
+/* ParamNet training's backward, one piece at a time, through the host helper pf_param_backward runs it with (same partition,
+ * same reduction order).  DEVICE pointers; scratch is allocated, sized by a dry run and filled with NaN bytes, inside the call,
+ * which ends with a stream synchronisation.  Every argument is checked before anything is launched (PF_ERR_ARG).
+ *   pn_wgrad: out[N][K] = sum over r < R of dy[r * ldy + n] * X[r][k], X = x (fp32, row pitch ldx; op 1: GELU(x)) or
+ *     x_hi + x_lo (split planes, pitch ldx, op 0), on the GEMM engine as S grouped row chunks of `chunk` rows; S and chunk out.
+ *   pn_colsum: out[c] = sum over r of src[r * C + c].
+ *   pn_ln_bwd: LayerNorm (eps 1e-6) backward over rows of C channels (a multiple of 32, <= 768): dx written, d weight at g,
+ *     d bias at g + C.
+ *   pn_dw7_bwd: depthwise 7x7 (pad 3) on NHWC [B, H, W, C] (C a multiple of 32): dw [50][C] (49 taps (ky, kx), then the bias)
+ *     from x and dt = d output; dx = d input (the forward kernel with w_rot, the kernel rotated by 180 degrees, [49][C]).
+ *   pn_stem_bwd: 4x4 / stride 4 stem on pin [B, 4 OH, 4 OW, 4] (channel 3 unused) from dS [B, OH, OW, 96]: dw [49][96]
+ *     ((ky, kx, ci) rows, then the bias); dpin channels 0-2 from w [48][96] (channel 3 is not written).
+ *   rows_per_block (may be NULL): image rows per partial sum of the weight-gradient kernel.
+ *   pn_fields_grad: backward of the nearest resize [B, 3, IH, IW] -> dpin [B, OH, OW, 4]: dgrav [B, 2, IH, IW], dlat [B, 1, IH, IW].
+ *   pn_tail_bwd: mean pool -> LayerNorm(768) -> Linear 768 -> 5 of feat [n, HW, 768] from draw [n, 5]: dx [n, HW, 768];
+ *     grads: norm.w (768), norm.b (768), head.w (5 x 768), head.b (5).
+ *   pn_pw2_grads: from G [C][K], sdy [C], gamma [C], W = w_hi + w_lo [C][K], b [C]: dW = gamma G, db = gamma sdy,
+ *     dgamma = sum_k W G + b sdy.
+ *   pn_gelu_bwd: u[i] = dh[i] * GELU'(u[i]) in place (exact erf), and its split planes when hi / lo are given.
+ *   pn_scale_split: split planes of src [n / C][C] (times scale[c] when scale is not NULL).
+ *   pn_col2im2: the 2 x 2 / stride 2 patch matrix dP [B * H/2 * W/2][4 C] back to [B, H, W, C] (H, W even). */
+int pf_op_pn_wgrad(const float* dy, int ldy, const float* x, const void* x_hi, const void* x_lo, int op, int ldx, int64_t R, int N, int K,
+                   float* out, int* S, int* chunk, void* stream);
+int pf_op_pn_colsum(const float* src, int64_t R, int C, float* out, void* stream);
+int pf_op_pn_ln_bwd(const float* x, const float* dy, int64_t R, int C, const float* w, float* dx, float* g, void* stream);
+int pf_op_pn_dw7_bwd(const float* x, const float* dt, int B, int H, int W, int C, const float* w_rot, float* dw, float* dx, int* rows_per_block,
+                     void* stream);
+int pf_op_pn_stem_bwd(const float* pin, const float* dS, const float* w, int B, int OH, int OW, float* dw, float* dpin, int* rows_per_block,
+                      void* stream);
+int pf_op_pn_fields_grad(const float* dpin, int B, int IH, int IW, int OH, int OW, float* dgrav, float* dlat, void* stream);
+int pf_op_pn_tail_bwd(const float* feat, int n, int HW, const float* nw, const float* nb, const float* hw, const float* draw, float* dx,
+                      float* grads, void* stream);
+int pf_op_pn_pw2_grads(const float* G, const float* sdy, int C, int K, const float* gamma, const void* w_hi, const void* w_lo, const float* b,
+                       float* dW, float* db, float* dgamma, void* stream);
+int pf_op_pn_gelu_bwd(const float* dh, float* u, int64_t n, void* hi, void* lo, void* stream);
+int pf_op_pn_scale_split(const float* src, const float* scale, int64_t n, int C, void* hi, void* lo, void* stream);
+int pf_op_pn_col2im2(const float* dP, int B, int H, int W, int C, float* out, void* stream);
 int pf_op_layernorm(const float* x, float* y, int64_t rows, int C, const float* w, const float* b, float eps, void* stream);
 int pf_op_attention_tc(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream);   /* q / kv split into bf16 hi/lo planes first, then the mma.sync core as the forward graph runs it */
 int pf_op_attention_tc_bf16(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream); /* the same in the bf16 precision mode: one mma.sync per product on bf16(q), bf16(k), bf16(P), bf16(v) */

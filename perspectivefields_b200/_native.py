@@ -206,6 +206,17 @@ def lib():
         "pf_rectify_workspace": (i64, [ctypes.POINTER(pf_rectify_image), i32]),
         "pf_rectify_views": (i32, [i32, ctypes.POINTER(pf_rectify_image), i32, vp, vp, vp, vp, i32, vp, i32, i32, ctypes.c_double, i32,
                                    ctypes.POINTER(ctypes.c_int32), vp, vp, vp, i64, vp]),
+        "pf_op_pn_wgrad": (i32, [vp, i32, vp, vp, vp, i32, i32, i64, i32, i32, vp, ctypes.POINTER(i32), ctypes.POINTER(i32), vp]),
+        "pf_op_pn_colsum": (i32, [vp, i64, i32, vp, vp]),
+        "pf_op_pn_ln_bwd": (i32, [vp, vp, i64, i32, vp, vp, vp, vp]),
+        "pf_op_pn_dw7_bwd": (i32, [vp, vp, i32, i32, i32, i32, vp, vp, vp, ctypes.POINTER(i32), vp]),
+        "pf_op_pn_stem_bwd": (i32, [vp, vp, vp, i32, i32, i32, vp, vp, ctypes.POINTER(i32), vp]),
+        "pf_op_pn_fields_grad": (i32, [vp, i32, i32, i32, i32, i32, vp, vp, vp]),
+        "pf_op_pn_tail_bwd": (i32, [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]),
+        "pf_op_pn_pw2_grads": (i32, [vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp]),
+        "pf_op_pn_gelu_bwd": (i32, [vp, vp, i64, vp, vp, vp]),
+        "pf_op_pn_scale_split": (i32, [vp, vp, i64, i32, vp, vp, vp]),
+        "pf_op_pn_col2im2": (i32, [vp, i32, i32, i32, i32, vp, vp]),
         "pf_op_layernorm": (i32, [vp, vp, i64, i32, vp, vp, f32, vp]),
         "pf_op_attention_tc": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
         "pf_op_attention_tc_bf16": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
@@ -259,7 +270,9 @@ EXPORTS = ["pf_abi_version", "pf_last_error", "pf_kernel_launch_count", "pf_crea
            "pf_op_conv_gemm", "pf_op_tma", "pf_op_tma_bf16", "pf_op_conv1_ring", "pf_tma_pick_tile", "pf_op_layernorm",
            "pf_op_attention_tc", "pf_op_attention_tc_bf16", "pf_op_attention_tc_keys", "pf_op_dwconv3x3_gelu",
            "pf_op_dwconv7x7", "pf_op_upsample2x", "pf_op_preprocess", "pf_op_preprocess_sized", "pf_op_fill_stream", "pf_op_resize_u8",
-           "pf_op_resize_f32", "pf_op_argmax_decode", "pf_op_pred_argmax_decode", "pf_op_postprocess", "pf_op_postprocess_sized"]
+           "pf_op_resize_f32", "pf_op_argmax_decode", "pf_op_pred_argmax_decode", "pf_op_postprocess", "pf_op_postprocess_sized",
+           "pf_op_pn_wgrad", "pf_op_pn_colsum", "pf_op_pn_ln_bwd", "pf_op_pn_dw7_bwd", "pf_op_pn_stem_bwd", "pf_op_pn_fields_grad",
+           "pf_op_pn_tail_bwd", "pf_op_pn_pw2_grads", "pf_op_pn_gelu_bwd", "pf_op_pn_scale_split", "pf_op_pn_col2im2"]
 
 
 class PfError(RuntimeError):

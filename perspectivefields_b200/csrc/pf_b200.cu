@@ -1086,12 +1086,13 @@ static int pn_tsplit(Fwd& F, const float* src, const SplitT* ssrc, int ld, long 
   return PF_OK;
 }
 static int pn_wgrad(Fwd& F, const SplitT& aT, const SplitT& bT, int N, int K, const WgPlan& pl, float* part) {
-  if (F.dry) return PF_OK;
   TmaGemmParams p{};
   p.M = N; p.N = K; p.K = pl.chunk; p.Cin = pl.chunk; p.a_gc = pl.chunk; p.groups = pl.S;
   p.C = part; p.ldc = K; p.c_gcoff = N * K;
   const int bn = tma_pick_bn(K, MODE_GEMM), kb = tma_pick_kb(bn, pl.chunk, MODE_GEMM);
+  // (checked in the sizing dry run too, so that a shape the engine cannot run fails before anything is launched)
   if (const char* msg = gemm_tma_check(MODE_GEMM, p, bn, kb, false, false, F.np())) return fail(PF_ERR_ARG, "weight-gradient GEMM (bn %d, kb %d): %s", bn, kb, msg);
+  if (F.dry) return PF_OK;
   TmaMaps maps{};
   const char* msg = F.map2d(&maps.a_hi, aT.hi, pl.Rp, N, pl.Rp, 128, kb);
   if (!msg) msg = F.map2d(&maps.a_lo, aT.lo, pl.Rp, N, pl.Rp, 128, kb);
@@ -1102,9 +1103,11 @@ static int pn_wgrad(Fwd& F, const SplitT& aT, const SplitT& bT, int N, int K, co
   F.picked_bn = bn; F.picked_kb = kb; F.picked_sched = 1;
   return F.launch_tma(MODE_GEMM, maps, p, bn, kb, false);
 }
-static int pn_wgrad_full(Fwd& F, const float* dy, int ldy, const SplitT* xs, const float* xf, int op, int ldx, long long R, int N, int K, float* out) {
+static int pn_wgrad_full(Fwd& F, const float* dy, int ldy, const SplitT* xs, const float* xf, int op, int ldx, long long R, int N, int K, float* out,
+                         WgPlan* plan = nullptr) {
   const long long m = F.ar.mark();
   const WgPlan pl = pn_wg_plan(F.e, R, N, K);
+  if (plan) *plan = pl;
   SplitT aT, bT;
   TRY(pn_tsplit(F, dy, nullptr, ldy, R, N, pl, false, 0, aT));
   TRY(pn_tsplit(F, xf, xs, ldx, R, K, pl, true, op, bT));
@@ -1118,6 +1121,38 @@ static int pn_wgrad_full(Fwd& F, const float* dy, int ldy, const SplitT* xs, con
 static int pn_dw_launch(Fwd& F, const float* x, float* y, int rh, int rw, int C, const float* w, const float* b) {
   if (!F.dry) LAUNCHED(launch_pdl(dwconv7x7_kernel, dim3(ew_grid((long long)F.n * ((rh + 1) / 2) * ((rw + PF_DW7_PX - 1) / PF_DW7_PX) * (C / 4))), dim3(256), 0, F.st,
                                   x, y, F.n, rh, rw, C, w, b));
+  return PF_OK;
+}
+
+// Image rows per block of the depthwise and stem weight-gradient kernels: at most 1024 partials, one row each while that suffices
+static int pn_rows_per_block(int rows) { return std::max(1, cdiv(rows, 1024)); }
+
+// depthwise 7x7 weight and bias gradients of the F.n images [rh, rw, C]: out [50][C] (49 taps, then the bias)
+static int pn_dw7_wgrad(Fwd& F, const float* xin, const float* dt, int rh, int rw, int C, float* out, int* rpb_out = nullptr) {
+  const int rows = F.n * rh, rpb = pn_rows_per_block(rows), np_ = cdiv(rows, rpb);
+  if (rpb_out) *rpb_out = rpb;
+  const long long m = F.ar.mark();
+  float* part = F.ar.f((long long)np_ * 50 * C);
+  if (!F.dry) LAUNCHED((dw7_wgrad_kernel<<<dim3(np_, C / 32), 256, 0, F.st>>>(xin, dt, F.n, rh, rw, C, rpb, part), cudaGetLastError()));
+  TRY(pn_reduce(F, part, np_, 50LL * C, out));
+  F.ar.release(m);
+  return PF_OK;
+}
+
+static int pn_pw2_grads(Fwd& F, const float* G, const float* sdy, int C, int K, const float* gamma, const GemmW& w2, float* dW, float* db, float* dgamma) {
+  if (!F.dry) LAUNCHED((pw2_grads_kernel<<<cdiv(C, 8), 256, 0, F.st>>>(G, sdy, C, K, gamma, w2.hi, w2.lo, w2.b, dW, db, dgamma), cudaGetLastError()));
+  return PF_OK;
+}
+static int pn_gelu_bwd(Fwd& F, const float* dh, float* u, long long n, __nv_bfloat16* hi, __nv_bfloat16* lo) {
+  if (!F.dry) LAUNCHED((gelu_bwd_kernel<<<ew_grid(n), 256, 0, F.st>>>(dh, u, n, hi, lo), cudaGetLastError()));
+  return PF_OK;
+}
+static int pn_scale_split(Fwd& F, const float* src, const float* scale, long long n, int C, const SplitT& out) {
+  if (!F.dry) LAUNCHED((scale_split_kernel<<<ew_grid(n), 256, 0, F.st>>>(src, scale, n, C, out.hi, out.lo), cudaGetLastError()));
+  return PF_OK;
+}
+static int pn_col2im2(Fwd& F, const float* dP, int rh, int rw, int C, float* out) {
+  if (!F.dry) LAUNCHED((col2im2_kernel<<<ew_grid((long long)F.n * rh * rw * C), 256, 0, F.st>>>(dP, F.n, rh, rw, C, out), cudaGetLastError()));
   return PF_OK;
 }
 
@@ -1149,18 +1184,17 @@ static int pn_block_bwd(Fwd& F, int s, int j, const float* xin, float* dx, int r
     float* sdx = ar.f(C);
     TRY(pn_wgrad_full(F, dx, C, nullptr, u, 1, 4 * C, R, C, 4 * C, G));
     TRY(pn_colsum(F, dx, R, C, sdx));
-    if (!dry) LAUNCHED((pw2_grads_kernel<<<cdiv(C, 8), 256, 0, st>>>(G, sdx, C, 4 * C, b.gamma, b.pw2.hi, b.pw2.lo, b.pw2.b, grads + pn_goff(P + "pw2.w"),
-                                                                  grads + pn_goff(P + "pw2.b"), grads + pn_goff(P + "gamma")), cudaGetLastError()));
+    TRY(pn_pw2_grads(F, G, sdx, C, 4 * C, b.gamma, b.pw2, grads + pn_goff(P + "pw2.w"), grads + pn_goff(P + "pw2.b"), grads + pn_goff(P + "gamma")));
     ar.release(m1);
   }
   // dh = (gamma dx) W2, then du = dh GELU'(u), written over u
   {
     const long long m1 = ar.mark();
     SplitT dz = F.salloc(R, C);
-    if (!dry) LAUNCHED((scale_split_kernel<<<ew_grid(R * C), 256, 0, st>>>(dx, b.gamma, R * C, C, dz.hi, dz.lo), cudaGetLastError()));
+    TRY(pn_scale_split(F, dx, b.gamma, R * C, C, dz));
     float* dh = ar.f(R * 4 * C);
     { Fwd::Epi o; o.C = dh; o.ldc = 4 * C; TRY(F.tgemm(dz, R, C, 0, T.pw2_t[s][j], 4 * C, o)); }
-    if (!dry) LAUNCHED((gelu_bwd_kernel<<<ew_grid(R * 4 * C), 256, 0, st>>>(dh, u, R * 4 * C, nullptr, nullptr), cudaGetLastError()));
+    TRY(pn_gelu_bwd(F, dh, u, R * 4 * C, nullptr, nullptr));
     ar.release(m1);
   }
   // pwconv1 weight and bias
@@ -1171,7 +1205,7 @@ static int pn_block_bwd(Fwd& F, int s, int j, const float* xin, float* dx, int r
   {
     const long long m1 = ar.mark();
     SplitT du = F.salloc(R, 4 * C);
-    if (!dry) LAUNCHED((scale_split_kernel<<<ew_grid(R * 4 * C), 256, 0, st>>>(u, nullptr, R * 4 * C, 4 * C, du.hi, du.lo), cudaGetLastError()));
+    TRY(pn_scale_split(F, u, nullptr, R * 4 * C, 4 * C, du));
     Fwd::Epi o; o.C = dy; o.ldc = C;
     TRY(F.tgemm(du, R, 4 * C, 0, T.pw1_t[s][j], C, o));
     ar.release(m1);
@@ -1179,14 +1213,7 @@ static int pn_block_bwd(Fwd& F, int s, int j, const float* xin, float* dx, int r
   float* dt = ar.f(R * C);
   TRY(pn_ln_bwd(F, t, dy, R, C, b.ln.w, dt, grads + pn_goff(P + "ln.w")));
   // depthwise 7x7: weight and bias, then the data gradient (the forward kernel with the rotated kernel) added to the residual's
-  {
-    const int rows = F.n * rh, rpb = std::max(1, cdiv(rows, 1024)), np_ = cdiv(rows, rpb);
-    const long long m1 = ar.mark();
-    float* part = ar.f((long long)np_ * 50 * C);
-    if (!dry) LAUNCHED((dw7_wgrad_kernel<<<dim3(np_, C / 32), 256, 0, st>>>(xin, dt, F.n, rh, rw, C, rpb, part), cudaGetLastError()));
-    TRY(pn_reduce(F, part, np_, 50LL * C, grads + pn_goff(P + "dw.w")));
-    ar.release(m1);
-  }
+  TRY(pn_dw7_wgrad(F, xin, dt, rh, rw, C, grads + pn_goff(P + "dw.w")));
   TRY(pn_dw_launch(F, dt, dy, rh, rw, C, T.dw_rot[s][j], T.zero));
   if (!dry) LAUNCHED((add_inplace_kernel<<<ew_grid(R * C), 256, 0, st>>>(dx, dy, R * C), cudaGetLastError()));
   ar.release(m0);
@@ -1211,15 +1238,49 @@ static int pn_downsample_bwd(Fwd& F, int s, const float* xprev, int rh, int rw, 
   {
     const long long m1 = ar.mark();
     SplitT d = F.salloc(R2, C);
-    if (!F.dry) LAUNCHED((scale_split_kernel<<<ew_grid(R2 * C), 256, 0, F.st>>>(dxn, nullptr, R2 * C, C, d.hi, d.lo), cudaGetLastError()));
+    TRY(pn_scale_split(F, dxn, nullptr, R2 * C, C, d));
     float* dP = ar.f(R2 * 4 * Cp);
     Fwd::Epi o; o.C = dP; o.ldc = 4 * Cp;
     TRY(F.tgemm(d, R2, C, 0, e->pn_train.ds_t[s], 4 * Cp, o));
-    if (!F.dry) LAUNCHED((col2im2_kernel<<<ew_grid(R * Cp), 256, 0, F.st>>>(dP, F.n, rh, rw, Cp, dln), cudaGetLastError()));
+    TRY(pn_col2im2(F, dP, rh, rw, Cp, dln));
     ar.release(m1);
   }
   TRY(pn_ln_bwd(F, xprev, dln, R, Cp, e->pn_ds_ln[s].w, dprev, grads + pn_goff(P + "ln.w")));
   ar.release(m0);
+  return PF_OK;
+}
+
+// tail (pool -> LayerNorm(768) -> head) backward of the F.n pairs: dx [n, HW, 768] and the tail's gradients at g (norm.w, norm.b,
+// head.w, head.b: kTailGrads values)
+static int pn_tail_bwd(Fwd& F, const float* feat, int HW, const float* nw, const float* nb, const float* hw, const float* draw, float* dx, float* g) {
+  const long long m = F.ar.mark();
+  float* part = F.ar.f((long long)F.n * kTailGrads);
+  if (!F.dry) LAUNCHED((param_tail_bwd_kernel<<<F.n, 256, 0, F.st>>>(feat, HW, nw, nb, hw, draw, dx, part), cudaGetLastError()));
+  TRY(pn_reduce(F, part, F.n, kTailGrads, g));
+  F.ar.release(m);
+  return PF_OK;
+}
+
+// stem weight and bias gradients from the packed input [n, 4 OH, 4 OW, 4] and dS [n, OH, OW, 96]: out [49][96] (48 weight rows
+// (ky, kx, ci), then the bias)
+static int pn_stem_wgrad(Fwd& F, const float* pin, const float* dS, int OH, int OW, float* out, int* rpb_out = nullptr) {
+  const int rows = F.n * OH, rpb = pn_rows_per_block(rows), np_ = cdiv(rows, rpb);
+  if (rpb_out) *rpb_out = rpb;
+  const long long m = F.ar.mark();
+  float* part = F.ar.f((long long)np_ * 49 * 96);
+  if (!F.dry) LAUNCHED((stem_wgrad_kernel<<<dim3(np_, 3), 256, 0, F.st>>>(pin, dS, F.n, OH, OW, rpb, part), cudaGetLastError()));
+  TRY(pn_reduce(F, part, np_, 49LL * 96, out));
+  F.ar.release(m);
+  return PF_OK;
+}
+static int pn_stem_dgrad(Fwd& F, const float* dS, const float* w, int OH, int OW, float* dpin) {
+  if (!F.dry) LAUNCHED((stem_dgrad_kernel<<<ew_grid((long long)F.n * OH * OW * 48), 256, 0, F.st>>>(dS, w, F.n, OH, OW, dpin), cudaGetLastError()));
+  return PF_OK;
+}
+// backward of the nearest resize of the fields IH x IW -> OH x OW (pack_fields_kernel)
+static int pn_fields_grad(Fwd& F, const float* dpin, int IH, int IW, int OH, int OW, float* dgrav, float* dlat) {
+  if (!F.dry)
+    LAUNCHED((unpack_fields_grad_kernel<<<(unsigned)cdivl((long long)F.n * IH * IW, 256), 256, 0, F.st>>>(dpin, F.n, IH, IW, OH, OW, dgrav, dlat), cudaGetLastError()));
   return PF_OK;
 }
 
@@ -1235,14 +1296,7 @@ static int bwd_paramnet(Fwd& F, const PnSaved& sv, const float* draw, float* gra
   rh[0] = SH / 4; rw[0] = SW / 4;
   for (int s = 1; s < 4; ++s) { rh[s] = rh[s - 1] / 2; rw[s] = rw[s - 1] / 2; }
   float* dx = ar.f((long long)n * rh[3] * rw[3] * 768);
-  {
-    const long long m = ar.mark();
-    float* part = ar.f((long long)n * kTailGrads);
-    if (!F.dry) LAUNCHED((param_tail_bwd_kernel<<<n, 256, 0, F.st>>>(sv.xs[3][kCnxDepths[3]], rh[3] * rw[3], e->pn_norm.w, e->pn_norm.b, e->pn_head_w, draw, dx, part),
-                          cudaGetLastError()));
-    TRY(pn_reduce(F, part, n, kTailGrads, grads + pn_goff("pn.norm.w")));
-    ar.release(m);
-  }
+  TRY(pn_tail_bwd(F, sv.xs[3][kCnxDepths[3]], rh[3] * rw[3], e->pn_norm.w, e->pn_norm.b, e->pn_head_w, draw, dx, grads + pn_goff("pn.norm.w")));
   for (int s = 3; s >= 0; --s) {
     for (int j = kCnxDepths[s] - 1; j >= 0; --j) TRY(pn_block_bwd(F, s, j, sv.xs[s][j], dx, rh[s], rw[s], grads));
     if (s > 0) {
@@ -1255,21 +1309,11 @@ static int bwd_paramnet(Fwd& F, const PnSaved& sv, const float* draw, float* gra
   const long long R0 = (long long)n * rh[0] * rw[0];
   float* dstem = ar.f(R0 * 96);
   TRY(pn_ln_bwd(F, sv.stem_pre, dx, R0, 96, e->pn_stem_ln.w, dstem, grads + pn_goff("pn.stem.ln.w")));
-  {
-    const int rows = n * rh[0], rpb = std::max(1, cdiv(rows, 1024)), np_ = cdiv(rows, rpb);
-    const long long m = ar.mark();
-    float* part = ar.f((long long)np_ * 49 * 96);
-    if (!F.dry) LAUNCHED((stem_wgrad_kernel<<<dim3(np_, 3), 256, 0, F.st>>>(sv.pin, dstem, n, rh[0], rw[0], rpb, part), cudaGetLastError()));
-    TRY(pn_reduce(F, part, np_, 49LL * 96, grads + pn_goff("pn.stem.w")));
-    ar.release(m);
-  }
+  TRY(pn_stem_wgrad(F, sv.pin, dstem, rh[0], rw[0], grads + pn_goff("pn.stem.w")));
   if (dgrav) {
     float* dpin = ar.f((long long)n * SH * SW * 4);
-    if (!F.dry) {
-      LAUNCHED((stem_dgrad_kernel<<<ew_grid(R0 * 48), 256, 0, F.st>>>(dstem, e->pn_stem_w, n, rh[0], rw[0], dpin), cudaGetLastError()));
-      LAUNCHED((unpack_fields_grad_kernel<<<(unsigned)cdivl((long long)n * e->net_h * e->net_w, 256), 256, 0, F.st>>>(dpin, n, e->net_h, e->net_w, SH, SW, dgrav, dlat),
-                cudaGetLastError()));
-    }
+    TRY(pn_stem_dgrad(F, dstem, e->pn_stem_w, rh[0], rw[0], dpin));
+    TRY(pn_fields_grad(F, dpin, e->net_h, e->net_w, SH, SW, dgrav, dlat));
   }
   return PF_OK;
 }
@@ -1885,6 +1929,111 @@ static int op_tma(pf_tma_op* op, void* stream, bool bf16) {
   if (r == PF_OK) { op->picked_bn = F.picked_bn; op->picked_kb = F.picked_kb; op->picked_sched = F.picked_sched; }
   return r;
 }
+}  // extern "C"
+
+// ParamNet backward pieces, one host helper of bwd_paramnet each: a temporary engine for the current device, scratch sized by a
+// dry run of the same body and filled with 0xFF bytes (NaN: a read of memory no kernel wrote poisons the result), a sync at the end.
+template <class Body>
+static int pn_op_run(const char* name, int n, void* stream, Body body) {
+  TRY(configure_current_device());
+  pf_engine tmp;
+  CU(cudaGetDevice(&tmp.device));
+  CU(cudaDeviceGetAttribute(&tmp.sm_count, cudaDevAttrMultiProcessorCount, tmp.device));
+  Fwd T{&tmp, Arena{}, nullptr, true, n};
+  T.ar.dry = true;
+  TRY(body(T));
+  const long long bytes = T.ar.peak + 4096;
+  cudaStream_t st = (cudaStream_t)stream;
+  char* scratch = nullptr;
+  CU(cudaMalloc(&scratch, bytes));
+  Fwd F{&tmp, Arena{}, st, false, n};
+  F.ar.base = scratch; F.ar.cap = bytes;
+  const cudaError_t me = cudaMemsetAsync(scratch, 0xFF, bytes, st);
+  int r = me == cudaSuccess ? body(F) : fail(PF_ERR_CUDA, "%s: %s", name, cudaGetErrorString(me));
+  const cudaError_t se = cudaStreamSynchronize(st);
+  cudaFree(scratch);
+  if (r == PF_OK && se != cudaSuccess) r = fail(PF_ERR_CUDA, "%s: %s", name, cudaGetErrorString(se));
+  return r;
+}
+static bool al16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
+extern "C" {
+
+int pf_op_pn_wgrad(const float* dy, int ldy, const float* x, const void* x_hi, const void* x_lo, int op, int ldx, int64_t R, int N, int K, float* out,
+                   int* S, int* chunk, void* stream) {
+  if (!dy || !out || !S || !chunk) return fail(PF_ERR_ARG, "pf_op_pn_wgrad: null argument");
+  if (!x_hi != !x_lo || !x == !x_hi) return fail(PF_ERR_ARG, "pf_op_pn_wgrad: the source is x or the pair x_hi / x_lo");
+  if ((op != 0 && op != 1) || (op == 1 && !x)) return fail(PF_ERR_ARG, "pf_op_pn_wgrad: op %d (1, the GELU, needs the fp32 source)", op);
+  if (R < 1 || R > INT32_MAX || N < 1 || K < 1 || ldy < N || ldx < K) return fail(PF_ERR_ARG, "pf_op_pn_wgrad: R %lld, N %d, K %d, ldy %d, ldx %d", (long long)R, N, K, ldy, ldx);
+  const SplitT xs{(__nv_bfloat16*)x_hi, (__nv_bfloat16*)x_lo, ldx};
+  WgPlan pl{};
+  const int r = pn_op_run("pf_op_pn_wgrad", 1, stream, [&](Fwd& F) { return pn_wgrad_full(F, dy, ldy, x ? nullptr : &xs, x, op, ldx, R, N, K, out, &pl); });
+  *S = pl.S;
+  *chunk = pl.chunk;
+  return r;
+}
+int pf_op_pn_colsum(const float* src, int64_t R, int C, float* out, void* stream) {
+  if (!src || !out || R < 1 || C < 1) return fail(PF_ERR_ARG, "pf_op_pn_colsum: bad argument");
+  return pn_op_run("pf_op_pn_colsum", 1, stream, [&](Fwd& F) { return pn_colsum(F, src, R, C, out); });
+}
+int pf_op_pn_ln_bwd(const float* x, const float* dy, int64_t R, int C, const float* w, float* dx, float* g, void* stream) {
+  if (!x || !dy || !w || !dx || !g) return fail(PF_ERR_ARG, "pf_op_pn_ln_bwd: null argument");
+  if (R < 1 || C < 32 || C > 768 || C % 32) return fail(PF_ERR_ARG, "pf_op_pn_ln_bwd: R %lld, C %d (a multiple of 32 up to 768)", (long long)R, C);
+  return pn_op_run("pf_op_pn_ln_bwd", 1, stream, [&](Fwd& F) { return pn_ln_bwd(F, x, dy, R, C, w, dx, g); });
+}
+int pf_op_pn_dw7_bwd(const float* x, const float* dt, int B, int H, int W, int C, const float* w_rot, float* dw, float* dx, int* rows_per_block, void* stream) {
+  if (!x || !dt || !w_rot || !dw || !dx) return fail(PF_ERR_ARG, "pf_op_pn_dw7_bwd: null argument");
+  if (!al16(x) || !al16(dt) || !al16(w_rot) || !al16(dx)) return fail(PF_ERR_ARG, "pf_op_pn_dw7_bwd: x, dt, w_rot and dx must be 16-byte aligned");
+  if (B < 1 || H < 1 || W < 1 || C < 32 || C % 32 || (long long)B * H * W * C > INT32_MAX)
+    return fail(PF_ERR_ARG, "pf_op_pn_dw7_bwd: B %d, H %d, W %d, C %d (a multiple of 32)", B, H, W, C);
+  return pn_op_run("pf_op_pn_dw7_bwd", B, stream, [&](Fwd& F) {
+    float* zero = F.ar.f(C);
+    if (!F.dry) CU(cudaMemsetAsync(zero, 0, (size_t)C * 4, F.st));
+    TRY(pn_dw7_wgrad(F, x, dt, H, W, C, dw, rows_per_block));
+    return pn_dw_launch(F, dt, dx, H, W, C, w_rot, zero);
+  });
+}
+int pf_op_pn_stem_bwd(const float* pin, const float* dS, const float* w, int B, int OH, int OW, float* dw, float* dpin, int* rows_per_block, void* stream) {
+  if (!pin || !dS || !w || !dw || !dpin) return fail(PF_ERR_ARG, "pf_op_pn_stem_bwd: null argument");
+  if (!al16(pin)) return fail(PF_ERR_ARG, "pf_op_pn_stem_bwd: pin must be 16-byte aligned");
+  if (B < 1 || OH < 1 || OW < 1) return fail(PF_ERR_ARG, "pf_op_pn_stem_bwd: B %d, OH %d, OW %d", B, OH, OW);
+  return pn_op_run("pf_op_pn_stem_bwd", B, stream, [&](Fwd& F) {
+    TRY(pn_stem_wgrad(F, pin, dS, OH, OW, dw, rows_per_block));
+    return pn_stem_dgrad(F, dS, w, OH, OW, dpin);
+  });
+}
+int pf_op_pn_fields_grad(const float* dpin, int B, int IH, int IW, int OH, int OW, float* dgrav, float* dlat, void* stream) {
+  if (!dpin || !dgrav || !dlat) return fail(PF_ERR_ARG, "pf_op_pn_fields_grad: null argument");
+  if (!al16(dpin)) return fail(PF_ERR_ARG, "pf_op_pn_fields_grad: dpin must be 16-byte aligned");
+  if (B < 1 || IH < 1 || IW < 1 || OH < 1 || OW < 1) return fail(PF_ERR_ARG, "pf_op_pn_fields_grad: B %d, %dx%d -> %dx%d", B, IH, IW, OH, OW);
+  return pn_op_run("pf_op_pn_fields_grad", B, stream, [&](Fwd& F) { return pn_fields_grad(F, dpin, IH, IW, OH, OW, dgrav, dlat); });
+}
+int pf_op_pn_tail_bwd(const float* feat, int n, int HW, const float* nw, const float* nb, const float* hw, const float* draw, float* dx, float* grads, void* stream) {
+  if (!feat || !nw || !nb || !hw || !draw || !dx || !grads) return fail(PF_ERR_ARG, "pf_op_pn_tail_bwd: null argument");
+  if (n < 1 || HW < 1) return fail(PF_ERR_ARG, "pf_op_pn_tail_bwd: n %d, HW %d", n, HW);
+  return pn_op_run("pf_op_pn_tail_bwd", n, stream, [&](Fwd& F) { return pn_tail_bwd(F, feat, HW, nw, nb, hw, draw, dx, grads); });
+}
+int pf_op_pn_pw2_grads(const float* G, const float* sdy, int C, int K, const float* gamma, const void* w_hi, const void* w_lo, const float* b, float* dW, float* db,
+                       float* dgamma, void* stream) {
+  if (!G || !sdy || !gamma || !w_hi || !w_lo || !b || !dW || !db || !dgamma) return fail(PF_ERR_ARG, "pf_op_pn_pw2_grads: null argument");
+  if (C < 1 || K < 1) return fail(PF_ERR_ARG, "pf_op_pn_pw2_grads: C %d, K %d", C, K);
+  const GemmW w2{(const __nv_bfloat16*)w_hi, (const __nv_bfloat16*)w_lo, b};
+  return pn_op_run("pf_op_pn_pw2_grads", 1, stream, [&](Fwd& F) { return pn_pw2_grads(F, G, sdy, C, K, gamma, w2, dW, db, dgamma); });
+}
+int pf_op_pn_gelu_bwd(const float* dh, float* u, int64_t n, void* hi, void* lo, void* stream) {
+  if (!dh || !u || n < 1 || !hi != !lo) return fail(PF_ERR_ARG, "pf_op_pn_gelu_bwd: bad argument");
+  return pn_op_run("pf_op_pn_gelu_bwd", 1, stream, [&](Fwd& F) { return pn_gelu_bwd(F, dh, u, n, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo); });
+}
+int pf_op_pn_scale_split(const float* src, const float* scale, int64_t n, int C, void* hi, void* lo, void* stream) {
+  if (!src || !hi || !lo || n < 1 || C < 1 || n % C) return fail(PF_ERR_ARG, "pf_op_pn_scale_split: bad argument");
+  const SplitT out{(__nv_bfloat16*)hi, (__nv_bfloat16*)lo, C};
+  return pn_op_run("pf_op_pn_scale_split", 1, stream, [&](Fwd& F) { return pn_scale_split(F, src, scale, n, C, out); });
+}
+int pf_op_pn_col2im2(const float* dP, int B, int H, int W, int C, float* out, void* stream) {
+  if (!dP || !out || B < 1 || H < 2 || W < 2 || H % 2 || W % 2 || C < 1) return fail(PF_ERR_ARG, "pf_op_pn_col2im2: bad argument");
+  return pn_op_run("pf_op_pn_col2im2", B, stream, [&](Fwd& F) { return pn_col2im2(F, dP, H, W, C, out); });
+}
+
 int pf_op_tma(pf_tma_op* op, void* stream) { return op_tma(op, stream, false); }
 int pf_op_tma_bf16(pf_tma_op* op, void* stream) { return op_tma(op, stream, true); }
 int pf_op_conv1_ring(const void* c_hi, const void* c_lo, int B, int H, int W, const float* wf, const float* bias, float* out,

@@ -58,17 +58,17 @@ def _fields(kind, n, h, w, seed):
     return torch.from_numpy(np.stack(ups).astype(np.float32)), torch.from_numpy(np.stack(lats).astype(np.float32))
 
 
-def _oracle(sd, version, grav, lat, inputs):
-    """float64 autograd on the CPU: (losses, {param key: grad}, (d gravity, d latitude), raw)."""
+def _oracle(sd, version, grav, lat, inputs, device="cpu"):
+    """float64 autograd on `device`: (losses, {param key: grad}, (d gravity, d latitude), raw)."""
     cfg = VARIANTS[version]
-    p = {k: v.double().clone().requires_grad_(True) for k, v in sd.items() if k.startswith("param_net.backbone.")}
-    g = grav.double().clone().requires_grad_(True)
-    la = lat.double().clone().requires_grad_(True)
+    p = {k: v.double().to(device).requires_grad_(True) for k, v in sd.items() if k.startswith("param_net.backbone.")}
+    g = grav.double().to(device).requires_grad_(True)
+    la = lat.double().to(device).requires_grad_(True)
     images = torch.cat((g, la), 1)
     if cfg["param_net"] != "ParamNet":
         images = F.interpolate(images, (cfg["input_size"], cfg["input_size"]))
     raw = om.convnext_t(p, images)
-    gt = torch.from_numpy(metrics.param_targets(inputs, grav.shape[0], cfg["param_net"], cfg["predict_params"])).double()
+    gt = torch.from_numpy(metrics.param_targets(inputs, grav.shape[0], cfg["param_net"], cfg["predict_params"])).double().to(device)
     lw = float(make_cfg(version).MODEL.PARAM_DECODER.LOSS_WEIGHT)
     losses = metrics.param_net_losses(raw, gt, cfg["param_net"], cfg["predict_params"], lw)
     sum(losses.values()).backward()
@@ -85,18 +85,21 @@ def _grads(params):
 
 
 # ------------------------------------------------------------------------------------------------ 1. oracle parity
-CASES = [(v, kind, None) for v in VERSIONS for kind in ("camera", "random")] + [
-    (CENTRED, "camera", (256, 384)), (GSV_UNC, "random", (256, 384))]
+# n = 13 centred pairs at 320 x 320: 1040 stem rows, past the 1024 partials of the depthwise and stem weight-gradient kernels,
+# so their blocks take two image rows each; its float64 oracle runs on the GPU
+CASES = [(v, kind, None, 3) for v in VERSIONS for kind in ("camera", "random")] + [
+    (CENTRED, "camera", (256, 384), 3), (GSV_UNC, "random", (256, 384), 3), (CENTRED, "camera", None, 13)]
+# the ids the cases had before the batch size was a parameter (pytest's own for the first three values), "-n<n>" otherwise
+CASE_IDS = [f"{v}-{k}-{'None' if r is None else f'resize{i}'}" + ("" if n == 3 else f"-n{n}") for i, (v, k, r, n) in enumerate(CASES)]
 
 
-@pytest.mark.parametrize("version,kind,resize", CASES)
-def test_gradients_match_the_oracle(version, kind, resize):
+@pytest.mark.parametrize("version,kind,resize,n", CASES, ids=CASE_IDS)
+def test_gradients_match_the_oracle(version, kind, resize, n):
     m, sd = _model(version, resize=resize)
     h, w = m.net_size()
-    n = 3
     grav, lat = _fields(kind, n, h, w, seed=31)
     inputs = op.targets(n, seed=41)
-    o_losses, o_grads, (o_dg, o_dl), raw, gt = _oracle(sd, version, grav, lat, inputs)
+    o_losses, o_grads, (o_dg, o_dl), raw, gt = _oracle(sd, version, grav, lat, inputs, device="cuda" if n > 3 else "cpu")
     if VARIANTS[version]["param_net"] == "ParamNet":
         # the L1 loss has a kink at raw = gt: every compared entry must be clear of it
         assert (raw - gt)[:, :3].abs().min() > 1e-3
@@ -111,7 +114,7 @@ def test_gradients_match_the_oracle(version, kind, resize):
     assert _normwise(dfields["pred_latitude"], o_dl) <= 1e-3
     if VARIANTS[version]["param_net"] != "ParamNet":
         # the nearest sub-sample reads few pixels: the rest of the field gradient is exactly zero, as in autograd
-        assert torch.equal(dfields["pred_gravity"].cpu() == 0, o_dg == 0)
+        assert torch.equal(dfields["pred_gravity"].cpu() == 0, o_dg.cpu() == 0)
 
 
 # one bf16 product per MMA: worst error measured on an H100 6.9e-3 (DESIGN.md, ParamNet training); bound with a 3x margin
