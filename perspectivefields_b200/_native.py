@@ -6,18 +6,20 @@ compute entry point needs the CUDA library and an H100 (sm_90a).
 import ctypes
 import os
 import subprocess
+from concurrent.futures import ThreadPoolExecutor
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(_HERE)
 LIB_PATH = os.path.join(_HERE, "libpf_b200.so")
 SRC_DIR = os.path.join(_HERE, "csrc")
+OBJ_DIR = os.path.join(_HERE, "build")
 HEADER = os.path.join(ROOT, "include", "pf_b200.h")
 
 PF_F32, PF_BF16 = 0, 1
 PF_PARAM_NONE, PF_PARAM_CENTERED, PF_PARAM_UNCENTERED = 0, 1, 2
 
-NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
-              "-Xcompiler", "-fPIC", "-shared", "-ldl"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
+LINK_FLAGS = ["-shared", "-ldl"]
 
 
 class pf_model_desc(ctypes.Structure):
@@ -116,7 +118,7 @@ class pf_tma_op(ctypes.Structure):
 
 
 def _sources():
-    return sorted(os.path.join(SRC_DIR, f) for f in os.listdir(SRC_DIR) if f.endswith((".cu", ".cuh"))) + [HEADER]
+    return sorted(os.path.join(SRC_DIR, f) for f in os.listdir(SRC_DIR) if f.endswith((".cu", ".cuh", ".h"))) + [HEADER]
 
 
 def needs_build():
@@ -126,20 +128,36 @@ def needs_build():
     return any(os.path.getmtime(s) > t for s in _sources())
 
 
-def build(force=False, verbose=False):
-    """Compile csrc/pf_b200.cu for sm_90a into libpf_b200.so next to this file (nvcc cross-compiles without a GPU)."""
-    if not force and not needs_build():
-        return LIB_PATH
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    cmd = [nvcc] + NVCC_FLAGS + [os.path.join(SRC_DIR, "pf_b200.cu"), "-o", LIB_PATH + ".tmp"]
-    if verbose:
-        cmd.insert(1, "-Xptxas=-v")
+def _stale(obj):
+    """An object is stale when it, or the dependency list nvcc wrote beside it, is missing or older than a file it was built from."""
+    if not (os.path.exists(obj) and os.path.exists(obj + ".d")):
+        return True
+    deps = open(obj + ".d").read().replace("\\\n", " ").split(":", 1)[1].split()
+    t = os.path.getmtime(obj)
+    return any(not os.path.exists(d) or os.path.getmtime(d) > t for d in deps)
+
+
+def _nvcc(args, out, verbose):
+    cmd = [os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")] + args + ["-o", out + ".tmp"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("nvcc failed:\n" + " ".join(cmd) + "\n" + r.stdout + r.stderr)
-    os.replace(LIB_PATH + ".tmp", LIB_PATH)
+    os.replace(out + ".tmp", out)
     if verbose:
         print(r.stderr)
+
+
+def build(force=False, verbose=False):
+    """Compile every csrc/*.cu for sm_90a (nvcc cross-compiles without a GPU), in parallel, into build/, and link them into
+    libpf_b200.so next to this file.  Objects whose sources have not changed since they were built are reused unless force."""
+    if not force and not needs_build():
+        return LIB_PATH
+    os.makedirs(OBJ_DIR, exist_ok=True)
+    objs = {os.path.join(OBJ_DIR, f[:-3] + ".o"): os.path.join(SRC_DIR, f) for f in sorted(os.listdir(SRC_DIR)) if f.endswith(".cu")}
+    flags = NVCC_FLAGS + (["-Xptxas=-v"] if verbose else [])
+    with ThreadPoolExecutor(os.cpu_count()) as pool:
+        list(pool.map(lambda o: _nvcc(flags + ["-MD", "-MF", o + ".d", "-c", objs[o]], o, verbose), [o for o in objs if force or _stale(o)]))
+    _nvcc(LINK_FLAGS + list(objs), LIB_PATH, verbose)
     return LIB_PATH
 
 

@@ -11,6 +11,18 @@ constexpr int kNet = 320;  // network working resolution (every shipped config: 
 __host__ __device__ inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 __host__ __device__ inline long long cdivl(long long a, long long b) { return (a + b - 1) / b; }
 
+// grid of a 256-thread grid-stride launch over `total` items
+inline unsigned ew_grid(long long total) {
+  long long g = cdivl(total, 256);
+  const long long cap = 132LL * 32;
+  return (unsigned)(g < cap ? (g > 0 ? g : 1) : cap);
+}
+
+// Bin widths in degrees of the gravity (NC - 1 angle bins plus the "no direction" bin NC - 1) and latitude classes, shared by
+// the decoders of layers.cuh and the encoders of metrics.cuh (utils/utils.py:94-162).
+__host__ __device__ __forceinline__ float gravity_bin_deg(int NC) { return 360.0f / (float)(NC - 1); }
+__host__ __device__ __forceinline__ float latitude_bin_deg(int NC) { return 180.0f / (float)NC; }
+
 // ---------------------------------------------------------------- programmatic dependent launch (PDL)
 // The forward graph is ~450 dependent launches of 10-60 us kernels.  Kernels launched with
 // cudaLaunchAttributeProgrammaticStreamSerialization may begin (block scheduling, prologue: barrier init,

@@ -28,38 +28,12 @@
 #include <cuda.h>
 
 #include "tc_ptx.cuh"
+#include "tma_host.cuh"
 
 namespace pf {
 
-constexpr int MODE_GEMM = 0, MODE_HALO = 1;
 constexpr int kTmaThreads = 384;   // warpgroup 0: producers;  warpgroups 1-2: MMA + epilogue
 constexpr int kHaloBytes = 180 * 128;   // one bf16 plane of an 18 x 10 pixel x 64 channel halo (what one TMA box delivers)
-
-struct TmaGemmParams {
-  int M;                    // MODE_GEMM: rows
-  int B, H, W;              // MODE_HALO: images, spatial size (output == input)
-  int Cin;                  // MODE_HALO: input channels per group (multiple of 64);  MODE_GEMM: K
-  int N, K;
-  int a_c0, a_gc;           // channel coordinate of the first input channel in A's tensor map, step per group
-  int c_split, a2_c0;       // MODE_HALO dual source: input channels >= c_split come from the A2 maps at a2_c0 + (ci - c_split); 0 = off
-  int groups;
-  int b_row0;               // first row of this launch's weights in the B tensor map (resident-weight launches fold the group in)
-  // epilogue:  v = acc + bias;  v = act(v);  v *= gamma;  v += relu?(res);  v += res2
-  const float* bias; int bias_mode, bias_gstride;
-  int act; const float* gamma;
-  const float* res;  int ldr, r_coff, r_gcoff, res_relu;
-  const float* res2; int ldr2, r2_coff, r2_gcoff;
-  float* C; int ldc, c_coff, c_gcoff;                                           // fp32 output (may be null)
-  __nv_bfloat16* Shi; __nv_bfloat16* Slo; int lds, s_coff, s_gcoff, split_relu; // split output (may be null)
-  // MODE_HALO, N = 32 (conv_fuse_conv1): fused prediction tail -- 1x1 conv 32 -> pred_nc (gravity_head.py:175 /
-  // latitude_head.py:174) + F.normalize (pred_mode 1, gravity_head.py:192-193) or clamp to [-1,1] (pred_mode 2,
-  // latitude_head.py:191-192), written NCHW to pred_out; replaces the separate pred_tail_kernel pass over conv1's output
-  const float* pred_w; const float* pred_b; float* pred_out; int pred_nc, pred_mode;
-  // MODE_HALO, N = BN = 128: the four 32-column chunks are the four output phases (py, px) of a convolution composed with the
-  // bilinear x2 upsample in front of it (weights.py:_compose_up2_conv3): chunk ph, low-res pixel (y, x) -> pixel
-  // (2y + ph/2, 2x + ph%2) of the 2H x 2W output, 32 channels.  C / S / the prediction tail are addressed on that grid.
-  int phase4;
-};
 
 // KB = K elements per pipeline step: 32 (64 B rows, SWIZZLE_64B) for wide tiles, 64 (128 B rows, SWIZZLE_128B) for narrow ones
 // where a 32-wide step would be shorter than the barrier round trip that feeds it.
@@ -103,10 +77,6 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];\n" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
-
-struct TmaMaps {   // passed by value as a __grid_constant__ kernel parameter
-  CUtensorMap a_hi, a_lo, a2_hi, a2_lo, b_hi, b_lo;
-};
 
 template <int BN, int MODE, int KB, bool PP = false, int NP = 3>
 __global__ void __launch_bounds__(kTmaThreads, 1) gemm_tma_kernel(const __grid_constant__ TmaMaps maps, const TmaGemmParams p, int tiles_x, int tiles_y) {

@@ -370,12 +370,6 @@ __global__ void __launch_bounds__(256, PF_DW7_MINBLOCKS) dwconv7x7_kernel(const 
   }
 }
 
-inline unsigned ew_grid(long long total) {
-  long long g = cdivl(total, 256);
-  const long long cap = 132LL * 32;
-  return (unsigned)(g < cap ? (g > 0 ? g : 1) : cap);
-}
-
 // =====================================================================================================
 // Bilinear x2 upsample, align_corners=False (decode_head.py:284-286, gravity_head.py:172): taps {0.25, 0.75},
 // edges clamped.  ATen: src = 0.5*(dst+0.5)-0.5 clamped at 0, i1 = min(i0+1, in-1).  NHWC, float4 per thread.
@@ -679,11 +673,6 @@ __global__ void __launch_bounds__(256) conv1_ring_kernel(const __nv_bfloat16* __
   }
 }
 constexpr int kRingSmem = (128 * kRingPx + 2 * 64 * 32) * 4;
-
-// Bin widths in degrees of the gravity (NC - 1 angle bins plus the "no direction" bin NC - 1) and latitude classes, shared by
-// the decoders below and the encoders of metrics.cuh (utils/utils.py:94-162).
-__host__ __device__ __forceinline__ float gravity_bin_deg(int NC) { return 360.0f / (float)(NC - 1); }
-__host__ __device__ __forceinline__ float latitude_bin_deg(int NC) { return 180.0f / (float)NC; }
 
 // Bin decode shared by the two classification kernels (utils/utils.py:114-130 and :148-162).
 __device__ __forceinline__ void decode_bin_store(float* __restrict__ field, int b, int r, int HW, int NC, int bi, int is_gravity) {

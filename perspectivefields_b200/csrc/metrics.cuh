@@ -7,7 +7,6 @@
 #include <stdint.h>
 
 #include "common.cuh"
-#include "layers.cuh"
 
 namespace pf {
 

@@ -1,47 +1,25 @@
 // libpf_b200.so -- C ABI (include/pf_b200.h) and forward orchestration of the H100-native (sm_90a) PerspectiveFields
 // inference engine.  One engine per device; pf_forward enqueues the whole graph of
 // perspective2d/perspectivefields.py:223-272 on the caller's stream.
-#include "../../include/pf_b200.h"
-
-#include <cuda_runtime.h>
-#include <nvtx3/nvToolsExt.h>
-
-#include <atomic>
 #include <cctype>
 #include <cmath>
-#include <cstdarg>
-#include <cstdio>
-#include <cstdlib>
 #include <cstring>
-#include <map>
 #include <mutex>
-#include <string>
-#include <functional>
-#include <unordered_map>
-#include <vector>
 
-#include "common.cuh"
-#include "tma_host.cuh"
+#include "engine.h"
 #include "attention_mma.cuh"
 #include "layers.cuh"
 #include "prepost.cuh"
-#include "pano.cuh"
-#include "equi.cuh"
-#include "draw.cuh"
-#include "metrics.cuh"
-#include "calib.cuh"
-#include "rectify.cuh"
-#include "comm.cuh"
-#include "jpeg.cuh"
-#include "paramnet_train.cuh"
 
-using namespace pf;
+// ----------------------------------------------------------------------------------------------- shared state (host.h)
+namespace pf {
 
-// ----------------------------------------------------------------------------------------------- errors
 static thread_local std::string g_err;
-static std::atomic<long long> g_launches{0};
+std::atomic<long long> g_launches{0};
+char g_crumb[96] = "";
+thread_local KernelProf* tl_kp = nullptr;
 
-static int fail(int code, const char* fmt, ...) {
+int fail(int code, const char* fmt, ...) {
   char buf[1024];
   va_list ap;
   va_start(ap, fmt);
@@ -50,153 +28,32 @@ static int fail(int code, const char* fmt, ...) {
   g_err = buf;
   return code;
 }
-#define CU(expr)                                                                                    \
-  do {                                                                                              \
-    cudaError_t e__ = (expr);                                                                       \
-    if (e__ != cudaSuccess) return fail(PF_ERR_CUDA, "%s: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-  } while (0)
-// PF_SYNC_DEBUG=1 in the environment: synchronise after every launch so that a device fault is reported at the launch that
-// caused it (debugging aid; never set in production)
-static char g_crumb[96] = "";   // name of the last debug tap taken (breadcrumb for the error text)
-static bool sync_debug() {
-  static int v = -1;
-  if (v < 0) v = getenv("PF_SYNC_DEBUG") ? 1 : 0;
-  return v == 1;
+
+int configure_device(int device) {
+  static std::mutex mu;
+  static std::vector<char> done;
+  std::lock_guard<std::mutex> lock(mu);
+  if (device < (int)done.size() && done[device]) return PF_OK;
+  CU(gemm_tma_configure_device(3));
+  CU(gemm_tma_configure_device(1));
+  CU(attention_mma_configure_device());
+  CU(cudaFuncSetAttribute(conv1_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kRingSmem));
+  CU(cudaFuncSetAttribute(preprocess_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPreSmemBytes));
+  CU(cudaFuncSetAttribute(postprocess_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPostSmemMax));
+  if (device >= (int)done.size()) done.resize(device + 1, 0);
+  done[device] = 1;
+  return PF_OK;
 }
-// pf_profile_kernels_*: a CUDA-event pair around EVERY launch of the forward graph (in-pipeline time per kernel, bench.py's
-// "per_kernel" table).  Off by default: the event records cost a few percent, so bench.py uses a separate pass for it.
-// The state lives in the engine; the launch macro reaches it through a thread-local pointer that pf_forward sets for the
-// duration of the call (operator entry points run with it unset).
-struct KernelProf {
-  bool on = false;
-  cudaStream_t st = nullptr;
-  std::vector<cudaEvent_t> pool;
-  size_t used = 0;
-  struct Rec { const char* expr; cudaEvent_t a, b; };
-  std::vector<Rec> recs;
-  cudaEvent_t next() { return used < pool.size() ? pool[used++] : nullptr; }
-};
-static thread_local KernelProf* tl_kp = nullptr;
-#define LAUNCHED(expr)                                                                              \
-  do {                                                                                              \
-    KernelProf* kp__ = tl_kp;                                                                       \
-    cudaEvent_t ka__ = (kp__ && kp__->on) ? kp__->next() : nullptr;                                 \
-    if (ka__) cudaEventRecord(ka__, kp__->st);                                                      \
-    cudaError_t e__ = (expr);                                                                       \
-    g_launches.fetch_add(1, std::memory_order_relaxed);                                             \
-    if (ka__) {                                                                                     \
-      cudaEvent_t kb__ = kp__->next();                                                              \
-      if (kb__) { cudaEventRecord(kb__, kp__->st); kp__->recs.push_back({#expr, ka__, kb__}); }     \
-    }                                                                                               \
-    if (e__ == cudaSuccess && sync_debug()) e__ = cudaDeviceSynchronize();                          \
-    if (e__ != cudaSuccess) return fail(PF_ERR_CUDA, "%s: %s (%s:%d, after tap '%s')", #expr, cudaGetErrorString(e__), __FILE__, __LINE__, g_crumb); \
-  } while (0)
-// NVTX range per section of the forward graph (visible in Nsight Systems / ncu --nvtx; a few ns when no tool is attached)
-struct NvtxRange {
-  explicit NvtxRange(const char* name) { nvtxRangePushA(name); }
-  ~NvtxRange() { nvtxRangePop(); }
-};
-#define TRY(expr)                \
-  do {                           \
-    int r__ = (expr);            \
-    if (r__ != PF_OK) return r__; \
-  } while (0)
+int configure_current_device() {
+  int dev = 0;
+  CU(cudaGetDevice(&dev));
+  return configure_device(dev);
+}
 
-// ----------------------------------------------------------------------------------------------- model constants
-static const int kMitDims[4] = {64, 128, 320, 512};
-static const int kMitHeads[4] = {1, 2, 5, 8};
-static const int kMitDepths[4] = {3, 4, 18, 3};
-static const int kMitSr[4] = {8, 4, 2, 1};
-static const int kCnxDims[4] = {96, 192, 384, 768};
-static const int kCnxDepths[4] = {3, 3, 9, 3};
-
-struct WeightRef { const void* p; long long numel; int dtype; };
-struct GemmW { const __nv_bfloat16* hi = nullptr; const __nv_bfloat16* lo = nullptr; const float* b = nullptr; };
-struct LnW { const float* w = nullptr; const float* b = nullptr; };
-
-struct MitBlockW { LnW ln1, srln, ln2; GemmW q, sr, kv, proj, fc1, fc2; const float* dw_w; const float* dw_b; };
-struct CnxBlockW { const float* dw_w; const float* dw_b; LnW ln; GemmW pw1, pw2; const float* gamma; };
-
-struct Arena {
-  char* base = nullptr;
-  long long cap = 0, off = 0, peak = 0;
-  bool dry = false, keep = false;  // keep: debug mode, never recycle
-  void* alloc(long long bytes) {
-    off = (off + 255) & ~255LL;
-    void* p = dry ? nullptr : base + off;
-    off += bytes;
-    if (off > peak) peak = off;
-    return p;
-  }
-  float* f(long long n) { return (float*)alloc(n * 4); }
-  long long mark() const { return off; }
-  void release(long long m) { if (!keep) off = m; }
-};
-
-struct pf_engine {
-  int device = 0;
-  pf_model_desc desc{};
-  int net_h = kNet, net_w = kNet;     // working size (DATALOADER.RESIZE = [net_h, net_w]): multiples of 32 in [64, 640] (pf_create_sized)
-  bool finalized = false;
-  std::unordered_map<std::string, WeightRef> weights;
-  // resolved weights
-  LnW embed_ln[4], stage_norm[4];
-  GemmW embed[4];  // [1..3] used
-  GemmW embed1g, llencg;  // 7x7 stems as [64][160] GEMMs
-  std::vector<MitBlockW> blocks[4];
-  GemmW proc[4];   // composed linear_c{l} o linear_c{l}_proc, both heads side by side (N = 512), index lvl-1
-  GemmW rcu[4][2][2];  // [fusion-1][unit-1][conv-1], grouped over the two heads
-  GemmW conv0;
-  GemmW conv1p;                       // conv_fuse_conv1 composed with the x2 upsample in front of it: 4 phases x 32 outputs per head
-  const float *conv1f_w, *conv1f_b;   // plain fp32 conv_fuse_conv1 [head][tap][ci][o] / bias, for the border-ring kernel
-  bool use_pdl = true;                // option "pdl": programmatic dependent launch of the graph's kernels (common.cuh)
-  bool decode_only = false;           // option "decode_only": classification heads return decoded fields, logits are never written
-  const float *pred_g_w, *pred_g_b, *pred_l_w, *pred_l_b;
-  const float *pn_stem_w, *pn_stem_b;
-  LnW pn_stem_ln, pn_ds_ln[4], pn_norm;
-  GemmW pn_ds[4];
-  std::vector<CnxBlockW> pn_blocks[4];
-  const float *pn_head_w, *pn_head_b;
-  // ParamNet training only (pf_param_backward, resolved there): transposed split copies of the GEMM weights for the data
-  // gradients, the depthwise kernels rotated by 180 degrees and a zero bias for the depthwise data gradient
-  struct PnTrainW { GemmW ds_t[4]; std::vector<GemmW> pw1_t[4], pw2_t[4]; std::vector<const float*> dw_rot[4]; const float* zero = nullptr; } pn_train;
-  // Pillow resample tables, cached per (input size, output size) in one device slab owned by the engine (bump allocation; built on the host
-  // into a pinned mirror of the slab and copied with cudaMemcpyAsync on the caller's stream: no allocation and no
-  // synchronising copy inside pf_forward)
-  struct DevTable { int ksize; int* bounds; int* coeffs; };
-  std::map<std::pair<int, int>, DevTable> tables;
-  char* table_dev = nullptr;
-  char* table_host = nullptr;       // pinned
-  long long table_off = 0;
-  KernelProf kp;                    // pf_profile_kernels_*
-  // per-launch profiling of the GEMM engine (bench.py roofline leg): CUDA events on the launch stream
-  // tensor maps are pure functions of (pointer, shape, box): cached across calls (the arena hands out the same addresses for the
-  // same batch size), which takes cuTensorMapEncodeTiled (~5 us each, ~1800 per forward) off the launch path
-  struct MapKey {
-    const void* base; long long d0, d1, d2; int kind, box, kb;
-    bool operator==(const MapKey& o) const { return base == o.base && d0 == o.d0 && d1 == o.d1 && d2 == o.d2 && kind == o.kind && box == o.box && kb == o.kb; }
-  };
-  struct MapKeyHash {
-    size_t operator()(const MapKey& k) const {
-      size_t h = std::hash<const void*>()(k.base);
-      for (long long v : {k.d0, k.d1, k.d2, (long long)k.kind, (long long)k.box, (long long)k.kb}) h = h * 1000003u ^ std::hash<long long>()(v);
-      return h;
-    }
-  };
-  std::unordered_map<MapKey, CUtensorMap, MapKeyHash> map_cache;
-  bool bf16 = false;          // option "bf16": every tensor-core product is one bf16 MMA (hi * hi) instead of three; read per launch
-  int sm_count = 132;
-  bool profile = false;
-  struct ProfRec { cudaEvent_t a, b; double flops; int cfg; int M, N, K, KH, stride, groups, Cin; };
-  std::vector<ProfRec> prof;
-  std::vector<cudaEvent_t> ev_pool;   // events are created once and recycled: no create/destroy inside a timed region
-  // debug taps
-  bool debug = false;
-  std::vector<std::pair<std::string, std::pair<const float*, long long>>> taps;
-};
+}  // namespace pf
 
 // ----------------------------------------------------------------------------------------------- weight lookup
-static int get_w(pf_engine* e, const std::string& name, int dtype, long long numel, const void** out) {
+int get_w(pf_engine* e, const std::string& name, int dtype, long long numel, const void** out) {
   auto it = e->weights.find(name);
   if (it == e->weights.end()) return fail(PF_ERR_WEIGHT, "missing weight '%s'", name.c_str());
   if (it->second.dtype != dtype) return fail(PF_ERR_WEIGHT, "weight '%s': wrong dtype", name.c_str());
@@ -204,7 +61,7 @@ static int get_w(pf_engine* e, const std::string& name, int dtype, long long num
   *out = it->second.p;
   return PF_OK;
 }
-static int get_f(pf_engine* e, const std::string& n, long long numel, const float** out) { return get_w(e, n, PF_F32, numel, (const void**)out); }
+int get_f(pf_engine* e, const std::string& n, long long numel, const float** out) { return get_w(e, n, PF_F32, numel, (const void**)out); }
 static int get_gemm(pf_engine* e, const std::string& n, long long N, long long K, long long nbias, GemmW* g, int groups = 1) {
   TRY(get_w(e, n + ".whi", PF_BF16, groups * N * K, (const void**)&g->hi));
   TRY(get_w(e, n + ".wlo", PF_BF16, groups * N * K, (const void**)&g->lo));
@@ -308,215 +165,45 @@ static int resolve_weights(pf_engine* e) {
   return PF_OK;
 }
 
-// ----------------------------------------------------------------------------------------------- op helpers
-struct Fwd {
-  pf_engine* e;
-  Arena ar;
-  cudaStream_t st;
-  bool dry;
-  int n;
-
-  // debug taps: snapshot the tensor into a private buffer (many intermediates are updated in place later)
-  int tap(const char* name, const float* p, long long numel) {
-    if (!e->debug) return PF_OK;
-    float* cp = ar.f(numel);
-    if (dry) return PF_OK;
-    snprintf(g_crumb, sizeof g_crumb, "%s", name);
-    if (sync_debug()) fprintf(stderr, "[pf tap] %s cp=%p (+%lld of cap %lld) p=%p numel=%lld\n", name, (void*)cp, (long long)((char*)cp - ar.base), ar.cap, (const void*)p, numel);
-    CU(cudaMemcpyAsync(cp, p, numel * 4, cudaMemcpyDeviceToDevice, st));
-    if (sync_debug()) CU(cudaDeviceSynchronize());
-    e->taps.push_back({name, {cp, numel}});
-    return PF_OK;
+// ----------------------------------------------------------------------------------------------- Fwd members that launch graph kernels
+int Fwd::tap_split(const char* name, const SplitT& t, long long numel) {
+  if (!e->debug) return PF_OK;
+  float* cp = ar.f(numel);
+  if (dry) return PF_OK;
+  snprintf(g_crumb, sizeof g_crumb, "%s", name);
+  LAUNCHED((merge_split_kernel<<<(unsigned)cdivl(numel, 256), 256, 0, st>>>(t.hi, t.lo, cp, numel), cudaGetLastError()));
+  e->taps.push_back({name, {cp, numel}});
+  return PF_OK;
+}
+int Fwd::tconv_gather(const SplitT& A, int B, int H, int W, int Cin, int KH, int stride, int pad, const GemmW& w, int N, const Epi& o) {
+  const int OH = (H + 2 * pad - KH) / stride + 1, OW = (W + 2 * pad - KH) / stride + 1;
+  const long long M = (long long)B * OH * OW;
+  const int K = KH * KH * Cin;
+  const long long m = ar.mark();
+  SplitT col = salloc(M, K);
+  if (!dry) {
+    if (Cin % 8) return fail(PF_ERR_ARG, "tconv_gather: Cin %% 8");
+    LAUNCHED(launch_pdl(im2col_split_kernel, dim3(ew_grid(M * K / 8)), dim3(256), 0, st, A.hi, A.lo, A.ld, col.hi, col.lo, B, H, W, Cin, OH, OW, KH, stride, pad));
   }
-  int tapf(const float* p, long long numel, const char* fmt, ...) {
-    if (!e->debug) return PF_OK;
-    char buf[96];
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(buf, sizeof buf, fmt, ap);
-    va_end(ap);
-    return tap(buf, p, numel);
-  }
-
-  // ------------------------------------------------------------------------------------------ TMA engine helpers
-  SplitT salloc(long long pixels, int ld) {
-    SplitT t;
-    t.hi = (__nv_bfloat16*)ar.alloc(pixels * ld * 2);
-    t.lo = (__nv_bfloat16*)ar.alloc(pixels * ld * 2);
-    t.ld = ld;
-    return t;
-  }
-  int tap_split(const char* name, const SplitT& t, long long numel) {
-    if (!e->debug) return PF_OK;
-    float* cp = ar.f(numel);
-    if (dry) return PF_OK;
-    snprintf(g_crumb, sizeof g_crumb, "%s", name);
-    LAUNCHED((merge_split_kernel<<<(unsigned)cdivl(numel, 256), 256, 0, st>>>(t.hi, t.lo, cp, numel), cudaGetLastError()));
-    e->taps.push_back({name, {cp, numel}});
-    return PF_OK;
-  }
-  // (two names so that the per-kernel profile separates the GEMM-mode and halo-mode launches)
-  static cudaError_t gemm_tma_gemm_mode(const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, bool pp, int np, int sms, cudaStream_t st, const PredTail* pred) {
-    return gemm_tma_launch(MODE_GEMM, maps, p, bn, kb, pp, np, sms, st, pred);
-  }
-  static cudaError_t gemm_tma_halo_mode(const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, bool pp, int np, int sms, cudaStream_t st, const PredTail* pred) {
-    return gemm_tma_launch(MODE_HALO, maps, p, bn, kb, pp, np, sms, st, pred);
-  }
-  // bf16 products per output of the tensor-core launches: 3 (split precision) or 1 (option "bf16")
-  int np() const { return e->bf16 ? 1 : 3; }
-  int force_bn = 0, force_kb = 0;     // pf_op_tma: tile override (0 = the dispatcher's choice)
-  int force_sched = 0;                // pf_op_tma: GEMM-mode schedule override (0 = the dispatcher's choice, 1 cooperative, 2 ping-pong)
-  int picked_bn = 0, picked_kb = 0, picked_sched = 0;   // (bn, kb, schedule) of the last TMA launch
-  // the one place a launch's (bn, kb) and schedule are chosen: tgemm / thalo build the A and B maps with them and hand them to
-  // launch_tma.  pp: the ping-pong schedule (GEMM mode only).
-  int pick_tile(int mode, const TmaGemmParams& p, const PredTail* pred, int& bn, int& kb, bool& pp) {
-    tma_pick_tile(mode, p.M, p.N, p.K, e->sm_count, bn, kb);
-    if (force_bn) { bn = force_bn; kb = tma_pick_kb(bn, p.K, mode); }
-    if (force_kb) kb = force_kb;
-    pp = mode == MODE_GEMM && (force_sched ? force_sched == 2 : tma_pick_pingpong(p.M, p.N, p.K, bn, e->sm_count));
-    if (const char* msg = gemm_tma_check(mode, p, bn, kb, pred != nullptr, pp, np())) return fail(PF_ERR_ARG, "TMA engine, %s (bn %d, kb %d): %s", mode == MODE_GEMM ? "GEMM mode" : "halo mode", bn, kb, msg);
-    picked_bn = bn; picked_kb = kb; picked_sched = mode == MODE_GEMM ? (pp ? 2 : 1) : 0;
-    return PF_OK;
-  }
-  int launch_tma(int mode, const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, bool pp, const PredTail* pred = nullptr) {
-    if (e->profile) {
-      pf_engine::ProfRec r{};
-      for (cudaEvent_t* ev : {&r.a, &r.b}) {
-        if (e->ev_pool.empty()) { CU(cudaEventCreate(ev)); }
-        else { *ev = e->ev_pool.back(); e->ev_pool.pop_back(); }
-      }
-      const double Mrows = mode == MODE_GEMM ? (double)p.M : (double)p.B * p.H * p.W;
-      r.flops = 2.0 * Mrows * (double)p.N * (double)p.K * (double)p.groups;
-      r.cfg = mode == MODE_GEMM ? 5 : 6;
-      r.M = (int)Mrows; r.N = p.N; r.K = p.K; r.KH = mode == MODE_GEMM ? 1 : 3; r.stride = 1; r.groups = p.groups; r.Cin = p.Cin;
-      CU(cudaEventRecord(r.a, st));
-      if (mode == MODE_GEMM) LAUNCHED(gemm_tma_gemm_mode(maps, p, bn, kb, pp, np(), e->sm_count, st, pred));
-      else LAUNCHED(gemm_tma_halo_mode(maps, p, bn, kb, pp, np(), e->sm_count, st, pred));
-      CU(cudaEventRecord(r.b, st));
-      e->prof.push_back(r);
-      return PF_OK;
-    }
-    if (mode == MODE_GEMM) LAUNCHED(gemm_tma_gemm_mode(maps, p, bn, kb, pp, np(), e->sm_count, st, pred));
-    else LAUNCHED(gemm_tma_halo_mode(maps, p, bn, kb, pp, np(), e->sm_count, st, pred));
-    return PF_OK;
-  }
-  struct Epi {   // epilogue options of one TMA GEMM / conv
-    float* C = nullptr; int ldc = 0, c_coff = 0, c_gcoff = 0;
-    SplitT S; int s_coff = 0, s_gcoff = 0, split_relu = 0;
-    int act = 0; const float* gamma = nullptr;
-    const float* res = nullptr; int ldr = 0, r_coff = 0, r_gcoff = 0, res_relu = 0;
-    const float* res2 = nullptr; int ldr2 = 0, r2_coff = 0, r2_gcoff = 0;
-    int bias_mode = 1;
-    int phase4 = 0;   // halo mode, N = 128: columns are 4 output phases x 32 channels of a 2H x 2W output (TmaGemmParams::phase4)
-  };
-  static void fill_epi(TmaGemmParams& p, const GemmW& w, const Epi& o, int bias_gstride) {
-    p.bias = w.b; p.bias_mode = w.b ? o.bias_mode : 0; p.bias_gstride = bias_gstride;
-    p.act = o.act; p.gamma = o.gamma;
-    p.res = o.res; p.ldr = o.ldr; p.r_coff = o.r_coff; p.r_gcoff = o.r_gcoff; p.res_relu = o.res_relu;
-    p.res2 = o.res2; p.ldr2 = o.ldr2; p.r2_coff = o.r2_coff; p.r2_gcoff = o.r2_gcoff;
-    p.C = o.C; p.ldc = o.ldc; p.c_coff = o.c_coff; p.c_gcoff = o.c_gcoff;
-    p.Shi = o.S.hi; p.Slo = o.S.lo; p.lds = o.S.ld; p.s_coff = o.s_coff; p.s_gcoff = o.s_gcoff; p.split_relu = o.split_relu;
-    p.phase4 = o.phase4;
-  }
-  // cached tensor-map constructors
-  template <class F>
-  const char* cached_map(CUtensorMap* out, const pf_engine::MapKey& key, F&& make) {
-    auto it = e->map_cache.find(key);
-    if (it != e->map_cache.end()) { *out = it->second; return nullptr; }
-    const char* msg = make(out);
-    if (!msg) {
-      if (e->map_cache.size() > 20000) e->map_cache.clear();
-      e->map_cache.emplace(key, *out);
-    }
-    return msg;
-  }
-  const char* map2d(CUtensorMap* m, const void* base, long long cols, long long rows, long long ld, int box_rows, int kb) {
-    return cached_map(m, pf_engine::MapKey{base, cols, rows, ld, 0, box_rows, kb}, [&](CUtensorMap* o) { return tma_map_2d(o, base, cols, rows, ld, box_rows, kb); });
-  }
-  const char* map_halo(CUtensorMap* m, const void* base, int B, int H, int W, int ld) {
-    return cached_map(m, pf_engine::MapKey{base, ((long long)B << 32) | (unsigned)H, W, ld, 3, 0, 0}, [&](CUtensorMap* o) { return tma_map_halo(o, base, B, H, W, ld); });
-  }
-  // C[M, N] = A[M, K] W^T : A = split planes with row pitch A.ld, first channel a_c0
-  int tgemm(const SplitT& A, long long M, int K, int a_c0, const GemmW& w, int N, const Epi& o) {
-    if (dry) return PF_OK;
-    if (K % 32 || N % 32 || A.ld % 8) return fail(PF_ERR_ARG, "tgemm: K/N must be multiples of 32");
-    if (o.res2 || o.bias_mode == 2) return fail(PF_ERR_ARG, "tgemm: second residual / border-class bias are halo-mode features");
-    TmaGemmParams p{};
-    p.M = (int)M; p.Cin = K; p.N = N; p.K = K; p.a_c0 = a_c0; p.groups = 1;
-    fill_epi(p, w, o, 0);
-    TmaMaps maps{};
-    int bn, kb;
-    bool pp;
-    TRY(pick_tile(MODE_GEMM, p, nullptr, bn, kb, pp));
-    const char* msg = nullptr;
-    const int a_rows = pp ? 64 : 128;     // A box = one tile's rows
-    if (!msg) msg = map2d(&maps.a_hi, A.hi, A.ld, M, A.ld, a_rows, kb);
-    if (!msg) msg = map2d(&maps.a_lo, A.lo, A.ld, M, A.ld, a_rows, kb);
-    if (!msg) msg = map2d(&maps.b_hi, w.hi, K, N, K, bn, kb);
-    if (!msg) msg = map2d(&maps.b_lo, w.lo, K, N, K, bn, kb);
-    if (msg) return fail(PF_ERR_CUDA, "%s", msg);
-    maps.a2_hi = maps.a_hi; maps.a2_lo = maps.a_lo;
-    return launch_tma(MODE_GEMM, maps, p, bn, kb, pp);
-  }
-  // 3x3 / stride 1 / pad 1 convolution on split NHWC planes (optionally a second source for channels >= c_split)
-  int thalo(const SplitT& A, int a_c0, int a_gc, const SplitT* A2, int c_split, int a2_c0, int B, int H, int W, int Cin, const GemmW& w, int N,
-            int groups, int bias_gstride, const Epi& o, const PredTail* pred = nullptr) {
-    if (dry) return PF_OK;
-    if (Cin % 64 || N % 32 || (A2 && c_split % 64)) return fail(PF_ERR_ARG, "thalo: Cin must be a multiple of 64, N of 32");
-    // the nine border classes (weights.py:_compose_proc) assume a pixel is never both the first and the last of a row / column
-    if (w.b && o.bias_mode == 2 && (H < 2 || W < 2)) return fail(PF_ERR_ARG, "thalo: border-class bias needs H, W >= 2 (got %dx%d)", H, W);
-    TmaGemmParams p{};
-    p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.N = N; p.K = 9 * Cin; p.a_c0 = a_c0; p.a_gc = a_gc; p.groups = groups;
-    p.c_split = A2 ? c_split : 0; p.a2_c0 = a2_c0;
-    fill_epi(p, w, o, bias_gstride);
-    TmaMaps maps{};
-    int bn, kb;
-    bool pp;
-    TRY(pick_tile(MODE_HALO, p, pred, bn, kb, pp));
-    const char* msg = nullptr;
-    if (!msg) msg = map_halo(&maps.a_hi, A.hi, B, H, W, A.ld);
-    if (!msg) msg = map_halo(&maps.a_lo, A.lo, B, H, W, A.ld);
-    if (A2) {
-      if (!msg) msg = map_halo(&maps.a2_hi, A2->hi, B, H, W, A2->ld);
-      if (!msg) msg = map_halo(&maps.a2_lo, A2->lo, B, H, W, A2->ld);
-    } else { maps.a2_hi = maps.a_hi; maps.a2_lo = maps.a_lo; }
-    if (!msg) msg = map2d(&maps.b_hi, w.hi, p.K, (long long)groups * N, p.K, bn, kb);
-    if (!msg) msg = map2d(&maps.b_lo, w.lo, p.K, (long long)groups * N, p.K, bn, kb);
-    if (msg) return fail(PF_ERR_CUDA, "%s", msg);
-    return launch_tma(MODE_HALO, maps, p, bn, kb, pp, pred);
-  }
-  // strided / patchifying convolution = patch gather on split planes + TMA GEMM
-  int tconv_gather(const SplitT& A, int B, int H, int W, int Cin, int KH, int stride, int pad, const GemmW& w, int N, const Epi& o) {
-    const int OH = (H + 2 * pad - KH) / stride + 1, OW = (W + 2 * pad - KH) / stride + 1;
-    const long long M = (long long)B * OH * OW;
-    const int K = KH * KH * Cin;
-    const long long m = ar.mark();
-    SplitT col = salloc(M, K);
-    if (!dry) {
-      if (Cin % 8) return fail(PF_ERR_ARG, "tconv_gather: Cin %% 8");
-      LAUNCHED(launch_pdl(im2col_split_kernel, dim3(ew_grid(M * K / 8)), dim3(256), 0, st, A.hi, A.lo, A.ld, col.hi, col.lo, B, H, W, Cin, OH, OW, KH, stride, pad));
-    }
-    int r = tgemm(col, M, K, 0, w, N, o);
-    ar.release(m);
-    return r;
-  }
-  int ln_split(const float* x, const SplitT& y, long long rows, int C, const LnW& w, float eps, float* yf = nullptr) {
-    if (dry) return PF_OK;
-    LAUNCHED(layernorm_launch(x, yf, rows, C, w.w, w.b, eps, st, y));
-    return PF_OK;
-  }
-  // LayerNorm whose output is (also) written in patch order for a k = s = sr convolution on the RH x RW map (y may be empty)
-  int ln_split_patch(const float* x, const SplitT& y, const SplitT& patch, long long rows, int C, const LnW& w, float eps, int RH, int RW, int sr) {
-    if (dry) return PF_OK;
-    LAUNCHED(layernorm_launch(x, nullptr, rows, C, w.w, w.b, eps, st, y, patch, RH, RW, sr));
-    return PF_OK;
-  }
-  int ln(const float* x, float* y, long long rows, int C, const LnW& w, float eps) {
-    if (dry) return PF_OK;
-    LAUNCHED(layernorm_launch(x, y, rows, C, w.w, w.b, eps, st));
-    return PF_OK;
-  }
-};
+  int r = tgemm(col, M, K, 0, w, N, o);
+  ar.release(m);
+  return r;
+}
+int Fwd::ln_split(const float* x, const SplitT& y, long long rows, int C, const LnW& w, float eps, float* yf) {
+  if (dry) return PF_OK;
+  LAUNCHED(layernorm_launch(x, yf, rows, C, w.w, w.b, eps, st, y));
+  return PF_OK;
+}
+int Fwd::ln_split_patch(const float* x, const SplitT& y, const SplitT& patch, long long rows, int C, const LnW& w, float eps, int RH, int RW, int sr) {
+  if (dry) return PF_OK;
+  LAUNCHED(layernorm_launch(x, nullptr, rows, C, w.w, w.b, eps, st, y, patch, RH, RW, sr));
+  return PF_OK;
+}
+int Fwd::ln(const float* x, float* y, long long rows, int C, const LnW& w, float eps) {
+  if (dry) return PF_OK;
+  LAUNCHED(layernorm_launch(x, y, rows, C, w.w, w.b, eps, st));
+  return PF_OK;
+}
 
 // ----------------------------------------------------------------------------------------------- the forward graph
 constexpr long long kTableSlabBytes = 8LL << 20;   // ~370 tables of a 2048-pixel axis; reset (after a stream sync) when full
@@ -685,19 +372,9 @@ static int fwd_tails_post(Fwd& F, const pf_batch* bt, const float* conv1_out, Po
                            bt->latitude_original, cls_l ? 0 : 1, d_post, st));
   return PF_OK;
 }
-
 // =============================================================================================== the forward graph
 // The whole network on the TMA -> wgmma engine: every GEMM input is a pre-split bf16 hi/lo tensor written by its producer
 // (LayerNorm, attention, depthwise conv, upsample, stem gather, or the previous GEMM's epilogue).
-// What ParamNet training keeps from its forward for the backward (pf_param_train_forward -> pf_param_backward): the packed input,
-// the stem's pre-LayerNorm output and the residual stream before and after every block (xs[s][j] = input of block j of stage s,
-// xs[s][depth] = the stage's output).  Everything else is recomputed.
-struct PnSaved {
-  float* pin = nullptr;
-  float* stem_pre = nullptr;
-  float* xs[4][10] = {};
-};
-static int fwd_paramnet(Fwd& F, const float* grav, const float* lat, float* params, float* raw, const PnSaved* sv = nullptr);
 static int run_forward(Fwd& F, const pf_batch* bt) {
   pf_engine* e = F.e;
   const pf_model_desc& D = e->desc;
@@ -883,7 +560,7 @@ static int run_forward(Fwd& F, const pf_batch* bt) {
 // ParamNet (ConvNeXt-T) on fields at the working size, the last section of pf_forward (on the heads' outputs) and all of
 // pf_param_forward (on the caller's fields): grav [n,2,NH,NW] up vectors, lat [n,1,NH,NW] sin(latitude) -> params [n,8]
 // (pf_batch.params layout) and, when raw is non-NULL, the head's five outputs before any scaling as [n,5].
-static int fwd_paramnet(Fwd& F, const float* grav, const float* lat, float* params, float* raw, const PnSaved* sv) {
+int fwd_paramnet(Fwd& F, const float* grav, const float* lat, float* params, float* raw, const PnSaved* sv) {
   pf_engine* e = F.e;
   const pf_model_desc& D = e->desc;
   const int n = F.n;
@@ -938,402 +615,9 @@ static int fwd_paramnet(Fwd& F, const float* grav, const float* lat, float* para
   return PF_OK;
 }
 
-// ----------------------------------------------------------------------------------------------- ParamNet training
-// The fields' size at the ConvNeXt input (centred: the working size; uncentred: INPUT_SIZE square)
-static void pn_input_size(const pf_engine* e, int* SH, int* SW) {
-  const bool centered = e->desc.param_net == PF_PARAM_CENTERED;
-  *SH = centered ? e->net_h : e->desc.param_input_size;
-  *SW = centered ? e->net_w : e->desc.param_input_size;
-}
-
-// The saved activations sit at the start of the workspace, so the training forward and the backward find them at the same place.
-static void pn_saved_alloc(Fwd& F, PnSaved& sv) {
-  int SH, SW;
-  pn_input_size(F.e, &SH, &SW);
-  const long long n = F.n;
-  sv.pin = F.ar.f(n * SH * SW * 4);
-  int rh = SH / 4, rw = SW / 4;
-  sv.stem_pre = F.ar.f(n * rh * rw * 96);
-  for (int s = 0; s < 4; ++s) {
-    if (s > 0) { rh /= 2; rw /= 2; }
-    for (int j = 0; j <= kCnxDepths[s]; ++j) sv.xs[s][j] = F.ar.f(n * rh * rw * kCnxDims[s]);
-  }
-}
-
-// Gradient buffer of pf_param_backward: one fp32 tensor per ParamNet parameter in the engine's layout, back to back in this order
-// (a parameter's weight and bias are adjacent: the reductions write both at once).
-struct PnGradEntry { std::string name; long long off, numel; };
-static const std::vector<PnGradEntry>& pn_grad_layout() {
-  static const std::vector<PnGradEntry> v = [] {
-    std::vector<PnGradEntry> out;
-    long long off = 0;
-    auto add = [&](const std::string& nm, long long k) { out.push_back({nm, off, k}); off += k; };
-    add("pn.stem.w", 48 * 96); add("pn.stem.b", 96); add("pn.stem.ln.w", 96); add("pn.stem.ln.b", 96);
-    char nm[64];
-    for (int s = 0; s < 4; ++s) {
-      const int C = kCnxDims[s];
-      if (s > 0) {
-        const int Cp = kCnxDims[s - 1];
-        snprintf(nm, sizeof nm, "pn.ds%d.", s);
-        std::string P(nm);
-        add(P + "ln.w", Cp); add(P + "ln.b", Cp); add(P + "w", 4LL * Cp * C); add(P + "b", C);
-      }
-      for (int j = 0; j < kCnxDepths[s]; ++j) {
-        snprintf(nm, sizeof nm, "pn.s%d.b%d.", s, j);
-        std::string P(nm);
-        add(P + "dw.w", 49LL * C); add(P + "dw.b", C); add(P + "ln.w", C); add(P + "ln.b", C);
-        add(P + "pw1.w", 4LL * C * C); add(P + "pw1.b", 4 * C); add(P + "pw2.w", 4LL * C * C); add(P + "pw2.b", C); add(P + "gamma", C);
-      }
-    }
-    add("pn.norm.w", 768); add("pn.norm.b", 768); add("pn.head.w", 5 * 768); add("pn.head.b", 5);
-    return out;
-  }();
-  return v;
-}
-static long long pn_grad_numel() { const auto& v = pn_grad_layout(); return v.back().off + v.back().numel; }
-static long long pn_goff(const std::string& name) {
-  static const std::unordered_map<std::string, long long> m = [] {
-    std::unordered_map<std::string, long long> r;
-    for (const auto& g : pn_grad_layout()) r[g.name] = g.off;
-    return r;
-  }();
-  return m.at(name);
-}
-
-static int resolve_train_weights(pf_engine* e) {
-  auto& T = e->pn_train;
-  char nm[96];
-  for (int s = 1; s < 4; ++s) {
-    const long long numel = 4LL * kCnxDims[s - 1] * kCnxDims[s];
-    snprintf(nm, sizeof nm, "pn.ds%d.t", s);
-    std::string P(nm);
-    TRY(get_w(e, P + ".whi", PF_BF16, numel, (const void**)&T.ds_t[s].hi));
-    TRY(get_w(e, P + ".wlo", PF_BF16, numel, (const void**)&T.ds_t[s].lo));
-  }
-  for (int s = 0; s < 4; ++s) {
-    const int C = kCnxDims[s];
-    T.pw1_t[s].assign(kCnxDepths[s], GemmW());
-    T.pw2_t[s].assign(kCnxDepths[s], GemmW());
-    T.dw_rot[s].assign(kCnxDepths[s], nullptr);
-    for (int j = 0; j < kCnxDepths[s]; ++j) {
-      snprintf(nm, sizeof nm, "pn.s%d.b%d.", s, j);
-      std::string P(nm);
-      for (int k = 0; k < 2; ++k) {
-        GemmW& g = k ? T.pw2_t[s][j] : T.pw1_t[s][j];
-        const std::string q = P + (k ? "pw2t" : "pw1t");
-        TRY(get_w(e, q + ".whi", PF_BF16, 4LL * C * C, (const void**)&g.hi));
-        TRY(get_w(e, q + ".wlo", PF_BF16, 4LL * C * C, (const void**)&g.lo));
-      }
-      TRY(get_f(e, P + "dw.wr", 49LL * C, &T.dw_rot[s][j]));
-    }
-  }
-  TRY(get_f(e, "pn.zero", 768, &T.zero));
-  return PF_OK;
-}
-
-static int pn_reduce(Fwd& F, const float* part, int P, long long L, float* out) {
-  if (!F.dry) LAUNCHED((reduce_partials_kernel<<<(unsigned)cdivl(L, 32), 256, 0, F.st>>>(part, P, L, out), cudaGetLastError()));
-  return PF_OK;
-}
-// out[c] = sum over the R rows of src [R x C]
-static int pn_colsum(Fwd& F, const float* src, long long R, int C, float* out) {
-  const long long rpb = std::max(256LL, cdivl(R, 2048));
-  const int P = (int)cdivl(R, rpb);
-  const long long m = F.ar.mark();
-  float* part = F.ar.f((long long)P * C);
-  if (!F.dry) LAUNCHED((colsum_partial_kernel<<<dim3(P, cdiv(C, 32)), 256, 0, F.st>>>(src, R, C, rpb, part), cudaGetLastError()));
-  TRY(pn_reduce(F, part, P, C, out));
-  F.ar.release(m);
-  return PF_OK;
-}
-// LayerNorm backward: dx (written) and the weight / bias gradients at g, g + C
-static int pn_ln_bwd(Fwd& F, const float* x, const float* dy, long long R, int C, const float* w, float* dx, float* g) {
-  const long long rpb = std::max(64LL, cdivl(R, 2048));
-  const int P = (int)cdivl(R, rpb);
-  const long long m = F.ar.mark();
-  float* part = F.ar.f((long long)P * 2 * C);
-  if (!F.dry) LAUNCHED((ln_bwd_kernel<<<P, 256, 0, F.st>>>(x, dy, R, C, w, 1e-6f, rpb, dx, part), cudaGetLastError()));
-  TRY(pn_reduce(F, part, P, 2LL * C, g));
-  F.ar.release(m);
-  return PF_OK;
-}
-
-// Weight gradient dW[N x K] = sum over R rows of dY[r][n] X[r][k] on the GEMM engine: the rows are cut into S chunks, each chunk is
-// one group of a grouped GEMM-mode launch (A = dY^T [N][S chunk], B = X^T [S][K][chunk], both transposed split copies), which writes
-// per-chunk partials [S][N][K]; pn_reduce adds them in order.  S is chosen from the shapes so that the launch fills the SMs.
-struct WgPlan { int S, chunk; long long Rp; };
-static WgPlan pn_wg_plan(const pf_engine* e, long long R, int N, int K) {
-  const int bn = tma_pick_bn(K, MODE_GEMM);
-  const long long tiles = (long long)cdiv(N, 128) * cdiv(K, bn);
-  long long S = cdivl(2LL * e->sm_count, tiles);
-  S = std::min(S, std::max(1LL, R / 1024));
-  S = std::max(1LL, std::min(S, 256LL));
-  WgPlan p;
-  p.chunk = (int)(cdivl(cdivl(R, S), 64) * 64);
-  p.S = (int)cdivl(R, p.chunk);
-  p.Rp = (long long)p.S * p.chunk;
-  return p;
-}
-// transposed split copy of [R x C] (fp32 src with row pitch ld, or split planes ssrc): layout A [C][Rp], layout B [S][C][chunk]
-static int pn_tsplit(Fwd& F, const float* src, const SplitT* ssrc, int ld, long long R, int C, const WgPlan& pl, bool layout_b, int op, SplitT& out) {
-  out = F.salloc(pl.Rp, C);
-  if (F.dry) return PF_OK;
-  const long long sS = layout_b ? (long long)C * pl.chunk : pl.chunk, sC = layout_b ? pl.chunk : pl.Rp;
-  const dim3 grid((unsigned)cdivl(pl.Rp, 32), (unsigned)cdiv(C, 32));
-  if (ssrc) LAUNCHED((transpose_split_kernel<true, 0><<<grid, 256, 0, F.st>>>(nullptr, ssrc->hi, ssrc->lo, ld, R, pl.Rp, C, pl.chunk, sS, sC, out.hi, out.lo), cudaGetLastError()));
-  else if (op == 1) LAUNCHED((transpose_split_kernel<false, 1><<<grid, 256, 0, F.st>>>(src, nullptr, nullptr, ld, R, pl.Rp, C, pl.chunk, sS, sC, out.hi, out.lo), cudaGetLastError()));
-  else LAUNCHED((transpose_split_kernel<false, 0><<<grid, 256, 0, F.st>>>(src, nullptr, nullptr, ld, R, pl.Rp, C, pl.chunk, sS, sC, out.hi, out.lo), cudaGetLastError()));
-  return PF_OK;
-}
-static int pn_wgrad(Fwd& F, const SplitT& aT, const SplitT& bT, int N, int K, const WgPlan& pl, float* part) {
-  TmaGemmParams p{};
-  p.M = N; p.N = K; p.K = pl.chunk; p.Cin = pl.chunk; p.a_gc = pl.chunk; p.groups = pl.S;
-  p.C = part; p.ldc = K; p.c_gcoff = N * K;
-  const int bn = tma_pick_bn(K, MODE_GEMM), kb = tma_pick_kb(bn, pl.chunk, MODE_GEMM);
-  // (checked in the sizing dry run too, so that a shape the engine cannot run fails before anything is launched)
-  if (const char* msg = gemm_tma_check(MODE_GEMM, p, bn, kb, false, false, F.np())) return fail(PF_ERR_ARG, "weight-gradient GEMM (bn %d, kb %d): %s", bn, kb, msg);
-  if (F.dry) return PF_OK;
-  TmaMaps maps{};
-  const char* msg = F.map2d(&maps.a_hi, aT.hi, pl.Rp, N, pl.Rp, 128, kb);
-  if (!msg) msg = F.map2d(&maps.a_lo, aT.lo, pl.Rp, N, pl.Rp, 128, kb);
-  if (!msg) msg = F.map2d(&maps.b_hi, bT.hi, pl.chunk, (long long)pl.S * K, pl.chunk, bn, kb);
-  if (!msg) msg = F.map2d(&maps.b_lo, bT.lo, pl.chunk, (long long)pl.S * K, pl.chunk, bn, kb);
-  if (msg) return fail(PF_ERR_CUDA, "%s", msg);
-  maps.a2_hi = maps.a_hi; maps.a2_lo = maps.a_lo;
-  F.picked_bn = bn; F.picked_kb = kb; F.picked_sched = 1;
-  return F.launch_tma(MODE_GEMM, maps, p, bn, kb, false);
-}
-static int pn_wgrad_full(Fwd& F, const float* dy, int ldy, const SplitT* xs, const float* xf, int op, int ldx, long long R, int N, int K, float* out,
-                         WgPlan* plan = nullptr) {
-  const long long m = F.ar.mark();
-  const WgPlan pl = pn_wg_plan(F.e, R, N, K);
-  if (plan) *plan = pl;
-  SplitT aT, bT;
-  TRY(pn_tsplit(F, dy, nullptr, ldy, R, N, pl, false, 0, aT));
-  TRY(pn_tsplit(F, xf, xs, ldx, R, K, pl, true, op, bT));
-  float* part = F.ar.f((long long)pl.S * N * K);
-  TRY(pn_wgrad(F, aT, bT, N, K, pl, part));
-  TRY(pn_reduce(F, part, pl.S, (long long)N * K, out));
-  F.ar.release(m);
-  return PF_OK;
-}
-
-static int pn_dw_launch(Fwd& F, const float* x, float* y, int rh, int rw, int C, const float* w, const float* b) {
+int pn_dw_launch(Fwd& F, const float* x, float* y, int rh, int rw, int C, const float* w, const float* b) {
   if (!F.dry) LAUNCHED(launch_pdl(dwconv7x7_kernel, dim3(ew_grid((long long)F.n * ((rh + 1) / 2) * ((rw + PF_DW7_PX - 1) / PF_DW7_PX) * (C / 4))), dim3(256), 0, F.st,
                                   x, y, F.n, rh, rw, C, w, b));
-  return PF_OK;
-}
-
-// Image rows per block of the depthwise and stem weight-gradient kernels: at most 1024 partials, one row each while that suffices
-static int pn_rows_per_block(int rows) { return std::max(1, cdiv(rows, 1024)); }
-
-// depthwise 7x7 weight and bias gradients of the F.n images [rh, rw, C]: out [50][C] (49 taps, then the bias)
-static int pn_dw7_wgrad(Fwd& F, const float* xin, const float* dt, int rh, int rw, int C, float* out, int* rpb_out = nullptr) {
-  const int rows = F.n * rh, rpb = pn_rows_per_block(rows), np_ = cdiv(rows, rpb);
-  if (rpb_out) *rpb_out = rpb;
-  const long long m = F.ar.mark();
-  float* part = F.ar.f((long long)np_ * 50 * C);
-  if (!F.dry) LAUNCHED((dw7_wgrad_kernel<<<dim3(np_, C / 32), 256, 0, F.st>>>(xin, dt, F.n, rh, rw, C, rpb, part), cudaGetLastError()));
-  TRY(pn_reduce(F, part, np_, 50LL * C, out));
-  F.ar.release(m);
-  return PF_OK;
-}
-
-static int pn_pw2_grads(Fwd& F, const float* G, const float* sdy, int C, int K, const float* gamma, const GemmW& w2, float* dW, float* db, float* dgamma) {
-  if (!F.dry) LAUNCHED((pw2_grads_kernel<<<cdiv(C, 8), 256, 0, F.st>>>(G, sdy, C, K, gamma, w2.hi, w2.lo, w2.b, dW, db, dgamma), cudaGetLastError()));
-  return PF_OK;
-}
-static int pn_gelu_bwd(Fwd& F, const float* dh, float* u, long long n, __nv_bfloat16* hi, __nv_bfloat16* lo) {
-  if (!F.dry) LAUNCHED((gelu_bwd_kernel<<<ew_grid(n), 256, 0, F.st>>>(dh, u, n, hi, lo), cudaGetLastError()));
-  return PF_OK;
-}
-static int pn_scale_split(Fwd& F, const float* src, const float* scale, long long n, int C, const SplitT& out) {
-  if (!F.dry) LAUNCHED((scale_split_kernel<<<ew_grid(n), 256, 0, F.st>>>(src, scale, n, C, out.hi, out.lo), cudaGetLastError()));
-  return PF_OK;
-}
-static int pn_col2im2(Fwd& F, const float* dP, int rh, int rw, int C, float* out) {
-  if (!F.dry) LAUNCHED((col2im2_kernel<<<ew_grid((long long)F.n * rh * rw * C), 256, 0, F.st>>>(dP, F.n, rh, rw, C, out), cudaGetLastError()));
-  return PF_OK;
-}
-
-// One ConvNeXt block backward: dx holds d loss / d(block output) and becomes d loss / d(block input).  Recomputes dwconv -> LN ->
-// pwconv1 from the saved input.
-static int pn_block_bwd(Fwd& F, int s, int j, const float* xin, float* dx, int rh, int rw, float* grads) {
-  pf_engine* e = F.e;
-  Arena& ar = F.ar;
-  const bool dry = F.dry;
-  cudaStream_t st = F.st;
-  const int C = kCnxDims[s];
-  const long long R = (long long)F.n * rh * rw;
-  const CnxBlockW& b = e->pn_blocks[s][j];
-  const auto& T = e->pn_train;
-  char nm[64];
-  snprintf(nm, sizeof nm, "pn.s%d.b%d.", s, j);
-  const std::string P(nm);
-  const long long m0 = ar.mark();
-  float* t = ar.f(R * C);
-  TRY(pn_dw_launch(F, xin, t, rh, rw, C, b.dw_w, b.dw_b));
-  SplitT ys = F.salloc(R, C);
-  TRY(F.ln_split(t, ys, R, C, b.ln, 1e-6f));
-  float* u = ar.f(R * 4 * C);                     // pwconv1 output before the GELU
-  { Fwd::Epi o; o.C = u; o.ldc = 4 * C; TRY(F.tgemm(ys, R, C, 0, b.pw1, 4 * C, o)); }
-  // pwconv2 and gamma from G = dx^T GELU(u) and the column sums of dx
-  {
-    const long long m1 = ar.mark();
-    float* G = ar.f(4LL * C * C);
-    float* sdx = ar.f(C);
-    TRY(pn_wgrad_full(F, dx, C, nullptr, u, 1, 4 * C, R, C, 4 * C, G));
-    TRY(pn_colsum(F, dx, R, C, sdx));
-    TRY(pn_pw2_grads(F, G, sdx, C, 4 * C, b.gamma, b.pw2, grads + pn_goff(P + "pw2.w"), grads + pn_goff(P + "pw2.b"), grads + pn_goff(P + "gamma")));
-    ar.release(m1);
-  }
-  // dh = (gamma dx) W2, then du = dh GELU'(u), written over u
-  {
-    const long long m1 = ar.mark();
-    SplitT dz = F.salloc(R, C);
-    TRY(pn_scale_split(F, dx, b.gamma, R * C, C, dz));
-    float* dh = ar.f(R * 4 * C);
-    { Fwd::Epi o; o.C = dh; o.ldc = 4 * C; TRY(F.tgemm(dz, R, C, 0, T.pw2_t[s][j], 4 * C, o)); }
-    TRY(pn_gelu_bwd(F, dh, u, R * 4 * C, nullptr, nullptr));
-    ar.release(m1);
-  }
-  // pwconv1 weight and bias
-  TRY(pn_wgrad_full(F, u, 4 * C, &ys, nullptr, 0, C, R, 4 * C, C, grads + pn_goff(P + "pw1.w")));
-  TRY(pn_colsum(F, u, R, 4 * C, grads + pn_goff(P + "pw1.b")));
-  // dy = du W1
-  float* dy = ar.f(R * C);
-  {
-    const long long m1 = ar.mark();
-    SplitT du = F.salloc(R, 4 * C);
-    TRY(pn_scale_split(F, u, nullptr, R * 4 * C, 4 * C, du));
-    Fwd::Epi o; o.C = dy; o.ldc = C;
-    TRY(F.tgemm(du, R, 4 * C, 0, T.pw1_t[s][j], C, o));
-    ar.release(m1);
-  }
-  float* dt = ar.f(R * C);
-  TRY(pn_ln_bwd(F, t, dy, R, C, b.ln.w, dt, grads + pn_goff(P + "ln.w")));
-  // depthwise 7x7: weight and bias, then the data gradient (the forward kernel with the rotated kernel) added to the residual's
-  TRY(pn_dw7_wgrad(F, xin, dt, rh, rw, C, grads + pn_goff(P + "dw.w")));
-  TRY(pn_dw_launch(F, dt, dy, rh, rw, C, T.dw_rot[s][j], T.zero));
-  if (!dry) LAUNCHED((add_inplace_kernel<<<ew_grid(R * C), 256, 0, st>>>(dx, dy, R * C), cudaGetLastError()));
-  ar.release(m0);
-  return PF_OK;
-}
-
-// Downsample s (LayerNorm, then the 2x2 / stride 2 conv) backward: dxn = d loss / d(its output) -> dprev = d loss / d(its input xprev)
-static int pn_downsample_bwd(Fwd& F, int s, const float* xprev, int rh, int rw, const float* dxn, float* dprev, float* grads) {
-  pf_engine* e = F.e;
-  Arena& ar = F.ar;
-  const int Cp = kCnxDims[s - 1], C = kCnxDims[s];
-  const long long R = (long long)F.n * rh * rw, R2 = R / 4;
-  char nm[64];
-  snprintf(nm, sizeof nm, "pn.ds%d.", s);
-  const std::string P(nm);
-  const long long m0 = ar.mark();
-  SplitT patch = F.salloc(R2, 4 * Cp);
-  TRY(F.ln_split_patch(xprev, SplitT(), patch, R, Cp, e->pn_ds_ln[s], 1e-6f, rh, rw, 2));
-  TRY(pn_wgrad_full(F, dxn, C, &patch, nullptr, 0, 4 * Cp, R2, C, 4 * Cp, grads + pn_goff(P + "w")));
-  TRY(pn_colsum(F, dxn, R2, C, grads + pn_goff(P + "b")));
-  float* dln = ar.f(R * Cp);
-  {
-    const long long m1 = ar.mark();
-    SplitT d = F.salloc(R2, C);
-    TRY(pn_scale_split(F, dxn, nullptr, R2 * C, C, d));
-    float* dP = ar.f(R2 * 4 * Cp);
-    Fwd::Epi o; o.C = dP; o.ldc = 4 * Cp;
-    TRY(F.tgemm(d, R2, C, 0, e->pn_train.ds_t[s], 4 * Cp, o));
-    TRY(pn_col2im2(F, dP, rh, rw, Cp, dln));
-    ar.release(m1);
-  }
-  TRY(pn_ln_bwd(F, xprev, dln, R, Cp, e->pn_ds_ln[s].w, dprev, grads + pn_goff(P + "ln.w")));
-  ar.release(m0);
-  return PF_OK;
-}
-
-// tail (pool -> LayerNorm(768) -> head) backward of the F.n pairs: dx [n, HW, 768] and the tail's gradients at g (norm.w, norm.b,
-// head.w, head.b: kTailGrads values)
-static int pn_tail_bwd(Fwd& F, const float* feat, int HW, const float* nw, const float* nb, const float* hw, const float* draw, float* dx, float* g) {
-  const long long m = F.ar.mark();
-  float* part = F.ar.f((long long)F.n * kTailGrads);
-  if (!F.dry) LAUNCHED((param_tail_bwd_kernel<<<F.n, 256, 0, F.st>>>(feat, HW, nw, nb, hw, draw, dx, part), cudaGetLastError()));
-  TRY(pn_reduce(F, part, F.n, kTailGrads, g));
-  F.ar.release(m);
-  return PF_OK;
-}
-
-// stem weight and bias gradients from the packed input [n, 4 OH, 4 OW, 4] and dS [n, OH, OW, 96]: out [49][96] (48 weight rows
-// (ky, kx, ci), then the bias)
-static int pn_stem_wgrad(Fwd& F, const float* pin, const float* dS, int OH, int OW, float* out, int* rpb_out = nullptr) {
-  const int rows = F.n * OH, rpb = pn_rows_per_block(rows), np_ = cdiv(rows, rpb);
-  if (rpb_out) *rpb_out = rpb;
-  const long long m = F.ar.mark();
-  float* part = F.ar.f((long long)np_ * 49 * 96);
-  if (!F.dry) LAUNCHED((stem_wgrad_kernel<<<dim3(np_, 3), 256, 0, F.st>>>(pin, dS, F.n, OH, OW, rpb, part), cudaGetLastError()));
-  TRY(pn_reduce(F, part, np_, 49LL * 96, out));
-  F.ar.release(m);
-  return PF_OK;
-}
-static int pn_stem_dgrad(Fwd& F, const float* dS, const float* w, int OH, int OW, float* dpin) {
-  if (!F.dry) LAUNCHED((stem_dgrad_kernel<<<ew_grid((long long)F.n * OH * OW * 48), 256, 0, F.st>>>(dS, w, F.n, OH, OW, dpin), cudaGetLastError()));
-  return PF_OK;
-}
-// backward of the nearest resize of the fields IH x IW -> OH x OW (pack_fields_kernel)
-static int pn_fields_grad(Fwd& F, const float* dpin, int IH, int IW, int OH, int OW, float* dgrav, float* dlat) {
-  if (!F.dry)
-    LAUNCHED((unpack_fields_grad_kernel<<<(unsigned)cdivl((long long)F.n * IH * IW, 256), 256, 0, F.st>>>(dpin, F.n, IH, IW, OH, OW, dgrav, dlat), cudaGetLastError()));
-  return PF_OK;
-}
-
-// ParamNet backward from draw [n, 5] (d loss / d raw head outputs) over the activations pf_param_train_forward saved: every
-// parameter gradient into grads (pn_grad_layout, overwritten) and, when dgrav / dlat are non-NULL, the fields' gradients.
-static int bwd_paramnet(Fwd& F, const PnSaved& sv, const float* draw, float* grads, float* dgrav, float* dlat) {
-  pf_engine* e = F.e;
-  Arena& ar = F.ar;
-  const int n = F.n;
-  int SH, SW;
-  pn_input_size(e, &SH, &SW);
-  int rh[4], rw[4];
-  rh[0] = SH / 4; rw[0] = SW / 4;
-  for (int s = 1; s < 4; ++s) { rh[s] = rh[s - 1] / 2; rw[s] = rw[s - 1] / 2; }
-  float* dx = ar.f((long long)n * rh[3] * rw[3] * 768);
-  TRY(pn_tail_bwd(F, sv.xs[3][kCnxDepths[3]], rh[3] * rw[3], e->pn_norm.w, e->pn_norm.b, e->pn_head_w, draw, dx, grads + pn_goff("pn.norm.w")));
-  for (int s = 3; s >= 0; --s) {
-    for (int j = kCnxDepths[s] - 1; j >= 0; --j) TRY(pn_block_bwd(F, s, j, sv.xs[s][j], dx, rh[s], rw[s], grads));
-    if (s > 0) {
-      float* dprev = ar.f((long long)n * rh[s - 1] * rw[s - 1] * kCnxDims[s - 1]);
-      TRY(pn_downsample_bwd(F, s, sv.xs[s - 1][kCnxDepths[s - 1]], rh[s - 1], rw[s - 1], dx, dprev, grads));
-      dx = dprev;
-    }
-  }
-  // stem: LayerNorm, then the 4x4 / stride 4 conv
-  const long long R0 = (long long)n * rh[0] * rw[0];
-  float* dstem = ar.f(R0 * 96);
-  TRY(pn_ln_bwd(F, sv.stem_pre, dx, R0, 96, e->pn_stem_ln.w, dstem, grads + pn_goff("pn.stem.ln.w")));
-  TRY(pn_stem_wgrad(F, sv.pin, dstem, rh[0], rw[0], grads + pn_goff("pn.stem.w")));
-  if (dgrav) {
-    float* dpin = ar.f((long long)n * SH * SW * 4);
-    TRY(pn_stem_dgrad(F, dstem, e->pn_stem_w, rh[0], rw[0], dpin));
-    TRY(pn_fields_grad(F, dpin, e->net_h, e->net_w, SH, SW, dgrav, dlat));
-  }
-  return PF_OK;
-}
-
-// the two training passes, each starting with the saved activations at the bottom of the workspace
-static int pn_train_pass(Fwd& F, bool backward, const float* grav, const float* lat, float* raw, const float* draw, float* grads, float* dgrav, float* dlat) {
-  PnSaved sv;
-  pn_saved_alloc(F, sv);
-  if (backward) return bwd_paramnet(F, sv, draw, grads, dgrav, dlat);
-  float* params = F.ar.f((long long)F.n * 8);
-  return fwd_paramnet(F, grav, lat, params, raw, &sv);
-}
-static int pn_train_peak(pf_handle h, int n, long long* peak) {
-  *peak = 0;
-  for (int b = 0; b < 2; ++b) {
-    Fwd T{h, Arena{}, nullptr, true, n};
-    T.ar.dry = true;
-    TRY(pn_train_pass(T, b == 1, nullptr, nullptr, nullptr, nullptr, nullptr, b == 1 ? (float*)1 : nullptr, nullptr));
-    *peak = std::max(*peak, T.ar.peak);
-  }
   return PF_OK;
 }
 
@@ -1343,29 +627,6 @@ extern "C" {
 int pf_abi_version(void) { return PF_ABI_VERSION; }
 const char* pf_last_error(void) { return g_err.c_str(); }
 int64_t pf_kernel_launch_count(void) { return g_launches.load(); }
-
-// The opt-in for more than 48 KB of dynamic shared memory is a per-device attribute of each kernel: set for every kernel of the
-// library on every device an engine (or an operator entry point) uses, once per device and thread-safe.
-static int configure_device(int device) {
-  static std::mutex mu;
-  static std::vector<char> done;
-  std::lock_guard<std::mutex> lock(mu);
-  if (device < (int)done.size() && done[device]) return PF_OK;
-  CU(gemm_tma_configure_device(3));
-  CU(gemm_tma_configure_device(1));
-  CU(attention_mma_configure_device());
-  CU(cudaFuncSetAttribute(conv1_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kRingSmem));
-  CU(cudaFuncSetAttribute(preprocess_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPreSmemBytes));
-  CU(cudaFuncSetAttribute(postprocess_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPostSmemMax));
-  if (device >= (int)done.size()) done.resize(device + 1, 0);
-  done[device] = 1;
-  return PF_OK;
-}
-static int configure_current_device() {
-  int dev = 0;
-  CU(cudaGetDevice(&dev));
-  return configure_device(dev);
-}
 
 // a working size the engine supports: H and W multiples of 32 in [64, 640] (the smallest head level is then at least 2 x 2, which
 // the border-class bias needs) with at most kAmMaxKeys attention keys (H/32) * (W/32)
@@ -1525,65 +786,6 @@ int pf_param_forward(pf_handle h, int n, const float* gravity, const float* lati
   return r;
 }
 
-static int pn_train_check(const char* fn, pf_handle h, int n, void* workspace, int64_t workspace_bytes) {
-  if (!h) return fail(PF_ERR_ARG, "%s: null handle", fn);
-  if (!h->finalized) return fail(PF_ERR_WEIGHT, "%s: pf_finalize has not succeeded", fn);
-  if (h->desc.param_net == PF_PARAM_NONE) return fail(PF_ERR_ARG, "%s: this model has no ParamNet", fn);
-  if (n < 1) return fail(PF_ERR_ARG, "%s: n = %d, at least 1 pair of fields is needed", fn, n);
-  if (!workspace) return fail(PF_ERR_ARG, "%s: null workspace", fn);
-  long long peak = 0;
-  TRY(pn_train_peak(h, n, &peak));
-  if (peak > workspace_bytes) return fail(PF_ERR_ARG, "%s: workspace %lld B < required %lld B", fn, (long long)workspace_bytes, peak);
-  if (((uintptr_t)workspace & 255) != 0) return fail(PF_ERR_ARG, "%s: workspace must be 256-byte aligned", fn);
-  return PF_OK;
-}
-
-int64_t pf_param_train_workspace_bytes(pf_handle h, int n) {
-  if (!h || n < 1) return fail(PF_ERR_ARG, "pf_param_train_workspace_bytes: bad argument");
-  if (!h->finalized) return fail(PF_ERR_WEIGHT, "pf_param_train_workspace_bytes: pf_finalize has not succeeded");
-  if (h->desc.param_net == PF_PARAM_NONE) return fail(PF_ERR_ARG, "pf_param_train_workspace_bytes: this model has no ParamNet");
-  long long peak = 0;
-  TRY(pn_train_peak(h, n, &peak));
-  return peak + 4096;
-}
-
-int pf_param_train_forward(pf_handle h, int n, const float* gravity, const float* latitude, float* raw, void* workspace, int64_t workspace_bytes,
-                           void* stream) {
-  TRY(pn_train_check("pf_param_train_forward", h, n, workspace, workspace_bytes));
-  if (!gravity || !latitude || !raw) return fail(PF_ERR_ARG, "pf_param_train_forward: null gravity / latitude / raw");
-  CU(cudaSetDevice(h->device));
-  Fwd F{h, Arena{}, (cudaStream_t)stream, false, n};
-  F.ar.base = (char*)workspace;
-  F.ar.cap = workspace_bytes;
-  NvtxRange r_("pf:paramnet_train_forward");
-  return pn_train_pass(F, false, gravity, latitude, raw, nullptr, nullptr, nullptr, nullptr);
-}
-
-int pf_param_backward(pf_handle h, int n, const float* draw, float* grads, float* grad_gravity, float* grad_latitude, void* workspace,
-                      int64_t workspace_bytes, void* stream) {
-  TRY(pn_train_check("pf_param_backward", h, n, workspace, workspace_bytes));
-  if (!draw || !grads) return fail(PF_ERR_ARG, "pf_param_backward: null draw / grads");
-  if ((grad_gravity == nullptr) != (grad_latitude == nullptr)) return fail(PF_ERR_ARG, "pf_param_backward: grad_gravity and grad_latitude are both NULL or both set");
-  TRY(resolve_train_weights(h));
-  CU(cudaSetDevice(h->device));
-  Fwd F{h, Arena{}, (cudaStream_t)stream, false, n};
-  F.ar.base = (char*)workspace;
-  F.ar.cap = workspace_bytes;
-  NvtxRange r_("pf:paramnet_backward");
-  return pn_train_pass(F, true, nullptr, nullptr, nullptr, draw, grads, grad_gravity, grad_latitude);
-}
-
-int64_t pf_param_grad_numel(void) { return pn_grad_numel(); }
-
-int pf_param_grad_entry(int i, const char** name, int64_t* offset, int64_t* numel) {
-  const auto& v = pn_grad_layout();
-  if (i < 0 || i >= (int)v.size() || !name || !offset || !numel) return fail(PF_ERR_ARG, "pf_param_grad_entry: bad argument");
-  *name = v[i].name.c_str();
-  *offset = v[i].off;
-  *numel = v[i].numel;
-  return PF_OK;
-}
-
 int pf_profile_enable(pf_handle h, int on) {
   if (!h) return fail(PF_ERR_ARG, "null handle");
   h->profile = on != 0;
@@ -1705,182 +907,43 @@ int pf_debug_copy(pf_handle h, const char* name, float* dst, int64_t numel, void
   return fail(PF_ERR_ARG, "pf_debug_copy: no tap '%s'", name);
 }
 
-// ---- multi-GPU gather (NCCL point-to-point; SURVEY.md 8e) ---------------------------------------------------
-#define NCCL_TRY(expr)                                                                                              \
-  do {                                                                                                              \
-    int r__ = (expr);                                                                                               \
-    if (r__ != kNcclSuccess) return fail(PF_ERR_CUDA, "%s: %s", #expr, api.GetErrorString ? api.GetErrorString(r__) : "NCCL error"); \
-  } while (0)
-int pf_comm_unique_id(void* id128) {
-  if (!id128) return fail(PF_ERR_ARG, "pf_comm_unique_id: null argument");
-  const NcclApi& api = nccl_api();
-  if (api.error) return fail(PF_ERR_CUDA, "%s", api.error);
-  static_assert(sizeof(NcclUniqueId) == 128, "ncclUniqueId is 128 bytes");
-  NCCL_TRY(api.GetUniqueId((NcclUniqueId*)id128));
-  return PF_OK;
-}
-int pf_comm_create(int device, int rank, int nranks, const void* id128, pf_comm_handle* out) {
-  if (!id128 || !out || nranks < 1 || rank < 0 || rank >= nranks) return fail(PF_ERR_ARG, "pf_comm_create: bad argument");
-  const NcclApi& api = nccl_api();
-  if (api.error) return fail(PF_ERR_CUDA, "%s", api.error);
-  CU(cudaSetDevice(device));
-  NcclUniqueId id;
-  memcpy(&id, id128, sizeof id);
-  pf_comm* c = new pf_comm();
-  c->device = device; c->rank = rank; c->nranks = nranks;
-  const int r = api.CommInitRank(&c->comm, nranks, id, rank);
-  if (r != kNcclSuccess) { delete c; return fail(PF_ERR_CUDA, "ncclCommInitRank: %s", api.GetErrorString(r)); }
-  *out = c;
-  return PF_OK;
-}
-int pf_comm_destroy(pf_comm_handle c) {
-  if (!c) return PF_OK;
-  const NcclApi& api = nccl_api();
-  cudaSetDevice(c->device);
-  if (c->comm && api.CommDestroy) api.CommDestroy(c->comm);
-  delete c;
-  return PF_OK;
-}
-int pf_gather(pf_comm_handle c, int root, int count, void* const* dev_ptrs, const int64_t* bytes, const int32_t* peer, void* stream) {
-  if (!c || count < 0 || root < 0 || root >= c->nranks || (count > 0 && (!dev_ptrs || !bytes))) return fail(PF_ERR_ARG, "pf_gather: bad argument");
-  if (c->rank == root && count > 0 && !peer) return fail(PF_ERR_ARG, "pf_gather: the root needs the source rank of every segment");
-  const NcclApi& api = nccl_api();
-  CU(cudaSetDevice(c->device));
-  if (count == 0) return PF_OK;
-  NCCL_TRY(api.GroupStart());
-  for (int i = 0; i < count; ++i) {
-    int r;
-    if (c->rank == root) {
-      if (peer[i] < 0 || peer[i] >= c->nranks || peer[i] == root) { api.GroupEnd(); return fail(PF_ERR_ARG, "pf_gather: segment %d comes from rank %d", i, peer[i]); }
-      r = api.Recv(dev_ptrs[i], (size_t)bytes[i], kNcclUint8, peer[i], c->comm, (cudaStream_t)stream);
-    } else {
-      r = api.Send(dev_ptrs[i], (size_t)bytes[i], kNcclUint8, root, c->comm, (cudaStream_t)stream);
-    }
-    if (r != kNcclSuccess) { api.GroupEnd(); return fail(PF_ERR_CUDA, "ncclSend/Recv: %s", api.GetErrorString(r)); }
-  }
-  NCCL_TRY(api.GroupEnd());
+}  // extern "C"
+
+// ----------------------------------------------------------------------------------------------- single-operator entry points
+int op_engine(pf_engine& e, bool bf16) {
+  TRY(configure_current_device());
+  CU(cudaGetDevice(&e.device));
+  CU(cudaDeviceGetAttribute(&e.sm_count, cudaDevAttrMultiProcessorCount, e.device));
+  e.bf16 = bf16;
   return PF_OK;
 }
 
-// ---- decode front-end (nvJPEG; SURVEY.md 8f-2) ------------------------------------------------------------------
-int pf_jpeg_create(int device, int max_threads, pf_jpeg_handle* out) {
-  if (!out) return fail(PF_ERR_ARG, "pf_jpeg_create: null argument");
-  const NvjpegApi& api = nvjpeg_api();
-  if (api.error) return fail(PF_ERR_CUDA, "%s", api.error);
-  CU(cudaSetDevice(device));
-  pf_jpeg* j = new pf_jpeg();
-  j->device = device;
-  if (api.CreateSimple(&j->handle) != NVJPEG_STATUS_SUCCESS) { delete j; return fail(PF_ERR_CUDA, "nvjpegCreateSimple failed"); }
-  int nt = max_threads > 0 ? max_threads : (int)std::thread::hardware_concurrency() / 2;
-  nt = nt < 1 ? 1 : (nt > 32 ? 32 : nt);
-  j->workers.resize(nt);
-  bool ok = cudaEventCreateWithFlags(&j->start, cudaEventDisableTiming) == cudaSuccess;
-  for (auto& w : j->workers) {
-    ok = ok && api.StateCreate(j->handle, &w.state) == NVJPEG_STATUS_SUCCESS;
-    ok = ok && cudaStreamCreateWithFlags(&w.stream, cudaStreamNonBlocking) == cudaSuccess;
-    ok = ok && cudaEventCreateWithFlags(&w.done, cudaEventDisableTiming) == cudaSuccess;
-  }
-  if (!ok) { pf_jpeg_destroy(j); return fail(PF_ERR_CUDA, "pf_jpeg_create: decoder state / stream creation failed"); }
-  *out = j;
-  return PF_OK;
-}
-int pf_jpeg_destroy(pf_jpeg_handle j) {
-  if (!j) return PF_OK;
-  const NvjpegApi& api = nvjpeg_api();
-  cudaSetDevice(j->device);
-  for (auto& w : j->workers) {
-    if (w.stream) cudaStreamSynchronize(w.stream);
-    if (w.state) api.StateDestroy(w.state);
-    if (w.stream) cudaStreamDestroy(w.stream);
-    if (w.done) cudaEventDestroy(w.done);
-  }
-  if (j->start) cudaEventDestroy(j->start);
-  if (j->handle) api.Destroy(j->handle);
-  delete j;
-  return PF_OK;
-}
-int pf_jpeg_info(pf_jpeg_handle j, const uint8_t* data, int64_t length, int32_t* height, int32_t* width) {
-  if (!j || !data || length < 4 || !height || !width) return fail(PF_ERR_ARG, "pf_jpeg_info: bad argument");
-  const NvjpegApi& api = nvjpeg_api();
-  int nc = 0, ws[NVJPEG_MAX_COMPONENT] = {0}, hs[NVJPEG_MAX_COMPONENT] = {0};
-  nvjpegChromaSubsampling_t ss;
-  if (api.GetImageInfo(j->handle, data, (size_t)length, &nc, &ss, ws, hs) != NVJPEG_STATUS_SUCCESS) return fail(PF_ERR_ARG, "pf_jpeg_info: not a decodable JPEG stream");
-  *height = hs[0]; *width = ws[0];
-  return PF_OK;
-}
-int pf_jpeg_decode_batch(pf_jpeg_handle j, int n, const uint8_t* const* data, const int64_t* length, const int32_t* height, const int32_t* width,
-                         uint8_t* blob, const int64_t* offset, void* stream) {
-  if (!j || n < 1 || !data || !length || !height || !width || !blob || !offset) return fail(PF_ERR_ARG, "pf_jpeg_decode_batch: bad argument");
-  const NvjpegApi& api = nvjpeg_api();
-  CU(cudaSetDevice(j->device));
-  cudaStream_t st = (cudaStream_t)stream;
-  // the workers' streams start after everything already queued on the caller's stream (the blob may be in use by an earlier forward)
-  CU(cudaEventRecord(j->start, st));
-  const int nt = (int)j->workers.size() < n ? (int)j->workers.size() : n;
-  std::atomic<int> next{0}, failed{-1};
-  auto work = [&](int t) {
-    cudaSetDevice(j->device);
-    pf_jpeg::Worker& w = j->workers[t];
-    cudaStreamWaitEvent(w.stream, j->start, 0);
-    for (int i = next.fetch_add(1); i < n; i = next.fetch_add(1)) {
-      nvjpegImage_t dst{};
-      dst.channel[0] = blob + offset[i];
-      dst.pitch[0] = (size_t)width[i] * 3;
-      if (api.Decode(j->handle, w.state, data[i], (size_t)length[i], NVJPEG_OUTPUT_BGRI, &dst, w.stream) != NVJPEG_STATUS_SUCCESS) failed.store(i);
-    }
-    cudaEventRecord(w.done, w.stream);
-  };
-  std::vector<std::thread> threads;
-  for (int t = 1; t < nt; ++t) threads.emplace_back(work, t);
-  work(0);
-  for (auto& th : threads) th.join();
-  for (int t = 0; t < nt; ++t) CU(cudaStreamWaitEvent(st, j->workers[t].done, 0));
-  if (failed.load() >= 0) return fail(PF_ERR_ARG, "pf_jpeg_decode_batch: image %d could not be decoded", failed.load());
+// a host array copied into the op's scratch on its stream
+template <class T>
+static int op_upload(Fwd& F, const T* src, size_t count, T** dst) {
+  *dst = (T*)F.ar.alloc((long long)(count * sizeof(T)));
+  if (!F.dry) CU(cudaMemcpyAsync(*dst, src, count * sizeof(T), cudaMemcpyHostToDevice, F.st));
   return PF_OK;
 }
 
-// ---- single-operator entry points ------------------------------------------------------------------------
+extern "C" {
+
 int pf_op_conv_gemm(const float* x, int B, int H, int W, int Cin, const void* whi, const void* wlo, const float* bias, int N, int KH, int KW,
                     int stride, int pad, int in_relu, int act, const float* res, int res_relu, float* y, void* stream) {
   // split the input the way a producer kernel would, then run the same helpers the forward graph uses
   if (!x || !whi || !wlo || !y) return fail(PF_ERR_ARG, "pf_op_conv_gemm: null argument");
   if (KH != KW) return fail(PF_ERR_ARG, "pf_op_conv_gemm: square filters only");
-  TRY(configure_current_device());
-  cudaStream_t st = (cudaStream_t)stream;
-  int dev = 0;
-  CU(cudaGetDevice(&dev));
-  cudaDeviceProp prop;
-  CU(cudaGetDeviceProperties(&prop, dev));
-  pf_engine tmp;
-  tmp.device = dev;
-  tmp.sm_count = prop.multiProcessorCount;
-  const int OH = (H + 2 * pad - KH) / stride + 1, OW = (W + 2 * pad - KW) / stride + 1;
-  const long long nx = (long long)B * H * W * Cin;
-  const long long colb = (long long)B * OH * OW * KH * KW * Cin * 4 + (1 << 20);
-  char* scratch = nullptr;
-  CU(cudaMalloc(&scratch, nx * 4 + colb + 4096));
-  Fwd F{&tmp, Arena{}, st, false, B};
-  F.ar.base = scratch; F.ar.cap = nx * 4 + colb + 4096;
-  SplitT A = F.salloc((long long)B * H * W, Cin);
-  int r = PF_OK;
-  {
-    cudaError_t le = (split_kernel<<<(unsigned)cdivl(nx, 256), 256, 0, st>>>(x, A.hi, A.lo, nx, in_relu), cudaGetLastError());
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    if (le != cudaSuccess) r = fail(PF_ERR_CUDA, "split_kernel: %s", cudaGetErrorString(le));
-  }
-  GemmW w{(const __nv_bfloat16*)whi, (const __nv_bfloat16*)wlo, bias};
+  const GemmW w{(const __nv_bfloat16*)whi, (const __nv_bfloat16*)wlo, bias};
   Fwd::Epi o;
   o.C = y; o.ldc = N; o.act = act; o.res = res; o.ldr = N; o.res_relu = res_relu;
-  if (r == PF_OK) {
-    if (KH == 3 && stride == 1 && pad == 1 && Cin % 64 == 0) r = F.thalo(A, 0, 0, nullptr, 0, 0, B, H, W, Cin, w, N, 1, 0, o);
-    else if (KH == 1 && stride == 1 && pad == 0) r = F.tgemm(A, (long long)B * H * W, Cin, 0, w, N, o);
-    else r = F.tconv_gather(A, B, H, W, Cin, KH, stride, pad, w, N, o);
-  }
-  cudaError_t se = cudaStreamSynchronize(st);
-  cudaFree(scratch);
-  if (r != PF_OK) return r;
-  if (se != cudaSuccess) return fail(PF_ERR_CUDA, "pf_op_conv_gemm: %s", cudaGetErrorString(se));
-  return PF_OK;
+  return op_run("pf_op_conv_gemm", B, stream, [&](Fwd& F) -> int {
+    const long long nx = (long long)B * H * W * Cin;
+    SplitT A = F.salloc((long long)B * H * W, Cin);
+    if (!F.dry) LAUNCHED((split_kernel<<<(unsigned)cdivl(nx, 256), 256, 0, F.st>>>(x, A.hi, A.lo, nx, in_relu), cudaGetLastError()));
+    if (KH == 3 && stride == 1 && pad == 1 && Cin % 64 == 0) return F.thalo(A, 0, 0, nullptr, 0, 0, B, H, W, Cin, w, N, 1, 0, o);
+    if (KH == 1 && stride == 1 && pad == 0) return F.tgemm(A, (long long)B * H * W, Cin, 0, w, N, o);
+    return F.tconv_gather(A, B, H, W, Cin, KH, stride, pad, w, N, o);
+  });
 }
 static int op_tma(pf_tma_op* op, void* stream, bool bf16) {
   if (!op || !op->a_hi || !op->a_lo || !op->w_hi || !op->w_lo) return fail(PF_ERR_ARG, "pf_op_tma: null argument");
@@ -1894,15 +957,8 @@ static int op_tma(pf_tma_op* op, void* stream, bool bf16) {
   if (q.mode == MODE_GEMM && (q.groups != 1 || q.a2_hi || q.phase4 || q.npred || q.M < 1 || q.M > INT32_MAX))
     return fail(PF_ERR_ARG, "pf_op_tma: GEMM mode runs one group of 1..2^31-1 rows without A2, phase4 or prediction tail");
   if (q.mode == MODE_HALO && (q.B < 1 || q.H < 1 || q.W < 1)) return fail(PF_ERR_ARG, "pf_op_tma: image size %dx%dx%d", q.B, q.H, q.W);
-  TRY(configure_current_device());
-  int dev = 0;
-  CU(cudaGetDevice(&dev));
-  cudaDeviceProp prop;
-  CU(cudaGetDeviceProperties(&prop, dev));
   pf_engine tmp;
-  tmp.device = dev;
-  tmp.sm_count = prop.multiProcessorCount;
-  tmp.bf16 = bf16;
+  TRY(op_engine(tmp, bf16));
   Fwd F{&tmp, Arena{}, (cudaStream_t)stream, false, q.B};
   if (q.force_sched < 0 || q.force_sched > 2 || (q.force_sched && q.mode != MODE_GEMM)) return fail(PF_ERR_ARG, "pf_op_tma: force_sched %d", q.force_sched);
   F.force_bn = q.force_bn; F.force_kb = q.force_kb; F.force_sched = q.force_sched;
@@ -1929,111 +985,6 @@ static int op_tma(pf_tma_op* op, void* stream, bool bf16) {
   if (r == PF_OK) { op->picked_bn = F.picked_bn; op->picked_kb = F.picked_kb; op->picked_sched = F.picked_sched; }
   return r;
 }
-}  // extern "C"
-
-// ParamNet backward pieces, one host helper of bwd_paramnet each: a temporary engine for the current device, scratch sized by a
-// dry run of the same body and filled with 0xFF bytes (NaN: a read of memory no kernel wrote poisons the result), a sync at the end.
-template <class Body>
-static int pn_op_run(const char* name, int n, void* stream, Body body) {
-  TRY(configure_current_device());
-  pf_engine tmp;
-  CU(cudaGetDevice(&tmp.device));
-  CU(cudaDeviceGetAttribute(&tmp.sm_count, cudaDevAttrMultiProcessorCount, tmp.device));
-  Fwd T{&tmp, Arena{}, nullptr, true, n};
-  T.ar.dry = true;
-  TRY(body(T));
-  const long long bytes = T.ar.peak + 4096;
-  cudaStream_t st = (cudaStream_t)stream;
-  char* scratch = nullptr;
-  CU(cudaMalloc(&scratch, bytes));
-  Fwd F{&tmp, Arena{}, st, false, n};
-  F.ar.base = scratch; F.ar.cap = bytes;
-  const cudaError_t me = cudaMemsetAsync(scratch, 0xFF, bytes, st);
-  int r = me == cudaSuccess ? body(F) : fail(PF_ERR_CUDA, "%s: %s", name, cudaGetErrorString(me));
-  const cudaError_t se = cudaStreamSynchronize(st);
-  cudaFree(scratch);
-  if (r == PF_OK && se != cudaSuccess) r = fail(PF_ERR_CUDA, "%s: %s", name, cudaGetErrorString(se));
-  return r;
-}
-static bool al16(const void* p) { return ((uintptr_t)p & 15) == 0; }
-
-extern "C" {
-
-int pf_op_pn_wgrad(const float* dy, int ldy, const float* x, const void* x_hi, const void* x_lo, int op, int ldx, int64_t R, int N, int K, float* out,
-                   int* S, int* chunk, void* stream) {
-  if (!dy || !out || !S || !chunk) return fail(PF_ERR_ARG, "pf_op_pn_wgrad: null argument");
-  if (!x_hi != !x_lo || !x == !x_hi) return fail(PF_ERR_ARG, "pf_op_pn_wgrad: the source is x or the pair x_hi / x_lo");
-  if ((op != 0 && op != 1) || (op == 1 && !x)) return fail(PF_ERR_ARG, "pf_op_pn_wgrad: op %d (1, the GELU, needs the fp32 source)", op);
-  if (R < 1 || R > INT32_MAX || N < 1 || K < 1 || ldy < N || ldx < K) return fail(PF_ERR_ARG, "pf_op_pn_wgrad: R %lld, N %d, K %d, ldy %d, ldx %d", (long long)R, N, K, ldy, ldx);
-  const SplitT xs{(__nv_bfloat16*)x_hi, (__nv_bfloat16*)x_lo, ldx};
-  WgPlan pl{};
-  const int r = pn_op_run("pf_op_pn_wgrad", 1, stream, [&](Fwd& F) { return pn_wgrad_full(F, dy, ldy, x ? nullptr : &xs, x, op, ldx, R, N, K, out, &pl); });
-  *S = pl.S;
-  *chunk = pl.chunk;
-  return r;
-}
-int pf_op_pn_colsum(const float* src, int64_t R, int C, float* out, void* stream) {
-  if (!src || !out || R < 1 || C < 1) return fail(PF_ERR_ARG, "pf_op_pn_colsum: bad argument");
-  return pn_op_run("pf_op_pn_colsum", 1, stream, [&](Fwd& F) { return pn_colsum(F, src, R, C, out); });
-}
-int pf_op_pn_ln_bwd(const float* x, const float* dy, int64_t R, int C, const float* w, float* dx, float* g, void* stream) {
-  if (!x || !dy || !w || !dx || !g) return fail(PF_ERR_ARG, "pf_op_pn_ln_bwd: null argument");
-  if (R < 1 || C < 32 || C > 768 || C % 32) return fail(PF_ERR_ARG, "pf_op_pn_ln_bwd: R %lld, C %d (a multiple of 32 up to 768)", (long long)R, C);
-  return pn_op_run("pf_op_pn_ln_bwd", 1, stream, [&](Fwd& F) { return pn_ln_bwd(F, x, dy, R, C, w, dx, g); });
-}
-int pf_op_pn_dw7_bwd(const float* x, const float* dt, int B, int H, int W, int C, const float* w_rot, float* dw, float* dx, int* rows_per_block, void* stream) {
-  if (!x || !dt || !w_rot || !dw || !dx) return fail(PF_ERR_ARG, "pf_op_pn_dw7_bwd: null argument");
-  if (!al16(x) || !al16(dt) || !al16(w_rot) || !al16(dx)) return fail(PF_ERR_ARG, "pf_op_pn_dw7_bwd: x, dt, w_rot and dx must be 16-byte aligned");
-  if (B < 1 || H < 1 || W < 1 || C < 32 || C % 32 || (long long)B * H * W * C > INT32_MAX)
-    return fail(PF_ERR_ARG, "pf_op_pn_dw7_bwd: B %d, H %d, W %d, C %d (a multiple of 32)", B, H, W, C);
-  return pn_op_run("pf_op_pn_dw7_bwd", B, stream, [&](Fwd& F) {
-    float* zero = F.ar.f(C);
-    if (!F.dry) CU(cudaMemsetAsync(zero, 0, (size_t)C * 4, F.st));
-    TRY(pn_dw7_wgrad(F, x, dt, H, W, C, dw, rows_per_block));
-    return pn_dw_launch(F, dt, dx, H, W, C, w_rot, zero);
-  });
-}
-int pf_op_pn_stem_bwd(const float* pin, const float* dS, const float* w, int B, int OH, int OW, float* dw, float* dpin, int* rows_per_block, void* stream) {
-  if (!pin || !dS || !w || !dw || !dpin) return fail(PF_ERR_ARG, "pf_op_pn_stem_bwd: null argument");
-  if (!al16(pin)) return fail(PF_ERR_ARG, "pf_op_pn_stem_bwd: pin must be 16-byte aligned");
-  if (B < 1 || OH < 1 || OW < 1) return fail(PF_ERR_ARG, "pf_op_pn_stem_bwd: B %d, OH %d, OW %d", B, OH, OW);
-  return pn_op_run("pf_op_pn_stem_bwd", B, stream, [&](Fwd& F) {
-    TRY(pn_stem_wgrad(F, pin, dS, OH, OW, dw, rows_per_block));
-    return pn_stem_dgrad(F, dS, w, OH, OW, dpin);
-  });
-}
-int pf_op_pn_fields_grad(const float* dpin, int B, int IH, int IW, int OH, int OW, float* dgrav, float* dlat, void* stream) {
-  if (!dpin || !dgrav || !dlat) return fail(PF_ERR_ARG, "pf_op_pn_fields_grad: null argument");
-  if (!al16(dpin)) return fail(PF_ERR_ARG, "pf_op_pn_fields_grad: dpin must be 16-byte aligned");
-  if (B < 1 || IH < 1 || IW < 1 || OH < 1 || OW < 1) return fail(PF_ERR_ARG, "pf_op_pn_fields_grad: B %d, %dx%d -> %dx%d", B, IH, IW, OH, OW);
-  return pn_op_run("pf_op_pn_fields_grad", B, stream, [&](Fwd& F) { return pn_fields_grad(F, dpin, IH, IW, OH, OW, dgrav, dlat); });
-}
-int pf_op_pn_tail_bwd(const float* feat, int n, int HW, const float* nw, const float* nb, const float* hw, const float* draw, float* dx, float* grads, void* stream) {
-  if (!feat || !nw || !nb || !hw || !draw || !dx || !grads) return fail(PF_ERR_ARG, "pf_op_pn_tail_bwd: null argument");
-  if (n < 1 || HW < 1) return fail(PF_ERR_ARG, "pf_op_pn_tail_bwd: n %d, HW %d", n, HW);
-  return pn_op_run("pf_op_pn_tail_bwd", n, stream, [&](Fwd& F) { return pn_tail_bwd(F, feat, HW, nw, nb, hw, draw, dx, grads); });
-}
-int pf_op_pn_pw2_grads(const float* G, const float* sdy, int C, int K, const float* gamma, const void* w_hi, const void* w_lo, const float* b, float* dW, float* db,
-                       float* dgamma, void* stream) {
-  if (!G || !sdy || !gamma || !w_hi || !w_lo || !b || !dW || !db || !dgamma) return fail(PF_ERR_ARG, "pf_op_pn_pw2_grads: null argument");
-  if (C < 1 || K < 1) return fail(PF_ERR_ARG, "pf_op_pn_pw2_grads: C %d, K %d", C, K);
-  const GemmW w2{(const __nv_bfloat16*)w_hi, (const __nv_bfloat16*)w_lo, b};
-  return pn_op_run("pf_op_pn_pw2_grads", 1, stream, [&](Fwd& F) { return pn_pw2_grads(F, G, sdy, C, K, gamma, w2, dW, db, dgamma); });
-}
-int pf_op_pn_gelu_bwd(const float* dh, float* u, int64_t n, void* hi, void* lo, void* stream) {
-  if (!dh || !u || n < 1 || !hi != !lo) return fail(PF_ERR_ARG, "pf_op_pn_gelu_bwd: bad argument");
-  return pn_op_run("pf_op_pn_gelu_bwd", 1, stream, [&](Fwd& F) { return pn_gelu_bwd(F, dh, u, n, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo); });
-}
-int pf_op_pn_scale_split(const float* src, const float* scale, int64_t n, int C, void* hi, void* lo, void* stream) {
-  if (!src || !hi || !lo || n < 1 || C < 1 || n % C) return fail(PF_ERR_ARG, "pf_op_pn_scale_split: bad argument");
-  const SplitT out{(__nv_bfloat16*)hi, (__nv_bfloat16*)lo, C};
-  return pn_op_run("pf_op_pn_scale_split", 1, stream, [&](Fwd& F) { return pn_scale_split(F, src, scale, n, C, out); });
-}
-int pf_op_pn_col2im2(const float* dP, int B, int H, int W, int C, float* out, void* stream) {
-  if (!dP || !out || B < 1 || H < 2 || W < 2 || H % 2 || W % 2 || C < 1) return fail(PF_ERR_ARG, "pf_op_pn_col2im2: bad argument");
-  return pn_op_run("pf_op_pn_col2im2", B, stream, [&](Fwd& F) { return pn_col2im2(F, dP, H, W, C, out); });
-}
-
 int pf_op_tma(pf_tma_op* op, void* stream) { return op_tma(op, stream, false); }
 int pf_op_tma_bf16(pf_tma_op* op, void* stream) { return op_tma(op, stream, true); }
 int pf_op_conv1_ring(const void* c_hi, const void* c_lo, int B, int H, int W, const float* wf, const float* bias, float* out,
@@ -2092,578 +1043,26 @@ int pf_camera_fields_vp(int device, const pf_camera* cams, const double* vp, int
   return PF_OK;
 }
 
-// PanoCam.crop_distortion (utils/panocam.py:559-752) for n views of one panorama: the host builds each view's rotation matrices
-// (:617-655), minimal focal length and disk (:592-594, :696-705) in float64 once; one launch per kPanoChunk views.
-int pf_pano_views(int device, const uint8_t* pano, int pano_h, int pano_w, const pf_pano_view* views, int n, uint8_t* im, float* ntheta,
-                  float* nphi, float* up, float* lat, float* xy, double* offset, int32_t* status, void* stream) {
-  if (!pano || !views || n < 1) return fail(PF_ERR_ARG, "pf_pano_views: null panorama / views or n < 1");
-  if (pano_h < 2 || pano_w < 2) return fail(PF_ERR_ARG, "pf_pano_views: panorama of %dx%d (needs at least 2x2)", pano_h, pano_w);
-  if (!im && !ntheta && !nphi && !up && !lat && !xy && !offset && !status) return fail(PF_ERR_ARG, "pf_pano_views: no output");
-  for (int i = 0; i < n; ++i) {
-    const pf_pano_view& c = views[i];
-    if (c.height < 1 || c.width < 1) return fail(PF_ERR_ARG, "pf_pano_views: view %d has size %dx%d", i, c.height, c.width);
-    if (!std::isfinite(c.f) || !(c.f > 0.0) || !std::isfinite(c.xi) || !std::isfinite(c.az) || !std::isfinite(c.el) || !std::isfinite(c.roll))
-      return fail(PF_ERR_ARG, "pf_pano_views: view %d: f must be finite and > 0, xi and the angles finite (f %g, xi %g)", i, c.f, c.xi);
-    if (c.im_offset < 0 || c.field_offset < 0) return fail(PF_ERR_ARG, "pf_pano_views: view %d has a negative offset", i);
-  }
-  CU(cudaSetDevice(device));
-  PanoMap m{};
-  m.Hp = pano_h; m.Wp = pano_w;
-  m.ax = (M_PI - -M_PI) / ((pano_w - 1.0) - 0);   // :680-687, python's own expressions
-  m.bx = M_PI - m.ax * (pano_w - 1.0);
-  m.iax = 1.0 / m.ax;
-  m.ay = (-M_PI / 2.0 - M_PI / 2.0) / ((pano_h - 1.0) - 0);
-  m.by = M_PI / 2.0 - m.ay * 0;
-  m.iay = 1.0 / m.ay;
-  auto rad = [](double deg) { return deg * M_PI / 180; };
-  for (int i0 = 0; i0 < n; i0 += kPanoChunk) {
-    const int cnt = n - i0 < kPanoChunk ? n - i0 : kPanoChunk;
-    PanoBatch b{};
-    long long max_px = 1;
-    for (int i = 0; i < cnt; ++i) {
-      const pf_pano_view& c = views[i0 + i];
-      PanoView& o = b.v[i];
-      o.H = c.height; o.W = c.width;
-      o.f = c.f; o.xi = c.xi; o.one_m_xi2 = 1 - c.xi * c.xi;
-      o.u0 = c.width / 2.0; o.v0 = c.height / 2.0;
-      const double ce = cos(rad(c.el)), se = sin(rad(c.el)), ca = cos(rad(c.az)), sa = sin(rad(c.az)), cr = cos(rad(c.roll)), sr = sin(rad(c.roll));
-      const double rel[9] = {1.0, 0.0, 0.0, 0.0, ce, -se, 0.0, se, ce};
-      const double raz[9] = {ca, 0.0, sa, 0.0, 1.0, 0.0, -sa, 0.0, ca};
-      const double rroll[9] = {cr, -sr, 0.0, sr, cr, 0.0, 0.0, 0.0, 1.0};
-      memcpy(o.rel, rel, sizeof rel); memcpy(o.raz, raz, sizeof raz); memcpy(o.rroll, rroll, sizeof rroll);
-      // minfocal(u0, v0, xi, 1, 1) (:64-70): NaN unless xi > 1, and f < NaN is false
-      const double fmin = sqrt(-(1 - c.xi * c.xi) * ((1 - o.u0) * (1 - o.u0) + (1 - o.v0) * (1 - o.v0))) * 1.0001;
-      o.masked = c.f < fmin;
-      const double r = sqrt(-(c.f * c.f) / (1 - c.xi * c.xi));   // diskradius (:18-19)
-      o.r2 = r * r;
-      o.ci0 = nearbyint(c.height / 2.0); o.ci1 = nearbyint(c.width / 2.0);   // np.round: half to even (the default rounding mode)
-      o.im_off = c.im_offset; o.fld_off = c.field_offset;
-      const long long px = (long long)c.height * c.width;
-      if (px > max_px) max_px = px;
-    }
-    const dim3 grid((unsigned)cdivl(max_px, (long long)kPanoThreads * kPanoPix) + 1, (unsigned)cnt);
-    LAUNCHED((pano_views_kernel<<<grid, kPanoThreads, 0, (cudaStream_t)stream>>>(b, m, pano, im, ntheta, nphi, up, lat, xy, offset, status, i0),
-              cudaGetLastError()));
-  }
-  return PF_OK;
-}
-
-// PanoCam.crop_equi / get_image (utils/panocam.py:121-249) for n views of one panorama: the host computes each view's fov_x
-// (:216-218, the wrapper's own expression), focal length and the sines and cosines of its angles once; one launch per kEquiChunk views.
-int pf_equi_views(int device, const void* pano, int pano_h, int pano_w, int channels, int dtype, const pf_equi_view* views, int n, int mode,
-                  int out_kind, int swap_rb, void* im, void* stream) {
-  if (!pano || !views || !im || n < 1) return fail(PF_ERR_ARG, "pf_equi_views: null panorama / views / im or n < 1");
-  if (pano_h < 1 || pano_w < 1) return fail(PF_ERR_ARG, "pf_equi_views: panorama of %dx%d", pano_h, pano_w);
-  if (channels != 1 && channels != 3) return fail(PF_ERR_ARG, "pf_equi_views: %d channels (1 or 3)", channels);
-  if (dtype != PF_EQUI_U8 && dtype != PF_EQUI_F32) return fail(PF_ERR_ARG, "pf_equi_views: unknown dtype %d", dtype);
-  if (mode != PF_EQUI_BILINEAR && mode != PF_EQUI_NEAREST) return fail(PF_ERR_ARG, "pf_equi_views: unknown mode %d", mode);
-  if (out_kind != PF_EQUI_CAST && out_kind != PF_EQUI_UNIT) return fail(PF_ERR_ARG, "pf_equi_views: unknown out_kind %d", out_kind);
-  if (out_kind == PF_EQUI_UNIT && dtype != PF_EQUI_U8) return fail(PF_ERR_ARG, "pf_equi_views: the unit path needs a uint8 panorama");
-  if (swap_rb != 0 && (swap_rb != 1 || channels != 3)) return fail(PF_ERR_ARG, "pf_equi_views: swap_rb must be 0, or 1 with 3 channels");
-  const int esize = dtype == PF_EQUI_F32 ? 4 : 1;
-  std::vector<double> fov_x(n);
-  for (int i = 0; i < n; ++i) {
-    const pf_equi_view& c = views[i];
-    if (c.height < 1 || c.width < 1) return fail(PF_ERR_ARG, "pf_equi_views: view %d has size %dx%d", i, c.height, c.width);
-    if (!std::isfinite(c.azimuth) || !std::isfinite(c.elevation) || !std::isfinite(c.roll))
-      return fail(PF_ERR_ARG, "pf_equi_views: view %d: non-finite angle", i);
-    if (!std::isfinite(c.vfov) || !(c.vfov > 0.0 && c.vfov < 180.0) || !std::isfinite(c.ar) || !(c.ar > 0.0))
-      return fail(PF_ERR_ARG, "pf_equi_views: view %d: vfov %g must lie in (0, 180) and ar %g be finite and > 0", i, c.vfov, c.ar);
-    fov_x[i] = 2 * atan(tan(c.vfov * M_PI / 180.0 / 2) * c.ar) * 180 / M_PI;
-    if (!(fov_x[i] > 0.0 && fov_x[i] < 180.0)) return fail(PF_ERR_ARG, "pf_equi_views: view %d: fov_x %g must lie in (0, 180)", i, fov_x[i]);
-    if (c.offset < 0 || c.offset % esize != 0) return fail(PF_ERR_ARG, "pf_equi_views: view %d: offset %lld (>= 0, a multiple of %d)", i,
-                                                          (long long)c.offset, esize);
-  }
-  CU(cudaSetDevice(device));
-  EquiMap m{};
-  m.Hp = pano_h; m.Wp = pano_w; m.C = channels;
-  m.nearest = mode == PF_EQUI_NEAREST; m.swap_rb = swap_rb;
-  m.su = pano_w / (2 * M_PI); m.sv = pano_h / M_PI;
-  for (int i0 = 0; i0 < n; i0 += kEquiChunk) {
-    const int cnt = n - i0 < kEquiChunk ? n - i0 : kEquiChunk;
-    EquiBatch b{};
-    long long max_px = 1;
-    for (int i = 0; i < cnt; ++i) {
-      const pf_equi_view& c = views[i0 + i];
-      EquiView& o = b.v[i];
-      o.H = c.height; o.W = c.width;
-      o.f = c.width / (2 * tan(fov_x[i0 + i] * M_PI / 180 / 2));
-      o.u0 = c.width / 2.0; o.v0 = c.height / 2.0;
-      const double roll = c.roll / 180 * M_PI, el = c.elevation / 180 * M_PI, az = c.azimuth / 180 * M_PI;   // the wrapper's rot dict
-      o.cr = cos(roll); o.sr = sin(roll); o.ce = cos(el); o.se = sin(el); o.ca = cos(az); o.sa = sin(az);
-      o.off = c.offset;
-      const long long px = (long long)c.height * c.width;
-      if (px > max_px) max_px = px;
-    }
-    const dim3 grid((unsigned)cdivl(max_px, (long long)kEquiThreads * kEquiPix), (unsigned)cnt);
-    cudaStream_t st = (cudaStream_t)stream;
-    unsigned char* out = (unsigned char*)im;
-    if (dtype == PF_EQUI_F32)
-      LAUNCHED((equi_views_kernel<float, false><<<grid, kEquiThreads, 0, st>>>(b, m, (const float*)pano, out), cudaGetLastError()));
-    else if (out_kind == PF_EQUI_UNIT)
-      LAUNCHED((equi_views_kernel<unsigned char, true><<<grid, kEquiThreads, 0, st>>>(b, m, (const unsigned char*)pano, out), cudaGetLastError()));
-    else
-      LAUNCHED((equi_views_kernel<unsigned char, false><<<grid, kEquiThreads, 0, st>>>(b, m, (const unsigned char*)pano, out), cudaGetLastError()));
-  }
-  return PF_OK;
-}
-
-// ----------------------------------------------------------------------------------------------- batched feature calls
-static long long align256(long long b) { return (b + 255) / 256 * 256; }
-
-// A caller-provided workspace carved into 256-byte-aligned sections, in the order they are added: at[k] is the byte offset of
-// section k; the first holds the per-image descriptors (upload_descriptors)
-struct WsLayout {
-  long long at[4] = {}, total = 0;
-  int count = 0;
-  WsLayout& add(long long bytes) { at[count++] = total; total += align256(bytes); return *this; }
-};
-
-static int check_workspace(const char* fn, const void* ws, int64_t bytes, long long need) {
-  if (bytes < need) return fail(PF_ERR_WORKSPACE, "%s: workspace %lld B < required %lld B", fn, (long long)bytes, need);
-  if (((uintptr_t)ws & 255) != 0) return fail(PF_ERR_ARG, "%s: workspace must be 256-byte aligned", fn);
-  return PF_OK;
-}
-
-static int upload_descriptors(const void* d, size_t bytes, void* ws, cudaStream_t st) {
-  CU(cudaMemcpyAsync(ws, d, bytes, cudaMemcpyHostToDevice, st));
-  return PF_OK;
-}
-
-// The per-image offset rule of the batched calls: a required offset is >= 0; an optional one is -1 (absent) or >= 0, and then
-// the buffer it points into must be given
-static int check_offsets(const char* fn, int i, std::initializer_list<long long> required,
-                         std::initializer_list<std::pair<long long, const void*>> optional = {}) {
-  for (const long long o : required)
-    if (o < 0) return fail(PF_ERR_ARG, "%s: image %d has a negative offset", fn, i);
-  for (const auto& [o, buf] : optional) {
-    if (o < -1) return fail(PF_ERR_ARG, "%s: image %d has a negative offset", fn, i);
-    if (o >= 0 && !buf) return fail(PF_ERR_ARG, "%s: image %d has an offset into a NULL buffer", fn, i);
-  }
-  return PF_OK;
-}
-
-// matplotlib's "seismic" map as the 256-entry table it samples (LinearSegmentedColormap.from_list: anchors at 0, 1/4, 1/2, 3/4, 1,
-// linear interpolation at i / 255), and t -> entry min(floor(256 t), 255); levels linspace(-pi/2, pi/2, 19).
-static DrawStyle draw_style() {
-  static const double anchors[5][3] = {{0.0, 0.0, 0.3}, {0.0, 0.0, 1.0}, {1.0, 1.0, 1.0}, {1.0, 0.0, 0.0}, {0.5, 0.0, 0.0}};
-  auto seismic = [&](double t, int ch) {
-    const int e = std::min((int)std::floor(256.0 * t), 255);
-    const double x = e / 255.0;
-    const int s = std::min((int)(x * 4.0), 3);
-    const double dist = (x - s / 4.0) / 0.25;
-    return 255.0 * (dist * (anchors[s + 1][ch] - anchors[s][ch]) + anchors[s][ch]);
-  };
-  DrawStyle st{};
-  const int nb = kDrawLevels - 1;
-  for (int k = 0; k < kDrawLevels; ++k) {
-    st.lev[k] = (float)(k == nb ? M_PI / 2 : -M_PI / 2 + k * (M_PI / nb));
-    for (int ch = 0; ch < 3; ++ch) {
-      st.line[k][ch] = (float)seismic((double)k / nb, ch);
-      if (k < nb) st.band[k][ch] = (float)seismic((k + 0.5) / nb, ch);
-    }
-  }
-  return st;
-}
-
-int pf_draw_fields(int device, const pf_draw_canvas* cs, int n, const uint8_t* img, uint8_t* out, const float* lat, const float* up, void* stream) {
-  if (!cs || n < 1 || !img || !out) return fail(PF_ERR_ARG, "pf_draw_fields: null canvases / img / out or n < 1");
-  auto unit = [](float x) { return std::isfinite(x) && x >= 0.f && x <= 1.f; };
-  for (int i = 0; i < n; ++i) {
-    const pf_draw_canvas& c = cs[i];
-    if (c.height < 1 || c.width < 1 || (long long)c.height * c.width >= (1LL << 31))
-      return fail(PF_ERR_ARG, "pf_draw_fields: canvas %d has size %dx%d", i, c.height, c.width);
-    TRY(check_offsets("pf_draw_fields", i, {c.img_offset, c.out_offset}));
-    if (!unit(c.alpha_fill) || !unit(c.alpha_line)) return fail(PF_ERR_ARG, "pf_draw_fields: canvas %d: alphas must lie in [0, 1]", i);
-    if (c.draw_lat && (!lat || c.lat_offset < 0)) return fail(PF_ERR_ARG, "pf_draw_fields: canvas %d draws the latitude without a latitude map", i);
-    if (c.draw_up) {
-      if (!up || c.up_offset < 0 || c.up_stride[0] < 0 || c.up_stride[1] < 0 || c.up_stride[2] < 0)
-        return fail(PF_ERR_ARG, "pf_draw_fields: canvas %d draws arrows without an up field, or with a negative offset / stride", i);
-      if (c.density < 1 || c.arrow_inv_len < 1 || c.width / c.density < 1 || c.height / c.density < 1)
-        return fail(PF_ERR_ARG, "pf_draw_fields: canvas %d (%dx%d): density %d and arrow_inv_len %d must be >= 1 and leave W // density, "
-                    "H // density >= 1", i, c.height, c.width, c.density, c.arrow_inv_len);
-      if (!unit(c.arrow_rgb[0]) || !unit(c.arrow_rgb[1]) || !unit(c.arrow_rgb[2])) return fail(PF_ERR_ARG, "pf_draw_fields: canvas %d: arrow colour outside [0, 1]", i);
-    }
-  }
-  CU(cudaSetDevice(device));
-  const DrawStyle st = draw_style();
-  for (int i0 = 0; i0 < n; i0 += kDrawChunk) {
-    const int cnt = n - i0 < kDrawChunk ? n - i0 : kDrawChunk;
-    DrawBatch b{};
-    long long max_tiles = 1;
-    for (int i = 0; i < cnt; ++i) {
-      const pf_draw_canvas& c = cs[i0 + i];
-      DrawCanvas& o = b.c[i];
-      o.H = c.height; o.W = c.width;
-      o.tiles_x = cdiv(c.width, kDrawTW);
-      o.draw_lat = c.draw_lat != 0; o.draw_up = c.draw_up != 0;
-      o.alpha_fill = c.alpha_fill; o.alpha_line = c.alpha_line;
-      o.img_off = c.img_offset; o.out_off = c.out_offset; o.lat_off = c.lat_offset; o.up_off = c.up_offset;
-      o.us_row = c.up_stride[0]; o.us_col = c.up_stride[1]; o.us_comp = c.up_stride[2];
-      if (o.draw_up) {
-        o.sx = c.width / c.density; o.sy = c.height / c.density;
-        o.nx = cdiv(c.width, o.sx); o.ny = cdiv(c.height, o.sy);
-        // np.sqrt(W^2 + H^2) // arrow_inv_len with Python's float floor division
-        const double diag = std::sqrt((double)c.width * c.width + (double)c.height * c.height), q = c.arrow_inv_len;
-        const double mod = std::fmod(diag, q), div = (diag - mod) / q;
-        double fl = std::floor(div);
-        if (div - fl > 0.5) fl += 1.0;
-        o.len = (float)fl;
-        const double sq = std::sqrt((double)o.nx * o.ny);                        // quiver's default width: 0.06 span / clip(sqrt(N), 8, 25)
-        o.w = (float)(0.06 * c.width / std::min(std::max(sq, 8.0), 25.0));
-        for (int ch = 0; ch < 3; ++ch) o.rgb[ch] = 255.f * c.arrow_rgb[ch];
-      }
-      const long long tiles = (long long)o.tiles_x * cdiv(c.height, kDrawTH);
-      if (tiles > max_tiles) max_tiles = tiles;
-    }
-    const dim3 grid((unsigned)max_tiles, (unsigned)cnt);
-    LAUNCHED((draw_fields_kernel<<<grid, kDrawThreads, 0, (cudaStream_t)stream>>>(b, st, img, out, lat, up), cudaGetLastError()));
-  }
-  return PF_OK;
-}
-
-// ----------------------------------------------------------------------------------------------- scoring (metrics.cuh)
-static bool gravity_classes_ok(int c) { return c == 2 || c >= 3; }
-static bool latitude_classes_ok(int c) { return c >= 1; }
-
-int pf_encode_fields(int device, int n, int H, int W, const float* up, const int64_t* up_stride, const float* lat, const int64_t* lat_stride,
-                     int lat_rad, int gravity_classes, int latitude_classes, void* gt_gravity, void* gt_latitude, void* stream) {
-  if (n < 1 || H < 1 || W < 1 || (long long)n * H * W >= (1LL << 40)) return fail(PF_ERR_ARG, "pf_encode_fields: bad batch %d x %d x %d", n, H, W);
-  if (!up && !lat) return fail(PF_ERR_ARG, "pf_encode_fields: neither an up nor a latitude field");
-  if (up && (!up_stride || !gt_gravity || !gravity_classes_ok(gravity_classes)))
-    return fail(PF_ERR_ARG, "pf_encode_fields: the up field needs strides, an output and gravity_classes 2 or >= 3 (got %d)", gravity_classes);
-  if (lat && (!lat_stride || !gt_latitude || !latitude_classes_ok(latitude_classes)))
-    return fail(PF_ERR_ARG, "pf_encode_fields: the latitude field needs strides, an output and latitude_classes >= 1 (got %d)", latitude_classes);
-  if (lat_rad != 0 && lat_rad != 1) return fail(PF_ERR_ARG, "pf_encode_fields: lat_rad must be 0 or 1");
-  EncodeArgs a{};
-  a.n = n; a.H = H; a.W = W; a.up = up; a.lat = lat; a.lat_rad = lat_rad; a.gc = gravity_classes; a.lc = latitude_classes;
-  a.gt_g = gt_gravity; a.gt_l = gt_latitude;
-  if (up) { a.us_img = up_stride[0]; a.us_row = up_stride[1]; a.us_col = up_stride[2]; a.us_comp = up_stride[3]; }
-  if (lat) { a.ls_img = lat_stride[0]; a.ls_row = lat_stride[1]; a.ls_col = lat_stride[2]; }
-  CU(cudaSetDevice(device));
-  const long long px = (long long)n * H * W;
-  LAUNCHED((encode_fields_kernel<<<(unsigned)cdivl(px, kMetThreads), kMetThreads, 0, (cudaStream_t)stream>>>(a), cudaGetLastError()));
-  return PF_OK;
-}
-
-// Blocks of the loss passes: classification (gravity, latitude) or regression (one pass over both heads)
-static void loss_blocks(int n, int H, int W, int gc, long long* bg, long long* bl) {
-  const long long px = (long long)n * H * W;
-  if (gc == 2) { *bg = cdivl(px, (long long)kMetThreads * kRegPix); *bl = 0; }
-  else { *bg = cdivl(px / kCePix, kMetThreads); *bl = *bg; }
-}
-int64_t pf_head_losses_workspace(int n, int H, int W, int gravity_classes, int latitude_classes) {
-  if (n < 1 || H < 1 || W < 1) return fail(PF_ERR_ARG, "pf_head_losses_workspace: bad batch %d x %d x %d", n, H, W);
-  if (!((gravity_classes == 2 && latitude_classes == 1) || (gravity_classes >= 3 && latitude_classes >= 2)))
-    return fail(PF_ERR_ARG, "pf_head_losses_workspace: heads %d / %d: both regression (2 / 1) or both classification", gravity_classes, latitude_classes);
-  long long bg, bl;
-  loss_blocks(n, H, W, gravity_classes, &bg, &bl);
-  return gravity_classes == 2 ? align256(bg * kRegSums * 8) + align256(bg * kRegCounts * 8) : align256((bg + bl) * 8) * 2;
-}
-
-int pf_head_losses(int device, int n, int H, int W, int gravity_classes, const float* pred_gravity, const void* gt_gravity, int latitude_classes,
-                   const float* pred_latitude, const void* gt_latitude, int gravity_ignore, int latitude_ignore, float gravity_weight,
-                   float latitude_weight, float* losses, void* workspace, int64_t workspace_bytes, void* stream) {
-  const int64_t need = pf_head_losses_workspace(n, H, W, gravity_classes, latitude_classes);
-  if (need < 0) return (int)need;
-  if (!pred_gravity || !gt_gravity || !pred_latitude || !gt_latitude || !losses || !workspace)
-    return fail(PF_ERR_ARG, "pf_head_losses: null prediction / target / losses / workspace");
-  TRY(check_workspace("pf_head_losses", workspace, workspace_bytes, need));
-  const bool cls = gravity_classes != 2;
-  if (cls && (((long long)H * W) % kCePix != 0 || ((uintptr_t)pred_gravity & 15) || ((uintptr_t)pred_latitude & 15)))
-    return fail(PF_ERR_ARG, "pf_head_losses: classification logits need H * W %% 4 == 0 and 16-byte aligned planes");
-  if (cls && ((long long)latitude_classes * H * W >= (1LL << 40))) return fail(PF_ERR_ARG, "pf_head_losses: logits too large");
-  CU(cudaSetDevice(device));
-  cudaStream_t st = (cudaStream_t)stream;
-  long long bg, bl;
-  loss_blocks(n, H, W, gravity_classes, &bg, &bl);
-  double* psum = (double*)workspace;
-  const int HW = H * W;
-  if (cls) {
-    long long* pcnt = (long long*)((char*)workspace + align256((bg + bl) * 8));
-    const CeHead g{pred_gravity, (const long long*)gt_gravity, gravity_classes, gravity_ignore, (int)bg};
-    const CeHead l{pred_latitude, (const long long*)gt_latitude, latitude_classes, latitude_ignore, (int)bl};
-    LAUNCHED((cross_entropy_kernel<<<(unsigned)(bg + bl), kMetThreads, 0, st>>>(g, l, n, HW, psum, pcnt), cudaGetLastError()));
-    LAUNCHED((loss_finish_kernel<<<1, kMetThreads, 0, st>>>(0, (int)bg, (int)(bg + bl), psum, pcnt, 0, gravity_weight, latitude_weight, losses),
-              cudaGetLastError()));
-  } else {
-    long long* pcnt = (long long*)((char*)workspace + align256(bg * kRegSums * 8));
-    const RegArgs a{pred_gravity, (const float*)gt_gravity, pred_latitude, (const float*)gt_latitude, n, H, W};
-    LAUNCHED((regression_loss_kernel<<<(unsigned)bg, kMetThreads, 0, st>>>(a, (int)bg, psum, pcnt), cudaGetLastError()));
-    LAUNCHED((loss_finish_kernel<<<1, kMetThreads, 0, st>>>(1, (int)bg, (int)bg, psum, pcnt, (long long)n * HW, gravity_weight, latitude_weight, losses),
-              cudaGetLastError()));
-  }
-  return PF_OK;
-}
-
-// Workspace layout of pf_field_errors: device descriptors | fp64 sums [2][blocks] | counts [2][1 + 8][blocks] | maps if not given
-static int field_errors_layout(const pf_field_image* im, int n, int with_maps, WsLayout* lay, long long* blocks_out = nullptr,
-                               long long* pixels_out = nullptr) {
-  if (!im || n < 1) return fail(PF_ERR_ARG, "pf_field_errors: null images or n < 1");
-  long long blocks = 0, pixels = 0;
-  for (int i = 0; i < n; ++i) {
-    if (im[i].height < 1 || im[i].width < 1 || (long long)im[i].height * im[i].width >= (1LL << 31))
-      return fail(PF_ERR_ARG, "pf_field_errors: image %d has size %dx%d", i, im[i].height, im[i].width);
-    const long long hw = (long long)im[i].height * im[i].width;
-    blocks += cdivl(hw, kFeTile);
-    pixels += hw;
-  }
-  if (blocks >= (1LL << 31)) return fail(PF_ERR_ARG, "pf_field_errors: too many pixels");
-  lay->add((long long)n * sizeof(FeImage)).add(2 * blocks * 8).add(2LL * (1 + kFeMaxThr) * blocks * 4).add(with_maps ? 0 : 2 * pixels * 4);
-  if (blocks_out) *blocks_out = blocks;
-  if (pixels_out) *pixels_out = pixels;
-  return PF_OK;
-}
-int64_t pf_field_errors_workspace(const pf_field_image* images, int n, int with_maps) {
-  WsLayout lay;
-  TRY(field_errors_layout(images, n, with_maps, &lay));
-  return lay.total;
-}
-
-int pf_field_errors(int device, const pf_field_image* images, int n, const float* pred_up, const float* pred_lat, const float* gt_up,
-                    const float* gt_lat, const uint8_t* mask, int lat_rad, const double* thresholds, int n_thresholds, float* up_maps,
-                    float* lat_maps, int64_t* count, double* mean, double* median, double* fraction, void* workspace,
-                    int64_t workspace_bytes, void* stream) {
-  if ((up_maps == nullptr) != (lat_maps == nullptr)) return fail(PF_ERR_ARG, "pf_field_errors: give both maps or neither");
-  WsLayout lay;
-  long long blocks, pixels;
-  TRY(field_errors_layout(images, n, up_maps != nullptr, &lay, &blocks, &pixels));
-  if (!pred_up || !pred_lat || !gt_up || !gt_lat || !count || !mean || !median || !workspace)
-    return fail(PF_ERR_ARG, "pf_field_errors: null field / output / workspace");
-  if (n_thresholds < 0 || n_thresholds > kFeMaxThr || (n_thresholds > 0 && (!thresholds || !fraction)))
-    return fail(PF_ERR_ARG, "pf_field_errors: %d thresholds (0 to %d, with a fraction output)", n_thresholds, kFeMaxThr);
-  for (int k = 0; k < n_thresholds; ++k)
-    if (std::isnan(thresholds[k])) return fail(PF_ERR_ARG, "pf_field_errors: threshold %d is NaN", k);
-  if (lat_rad != 0 && lat_rad != 1) return fail(PF_ERR_ARG, "pf_field_errors: lat_rad must be 0 or 1");
-  TRY(check_workspace("pf_field_errors", workspace, workspace_bytes, lay.total));
-  std::vector<FeImage> d(n);
-  long long block0 = 0, map_off = 0;
-  for (int i = 0; i < n; ++i) {
-    const pf_field_image& c = images[i];
-    TRY(check_offsets("pf_field_errors", i, {c.pred_up_offset, c.pred_lat_offset, c.gt_up_offset, c.gt_lat_offset}, {{c.mask_offset, mask}}));
-    FeImage& o = d[i];
-    o.H = c.height; o.W = c.width;
-    o.pu_off = c.pred_up_offset; o.pu_sr = c.pred_up_stride[0]; o.pu_sc = c.pred_up_stride[1]; o.pu_sk = c.pred_up_stride[2];
-    o.pl_off = c.pred_lat_offset;
-    o.gu_off = c.gt_up_offset; o.gu_sr = c.gt_up_stride[0]; o.gu_sc = c.gt_up_stride[1]; o.gu_sk = c.gt_up_stride[2];
-    o.gl_off = c.gt_lat_offset;
-    o.mask_off = c.mask_offset;
-    o.map_off = map_off;
-    const long long hw = (long long)c.height * c.width;
-    o.block0 = (int)block0; o.nblk = (int)cdivl(hw, kFeTile);
-    block0 += o.nblk; map_off += hw;
-  }
-  CU(cudaSetDevice(device));
-  cudaStream_t st = (cudaStream_t)stream;
-  char* ws = (char*)workspace;
-  FeArgs a{};
-  a.im = (const FeImage*)ws; a.n = n; a.nblocks = (int)blocks;
-  a.pu = pred_up; a.pl = pred_lat; a.gu = gt_up; a.gl = gt_lat; a.mask = mask;
-  a.lat_rad = lat_rad; a.T = n_thresholds;
-  for (int k = 0; k < n_thresholds; ++k) a.thr[k] = thresholds[k];
-  a.map_up = up_maps ? up_maps : (float*)(ws + lay.at[3]);
-  a.map_lat = lat_maps ? lat_maps : (float*)(ws + lay.at[3]) + pixels;
-  a.psum = (double*)(ws + lay.at[1]); a.pcnt = (int*)(ws + lay.at[2]);
-  TRY(upload_descriptors(d.data(), d.size() * sizeof(d[0]), ws, st));
-  LAUNCHED((field_errors_kernel<<<(unsigned)blocks, kMetThreads, 0, st>>>(a), cudaGetLastError()));
-  const FeOut o{(long long*)count, mean, median, fraction};
-  LAUNCHED((field_stats_kernel<<<dim3((unsigned)n, 2), kFeSelThreads, 0, st>>>(a, o), cudaGetLastError()));
-  return PF_OK;
-}
-
-// ----------------------------------------------------------------------------------------------- camera fit (calib.cuh)
-// Workspace layout of pf_fit_camera: device descriptors | per-image state | fp64 partials [kFitQ][pass blocks]
-constexpr int kFitMaxIterations = 1000;
-static int fit_layout(const pf_fit_image* im, int n, WsLayout* lay, long long* blocks_out = nullptr) {
-  if (!im || n < 1) return fail(PF_ERR_ARG, "pf_fit_camera: null images or n < 1");
-  long long blocks = 0;
-  for (int i = 0; i < n; ++i) {
-    if (im[i].height < 3 || im[i].width < 3 || (long long)im[i].height * im[i].width >= (1LL << 31))
-      return fail(PF_ERR_ARG, "pf_fit_camera: image %d has size %dx%d (3x3 at least)", i, im[i].height, im[i].width);
-    blocks += cdivl((long long)im[i].height * im[i].width, kFitTile);
-  }
-  if (blocks >= (1LL << 31)) return fail(PF_ERR_ARG, "pf_fit_camera: too many pixels");
-  lay->add((long long)n * sizeof(FitImage)).add((long long)n * sizeof(FitState)).add((long long)kFitQ * blocks * 8);
-  if (blocks_out) *blocks_out = blocks;
-  return PF_OK;
-}
-int64_t pf_fit_camera_workspace(const pf_fit_image* images, int n) {
-  WsLayout lay;
-  TRY(fit_layout(images, n, &lay));
-  return lay.total;
-}
-
-// Enables programmatic dependent launch for the calling thread while alive (the fit's kernels wait on their predecessor with
-// griddepcontrol.wait before their first global access)
-struct PdlScope {
-  explicit PdlScope(bool on) { pdl_enabled() = on; }
-  ~PdlScope() { pdl_enabled() = false; }
-};
-
-int pf_fit_camera(int device, const pf_fit_image* images, int n, const float* up_base, const float* lat_base, const uint8_t* mask_base,
-                  int principal_point, double huber, int max_iterations, double* params, double* cost, int32_t* iterations,
-                  int32_t* status, void* workspace, int64_t workspace_bytes, void* stream) {
-  WsLayout lay;
-  long long blocks;
-  TRY(fit_layout(images, n, &lay, &blocks));
-  if (!up_base || !lat_base || !params || !cost || !iterations || !status || !workspace)
-    return fail(PF_ERR_ARG, "pf_fit_camera: null field / output / workspace");
-  if (principal_point != 0 && principal_point != 1) return fail(PF_ERR_ARG, "pf_fit_camera: principal_point must be 0 or 1");
-  if (!(huber == 0.0 || (std::isfinite(huber) && huber > 0.0)))
-    return fail(PF_ERR_ARG, "pf_fit_camera: huber must be 0 (least squares) or finite and > 0, got %g", huber);
-  if (max_iterations < 1 || max_iterations > kFitMaxIterations)
-    return fail(PF_ERR_ARG, "pf_fit_camera: max_iterations %d outside 1 .. %d", max_iterations, kFitMaxIterations);
-  TRY(check_workspace("pf_fit_camera", workspace, workspace_bytes, lay.total));
-  std::vector<FitImage> d(n);
-  long long block0 = 0;
-  for (int i = 0; i < n; ++i) {
-    const pf_fit_image& c = images[i];
-    TRY(check_offsets("pf_fit_camera", i, {c.up_offset, c.lat_offset}, {{c.mask_offset, mask_base}}));
-    if (c.up_stride[0] < 0 || c.up_stride[1] < 0 || c.up_stride[2] < 0) return fail(PF_ERR_ARG, "pf_fit_camera: image %d has a negative stride", i);
-    if (!std::isnan(c.init[0])) {
-      bool fin = true;
-      for (int k = 0; k < 5; ++k) fin = fin && std::isfinite(c.init[k]);
-      if (!fin || !(c.init[2] > 0.0)) return fail(PF_ERR_ARG, "pf_fit_camera: image %d: init must be finite with f_rel > 0 (or a NaN roll)", i);
-    }
-    FitImage& o = d[i];
-    o.H = c.height; o.W = c.width;
-    o.up_off = c.up_offset; o.up_sr = c.up_stride[0]; o.up_sc = c.up_stride[1]; o.up_sk = c.up_stride[2];
-    o.lat_off = c.lat_offset;
-    o.mask_off = c.mask_offset;
-    for (int k = 0; k < 5; ++k) o.init[k] = c.init[k];
-    o.block0 = (int)block0; o.nblk = (int)cdivl((long long)c.height * c.width, kFitTile);
-    block0 += o.nblk;
-  }
-  CU(cudaSetDevice(device));
-  cudaStream_t st = (cudaStream_t)stream;
-  char* ws = (char*)workspace;
-  FitArgs a{};
-  a.im = (const FitImage*)ws; a.st = (FitState*)(ws + lay.at[1]); a.n = n; a.nblocks = (int)blocks;
-  a.up = up_base; a.lat = lat_base; a.mask = mask_base;
-  a.huber = huber; a.max_iter = max_iterations;
-  a.part = (double*)(ws + lay.at[2]);
-  a.params = params; a.cost = cost; a.iters = iterations; a.status = status;
-  TRY(upload_descriptors(d.data(), d.size() * sizeof(d[0]), ws, st));
-  const PdlScope pdl(!sync_debug());
-  const dim3 pass_grid((unsigned)blocks), step_grid((unsigned)cdiv(n, kFitStepWarps));
-  LAUNCHED(launch_pdl(fit_init_kernel, dim3(n), dim3(64), 0, st, a, principal_point));
-  for (int it = 0; it < max_iterations; ++it) {
-    if (principal_point) {
-      LAUNCHED(launch_pdl(fit_pass_kernel<5>, pass_grid, dim3(kFitThreads), 0, st, a));
-      LAUNCHED(launch_pdl(fit_step_kernel<5>, step_grid, dim3(32 * kFitStepWarps), 0, st, a));
-    } else {
-      LAUNCHED(launch_pdl(fit_pass_kernel<3>, pass_grid, dim3(kFitThreads), 0, st, a));
-      LAUNCHED(launch_pdl(fit_step_kernel<3>, step_grid, dim3(32 * kFitStepWarps), 0, st, a));
-    }
-  }
-  return PF_OK;
-}
-
-// ----------------------------------------------------------------------------------------------- upright warp (rectify.cuh)
-// Workspace layout of pf_rectify_views: device descriptors | per-image maps
-static int rectify_layout(const pf_rectify_image* im, int n, WsLayout* lay) {
-  if (!im || n < 1) return fail(PF_ERR_ARG, "pf_rectify_views: null images or n < 1");
-  if (n > 65535) return fail(PF_ERR_ARG, "pf_rectify_views: %d images (at most 65535 per call)", n);
-  for (int i = 0; i < n; ++i) {
-    const pf_rectify_image& c = im[i];
-    if (c.height < 1 || c.width < 1 || (long long)c.height * c.width >= (1LL << 31))
-      return fail(PF_ERR_ARG, "pf_rectify_views: image %d has input size %dx%d", i, c.height, c.width);
-    if (c.out_height < 1 || c.out_width < 1 || (long long)c.out_height * c.out_width >= (1LL << 31))
-      return fail(PF_ERR_ARG, "pf_rectify_views: image %d has output size %dx%d", i, c.out_height, c.out_width);
-  }
-  lay->add((long long)n * sizeof(RectImage)).add((long long)n * sizeof(RectMap));
-  return PF_OK;
-}
-int64_t pf_rectify_workspace(const pf_rectify_image* images, int n) {
-  WsLayout lay;
-  TRY(rectify_layout(images, n, &lay));
-  return lay.total;
-}
-
-int pf_rectify_views(int device, const pf_rectify_image* images, int n, const uint8_t* in_base, uint8_t* out_base, uint8_t* mask_base,
-                     float* map_base, int channels, const double* params, int keep_pitch, int focal_mode, double vfov, int sampler,
-                     const int32_t* fill, double* camera, int32_t* status, void* workspace, int64_t workspace_bytes, void* stream) {
-  WsLayout lay;
-  TRY(rectify_layout(images, n, &lay));
-  if (!in_base || !out_base || !params || !camera || !status || !workspace)
-    return fail(PF_ERR_ARG, "pf_rectify_views: null input / output / params / camera / status / workspace");
-  if (channels != 1 && channels != 3) return fail(PF_ERR_ARG, "pf_rectify_views: %d channels (1 or 3)", channels);
-  if (keep_pitch != 0 && keep_pitch != 1) return fail(PF_ERR_ARG, "pf_rectify_views: keep_pitch must be 0 or 1");
-  if (focal_mode != PF_RECTIFY_SAME && focal_mode != PF_RECTIFY_VFOV && focal_mode != PF_RECTIFY_FILL)
-    return fail(PF_ERR_ARG, "pf_rectify_views: unknown focal mode %d", focal_mode);
-  if (focal_mode == PF_RECTIFY_VFOV && !(std::isfinite(vfov) && vfov > 0.0 && vfov < 180.0))
-    return fail(PF_ERR_ARG, "pf_rectify_views: vfov %g must lie in (0, 180) degrees", vfov);
-  if (sampler != PF_RECTIFY_BILINEAR && sampler != PF_RECTIFY_NEAREST) return fail(PF_ERR_ARG, "pf_rectify_views: unknown sampler %d", sampler);
-  unsigned char fv[3] = {0, 0, 0};
-  for (int c = 0; fill && c < channels; ++c) {
-    if (fill[c] < 0 || fill[c] > 255) return fail(PF_ERR_ARG, "pf_rectify_views: fill[%d] = %d outside 0 .. 255", c, fill[c]);
-    fv[c] = (unsigned char)fill[c];
-  }
-  TRY(check_workspace("pf_rectify_views", workspace, workspace_bytes, lay.total));
-  std::vector<RectImage> d(n);
-  long long max_px = 1;
-  for (int i = 0; i < n; ++i) {
-    const pf_rectify_image& c = images[i];
-    TRY(check_offsets("pf_rectify_views", i, {c.in_offset, c.out_offset}, {{c.mask_offset, mask_base}, {c.map_offset, map_base}}));
-    RectImage& o = d[i];
-    o.H = c.height; o.W = c.width; o.Ho = c.out_height; o.Wo = c.out_width;
-    o.in_off = c.in_offset; o.out_off = c.out_offset; o.mask_off = c.mask_offset; o.map_off = c.map_offset;
-    max_px = std::max(max_px, (long long)c.out_height * c.out_width);
-  }
-  if (cdivl(max_px, (long long)kRectThreads * kRectPix) >= (1LL << 31)) return fail(PF_ERR_ARG, "pf_rectify_views: output too large");
-  CU(cudaSetDevice(device));
-  cudaStream_t st = (cudaStream_t)stream;
-  char* ws = (char*)workspace;
-  RectArgs a{};
-  a.im = (const RectImage*)ws; a.map = (RectMap*)(ws + lay.at[1]); a.n = n;
-  a.params = params; a.camera = camera; a.status = status;
-  a.keep_pitch = keep_pitch; a.focal_mode = focal_mode; a.vfov = vfov;
-  a.in = in_base; a.out = out_base; a.mask = mask_base; a.xy = map_base;
-  for (int c = 0; c < 3; ++c) a.fill[c] = fv[c];
-  TRY(upload_descriptors(d.data(), d.size() * sizeof(d[0]), ws, st));
-  const PdlScope pdl(!sync_debug());
-  LAUNCHED(launch_pdl(rectify_setup_kernel, dim3((unsigned)cdiv(n, 128)), dim3(128), 0, st, a));
-  const dim3 grid((unsigned)cdivl(max_px, (long long)kRectThreads * kRectPix), (unsigned)n);
-  const bool nearest = sampler == PF_RECTIFY_NEAREST;
-  if (channels == 3)
-    LAUNCHED(nearest ? launch_pdl(rectify_warp_kernel<3, true>, grid, dim3(kRectThreads), 0, st, a)
-                     : launch_pdl(rectify_warp_kernel<3, false>, grid, dim3(kRectThreads), 0, st, a));
-  else
-    LAUNCHED(nearest ? launch_pdl(rectify_warp_kernel<1, true>, grid, dim3(kRectThreads), 0, st, a)
-                     : launch_pdl(rectify_warp_kernel<1, false>, grid, dim3(kRectThreads), 0, st, a));
-  return PF_OK;
-}
-
-static int upload_table(const ResampleTable& t, int** bounds, int** coeffs) {
-  CU(cudaMalloc(bounds, t.bounds.size() * 4));
-  CU(cudaMalloc(coeffs, t.coeffs.size() * 4));
-  CU(cudaMemcpy(*bounds, t.bounds.data(), t.bounds.size() * 4, cudaMemcpyHostToDevice));
-  CU(cudaMemcpy(*coeffs, t.coeffs.data(), t.coeffs.size() * 4, cudaMemcpyHostToDevice));
-  return PF_OK;
-}
 int pf_op_resize_u8(const uint8_t* img, int H, int W, int new_h, int new_w, uint8_t* out, void* stream) {
   if (!img || !out || H < 1 || W < 1 || new_h < 1 || new_w < 1) return fail(PF_ERR_ARG, "pf_op_resize_u8: bad argument");
-  cudaStream_t st = (cudaStream_t)stream;
   if (H == new_h && W == new_w) {   // Pillow returns a copy when the size does not change
-    CU(cudaMemcpyAsync(out, img, (size_t)H * W * 3, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(out, img, (size_t)H * W * 3, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
     return PF_OK;
   }
-  ResampleTable tx = make_resample_table(W, new_w), ty = make_resample_table(H, new_h);
-  int *bx = nullptr, *cx = nullptr, *by = nullptr, *cy = nullptr;
-  unsigned char* tmp = nullptr;
-  int r = upload_table(tx, &bx, &cx);
-  if (r == PF_OK) r = upload_table(ty, &by, &cy);
-  if (r == PF_OK && cudaMalloc(&tmp, (size_t)H * new_w * 3) != cudaSuccess) r = fail(PF_ERR_CUDA, "pf_op_resize_u8: cudaMalloc");
-  if (r == PF_OK) {
+  const ResampleTable tx = make_resample_table(W, new_w), ty = make_resample_table(H, new_h);
+  return op_run("pf_op_resize_u8", 1, stream, [&](Fwd& F) -> int {
+    int *bx, *cx, *by, *cy;
+    TRY(op_upload(F, tx.bounds.data(), tx.bounds.size(), &bx));
+    TRY(op_upload(F, tx.coeffs.data(), tx.coeffs.size(), &cx));
+    TRY(op_upload(F, ty.bounds.data(), ty.bounds.size(), &by));
+    TRY(op_upload(F, ty.coeffs.data(), ty.coeffs.size(), &cy));
+    unsigned char* tmp = (unsigned char*)F.ar.alloc((long long)H * new_w * 3);
+    if (F.dry) return PF_OK;
     // Pillow runs the horizontal pass first (over the rows the vertical pass needs: all of them here), each pass rounded to uint8
-    cudaError_t le = (resize_u8_h_kernel<<<(unsigned)cdivl((long long)H * new_w, 256), 256, 0, st>>>(img, H, W, new_w, bx, cx, tx.ksize, tmp), cudaGetLastError());
-    if (le == cudaSuccess) le = (resize_u8_v_kernel<<<(unsigned)cdivl((long long)new_h * new_w, 256), 256, 0, st>>>(tmp, H, new_w, new_h, by, cy, ty.ksize, out), cudaGetLastError());
-    g_launches.fetch_add(2, std::memory_order_relaxed);
-    if (le == cudaSuccess) le = cudaStreamSynchronize(st);
-    if (le != cudaSuccess) r = fail(PF_ERR_CUDA, "pf_op_resize_u8: %s", cudaGetErrorString(le));
-  }
-  cudaFree(bx); cudaFree(cx); cudaFree(by); cudaFree(cy); cudaFree(tmp);
-  return r;
+    LAUNCHED((resize_u8_h_kernel<<<(unsigned)cdivl((long long)H * new_w, 256), 256, 0, F.st>>>(img, H, W, new_w, bx, cx, tx.ksize, tmp), cudaGetLastError()));
+    LAUNCHED((resize_u8_v_kernel<<<(unsigned)cdivl((long long)new_h * new_w, 256), 256, 0, F.st>>>(tmp, H, new_w, new_h, by, cy, ty.ksize, out), cudaGetLastError()));
+    return PF_OK;
+  });
 }
 int pf_op_resize_f32(const float* img, int H, int W, int C, int new_h, int new_w, float* out, void* stream) {
   if (!img || !out || H < 1 || W < 1 || C < 1 || new_h < 1 || new_w < 1) return fail(PF_ERR_ARG, "pf_op_resize_f32: bad argument");
@@ -2685,8 +1084,6 @@ int pf_op_pred_argmax_decode(const float* feat, int ld, int coff, const float* w
 int pf_op_postprocess(const float* vec, const float* lat, int n, const int32_t* height, const int32_t* width, float* gravity_original,
                       const int64_t* gravity_original_offset, float* latitude_original, const int64_t* latitude_original_offset, int lat_is_sin,
                       void* stream) {
-  if (!vec || !lat || n < 1 || !height || !width || !gravity_original || !gravity_original_offset || !latitude_original || !latitude_original_offset)
-    return fail(PF_ERR_ARG, "pf_op_postprocess: bad argument");
   return pf_op_postprocess_sized(vec, lat, n, kNet, kNet, height, width, gravity_original, gravity_original_offset, latitude_original, latitude_original_offset,
                                  lat_is_sin, stream);
 }
@@ -2696,15 +1093,12 @@ int pf_op_postprocess_sized(const float* vec, const float* lat, int n, int net_h
   if (!vec || !lat || n < 1 || !height || !width || !gravity_original || !gravity_original_offset || !latitude_original || !latitude_original_offset)
     return fail(PF_ERR_ARG, "pf_op_postprocess: bad argument");
   if (!net_size_ok(net_h, net_w)) return fail(PF_ERR_ARG, "pf_op_postprocess: unsupported working size %dx%d", net_h, net_w);
-  TRY(configure_current_device());
-  PostImage* d_post = nullptr;
-  CU(cudaMalloc(&d_post, n * sizeof(PostImage)));
-  int r = launch_postprocess(vec, lat, n, net_h, net_w, height, width, gravity_original_offset, latitude_original_offset, gravity_original, latitude_original,
-                             lat_is_sin, d_post, (cudaStream_t)stream);
-  cudaError_t se = cudaStreamSynchronize((cudaStream_t)stream);
-  cudaFree(d_post);
-  if (r == PF_OK && se != cudaSuccess) r = fail(PF_ERR_CUDA, "pf_op_postprocess: %s", cudaGetErrorString(se));
-  return r;
+  return op_run("pf_op_postprocess", n, stream, [&](Fwd& F) -> int {
+    PostImage* d_post = (PostImage*)F.ar.alloc((long long)n * sizeof(PostImage));
+    if (F.dry) return PF_OK;
+    return launch_postprocess(vec, lat, n, net_h, net_w, height, width, gravity_original_offset, latitude_original_offset, gravity_original,
+                              latitude_original, lat_is_sin, d_post, F.st);
+  });
 }
 
 int pf_op_fill_stream(float* dst, int64_t numel, float value, void* stream) {
@@ -2719,37 +1113,16 @@ int pf_op_layernorm(const float* x, float* y, int64_t rows, int C, const float* 
 static int op_attention_tc(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream, int np, int nkv = kAmKeys) {
   if (!q || !kv || !out || C != heads * kAmD) return fail(PF_ERR_ARG, "pf_op_attention_tc: head_dim must be 64");
   if (B < 1 || N < 1 || nkv < 1 || nkv > kAmMaxKeys) return fail(PF_ERR_ARG, "pf_op_attention_tc: B %d, N %d, %d keys (1..%d)", B, N, nkv, kAmMaxKeys);
-  TRY(configure_current_device());
-  cudaStream_t st = (cudaStream_t)stream;
-  int dev = 0;
-  CU(cudaGetDevice(&dev));
-  cudaDeviceProp prop;
-  CU(cudaGetDeviceProperties(&prop, dev));
-  pf_engine tmp;
-  tmp.device = dev;
-  tmp.sm_count = prop.multiProcessorCount;
-  const long long nq = (long long)B * N * C, nkve = (long long)B * nkv * 2 * C;
-  char* scratch = nullptr;
-  CU(cudaMalloc(&scratch, (2 * nq + nkve) * 4 + 8192));
-  Fwd F{&tmp, Arena{}, st, false, B};
-  F.ar.base = scratch; F.ar.cap = (2 * nq + nkve) * 4 + 8192;
-  SplitT qs = F.salloc((long long)B * N, C), kvs = F.salloc((long long)B * nkv, 2 * C), as = F.salloc((long long)B * N, C);
-  int r = PF_OK;
-  cudaError_t le = (split_kernel<<<(unsigned)cdivl(nq, 256), 256, 0, st>>>(q, qs.hi, qs.lo, nq, 0), cudaGetLastError());
-  if (le == cudaSuccess) le = (split_kernel<<<(unsigned)cdivl(nkve, 256), 256, 0, st>>>(kv, kvs.hi, kvs.lo, nkve, 0), cudaGetLastError());
-  if (le != cudaSuccess) r = fail(PF_ERR_CUDA, "split_kernel: %s", cudaGetErrorString(le));
-  if (r == PF_OK) {
-    le = attention_mma_launch(nullptr, B, N, C, heads, st, as, qs, kvs, np, nkv);
-    if (le != cudaSuccess) r = fail(PF_ERR_CUDA, "attention_mma_launch: %s", cudaGetErrorString(le));
-  }
-  if (r == PF_OK) {
-    le = (merge_split_kernel<<<(unsigned)cdivl(nq, 256), 256, 0, st>>>(as.hi, as.lo, out, nq), cudaGetLastError());
-    if (le != cudaSuccess) r = fail(PF_ERR_CUDA, "merge_split_kernel: %s", cudaGetErrorString(le));
-  }
-  cudaError_t se = cudaStreamSynchronize(st);
-  cudaFree(scratch);
-  if (r == PF_OK && se != cudaSuccess) r = fail(PF_ERR_CUDA, "pf_op_attention_tc: %s", cudaGetErrorString(se));
-  return r;
+  return op_run("pf_op_attention_tc", B, stream, [&](Fwd& F) -> int {
+    const long long nq = (long long)B * N * C, nkve = (long long)B * nkv * 2 * C;
+    SplitT qs = F.salloc((long long)B * N, C), kvs = F.salloc((long long)B * nkv, 2 * C), as = F.salloc((long long)B * N, C);
+    if (F.dry) return PF_OK;
+    LAUNCHED((split_kernel<<<(unsigned)cdivl(nq, 256), 256, 0, F.st>>>(q, qs.hi, qs.lo, nq, 0), cudaGetLastError()));
+    LAUNCHED((split_kernel<<<(unsigned)cdivl(nkve, 256), 256, 0, F.st>>>(kv, kvs.hi, kvs.lo, nkve, 0), cudaGetLastError()));
+    LAUNCHED(attention_mma_launch(nullptr, B, N, C, heads, F.st, as, qs, kvs, np, nkv));
+    LAUNCHED((merge_split_kernel<<<(unsigned)cdivl(nq, 256), 256, 0, F.st>>>(as.hi, as.lo, out, nq), cudaGetLastError()));
+    return PF_OK;
+  });
 }
 int pf_op_attention_tc(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream) {
   return op_attention_tc(q, kv, out, B, N, C, heads, stream, 3);
@@ -2781,31 +1154,26 @@ int pf_op_preprocess(const uint8_t* img, int H, int W, const float* mean3, const
 int pf_op_preprocess_sized(const uint8_t* img, int H, int W, int net_h, int net_w, const float* mean3, const float* std3, float* y, void* stream) {
   if (!img || !mean3 || !std3 || !y || H < 1 || W < 1) return fail(PF_ERR_ARG, "pf_op_preprocess: bad argument");
   if (!net_size_ok(net_h, net_w)) return fail(PF_ERR_ARG, "pf_op_preprocess: unsupported working size %dx%d", net_h, net_w);
-  TRY(configure_current_device());
   // standalone tables (not cached): test entry point only
-  ResampleTable tx = make_resample_table(W, net_w), ty = make_resample_table(H, net_h);
+  const ResampleTable tx = make_resample_table(W, net_w), ty = make_resample_table(H, net_h);
   const int max_rows = pre_max_smem_rows(net_w);
   if (ty.ksize + 1 > max_rows) return fail(PF_ERR_ARG, "image too tall");
-  int *bx, *cx, *by, *cy;
-  PreImage* d;
-  CU(cudaMalloc(&bx, tx.bounds.size() * 4)); CU(cudaMalloc(&cx, tx.coeffs.size() * 4));
-  CU(cudaMalloc(&by, ty.bounds.size() * 4)); CU(cudaMalloc(&cy, ty.coeffs.size() * 4));
-  CU(cudaMalloc(&d, sizeof(PreImage)));
-  CU(cudaMemcpy(bx, tx.bounds.data(), tx.bounds.size() * 4, cudaMemcpyHostToDevice));
-  CU(cudaMemcpy(cx, tx.coeffs.data(), tx.coeffs.size() * 4, cudaMemcpyHostToDevice));
-  CU(cudaMemcpy(by, ty.bounds.data(), ty.bounds.size() * 4, cudaMemcpyHostToDevice));
-  CU(cudaMemcpy(cy, ty.coeffs.data(), ty.coeffs.size() * 4, cudaMemcpyHostToDevice));
-  PreImage pi{0, H, W, tx.ksize, ty.ksize, bx, cx, by, cy};
-  CU(cudaMemcpy(d, &pi, sizeof pi, cudaMemcpyHostToDevice));
-  int rows = pre_rows_needed(H, net_h);
-  if (rows > max_rows) rows = max_rows;
-  const int smem = rows * net_w * 3;
-  LAUNCHED((preprocess_kernel<<<dim3(net_h / kPreRows, 1), net_w, smem, (cudaStream_t)stream>>>(img, d, y, mean3[0], mean3[1], mean3[2], std3[0], std3[1], std3[2], rows,
-                                                                                                 net_h, net_w),
-            cudaGetLastError()));
-  CU(cudaStreamSynchronize((cudaStream_t)stream));
-  cudaFree(bx); cudaFree(cx); cudaFree(by); cudaFree(cy); cudaFree(d);
-  return PF_OK;
+  const int rows = std::min(pre_rows_needed(H, net_h), max_rows);
+  return op_run("pf_op_preprocess", 1, stream, [&](Fwd& F) -> int {
+    int *bx, *cx, *by, *cy;
+    TRY(op_upload(F, tx.bounds.data(), tx.bounds.size(), &bx));
+    TRY(op_upload(F, tx.coeffs.data(), tx.coeffs.size(), &cx));
+    TRY(op_upload(F, ty.bounds.data(), ty.bounds.size(), &by));
+    TRY(op_upload(F, ty.coeffs.data(), ty.coeffs.size(), &cy));
+    const PreImage pi{0, H, W, tx.ksize, ty.ksize, bx, cx, by, cy};
+    PreImage* d;
+    TRY(op_upload(F, &pi, 1, &d));
+    if (F.dry) return PF_OK;
+    LAUNCHED((preprocess_kernel<<<dim3(net_h / kPreRows, 1), net_w, rows * net_w * 3, F.st>>>(img, d, y, mean3[0], mean3[1], mean3[2], std3[0], std3[1], std3[2],
+                                                                                         rows, net_h, net_w),
+              cudaGetLastError()));
+    return PF_OK;
+  });
 }
 
 }  // extern "C"

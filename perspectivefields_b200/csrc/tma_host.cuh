@@ -1,5 +1,6 @@
-// Host side of the TMA engine: tensor-map construction (cuTensorMapEncodeTiled through the runtime's driver entry point,
-// so libcuda is not linked) and the launcher of gemm_tma_kernel.
+// Host side of the TMA engine: the launch parameters it shares with gemm_tma_kernel (gemm_tma.cuh), tensor-map construction
+// (cuTensorMapEncodeTiled through the runtime's driver entry point, so libcuda is not linked), the tile pickers, the list of
+// instantiations and the launcher, which gemm_tma.cu compiles together with the kernel.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -7,9 +8,41 @@
 #include <cstdlib>
 #include <string>
 
-#include "gemm_tma.cuh"
+#include "tc_ptx.cuh"
 
 namespace pf {
+
+constexpr int MODE_GEMM = 0, MODE_HALO = 1;
+
+struct TmaGemmParams {
+  int M;                    // MODE_GEMM: rows
+  int B, H, W;              // MODE_HALO: images, spatial size (output == input)
+  int Cin;                  // MODE_HALO: input channels per group (multiple of 64);  MODE_GEMM: K
+  int N, K;
+  int a_c0, a_gc;           // channel coordinate of the first input channel in A's tensor map, step per group
+  int c_split, a2_c0;       // MODE_HALO dual source: input channels >= c_split come from the A2 maps at a2_c0 + (ci - c_split); 0 = off
+  int groups;
+  int b_row0;               // first row of this launch's weights in the B tensor map (resident-weight launches fold the group in)
+  // epilogue:  v = acc + bias;  v = act(v);  v *= gamma;  v += relu?(res);  v += res2
+  const float* bias; int bias_mode, bias_gstride;
+  int act; const float* gamma;
+  const float* res;  int ldr, r_coff, r_gcoff, res_relu;
+  const float* res2; int ldr2, r2_coff, r2_gcoff;
+  float* C; int ldc, c_coff, c_gcoff;                                           // fp32 output (may be null)
+  __nv_bfloat16* Shi; __nv_bfloat16* Slo; int lds, s_coff, s_gcoff, split_relu; // split output (may be null)
+  // MODE_HALO, N = 32 (conv_fuse_conv1): fused prediction tail -- 1x1 conv 32 -> pred_nc (gravity_head.py:175 /
+  // latitude_head.py:174) + F.normalize (pred_mode 1, gravity_head.py:192-193) or clamp to [-1,1] (pred_mode 2,
+  // latitude_head.py:191-192), written NCHW to pred_out; replaces the separate pred_tail_kernel pass over conv1's output
+  const float* pred_w; const float* pred_b; float* pred_out; int pred_nc, pred_mode;
+  // MODE_HALO, N = BN = 128: the four 32-column chunks are the four output phases (py, px) of a convolution composed with the
+  // bilinear x2 upsample in front of it (weights.py:_compose_up2_conv3): chunk ph, low-res pixel (y, x) -> pixel
+  // (2y + ph/2, 2x + ph%2) of the 2H x 2W output, 32 channels.  C / S / the prediction tail are addressed on that grid.
+  int phase4;
+};
+
+struct TmaMaps {   // passed by value as a __grid_constant__ kernel parameter
+  CUtensorMap a_hi, a_lo, a2_hi, a2_lo, b_hi, b_lo;
+};
 
 typedef CUresult (*PFN_tensorMapEncodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                              const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -112,39 +145,8 @@ inline bool tma_pick_pingpong(long long M, int N, int K, int bn, int sm_count) {
 
 struct PredTail { const float* w; const float* b; float* out; int nc, mode; };   // per group, see TmaGemmParams::pred_*
 
-template <int BN, int MODE, int KB, bool PP = false, int NP = 3>
-inline cudaError_t gemm_tma_launch_bn(const TmaMaps& maps, const TmaGemmParams& p, int sm_count, cudaStream_t st, const PredTail* pred) {
-  using Cfg = TmaCfg<BN, MODE, KB, PP, NP>;   // (the > 48 KB shared-memory opt-in is per device: gemm_tma_configure_device, at pf_create)
-  const int tiles_x = MODE == MODE_HALO ? cdiv(p.W, kHtTileW) : 0, tiles_y = MODE == MODE_HALO ? cdiv(p.H, kHtTileH) : 0;
-  const long long m_tiles = MODE == MODE_GEMM ? cdiv(p.M, Cfg::kTileM) : (long long)p.B * tiles_x * tiles_y;
-  const long long total = m_tiles * cdiv(p.N, BN) * p.groups;
-  const unsigned grid = (unsigned)(total < sm_count ? total : sm_count);
-  // resident-weight mode (single chunk, one N tile) assumes every tile of a CTA uses the same weights: one group per launch
-  // (a fused prediction tail is per group as well: same decomposition)
-  if (MODE == MODE_HALO && ((p.Cin == 64 && 9 * (64 / KB) <= Cfg::kStages && (p.groups > 1 || cdiv(p.N, BN) > 1)) || pred)) {
-    cudaError_t last = cudaSuccess;
-    for (int g = 0; g < p.groups; ++g)
-      for (int nt = 0; nt < cdiv(p.N, BN); ++nt) {
-        TmaGemmParams q = p;     // fold group g / N tile nt into the offsets of a single-group, single-tile launch
-        q.groups = 1;
-        q.a_c0 = p.a_c0 + g * p.a_gc;
-        q.bias = p.bias ? p.bias + (long long)g * p.bias_gstride : nullptr;
-        q.c_coff = p.c_coff + g * p.c_gcoff; q.s_coff = p.s_coff + g * p.s_gcoff;
-        q.r_coff = p.r_coff + g * p.r_gcoff; q.r2_coff = p.r2_coff + g * p.r2_gcoff;
-        q.b_row0 = g * p.N;
-        if (pred) { q.pred_w = pred[g].w; q.pred_b = pred[g].b; q.pred_out = pred[g].out; q.pred_nc = pred[g].nc; q.pred_mode = pred[g].mode; }
-        if (cdiv(p.N, BN) > 1) return cudaErrorInvalidValue;   // (not needed by the network: conv_fuse_conv1 has one N tile)
-        const unsigned gr = (unsigned)(m_tiles < sm_count ? m_tiles : sm_count);
-        last = launch_pdl(gemm_tma_kernel<BN, MODE, KB, false, NP>, dim3(gr), dim3(kTmaThreads), Cfg::kSmemBytes, st, maps, q, tiles_x, tiles_y);
-        if (last != cudaSuccess) return last;
-      }
-    return last;
-  }
-  return launch_pdl(gemm_tma_kernel<BN, MODE, KB, PP, NP>, dim3(grid), dim3(kTmaThreads), Cfg::kSmemBytes, st, maps, p, tiles_x, tiles_y);
-}
-
-// every instantiation the dispatcher below can reach: X(BN, MODE, KB).  Each one exists with three products and with one (the
-// bf16 precision mode picks the same tiles).
+// every instantiation the dispatcher (gemm_tma_launch) can reach: X(BN, MODE, KB).  Each one exists with three products and
+// with one (the bf16 precision mode picks the same tiles).
 #define PF_TMA_VARIANTS(X)                                                                                                  \
   X(256, MODE_GEMM, 32) X(224, MODE_GEMM, 32) X(192, MODE_GEMM, 32) X(160, MODE_GEMM, 32) X(128, MODE_GEMM, 32) X(96, MODE_GEMM, 32) \
   X(64, MODE_GEMM, 32) X(32, MODE_GEMM, 32) X(64, MODE_GEMM, 64) X(32, MODE_GEMM, 64)                                        \
@@ -155,70 +157,13 @@ inline cudaError_t gemm_tma_launch_bn(const TmaMaps& maps, const TmaGemmParams& 
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a per-device (per-context) attribute: called once for every device an engine is
 // created on (pf_create) and every product count np (3 or 1) -- not behind a process-wide flag.
-template <int NP>
-inline cudaError_t gemm_tma_configure_np() {
-  cudaError_t e = cudaSuccess;
-#define PF_TMA_CFG(BN_, MODE_, KB_)                                                                                          \
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_tma_kernel<BN_, MODE_, KB_, false, NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, TmaCfg<BN_, MODE_, KB_, false, NP>::kSmemBytes);
-  PF_TMA_VARIANTS(PF_TMA_CFG)
-#undef PF_TMA_CFG
-#define PF_TMA_CFG_PP(BN_, KB_)                                                                                               \
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_tma_kernel<BN_, MODE_GEMM, KB_, true, NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, TmaCfg<BN_, MODE_GEMM, KB_, true, NP>::kSmemBytes);
-  PF_TMA_PINGPONG_VARIANTS(PF_TMA_CFG_PP)
-#undef PF_TMA_CFG_PP
-  return e;
-}
-inline cudaError_t gemm_tma_configure_device(int np) {
-  return np == 1 ? gemm_tma_configure_np<1>() : (np == 3 ? gemm_tma_configure_np<3>() : cudaErrorInvalidValue);
-}
-
+cudaError_t gemm_tma_configure_device(int np);
 // ring depth of an instantiation, 0 if PF_TMA_VARIANTS (pp: PF_TMA_PINGPONG_VARIANTS) does not list it or np is not 3 or 1
-template <int NP>
-inline int tma_stages_np(int mode, int bn, int kb, bool pp) {
-#define PF_TMA_NS(BN_, MODE_, KB_) if (!pp && mode == MODE_ && bn == BN_ && kb == KB_) return TmaCfg<BN_, MODE_, KB_, false, NP>::kStages;
-  PF_TMA_VARIANTS(PF_TMA_NS)
-#undef PF_TMA_NS
-#define PF_TMA_NS_PP(BN_, KB_) if (pp && mode == MODE_GEMM && bn == BN_ && kb == KB_) return TmaCfg<BN_, MODE_GEMM, KB_, true, NP>::kStages;
-  PF_TMA_PINGPONG_VARIANTS(PF_TMA_NS_PP)
-#undef PF_TMA_NS_PP
-  return 0;
-}
-inline int tma_stages(int mode, int bn, int kb, bool pp, int np) {
-  return np == 1 ? tma_stages_np<1>(mode, bn, kb, pp) : (np == 3 ? tma_stages_np<3>(mode, bn, kb, pp) : 0);
-}
-
-// Why the (bn, kb) instantiation with np products cannot compute p: nullptr when it can.  Every case here would otherwise launch
-// something that computes a different result (a K tail, a prediction tail or phase layout the tile width does not implement) or
-// that gemm_tma_launch_bn refuses after the fact (resident weights over several N tiles).  Whether the weights are resident
-// depends on the ring depth, so on np: the one-product ring is deeper.
-inline const char* gemm_tma_check(int mode, const TmaGemmParams& p, int bn, int kb, bool pred, bool pp, int np) {
-  const int ns = tma_stages(mode, bn, kb, pp, np);
-  if (!ns) return pp ? "no ping-pong engine instantiation for this (mode, bn, kb)" : "no engine instantiation for this (mode, bn, kb)";
-  if (mode == MODE_GEMM) return p.K % kb ? "GEMM mode: K must be a multiple of the K step" : nullptr;
-  if (p.phase4 && (p.N != 128 || bn != 128)) return "phase4 needs N = 128 in one 128-wide tile";
-  if (pred && bn != (p.phase4 ? 128 : 32)) return "the fused prediction tail needs N = 32 (phase4: 128) in one tile";
-  const bool resident = p.Cin == 64 && 9 * (64 / kb) <= ns;
-  if ((resident || pred) && cdiv(p.N, bn) > 1) return "resident weights (Cin = 64) and the prediction tail need one N tile per launch";
-  return nullptr;
-}
-
-template <int NP>
-inline cudaError_t gemm_tma_launch_np(int mode, const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, bool pp, int sm_count, cudaStream_t st,
-                                      const PredTail* pred) {
-#define PF_TMA_CASE(BN_, MODE_, KB_) if (!pp && mode == MODE_ && bn == BN_ && kb == KB_) return gemm_tma_launch_bn<BN_, MODE_, KB_, false, NP>(maps, p, sm_count, st, pred);
-  PF_TMA_VARIANTS(PF_TMA_CASE)
-#undef PF_TMA_CASE
-#define PF_TMA_CASE_PP(BN_, KB_) if (pp && mode == MODE_GEMM && bn == BN_ && kb == KB_) return gemm_tma_launch_bn<BN_, MODE_GEMM, KB_, true, NP>(maps, p, sm_count, st, pred);
-  PF_TMA_PINGPONG_VARIANTS(PF_TMA_CASE_PP)
-#undef PF_TMA_CASE_PP
-  return cudaErrorInvalidValue;
-}
+int tma_stages(int mode, int bn, int kb, bool pp, int np);
+// Why the (bn, kb) instantiation with np products cannot compute p: nullptr when it can.
+const char* gemm_tma_check(int mode, const TmaGemmParams& p, int bn, int kb, bool pred, bool pp, int np);
 // np = bf16 products per output: 3 (split precision) or 1 (bf16 precision mode)
-inline cudaError_t gemm_tma_launch(int mode, const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, bool pp, int np, int sm_count, cudaStream_t st,
-                                   const PredTail* pred = nullptr) {
-  if (np == 1) return gemm_tma_launch_np<1>(mode, maps, p, bn, kb, pp, sm_count, st, pred);
-  if (np == 3) return gemm_tma_launch_np<3>(mode, maps, p, bn, kb, pp, sm_count, st, pred);
-  return cudaErrorInvalidValue;
-}
+cudaError_t gemm_tma_launch(int mode, const TmaMaps& maps, const TmaGemmParams& p, int bn, int kb, bool pp, int np, int sm_count, cudaStream_t st,
+                            const PredTail* pred = nullptr);
 
 }  // namespace pf
