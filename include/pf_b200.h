@@ -483,6 +483,36 @@ int pf_op_attention_tc_keys(const float* q, const float* kv, float* out, int B, 
 int pf_op_dwconv3x3_gelu(const float* x, float* y, int B, int H, int W, int C, const float* w9c, const float* bias, void* stream);
 int pf_op_dwconv7x7(const float* x, float* y, int B, int H, int W, int C, const float* w49c, const float* bias, void* stream);
 int pf_op_upsample2x(const float* x, float* y, int B, int H, int W, int C, void* stream);
+/* The forward graph's CUDA-core kernels one launch at a time, each through the host helper pf_forward launches it with (same
+ * grid, block and arguments); pf_op_layernorm, pf_op_dwconv3x3_gelu, pf_op_dwconv7x7 and pf_op_upsample2x above go the same
+ * way.  DEVICE pointers; the call ends with a stream synchronisation.  Every argument is checked before anything is launched
+ * (PF_ERR_ARG), including shapes whose indices would leave the 32-bit range the kernel computes them in.  Pointers read or
+ * written 16 bytes at a time (NHWC activations, split planes, weights of the depthwise convs) must be 16-byte aligned.  A split
+ * output is a pair of bf16 planes hi / lo with hi + lo = the fp32 result (hi = its round-to-nearest-even bf16).
+ *   layernorm_ex: LayerNorm over rows of C channels (a multiple of 4 up to 768) into any non-empty set of y (fp32), hi / lo (split,
+ *     row order) and phi / plo (split, the im2col order of a k = s = sr convolution on RH x RW maps: token (b, y, x) goes to row
+ *     (b, y / sr, x / sr), columns ((y % sr) sr + x % sr) C ..; RH, RW multiples of sr, rows a multiple of RH RW).
+ *   dwconv3x3_gelu_ex: depthwise 3x3 (pad 1) + bias + GELU on NHWC [B, H, W, C] into y and / or hi / lo.
+ *   upsample2x_ex: x2 bilinear upsample of channels icoff .. icoff + C - 1 of [B, H, W, ldi] into channels ocoff .. of
+ *     [B, 2H, 2W, ldo], as y and / or hi / lo (pitch ldo); all four multiples of 4.
+ *   stem_gather: the 7 x 7 / stride (2 or 4) / pad 3 patch matrix of channels 0-2 of x0 [B, IH, IW, 4] as split planes
+ *     [B * OH * OW][160], columns (ky, kx, c), 147 .. 159 zero; OH = (IH - 1) / stride + 1, OW likewise.
+ *   pn_stem: ParamNet stem conv 4 x 4 / 4 + bias of channels 0-2 of pin [B, SH, SW, 4] -> [B, SH / 4, SW / 4, 96]; w [(ky, kx, ci)][96].
+ *   pack_fields: up fields [B, 2, IH, IW] and latitude [B, 1, IH, IW] nearest-resampled to [B, OH, OW, 4] (channel 3 zero).
+ *   param_tail: ParamNet tail of feat [n, HW, 768]: mean pool, LayerNorm (eps 1e-6; nw, nb), Linear 768 -> 5 (hw [5][768], hb),
+ *     parameter scaling of kind PF_PARAM_CENTERED / PF_PARAM_UNCENTERED into params [n][8] (pf_batch.params); raw [n][5] may be NULL.
+ *   pred_tail: 1x1 conv 32 -> NC (w [NC][32], b [NC]) of channels coff .. coff + 31 of feat [B * HW, ld] -> NCHW out [B, NC, HW];
+ *     mode 0 raw, 1 F.normalize over 2 channels (NC = 2), 2 clamp to [-1, 1]; NC <= 256. */
+int pf_op_layernorm_ex(const float* x, float* y, void* hi, void* lo, void* phi, void* plo, int64_t rows, int C, const float* w, const float* b,
+                       float eps, int RH, int RW, int sr, void* stream);
+int pf_op_dwconv3x3_gelu_ex(const float* x, int B, int H, int W, int C, const float* w9c, const float* bias, float* y, void* hi, void* lo, void* stream);
+int pf_op_upsample2x_ex(const float* x, int ldi, int icoff, float* y, int ldo, int ocoff, void* hi, void* lo, int B, int H, int W, int C, void* stream);
+int pf_op_stem_gather(const float* x0, int B, int IH, int IW, int stride, void* hi, void* lo, void* stream);
+int pf_op_pn_stem(const float* pin, int B, int SH, int SW, const float* w, const float* b, float* out, void* stream);
+int pf_op_pack_fields(const float* grav, const float* lat, int B, int IH, int IW, int OH, int OW, float* out, void* stream);
+int pf_op_param_tail(const float* feat, int n, int HW, const float* nw, const float* nb, const float* hw, const float* hb, int kind, float* params,
+                     float* raw, void* stream);
+int pf_op_pred_tail(const float* feat, int ld, int coff, const float* w, const float* b, float* out, int B, int HW, int NC, int mode, void* stream);
 /* Pillow-exact resize + normalise of ONE uint8 HWC image -> [320,320,4] fp32 (b,g,r,0). */
 int pf_op_preprocess(const uint8_t* img_dev, int H, int W, const float* mean3, const float* std3, float* y, void* stream);
 /* the same to [net_h,net_w,4] (a working size pf_create_sized accepts) */

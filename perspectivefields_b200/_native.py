@@ -242,6 +242,14 @@ def lib():
         "pf_op_dwconv3x3_gelu": (i32, [vp, vp, i32, i32, i32, i32, vp, vp, vp]),
         "pf_op_dwconv7x7": (i32, [vp, vp, i32, i32, i32, i32, vp, vp, vp]),
         "pf_op_upsample2x": (i32, [vp, vp, i32, i32, i32, i32, vp]),
+        "pf_op_layernorm_ex": (i32, [vp, vp, vp, vp, vp, vp, i64, i32, vp, vp, f32, i32, i32, i32, vp]),
+        "pf_op_dwconv3x3_gelu_ex": (i32, [vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]),
+        "pf_op_upsample2x_ex": (i32, [vp, i32, i32, vp, i32, i32, vp, vp, i32, i32, i32, i32, vp]),
+        "pf_op_stem_gather": (i32, [vp, i32, i32, i32, i32, vp, vp, vp]),
+        "pf_op_pn_stem": (i32, [vp, i32, i32, i32, vp, vp, vp, vp]),
+        "pf_op_pack_fields": (i32, [vp, vp, i32, i32, i32, i32, i32, vp, vp]),
+        "pf_op_param_tail": (i32, [vp, i32, i32, vp, vp, vp, vp, i32, vp, vp, vp]),
+        "pf_op_pred_tail": (i32, [vp, i32, i32, vp, vp, vp, i32, i32, i32, i32, vp]),
         "pf_op_preprocess": (i32, [vp, i32, i32, ctypes.POINTER(f32), ctypes.POINTER(f32), vp, vp]),
         "pf_op_preprocess_sized": (i32, [vp, i32, i32, i32, i32, ctypes.POINTER(f32), ctypes.POINTER(f32), vp, vp]),
         "pf_op_resize_u8": (i32, [vp, i32, i32, i32, i32, vp, vp]),
@@ -290,7 +298,9 @@ EXPORTS = ["pf_abi_version", "pf_last_error", "pf_kernel_launch_count", "pf_crea
            "pf_op_dwconv7x7", "pf_op_upsample2x", "pf_op_preprocess", "pf_op_preprocess_sized", "pf_op_fill_stream", "pf_op_resize_u8",
            "pf_op_resize_f32", "pf_op_argmax_decode", "pf_op_pred_argmax_decode", "pf_op_postprocess", "pf_op_postprocess_sized",
            "pf_op_pn_wgrad", "pf_op_pn_colsum", "pf_op_pn_ln_bwd", "pf_op_pn_dw7_bwd", "pf_op_pn_stem_bwd", "pf_op_pn_fields_grad",
-           "pf_op_pn_tail_bwd", "pf_op_pn_pw2_grads", "pf_op_pn_gelu_bwd", "pf_op_pn_scale_split", "pf_op_pn_col2im2"]
+           "pf_op_pn_tail_bwd", "pf_op_pn_pw2_grads", "pf_op_pn_gelu_bwd", "pf_op_pn_scale_split", "pf_op_pn_col2im2",
+           "pf_op_layernorm_ex", "pf_op_dwconv3x3_gelu_ex", "pf_op_upsample2x_ex", "pf_op_stem_gather", "pf_op_pn_stem",
+           "pf_op_pack_fields", "pf_op_param_tail", "pf_op_pred_tail"]
 
 
 class PfError(RuntimeError):

@@ -286,8 +286,27 @@ struct Fwd {
   int tconv_gather(const SplitT& A, int B, int H, int W, int Cin, int KH, int stride, int pad, const GemmW& w, int N, const Epi& o);
   int ln_split(const float* x, const SplitT& y, long long rows, int C, const LnW& w, float eps, float* yf = nullptr);
   // LayerNorm whose output is (also) written in patch order for a k = s = sr convolution on the RH x RW map (y may be empty)
-  int ln_split_patch(const float* x, const SplitT& y, const SplitT& patch, long long rows, int C, const LnW& w, float eps, int RH, int RW, int sr);
+  int ln_split_patch(const float* x, const SplitT& y, const SplitT& patch, long long rows, int C, const LnW& w, float eps, int RH, int RW, int sr,
+                     float* yf = nullptr);
   int ln(const float* x, float* y, long long rows, int C, const LnW& w, float eps);
+  // The graph's other CUDA-core kernels (layers.cuh) on the n images of this pass.  Each helper is the only place its kernel is
+  // launched from, and it rejects (PF_ERR_ARG, also in the sizing dry run) a shape whose indices would leave the 32-bit range the
+  // kernel computes them in.
+  // depthwise 3x3 + GELU on [n, H, W, C]: fp32 y and / or split planes s (the graph writes the planes only)
+  int dw3_gelu(const float* x, float* y, const SplitT& s, int H, int W, int C, const float* w, const float* b);
+  // x2 bilinear upsample of channels icoff .. icoff + C - 1 of [n, H, W, ldi] into channels ocoff .. of [n, 2H, 2W, ldo]: fp32 y
+  // and / or split planes s (pitch ldo as well)
+  int up2x(const float* x, int ldi, int icoff, float* y, int ldo, int ocoff, const SplitT& s, int H, int W, int C);
+  // 7x7 / stride (2 or 4) / pad 3 patch matrix of x0 [n, IH, IW, 4] (channels 0-2) as split planes [n * OH * OW][160]
+  int stem_gather(const float* x0, const SplitT& col, int IH, int IW, int stride);
+  // ParamNet stem conv 4x4 / 4, 3 -> 96, on pin [n, SH, SW, 4] -> out [n, SH / 4, SW / 4, 96]
+  int pn_stem(const float* pin, int SH, int SW, const float* w, const float* b, float* out);
+  // ParamNet input: fields [n, 2 | 1, IH, IW] nearest-resampled to [n, OH, OW, 4]
+  int pack_fields(const float* grav, const float* lat, int IH, int IW, int OH, int OW, float* out);
+  // ParamNet tail on feat [n, HW, 768]: params [n][8], raw [n][5] (may be NULL); kind = PF_PARAM_CENTERED / _UNCENTERED
+  int param_tail(const float* feat, int HW, const LnW& norm, const float* hw, const float* hb, int kind, float* params, float* raw);
+  // 1x1 conv 32 -> NC on channels icoff .. icoff + 31 of [n * HW, ldi] -> NCHW out; mode 0 raw, 1 normalise (NC 2), 2 clamp
+  int pred_tail(const float* in, int ldi, int icoff, const float* w, const float* b, float* out, int HW, int NC, int mode);
 };
 
 
@@ -301,7 +320,8 @@ struct PnSaved {
   float* xs[4][10] = {};
 };
 int fwd_paramnet(Fwd& F, const float* grav, const float* lat, float* params, float* raw, const PnSaved* sv = nullptr);
-// depthwise 7x7 convolution of the F.n images [rh, rw, C] (the forward's kernel; ParamNet training runs its data gradient with it)
+// depthwise 7x7 convolution of the F.n images [rh, rw, C] (the forward's kernel; ParamNet training runs its data gradient with it);
+// rejects the shapes Fwd::dw3_gelu rejects
 int pn_dw_launch(Fwd& F, const float* x, float* y, int rh, int rw, int C, const float* w, const float* b);
 
 // ----------------------------------------------------------------------------------------------- single-operator entry points

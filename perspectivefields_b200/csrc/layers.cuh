@@ -196,7 +196,7 @@ __global__ void __launch_bounds__(256, PF_DW3_MINBLOCKS) dwconv3x3_gelu_kernel(c
   // thread = 4 channels x (2 rows x PX consecutive pixels): 4 (PX + 2) activation + 9 weight loads (float4) for 2 PX outputs
   constexpr int PX = PF_DW3_PX;
   const unsigned C4 = (unsigned)C >> 2, XG = ((unsigned)W + PX - 1) / PX, YG = ((unsigned)H + 1) >> 1;
-  const unsigned total = (unsigned)B * YG * XG * C4;      // < 2^31 for every layer of the network (checked by the host): 32-bit index math
+  const unsigned total = (unsigned)B * YG * XG * C4;      // B H W C / 4 < 2^31, checked by Fwd::dw3_gelu (pf_b200.cu): 32-bit index math
   const unsigned rs = (unsigned)W * C4;                   // row stride in float4
   const float4* __restrict__ in4 = reinterpret_cast<const float4*>(in);
   const float4* __restrict__ w4 = reinterpret_cast<const float4*>(w);
@@ -313,7 +313,7 @@ __global__ void __launch_bounds__(256, PF_DW7_MINBLOCKS) dwconv7x7_kernel(const 
   constexpr int PX = PF_DW7_PX;
   const unsigned C4 = (unsigned)C >> 2, XG = ((unsigned)W + PX - 1) / PX, YG = ((unsigned)H + 1) >> 1;
   const unsigned total = (unsigned)B * YG * XG * C4;
-  const unsigned rs = (unsigned)W * C4;                   // row stride in float4 (32-bit index arithmetic as dwconv3x3_gelu_kernel)
+  const unsigned rs = (unsigned)W * C4;                   // row stride in float4 (32-bit index arithmetic as dwconv3x3_gelu_kernel, bound checked by pn_dw_launch)
   const float4* __restrict__ in4 = reinterpret_cast<const float4*>(in);
   const float4* __restrict__ w4 = reinterpret_cast<const float4*>(w);
   for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
@@ -378,7 +378,7 @@ __global__ void __launch_bounds__(256, PF_DW7_MINBLOCKS) dwconv7x7_kernel(const 
 // float4 loads (3 rows x 4 columns, clamped) for 32 results, separable (horizontal, then vertical) -- a third of the loads and
 // half of the instructions of the one-output-pixel-per-thread version.  out[2i] = 0.25 in[i-1] + 0.75 in[i], out[2i+1] =
 // 0.75 in[i] + 0.25 in[i+1]; at the clamped edges both taps are the same pixel and fmaf(0.75, a, 0.25 a) returns a exactly.
-// Index arithmetic is 32-bit in float4 units.
+// Index arithmetic is 32-bit in float4 units (B H W ldi / 4 and 4 B H W ldo / 4 < 2^31, checked by Fwd::up2x in pf_b200.cu).
 inline long long upsample2x_threads(int B, int H, int W, int C) { return (long long)B * H * ((W + 1) / 2) * (C / 4); }
 __global__ void __launch_bounds__(256) upsample2x_kernel(const float* __restrict__ in, int ldi, int icoff, float* __restrict__ out, int ldo, int ocoff,
                                                          int B, int H, int W, int C, __nv_bfloat16* __restrict__ shi = nullptr, __nv_bfloat16* __restrict__ slo = nullptr) {

@@ -189,19 +189,90 @@ int Fwd::tconv_gather(const SplitT& A, int B, int H, int W, int Cin, int KH, int
   ar.release(m);
   return r;
 }
+// The shapes layernorm_launch accepts, checked before the launch (the launcher itself fails after the launch counter has moved):
+// C a multiple of 4 up to 768 and rows * C / 4 < 2^32 (the kernel's float4 indices are 32-bit); the patch order needs an RH x RW
+// map that sr divides and whose images tile the rows.
+static int ln_check(long long rows, int C, bool patch, int RH, int RW, int sr) {
+  if (rows < 1 || C < 4 || C % 4 || C > 768 || rows * (C / 4) >= (1LL << 32)) return fail(PF_ERR_ARG, "LayerNorm: %lld rows of %d channels", rows, C);
+  if (patch && (RH < 1 || RW < 1 || sr < 1 || RH % sr || RW % sr || rows % ((long long)RH * RW)))
+    return fail(PF_ERR_ARG, "LayerNorm: patch order of %lld rows as %dx%d maps with sr %d", rows, RH, RW, sr);
+  return PF_OK;
+}
 int Fwd::ln_split(const float* x, const SplitT& y, long long rows, int C, const LnW& w, float eps, float* yf) {
+  TRY(ln_check(rows, C, false, 0, 0, 0));
   if (dry) return PF_OK;
   LAUNCHED(layernorm_launch(x, yf, rows, C, w.w, w.b, eps, st, y));
   return PF_OK;
 }
-int Fwd::ln_split_patch(const float* x, const SplitT& y, const SplitT& patch, long long rows, int C, const LnW& w, float eps, int RH, int RW, int sr) {
+int Fwd::ln_split_patch(const float* x, const SplitT& y, const SplitT& patch, long long rows, int C, const LnW& w, float eps, int RH, int RW, int sr, float* yf) {
+  TRY(ln_check(rows, C, true, RH, RW, sr));
   if (dry) return PF_OK;
-  LAUNCHED(layernorm_launch(x, nullptr, rows, C, w.w, w.b, eps, st, y, patch, RH, RW, sr));
+  LAUNCHED(layernorm_launch(x, yf, rows, C, w.w, w.b, eps, st, y, patch, RH, RW, sr));
   return PF_OK;
 }
 int Fwd::ln(const float* x, float* y, long long rows, int C, const LnW& w, float eps) {
+  TRY(ln_check(rows, C, false, 0, 0, 0));
   if (dry) return PF_OK;
   LAUNCHED(layernorm_launch(x, y, rows, C, w.w, w.b, eps, st));
+  return PF_OK;
+}
+
+// The element-wise kernels below form their indices in 32-bit arithmetic, most of them unsigned in float4 units, and the
+// grid-stride loops advance an unsigned counter by one grid of threads: every index a kernel forms stays below 2^31, which also
+// keeps that counter from wrapping.
+static bool fits31(long long n) { return n >= 0 && n < (1LL << 31); }
+
+int Fwd::dw3_gelu(const float* x, float* y, const SplitT& s, int H, int W, int C, const float* w, const float* b) {
+  if (n < 1 || H < 1 || W < 1 || C < 4 || C % 4 || !fits31((long long)n * H * W * (C / 4)))
+    return fail(PF_ERR_ARG, "dwconv3x3_gelu: %d images of %dx%d x %d channels", n, H, W, C);
+  if (dry) return PF_OK;
+  LAUNCHED(launch_pdl(dwconv3x3_gelu_kernel, dim3(ew_grid((long long)n * ((H + 1) / 2) * ((W + PF_DW3_PX - 1) / PF_DW3_PX) * (C / 4))), dim3(256), 0, st,
+                      x, y, n, H, W, C, w, b, s.hi, s.lo));
+  return PF_OK;
+}
+int Fwd::up2x(const float* x, int ldi, int icoff, float* y, int ldo, int ocoff, const SplitT& s, int H, int W, int C) {
+  if (n < 1 || H < 1 || W < 1 || C < 4 || (C | ldi | icoff | ldo | ocoff) % 4 || icoff < 0 || ocoff < 0 || icoff + C > ldi || ocoff + C > ldo ||
+      !fits31((long long)n * H * W * (ldi / 4)) || !fits31(4LL * n * H * W * (ldo / 4)))
+    return fail(PF_ERR_ARG, "upsample2x: %d images of %dx%d, channels %d..%d of %d -> %d..%d of %d", n, H, W, icoff, icoff + C - 1, ldi, ocoff, ocoff + C - 1, ldo);
+  if (dry) return PF_OK;
+  LAUNCHED(launch_pdl(upsample2x_kernel, dim3(ew_grid(upsample2x_threads(n, H, W, C))), dim3(256), 0, st, x, ldi, icoff, y, ldo, ocoff, n, H, W, C, s.hi, s.lo));
+  return PF_OK;
+}
+int Fwd::stem_gather(const float* x0, const SplitT& col, int IH, int IW, int stride) {
+  const int OH = (IH - 1) / stride + 1, OW = (IW - 1) / stride + 1;     // 7 x 7, pad 3
+  if (n < 1 || IH < 1 || IW < 1 || (stride != 2 && stride != 4) || !fits31(4LL * n * IH * IW) || !fits31(stem_gather_threads(n, OH, OW)))
+    return fail(PF_ERR_ARG, "stem_gather: %d images of %dx%d, stride %d", n, IH, IW, stride);
+  if (dry) return PF_OK;
+  LAUNCHED(launch_pdl(stem_gather_kernel, dim3(ew_grid(stem_gather_threads(n, OH, OW))), dim3(256), 0, st, x0, col.hi, col.lo, n, OH, OW, stride, IH, IW));
+  return PF_OK;
+}
+int Fwd::pn_stem(const float* pin, int SH, int SW, const float* w, const float* b, float* out) {
+  if (n < 1 || SH < 4 || SW < 4 || !fits31(4LL * n * SH * SW)) return fail(PF_ERR_ARG, "ParamNet stem: %d images of %dx%d", n, SH, SW);
+  if (dry) return PF_OK;
+  LAUNCHED((stem_conv_launch<4, 4, 4, 0, 96>(pin, 4, n, SH, SW, w, b, out, st)));
+  return PF_OK;
+}
+int Fwd::pack_fields(const float* grav, const float* lat, int IH, int IW, int OH, int OW, float* out) {
+  if (n < 1 || IH < 1 || IW < 1 || OH < 1 || OW < 1 || !fits31((long long)IH * IW) || !fits31((long long)n * OH * OW))
+    return fail(PF_ERR_ARG, "pack_fields: %d images of %dx%d -> %dx%d", n, IH, IW, OH, OW);
+  if (dry) return PF_OK;
+  LAUNCHED((pack_fields_kernel<<<(unsigned)cdivl((long long)n * OH * OW, 256), 256, 0, st>>>(grav, lat, out, n, IH, IW, OH, OW), cudaGetLastError()));
+  return PF_OK;
+}
+int Fwd::param_tail(const float* feat, int HW, const LnW& norm, const float* hw, const float* hb, int kind, float* params, float* raw) {
+  if (n < 1 || HW < 1 || (kind != PF_PARAM_CENTERED && kind != PF_PARAM_UNCENTERED) || !fits31(8LL * n))
+    return fail(PF_ERR_ARG, "param_tail: %d images of %d pixels, kind %d", n, HW, kind);
+  if (dry) return PF_OK;
+  LAUNCHED((param_tail_kernel<<<n, 256, 0, st>>>(feat, HW, norm.w, norm.b, hw, hb, params, raw, kind), cudaGetLastError()));
+  return PF_OK;
+}
+int Fwd::pred_tail(const float* in, int ldi, int icoff, const float* w, const float* b, float* out, int HW, int NC, int mode) {
+  // weights and bias in shared memory (NC * 33 floats); mode 1 normalises the two channels of an up vector
+  if (n < 1 || HW < 1 || NC < 1 || NC > 256 || mode < 0 || mode > 2 || (mode == 1 && NC != 2) || (ldi | icoff) % 4 || icoff < 0 || icoff + 32 > ldi ||
+      !fits31((long long)n * HW))
+    return fail(PF_ERR_ARG, "pred_tail: %d images of %d pixels, %d classes, mode %d, channels %d.. of %d", n, HW, NC, mode, icoff, ldi);
+  if (dry) return PF_OK;
+  LAUNCHED((pred_tail_kernel<<<(unsigned)cdivl((long long)n * HW, 128), 128, NC * 33 * 4, st>>>(in, ldi, icoff, w, b, out, n, HW, NC, mode), cudaGetLastError()));
   return PF_OK;
 }
 
@@ -329,11 +400,8 @@ static int fwd_tails_post(Fwd& F, const pf_batch* bt, const float* conv1_out, Po
     // debug taps: the raw prediction-conv outputs before normalise / clamp (oracle taps g.raw / l.raw)
     float* rg = ar.f((long long)n * D.gravity_classes * HW);
     float* rl = ar.f((long long)n * D.latitude_classes * HW);
-    if (!dry) {
-      const unsigned grid = (unsigned)cdivl((long long)n * HW, 128);
-      LAUNCHED((pred_tail_kernel<<<grid, 128, D.gravity_classes * 33 * 4, st>>>(conv1_out, 64, 0, e->pred_g_w, e->pred_g_b, rg, n, HW, D.gravity_classes, 0), cudaGetLastError()));
-      LAUNCHED((pred_tail_kernel<<<grid, 128, D.latitude_classes * 33 * 4, st>>>(conv1_out, 64, 32, e->pred_l_w, e->pred_l_b, rl, n, HW, D.latitude_classes, 0), cudaGetLastError()));
-    }
+    TRY(F.pred_tail(conv1_out, 64, 0, e->pred_g_w, e->pred_g_b, rg, HW, D.gravity_classes, 0));
+    TRY(F.pred_tail(conv1_out, 64, 32, e->pred_l_w, e->pred_l_b, rl, HW, D.latitude_classes, 0));
     TRY(F.tap("head.raw_g", rg, (long long)n * D.gravity_classes * HW));
     TRY(F.tap("head.raw_l", rl, (long long)n * D.latitude_classes * HW));
   }
@@ -348,12 +416,9 @@ static int fwd_tails_post(Fwd& F, const pf_batch* bt, const float* conv1_out, Po
     }
   } else {
     // prediction tails -> NCHW outputs (returned to the caller)
-    if (!dry && !pred_done) {
-      const unsigned grid = (unsigned)cdivl((long long)n * HW, 128);
-      LAUNCHED((pred_tail_kernel<<<grid, 128, D.gravity_classes * 33 * 4, st>>>(conv1_out, 64, 0, e->pred_g_w, e->pred_g_b, bt->pred_gravity, n, HW,
-                                                                             D.gravity_classes, D.gravity_classes == 2 ? 1 : 0), cudaGetLastError()));
-      LAUNCHED((pred_tail_kernel<<<grid, 128, D.latitude_classes * 33 * 4, st>>>(conv1_out, 64, 32, e->pred_l_w, e->pred_l_b, bt->pred_latitude, n, HW,
-                                                                              D.latitude_classes, D.latitude_classes == 1 ? 2 : 0), cudaGetLastError()));
+    if (!pred_done) {
+      TRY(F.pred_tail(conv1_out, 64, 0, e->pred_g_w, e->pred_g_b, dry ? nullptr : bt->pred_gravity, HW, D.gravity_classes, D.gravity_classes == 2 ? 1 : 0));
+      TRY(F.pred_tail(conv1_out, 64, 32, e->pred_l_w, e->pred_l_b, dry ? nullptr : bt->pred_latitude, HW, D.latitude_classes, D.latitude_classes == 1 ? 2 : 0));
     }
     if (cls_g) {
       float* dv = ar.f((long long)n * 2 * HW);
@@ -408,7 +473,7 @@ static int run_forward(Fwd& F, const pf_batch* bt) {
     const long long m = ar.mark();
     const long long M = (long long)n * LH * LW;
     SplitT col = F.salloc(M, 160);
-    if (!dry) LAUNCHED(launch_pdl(stem_gather_kernel, dim3(ew_grid(stem_gather_threads(n, LH, LW))), dim3(256), 0, st, x0, col.hi, col.lo, n, LH, LW, 2, NH, NW));
+    TRY(F.stem_gather(x0, col, NH, NW, 2));
     Epi o; o.S = ll; o.act = 1;
     TRY(F.tgemm(col, M, 160, 0, e->llencg, 64, o));
     ar.release(m);
@@ -436,7 +501,7 @@ static int run_forward(Fwd& F, const pf_batch* bt) {
     if (s == 0) {
       const long long mm = ar.mark();
       SplitT col = F.salloc(rows, 160);
-      if (!dry) LAUNCHED(launch_pdl(stem_gather_kernel, dim3(ew_grid(stem_gather_threads(n, RH[0], RW[0]))), dim3(256), 0, st, x0, col.hi, col.lo, n, RH[0], RW[0], 4, NH, NW));
+      TRY(F.stem_gather(x0, col, NH, NW, 4));
       Epi o; o.C = tf; o.ldc = C;
       TRY(F.tgemm(col, rows, 160, 0, e->embed1g, 64, o));
       ar.release(mm);
@@ -463,7 +528,7 @@ static int run_forward(Fwd& F, const pf_batch* bt) {
       TRY(F.tapf(x, rows * C, "mit.s%d.b%d.attn", s + 1, i));
       TRY(F.ln_split(x, t1, rows, C, b.ln2, 1e-6f));
       { Epi o; o.C = h1; o.ldc = 4 * C; TRY(F.tgemm(t1, rows, C, 0, b.fc1, 4 * C, o)); }
-      if (!dry) LAUNCHED(launch_pdl(dwconv3x3_gelu_kernel, dim3(ew_grid((long long)n * ((RH[s] + 1) / 2) * ((RW[s] + PF_DW3_PX - 1) / PF_DW3_PX) * C)), dim3(256), 0, st, h1, nullptr, n, RH[s], RW[s], 4 * C, b.dw_w, b.dw_b, h2.hi, h2.lo));
+      TRY(F.dw3_gelu(h1, nullptr, h2, RH[s], RW[s], 4 * C, b.dw_w, b.dw_b));
       { Epi o; o.C = x; o.ldc = C; o.res = x; o.ldr = C; TRY(F.tgemm(h2, rows, 4 * C, 0, b.fc2, C, o)); }
       TRY(F.tapf(x, rows * C, "mit.s%d.b%d", s + 1, i));
     }
@@ -510,12 +575,12 @@ static int run_forward(Fwd& F, const pf_batch* bt) {
       { Epi o; o.C = w2; o.ldc = 512; o.res = of; o.ldr = 512; o.res_relu = 1; TRY(rcu(u, e->rcu[lvl - 1][1][1], o)); }
       if (lvl > 1) {
         float* up = ar.f(px * 4 * 512);
-        if (!dry) LAUNCHED(launch_pdl(upsample2x_kernel, dim3(ew_grid(upsample2x_threads(n, rh, rw, 512))), dim3(256), 0, st, w2, 512, 0, up, 512, 0, n, rh, rw, 512, nullptr, nullptr));
+        TRY(F.up2x(w2, 512, 0, up, 512, 0, SplitT(), rh, rw, 512));
         fused = up;
         TRY(F.tapf(up, px * 4 * 512, "head.fusion%d", lvl));
       } else {
         fused_s = F.salloc(px * 4, 512);
-        if (!dry) LAUNCHED(launch_pdl(upsample2x_kernel, dim3(ew_grid(upsample2x_threads(n, rh, rw, 512))), dim3(256), 0, st, w2, 512, 0, nullptr, 512, 0, n, rh, rw, 512, fused_s.hi, fused_s.lo));
+        TRY(F.up2x(w2, 512, 0, nullptr, 512, 0, fused_s, rh, rw, 512));
         TRY(F.tap_split("head.fusion1", fused_s, px * 4 * 512));
       }
     }
@@ -575,11 +640,11 @@ int fwd_paramnet(Fwd& F, const float* grav, const float* lat, float* params, flo
     const bool centered = D.param_net == PF_PARAM_CENTERED;
     const int SH = centered ? NH : D.param_input_size, SW = centered ? NW : D.param_input_size;
     float* pin = sv ? sv->pin : ar.f((long long)n * SH * SW * 4);
-    if (!dry) LAUNCHED((pack_fields_kernel<<<(unsigned)cdivl((long long)n * SH * SW, 256), 256, 0, st>>>(grav, lat, pin, n, NH, NW, SH, SW), cudaGetLastError()));
+    TRY(F.pack_fields(grav, lat, NH, NW, SH, SW, pin));
     int rh = SH / 4, rw = SW / 4;
     float* x = sv ? sv->xs[0][0] : ar.f((long long)n * rh * rw * 96);
     float* stem = sv ? sv->stem_pre : x;
-    if (!dry) LAUNCHED((stem_conv_launch<4, 4, 4, 0, 96>(pin, 4, n, SH, SW, e->pn_stem_w, e->pn_stem_b, stem, st)));
+    TRY(F.pn_stem(pin, SH, SW, e->pn_stem_w, e->pn_stem_b, stem));
     TRY(F.ln(stem, x, (long long)n * rh * rw, 96, e->pn_stem_ln, 1e-6f));
     for (int s = 0; s < 4; ++s) {
       const int C = kCnxDims[s];
@@ -598,7 +663,7 @@ int fwd_paramnet(Fwd& F, const float* grav, const float* lat, float* params, flo
       SplitT h = F.salloc(rows, 4 * C);
       for (int j = 0; j < kCnxDepths[s]; ++j) {
         const CnxBlockW& b = e->pn_blocks[s][j];
-        if (!dry) LAUNCHED(launch_pdl(dwconv7x7_kernel, dim3(ew_grid((long long)n * ((rh + 1) / 2) * ((rw + PF_DW7_PX - 1) / PF_DW7_PX) * (C / 4))), dim3(256), 0, st, x, yf, n, rh, rw, C, b.dw_w, b.dw_b));
+        TRY(pn_dw_launch(F, x, yf, rh, rw, C, b.dw_w, b.dw_b));
         TRY(F.ln_split(yf, y, rows, C, b.ln, 1e-6f));
         { Epi o; o.S = h; o.act = 2; TRY(F.tgemm(y, rows, C, 0, b.pw1, 4 * C, o)); }
         float* xo = sv ? sv->xs[s][j + 1] : x;     // training keeps every block's input: out of place, same arithmetic
@@ -607,15 +672,15 @@ int fwd_paramnet(Fwd& F, const float* grav, const float* lat, float* params, flo
       }
       TRY(F.tapf(x, rows * C, "cnx.s%d", s));
     }
-    if (!dry) {
-      if (!params) return fail(PF_ERR_ARG, "params output is NULL");
-      LAUNCHED((param_tail_kernel<<<n, 256, 0, st>>>(x, rh * rw, e->pn_norm.w, e->pn_norm.b, e->pn_head_w, e->pn_head_b, params, raw, D.param_net), cudaGetLastError()));
-    }
+    if (!dry && !params) return fail(PF_ERR_ARG, "params output is NULL");
+    TRY(F.param_tail(x, rh * rw, e->pn_norm, e->pn_head_w, e->pn_head_b, D.param_net, params, raw));
   }
   return PF_OK;
 }
 
 int pn_dw_launch(Fwd& F, const float* x, float* y, int rh, int rw, int C, const float* w, const float* b) {
+  if (F.n < 1 || rh < 1 || rw < 1 || C < 4 || C % 4 || !fits31((long long)F.n * rh * rw * (C / 4)))
+    return fail(PF_ERR_ARG, "dwconv7x7: %d images of %dx%d x %d channels", F.n, rh, rw, C);
   if (!F.dry) LAUNCHED(launch_pdl(dwconv7x7_kernel, dim3(ew_grid((long long)F.n * ((rh + 1) / 2) * ((rw + PF_DW7_PX - 1) / PF_DW7_PX) * (C / 4))), dim3(256), 0, F.st,
                                   x, y, F.n, rh, rw, C, w, b));
   return PF_OK;
@@ -918,6 +983,8 @@ int op_engine(pf_engine& e, bool bf16) {
   return PF_OK;
 }
 
+static bool al16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
 // a host array copied into the op's scratch on its stream
 template <class T>
 static int op_upload(Fwd& F, const T* src, size_t count, T** dst) {
@@ -1106,10 +1173,6 @@ int pf_op_fill_stream(float* dst, int64_t numel, float value, void* stream) {
   LAUNCHED((fill_stream_kernel<<<132 * 16, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<float4*>(dst), numel / 4, value), cudaGetLastError()));
   return PF_OK;
 }
-int pf_op_layernorm(const float* x, float* y, int64_t rows, int C, const float* w, const float* b, float eps, void* stream) {
-  LAUNCHED(layernorm_launch(x, y, rows, C, w, b, eps, (cudaStream_t)stream));
-  return PF_OK;
-}
 static int op_attention_tc(const float* q, const float* kv, float* out, int B, int N, int C, int heads, void* stream, int np, int nkv = kAmKeys) {
   if (!q || !kv || !out || C != heads * kAmD) return fail(PF_ERR_ARG, "pf_op_attention_tc: head_dim must be 64");
   if (B < 1 || N < 1 || nkv < 1 || nkv > kAmMaxKeys) return fail(PF_ERR_ARG, "pf_op_attention_tc: B %d, N %d, %d keys (1..%d)", B, N, nkv, kAmMaxKeys);
@@ -1133,20 +1196,71 @@ int pf_op_attention_tc_bf16(const float* q, const float* kv, float* out, int B, 
 int pf_op_attention_tc_keys(const float* q, const float* kv, float* out, int B, int N, int NKV, int C, int heads, int bf16, void* stream) {
   return op_attention_tc(q, kv, out, B, N, C, heads, stream, bf16 ? 1 : 3, NKV);
 }
+// The forward graph's CUDA-core kernels, each through the Fwd helper the graph launches it with (same grid, block and arguments).
+int pf_op_layernorm(const float* x, float* y, int64_t rows, int C, const float* w, const float* b, float eps, void* stream) {
+  return pf_op_layernorm_ex(x, y, nullptr, nullptr, nullptr, nullptr, rows, C, w, b, eps, 0, 0, 0, stream);
+}
+int pf_op_layernorm_ex(const float* x, float* y, void* hi, void* lo, void* phi, void* plo, int64_t rows, int C, const float* w, const float* b,
+                       float eps, int RH, int RW, int sr, void* stream) {
+  if (!x || !w || !b || !hi != !lo || !phi != !plo || (!y && !hi && !phi)) return fail(PF_ERR_ARG, "pf_op_layernorm_ex: null input, half a split pair or no output");
+  if (!al16(x) || !al16(y) || !al16(w) || !al16(b) || !al16(hi) || !al16(lo) || !al16(phi) || !al16(plo)) return fail(PF_ERR_ARG, "pf_op_layernorm_ex: unaligned pointer");
+  if (!(eps > 0.f)) return fail(PF_ERR_ARG, "pf_op_layernorm_ex: eps %g", eps);
+  const SplitT s{(__nv_bfloat16*)hi, (__nv_bfloat16*)lo, C}, p{(__nv_bfloat16*)phi, (__nv_bfloat16*)plo, C};
+  const LnW lw{w, b};
+  return op_run("pf_op_layernorm_ex", 1, stream, [&](Fwd& F) {
+    if (phi) return F.ln_split_patch(x, s, p, rows, C, lw, eps, RH, RW, sr, y);
+    if (hi) return F.ln_split(x, s, rows, C, lw, eps, y);
+    return F.ln(x, y, rows, C, lw, eps);
+  });
+}
 int pf_op_dwconv3x3_gelu(const float* x, float* y, int B, int H, int W, int C, const float* w, const float* bias, void* stream) {
-  if (C % 4) return fail(PF_ERR_ARG, "C %% 4");
-  LAUNCHED(launch_pdl(dwconv3x3_gelu_kernel, dim3(ew_grid((long long)B * ((H + 1) / 2) * ((W + PF_DW3_PX - 1) / PF_DW3_PX) * (C / 4))), dim3(256), 0, (cudaStream_t)stream, x, y, B, H, W, C, w, bias, nullptr, nullptr));
-  return PF_OK;
+  return pf_op_dwconv3x3_gelu_ex(x, B, H, W, C, w, bias, y, nullptr, nullptr, stream);
+}
+int pf_op_dwconv3x3_gelu_ex(const float* x, int B, int H, int W, int C, const float* w, const float* bias, float* y, void* hi, void* lo, void* stream) {
+  if (!x || !w || !bias || !hi != !lo || (!y && !hi)) return fail(PF_ERR_ARG, "pf_op_dwconv3x3_gelu_ex: null input, half a split pair or no output");
+  if (!al16(x) || !al16(w) || !al16(bias) || !al16(y) || !al16(hi) || !al16(lo)) return fail(PF_ERR_ARG, "pf_op_dwconv3x3_gelu_ex: unaligned pointer");
+  const SplitT s{(__nv_bfloat16*)hi, (__nv_bfloat16*)lo, C};
+  return op_run("pf_op_dwconv3x3_gelu_ex", B, stream, [&](Fwd& F) { return F.dw3_gelu(x, y, s, H, W, C, w, bias); });
 }
 int pf_op_dwconv7x7(const float* x, float* y, int B, int H, int W, int C, const float* w, const float* bias, void* stream) {
-  if (C % 4) return fail(PF_ERR_ARG, "C %% 4");
-  LAUNCHED(launch_pdl(dwconv7x7_kernel, dim3(ew_grid((long long)B * ((H + 1) / 2) * ((W + PF_DW7_PX - 1) / PF_DW7_PX) * (C / 4))), dim3(256), 0, (cudaStream_t)stream, x, y, B, H, W, C, w, bias));
-  return PF_OK;
+  if (!x || !y || !w || !bias) return fail(PF_ERR_ARG, "pf_op_dwconv7x7: null argument");
+  if (!al16(x) || !al16(y) || !al16(w) || !al16(bias)) return fail(PF_ERR_ARG, "pf_op_dwconv7x7: unaligned pointer");
+  return op_run("pf_op_dwconv7x7", B, stream, [&](Fwd& F) { return pn_dw_launch(F, x, y, H, W, C, w, bias); });
 }
 int pf_op_upsample2x(const float* x, float* y, int B, int H, int W, int C, void* stream) {
-  if (C % 4) return fail(PF_ERR_ARG, "C %% 4");
-  LAUNCHED(launch_pdl(upsample2x_kernel, dim3(ew_grid(upsample2x_threads(B, H, W, C))), dim3(256), 0, (cudaStream_t)stream, x, C, 0, y, C, 0, B, H, W, C, nullptr, nullptr));
-  return PF_OK;
+  return pf_op_upsample2x_ex(x, C, 0, y, C, 0, nullptr, nullptr, B, H, W, C, stream);
+}
+int pf_op_upsample2x_ex(const float* x, int ldi, int icoff, float* y, int ldo, int ocoff, void* hi, void* lo, int B, int H, int W, int C, void* stream) {
+  if (!x || !hi != !lo || (!y && !hi)) return fail(PF_ERR_ARG, "pf_op_upsample2x_ex: null input, half a split pair or no output");
+  if (!al16(x) || !al16(y) || !al16(hi) || !al16(lo)) return fail(PF_ERR_ARG, "pf_op_upsample2x_ex: unaligned pointer");
+  const SplitT s{(__nv_bfloat16*)hi, (__nv_bfloat16*)lo, ldo};
+  return op_run("pf_op_upsample2x_ex", B, stream, [&](Fwd& F) { return F.up2x(x, ldi, icoff, y, ldo, ocoff, s, H, W, C); });
+}
+int pf_op_stem_gather(const float* x0, int B, int IH, int IW, int stride, void* hi, void* lo, void* stream) {
+  if (!x0 || !hi || !lo) return fail(PF_ERR_ARG, "pf_op_stem_gather: null argument");
+  if (!al16(hi) || !al16(lo)) return fail(PF_ERR_ARG, "pf_op_stem_gather: unaligned pointer");
+  const SplitT col{(__nv_bfloat16*)hi, (__nv_bfloat16*)lo, 160};
+  return op_run("pf_op_stem_gather", B, stream, [&](Fwd& F) { return F.stem_gather(x0, col, IH, IW, stride); });
+}
+int pf_op_pn_stem(const float* pin, int B, int SH, int SW, const float* w, const float* b, float* out, void* stream) {
+  if (!pin || !w || !b || !out) return fail(PF_ERR_ARG, "pf_op_pn_stem: null argument");
+  return op_run("pf_op_pn_stem", B, stream, [&](Fwd& F) { return F.pn_stem(pin, SH, SW, w, b, out); });
+}
+int pf_op_pack_fields(const float* grav, const float* lat, int B, int IH, int IW, int OH, int OW, float* out, void* stream) {
+  if (!grav || !lat || !out) return fail(PF_ERR_ARG, "pf_op_pack_fields: null argument");
+  if (!al16(out)) return fail(PF_ERR_ARG, "pf_op_pack_fields: unaligned output");
+  return op_run("pf_op_pack_fields", B, stream, [&](Fwd& F) { return F.pack_fields(grav, lat, IH, IW, OH, OW, out); });
+}
+int pf_op_param_tail(const float* feat, int n, int HW, const float* nw, const float* nb, const float* hw, const float* hb, int kind, float* params, float* raw,
+                     void* stream) {
+  if (!feat || !nw || !nb || !hw || !hb || !params) return fail(PF_ERR_ARG, "pf_op_param_tail: null argument");
+  const LnW norm{nw, nb};
+  return op_run("pf_op_param_tail", n, stream, [&](Fwd& F) { return F.param_tail(feat, HW, norm, hw, hb, kind, params, raw); });
+}
+int pf_op_pred_tail(const float* feat, int ld, int coff, const float* w, const float* b, float* out, int B, int HW, int NC, int mode, void* stream) {
+  if (!feat || !w || !b || !out) return fail(PF_ERR_ARG, "pf_op_pred_tail: null argument");
+  if (!al16(feat)) return fail(PF_ERR_ARG, "pf_op_pred_tail: unaligned input");
+  return op_run("pf_op_pred_tail", B, stream, [&](Fwd& F) { return F.pred_tail(feat, ld, coff, w, b, out, HW, NC, mode); });
 }
 int pf_op_preprocess(const uint8_t* img, int H, int W, const float* mean3, const float* std3, float* y, void* stream) {
   return pf_op_preprocess_sized(img, H, W, kNet, kNet, mean3, std3, y, stream);
