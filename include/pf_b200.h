@@ -323,6 +323,17 @@ int64_t pf_fit_camera_workspace(const pf_fit_image* images, int n);
 int pf_fit_camera(int device, const pf_fit_image* images, int n, const float* up_base, const float* lat_base, const uint8_t* mask_base,
                   int principal_point, double huber, int max_iterations, double* params, double* cost, int32_t* iterations,
                   int32_t* status, void* workspace, int64_t workspace_bytes, void* stream);
+/* The same fit over groups of images taken with one camera (DESIGN.md section 1, "Shared intrinsics"): image i belongs to group
+ * group_of[i] (a HOST int32[n], values 0 .. ngroups - 1, every group non-empty); each image has its own roll and pitch, each
+ * group one f_rel (and, with principal_point, one cx_rel, cy_rel), all relative to each image's own size.  params as above,
+ * with the group's shared values bit-identical across its members; cost[i] = image i's own cost at the group's final point;
+ * iterations[i], status[i] = the group's cost evaluations and status, except status 2 (NaN params and cost) for an image
+ * with fewer than 2 valid residuals or a zero on its roll / pitch diagonal, and for every image of a group left with fewer
+ * residuals than parameters.  workspace: DEVICE, 256-byte aligned, pf_fit_camera_groups_workspace bytes. */
+int64_t pf_fit_camera_groups_workspace(const pf_fit_image* images, int n, const int32_t* group_of, int ngroups);
+int pf_fit_camera_groups(int device, const pf_fit_image* images, int n, const int32_t* group_of, int ngroups, const float* up_base,
+                         const float* lat_base, const uint8_t* mask_base, int principal_point, double huber, int max_iterations, double* params,
+                         double* cost, int32_t* iterations, int32_t* status, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---- upright warp: straightened images from camera parameters (csrc/rectify.cuh) --------------------------------------------
  * Warps each uint8 image (1 or 3 channels, HWC) to a camera with roll 0, pitch 0 (or the input pitch with keep_pitch), a centred

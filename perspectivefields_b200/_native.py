@@ -221,6 +221,9 @@ def lib():
                                   vp, vp, vp, vp, vp, vp, vp, i64, vp]),
         "pf_fit_camera_workspace": (i64, [ctypes.POINTER(pf_fit_image), i32]),
         "pf_fit_camera": (i32, [i32, ctypes.POINTER(pf_fit_image), i32, vp, vp, vp, i32, ctypes.c_double, i32, vp, vp, vp, vp, vp, i64, vp]),
+        "pf_fit_camera_groups_workspace": (i64, [ctypes.POINTER(pf_fit_image), i32, ctypes.POINTER(ctypes.c_int32), i32]),
+        "pf_fit_camera_groups": (i32, [i32, ctypes.POINTER(pf_fit_image), i32, ctypes.POINTER(ctypes.c_int32), i32, vp, vp, vp, i32, ctypes.c_double,
+                                       i32, vp, vp, vp, vp, vp, i64, vp]),
         "pf_rectify_workspace": (i64, [ctypes.POINTER(pf_rectify_image), i32]),
         "pf_rectify_views": (i32, [i32, ctypes.POINTER(pf_rectify_image), i32, vp, vp, vp, vp, i32, vp, i32, i32, ctypes.c_double, i32,
                                    ctypes.POINTER(ctypes.c_int32), vp, vp, vp, i64, vp]),
@@ -291,7 +294,8 @@ EXPORTS = ["pf_abi_version", "pf_last_error", "pf_kernel_launch_count", "pf_crea
            "pf_profile_kernels_read", "pf_set_option", "pf_debug_enable", "pf_debug_count", "pf_debug_name", "pf_debug_numel",
            "pf_debug_copy", "pf_camera_fields", "pf_camera_fields_vp", "pf_pano_views", "pf_equi_views", "pf_draw_fields",
            "pf_encode_fields", "pf_head_losses_workspace", "pf_head_losses", "pf_field_errors_workspace", "pf_field_errors",
-           "pf_fit_camera_workspace", "pf_fit_camera", "pf_rectify_workspace", "pf_rectify_views", "pf_comm_unique_id", "pf_comm_create", "pf_comm_destroy", "pf_gather",
+           "pf_fit_camera_workspace", "pf_fit_camera", "pf_fit_camera_groups_workspace", "pf_fit_camera_groups",
+           "pf_rectify_workspace", "pf_rectify_views", "pf_comm_unique_id", "pf_comm_create", "pf_comm_destroy", "pf_gather",
            "pf_jpeg_create", "pf_jpeg_destroy", "pf_jpeg_info", "pf_jpeg_decode_batch",
            "pf_op_conv_gemm", "pf_op_tma", "pf_op_tma_bf16", "pf_op_conv1_ring", "pf_tma_pick_tile", "pf_op_layernorm",
            "pf_op_attention_tc", "pf_op_attention_tc_bf16", "pf_op_attention_tc_keys", "pf_op_dwconv3x3_gelu",

@@ -3,11 +3,16 @@
 ``fit_camera`` fits roll, pitch, focal length and optionally the principal point to the up and latitude fields of each image
 by Levenberg-Marquardt (this project's rule, DESIGN.md section 1 "Camera fit").  It gives every field-only variant
 (``PersNet-360Cities``) the camera parameters its ParamNet-less model lacks, and gives ParamNet variants a geometric check or
-refinement of theirs.  Its output has the keys of a ParamNet variant's results, so ``metrics.param_errors``,
-``panocam.fields_from_predictions`` and ``viz.draw_from_r_p_f_cx_cy`` take it unchanged.
+refinement of theirs.  With ``groups`` it fits images taken with one camera together (the frames of a video, a burst, one
+phone's photos): each image keeps its own roll and pitch, and each group gets one focal length (and principal point), which one
+image alone constrains least (DESIGN.md section 1, "Shared intrinsics").  Its output has the keys of a ParamNet variant's
+results, so ``metrics.param_errors``, ``panocam.fields_from_predictions`` and ``viz.draw_from_r_p_f_cx_cy`` take it unchanged.
 """
+import ctypes
 import math
+import numbers
 
+import numpy as np
 import torch
 
 from . import _batch, _native
@@ -35,7 +40,23 @@ def _init_from_results(results):
     return out
 
 
-def fit_camera(results, principal_point=False, init="fields", mask=None, huber=None, max_iterations=50):
+def _group_ids(groups, n):
+    """Labels compacted in order of first appearance: (int32 group of each image, number of groups)."""
+    try:
+        labels = list(groups)
+    except TypeError:
+        raise ValueError(f"groups must be None or a sequence of {n} integers, got {groups!r}") from None
+    if len(labels) != n:
+        raise ValueError(f"{n} results but {len(labels)} group labels")
+    ids = {}
+    for i, v in enumerate(labels):
+        if isinstance(v, (bool, np.bool_)) or not isinstance(v, numbers.Integral):
+            raise ValueError(f"groups[{i}] must be an integer, got {v!r}")
+        ids.setdefault(int(v), len(ids))
+    return (ctypes.c_int32 * n)(*(ids[int(v)] for v in labels)), len(ids)
+
+
+def fit_camera(results, principal_point=False, init="fields", mask=None, huber=None, max_iterations=50, groups=None):
     """Fit one camera per image to ``results[i]["pred_gravity_original"]`` ([2, H, W] up vectors) and
     ``["pred_latitude_original"]`` ([H, W], degrees), read in place; sizes may differ within one call.  A dict of ground-truth
     fields works too, e.g. ``{"pred_gravity_original": up.permute(2, 0, 1), "pred_latitude_original": lat}``.
@@ -45,7 +66,14 @@ def fit_camera(results, principal_point=False, init="fields", mask=None, huber=N
       carry; this reads them on the host, the one case that synchronises).
     - ``mask``: None or a list of bool [H, W] tensors (None entries allowed) that restricts both fields.
     - ``huber``: None (least squares) or the Huber scale delta in radians (``least_squares(loss="huber", f_scale=delta)``).
-    - ``max_iterations``: the most cost evaluations per image (1 .. 1000).
+    - ``max_iterations``: the most cost evaluations per image (1 .. 1000), per group with ``groups``.
+    - ``groups``: None (one camera per image) or a sequence of n integers (numpy integers too, not bools): images with equal
+      labels were taken with one camera.  They are fitted together, with their own roll and pitch and one shared f_rel (and,
+      with ``principal_point``, one cx_rel, cy_rel), relative to each image's own size: a group may mix resolutions only if
+      they are scaled copies of one camera (this is not checked).  The shared values are bit-identical across the group;
+      ``fit_cost`` is each image's own cost at the group's final point, and ``fit_iterations`` and ``fit_status`` are the
+      group's, except that an image with too few valid residuals is dropped from its group with status 2.  The start of the
+      shared values is the mean of the members' starts.
 
     Returns one dict per image, as 0-dim float64 CUDA tensors in degrees: the keys of a centred (``principal_point=False``:
     ``pred_roll, pred_pitch, pred_vfov, pred_rel_focal, pred_general_vfov, pred_rel_cx, pred_rel_cy``) or uncentred ParamNet
@@ -65,6 +93,7 @@ def fit_camera(results, principal_point=False, init="fields", mask=None, huber=N
     n = len(results)
     if mask is not None and len(mask) != n:
         raise ValueError(f"{n} results but {len(mask)} masks")
+    group_of = None if groups is None else _group_ids(groups, n)
     if n == 0:
         return []
     pu, pl, ms, dev = _batch.prediction_fields(results, mask, 3)
@@ -80,15 +109,21 @@ def fit_camera(results, principal_point=False, init="fields", mask=None, huber=N
         d.mask_offset = _batch.offset(ms[i], bm)
         d.init[:] = starts[i]
     with torch.cuda.device(dev):
-        ws = _batch.workspace(L.pf_fit_camera_workspace(descs, n), dev)
+        if group_of is None:
+            ws = _batch.workspace(L.pf_fit_camera_workspace(descs, n), dev)
+        else:
+            ws = _batch.workspace(L.pf_fit_camera_groups_workspace(descs, n, group_of[0], group_of[1]), dev)
         params = torch.empty((n, 5), dtype=torch.float64, device=dev)
         cost = torch.empty(n, dtype=torch.float64, device=dev)
         its = torch.empty(n, dtype=torch.int32, device=dev)
         status = torch.empty(n, dtype=torch.int32, device=dev)
         stream = torch.cuda.current_stream(dev).cuda_stream
-        _native.check(L.pf_fit_camera(dev.index, descs, n, bu, bl, bm or None, int(principal_point), float(huber or 0.0), max_iterations,
-                                      params.data_ptr(), cost.data_ptr(), its.data_ptr(), status.data_ptr(), ws.data_ptr(), ws.numel(),
-                                      stream))
+        fields = (bu, bl, bm or None, int(principal_point), float(huber or 0.0), max_iterations, params.data_ptr(), cost.data_ptr(),
+                  its.data_ptr(), status.data_ptr(), ws.data_ptr(), ws.numel(), stream)
+        if group_of is None:
+            _native.check(L.pf_fit_camera(dev.index, descs, n, *fields))
+        else:
+            _native.check(L.pf_fit_camera_groups(dev.index, descs, n, group_of[0], group_of[1], *fields))
         roll, pitch, f, cx, cy = params.t()
         gv = general_vfov(cx, cy, 1, f, True)
         if principal_point:

@@ -16,6 +16,9 @@
 // candidate, as per-block fp64 partials) and fit_step_kernel (reduce the partials in a fixed order, accept or reject, solve the
 // damped normal equations by Cholesky, write the next candidate or the result).  Images that have stopped cost their pass
 // blocks one early exit.  No floating-point atomic decides a value: repeated calls are bit-identical.
+//
+// Groups of images with shared intrinsics (pf_fit_camera_groups, "shared intrinsics" below) reuse the start and the pass, and
+// replace the step by fit_reduce_kernel (each image's sums) and fit_group_step_kernel (one Schur-complement step per group).
 #pragma once
 #include <stdint.h>
 
@@ -301,8 +304,21 @@ __device__ void fit_finish(const FitArgs& a, int i, FitState& s, int status) {
   s.status = status;
 }
 
-// One warp per image: the partials of its last pass summed in a fixed order (lane-strided serial sums, then a shuffle tree),
-// then lane 0 runs one step of the loop.
+// The partials of image d's last pass summed in a fixed order by one warp: lane-strided serial sums, then a shuffle tree.
+// Lane 0 holds the NQ sums.
+template <int P>
+__device__ __forceinline__ void fit_reduce_partials(const FitArgs& a, const FitImage& d, int lane, double (&v)[fit_nq(P)]) {
+#pragma unroll
+  for (int q = 0; q < fit_nq(P); ++q) {
+    double t = 0.0;
+    for (int b = lane; b < d.nblk; b += 32) t += a.part[(long long)q * a.nblocks + d.block0 + b];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) t += __shfl_down_sync(0xffffffffu, t, o);
+    v[q] = t;
+  }
+}
+
+// One warp per image: the partials of its last pass summed (fit_reduce_partials), then lane 0 runs one step of the loop.
 template <int P>
 __global__ void __launch_bounds__(32 * kFitStepWarps) fit_step_kernel(FitArgs a) {
   constexpr int NQ = fit_nq(P), NA = P * (P + 1) / 2;
@@ -315,14 +331,7 @@ __global__ void __launch_bounds__(32 * kFitStepWarps) fit_step_kernel(FitArgs a)
   if (s.status != kFitRunning) return;
   const FitImage d = a.im[i];
   double v[NQ];
-#pragma unroll
-  for (int q = 0; q < NQ; ++q) {
-    double t = 0.0;
-    for (int b = lane; b < d.nblk; b += 32) t += a.part[(long long)q * a.nblocks + d.block0 + b];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) t += __shfl_down_sync(0xffffffffu, t, o);
-    v[q] = t;
-  }
+  fit_reduce_partials<P>(a, d, lane, v);
   if (lane != 0) return;
   const double Cc = 0.5 * v[0];
   s.evals += 1;
@@ -359,6 +368,262 @@ __global__ void __launch_bounds__(32 * kFitStepWarps) fit_step_kernel(FitArgs a)
   if (small) { fit_finish<P>(a, i, s, 0); return; }
   if (s.evals >= a.max_iter) { fit_finish<P>(a, i, s, 1); return; }
   for (int k = 0; k < P; ++k) s.cand[k] = s.theta[k] + delta[k];
+}
+
+// ------------------------------------------------------------------------------------------------------ shared intrinsics
+// Groups of images from one camera (DESIGN.md section 1, "Shared intrinsics"): per-image roll and pitch, one s = ln f_rel (and
+// cx_rel, cy_rel with principal_point) per group.  The pass is fit_pass_kernel's; fit_reduce_kernel writes each running
+// image's sums, and fit_group_step_kernel (one block per group) takes one Levenberg-Marquardt step on the group's joint
+// normal equations by a Schur complement on the shared parameters.  An image's FitState keeps its own theta (the shared
+// entries equal the group's, bit for bit), A, g and C_i at the accepted point; status 2 marks a dropped member.
+constexpr int kFitGroupThreads = 256;
+
+struct FitGroupState {
+  double shared[3], cand[3];   // accepted (s, cx_rel, cy_rel) and the candidate's
+  double C, lambda;            // C_G at the accepted point
+  int evals, status;           // cost evaluations of the group so far; kFitRunning, or the group's final status
+};
+struct FitGroups {
+  const int* off;              // [ngroups + 1]: group G's members are mem[off[G] .. off[G + 1] - 1]
+  const int* mem;              // [n] image indices, in index order within each group
+  FitGroupState* gs;           // [ngroups]
+  double* sums;                // [n][kFitQ]: each running image's sums of its last pass
+  int ngroups;
+};
+
+// Entry (i, j), i <= j, of a P x P upper triangle stored row by row
+__host__ __device__ constexpr int fit_up(int P, int i, int j) { return i * P - i * (i - 1) / 2 + (j - i); }
+
+// Deterministic block sum of N values per thread (fixed shuffle trees, then the warps' partials in warp order); every thread
+// gets the same bits.  sh: [blockDim.x / 32][N] doubles in shared memory.
+template <int N>
+__device__ __forceinline__ void fit_block_sum(double (&v)[N], double* sh) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+#pragma unroll
+  for (int q = 0; q < N; ++q)
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v[q] += __shfl_down_sync(0xffffffffu, v[q], o);
+  __syncthreads();   // sh may still be read by the previous call
+  if (lane == 0)
+#pragma unroll
+    for (int q = 0; q < N; ++q) sh[warp * N + q] = v[q];
+  __syncthreads();
+#pragma unroll
+  for (int q = 0; q < N; ++q) {
+    double t = sh[q];
+    for (int w = 1; w < nw; ++w) t += sh[w * N + q];
+    v[q] = t;
+  }
+}
+
+// The damped local block B = A[ll] + lambda diag A[ll] of one image by Cholesky, kept as L's off-diagonal entry and the
+// reciprocals of its diagonal (two divisions per factorisation, none per solve): false if B is not positive definite
+struct FitLocal {
+  double r00, l10, r11;
+  __device__ __forceinline__ bool factor(const double* A, int P, double lambda) {
+    const double b00 = A[0] + lambda * A[0], b01 = A[1], b11 = A[P] + lambda * A[P];
+    if (!(b00 > 0.0)) return false;
+    r00 = 1.0 / sqrt(b00);
+    l10 = b01 * r00;
+    const double t = b11 - l10 * l10;
+    if (!(t > 0.0)) return false;
+    r11 = 1.0 / sqrt(t);
+    return true;
+  }
+  __device__ __forceinline__ void solve(double b0, double b1, double& x0, double& x1) const {   // B x = b
+    const double y0 = b0 * r00, y1 = (b1 - l10 * y0) * r11;
+    x1 = y1 * r11;
+    x0 = (y0 - l10 * x1) * r00;
+  }
+};
+
+// One thread per group: the shared entries of the start are the mean, in index order, of the members' starts
+__global__ void __launch_bounds__(128) fit_group_init_kernel(FitArgs a, FitGroups g) {
+  pdl_wait();
+  pdl_launch();
+  const int G = blockIdx.x * blockDim.x + threadIdx.x;
+  if (G >= g.ngroups) return;
+  const int m0 = g.off[G], m1 = g.off[G + 1];
+  double sh[3];
+  for (int k = 0; k < 3; ++k) {
+    double t = a.st[g.mem[m0]].cand[2 + k];
+    for (int j = m0 + 1; j < m1; ++j) t += a.st[g.mem[j]].cand[2 + k];
+    sh[k] = t / (double)(m1 - m0);
+  }
+  for (int j = m0; j < m1; ++j) {
+    FitState& s = a.st[g.mem[j]];
+    for (int k = 0; k < 3; ++k) s.cand[2 + k] = s.theta[2 + k] = sh[k];
+  }
+  FitGroupState& gs = g.gs[G];
+  for (int k = 0; k < 3; ++k) gs.shared[k] = gs.cand[k] = sh[k];
+  gs.C = 0.0; gs.lambda = kFitLambda0; gs.evals = 0; gs.status = kFitRunning;
+}
+
+// One warp per image: the sums of a running image's last pass (fit_reduce_partials) into g.sums
+template <int P>
+__global__ void __launch_bounds__(32 * kFitStepWarps) fit_reduce_kernel(FitArgs a, FitGroups g) {
+  constexpr int NQ = fit_nq(P);
+  pdl_wait();
+  pdl_launch();
+  const int lane = threadIdx.x & 31;
+  const int i = blockIdx.x * kFitStepWarps + (threadIdx.x >> 5);
+  if (i >= a.n || a.st[i].status != kFitRunning) return;
+  const FitImage d = a.im[i];
+  double v[NQ];
+  fit_reduce_partials<P>(a, d, lane, v);
+  if (lane == 0)
+#pragma unroll
+    for (int q = 0; q < NQ; ++q) g.sums[(long long)i * kFitQ + q] = v[q];
+}
+
+// One block per group: accept or reject the candidate on C_G, then solve (A + lambda diag A) delta = -g over the group's
+// parameters (locals l = roll, pitch of each member; shared s = K entries) by a Schur complement on the shared block:
+//   S = D_lambda - sum E_i^T B_i^-1 E_i,  b = -g_s + sum E_i^T B_i^-1 g_l,i,  S ds = b,  dl_i = B_i^-1 (-g_l,i - E_i ds).
+// Each thread takes members off[G] + threadIdx.x, + blockDim.x, ...; the sums over members are fixed-order block sums, and
+// every thread solves the K x K system on the same bits.
+template <int P>
+__global__ void __launch_bounds__(kFitGroupThreads, 1) fit_group_step_kernel(FitArgs a, FitGroups g) {
+  constexpr int K = P - 2, NK = K * (K + 1) / 2;
+  constexpr int OD = 0, OG = NK, OS = NK + K, OB = 2 * NK + K, OF = 2 * NK + 2 * K, NR = OF + 1;   // sums of the lambda loop
+  __shared__ double shr[kFitGroupThreads / 32 * NR];
+  pdl_wait();
+  pdl_launch();
+  FitGroupState& gs = g.gs[blockIdx.x];
+  if (gs.status != kFitRunning) return;
+  const int m0 = g.off[blockIdx.x], m1 = g.off[blockIdx.x + 1];
+  const int evals = gs.evals + 1;
+  double lambda = gs.lambda, C = gs.C, th[K], cs[K];
+#pragma unroll
+  for (int c = 0; c < K; ++c) { th[c] = gs.shared[c]; cs[c] = gs.cand[c]; }
+  auto accept = [&](FitState& s, const double* v) {
+    s.C = 0.5 * v[0];
+#pragma unroll
+    for (int k = 0; k < P; ++k) { s.theta[k] = s.cand[k]; s.g[k] = v[2 + k]; }
+#pragma unroll
+    for (int k = 0; k < P * (P + 1) / 2; ++k) s.A[k] = v[2 + P + k];
+  };
+  // One step; returns the group's final status, or kFitRunning.  gs is written only after the first block sum, when every
+  // thread has read it.
+  const int status = [&]() -> int {
+    if (evals == 1) {   // the start: drop members without a usable local block, then check what is left
+      double r[3 + K] = {};   // residuals, C_G, members kept, diag D
+      for (int j = m0 + (int)threadIdx.x; j < m1; j += blockDim.x) {
+        const int i = g.mem[j];
+        FitState& s = a.st[i];
+        const double* v = g.sums + (long long)i * kFitQ;
+        if (v[1] < 2.0 || v[2 + P + fit_up(P, 0, 0)] == 0.0 || v[2 + P + fit_up(P, 1, 1)] == 0.0) { s.status = 2; continue; }
+        r[0] += v[1]; r[1] += 0.5 * v[0]; r[2] += 1.0;
+#pragma unroll
+        for (int c = 0; c < K; ++c) r[3 + c] += v[2 + P + fit_up(P, 2 + c, 2 + c)];
+        accept(s, v);
+      }
+      fit_block_sum<3 + K>(r, shr);
+      bool bad = r[2] == 0.0 || r[0] < 2.0 * r[2] + K;
+#pragma unroll
+      for (int c = 0; c < K; ++c) bad = bad || r[3 + c] == 0.0;
+      if (bad) return 2;
+      C = r[1];
+    } else {
+      double r[1] = {0.0};
+      for (int j = m0 + (int)threadIdx.x; j < m1; j += blockDim.x) {
+        const int i = g.mem[j];
+        if (a.st[i].status == kFitRunning) r[0] += 0.5 * g.sums[(long long)i * kFitQ];
+      }
+      fit_block_sum<1>(r, shr);
+      if (r[0] < C) {   // accept
+        const bool done = C - r[0] <= kFitCostRtol * C;
+        C = r[0];
+        for (int j = m0 + (int)threadIdx.x; j < m1; j += blockDim.x) {
+          const int i = g.mem[j];
+          FitState& s = a.st[i];
+          if (s.status == kFitRunning) accept(s, g.sums + (long long)i * kFitQ);
+        }
+#pragma unroll
+        for (int c = 0; c < K; ++c) th[c] = cs[c];
+        lambda /= 10.0;
+        if (done) return 0;
+      } else {          // reject: keep theta, A, g
+        lambda *= 10.0;
+        if (lambda > kFitLambdaMax) return 0;
+      }
+    }
+    double ds[K];
+    bool ok = false;
+    while (lambda <= kFitLambdaMax) {
+      double r[NR] = {};   // D (upper triangle), g_s, sum E^T B^-1 E (upper triangle), sum E^T B^-1 g_l, members with B not PD
+      for (int j = m0 + (int)threadIdx.x; j < m1; j += blockDim.x) {
+        const FitState& s = a.st[g.mem[j]];
+        if (s.status != kFitRunning) continue;
+#pragma unroll
+        for (int c = 0, q = 0; c < K; ++c) {
+          r[OG + c] += s.g[2 + c];
+#pragma unroll
+          for (int e = c; e < K; ++e, ++q) r[OD + q] += s.A[fit_up(P, 2 + c, 2 + e)];
+        }
+        FitLocal B;
+        if (!B.factor(s.A, P, lambda)) { r[OF] += 1.0; continue; }
+        double X0[K], X1[K], y0, y1;
+        B.solve(s.g[0], s.g[1], y0, y1);
+#pragma unroll
+        for (int c = 0; c < K; ++c) B.solve(s.A[fit_up(P, 0, 2 + c)], s.A[fit_up(P, 1, 2 + c)], X0[c], X1[c]);
+#pragma unroll
+        for (int c = 0, q = 0; c < K; ++c) {
+          const double e0 = s.A[fit_up(P, 0, 2 + c)], e1 = s.A[fit_up(P, 1, 2 + c)];
+          r[OB + c] += e0 * y0 + e1 * y1;
+#pragma unroll
+          for (int e = c; e < K; ++e, ++q) r[OS + q] += e0 * X0[e] + e1 * X1[e];
+        }
+      }
+      fit_block_sum<NR>(r, shr);
+      if (r[OF] == 0.0) {
+        double S[NK], b[K];
+#pragma unroll
+        for (int c = 0, q = 0; c < K; ++c) {
+          b[c] = -r[OG + c] + r[OB + c];
+#pragma unroll
+          for (int e = c; e < K; ++e, ++q) S[q] = (e == c ? r[OD + q] + lambda * r[OD + q] : r[OD + q]) - r[OS + q];
+        }
+        if ((ok = cholesky_solve<K>(S, b, ds))) break;
+      }
+      lambda *= 10.0;
+    }
+    if (!ok) return 0;
+    double big[1] = {0.0};   // members with a local step above the tolerance
+    for (int j = m0 + (int)threadIdx.x; j < m1; j += blockDim.x) {
+      FitState& s = a.st[g.mem[j]];
+      if (s.status != kFitRunning) continue;
+      FitLocal B;
+      B.factor(s.A, P, lambda);   // positive definite: the same bits passed above
+      double b0 = -s.g[0], b1 = -s.g[1], x0, x1;
+#pragma unroll
+      for (int c = 0; c < K; ++c) { b0 -= s.A[fit_up(P, 0, 2 + c)] * ds[c]; b1 -= s.A[fit_up(P, 1, 2 + c)] * ds[c]; }
+      B.solve(b0, b1, x0, x1);
+      if (!(fabs(x0) <= kFitStepRtol * (1.0 + fabs(s.theta[0])) && fabs(x1) <= kFitStepRtol * (1.0 + fabs(s.theta[1])))) big[0] += 1.0;
+      s.cand[0] = s.theta[0] + x0; s.cand[1] = s.theta[1] + x1;
+#pragma unroll
+      for (int c = 0; c < K; ++c) s.cand[2 + c] = th[c] + ds[c];
+    }
+    fit_block_sum<1>(big, shr);
+    bool small = big[0] == 0.0;
+#pragma unroll
+    for (int c = 0; c < K; ++c) small = small && fabs(ds[c]) <= kFitStepRtol * (1.0 + fabs(th[c]));
+    if (small) return 0;
+    if (evals >= a.max_iter) return 1;
+    if (threadIdx.x == 0) {
+#pragma unroll
+      for (int c = 0; c < K; ++c) { gs.shared[c] = th[c]; gs.cand[c] = th[c] + ds[c]; }
+      gs.C = C; gs.lambda = lambda; gs.evals = evals;
+    }
+    return kFitRunning;
+  }();
+  if (status == kFitRunning) return;
+  for (int j = m0 + (int)threadIdx.x; j < m1; j += blockDim.x) {   // finish: every member, dropped ones with status 2
+    const int i = g.mem[j];
+    FitState& s = a.st[i];
+    s.evals = evals;
+    fit_finish<P>(a, i, s, s.status == 2 ? 2 : status);
+  }
+  if (threadIdx.x == 0) { gs.evals = evals; gs.status = status; }
 }
 
 }  // namespace pf

@@ -138,7 +138,7 @@ static long long align256(long long b) { return (b + 255) / 256 * 256; }
 // A caller-provided workspace carved into 256-byte-aligned sections, in the order they are added: at[k] is the byte offset of
 // section k; the first holds the per-image descriptors (upload_descriptors)
 struct WsLayout {
-  long long at[4] = {}, total = 0;
+  long long at[8] = {}, total = 0;
   int count = 0;
   WsLayout& add(long long bytes) { at[count++] = total; total += align256(bytes); return *this; }
 };
@@ -396,24 +396,54 @@ int pf_field_errors(int device, const pf_field_image* images, int n, const float
 }
 
 // ----------------------------------------------------------------------------------------------- camera fit (calib.cuh)
-// Workspace layout of pf_fit_camera: device descriptors | per-image state | fp64 partials [kFitQ][pass blocks]
+// Workspace layout of pf_fit_camera: device descriptors | per-image state | fp64 partials [kFitQ][pass blocks]; pf_fit_camera_groups
+// adds | per-group state | per-image sums [n][kFitQ] | the groups' member offsets [ngroups + 1] and members [n]
 constexpr int kFitMaxIterations = 1000;
-static int fit_layout(const pf_fit_image* im, int n, WsLayout* lay, long long* blocks_out = nullptr) {
-  if (!im || n < 1) return fail(PF_ERR_ARG, "pf_fit_camera: null images or n < 1");
+static int fit_layout(const char* fn, const pf_fit_image* im, int n, WsLayout* lay, long long* blocks_out = nullptr) {
+  if (!im || n < 1) return fail(PF_ERR_ARG, "%s: null images or n < 1", fn);
   long long blocks = 0;
   for (int i = 0; i < n; ++i) {
     if (im[i].height < 3 || im[i].width < 3 || (long long)im[i].height * im[i].width >= (1LL << 31))
-      return fail(PF_ERR_ARG, "pf_fit_camera: image %d has size %dx%d (3x3 at least)", i, im[i].height, im[i].width);
+      return fail(PF_ERR_ARG, "%s: image %d has size %dx%d (3x3 at least)", fn, i, im[i].height, im[i].width);
     blocks += cdivl((long long)im[i].height * im[i].width, kFitTile);
   }
-  if (blocks >= (1LL << 31)) return fail(PF_ERR_ARG, "pf_fit_camera: too many pixels");
+  if (blocks >= (1LL << 31)) return fail(PF_ERR_ARG, "%s: too many pixels", fn);
   lay->add((long long)n * sizeof(FitImage)).add((long long)n * sizeof(FitState)).add((long long)kFitQ * blocks * 8);
   if (blocks_out) *blocks_out = blocks;
   return PF_OK;
 }
 int64_t pf_fit_camera_workspace(const pf_fit_image* images, int n) {
   WsLayout lay;
-  TRY(fit_layout(images, n, &lay));
+  TRY(fit_layout("pf_fit_camera", images, n, &lay));
+  return lay.total;
+}
+
+// The groups in CSR form: csr[0 .. ngroups] member offsets, then the members of each group in index order
+static int fit_groups_layout(const pf_fit_image* im, int n, const int32_t* group_of, int ngroups, WsLayout* lay, long long* blocks_out = nullptr,
+                             std::vector<int>* csr = nullptr) {
+  TRY(fit_layout("pf_fit_camera_groups", im, n, lay, blocks_out));
+  if (!group_of || ngroups < 1) return fail(PF_ERR_ARG, "pf_fit_camera_groups: null group_of or ngroups < 1");
+  std::vector<int> off(ngroups + 1, 0);
+  for (int i = 0; i < n; ++i) {
+    if (group_of[i] < 0 || group_of[i] >= ngroups)
+      return fail(PF_ERR_ARG, "pf_fit_camera_groups: image %d has group %d outside 0 .. %d", i, group_of[i], ngroups - 1);
+    off[group_of[i] + 1] += 1;
+  }
+  for (int G = 0; G < ngroups; ++G) {
+    if (off[G + 1] == 0) return fail(PF_ERR_ARG, "pf_fit_camera_groups: group %d has no image", G);
+    off[G + 1] += off[G];
+  }
+  lay->add((long long)ngroups * sizeof(FitGroupState)).add((long long)n * kFitQ * 8).add((long long)(ngroups + 1 + n) * 4);
+  if (csr) {
+    csr->assign(off.begin(), off.end());
+    csr->resize(ngroups + 1 + n);
+    for (int i = 0; i < n; ++i) (*csr)[ngroups + 1 + off[group_of[i]]++] = i;
+  }
+  return PF_OK;
+}
+int64_t pf_fit_camera_groups_workspace(const pf_fit_image* images, int n, const int32_t* group_of, int ngroups) {
+  WsLayout lay;
+  TRY(fit_groups_layout(images, n, group_of, ngroups, &lay));
   return lay.total;
 }
 
@@ -424,32 +454,31 @@ struct PdlScope {
   ~PdlScope() { pdl_enabled() = false; }
 };
 
-int pf_fit_camera(int device, const pf_fit_image* images, int n, const float* up_base, const float* lat_base, const uint8_t* mask_base,
-                  int principal_point, double huber, int max_iterations, double* params, double* cost, int32_t* iterations,
-                  int32_t* status, void* workspace, int64_t workspace_bytes, void* stream) {
-  WsLayout lay;
-  long long blocks;
-  TRY(fit_layout(images, n, &lay, &blocks));
+// The argument checks both fits share and the kernels' arguments; uploads the descriptors into the workspace
+static int fit_prepare(const char* fn, const WsLayout& lay, long long blocks, const pf_fit_image* images, int n, const float* up_base,
+                       const float* lat_base, const uint8_t* mask_base, int principal_point, double huber, int max_iterations, double* params,
+                       double* cost, int32_t* iterations, int32_t* status, void* workspace, int64_t workspace_bytes, std::vector<FitImage>* d,
+                       FitArgs* a) {
   if (!up_base || !lat_base || !params || !cost || !iterations || !status || !workspace)
-    return fail(PF_ERR_ARG, "pf_fit_camera: null field / output / workspace");
-  if (principal_point != 0 && principal_point != 1) return fail(PF_ERR_ARG, "pf_fit_camera: principal_point must be 0 or 1");
+    return fail(PF_ERR_ARG, "%s: null field / output / workspace", fn);
+  if (principal_point != 0 && principal_point != 1) return fail(PF_ERR_ARG, "%s: principal_point must be 0 or 1", fn);
   if (!(huber == 0.0 || (std::isfinite(huber) && huber > 0.0)))
-    return fail(PF_ERR_ARG, "pf_fit_camera: huber must be 0 (least squares) or finite and > 0, got %g", huber);
+    return fail(PF_ERR_ARG, "%s: huber must be 0 (least squares) or finite and > 0, got %g", fn, huber);
   if (max_iterations < 1 || max_iterations > kFitMaxIterations)
-    return fail(PF_ERR_ARG, "pf_fit_camera: max_iterations %d outside 1 .. %d", max_iterations, kFitMaxIterations);
-  TRY(check_workspace("pf_fit_camera", workspace, workspace_bytes, lay.total));
-  std::vector<FitImage> d(n);
+    return fail(PF_ERR_ARG, "%s: max_iterations %d outside 1 .. %d", fn, max_iterations, kFitMaxIterations);
+  TRY(check_workspace(fn, workspace, workspace_bytes, lay.total));
+  d->resize(n);
   long long block0 = 0;
   for (int i = 0; i < n; ++i) {
     const pf_fit_image& c = images[i];
-    TRY(check_offsets("pf_fit_camera", i, {c.up_offset, c.lat_offset}, {{c.mask_offset, mask_base}}));
-    if (c.up_stride[0] < 0 || c.up_stride[1] < 0 || c.up_stride[2] < 0) return fail(PF_ERR_ARG, "pf_fit_camera: image %d has a negative stride", i);
+    TRY(check_offsets(fn, i, {c.up_offset, c.lat_offset}, {{c.mask_offset, mask_base}}));
+    if (c.up_stride[0] < 0 || c.up_stride[1] < 0 || c.up_stride[2] < 0) return fail(PF_ERR_ARG, "%s: image %d has a negative stride", fn, i);
     if (!std::isnan(c.init[0])) {
       bool fin = true;
       for (int k = 0; k < 5; ++k) fin = fin && std::isfinite(c.init[k]);
-      if (!fin || !(c.init[2] > 0.0)) return fail(PF_ERR_ARG, "pf_fit_camera: image %d: init must be finite with f_rel > 0 (or a NaN roll)", i);
+      if (!fin || !(c.init[2] > 0.0)) return fail(PF_ERR_ARG, "%s: image %d: init must be finite with f_rel > 0 (or a NaN roll)", fn, i);
     }
-    FitImage& o = d[i];
+    FitImage& o = (*d)[i];
     o.H = c.height; o.W = c.width;
     o.up_off = c.up_offset; o.up_sr = c.up_stride[0]; o.up_sc = c.up_stride[1]; o.up_sk = c.up_stride[2];
     o.lat_off = c.lat_offset;
@@ -458,16 +487,29 @@ int pf_fit_camera(int device, const pf_fit_image* images, int n, const float* up
     o.block0 = (int)block0; o.nblk = (int)cdivl((long long)c.height * c.width, kFitTile);
     block0 += o.nblk;
   }
+  char* ws = (char*)workspace;
+  *a = FitArgs{};
+  a->im = (const FitImage*)ws; a->st = (FitState*)(ws + lay.at[1]); a->n = n; a->nblocks = (int)blocks;
+  a->up = up_base; a->lat = lat_base; a->mask = mask_base;
+  a->huber = huber; a->max_iter = max_iterations;
+  a->part = (double*)(ws + lay.at[2]);
+  a->params = params; a->cost = cost; a->iters = iterations; a->status = status;
+  return PF_OK;
+}
+
+int pf_fit_camera(int device, const pf_fit_image* images, int n, const float* up_base, const float* lat_base, const uint8_t* mask_base,
+                  int principal_point, double huber, int max_iterations, double* params, double* cost, int32_t* iterations,
+                  int32_t* status, void* workspace, int64_t workspace_bytes, void* stream) {
+  WsLayout lay;
+  long long blocks;
+  TRY(fit_layout("pf_fit_camera", images, n, &lay, &blocks));
+  std::vector<FitImage> d;
+  FitArgs a;
+  TRY(fit_prepare("pf_fit_camera", lay, blocks, images, n, up_base, lat_base, mask_base, principal_point, huber, max_iterations, params, cost,
+                  iterations, status, workspace, workspace_bytes, &d, &a));
   CU(cudaSetDevice(device));
   cudaStream_t st = (cudaStream_t)stream;
-  char* ws = (char*)workspace;
-  FitArgs a{};
-  a.im = (const FitImage*)ws; a.st = (FitState*)(ws + lay.at[1]); a.n = n; a.nblocks = (int)blocks;
-  a.up = up_base; a.lat = lat_base; a.mask = mask_base;
-  a.huber = huber; a.max_iter = max_iterations;
-  a.part = (double*)(ws + lay.at[2]);
-  a.params = params; a.cost = cost; a.iters = iterations; a.status = status;
-  TRY(upload_descriptors(d.data(), d.size() * sizeof(d[0]), ws, st));
+  TRY(upload_descriptors(d.data(), d.size() * sizeof(d[0]), workspace, st));
   const PdlScope pdl(!sync_debug());
   const dim3 pass_grid((unsigned)blocks), step_grid((unsigned)cdiv(n, kFitStepWarps));
   LAUNCHED(launch_pdl(fit_init_kernel, dim3(n), dim3(64), 0, st, a, principal_point));
@@ -478,6 +520,46 @@ int pf_fit_camera(int device, const pf_fit_image* images, int n, const float* up
     } else {
       LAUNCHED(launch_pdl(fit_pass_kernel<3>, pass_grid, dim3(kFitThreads), 0, st, a));
       LAUNCHED(launch_pdl(fit_step_kernel<3>, step_grid, dim3(32 * kFitStepWarps), 0, st, a));
+    }
+  }
+  return PF_OK;
+}
+
+int pf_fit_camera_groups(int device, const pf_fit_image* images, int n, const int32_t* group_of, int ngroups, const float* up_base,
+                         const float* lat_base, const uint8_t* mask_base, int principal_point, double huber, int max_iterations, double* params,
+                         double* cost, int32_t* iterations, int32_t* status, void* workspace, int64_t workspace_bytes, void* stream) {
+  WsLayout lay;
+  long long blocks;
+  std::vector<int> csr;
+  TRY(fit_groups_layout(images, n, group_of, ngroups, &lay, &blocks, &csr));
+  std::vector<FitImage> d;
+  FitArgs a;
+  TRY(fit_prepare("pf_fit_camera_groups", lay, blocks, images, n, up_base, lat_base, mask_base, principal_point, huber, max_iterations, params,
+                  cost, iterations, status, workspace, workspace_bytes, &d, &a));
+  CU(cudaSetDevice(device));
+  cudaStream_t st = (cudaStream_t)stream;
+  char* ws = (char*)workspace;
+  FitGroups g{};
+  g.gs = (FitGroupState*)(ws + lay.at[3]);
+  g.sums = (double*)(ws + lay.at[4]);
+  g.off = (const int*)(ws + lay.at[5]);
+  g.mem = g.off + ngroups + 1;
+  g.ngroups = ngroups;
+  TRY(upload_descriptors(d.data(), d.size() * sizeof(d[0]), ws, st));
+  CU(cudaMemcpyAsync(ws + lay.at[5], csr.data(), csr.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  const PdlScope pdl(!sync_debug());
+  const dim3 pass_grid((unsigned)blocks), reduce_grid((unsigned)cdiv(n, kFitStepWarps)), group_grid((unsigned)ngroups);
+  LAUNCHED(launch_pdl(fit_init_kernel, dim3(n), dim3(64), 0, st, a, principal_point));
+  LAUNCHED(launch_pdl(fit_group_init_kernel, dim3((unsigned)cdiv(ngroups, 128)), dim3(128), 0, st, a, g));
+  for (int it = 0; it < max_iterations; ++it) {
+    if (principal_point) {
+      LAUNCHED(launch_pdl(fit_pass_kernel<5>, pass_grid, dim3(kFitThreads), 0, st, a));
+      LAUNCHED(launch_pdl(fit_reduce_kernel<5>, reduce_grid, dim3(32 * kFitStepWarps), 0, st, a, g));
+      LAUNCHED(launch_pdl(fit_group_step_kernel<5>, group_grid, dim3(kFitGroupThreads), 0, st, a, g));
+    } else {
+      LAUNCHED(launch_pdl(fit_pass_kernel<3>, pass_grid, dim3(kFitThreads), 0, st, a));
+      LAUNCHED(launch_pdl(fit_reduce_kernel<3>, reduce_grid, dim3(32 * kFitStepWarps), 0, st, a, g));
+      LAUNCHED(launch_pdl(fit_group_step_kernel<3>, group_grid, dim3(kFitGroupThreads), 0, st, a, g));
     }
   }
   return PF_OK;

@@ -4,6 +4,9 @@
 
 * ``fit_camera`` on 256 seeded noisy camera fields of 640 x 480 (2 degrees of angular noise on up, 1 degree on latitude, 1 %
   outliers): centred least squares, and uncentred Huber (delta 2 degrees);
+* ``fit_camera(groups=...)`` on the same batch with the intrinsics shared within each group (16 groups of 16, and one group of
+  256), against the per-image fit of that batch: ms per call, evaluations, pass / reduce / group-step kernel time, and the
+  focal-length error against the true cameras;
 * ``inference_batch`` of PersNet-360Cities on 32 images of 640 x 480, alone and followed by ``fit_camera``.
 
 Each pass reads 12 B per pixel (two float32 up components and one latitude), 0.94 GB for the batch; a device-to-device copy
@@ -24,14 +27,20 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 from metrics_bench import copy_ms, gpu_info, kernel_ms, timed  # noqa: E402
 
 
-def noisy_batch(n, h, w, seed=0):
+def noisy_batch(n, h, w, seed=0, group_size=1, focal_out=None):
+    """The seeded noisy batch; with group_size > 1 each run of group_size images shares the intrinsics (focal length and
+    principal point) of its first image.  focal_out, if given, receives the true f_rel of each image."""
     from perspectivefields_b200 import panocam
 
     g = torch.Generator().manual_seed(seed)
     u = lambda lo, hi: (torch.rand(n, generator=g, dtype=torch.float64) * (hi - lo) + lo).tolist()
     roll, pitch, vfov = u(-40, 40), u(-60, 60), u(35, 100)
     cx, cy = u(-0.1, 0.1), u(-0.1, 0.1)
+    shared = lambda v: [v[i - i % group_size] for i in range(n)]
+    vfov, cx, cy = shared(vfov), shared(cx), shared(cy)
     focal = [1 / (2 * math.tan(math.radians(v) / 2)) for v in vfov]
+    if focal_out is not None:
+        focal_out.extend(focal)
     ups, lats = panocam.camera_fields(focal, [h] * n, [w] * n, [math.radians(p) for p in pitch], [math.radians(r) for r in roll], cx, cy)
     gd = torch.Generator(device="cuda").manual_seed(seed)
     up = torch.stack(ups).permute(0, 3, 1, 2)                                  # [n, 2, H, W] view of the [n, H, W, 2] fields
@@ -75,6 +84,29 @@ def main():
             "pass_GB_per_s": nbytes / (pass_ms / batch_passes) / 1e6, "copy_ms_same_bytes_read": cms,
             "pass_time_over_copy_time": (pass_ms / batch_passes) / cms}
     del results
+    for gs in (16, 256):
+        focal = []
+        results = noisy_batch(n, h, w, group_size=gs, focal_out=focal)
+        f_true = torch.tensor(focal, dtype=torch.float64, device="cuda")
+        groups = [i // gs for i in range(n)]
+        for name, kw in (("centred_l2", {"principal_point": False}), ("uncentred_huber", {"principal_point": True, "huber": math.radians(2.0)})):
+            case = {}
+            for mode, extra in (("per_image", {}), ("grouped", {"groups": groups})):
+                fn = lambda: calibrate.fit_camera(results, **kw, **extra)
+                ms = timed(fn, args.iters)
+                out = fn()
+                its = torch.stack([o["fit_iterations"] for o in out]).float()
+                st = torch.stack([o["fit_status"] for o in out])
+                ferr = (torch.stack([o["pred_rel_focal"] for o in out]) - f_true).abs() / f_true
+                km = kernel_ms(fn, "fit_")
+                case[mode] = {
+                    "ms_per_call": ms, "launched_pass_pairs": int(its.max()), "mean_evaluations": float(its.mean()),
+                    "status_counts": torch.bincount(st, minlength=3).tolist(), "kernel_ms_per_call": km,
+                    "pass_ms": sum(v for k, v in km.items() if "pass" in k), "reduce_ms": sum(v for k, v in km.items() if "reduce" in k),
+                    "step_ms": sum(v for k, v in km.items() if "step" in k),
+                    "focal_rel_error_median": float(ferr.median()), "focal_rel_error_max": float(ferr.max())}
+            res["cases"][f"{name}_{n // gs}_groups_of_{gs}"] = case
+        del results
     m = U.make_model("PersNet-360Cities", seed=0, device="cuda")[0]
     imgs = [torch.from_numpy(x).cuda() for x in wg.smooth_images(32, h, w, seed=1)]
     inf_ms = timed(lambda: m.inference_batch(imgs), max(args.iters // 2, 3))
