@@ -95,6 +95,22 @@ int64_t pf_workspace_bytes(pf_handle h, int n, int max_h);
 /* Whole forward of perspectivefields.py:223-272 for one batch, enqueued on `stream` (a cudaStream_t). */
 int pf_forward(pf_handle h, const pf_batch* batch, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* Head confidence (DESIGN.md section 1): per pixel of each classification head, conf = max_c softmax(logits)_c in fp32 over all
+ * classes (73 gravity bins including the no-direction bin, 180 latitude bins), in [1/NC, 1].  Outputs, DEVICE, fp32, 4-byte
+ * aligned: gravity / latitude [n, net_h, net_w]; gravity_original / latitude_original the same maps resampled to each image's size
+ * (bilinear, align_corners=False, no antialias: the sampling of the latitude map), both laid out like pf_batch.latitude_original
+ * (image i's [H_i, W_i] block at latitude_original_offset[i]). */
+typedef struct pf_confidence {
+  float* gravity;
+  float* latitude;
+  float* gravity_original;
+  float* latitude_original;
+} pf_confidence;
+/* pf_forward plus the confidence maps, in either "decode_only" setting; every pf_forward output is bit-identical to pf_forward's.
+ * PF_ERR_ARG before anything is launched when either head is a regression head, conf or one of its pointers is NULL, or a
+ * pointer is not 4-byte aligned.  The workspace is pf_workspace_bytes' (the maps need no scratch). */
+int pf_forward_confidence(pf_handle h, const pf_batch* batch, const pf_confidence* conf, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ---- ParamNet on the caller's fields (param_network.py:46-69 ParamNet.forward, :193-221 ParamNetConvNextRegress.forward) -----
  * The ParamNet section of pf_forward (same kernels, same order, same results on the same fields) run on any fields at the
  * engine's working size net_h x net_w: gravity DEVICE float32 [n,2,net_h,net_w] up vectors, latitude [n,1,net_h,net_w]
@@ -334,6 +350,22 @@ int64_t pf_fit_camera_groups_workspace(const pf_fit_image* images, int n, const 
 int pf_fit_camera_groups(int device, const pf_fit_image* images, int n, const int32_t* group_of, int ngroups, const float* up_base,
                          const float* lat_base, const uint8_t* mask_base, int principal_point, double huber, int max_iterations, double* params,
                          double* cost, int32_t* iterations, int32_t* status, void* workspace, int64_t workspace_bytes, void* stream);
+/* The two fits with a weight per residual (DESIGN.md section 1, "Camera fit"): weight_base DEVICE float32 (NULL when every offset
+ * is -1); up_weight_offset / lat_weight_offset HOST int64 [n] (NULL: all -1), the float offset of image i's [H, W] row-major weight
+ * map of its up / latitude residuals, -1 for none.  A residual counts where it is valid and its weight w is finite and > 0 (any
+ * other weight drops it as the mask does); it adds w delta^2 rho((r / delta)^2) to 2 C and has the IRLS weight w rho'.  The
+ * closed-form start uses only pixels with w > 0.  All-ones weights give the unweighted results and 0 / 1 weights the results of
+ * the matching mask, bit for bit.  pf_fit_camera(..) = pf_fit_camera_weighted(.., NULL, NULL, NULL, ..), and
+ * likewise for the groups; the workspace sizes are the
+ * same pf_fit_camera_workspace / pf_fit_camera_groups_workspace queries. */
+int pf_fit_camera_weighted(int device, const pf_fit_image* images, int n, const float* up_base, const float* lat_base, const uint8_t* mask_base,
+                           const float* weight_base, const int64_t* up_weight_offset, const int64_t* lat_weight_offset, int principal_point,
+                           double huber, int max_iterations, double* params, double* cost, int32_t* iterations, int32_t* status, void* workspace,
+                           int64_t workspace_bytes, void* stream);
+int pf_fit_camera_groups_weighted(int device, const pf_fit_image* images, int n, const int32_t* group_of, int ngroups, const float* up_base,
+                                  const float* lat_base, const uint8_t* mask_base, const float* weight_base, const int64_t* up_weight_offset,
+                                  const int64_t* lat_weight_offset, int principal_point, double huber, int max_iterations, double* params,
+                                  double* cost, int32_t* iterations, int32_t* status, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---- upright warp: straightened images from camera parameters (csrc/rectify.cuh) --------------------------------------------
  * Warps each uint8 image (1 or 3 channels, HWC) to a camera with roll 0, pitch 0 (or the input pitch with keep_pitch), a centred

@@ -114,6 +114,48 @@ def prediction_fields(results, mask, min_size):
     return pu, pl, ms, dev
 
 
+CONFIDENCE_KEYS = ("pred_gravity_confidence_original", "pred_latitude_confidence_original")
+
+
+def fit_weights(weights, results, pu, dev):
+    """``fit_camera``'s ``weights`` for the fields ``prediction_fields`` returned (``pu``: the [H, W, 2] up views): None, "confidence"
+    (the two ``CONFIDENCE_KEYS`` maps of each result) or a list of n entries, each None or a pair (up weight, latitude weight) of
+    float32 [H, W] tensors on ``dev``, either of them None -> per image (up weight, latitude weight), contiguous or None.
+    ValueError for anything else, before any GPU work of the library."""
+    n = len(results)
+    if weights is None:
+        return [(None, None)] * n
+    if isinstance(weights, str):
+        if weights != "confidence":
+            raise ValueError(f"weights must be None, 'confidence' or a list of (up, latitude) weight pairs, got {weights!r}")
+        for i, r in enumerate(results):
+            for k in CONFIDENCE_KEYS:
+                if k not in r:
+                    raise ValueError(f"weights='confidence': results[{i}] has no {k!r} (run a model built with confidence=True)")
+        entries = [(r[CONFIDENCE_KEYS[0]], r[CONFIDENCE_KEYS[1]]) for r in results]
+        what = ["results[{i}]['" + k + "']" for k in CONFIDENCE_KEYS]
+    else:
+        if isinstance(weights, torch.Tensor) or not isinstance(weights, (list, tuple)):
+            raise ValueError(f"weights must be None, 'confidence' or a list of {n} entries, got {type(weights).__name__}")
+        entries = list(weights)
+        if len(entries) != n:
+            raise ValueError(f"{n} results but {len(entries)} weight entries")
+        what = ["weights[{i}][0]", "weights[{i}][1]"]
+    out = []
+    for i, e in enumerate(entries):
+        if e is None:
+            out.append((None, None))
+            continue
+        if not isinstance(e, (tuple, list)) or len(e) != 2:
+            raise ValueError(f"weights[{i}] must be None or a pair (up weight, latitude weight), got {type(e).__name__}")
+        h, w = int(pu[i].shape[0]), int(pu[i].shape[1])
+        for j, t in enumerate(e):
+            if t is not None and (not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or tuple(t.shape) != (h, w) or t.device != dev):
+                raise ValueError(f"{what[j].format(i=i)} must be None or a float32 [{h}, {w}] tensor on {dev}")
+        out.append(e)
+    return [tuple(None if t is None else t.contiguous() for t in e) for e in out]
+
+
 def _number(x, kinds):
     return isinstance(x, kinds) and not isinstance(x, (bool, np.bool_))
 

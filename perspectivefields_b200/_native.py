@@ -93,6 +93,12 @@ class pf_batch(ctypes.Structure):
                 ("params", ctypes.c_void_p)]
 
 
+class pf_confidence(ctypes.Structure):
+    """include/pf_b200.h: struct pf_confidence (the head-confidence outputs of pf_forward_confidence)."""
+    _fields_ = [("gravity", ctypes.c_void_p), ("latitude", ctypes.c_void_p), ("gravity_original", ctypes.c_void_p),
+                ("latitude_original", ctypes.c_void_p)]
+
+
 class pf_tma_pred(ctypes.Structure):
     """include/pf_b200.h: struct pf_tma_pred (fused prediction tail of one group)."""
     _fields_ = [("w", ctypes.c_void_p), ("b", ctypes.c_void_p), ("out", ctypes.c_void_p), ("nc", ctypes.c_int), ("mode", ctypes.c_int)]
@@ -186,6 +192,7 @@ def lib():
         "pf_finalize": (i32, [vp]),
         "pf_workspace_bytes": (i64, [vp, i32, i32]),
         "pf_forward": (i32, [vp, ctypes.POINTER(pf_batch), vp, i64, vp]),
+        "pf_forward_confidence": (i32, [vp, ctypes.POINTER(pf_batch), ctypes.POINTER(pf_confidence), vp, i64, vp]),
         "pf_param_workspace_bytes": (i64, [vp, i32]),
         "pf_param_forward": (i32, [vp, i32, vp, vp, vp, vp, vp, i64, vp]),
         "pf_param_train_workspace_bytes": (i64, [vp, i32]),
@@ -224,6 +231,10 @@ def lib():
         "pf_fit_camera_groups_workspace": (i64, [ctypes.POINTER(pf_fit_image), i32, ctypes.POINTER(ctypes.c_int32), i32]),
         "pf_fit_camera_groups": (i32, [i32, ctypes.POINTER(pf_fit_image), i32, ctypes.POINTER(ctypes.c_int32), i32, vp, vp, vp, i32, ctypes.c_double,
                                        i32, vp, vp, vp, vp, vp, i64, vp]),
+        "pf_fit_camera_weighted": (i32, [i32, ctypes.POINTER(pf_fit_image), i32, vp, vp, vp, vp, ctypes.POINTER(i64), ctypes.POINTER(i64), i32,
+                                         ctypes.c_double, i32, vp, vp, vp, vp, vp, i64, vp]),
+        "pf_fit_camera_groups_weighted": (i32, [i32, ctypes.POINTER(pf_fit_image), i32, ctypes.POINTER(ctypes.c_int32), i32, vp, vp, vp, vp,
+                                                ctypes.POINTER(i64), ctypes.POINTER(i64), i32, ctypes.c_double, i32, vp, vp, vp, vp, vp, i64, vp]),
         "pf_rectify_workspace": (i64, [ctypes.POINTER(pf_rectify_image), i32]),
         "pf_rectify_views": (i32, [i32, ctypes.POINTER(pf_rectify_image), i32, vp, vp, vp, vp, i32, vp, i32, i32, ctypes.c_double, i32,
                                    ctypes.POINTER(ctypes.c_int32), vp, vp, vp, i64, vp]),
@@ -289,12 +300,13 @@ def lib():
 
 
 EXPORTS = ["pf_abi_version", "pf_last_error", "pf_kernel_launch_count", "pf_create", "pf_create_sized", "pf_destroy", "pf_set_weight",
-           "pf_finalize", "pf_workspace_bytes", "pf_forward", "pf_param_workspace_bytes", "pf_param_forward", "pf_param_train_workspace_bytes",
+           "pf_finalize", "pf_workspace_bytes", "pf_forward", "pf_forward_confidence", "pf_param_workspace_bytes", "pf_param_forward", "pf_param_train_workspace_bytes",
            "pf_param_train_forward", "pf_param_backward", "pf_param_grad_numel", "pf_param_grad_entry", "pf_profile_enable", "pf_profile_read", "pf_profile_kernels_enable",
            "pf_profile_kernels_read", "pf_set_option", "pf_debug_enable", "pf_debug_count", "pf_debug_name", "pf_debug_numel",
            "pf_debug_copy", "pf_camera_fields", "pf_camera_fields_vp", "pf_pano_views", "pf_equi_views", "pf_draw_fields",
            "pf_encode_fields", "pf_head_losses_workspace", "pf_head_losses", "pf_field_errors_workspace", "pf_field_errors",
            "pf_fit_camera_workspace", "pf_fit_camera", "pf_fit_camera_groups_workspace", "pf_fit_camera_groups",
+           "pf_fit_camera_weighted", "pf_fit_camera_groups_weighted",
            "pf_rectify_workspace", "pf_rectify_views", "pf_comm_unique_id", "pf_comm_create", "pf_comm_destroy", "pf_gather",
            "pf_jpeg_create", "pf_jpeg_destroy", "pf_jpeg_info", "pf_jpeg_decode_batch",
            "pf_op_conv_gemm", "pf_op_tma", "pf_op_tma_bf16", "pf_op_conv1_ring", "pf_tma_pick_tile", "pf_op_layernorm",

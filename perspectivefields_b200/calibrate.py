@@ -56,7 +56,7 @@ def _group_ids(groups, n):
     return (ctypes.c_int32 * n)(*(ids[int(v)] for v in labels)), len(ids)
 
 
-def fit_camera(results, principal_point=False, init="fields", mask=None, huber=None, max_iterations=50, groups=None):
+def fit_camera(results, principal_point=False, init="fields", mask=None, huber=None, max_iterations=50, groups=None, weights=None):
     """Fit one camera per image to ``results[i]["pred_gravity_original"]`` ([2, H, W] up vectors) and
     ``["pred_latitude_original"]`` ([H, W], degrees), read in place; sizes may differ within one call.  A dict of ground-truth
     fields works too, e.g. ``{"pred_gravity_original": up.permute(2, 0, 1), "pred_latitude_original": lat}``.
@@ -74,6 +74,13 @@ def fit_camera(results, principal_point=False, init="fields", mask=None, huber=N
       ``fit_cost`` is each image's own cost at the group's final point, and ``fit_iterations`` and ``fit_status`` are the
       group's, except that an image with too few valid residuals is dropped from its group with status 2.  The start of the
       shared values is the mean of the members' starts.
+    - ``weights``: None, "confidence" (each result's ``pred_gravity_confidence_original`` / ``pred_latitude_confidence_original``,
+      what a model built with ``confidence=True`` returns) or a list of n entries, each None or a pair ``(w_up, w_lat)`` of float32
+      [H, W] tensors on the results' device (either may be None): per-pixel weights of the up and latitude residuals.  A residual
+      counts only where its weight is finite and > 0 (others are dropped as ``mask`` drops them); it adds ``w`` times its
+      cost term and has ``w`` times its IRLS weight, and the closed-form start uses only pixels with a usable weight (DESIGN.md
+      section 1, "Camera fit").  All-ones weights give the unweighted fit and 0 / 1 weights the fit
+      under the matching ``mask``, bit for bit.  Checked on the host, no synchronisation.
 
     Returns one dict per image, as 0-dim float64 CUDA tensors in degrees: the keys of a centred (``principal_point=False``:
     ``pred_roll, pred_pitch, pred_vfov, pred_rel_focal, pred_general_vfov, pred_rel_cx, pred_rel_cy``) or uncentred ParamNet
@@ -97,9 +104,14 @@ def fit_camera(results, principal_point=False, init="fields", mask=None, huber=N
     if n == 0:
         return []
     pu, pl, ms, dev = _batch.prediction_fields(results, mask, 3)
+    wts = _batch.fit_weights(weights, results, pu, dev)
     starts = _init_from_results(results) if init == "results" else [_NAN_INIT] * n
     L = _native.lib()
     bu, bl, bm = _batch.base(pu), _batch.base(pl), _batch.base(ms)
+    flat = [t for e in wts for t in e]
+    bw = _batch.base(flat)
+    uw = (ctypes.c_int64 * n)(*(_batch.offset(e[0], bw) for e in wts))
+    lw = (ctypes.c_int64 * n)(*(_batch.offset(e[1], bw) for e in wts))
     descs = (_native.pf_fit_image * n)()
     for i in range(n):
         d = descs[i]
@@ -118,12 +130,12 @@ def fit_camera(results, principal_point=False, init="fields", mask=None, huber=N
         its = torch.empty(n, dtype=torch.int32, device=dev)
         status = torch.empty(n, dtype=torch.int32, device=dev)
         stream = torch.cuda.current_stream(dev).cuda_stream
-        fields = (bu, bl, bm or None, int(principal_point), float(huber or 0.0), max_iterations, params.data_ptr(), cost.data_ptr(),
-                  its.data_ptr(), status.data_ptr(), ws.data_ptr(), ws.numel(), stream)
+        fields = (bu, bl, bm or None, bw or None, uw, lw, int(principal_point), float(huber or 0.0), max_iterations, params.data_ptr(),
+                  cost.data_ptr(), its.data_ptr(), status.data_ptr(), ws.data_ptr(), ws.numel(), stream)
         if group_of is None:
-            _native.check(L.pf_fit_camera(dev.index, descs, n, *fields))
+            _native.check(L.pf_fit_camera_weighted(dev.index, descs, n, *fields))
         else:
-            _native.check(L.pf_fit_camera_groups(dev.index, descs, n, group_of[0], group_of[1], *fields))
+            _native.check(L.pf_fit_camera_groups_weighted(dev.index, descs, n, group_of[0], group_of[1], *fields))
         roll, pitch, f, cx, cy = params.t()
         gv = general_vfov(cx, cy, 1, f, True)
         if principal_point:

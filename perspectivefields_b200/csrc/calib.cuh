@@ -9,7 +9,9 @@
 //                       roll, then pitch.
 // Residuals: r_u = atan2(u x p, u . p) where the prediction p is finite with |p| > 1e-5; r_l = rad(l_pred) - l where l_pred
 // is finite; both under the optional mask.  Cost C = 1/2 sum delta^2 rho((r / delta)^2) (scipy's least_squares with
-// f_scale = delta: rho(z) = z, or Huber's 2 sqrt(z) - 1 above 1), IRLS weights w = rho'.
+// f_scale = delta: rho(z) = z, or Huber's 2 sqrt(z) - 1 above 1), IRLS weights w = rho'.  With per-residual weights v (maps of
+// the up and latitude residuals, pf_fit_camera_weighted) a residual also needs a finite v > 0; it adds v delta^2 rho to 2 C and
+// has the IRLS weight v rho' (the Huber threshold applies to the unweighted r).
 //
 // Three kernels, chained with programmatic dependent launch and enqueued without synchronisation: fit_init_kernel (the
 // start), then max_iterations pairs of fit_pass_kernel (one cost evaluation: C, A = sum w J^T J and g = sum w J^T r at the
@@ -43,6 +45,7 @@ struct FitImage {
   long long mask_off;                      // bytes, -1: none
   int block0, nblk;                        // its blocks in the pass
   double init[5];                          // roll, pitch (radians), f_rel, cx_rel, cy_rel; NaN roll: the closed-form start
+  long long uw_off, lw_off;                // weights of the up / latitude residuals, [H, W] row-major floats; -1: none
 };
 struct FitState {
   double theta[5], cand[5];   // accepted parameters, the candidate the next pass evaluates
@@ -53,6 +56,7 @@ struct FitState {
 struct FitArgs {
   const FitImage* im; FitState* st; int n, nblocks;
   const float* up; const float* lat; const unsigned char* mask;
+  const float* wt;            // base of the weight maps (FitImage::uw_off / lw_off)
   double huber;               // 0: least squares
   int max_iter;
   double* part;               // [kFitQ][nblocks]
@@ -73,13 +77,24 @@ __device__ __forceinline__ bool up_usable(double px, double py) {
   return isfinite(px) && isfinite(py) && sqrt(px * px + py * py) > kFitUpMin;
 }
 
+// A residual weight that keeps its residual: finite and > 0 (NaN, infinities, zero and negative weights drop it)
+__device__ __forceinline__ bool weight_usable(float w) { return w > 0.0f && w < INFINITY; }
+
+// Weight of pixel q of a [H, W] weight map at off (-1: none, weight 1); 0 when unusable (the residual is dropped)
+__device__ __forceinline__ double fit_weight(const FitArgs& a, long long off, long long q) {
+  if (off < 0) return 1.0;
+  const float t = a.wt[off + q];
+  return weight_usable(t) ? (double)t : 0.0;
+}
+
 // ------------------------------------------------------------------------------------------------------------ start
 // One block of 64 threads per image, one thread per pixel of the 8 x 8 window of rows H/2 - 4 .. H/2 + 3 and the same columns
 // around W/2 (clipped to the image):
 //   roll0 = atan2(-sum px^, -sum py^) of the unit predictions (at the principal point up = (-sin r, -cos r));
 //   pitch0 = the window's mean latitude (latitude = pitch at the principal point);
 //   f0 = 1 / (H mean |grad l|), central differences where the four neighbours are valid (|grad l| = 1 / F there).
-// A term without a valid pixel falls back to roll 0, pitch 0, vfov 60 degrees.
+// A term without a valid pixel falls back to roll 0, pitch 0, vfov 60 degrees.  With weights, a pixel counts for the roll term only
+// where its up weight is usable, for the pitch and gradient terms (the four neighbours included) only where its latitude weight is.
 __global__ void __launch_bounds__(64) fit_init_kernel(FitArgs a, int principal_point) {
   __shared__ double shd[33];
   __shared__ int shi[33];
@@ -97,18 +112,19 @@ __global__ void __launch_bounds__(64) fit_init_kernel(FitArgs a, int principal_p
     int nu = 0, nl = 0, ng = 0;
     if (y >= 0 && y < d.H && x >= 0 && x < d.W) {
       auto ok = [&](int yy, int xx) { return d.mask_off < 0 || a.mask[d.mask_off + (long long)yy * d.W + xx] != 0; };
+      auto okl = [&](int yy, int xx) { return ok(yy, xx) && (d.lw_off < 0 || weight_usable(a.wt[d.lw_off + (long long)yy * d.W + xx])); };
       auto lat = [&](int yy, int xx) { return (double)a.lat[d.lat_off + (long long)yy * d.W + xx] * (kPi / 180.0); };
       if (ok(y, x)) {
         const float* p = a.up + d.up_off + y * d.up_sr + x * d.up_sc;
         const double px = p[0], py = p[d.up_sk];
-        if (up_usable(px, py)) {
+        if (up_usable(px, py) && (d.uw_off < 0 || weight_usable(a.wt[d.uw_off + (long long)y * d.W + x]))) {
           const double nn = sqrt(px * px + py * py);
           sx = px / nn; sy = py / nn; nu = 1;
         }
         const double l0 = lat(y, x);
-        if (isfinite(l0)) {
+        if (isfinite(l0) && okl(y, x)) {
           sl = l0; nl = 1;
-          if (y > 0 && y < d.H - 1 && x > 0 && x < d.W - 1 && ok(y, x + 1) && ok(y, x - 1) && ok(y + 1, x) && ok(y - 1, x)) {
+          if (y > 0 && y < d.H - 1 && x > 0 && x < d.W - 1 && okl(y, x + 1) && okl(y, x - 1) && okl(y + 1, x) && okl(y - 1, x)) {
             const double r = lat(y, x + 1), l = lat(y, x - 1), b = lat(y + 1, x), t = lat(y - 1, x);
             if (isfinite(r) && isfinite(l) && isfinite(b) && isfinite(t)) {
               const double gx = 0.5 * (r - l), gy = 0.5 * (b - t);
@@ -133,11 +149,14 @@ __global__ void __launch_bounds__(64) fit_init_kernel(FitArgs a, int principal_p
 }
 
 // ------------------------------------------------------------------------------------------------------------ pass
-template <int P>
-__device__ __forceinline__ void fit_accumulate(double (&acc)[fit_nq(P)], double r, const double (&J)[P], double huber) {
+// kW: the residual has weight v (> 0, finite): v c and v w in place of c and w.  Both products are exact for v = 1, and so is
+// the fused v c + acc[0] the compiler makes of the first: unit weights add the unweighted terms bit for bit.
+template <int P, bool kW = false>
+__device__ __forceinline__ void fit_accumulate(double (&acc)[fit_nq(P)], double r, const double (&J)[P], double huber, double v = 1.0) {
   const double ar = fabs(r);
   double c = r * r, w = 1.0;
   if (huber > 0.0 && ar > huber) { c = 2.0 * huber * ar - huber * huber; w = huber / ar; }
+  if constexpr (kW) { c = v * c; w = v * w; }
   acc[0] += c;
   acc[1] += 1.0;
 #pragma unroll
@@ -152,8 +171,8 @@ __device__ __forceinline__ void fit_accumulate(double (&acc)[fit_nq(P)], double 
 }
 
 // Blocks of kFitTile pixels, each within one image.  Writes plane q of the partials: 0 = sum delta^2 rho (2 C), 1 = residual
-// count, 2 .. 1 + P = g, then A's upper triangle row by row.
-template <int P>
+// count, 2 .. 1 + P = g, then A's upper triangle row by row.  kW: the launch has weight maps (an image without one has v = 1).
+template <int P, bool kW = false>
 __global__ void __launch_bounds__(kFitThreads) fit_pass_kernel(FitArgs a) {
   constexpr int NQ = fit_nq(P);
   __shared__ double shq[kFitThreads / 32][NQ];
@@ -185,6 +204,9 @@ __global__ void __launch_bounds__(kFitThreads) fit_pass_kernel(FitArgs a) {
     if (q >= HW) break;
     if (d.mask_off >= 0 && a.mask[d.mask_off + q] == 0) continue;
     const int y = (int)(q / d.W), x = (int)(q - (long long)y * d.W);
+    // (the weighted instantiation computes each residual and its Jacobian row in the same blocks as the unweighted one and only
+    // then reads the weight, so that the compiler makes the same instructions of them: unit weights and 0 / 1 weight maps give
+    // the unweighted and the masked sums bit for bit)
     {
       const float* p = a.up + d.up_off + y * d.up_sr + x * d.up_sc;
       const double px = p[0], py = p[d.up_sk];
@@ -203,7 +225,12 @@ __global__ void __launch_bounds__(kFitThreads) fit_pass_kernel(FitArgs a) {
           const double iu2 = 1.0 / u2;
 #pragma unroll
           for (int k = 0; k < P; ++k) J[k] = -(ux * duy[k] - uy * dux[k]) * iu2;
-          fit_accumulate<P>(acc, r, J, a.huber);
+          if constexpr (kW) {
+            const double v = fit_weight(a, d.uw_off, q);
+            if (v > 0.0) fit_accumulate<P, true>(acc, r, J, a.huber, v);
+          } else {
+            fit_accumulate<P>(acc, r, J, a.huber);
+          }
         }
       }
     }
@@ -227,7 +254,12 @@ __global__ void __launch_bounds__(kFitThreads) fit_pass_kernel(FitArgs a) {
           J[3] = (-(Wd * rF) * (ce * sr) + c * xx * (Wd * rF)) * ih;
           J[4] = (-(Hd * rF) * (ce * cr) + c * yy * (Hd * rF)) * ih;
         }
-        fit_accumulate<P>(acc, r, J, a.huber);
+        if constexpr (kW) {
+          const double v = fit_weight(a, d.lw_off, q);
+          if (v > 0.0) fit_accumulate<P, true>(acc, r, J, a.huber, v);
+        } else {
+          fit_accumulate<P>(acc, r, J, a.huber);
+        }
       }
     }
   }

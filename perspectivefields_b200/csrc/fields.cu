@@ -455,10 +455,12 @@ struct PdlScope {
 };
 
 // The argument checks both fits share and the kernels' arguments; uploads the descriptors into the workspace
+// (weighted: whether any image has a weight map, which selects the pass kernel's weighted instantiation)
 static int fit_prepare(const char* fn, const WsLayout& lay, long long blocks, const pf_fit_image* images, int n, const float* up_base,
-                       const float* lat_base, const uint8_t* mask_base, int principal_point, double huber, int max_iterations, double* params,
+                       const float* lat_base, const uint8_t* mask_base, const float* weight_base, const int64_t* up_weight_offset,
+                       const int64_t* lat_weight_offset, int principal_point, double huber, int max_iterations, double* params,
                        double* cost, int32_t* iterations, int32_t* status, void* workspace, int64_t workspace_bytes, std::vector<FitImage>* d,
-                       FitArgs* a) {
+                       FitArgs* a, bool* weighted) {
   if (!up_base || !lat_base || !params || !cost || !iterations || !status || !workspace)
     return fail(PF_ERR_ARG, "%s: null field / output / workspace", fn);
   if (principal_point != 0 && principal_point != 1) return fail(PF_ERR_ARG, "%s: principal_point must be 0 or 1", fn);
@@ -469,9 +471,12 @@ static int fit_prepare(const char* fn, const WsLayout& lay, long long blocks, co
   TRY(check_workspace(fn, workspace, workspace_bytes, lay.total));
   d->resize(n);
   long long block0 = 0;
+  *weighted = false;
   for (int i = 0; i < n; ++i) {
     const pf_fit_image& c = images[i];
-    TRY(check_offsets(fn, i, {c.up_offset, c.lat_offset}, {{c.mask_offset, mask_base}}));
+    const long long uw = up_weight_offset ? up_weight_offset[i] : -1, lw = lat_weight_offset ? lat_weight_offset[i] : -1;
+    TRY(check_offsets(fn, i, {c.up_offset, c.lat_offset}, {{c.mask_offset, mask_base}, {uw, weight_base}, {lw, weight_base}}));
+    *weighted = *weighted || uw >= 0 || lw >= 0;
     if (c.up_stride[0] < 0 || c.up_stride[1] < 0 || c.up_stride[2] < 0) return fail(PF_ERR_ARG, "%s: image %d has a negative stride", fn, i);
     if (!std::isnan(c.init[0])) {
       bool fin = true;
@@ -483,6 +488,7 @@ static int fit_prepare(const char* fn, const WsLayout& lay, long long blocks, co
     o.up_off = c.up_offset; o.up_sr = c.up_stride[0]; o.up_sc = c.up_stride[1]; o.up_sk = c.up_stride[2];
     o.lat_off = c.lat_offset;
     o.mask_off = c.mask_offset;
+    o.uw_off = uw; o.lw_off = lw;
     for (int k = 0; k < 5; ++k) o.init[k] = c.init[k];
     o.block0 = (int)block0; o.nblk = (int)cdivl((long long)c.height * c.width, kFitTile);
     block0 += o.nblk;
@@ -490,23 +496,38 @@ static int fit_prepare(const char* fn, const WsLayout& lay, long long blocks, co
   char* ws = (char*)workspace;
   *a = FitArgs{};
   a->im = (const FitImage*)ws; a->st = (FitState*)(ws + lay.at[1]); a->n = n; a->nblocks = (int)blocks;
-  a->up = up_base; a->lat = lat_base; a->mask = mask_base;
+  a->up = up_base; a->lat = lat_base; a->mask = mask_base; a->wt = weight_base;
   a->huber = huber; a->max_iter = max_iterations;
   a->part = (double*)(ws + lay.at[2]);
   a->params = params; a->cost = cost; a->iters = iterations; a->status = status;
   return PF_OK;
 }
 
+// One cost evaluation: the pass kernel's instantiation for 5 (principal_point) or 3 parameters, weighted or not
+static cudaError_t fit_pass_launch(int principal_point, bool weighted, dim3 grid, cudaStream_t st, const FitArgs& a) {
+  auto k = principal_point ? (weighted ? fit_pass_kernel<5, true> : fit_pass_kernel<5, false>) : (weighted ? fit_pass_kernel<3, true> : fit_pass_kernel<3, false>);
+  return launch_pdl(k, grid, dim3(kFitThreads), 0, st, a);
+}
+
 int pf_fit_camera(int device, const pf_fit_image* images, int n, const float* up_base, const float* lat_base, const uint8_t* mask_base,
                   int principal_point, double huber, int max_iterations, double* params, double* cost, int32_t* iterations,
                   int32_t* status, void* workspace, int64_t workspace_bytes, void* stream) {
+  return pf_fit_camera_weighted(device, images, n, up_base, lat_base, mask_base, nullptr, nullptr, nullptr, principal_point, huber, max_iterations,
+                                params, cost, iterations, status, workspace, workspace_bytes, stream);
+}
+
+int pf_fit_camera_weighted(int device, const pf_fit_image* images, int n, const float* up_base, const float* lat_base, const uint8_t* mask_base,
+                           const float* weight_base, const int64_t* up_weight_offset, const int64_t* lat_weight_offset, int principal_point,
+                           double huber, int max_iterations, double* params, double* cost, int32_t* iterations, int32_t* status, void* workspace,
+                           int64_t workspace_bytes, void* stream) {
   WsLayout lay;
   long long blocks;
   TRY(fit_layout("pf_fit_camera", images, n, &lay, &blocks));
   std::vector<FitImage> d;
   FitArgs a;
-  TRY(fit_prepare("pf_fit_camera", lay, blocks, images, n, up_base, lat_base, mask_base, principal_point, huber, max_iterations, params, cost,
-                  iterations, status, workspace, workspace_bytes, &d, &a));
+  bool weighted;
+  TRY(fit_prepare("pf_fit_camera", lay, blocks, images, n, up_base, lat_base, mask_base, weight_base, up_weight_offset, lat_weight_offset,
+                  principal_point, huber, max_iterations, params, cost, iterations, status, workspace, workspace_bytes, &d, &a, &weighted));
   CU(cudaSetDevice(device));
   cudaStream_t st = (cudaStream_t)stream;
   TRY(upload_descriptors(d.data(), d.size() * sizeof(d[0]), workspace, st));
@@ -515,10 +536,10 @@ int pf_fit_camera(int device, const pf_fit_image* images, int n, const float* up
   LAUNCHED(launch_pdl(fit_init_kernel, dim3(n), dim3(64), 0, st, a, principal_point));
   for (int it = 0; it < max_iterations; ++it) {
     if (principal_point) {
-      LAUNCHED(launch_pdl(fit_pass_kernel<5>, pass_grid, dim3(kFitThreads), 0, st, a));
+      LAUNCHED(fit_pass_launch(1, weighted, pass_grid, st, a));
       LAUNCHED(launch_pdl(fit_step_kernel<5>, step_grid, dim3(32 * kFitStepWarps), 0, st, a));
     } else {
-      LAUNCHED(launch_pdl(fit_pass_kernel<3>, pass_grid, dim3(kFitThreads), 0, st, a));
+      LAUNCHED(fit_pass_launch(0, weighted, pass_grid, st, a));
       LAUNCHED(launch_pdl(fit_step_kernel<3>, step_grid, dim3(32 * kFitStepWarps), 0, st, a));
     }
   }
@@ -528,14 +549,23 @@ int pf_fit_camera(int device, const pf_fit_image* images, int n, const float* up
 int pf_fit_camera_groups(int device, const pf_fit_image* images, int n, const int32_t* group_of, int ngroups, const float* up_base,
                          const float* lat_base, const uint8_t* mask_base, int principal_point, double huber, int max_iterations, double* params,
                          double* cost, int32_t* iterations, int32_t* status, void* workspace, int64_t workspace_bytes, void* stream) {
+  return pf_fit_camera_groups_weighted(device, images, n, group_of, ngroups, up_base, lat_base, mask_base, nullptr, nullptr, nullptr, principal_point,
+                                       huber, max_iterations, params, cost, iterations, status, workspace, workspace_bytes, stream);
+}
+
+int pf_fit_camera_groups_weighted(int device, const pf_fit_image* images, int n, const int32_t* group_of, int ngroups, const float* up_base,
+                                  const float* lat_base, const uint8_t* mask_base, const float* weight_base, const int64_t* up_weight_offset,
+                                  const int64_t* lat_weight_offset, int principal_point, double huber, int max_iterations, double* params,
+                                  double* cost, int32_t* iterations, int32_t* status, void* workspace, int64_t workspace_bytes, void* stream) {
   WsLayout lay;
   long long blocks;
   std::vector<int> csr;
   TRY(fit_groups_layout(images, n, group_of, ngroups, &lay, &blocks, &csr));
   std::vector<FitImage> d;
   FitArgs a;
-  TRY(fit_prepare("pf_fit_camera_groups", lay, blocks, images, n, up_base, lat_base, mask_base, principal_point, huber, max_iterations, params,
-                  cost, iterations, status, workspace, workspace_bytes, &d, &a));
+  bool weighted;
+  TRY(fit_prepare("pf_fit_camera_groups", lay, blocks, images, n, up_base, lat_base, mask_base, weight_base, up_weight_offset, lat_weight_offset,
+                  principal_point, huber, max_iterations, params, cost, iterations, status, workspace, workspace_bytes, &d, &a, &weighted));
   CU(cudaSetDevice(device));
   cudaStream_t st = (cudaStream_t)stream;
   char* ws = (char*)workspace;
@@ -553,11 +583,11 @@ int pf_fit_camera_groups(int device, const pf_fit_image* images, int n, const in
   LAUNCHED(launch_pdl(fit_group_init_kernel, dim3((unsigned)cdiv(ngroups, 128)), dim3(128), 0, st, a, g));
   for (int it = 0; it < max_iterations; ++it) {
     if (principal_point) {
-      LAUNCHED(launch_pdl(fit_pass_kernel<5>, pass_grid, dim3(kFitThreads), 0, st, a));
+      LAUNCHED(fit_pass_launch(1, weighted, pass_grid, st, a));
       LAUNCHED(launch_pdl(fit_reduce_kernel<5>, reduce_grid, dim3(32 * kFitStepWarps), 0, st, a, g));
       LAUNCHED(launch_pdl(fit_group_step_kernel<5>, group_grid, dim3(kFitGroupThreads), 0, st, a, g));
     } else {
-      LAUNCHED(launch_pdl(fit_pass_kernel<3>, pass_grid, dim3(kFitThreads), 0, st, a));
+      LAUNCHED(fit_pass_launch(0, weighted, pass_grid, st, a));
       LAUNCHED(launch_pdl(fit_reduce_kernel<3>, reduce_grid, dim3(32 * kFitStepWarps), 0, st, a, g));
       LAUNCHED(launch_pdl(fit_group_step_kernel<3>, group_grid, dim3(kFitGroupThreads), 0, st, a, g));
     }

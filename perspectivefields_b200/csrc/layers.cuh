@@ -708,6 +708,30 @@ __global__ void __launch_bounds__(256) argmax_decode_kernel(const float* __restr
   decode_bin_store(field, b, r, HW, NC, bi, is_gravity);
 }
 
+// Head confidence (DESIGN.md section 1): conf = max_c softmax(l)_c = 1 / sum_c exp(l_c - l_max) in fp32 over all NC classes.
+// Online form: a running maximum m and the sum s of exp(l_c - m), rescaled by exp(m_old - m) when the maximum grows.
+__device__ __forceinline__ void conf_update(float v, float& m, float& s) {
+  if (v > m) { s = s * expf(m - v) + 1.0f; m = v; }
+  else s += expf(v - m);
+}
+// argmax_decode_kernel plus the confidence, in one pass over the logits (the logits are read once).  conf: [B, HW].
+__global__ void __launch_bounds__(256) argmax_conf_decode_kernel(const float* __restrict__ logits, float* __restrict__ field, float* __restrict__ conf,
+                                                                 int B, int HW, int NC, int is_gravity) {
+  const long long pix = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (pix >= (long long)B * HW) return;
+  const int b = (int)(pix / HW), r = (int)(pix % HW);
+  const float* lp = logits + (long long)b * NC * HW + r;
+  float best = lp[0], s = 1.0f;
+  int bi = 0;
+  for (int c = 1; c < NC; ++c) {
+    const float v = __ldg(lp + (long long)c * HW);
+    if (v > best) { s = s * expf(best - v) + 1.0f; best = v; bi = c; }
+    else s += expf(v - best);
+  }
+  conf[pix] = 1.0f / s;
+  decode_bin_store(field, b, r, HW, NC, bi, is_gravity);
+}
+
 // Classification heads WITHOUT the logits (SURVEY.md 8f-3, option "decode_only"): 1x1 prediction conv 32 -> NC
 // (gravity_head.py:175 / latitude_head.py:174), argmax over the NC logits and bin decode in one pass; the 73 / 180-channel
 // logit tensors (103.6 MB per image) are never written.  Four lanes (a quad) share one pixel: lane q evaluates the classes
@@ -716,9 +740,12 @@ __global__ void __launch_bounds__(256) argmax_decode_kernel(const float* __restr
 // (larger logit wins, the lower class index on ties = torch.argmax's first maximal index).
 // in: [npix, ldi] NHWC (32 channels at icoff); weights [NC][32] + bias staged in shared memory with rows padded to 36 floats
 // (the four lanes of a quad read four different rows with 16-byte loads: no bank conflict).
+// kConf: also the head confidence into conf [B, HW]: each lane keeps a running (max, sum) over its classes (conf_update), and the
+// quad merges the pairs with the same two shuffles, s = s1 exp(m1 - m) + s2 exp(m2 - m).  kConf = false does not read conf.
+template <bool kConf>
 __global__ void __launch_bounds__(256) pred_argmax_decode_kernel(const float* __restrict__ in, int ldi, int icoff, const float* __restrict__ w,
                                                                  const float* __restrict__ bias, float* __restrict__ field, int B, int HW, int NC,
-                                                                 int is_gravity) {
+                                                                 int is_gravity, float* __restrict__ conf) {
   extern __shared__ __align__(16) float s_pw[];  // [NC][36] then [NC]
   for (int i = threadIdx.x; i < NC * 32; i += blockDim.x) s_pw[(i >> 5) * 36 + (i & 31)] = __ldg(w + i);
   float* s_b = s_pw + NC * 36;
@@ -740,7 +767,7 @@ __global__ void __launch_bounds__(256) pred_argmax_decode_kernel(const float* __
       const float4 t = __ldg(reinterpret_cast<const float4*>(in + pc * ldi + icoff + d));
       f[d] = t.x; f[d + 1] = t.y; f[d + 2] = t.z; f[d + 3] = t.w;
     }
-    float best = -INFINITY;
+    float best = -INFINITY, cm = -INFINITY, cs = 0.0f;
     int bi = 0x7fffffff;
     for (int c = q; c < NC; c += 4) {
       const float4* wr = reinterpret_cast<const float4*>(s_pw + c * 36);
@@ -751,14 +778,24 @@ __global__ void __launch_bounds__(256) pred_argmax_decode_kernel(const float* __
         v = fmaf(f[4 * d4], ww.x, v); v = fmaf(f[4 * d4 + 1], ww.y, v); v = fmaf(f[4 * d4 + 2], ww.z, v); v = fmaf(f[4 * d4 + 3], ww.w, v);
       }
       if (v > best || bi == 0x7fffffff) { best = v; bi = c; }      // strict '>': first maximal index of this lane's classes
+      if constexpr (kConf) conf_update(v, cm, cs);
     }
 #pragma unroll
     for (int o = 1; o < 4; o <<= 1) {
       const float ov = __shfl_xor_sync(0xffffffffu, best, o);
       const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
       if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
+      if constexpr (kConf) {
+        const float om = __shfl_xor_sync(0xffffffffu, cm, o), os = __shfl_xor_sync(0xffffffffu, cs, o);
+        const float m = fmaxf(cm, om);
+        cs = cs * expf(cm - m) + os * expf(om - m);
+        cm = m;
+      }
     }
-    if (live && q == 0) decode_bin_store(field, (int)(pix / HW), (int)(pix % HW), HW, NC, bi, is_gravity);
+    if (live && q == 0) {
+      decode_bin_store(field, (int)(pix / HW), (int)(pix % HW), HW, NC, bi, is_gravity);
+      if constexpr (kConf) conf[pix] = 1.0f / cs;
+    }
   }
 }
 

@@ -382,8 +382,9 @@ static int launch_postprocess(const float* vec, const float* lat, int n, int SH,
 }
 
 // prediction 1x1 convs (+ normalise / clamp) -> NCHW outputs, then argmax decode (classification) and resample to the
-// original resolutions.  conv1_out: [n,NH,NW,64] fp32 (gravity head channels 0-31, latitude head 32-63).
-static int fwd_tails_post(Fwd& F, const pf_batch* bt, const float* conv1_out, PostImage* d_post, bool pred_done = false) {
+// original resolutions.  conv1_out: [n,NH,NW,64] fp32 (gravity head channels 0-31, latitude head 32-63).  cf (classification
+// heads only, else NULL): the decode kernels also write the head confidence, resampled to the original sizes after the fields.
+static int fwd_tails_post(Fwd& F, const pf_batch* bt, const pf_confidence* cf, const float* conv1_out, PostImage* d_post, bool pred_done = false) {
   pf_engine* e = F.e;
   const pf_model_desc& D = e->desc;
   const int n = F.n;
@@ -409,10 +410,17 @@ static int fwd_tails_post(Fwd& F, const pf_batch* bt, const float* conv1_out, Po
     // option "decode_only": 1x1 conv + argmax + bin decode in one kernel; pred_gravity / pred_latitude hold the decoded fields
     if (!dry) {
       const unsigned grid = ew_grid((long long)n * HW * 4);
-      LAUNCHED((pred_argmax_decode_kernel<<<grid, 256, D.gravity_classes * 37 * 4, st>>>(conv1_out, 64, 0, e->pred_g_w, e->pred_g_b, bt->pred_gravity, n, HW,
-                                                                                      D.gravity_classes, 1), cudaGetLastError()));
-      LAUNCHED((pred_argmax_decode_kernel<<<grid, 256, D.latitude_classes * 37 * 4, st>>>(conv1_out, 64, 32, e->pred_l_w, e->pred_l_b, bt->pred_latitude, n, HW,
-                                                                                       D.latitude_classes, 0), cudaGetLastError()));
+      if (cf) {
+        LAUNCHED((pred_argmax_decode_kernel<true><<<grid, 256, D.gravity_classes * 37 * 4, st>>>(conv1_out, 64, 0, e->pred_g_w, e->pred_g_b, bt->pred_gravity,
+                                                                                              n, HW, D.gravity_classes, 1, cf->gravity), cudaGetLastError()));
+        LAUNCHED((pred_argmax_decode_kernel<true><<<grid, 256, D.latitude_classes * 37 * 4, st>>>(conv1_out, 64, 32, e->pred_l_w, e->pred_l_b, bt->pred_latitude,
+                                                                                               n, HW, D.latitude_classes, 0, cf->latitude), cudaGetLastError()));
+      } else {
+        LAUNCHED((pred_argmax_decode_kernel<false><<<grid, 256, D.gravity_classes * 37 * 4, st>>>(conv1_out, 64, 0, e->pred_g_w, e->pred_g_b, bt->pred_gravity,
+                                                                                               n, HW, D.gravity_classes, 1, nullptr), cudaGetLastError()));
+        LAUNCHED((pred_argmax_decode_kernel<false><<<grid, 256, D.latitude_classes * 37 * 4, st>>>(conv1_out, 64, 32, e->pred_l_w, e->pred_l_b, bt->pred_latitude,
+                                                                                                n, HW, D.latitude_classes, 0, nullptr), cudaGetLastError()));
+      }
     }
   } else {
     // prediction tails -> NCHW outputs (returned to the caller)
@@ -422,12 +430,18 @@ static int fwd_tails_post(Fwd& F, const pf_batch* bt, const float* conv1_out, Po
     }
     if (cls_g) {
       float* dv = ar.f((long long)n * 2 * HW);
-      if (!dry) LAUNCHED((argmax_decode_kernel<<<(unsigned)cdivl((long long)n * HW, 256), 256, 0, st>>>(bt->pred_gravity, dv, n, HW, D.gravity_classes, 1), cudaGetLastError()));
+      if (!dry && cf)
+        LAUNCHED((argmax_conf_decode_kernel<<<(unsigned)cdivl((long long)n * HW, 256), 256, 0, st>>>(bt->pred_gravity, dv, cf->gravity, n, HW, D.gravity_classes, 1),
+                  cudaGetLastError()));
+      else if (!dry) LAUNCHED((argmax_decode_kernel<<<(unsigned)cdivl((long long)n * HW, 256), 256, 0, st>>>(bt->pred_gravity, dv, n, HW, D.gravity_classes, 1), cudaGetLastError()));
       vec = dv;
     }
     if (cls_l) {
       float* dl = ar.f((long long)n * HW);
-      if (!dry) LAUNCHED((argmax_decode_kernel<<<(unsigned)cdivl((long long)n * HW, 256), 256, 0, st>>>(bt->pred_latitude, dl, n, HW, D.latitude_classes, 0), cudaGetLastError()));
+      if (!dry && cf)
+        LAUNCHED((argmax_conf_decode_kernel<<<(unsigned)cdivl((long long)n * HW, 256), 256, 0, st>>>(bt->pred_latitude, dl, cf->latitude, n, HW, D.latitude_classes, 0),
+                  cudaGetLastError()));
+      else if (!dry) LAUNCHED((argmax_decode_kernel<<<(unsigned)cdivl((long long)n * HW, 256), 256, 0, st>>>(bt->pred_latitude, dl, n, HW, D.latitude_classes, 0), cudaGetLastError()));
       lat = dl;
     }
   }
@@ -435,12 +449,19 @@ static int fwd_tails_post(Fwd& F, const pf_batch* bt, const float* conv1_out, Po
   if (!dry)
     TRY(launch_postprocess(vec, lat, n, e->net_h, e->net_w, bt->height, bt->width, bt->gravity_original_offset, bt->latitude_original_offset, bt->gravity_original,
                            bt->latitude_original, cls_l ? 0 : 1, d_post, st));
+  if (!dry && cf) {   // (d_post holds the per-image descriptors launch_postprocess uploaded, on the same stream)
+    int max_h = 1;
+    for (int i = 0; i < n; ++i) max_h = std::max(max_h, bt->height[i]);
+    LAUNCHED((conf_resample_kernel<<<dim3((unsigned)cdiv(max_h, kPostBand), (unsigned)n), kPostThreads, 0, st>>>(cf->gravity, cf->latitude, d_post,
+                                                                                                                cf->gravity_original, cf->latitude_original,
+                                                                                                                e->net_h, e->net_w), cudaGetLastError()));
+  }
   return PF_OK;
 }
 // =============================================================================================== the forward graph
 // The whole network on the TMA -> wgmma engine: every GEMM input is a pre-split bf16 hi/lo tensor written by its producer
 // (LayerNorm, attention, depthwise conv, upsample, stem gather, or the previous GEMM's epilogue).
-static int run_forward(Fwd& F, const pf_batch* bt) {
+static int run_forward(Fwd& F, const pf_batch* bt, const pf_confidence* cf = nullptr) {
   pf_engine* e = F.e;
   const pf_model_desc& D = e->desc;
   const int n = F.n;
@@ -612,7 +633,7 @@ static int run_forward(Fwd& F, const pf_batch* bt) {
     ar.release(m);
   }
   section("pf:tails_postprocess");
-  TRY(fwd_tails_post(F, bt, conv1_out, d_post, fuse_pred));
+  TRY(fwd_tails_post(F, bt, cf, conv1_out, d_post, fuse_pred));
 
   // ---------------- ParamNet (ConvNeXt-T on the predicted fields) -------------------------------------------
   if (D.param_net != PF_PARAM_NONE) {
@@ -772,15 +793,16 @@ int64_t pf_workspace_bytes(pf_handle h, int n, int max_h) {
   return F.ar.peak + 4096;
 }
 
-int pf_forward(pf_handle h, const pf_batch* bt, void* workspace, int64_t workspace_bytes, void* stream) {
-  if (!h || !bt || !workspace) return fail(PF_ERR_ARG, "pf_forward: null argument");
-  if (!h->finalized) return fail(PF_ERR_WEIGHT, "pf_forward: pf_finalize has not succeeded");
-  if (bt->n < 1) return fail(PF_ERR_ARG, "pf_forward: empty batch");
-  if ((bt->images_u8 != nullptr) == (bt->images_chw != nullptr)) return fail(PF_ERR_ARG, "pf_forward: exactly one of images_u8 / images_chw");
-  if (bt->images_u8 && !bt->image_offset) return fail(PF_ERR_ARG, "pf_forward: image_offset is NULL");
+// pf_forward and pf_forward_confidence (cf non-NULL, checked by the caller)
+static int forward_body(const char* fn, pf_handle h, const pf_batch* bt, const pf_confidence* cf, void* workspace, int64_t workspace_bytes, void* stream) {
+  if (!h || !bt || !workspace) return fail(PF_ERR_ARG, "%s: null argument", fn);
+  if (!h->finalized) return fail(PF_ERR_WEIGHT, "%s: pf_finalize has not succeeded", fn);
+  if (bt->n < 1) return fail(PF_ERR_ARG, "%s: empty batch", fn);
+  if ((bt->images_u8 != nullptr) == (bt->images_chw != nullptr)) return fail(PF_ERR_ARG, "%s: exactly one of images_u8 / images_chw", fn);
+  if (bt->images_u8 && !bt->image_offset) return fail(PF_ERR_ARG, "%s: image_offset is NULL", fn);
   if (!bt->height || !bt->width || !bt->pred_gravity || !bt->pred_latitude || !bt->gravity_original || !bt->latitude_original ||
       !bt->gravity_original_offset || !bt->latitude_original_offset)
-    return fail(PF_ERR_ARG, "pf_forward: null input/output pointer");
+    return fail(PF_ERR_ARG, "%s: null input/output pointer", fn);
   CU(cudaSetDevice(h->device));
   Fwd F{h, Arena{}, (cudaStream_t)stream, false, bt->n};
   F.ar.base = (char*)workspace;
@@ -790,17 +812,32 @@ int pf_forward(pf_handle h, const pf_batch* bt, void* workspace, int64_t workspa
     Fwd T{h, Arena{}, nullptr, true, bt->n};
     T.ar.dry = true; T.ar.keep = h->debug;
     TRY(run_forward(T, nullptr));
-    if (T.ar.peak > workspace_bytes) return fail(PF_ERR_WORKSPACE, "pf_forward: workspace %lld B < required %lld B", (long long)workspace_bytes, T.ar.peak);
+    if (T.ar.peak > workspace_bytes) return fail(PF_ERR_WORKSPACE, "%s: workspace %lld B < required %lld B", fn, (long long)workspace_bytes, T.ar.peak);
   }
-  if (((uintptr_t)workspace & 255) != 0) return fail(PF_ERR_ARG, "pf_forward: workspace must be 256-byte aligned");
+  if (((uintptr_t)workspace & 255) != 0) return fail(PF_ERR_ARG, "%s: workspace must be 256-byte aligned", fn);
   h->taps.clear();
   h->kp.st = (cudaStream_t)stream;
   tl_kp = &h->kp;
   pdl_enabled() = h->use_pdl && !h->kp.on && !h->profile && !sync_debug();   // (event records between launches defeat it anyway)
-  const int r = run_forward(F, bt);
+  const int r = run_forward(F, bt, cf);
   pdl_enabled() = false;
   tl_kp = nullptr;
   return r;
+}
+
+int pf_forward(pf_handle h, const pf_batch* bt, void* workspace, int64_t workspace_bytes, void* stream) {
+  return forward_body("pf_forward", h, bt, nullptr, workspace, workspace_bytes, stream);
+}
+
+int pf_forward_confidence(pf_handle h, const pf_batch* bt, const pf_confidence* cf, void* workspace, int64_t workspace_bytes, void* stream) {
+  if (!h || !cf) return fail(PF_ERR_ARG, "pf_forward_confidence: null argument");
+  if (h->desc.gravity_classes == 2 || h->desc.latitude_classes == 1)
+    return fail(PF_ERR_ARG, "pf_forward_confidence: confidence needs classification heads (this model has %d / %d classes)", h->desc.gravity_classes,
+                h->desc.latitude_classes);
+  const float* ptrs[4] = {cf->gravity, cf->latitude, cf->gravity_original, cf->latitude_original};
+  for (const float* p : ptrs)
+    if (!p || ((uintptr_t)p & 3)) return fail(PF_ERR_ARG, "pf_forward_confidence: a pf_confidence pointer is NULL or not 4-byte aligned");
+  return forward_body("pf_forward_confidence", h, bt, cf, workspace, workspace_bytes, stream);
 }
 
 // ParamNet alone on the caller's fields: the sizing dry run of fwd_paramnet (no launches)
@@ -1144,7 +1181,8 @@ int pf_op_argmax_decode(const float* logits, float* field, int B, int HW, int NC
 int pf_op_pred_argmax_decode(const float* feat, int ld, int coff, const float* w, const float* bias, float* field, int B, int HW, int NC, int is_gravity,
                              void* stream) {
   if (!feat || !w || !bias || !field || B < 1 || HW < 1 || NC < 1 || NC > 256 || (ld & 3) || (coff & 3)) return fail(PF_ERR_ARG, "pf_op_pred_argmax_decode: bad argument");
-  LAUNCHED((pred_argmax_decode_kernel<<<ew_grid((long long)B * HW * 4), 256, NC * 37 * 4, (cudaStream_t)stream>>>(feat, ld, coff, w, bias, field, B, HW, NC, is_gravity),
+  LAUNCHED((pred_argmax_decode_kernel<false><<<ew_grid((long long)B * HW * 4), 256, NC * 37 * 4, (cudaStream_t)stream>>>(feat, ld, coff, w, bias, field, B, HW, NC,
+                                                                                                                        is_gravity, nullptr),
             cudaGetLastError()));
   return PF_OK;
 }

@@ -184,6 +184,35 @@ __device__ __forceinline__ float fast_asinf(float x) {
 // The interpolation is evaluated as hx * (hy v00 + ly v10) + lx * (hy v01 + ly v11): ATen's bilinear kernel nests the two axes the
 // other way round (same weights, same products; the results differ by fp32 rounding only, ~1e-7 relative).
 constexpr int kPostRows = 4, kPostBand = 16, kPostThreads = 256, kPostMaxW = 3072;
+
+// The two head-confidence maps [n, SH, SW] resampled to the original sizes by postprocess_kernel's coordinate rule (bilinear,
+// align_corners=False, no antialias), into blobs laid out like latitude_original (PostImage::l_off).  Block = (band of
+// kPostBand output rows, image); each thread computes its pixels' indices and weights itself, so every width takes one path.
+__global__ void __launch_bounds__(kPostThreads) conf_resample_kernel(const float* __restrict__ cg, const float* __restrict__ cl, const PostImage* __restrict__ imgs,
+                                                                     float* __restrict__ og, float* __restrict__ ol, int SH, int SW) {
+  const PostImage im = imgs[blockIdx.y];
+  const int band0 = blockIdx.x * kPostBand;
+  if (band0 >= im.H) return;
+  const int rows = min(kPostBand, im.H - band0);
+  const float sch = (float)SH / (float)im.H, scw = (float)SW / (float)im.W;
+  const long long SHW = (long long)SH * SW;
+  const float* g = cg + (long long)blockIdx.y * SHW;
+  const float* l = cl + (long long)blockIdx.y * SHW;
+  const int total = rows * im.W;
+  for (int i = threadIdx.x; i < total; i += kPostThreads) {
+    const int yr = i / im.W, x = i - yr * im.W, y = band0 + yr;
+    const float sy = fmaxf(sch * ((float)y + 0.5f) - 0.5f, 0.f);
+    const int y0 = min((int)sy, SH - 1), y1 = y0 + (y0 < SH - 1);
+    const float ly = sy - (float)y0, hy = 1.f - ly;
+    const float sx = fmaxf(scw * ((float)x + 0.5f) - 0.5f, 0.f);
+    const int x0 = min((int)sx, SW - 1), x1 = x0 + (x0 < SW - 1);
+    const float lx = sx - (float)x0, hx = 1.f - lx;
+    const int i00 = y0 * SW + x0, i01 = y0 * SW + x1, i10 = y1 * SW + x0, i11 = y1 * SW + x1;
+    const long long o = im.l_off + (long long)y * im.W + x;
+    og[o] = hx * (hy * __ldg(g + i00) + ly * __ldg(g + i10)) + lx * (hy * __ldg(g + i01) + ly * __ldg(g + i11));
+    ol[o] = hx * (hy * __ldg(l + i00) + ly * __ldg(l + i10)) + lx * (hy * __ldg(l + i01) + ly * __ldg(l + i11));
+  }
+}
 // dynamic shared memory: the source-row buffer (kPostRows x (SW + 1) float4; 20.6 KB at SW = 320) + 8 B per output column
 inline int post_smem_bytes(int SW, int max_wp) { return kPostRows * (SW + 1) * 16 + max_wp * 8; }
 constexpr int kPostSmemMax = kPostRows * (kPreMaxW + 1) * 16 + kPostMaxW * 8;   // 65600 B

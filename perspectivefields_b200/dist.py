@@ -159,7 +159,11 @@ def inference_batch_sharded(model, img_bgr_list, gather_to=0, group=None, micro_
 
     ``model`` provides ``infer_raw(imgs) -> raw`` (the five output blobs of one micro-batch + host metadata),
     ``assemble_raw(raw) -> list[dict]`` and ``out_classes()`` (``PerspectiveFields`` does), optionally ``net_size()`` (the working
-    size of ``pred_gravity`` / ``pred_latitude``; 320 x 320 when absent)."""
+    size of ``pred_gravity`` / ``pred_latitude``; 320 x 320 when absent).  A model built with ``confidence=True`` is refused
+    (``ValueError``): the gather does not carry the confidence maps."""
+    if getattr(model, "_confidence", False):
+        raise ValueError("inference_batch_sharded does not gather the confidence maps of a confidence=True model; "
+                         "call inference_batch on each rank instead")
     if not dist.is_available() or not dist.is_initialized():
         return model.inference_batch(img_bgr_list)
     rank, world = dist.get_rank(group), dist.get_world_size(group)

@@ -74,6 +74,7 @@ class _Engine:
         self.ws_stream = None      # stream of the last forward that used the workspace
         self.ws_event = None       # ... and its completion
         self.decode_only = False
+        self.confidence = False      # pf_forward_confidence: the head-confidence maps as well
         self.pinned = None
         self.pinned_event = None
         self.dev_blob = None
@@ -184,6 +185,10 @@ class _Engine:
             "params": torch.empty((n, 8), dtype=torch.float32, device=dev),
             "g_off": g_off, "l_off": l_off, "h": h, "w": w,
         }
+        if self.confidence:
+            for k in ("gravity_confidence", "latitude_confidence"):
+                out[k] = torch.empty((n, self.net_h, self.net_w), dtype=torch.float32, device=dev)
+                out[k + "_original"] = torch.empty(int(hw.sum()), dtype=torch.float32, device=dev)
         ws = self._workspace(_native.check(self.L.pf_workspace_bytes(self.handle, n, int(h.max()))), cur)
         bt = _native.pf_batch()
         bt.n = n
@@ -199,7 +204,12 @@ class _Engine:
         bt.gravity_original, bt.gravity_original_offset = out["gravity_original"].data_ptr(), g_off.ctypes.data_as(i64p)
         bt.latitude_original, bt.latitude_original_offset = out["latitude_original"].data_ptr(), l_off.ctypes.data_as(i64p)
         bt.params = out["params"].data_ptr()
-        _native.check(self.L.pf_forward(self.handle, ctypes.byref(bt), ws.data_ptr(), ws.numel(), cur.cuda_stream))
+        if self.confidence:
+            cf = _native.pf_confidence(out["gravity_confidence"].data_ptr(), out["latitude_confidence"].data_ptr(),
+                                       out["gravity_confidence_original"].data_ptr(), out["latitude_confidence_original"].data_ptr())
+            _native.check(self.L.pf_forward_confidence(self.handle, ctypes.byref(bt), ctypes.byref(cf), ws.data_ptr(), ws.numel(), cur.cuda_stream))
+        else:
+            _native.check(self.L.pf_forward(self.handle, ctypes.byref(bt), ws.data_ptr(), ws.numel(), cur.cuda_stream))
         ev = torch.cuda.Event()
         ev.record(cur)
         self.ws_event = ev
@@ -288,7 +298,7 @@ class ResizeTransform:
 
 
 class PerspectiveFields(nn.Module):
-    def __init__(self, version="Paramnet-360Cities-edina-centered", logits=True, precision="fp32", resize=None):
+    def __init__(self, version="Paramnet-360Cities-edina-centered", logits=True, precision="fp32", resize=None, confidence=False):
         """``logits=False`` (classification variant only, SURVEY.md 8f-3; NOT the reference's behaviour): ``pred_gravity`` /
         ``pred_latitude`` hold the decoded fields ([2,320,320] up-vectors, [1,320,320] degrees) instead of the 73 / 180 raw logits,
         which are then never written (engine option "decode_only"); the ``*_original`` entries are unchanged.
@@ -303,7 +313,14 @@ class PerspectiveFields(nn.Module):
         order; ``None`` keeps the yaml's ``[320, 320]``.  H and W must be multiples of 32 in [64, 640] with (H/32) * (W/32) <= 256
         (``ValueError`` otherwise, before any GPU work).  ``cfg.DATALOADER.RESIZE``, ``aug`` and the ``[C, H, W]`` fields
         ``pred_gravity`` / ``pred_latitude`` follow it; ``forward`` expects ``[3, H, W]`` images.  Like ``precision`` it survives
-        ``.to()`` / ``load_state_dict``."""
+        ``.to()`` / ``load_state_dict``.
+
+        ``confidence=True`` (classification variant only, ``ValueError`` otherwise): every result also carries how sure each head is
+        at each pixel, ``max_c softmax(logits)_c`` over all of the head's classes (DESIGN.md section 1, "Head confidence"), in
+        [1/NC, 1]: ``pred_gravity_confidence`` / ``pred_latitude_confidence`` [H, W] at the working size and
+        ``pred_gravity_confidence_original`` / ``pred_latitude_confidence_original`` [height, width], resampled as the latitude
+        map is.  They follow the other keys, whose values are unchanged.  It combines with ``logits``, ``precision`` and
+        ``resize`` and survives ``.to()`` / ``load_state_dict``; ``calibrate.fit_camera(..., weights="confidence")`` reads it."""
         super().__init__()
         zoo = model_zoo[version]  # KeyError for unknown versions, like the reference (perspectivefields.py:127)
         self.version = version
@@ -328,6 +345,11 @@ class PerspectiveFields(nn.Module):
             if self._variant["gravity"] != "classification":
                 raise ValueError("logits=False only applies to the classification variant (PersNet-360Cities)")
             self._options["decode_only"] = 1
+        if not isinstance(confidence, bool):
+            raise ValueError(f"confidence must be a bool, got {confidence!r}")
+        if confidence and self._variant["gravity"] != "classification":
+            raise ValueError(f"confidence=True needs classification heads; {version} regresses its fields (PersNet-360Cities has them)")
+        self._confidence = bool(confidence)
         if precision not in ("fp32", "bf16"):
             raise ValueError(f"precision must be 'fp32' or 'bf16', got {precision!r}")
         if precision == "bf16":
@@ -433,6 +455,7 @@ class PerspectiveFields(nn.Module):
             for k, v in self._options.items():
                 _native.check(eng.L.pf_set_option(eng.handle, k.encode(), v))
             eng.decode_only = bool(self._options.get("decode_only", 0))
+            eng.confidence = self._confidence
             self._engine = eng
         self._pn_sync(self._engine)
         return self._engine
@@ -696,6 +719,12 @@ class PerspectiveFields(nn.Module):
                 d.update({"pred_roll": cols[0][i], "pred_pitch": cols[1][i], "pred_general_vfov": cols[2][i], "pred_rel_cx": cols[3][i],
                           "pred_rel_cy": cols[4][i], "pred_rel_focal": cols[5][i]})
             res.append(d)
+        if "gravity_confidence" in out:
+            hw = [h * w for h, w in zip(hs, ws)]
+            for k in ("gravity_confidence", "latitude_confidence", "gravity_confidence_original", "latitude_confidence_original"):
+                maps = out[k].unbind(0) if out[k].dim() == 3 else [t.view(h, w) for t, h, w in zip(out[k].split(hw), hs, ws)]
+                for i in range(n):
+                    res[i]["pred_" + k] = maps[i]
         return res
 
     # ------------------------------------------------------------------------------------------ scoring API
