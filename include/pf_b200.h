@@ -441,7 +441,8 @@ int pf_op_conv_gemm(const float* x, int B, int H, int W, int Cin, const void* wh
  *   v += res2[m * ldr2 + r2_coff + g * r2_gcoff + n]
  *   C[m * ldc + c_coff + g * c_gcoff + n] = v;  S planes at m * lds + s_coff + g * s_gcoff + n = split(relu?(v)) (split_relu).
  * phase4 (halo mode, N = 128): column 32 ph + c is channel c of output pixel (2y + ph / 2, 2x + ph % 2) of a 2H x 2W grid.
- * pred[g] (halo mode, npred = groups): fused 1x1 conv 32 -> nc + normalise (mode 1) / clamp (mode 2), NCHW into pred[g].out.
+ * pred[g] (halo mode, npred = groups): fused 1x1 conv 32 -> nc + normalise (mode 1) / clamp (mode 2), NCHW into pred[g].out;
+ * C and S may then both be NULL (the tails are the only output).
  * force_bn / force_kb: run this instantiation instead of the dispatcher's (0 = its choice); a pair the engine does not
  * instantiate, or cannot run this problem with, is PF_ERR_ARG before anything is launched.  picked_bn / picked_kb: what ran.
  * force_sched (GEMM mode): 0 = the dispatcher's schedule, 1 = cooperative (128-row tiles), 2 = ping-pong (64-row tiles, one

@@ -1053,7 +1053,8 @@ static int op_tma(pf_tma_op* op, void* stream, bool bf16) {
   if (!op || !op->a_hi || !op->a_lo || !op->w_hi || !op->w_lo) return fail(PF_ERR_ARG, "pf_op_tma: null argument");
   const pf_tma_op& q = *op;
   if (q.mode != MODE_GEMM && q.mode != MODE_HALO) return fail(PF_ERR_ARG, "pf_op_tma: mode %d", q.mode);
-  if (!q.C && !q.s_hi) return fail(PF_ERR_ARG, "pf_op_tma: no output (C and S are both NULL)");
+  // (a launch with fused prediction tails may write them alone: the forward's conv_fuse_conv1 of regression heads does)
+  if (!q.C && !q.s_hi && !q.npred) return fail(PF_ERR_ARG, "pf_op_tma: no output (C, S and the prediction tails are all NULL)");
   if (!q.s_hi != !q.s_lo || !q.a2_hi != !q.a2_lo) return fail(PF_ERR_ARG, "pf_op_tma: a split pair needs both planes");
   if (q.bias_mode < 0 || q.bias_mode > 2 || q.act < 0 || q.act > 2) return fail(PF_ERR_ARG, "pf_op_tma: bias_mode %d / act %d", q.bias_mode, q.act);
   if (q.groups < 1 || q.groups > 2 || q.N < 1) return fail(PF_ERR_ARG, "pf_op_tma: groups %d, N %d", q.groups, q.N);
