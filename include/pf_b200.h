@@ -367,6 +367,40 @@ int pf_fit_camera_groups_weighted(int device, const pf_fit_image* images, int n,
                                   const int64_t* lat_weight_offset, int principal_point, double huber, int max_iterations, double* params,
                                   double* cost, int32_t* iterations, int32_t* status, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- panorama levelling (csrc/calib.cuh, csrc/equi.cuh) ------------------------------------------------------------------------
+ * pf_fit_panorama: the tilt of each panorama from the fields of views cropped from it (DESIGN.md section 1, "Panorama levelling"):
+ * theta = (psi, phi) with T = Z(psi) X(phi) and the panorama's up direction g = T^T n, n = (0, -1, 0); view k (a crop of
+ * pf_equi_views' rule at pf_pano_crop k) sees the world up v_k = A_k^T g, A_k = Y(azimuth) X(elevation) Z(roll), with the
+ * crop's own intrinsics (F = W / (2 tan(fov_x / 2)), centred).  Residuals, weights, Huber cost, Levenberg-Marquardt rules and
+ * the status of pf_fit_camera_weighted, summed over the views of each panorama.  images: HOST [n] as pf_fit_camera reads them
+ * (init is not read); crops: HOST [n]; panorama_of: HOST int32 [n], values 0 .. npano - 1, every panorama with at least one view;
+ * init: HOST [npano][2] start (psi, phi) in degrees, or NULL for 0, 0.  Outputs (DEVICE), panorama P: angles[2P .. 2P + 1] =
+ * psi (|psi| <= 90) and phi ((-180, 180]) in degrees; up[3P ..] = g; rotation[9P ..] = the smallest rotation R with R n = g,
+ * row-major (pf_rotate_panoramas with it levels the panorama); cost, iterations, status (2: NaN outputs).  Enqueued on `stream`
+ * without synchronisation.  workspace: DEVICE, 256-byte aligned, pf_fit_panorama_workspace bytes. */
+typedef struct pf_pano_crop {
+  double vfov, azimuth, elevation, roll, ar;   /* degrees (vfov in (0, 180)), and the aspect ratio, as in pf_equi_view */
+} pf_pano_crop;
+int64_t pf_fit_panorama_workspace(const pf_fit_image* images, int n, const int32_t* panorama_of, int npano);
+int pf_fit_panorama(int device, const pf_fit_image* images, const pf_pano_crop* crops, int n, const int32_t* panorama_of, int npano,
+                    const float* up_base, const float* lat_base, const uint8_t* mask_base, const float* weight_base,
+                    const int64_t* up_weight_offset, const int64_t* lat_weight_offset, const double* init, double huber, int max_iterations,
+                    double* angles, double* up, double* rotation, double* cost, int32_t* iterations, int32_t* status, void* workspace,
+                    int64_t workspace_bytes, void* stream);
+/* pf_rotate_panoramas: out(d) = P(R_P d) for n equirectangular panoramas of any sizes in one launch (DESIGN.md section 1, "Panorama
+ * levelling"): in / out DEVICE blobs of [height, width, channels] panoramas of dtype enum pf_equi_dtype (element offsets),
+ * channels 1 or 3, mode enum pf_equi_mode (bilinear: uint8 rounded to nearest; nearest); map_base: DEVICE float32 [height, width,
+ * 2] input positions (u, v) per panorama at map_offset (floats; -1: none), or NULL; rotations: DEVICE float64 [n][9] row-major,
+ * read on the device.  workspace: DEVICE, 256-byte aligned, pf_rotate_panoramas_workspace bytes.  Every argument is checked before
+ * anything is launched (PF_ERR_ARG). */
+typedef struct pf_rotate_pano {
+  int32_t height, width;        /* >= 2 each */
+  int64_t in_offset, out_offset, map_offset;
+} pf_rotate_pano;
+int64_t pf_rotate_panoramas_workspace(const pf_rotate_pano* panos, int n);
+int pf_rotate_panoramas(int device, const pf_rotate_pano* panos, int n, int channels, int dtype, int mode, const void* in_base, void* out_base,
+                        float* map_base, const double* rotations, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ---- upright warp: straightened images from camera parameters (csrc/rectify.cuh) --------------------------------------------
  * Warps each uint8 image (1 or 3 channels, HWC) to a camera with roll 0, pitch 0 (or the input pitch with keep_pitch), a centred
  * principal point and the focal length of enum pf_rectify_focal, by the rule of DESIGN.md section 1 ("Upright warp").  Offsets are

@@ -66,6 +66,18 @@ class pf_rectify_image(ctypes.Structure):
                 ("in_offset", ctypes.c_int64), ("out_offset", ctypes.c_int64), ("mask_offset", ctypes.c_int64), ("map_offset", ctypes.c_int64)]
 
 
+class pf_pano_crop(ctypes.Structure):
+    """include/pf_b200.h: struct pf_pano_crop (the crop of one view of pf_fit_panorama)."""
+    _fields_ = [("vfov", ctypes.c_double), ("azimuth", ctypes.c_double), ("elevation", ctypes.c_double), ("roll", ctypes.c_double),
+                ("ar", ctypes.c_double)]
+
+
+class pf_rotate_pano(ctypes.Structure):
+    """include/pf_b200.h: struct pf_rotate_pano (one panorama of pf_rotate_panoramas)."""
+    _fields_ = [("height", ctypes.c_int32), ("width", ctypes.c_int32), ("in_offset", ctypes.c_int64), ("out_offset", ctypes.c_int64),
+                ("map_offset", ctypes.c_int64)]
+
+
 PF_RECTIFY_SAME, PF_RECTIFY_VFOV, PF_RECTIFY_FILL = 0, 1, 2
 PF_RECTIFY_BILINEAR, PF_RECTIFY_NEAREST = 0, 1
 
@@ -235,6 +247,12 @@ def lib():
                                          ctypes.c_double, i32, vp, vp, vp, vp, vp, i64, vp]),
         "pf_fit_camera_groups_weighted": (i32, [i32, ctypes.POINTER(pf_fit_image), i32, ctypes.POINTER(ctypes.c_int32), i32, vp, vp, vp, vp,
                                                 ctypes.POINTER(i64), ctypes.POINTER(i64), i32, ctypes.c_double, i32, vp, vp, vp, vp, vp, i64, vp]),
+        "pf_fit_panorama_workspace": (i64, [ctypes.POINTER(pf_fit_image), i32, ctypes.POINTER(ctypes.c_int32), i32]),
+        "pf_fit_panorama": (i32, [i32, ctypes.POINTER(pf_fit_image), ctypes.POINTER(pf_pano_crop), i32, ctypes.POINTER(ctypes.c_int32), i32, vp,
+                                  vp, vp, vp, ctypes.POINTER(i64), ctypes.POINTER(i64), ctypes.POINTER(ctypes.c_double), ctypes.c_double, i32,
+                                  vp, vp, vp, vp, vp, vp, vp, i64, vp]),
+        "pf_rotate_panoramas_workspace": (i64, [ctypes.POINTER(pf_rotate_pano), i32]),
+        "pf_rotate_panoramas": (i32, [i32, ctypes.POINTER(pf_rotate_pano), i32, i32, i32, i32, vp, vp, vp, vp, vp, i64, vp]),
         "pf_rectify_workspace": (i64, [ctypes.POINTER(pf_rectify_image), i32]),
         "pf_rectify_views": (i32, [i32, ctypes.POINTER(pf_rectify_image), i32, vp, vp, vp, vp, i32, vp, i32, i32, ctypes.c_double, i32,
                                    ctypes.POINTER(ctypes.c_int32), vp, vp, vp, i64, vp]),
@@ -306,7 +324,8 @@ EXPORTS = ["pf_abi_version", "pf_last_error", "pf_kernel_launch_count", "pf_crea
            "pf_debug_copy", "pf_camera_fields", "pf_camera_fields_vp", "pf_pano_views", "pf_equi_views", "pf_draw_fields",
            "pf_encode_fields", "pf_head_losses_workspace", "pf_head_losses", "pf_field_errors_workspace", "pf_field_errors",
            "pf_fit_camera_workspace", "pf_fit_camera", "pf_fit_camera_groups_workspace", "pf_fit_camera_groups",
-           "pf_fit_camera_weighted", "pf_fit_camera_groups_weighted",
+           "pf_fit_camera_weighted", "pf_fit_camera_groups_weighted", "pf_fit_panorama_workspace", "pf_fit_panorama",
+           "pf_rotate_panoramas_workspace", "pf_rotate_panoramas",
            "pf_rectify_workspace", "pf_rectify_views", "pf_comm_unique_id", "pf_comm_create", "pf_comm_destroy", "pf_gather",
            "pf_jpeg_create", "pf_jpeg_destroy", "pf_jpeg_info", "pf_jpeg_decode_batch",
            "pf_op_conv_gemm", "pf_op_tma", "pf_op_tma_bf16", "pf_op_conv1_ring", "pf_tma_pick_tile", "pf_op_layernorm",

@@ -7,6 +7,8 @@ refinement of theirs.  With ``groups`` it fits images taken with one camera toge
 phone's photos): each image keeps its own roll and pitch, and each group gets one focal length (and principal point), which one
 image alone constrains least (DESIGN.md section 1, "Shared intrinsics").  Its output has the keys of a ParamNet variant's
 results, so ``metrics.param_errors``, ``panocam.fields_from_predictions`` and ``viz.draw_from_r_p_f_cx_cy`` take it unchanged.
+``fit_panorama`` fits one tilt per equirectangular panorama to the fields of views cropped from it (DESIGN.md section 1,
+"Panorama levelling").
 """
 import ctypes
 import math
@@ -16,7 +18,7 @@ import numpy as np
 import torch
 
 from . import _batch, _native
-from .panocam import general_vfov, general_vfov_to_focal
+from .panocam import _check_equi_view, general_vfov, general_vfov_to_focal
 
 MAX_ITERATIONS = 1000
 _NAN_INIT = (math.nan,) * 5
@@ -152,3 +154,96 @@ def fit_camera(results, principal_point=False, init="fields", mask=None, huber=N
         d.update({"fit_cost": cost[i], "fit_iterations": its[i], "fit_status": status[i]})
         out.append(d)
     return out
+
+
+def _panorama_ids(panorama_of, n):
+    """n integers 0 .. npano - 1, each used -> (int32 ctypes array, npano)."""
+    try:
+        labels = list(panorama_of)
+    except TypeError:
+        raise ValueError(f"panorama_of must be a sequence of {n} integers, got {panorama_of!r}") from None
+    if len(labels) != n:
+        raise ValueError(f"{n} results but {len(labels)} panorama_of entries")
+    for i, v in enumerate(labels):
+        if isinstance(v, (bool, np.bool_)) or not isinstance(v, numbers.Integral) or int(v) < 0:
+            raise ValueError(f"panorama_of[{i}] must be an integer >= 0, got {v!r}")
+    npano = max(int(v) for v in labels) + 1
+    missing = sorted(set(range(npano)) - {int(v) for v in labels})
+    if missing:
+        raise ValueError(f"panorama_of names panoramas 0 .. {npano - 1} but none of the views belongs to {missing}")
+    return (ctypes.c_int32 * n)(*(int(v) for v in labels)), npano
+
+
+def fit_panorama(results, views, panorama_of, mask=None, weights=None, huber=None, max_iterations=50, init=None):
+    """Fit the tilt of equirectangular panoramas to the fields predicted on views cropped from them (DESIGN.md section 1,
+    "Panorama levelling").  View i is ``results[i]`` (fields as ``fit_camera`` reads them, in place), cropped by
+    ``panocam.crop_equi_views`` with ``views[i]`` (its ``(vfov, im_w, im_h, azimuth, elevation, roll, ar)`` tuple or dict, whose
+    size must be the fields'), from panorama ``panorama_of[i]`` (integers 0 .. npano - 1, each used).  All views of a panorama
+    share one unknown, its tilt T = Z(psi) X(phi) (pano roll psi, pano pitch phi; yaw is not observable): a panorama P with tilt
+    T shows P(d) = P_level(T d).
+
+    - ``mask``, ``weights`` (including ``"confidence"``), ``huber``, ``max_iterations``: as in ``fit_camera``, per view;
+      ``max_iterations`` counts cost evaluations of each panorama.
+    - ``init``: None (psi = phi = 0) or one ``(psi, phi)`` pair in degrees per panorama.
+
+    Returns one dict per panorama of CUDA tensors: ``pano_roll`` and ``pano_pitch`` (0-dim float64, degrees, |roll| <= 90 and
+    pitch in (-180, 180]), ``pano_up`` ([3], the panorama's up direction g = T^T (0, -1, 0) in its own pixel frame: x right, y
+    down, z at azimuth 0), ``rotation`` ([3, 3], the smallest rotation R with R (0, -1, 0) = g: ``rectify.rotate_panoramas``
+    with it levels the panorama), ``fit_cost``, ``fit_iterations`` and ``fit_status`` (as ``fit_camera``'s; status 2: NaN
+    outputs).  Nothing synchronises with the device; invalid arguments raise before any GPU work."""
+    if huber is not None:
+        if isinstance(huber, bool) or not isinstance(huber, (int, float)) or not math.isfinite(huber) or huber <= 0:
+            raise ValueError(f"huber must be None or a finite number > 0, got {huber!r}")
+    if isinstance(max_iterations, bool) or not isinstance(max_iterations, int) or not 1 <= max_iterations <= MAX_ITERATIONS:
+        raise ValueError(f"max_iterations must be an integer in 1 .. {MAX_ITERATIONS}, got {max_iterations!r}")
+    n = len(results)
+    if n == 0:
+        raise ValueError("no views")
+    vs = [_check_equi_view(v, i) for i, v in enumerate(views)]
+    if len(vs) != n:
+        raise ValueError(f"{n} results but {len(vs)} views")
+    if mask is not None and len(mask) != n:
+        raise ValueError(f"{n} results but {len(mask)} masks")
+    pano_of, npano = _panorama_ids(panorama_of, n)
+    starts = None
+    if init is not None:
+        starts = [tuple(p) if isinstance(p, (tuple, list, np.ndarray)) else p for p in init]
+        if len(starts) != npano or any(not isinstance(p, tuple) or len(p) != 2 for p in starts):
+            raise ValueError(f"init must be None or {npano} (pano_roll, pano_pitch) pairs in degrees")
+        starts = (ctypes.c_double * (2 * npano))(*(_batch.real(v, "init") for p in starts for v in p))
+    pu, pl, ms, dev = _batch.prediction_fields(results, mask, 3)
+    for i, v in enumerate(vs):
+        if (v[2], v[1]) != (int(pu[i].shape[0]), int(pu[i].shape[1])):
+            raise ValueError(f"views[{i}] is {v[2]} x {v[1]} but results[{i}] has fields of {pu[i].shape[0]} x {pu[i].shape[1]}")
+    wts = _batch.fit_weights(weights, results, pu, dev)
+    L = _native.lib()
+    bu, bl, bm = _batch.base(pu), _batch.base(pl), _batch.base(ms)
+    bw = _batch.base([t for e in wts for t in e])
+    uw = (ctypes.c_int64 * n)(*(_batch.offset(e[0], bw) for e in wts))
+    lw = (ctypes.c_int64 * n)(*(_batch.offset(e[1], bw) for e in wts))
+    descs = (_native.pf_fit_image * n)()
+    crops = (_native.pf_pano_crop * n)()
+    for i in range(n):
+        d = descs[i]
+        d.height, d.width = int(pu[i].shape[0]), int(pu[i].shape[1])
+        d.up_offset, d.up_stride[:] = _batch.offset(pu[i], bu), pu[i].stride()
+        d.lat_offset = _batch.offset(pl[i], bl)
+        d.mask_offset = _batch.offset(ms[i], bm)
+        d.init[:] = _NAN_INIT
+        vfov, _, _, az, el, roll, ar = vs[i]
+        crops[i] = _native.pf_pano_crop(vfov, az, el, roll, ar)
+    with torch.cuda.device(dev):
+        ws = _batch.workspace(L.pf_fit_panorama_workspace(descs, n, pano_of, npano), dev)
+        ang = torch.empty((npano, 2), dtype=torch.float64, device=dev)
+        up = torch.empty((npano, 3), dtype=torch.float64, device=dev)
+        rot = torch.empty((npano, 3, 3), dtype=torch.float64, device=dev)
+        cost = torch.empty(npano, dtype=torch.float64, device=dev)
+        its = torch.empty(npano, dtype=torch.int32, device=dev)
+        status = torch.empty(npano, dtype=torch.int32, device=dev)
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        _native.check(L.pf_fit_panorama(dev.index, descs, crops, n, pano_of, npano, bu, bl, bm or None, bw or None, uw, lw, starts,
+                                        float(huber or 0.0), max_iterations, ang.data_ptr(), up.data_ptr(), rot.data_ptr(), cost.data_ptr(),
+                                        its.data_ptr(), status.data_ptr(), ws.data_ptr(), ws.numel(), stream))
+    ang, cost, its, status = ang.unbind(0), cost.unbind(0), its.unbind(0), status.unbind(0)
+    return [{"pano_roll": ang[P][0], "pano_pitch": ang[P][1], "pano_up": up[P], "rotation": rot[P], "fit_cost": cost[P],
+             "fit_iterations": its[P], "fit_status": status[P]} for P in range(npano)]

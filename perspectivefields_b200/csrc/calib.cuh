@@ -21,6 +21,9 @@
 //
 // Groups of images with shared intrinsics (pf_fit_camera_groups, "shared intrinsics" below) reuse the start and the pass, and
 // replace the step by fit_reduce_kernel (each image's sums) and fit_group_step_kernel (one Schur-complement step per group).
+//
+// Panorama levelling (pf_fit_panorama, "panorama levelling" below) fits one tilt to all views cropped from a panorama: the pass
+// in terms of each view's world up direction v (fit_pass_kernel<3, kW, true>), fit_reduce_kernel, then fit_pano_step_kernel.
 #pragma once
 #include <stdint.h>
 
@@ -172,8 +175,11 @@ __device__ __forceinline__ void fit_accumulate(double (&acc)[fit_nq(P)], double 
 
 // Blocks of kFitTile pixels, each within one image.  Writes plane q of the partials: 0 = sum delta^2 rho (2 C), 1 = residual
 // count, 2 .. 1 + P = g, then A's upper triangle row by row.  kW: the launch has weight maps (an image without one has v = 1).
-template <int P, bool kW = false>
+// kV (P = 3, the panorama fit below): the model in terms of the world up direction v in camera coordinates, cand[0 .. 2] = v,
+// with fixed intrinsics F = init[2] (pixels), cx = (init[3] + 1/2) W, cy = (init[4] + 1/2) H; g and A are taken with respect to v.
+template <int P, bool kW = false, bool kV = false>
 __global__ void __launch_bounds__(kFitThreads) fit_pass_kernel(FitArgs a) {
+  static_assert(!kV || P == 3, "the v model has three parameters");
   constexpr int NQ = fit_nq(P);
   __shared__ double shq[kFitThreads / 32][NQ];
   pdl_wait();
@@ -184,10 +190,13 @@ __global__ void __launch_bounds__(kFitThreads) fit_pass_kernel(FitArgs a) {
   double th[5];
 #pragma unroll
   for (int k = 0; k < 5; ++k) th[k] = a.st[img].cand[k];
-  const double F = exp(th[2]) * d.H, cx = (th[3] + 0.5) * d.W, cy = (th[4] + 0.5) * d.H;
-  double sr, cr, se, ce;
-  sincos(th[0], &sr, &cr);
-  sincos(th[1], &se, &ce);
+  const double F = kV ? d.init[2] : exp(th[2]) * d.H;
+  const double cx = ((kV ? d.init[3] : th[3]) + 0.5) * d.W, cy = ((kV ? d.init[4] : th[4]) + 0.5) * d.H;
+  double sr = 0.0, cr = 0.0, se = 0.0, ce = 0.0;
+  if constexpr (!kV) {
+    sincos(th[0], &sr, &cr);
+    sincos(th[1], &se, &ce);
+  }
   const double Hd = d.H, Wd = d.W;
   // get_lat_general's grid: linspace((-W/2) - (cx - W/2), (W/2) - (cx - W/2), W), last sample exact (camera_fields_kernel)
   const double x0 = (-Wd / 2.0) - (cx - Wd / 2.0), x1 = (Wd / 2.0) - (cx - Wd / 2.0), sxg = (x1 - x0) / (Wd - 1.0);
@@ -212,15 +221,23 @@ __global__ void __launch_bounds__(kFitThreads) fit_pass_kernel(FitArgs a) {
       const double px = p[0], py = p[d.up_sk];
       if (up_usable(px, py)) {
         const double ex = cx - ((double)x + 0.5), ey = cy - ((double)y + 0.5);
-        const double ux = -sr * ce * F + se * ex, uy = -cr * ce * F + se * ey;
+        double ux, uy;
+        if constexpr (kV) { ux = F * th[0] + th[2] * ex; uy = F * th[1] + th[2] * ey; }
+        else { ux = -sr * ce * F + se * ex; uy = -cr * ce * F + se * ey; }
         const double u2 = ux * ux + uy * uy;
         if (u2 > 0.0) {
           const double r = atan2(ux * py - uy * px, ux * px + uy * py);
           // r = angle(p) - angle(u):  dr = -(ux duy - uy dux) / |u|^2
           double dux[P], duy[P], J[P];
-          dux[0] = -cr * ce * F;          duy[0] = sr * ce * F;
-          dux[1] = sr * se * F + ce * ex; duy[1] = cr * se * F + ce * ey;
-          dux[2] = -sr * ce * F;          duy[2] = -cr * ce * F;
+          if constexpr (kV) {   // u = F (vx, vy) + vz (ex, ey)
+            dux[0] = F;   duy[0] = 0.0;
+            dux[1] = 0.0; duy[1] = F;
+            dux[2] = ex;  duy[2] = ey;
+          } else {
+            dux[0] = -cr * ce * F;          duy[0] = sr * ce * F;
+            dux[1] = sr * se * F + ce * ex; duy[1] = cr * se * F + ce * ey;
+            dux[2] = -sr * ce * F;          duy[2] = -cr * ce * F;
+          }
           if constexpr (P == 5) { dux[3] = se * Wd; duy[3] = 0.0; dux[4] = 0.0; duy[4] = se * Hd; }
           const double iu2 = 1.0 / u2;
 #pragma unroll
@@ -239,6 +256,21 @@ __global__ void __launch_bounds__(kFitThreads) fit_pass_kernel(FitArgs a) {
       if (isfinite(lp)) {
         const double dx = x == d.W - 1 ? x1 : fma((double)x, sxg, x0), dy = y == d.H - 1 ? y1 : fma((double)y, syg, y0);
         const double xx = dx * rF, yy = dy * rF;
+        if constexpr (kV) {
+          // l = atan2(v . c, |v x c|) for the ray c = (xx, yy, 1); along the sphere dl = c . dv / |v x c|, J = -dl
+          const double s = th[0] * xx + th[1] * yy + th[2];
+          const double qx = th[1] - th[2] * yy, qy = th[2] * xx - th[0], qz = th[0] * yy - th[1] * xx;
+          const double h = sqrt(qx * qx + qy * qy + qz * qz), ih = 1.0 / h;
+          const double r = lp * (kPi / 180.0) - atan2(s, h);
+          const double J[P] = {-xx * ih, -yy * ih, -ih};
+          if constexpr (kW) {
+            const double v = fit_weight(a, d.lw_off, q);
+            if (v > 0.0) fit_accumulate<P, true>(acc, r, J, a.huber, v);
+          } else {
+            fit_accumulate<P>(acc, r, J, a.huber);
+          }
+          continue;
+        }
         const double xw = xx * cr - yy * sr;
         const double yw = xx * (ce * sr) + yy * (ce * cr) - se;
         const double zw = xx * (se * sr) + yy * (se * cr) + ce;
@@ -656,6 +688,192 @@ __global__ void __launch_bounds__(kFitGroupThreads, 1) fit_group_step_kernel(Fit
     fit_finish<P>(a, i, s, s.status == 2 ? 2 : status);
   }
   if (threadIdx.x == 0) { gs.evals = evals; gs.status = status; }
+}
+
+// ------------------------------------------------------------------------------------------------------ panorama levelling
+// Views cropped from one panorama share its tilt (DESIGN.md section 1, "Panorama levelling"): theta = (psi, phi), T = Z(psi) X(phi),
+// the panorama's up direction g = T^T n = (-sin psi, -cos psi cos phi, cos psi sin phi) for n = (0, -1, 0), and view k (crop
+// rotation A_k) sees the world up direction v_k = A_k^T g.  The pass is fit_pass_kernel<3, kW, true> (sums with respect to v),
+// fit_reduce_kernel writes each view's sums, and fit_pano_step_kernel (one warp per panorama) takes one Levenberg-Marquardt step
+// on A = sum D_k^T A_k D_k, g = sum D_k^T g_k with D_k = A_k^T dg/dtheta, then writes each member's next v_k.
+struct FitPanoState {
+  double theta[2], cand[2];   // accepted (psi, phi) and the candidate the next pass evaluates
+  double A[3], g[2], C;       // at theta (A: upper triangle)
+  double lambda;
+  int evals, status;
+};
+struct FitPanos {
+  const int* off;             // [npano + 1]: panorama P's views are mem[off[P] .. off[P + 1] - 1]
+  const int* mem;             // [n] view indices, in index order within each panorama
+  const double* rot;          // [n][9] A_k row-major
+  const double* init;         // [npano][2] start (psi, phi), radians
+  FitPanoState* ps;           // [npano]
+  double* sums;               // [n][kFitQ]: each view's sums of its last pass (fit_reduce_kernel)
+  int npano;
+  double* angles; double* up; double* R; double* cost; int* iters; int* status;   // outputs [npano][2], [3], [9], [1] ...
+};
+
+// g(theta) and its derivatives dg[m][k] = d g_m / d theta_k
+__device__ __forceinline__ void pano_gravity(const double (&th)[2], double (&gv)[3], double (&dg)[3][2]) {
+  double sp, cp, sf, cf;
+  sincos(th[0], &sp, &cp);
+  sincos(th[1], &sf, &cf);
+  gv[0] = -sp; gv[1] = -cp * cf; gv[2] = cp * sf;
+  dg[0][0] = -cp;      dg[0][1] = 0.0;
+  dg[1][0] = sp * cf;  dg[1][1] = cp * sf;
+  dg[2][0] = -sp * sf; dg[2][1] = cp * cf;
+}
+
+// The member views of panorama P taken by lanes lane, lane + 32, ...: candidate v_k = A_k^T g(th), or the final status
+__device__ __forceinline__ void pano_members(const FitArgs& a, const FitPanos& p, int P, int lane, const double (&th)[2], int status) {
+  double gv[3], dg[3][2];
+  pano_gravity(th, gv, dg);
+  for (int j = p.off[P] + lane; j < p.off[P + 1]; j += 32) {
+    const int i = p.mem[j];
+    FitState& s = a.st[i];
+    if (status == kFitRunning) {
+      const double* M = p.rot + 9LL * i;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) s.cand[c] = M[c] * gv[0] + M[3 + c] * gv[1] + M[6 + c] * gv[2];
+    }
+    s.status = status;
+  }
+}
+
+// One warp per panorama: the start (init, or psi = phi = 0) and every member's v_k
+__global__ void __launch_bounds__(32 * kFitStepWarps) fit_pano_init_kernel(FitArgs a, FitPanos p) {
+  pdl_wait();
+  pdl_launch();
+  const int P = blockIdx.x * kFitStepWarps + (threadIdx.x >> 5);
+  if (P >= p.npano) return;
+  const double th[2] = {p.init[2 * P], p.init[2 * P + 1]};
+  pano_members(a, p, P, threadIdx.x & 31, th, kFitRunning);
+  if ((threadIdx.x & 31) == 0) {
+    FitPanoState& s = p.ps[P];
+    for (int k = 0; k < 2; ++k) s.theta[k] = s.cand[k] = th[k];
+    s.C = 0.0; s.lambda = kFitLambda0; s.evals = 0; s.status = kFitRunning;
+  }
+}
+
+// (psi, phi) -> outputs: the pair with |psi| <= 90 degrees and phi in (-180, 180] ((psi, phi) and (180 - psi, phi + 180) give the
+// same g), g, and R = the smallest rotation with R n = g: I cos a + [w]x + w w^T / (1 + cos a) for w = n x g, cos a = n . g (180
+// degrees about x when g = -n)
+__device__ void pano_finish(const FitPanos& p, int P, const FitPanoState& s, int status) {
+  double* ang = p.angles + 2LL * P;
+  double* up = p.up + 3LL * P;
+  double* R = p.R + 9LL * P;
+  if (status == 2) {
+    ang[0] = ang[1] = NAN;
+    for (int k = 0; k < 3; ++k) up[k] = NAN;
+    for (int k = 0; k < 9; ++k) R[k] = NAN;
+    p.cost[P] = NAN;
+  } else {
+    double psi = wrap_pi(s.theta[0]), phi = s.theta[1];
+    if (fabs(psi) > kPi / 2.0) { psi = wrap_pi(kPi - psi); phi += kPi; }
+    phi = wrap_pi(phi);
+    const double th[2] = {psi, phi};
+    double gv[3], dg[3][2];
+    pano_gravity(th, gv, dg);
+    ang[0] = psi * (180.0 / kPi); ang[1] = phi * (180.0 / kPi);
+    for (int k = 0; k < 3; ++k) up[k] = gv[k];
+    const double c = -gv[1], wx = -gv[2], wz = gv[0];   // n = (0, -1, 0): w = n x g = (-gz, 0, gx)
+    if (1.0 + c > 0.0) {
+      const double q = 1.0 / (1.0 + c);
+      R[0] = c + wx * wx * q; R[1] = -wz;  R[2] = wx * wz * q;
+      R[3] = wz;              R[4] = c;    R[5] = -wx;
+      R[6] = wx * wz * q;     R[7] = wx;   R[8] = c + wz * wz * q;
+    } else {
+      for (int k = 0; k < 9; ++k) R[k] = 0.0;
+      R[0] = 1.0; R[4] = -1.0; R[8] = -1.0;
+    }
+    p.cost[P] = s.C;
+  }
+  p.iters[P] = s.evals;
+  p.status[P] = status;
+}
+
+// One warp per panorama: the members' sums at the candidate chained through D_k (lane-strided serial sums, then a shuffle tree:
+// a fixed order), then lane 0 runs fit_step_kernel's step on the 2 x 2 system, and the lanes write the members' next v_k.
+__global__ void __launch_bounds__(32 * kFitStepWarps) fit_pano_step_kernel(FitArgs a, FitPanos p) {
+  pdl_wait();
+  pdl_launch();
+  const int lane = threadIdx.x & 31;
+  const int P = blockIdx.x * kFitStepWarps + (threadIdx.x >> 5);
+  if (P >= p.npano) return;
+  FitPanoState& s = p.ps[P];
+  if (s.status != kFitRunning) return;
+  double gv[3], dg[3][2];
+  pano_gravity(s.cand, gv, dg);
+  double r[7] = {};   // 2 C, count, g[2], A[3]
+  for (int j = p.off[P] + lane; j < p.off[P + 1]; j += 32) {
+    const int i = p.mem[j];
+    const double* v = p.sums + (long long)i * kFitQ;
+    const double* M = p.rot + 9LL * i;
+    double D[3][2];
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+#pragma unroll
+      for (int k = 0; k < 2; ++k) D[c][k] = M[c] * dg[0][k] + M[3 + c] * dg[1][k] + M[6 + c] * dg[2][k];
+    const double Av[3][3] = {{v[5], v[6], v[7]}, {v[6], v[8], v[9]}, {v[7], v[9], v[10]}};
+    double AD[3][2];
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+#pragma unroll
+      for (int k = 0; k < 2; ++k) AD[c][k] = Av[c][0] * D[0][k] + Av[c][1] * D[1][k] + Av[c][2] * D[2][k];
+    r[0] += v[0];
+    r[1] += v[1];
+#pragma unroll
+    for (int k = 0; k < 2; ++k) r[2 + k] += D[0][k] * v[2] + D[1][k] * v[3] + D[2][k] * v[4];
+    r[4] += D[0][0] * AD[0][0] + D[1][0] * AD[1][0] + D[2][0] * AD[2][0];
+    r[5] += D[0][0] * AD[0][1] + D[1][0] * AD[1][1] + D[2][0] * AD[2][1];
+    r[6] += D[0][1] * AD[0][1] + D[1][1] * AD[1][1] + D[2][1] * AD[2][1];
+  }
+#pragma unroll
+  for (int q = 0; q < 7; ++q)
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) r[q] += __shfl_down_sync(0xffffffffu, r[q], o);
+  int status = kFitRunning;
+  double cand[2] = {0.0, 0.0};
+  if (lane == 0) {
+    status = [&]() -> int {
+      const double Cc = 0.5 * r[0];
+      s.evals += 1;
+      if (s.evals == 1) {   // the start
+        if (r[1] < 2.0 || r[4] == 0.0 || r[6] == 0.0) return 2;
+        s.C = Cc;
+        for (int k = 0; k < 2; ++k) { s.theta[k] = s.cand[k]; s.g[k] = r[2 + k]; }
+        for (int k = 0; k < 3; ++k) s.A[k] = r[4 + k];
+      } else if (Cc < s.C) {   // accept
+        const bool done = s.C - Cc <= kFitCostRtol * s.C;
+        s.C = Cc;
+        for (int k = 0; k < 2; ++k) { s.theta[k] = s.cand[k]; s.g[k] = r[2 + k]; }
+        for (int k = 0; k < 3; ++k) s.A[k] = r[4 + k];
+        s.lambda /= 10.0;
+        if (done) return 0;
+      } else {                 // reject: keep theta, A, g
+        s.lambda *= 10.0;
+        if (s.lambda > kFitLambdaMax) return 0;
+      }
+      double M[3], g[2] = {-s.g[0], -s.g[1]}, delta[2];
+      bool ok = false;
+      while (s.lambda <= kFitLambdaMax) {
+        M[0] = s.A[0] + s.lambda * s.A[0]; M[1] = s.A[1]; M[2] = s.A[2] + s.lambda * s.A[2];
+        if ((ok = cholesky_solve<2>(M, g, delta))) break;
+        s.lambda *= 10.0;
+      }
+      if (!ok) return 0;
+      if (fabs(delta[0]) <= kFitStepRtol * (1.0 + fabs(s.theta[0])) && fabs(delta[1]) <= kFitStepRtol * (1.0 + fabs(s.theta[1]))) return 0;
+      if (s.evals >= a.max_iter) return 1;
+      for (int k = 0; k < 2; ++k) s.cand[k] = s.theta[k] + delta[k];
+      return kFitRunning;
+    }();
+    if (status != kFitRunning) { pano_finish(p, P, s, status); s.status = status; }
+    cand[0] = s.cand[0]; cand[1] = s.cand[1];
+  }
+  status = __shfl_sync(0xffffffffu, status, 0);
+  cand[0] = __shfl_sync(0xffffffffu, cand[0], 0);
+  cand[1] = __shfl_sync(0xffffffffu, cand[1], 0);
+  pano_members(a, p, P, lane, cand, status);
 }
 
 }  // namespace pf

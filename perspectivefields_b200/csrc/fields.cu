@@ -595,6 +595,158 @@ int pf_fit_camera_groups_weighted(int device, const pf_fit_image* images, int n,
   return PF_OK;
 }
 
+// ----------------------------------------------------------------------------------------------- panorama levelling
+// Workspace layout of pf_fit_panorama: pf_fit_camera's | per-panorama state | per-view sums [n][kFitQ] | the panoramas' view
+// offsets [npano + 1] and views [n] | per-view A_k [n][9] and the starts [npano][2] (float64)
+static int fit_pano_layout(const pf_fit_image* im, int n, const int32_t* panorama_of, int npano, WsLayout* lay, long long* blocks_out = nullptr,
+                           std::vector<int>* csr = nullptr) {
+  const char* fn = "pf_fit_panorama";
+  TRY(fit_layout(fn, im, n, lay, blocks_out));
+  if (!panorama_of || npano < 1) return fail(PF_ERR_ARG, "%s: null panorama_of or npano < 1", fn);
+  std::vector<int> off(npano + 1, 0);
+  for (int i = 0; i < n; ++i) {
+    if (panorama_of[i] < 0 || panorama_of[i] >= npano)
+      return fail(PF_ERR_ARG, "%s: view %d has panorama %d outside 0 .. %d", fn, i, panorama_of[i], npano - 1);
+    off[panorama_of[i] + 1] += 1;
+  }
+  for (int P = 0; P < npano; ++P) {
+    if (off[P + 1] == 0) return fail(PF_ERR_ARG, "%s: panorama %d has no view", fn, P);
+    off[P + 1] += off[P];
+  }
+  lay->add((long long)npano * sizeof(FitPanoState)).add((long long)n * kFitQ * 8).add((long long)(npano + 1 + n) * 4)
+      .add((long long)(9 * n + 2 * npano) * 8);
+  if (csr) {
+    csr->assign(off.begin(), off.end());
+    csr->resize(npano + 1 + n);
+    for (int i = 0; i < n; ++i) (*csr)[npano + 1 + off[panorama_of[i]]++] = i;
+  }
+  return PF_OK;
+}
+int64_t pf_fit_panorama_workspace(const pf_fit_image* images, int n, const int32_t* panorama_of, int npano) {
+  WsLayout lay;
+  TRY(fit_pano_layout(images, n, panorama_of, npano, &lay));
+  return lay.total;
+}
+
+int pf_fit_panorama(int device, const pf_fit_image* images, const pf_pano_crop* crops, int n, const int32_t* panorama_of, int npano,
+                    const float* up_base, const float* lat_base, const uint8_t* mask_base, const float* weight_base,
+                    const int64_t* up_weight_offset, const int64_t* lat_weight_offset, const double* init, double huber, int max_iterations,
+                    double* angles, double* up, double* rotation, double* cost, int32_t* iterations, int32_t* status, void* workspace,
+                    int64_t workspace_bytes, void* stream) {
+  const char* fn = "pf_fit_panorama";
+  WsLayout lay;
+  long long blocks;
+  std::vector<int> csr;
+  TRY(fit_pano_layout(images, n, panorama_of, npano, &lay, &blocks, &csr));
+  if (!crops || !up || !rotation) return fail(PF_ERR_ARG, "%s: null crops / up / rotation", fn);
+  std::vector<pf_fit_image> ims(images, images + n);
+  for (auto& c : ims) c.init[0] = NAN;   // not read: the views' starts come from the panorama's
+  std::vector<FitImage> d;
+  FitArgs a;
+  bool weighted;
+  TRY(fit_prepare(fn, lay, blocks, ims.data(), n, up_base, lat_base, mask_base, weight_base, up_weight_offset, lat_weight_offset, 0, huber,
+                  max_iterations, angles, cost, iterations, status, workspace, workspace_bytes, &d, &a, &weighted));
+  std::vector<double> host(9 * (size_t)n + 2 * (size_t)npano, 0.0);
+  for (int i = 0; i < n; ++i) {
+    const pf_pano_crop& c = crops[i];
+    if (!std::isfinite(c.azimuth) || !std::isfinite(c.elevation) || !std::isfinite(c.roll))
+      return fail(PF_ERR_ARG, "%s: view %d: non-finite angle", fn, i);
+    if (!std::isfinite(c.vfov) || !(c.vfov > 0.0 && c.vfov < 180.0) || !std::isfinite(c.ar) || !(c.ar > 0.0))
+      return fail(PF_ERR_ARG, "%s: view %d: vfov %g must lie in (0, 180) and ar %g be finite and > 0", fn, i, c.vfov, c.ar);
+    const double fov_x = 2 * atan(tan(c.vfov * M_PI / 180.0 / 2) * c.ar) * 180 / M_PI;   // pf_equi_views' expressions
+    if (!(fov_x > 0.0 && fov_x < 180.0)) return fail(PF_ERR_ARG, "%s: view %d: fov_x %g must lie in (0, 180)", fn, i, fov_x);
+    d[i].init[2] = images[i].width / (2 * tan(fov_x * M_PI / 180 / 2));
+    d[i].init[3] = d[i].init[4] = 0.0;
+    const double roll = c.roll / 180 * M_PI, el = c.elevation / 180 * M_PI, az = c.azimuth / 180 * M_PI;
+    const double cr = cos(roll), sr = sin(roll), ce = cos(el), se = sin(el), ca = cos(az), sa = sin(az);
+    const double YX[9] = {ca, sa * se, sa * ce, 0.0, ce, -se, -sa, ca * se, ca * ce};   // Y(az) X(el)
+    const double Z[9] = {cr, -sr, 0.0, sr, cr, 0.0, 0.0, 0.0, 1.0};
+    for (int r = 0; r < 3; ++r)
+      for (int k = 0; k < 3; ++k) host[9 * i + 3 * r + k] = YX[3 * r] * Z[k] + YX[3 * r + 1] * Z[3 + k] + YX[3 * r + 2] * Z[6 + k];
+  }
+  for (int P = 0; init && P < npano; ++P) {
+    if (!std::isfinite(init[2 * P]) || !std::isfinite(init[2 * P + 1])) return fail(PF_ERR_ARG, "%s: panorama %d: non-finite init", fn, P);
+    host[9 * (size_t)n + 2 * P] = init[2 * P] * (M_PI / 180.0);
+    host[9 * (size_t)n + 2 * P + 1] = init[2 * P + 1] * (M_PI / 180.0);
+  }
+  CU(cudaSetDevice(device));
+  cudaStream_t st = (cudaStream_t)stream;
+  char* ws = (char*)workspace;
+  FitPanos p{};
+  p.ps = (FitPanoState*)(ws + lay.at[3]);
+  p.sums = (double*)(ws + lay.at[4]);
+  p.off = (const int*)(ws + lay.at[5]);
+  p.mem = p.off + npano + 1;
+  p.rot = (const double*)(ws + lay.at[6]);
+  p.init = p.rot + 9LL * n;
+  p.npano = npano;
+  p.angles = angles; p.up = up; p.R = rotation; p.cost = cost; p.iters = iterations; p.status = status;
+  FitGroups g{};
+  g.sums = p.sums;
+  TRY(upload_descriptors(d.data(), d.size() * sizeof(d[0]), ws, st));
+  CU(cudaMemcpyAsync(ws + lay.at[5], csr.data(), csr.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(ws + lay.at[6], host.data(), host.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+  const PdlScope pdl(!sync_debug());
+  const dim3 pass_grid((unsigned)blocks), reduce_grid((unsigned)cdiv(n, kFitStepWarps)), pano_grid((unsigned)cdiv(npano, kFitStepWarps));
+  auto pass = weighted ? fit_pass_kernel<3, true, true> : fit_pass_kernel<3, false, true>;
+  LAUNCHED(launch_pdl(fit_pano_init_kernel, pano_grid, dim3(32 * kFitStepWarps), 0, st, a, p));
+  for (int it = 0; it < max_iterations; ++it) {
+    LAUNCHED(launch_pdl(pass, pass_grid, dim3(kFitThreads), 0, st, a));
+    LAUNCHED(launch_pdl(fit_reduce_kernel<3>, reduce_grid, dim3(32 * kFitStepWarps), 0, st, a, g));
+    LAUNCHED(launch_pdl(fit_pano_step_kernel, pano_grid, dim3(32 * kFitStepWarps), 0, st, a, p));
+  }
+  return PF_OK;
+}
+
+// Workspace layout of pf_rotate_panoramas: device descriptors
+static int rotate_layout(const pf_rotate_pano* pn, int n, WsLayout* lay) {
+  if (!pn || n < 1) return fail(PF_ERR_ARG, "pf_rotate_panoramas: null panoramas or n < 1");
+  if (n > 65535) return fail(PF_ERR_ARG, "pf_rotate_panoramas: %d panoramas (at most 65535 per call)", n);
+  for (int i = 0; i < n; ++i)
+    if (pn[i].height < 2 || pn[i].width < 2 || (long long)pn[i].height * pn[i].width >= (1LL << 31))
+      return fail(PF_ERR_ARG, "pf_rotate_panoramas: panorama %d has size %dx%d (2x2 at least)", i, pn[i].height, pn[i].width);
+  lay->add((long long)n * sizeof(RotPano));
+  return PF_OK;
+}
+int64_t pf_rotate_panoramas_workspace(const pf_rotate_pano* panos, int n) {
+  WsLayout lay;
+  TRY(rotate_layout(panos, n, &lay));
+  return lay.total;
+}
+
+int pf_rotate_panoramas(int device, const pf_rotate_pano* panos, int n, int channels, int dtype, int mode, const void* in_base, void* out_base,
+                        float* map_base, const double* rotations, void* workspace, int64_t workspace_bytes, void* stream) {
+  const char* fn = "pf_rotate_panoramas";
+  WsLayout lay;
+  TRY(rotate_layout(panos, n, &lay));
+  if (!in_base || !out_base || !rotations || !workspace) return fail(PF_ERR_ARG, "%s: null input / output / rotations / workspace", fn);
+  if (channels != 1 && channels != 3) return fail(PF_ERR_ARG, "%s: %d channels (1 or 3)", fn, channels);
+  if (dtype != PF_EQUI_U8 && dtype != PF_EQUI_F32) return fail(PF_ERR_ARG, "%s: unknown dtype %d", fn, dtype);
+  if (mode != PF_EQUI_BILINEAR && mode != PF_EQUI_NEAREST) return fail(PF_ERR_ARG, "%s: unknown mode %d", fn, mode);
+  TRY(check_workspace(fn, workspace, workspace_bytes, lay.total));
+  std::vector<RotPano> d(n);
+  long long max_tiles = 1;
+  for (int i = 0; i < n; ++i) {
+    const pf_rotate_pano& c = panos[i];
+    TRY(check_offsets(fn, i, {c.in_offset, c.out_offset}, {{c.map_offset, map_base}}));
+    d[i] = RotPano{c.height, c.width, c.in_offset, c.out_offset, c.map_offset};
+    max_tiles = std::max(max_tiles, cdivl(c.height, kRotRows) * cdivl(c.width, kRotCols));
+  }
+  CU(cudaSetDevice(device));
+  cudaStream_t st = (cudaStream_t)stream;
+  TRY(upload_descriptors(d.data(), d.size() * sizeof(d[0]), workspace, st));
+  RotArgs a{};
+  a.pano = (const RotPano*)workspace; a.R = rotations;
+  a.in = in_base; a.out = out_base; a.map = map_base;
+  a.C = channels; a.nearest = mode == PF_EQUI_NEAREST;
+  const dim3 grid((unsigned)max_tiles, (unsigned)n);
+  if (dtype == PF_EQUI_F32)
+    LAUNCHED((rotate_panoramas_kernel<float><<<grid, kRotThreads, 0, st>>>(a), cudaGetLastError()));
+  else
+    LAUNCHED((rotate_panoramas_kernel<unsigned char><<<grid, kRotThreads, 0, st>>>(a), cudaGetLastError()));
+  return PF_OK;
+}
+
 // ----------------------------------------------------------------------------------------------- upright warp (rectify.cuh)
 // Workspace layout of pf_rectify_views: device descriptors | per-image maps
 static int rectify_layout(const pf_rectify_image* im, int n, WsLayout* lay) {

@@ -4,6 +4,8 @@
 vertical: this project's rule, DESIGN.md section 1 "Upright warp".  It takes the camera parameters every ParamNet variant's
 ``inference_batch`` results carry, or ``calibrate.fit_camera``'s output, straight from the device without synchronising, and
 returns images that ``PerspectiveFields.inference_batch`` accepts, with the output camera in a centred ParamNet variant's keys.
+``rotate_panoramas`` rotates equirectangular panoramas, and ``level_panoramas`` levels tilted ones from a model's predictions
+on their crops (DESIGN.md section 1, "Panorama levelling").
 """
 import ctypes
 import math
@@ -224,3 +226,165 @@ def upright(images, cameras, keep_pitch=False, focal="same", size=None, mode="bi
     res["camera"] = [dict(zip(OUTPUT_KEYS, c.unbind(0))) for c in cols_out]
     res["status"] = status
     return res
+
+
+PANO_MODES = {"bilinear": _native.PF_EQUI_BILINEAR, "nearest": _native.PF_EQUI_NEAREST}
+_PANO_DTYPES = {torch.uint8: _native.PF_EQUI_U8, torch.float32: _native.PF_EQUI_F32}
+ORTHONORMAL_TOL = 1e-9
+DEFAULT_LEVEL_VIEWS = tuple((70.0, 320, 320, float(az), 0.0, 0.0, 1.0) for az in range(0, 360, 45))
+
+
+def _check_panoramas(panos):
+    """-> (list of panoramas, torch dtype, channels, device or None for host arrays); no GPU work."""
+    if isinstance(panos, (torch.Tensor, np.ndarray)):
+        raise TypeError("panos must be a list of [Hp, Wp, 3] or [Hp, Wp] panoramas, not one array")
+    panos = list(panos)
+    if not panos:
+        raise ValueError("no panoramas")
+    on_dev = [isinstance(p, torch.Tensor) and p.is_cuda for p in panos]
+    if any(on_dev) and not all(on_dev):
+        raise TypeError("the list mixes CUDA tensors and host panoramas; pass one kind per call")
+    out, kinds = [], set()
+    for i, p in enumerate(panos):
+        if not on_dev[i]:
+            if isinstance(p, torch.Tensor):
+                raise TypeError(f"panos[{i}] is a CPU tensor: pass a numpy array or a CUDA tensor")
+            p = torch.from_numpy(np.ascontiguousarray(p))
+        if p.dtype not in _PANO_DTYPES:
+            raise TypeError(f"panos[{i}] must be uint8 or float32, got {p.dtype}")
+        if p.dim() not in (2, 3) or (p.dim() == 3 and p.shape[2] != 3):
+            raise TypeError(f"panos[{i}] must be [Hp, Wp, 3] or [Hp, Wp], got {list(p.shape)}")
+        if p.shape[0] < 2 or p.shape[1] < 2 or p.shape[0] * p.shape[1] >= 1 << 31:
+            raise ValueError(f"panos[{i}] has size {p.shape[0]} x {p.shape[1]} (2 x 2 at least)")
+        kinds.add((p.dtype, 1 if p.dim() == 2 else 3))
+        out.append(p)
+    if len(kinds) != 1:
+        raise TypeError("the panoramas mix dtypes or channel counts; pass one kind per call")
+    dev = out[0].device if on_dev[0] else None
+    if dev is not None and any(p.device != dev for p in out):
+        raise ValueError("the panoramas are on more than one CUDA device")
+    dtype, channels = kinds.pop()
+    return out, dtype, channels, dev
+
+
+def _rotations(rotations, n, dev):
+    """-> (CUDA float64 [n, 3, 3] tensors to stack or host arrays, device or None).  CUDA tensors are read as they are (no check, no
+    synchronisation); host rotations must be orthonormal with determinant +1 to ORTHONORMAL_TOL."""
+    if isinstance(rotations, torch.Tensor) and rotations.is_cuda:
+        if rotations.dtype != torch.float64 or tuple(rotations.shape) != (n, 3, 3):
+            raise ValueError(f"rotations as one CUDA tensor must be float64 [{n}, 3, 3], got {rotations.dtype} {list(rotations.shape)}")
+        return list(rotations.unbind(0)), rotations.device
+    rots = list(rotations)
+    if len(rots) != n:
+        raise ValueError(f"{n} panoramas but {len(rots)} rotations")
+    out, devs = [], set()
+    for i, r in enumerate(rots):
+        if isinstance(r, torch.Tensor) and r.is_cuda:
+            if r.dtype != torch.float64 or tuple(r.shape) != (3, 3):
+                raise ValueError(f"rotations[{i}] must be a float64 [3, 3] tensor, got {r.dtype} {list(r.shape)}")
+            devs.add(r.device)
+            out.append(r)
+            continue
+        m = np.asarray(r.numpy() if isinstance(r, torch.Tensor) else r, dtype=np.float64)
+        if m.shape != (3, 3) or not np.all(np.isfinite(m)):
+            raise ValueError(f"rotations[{i}] must be a finite 3 x 3 matrix, got shape {m.shape}")
+        if np.max(np.abs(m @ m.T - np.eye(3))) > ORTHONORMAL_TOL or abs(np.linalg.det(m) - 1.0) > ORTHONORMAL_TOL:
+            raise ValueError(f"rotations[{i}] is not a rotation (orthonormal with determinant 1 to {ORTHONORMAL_TOL})")
+        out.append(m)
+    if len(devs) > 1 or (dev is not None and devs and devs != {dev}):
+        raise ValueError("the rotations are on another CUDA device than the panoramas")
+    return out, (devs.pop() if devs else None)
+
+
+def rotate_panoramas(panos, rotations, mode="bilinear", outputs=()):
+    """Rotate equirectangular panoramas on the GPU: ``out(d) = P(R d)`` for every direction d (DESIGN.md section 1, "Panorama
+    levelling"), so ``rotate_panoramas(P, [fit["rotation"]])`` with ``calibrate.fit_panorama``'s output levels P.  One launch for
+    the whole list; sizes may differ.
+
+    - ``panos``: a list of uint8 or float32 [Hp, Wp, 3] or [Hp, Wp] panoramas (one dtype and channel count per call), CUDA
+      tensors read in place or numpy arrays uploaded once.  Pixel (i, j) is the direction at longitude 2 pi j / Wp - pi and
+      latitude pi/2 - pi i / Hp (x right, y down, z at longitude 0), so row 0 is the pole and only rows 1 .. Hp - 1 of a
+      panorama survive the identity unchanged.
+    - ``rotations``: one 3 x 3 matrix per panorama, as a CUDA float64 [n, 3, 3] tensor or a list of CUDA float64 [3, 3] tensors
+      (read on the device: not checked, no synchronisation) or of host arrays (checked to be rotations to 1e-9).
+    - ``mode``: "bilinear" (columns wrap, rows clamp, float64 weights; uint8 rounded to nearest) or "nearest".
+    - ``outputs``: () or ("map",): also a float32 [Hp, Wp, 2] map of the input position (u, v) each output pixel samples.
+
+    Returns a dict: ``im`` (list of CUDA views into one 16-byte-aligned blob, in the input dtype) and ``map`` if asked for.
+    Nothing synchronises with the device; invalid arguments raise before any GPU work."""
+    if mode not in PANO_MODES:
+        raise ValueError(f"mode must be one of {tuple(PANO_MODES)}, got {mode!r}")
+    outputs = (outputs,) if isinstance(outputs, str) else tuple(outputs)
+    bad = [o for o in outputs if o != "map"]
+    if bad:
+        raise ValueError(f"unknown outputs {bad}; choose from ('map',)")
+    src, dtype, channels, dev = _check_panoramas(panos)
+    n = len(src)
+    if n > 65535:
+        raise ValueError(f"{n} panoramas: at most 65535 per call")
+    rots, rdev = _rotations(rotations, n, dev)
+    dev = _batch.device(__name__, src[:1] + [r for r in rots if isinstance(r, torch.Tensor)][:1])
+    if rdev is not None and rdev != dev:
+        raise ValueError(f"the rotations are on {rdev}, the panoramas on {dev}")
+    L = _native.lib()
+    esize = 4 if dtype == torch.float32 else 1
+    shapes = [tuple(p.shape) for p in src]
+    out_offs, out_total = _batch.layout([math.prod(s) for s in shapes], 16 // esize)
+    map_offs, map_total = _batch.layout([2 * s[0] * s[1] for s in shapes], 4) if "map" in outputs else ([-1] * n, 0)
+    descs = (_native.pf_rotate_pano * n)()
+    with torch.cuda.device(dev):
+        if src[0].is_cuda:
+            src = [p.contiguous() for p in src]
+        else:
+            src = _batch.upload([p.numpy() for p in src], dtype, dev)
+        base = _batch.base(src)
+        for i, p in enumerate(src):
+            descs[i] = _native.pf_rotate_pano(shapes[i][0], shapes[i][1], _batch.offset(p, base), out_offs[i], map_offs[i])
+        host = [r for r in rots if not isinstance(r, torch.Tensor)]
+        up = iter(_batch.upload(host, torch.float64, dev)) if host else iter(())
+        R = torch.stack([r if isinstance(r, torch.Tensor) else next(up) for r in rots]).contiguous()
+        ws = _batch.workspace(L.pf_rotate_panoramas_workspace(descs, n), dev)
+        blob = torch.empty(out_total, dtype=dtype, device=dev)
+        xblob = torch.empty(map_total, dtype=torch.float32, device=dev) if "map" in outputs else None
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        _native.check(L.pf_rotate_panoramas(dev.index, descs, n, channels, _PANO_DTYPES[dtype], PANO_MODES[mode], base, blob.data_ptr(),
+                                            xblob.data_ptr() if xblob is not None else None, R.data_ptr(), ws.data_ptr(), ws.numel(),
+                                            stream))
+    res = {"im": _batch.views(blob, out_offs, shapes)}
+    if xblob is not None:
+        res["map"] = _batch.views(xblob, map_offs, [(s[0], s[1], 2) for s in shapes])
+    return res
+
+
+def level_panoramas(model, panos, views=None, mode="bilinear", weights=None, huber=None):
+    """Level tilted 360-degree panoramas with a Perspective Fields model, on the GPU from end to end: for each panorama,
+    ``panocam.crop_equi_views`` crops ``views``, ``model.inference_batch`` predicts their fields (one batch for all panoramas),
+    ``calibrate.fit_panorama`` fits each panorama's tilt to them, and ``rotate_panoramas`` rotates each panorama upright.
+
+    - ``panos``: a list of uint8 [Hp, Wp, 3] panoramas (CUDA tensors or numpy arrays) in the channel order the model's
+      ``inference_batch`` takes; the crops keep it.
+    - ``views``: the crops of every panorama, ``crop_equi_views``' ``(vfov, im_w, im_h, azimuth, elevation, roll, ar)`` tuples or
+      dicts; by default ``DEFAULT_LEVEL_VIEWS``, 8 crops of 320 x 320 at azimuth 0, 45, ..., 315 degrees, elevation 0, roll 0,
+      vfov 70 degrees, ar 1.  Which view set levels real panoramas best has not been measured, nor has the accuracy of the
+      levelling on real tilted panoramas.
+    - ``mode``: the sampler of the rotation; ``weights`` ("confidence" needs a model built with ``confidence=True``) and
+      ``huber``: as in ``calibrate.fit_panorama``.
+
+    Returns a dict: ``im`` (the levelled panoramas, ``rotate_panoramas``' output) and ``fits`` (``fit_panorama``'s dicts).
+    The fields the model predicts for a crop are its own: no ground truth is used."""
+    views = list(DEFAULT_LEVEL_VIEWS if views is None else views)
+    if not views:
+        raise ValueError("no views")
+    src, dtype, channels, dev = _check_panoramas(panos)
+    if dtype != torch.uint8 or channels != 3:
+        raise TypeError("level_panoramas needs uint8 [Hp, Wp, 3] panoramas (the model's input)")
+    from . import calibrate, panocam
+    if dev is None:   # host panoramas: uploaded once, for the crops and the rotation
+        dev = _batch.device(__name__)
+        src = [p.to(dev) for p in src]
+    crops = [c for p in src for c in panocam.crop_equi_views(p, views, outputs=())["im"]]
+    results = model.inference_batch(crops)
+    nv = len(views)
+    fits = calibrate.fit_panorama(results, views * len(src), [P for P in range(len(src)) for _ in range(nv)], weights=weights, huber=huber)
+    levelled = rotate_panoramas(src, [f["rotation"] for f in fits], mode)
+    return {"im": levelled["im"], "fits": fits}
