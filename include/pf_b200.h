@@ -164,6 +164,12 @@ int pf_profile_kernels_read(pf_handle h, char* buf, int cap);
  * "decode_only" (default 0; classification heads, SURVEY.md 8f-3): the 73 / 180 logits are never written -- the 1x1 prediction
  *   conv, argmax and bin decode (gravity_head.py:243-244 + utils/utils.py:114-130, latitude_head.py:205-208 + utils.py:148-162)
  *   run in one kernel and pred_gravity / pred_latitude receive the decoded fields [n,2,320,320] / [n,1,320,320] (degrees).
+ * "subbin" (default 0; classification heads only, PF_ERR_ARG on a model with regression heads, which is left as it was; NOT the
+ *   reference's decode, DESIGN.md section 1 "Sub-bin decode"): the argmax bin c of each head is refined to c + delta, delta in
+ *   [-1/2, 1/2] the vertex of the parabola through the logits of c and its two neighbours (the 72 up-direction bins as a circle;
+ *   no refinement in the no-direction bin and the two latitude pole bins), and decoded with the same formulas.  It changes the
+ *   decoded fields only -- pred_gravity / pred_latitude under "decode_only", the *_original fields -- in either "decode_only"
+ *   setting and with or without pf_forward_confidence; logits and confidence maps are unchanged.
  * "bf16" (default 0; NOT the reference's numerics, DESIGN.md section 3): every tensor-core product -- the TMA -> wgmma engine's
  *   GEMMs and 3x3 convolutions, the 7x7 stems and both products of the mma.sync attention core -- is one bf16 MMA of the
  *   operands' hi planes (bf16-rounded operands, fp32 accumulation) instead of the three of the split-precision scheme.  The
@@ -609,6 +615,13 @@ int pf_op_argmax_decode(const float* logits, float* field, int B, int HW, int NC
 /* the same decode WITHOUT materialised logits (option "decode_only"): 1x1 conv 32 -> NC on feat [B*HW, ld] (channels coff..coff+31,
  * weights [NC][32], bias [NC]) + argmax + bin decode in one kernel; logits bit-identical to the separate 1x1 conv kernel. */
 int pf_op_pred_argmax_decode(const float* feat, int ld, int coff, const float* w, const float* bias, float* field, int B, int HW, int NC,
+                             int is_gravity, void* stream);
+/* the two decodes above with the sub-bin refinement of option "subbin" (DESIGN.md section 1, "Sub-bin decode"); the argmax is
+ * theirs.  conf: NULL, or DEVICE float32 [B, HW] (4-byte aligned) that also receives the head confidence (pf_confidence), bit-identical
+ * to the confidence the unrefined kernels compute.  The fused form's neighbour logits come from the same fma chain as its argmax's,
+ * so on logits written by the separate 1x1 conv kernel both entry points give the same field bit for bit. */
+int pf_op_subbin_decode(const float* logits, float* field, float* conf, int B, int HW, int NC, int is_gravity, void* stream);
+int pf_op_pred_subbin_decode(const float* feat, int ld, int coff, const float* w, const float* bias, float* field, float* conf, int B, int HW, int NC,
                              int is_gravity, void* stream);
 /* resample of decoded fields to the original sizes (gravity_head.py:246-256, latitude_head.py:209-219, utils/utils.py:483-507):
  * vec [n,2,320,320], lat [n,1,320,320] -> blobs as in pf_batch; lat_is_sin: lat holds sin(latitude) (regression head). */

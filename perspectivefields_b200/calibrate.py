@@ -84,6 +84,9 @@ def fit_camera(results, principal_point=False, init="fields", mask=None, huber=N
       section 1, "Camera fit").  All-ones weights give the unweighted fit and 0 / 1 weights the fit
       under the matching ``mask``, bit for bit.  Checked on the host, no synchronisation.
 
+    The fields of a model built with ``decode="subbin"`` (continuous, DESIGN.md section 1 "Sub-bin decode") are read as they are:
+    nothing here changes for them.
+
     Returns one dict per image, as 0-dim float64 CUDA tensors in degrees: the keys of a centred (``principal_point=False``:
     ``pred_roll, pred_pitch, pred_vfov, pred_rel_focal, pred_general_vfov, pred_rel_cx, pred_rel_cy``) or uncentred ParamNet
     variant (``pred_roll, pred_pitch, pred_general_vfov, pred_rel_cx, pred_rel_cy, pred_rel_focal``), plus ``fit_cost`` (the

@@ -65,6 +65,7 @@ struct pf_engine {
   const float *conv1f_w, *conv1f_b;   // plain fp32 conv_fuse_conv1 [head][tap][ci][o] / bias, for the border-ring kernel
   bool use_pdl = true;                // option "pdl": programmatic dependent launch of the graph's kernels (common.cuh)
   bool decode_only = false;           // option "decode_only": classification heads return decoded fields, logits are never written
+  bool subbin = false;                // option "subbin": classification heads decode their argmax bin to a sub-bin position
   const float *pred_g_w, *pred_g_b, *pred_l_w, *pred_l_b;
   const float *pn_stem_w, *pn_stem_b;
   LnW pn_stem_ln, pn_ds_ln[4], pn_norm;

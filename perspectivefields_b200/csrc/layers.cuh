@@ -691,9 +691,42 @@ __device__ __forceinline__ void decode_bin_store(float* __restrict__ field, int 
   }
 }
 
+// Sub-bin decode (DESIGN.md section 1, "Sub-bin decode"): the argmax bin bi moved to p = bi + delta, delta in [-1/2, 1/2] the
+// vertex of the parabola through l0 = l(bi) and the logits lm / lp of its two neighbours, then decode_bin_store's formulas at p.
+// subbin_neighbours gives the neighbours' classes: the up head's direction bins 0 .. NC-2 form a circle (bin NC-1, no direction,
+// is never a neighbour and is not refined); the latitude head's are bi -+ 1, clamped, and its two pole bins are not refined.
+// Unrefined bins return bi itself, so every class read is in range.  delta = 0 gives decode_bin_store's value bit for bit.
+__device__ __forceinline__ int2 subbin_neighbours(int NC, int bi, int is_gravity) {
+  if (!is_gravity) return make_int2(max(bi - 1, 0), min(bi + 1, NC - 1));
+  if (bi >= NC - 1) return make_int2(bi, bi);
+  return make_int2(bi == 0 ? NC - 2 : bi - 1, bi == NC - 2 ? 0 : bi + 1);
+}
+__device__ __forceinline__ void subbin_decode_store(float* __restrict__ field, int b, int r, int HW, int NC, int bi, float l0, float lm, float lp,
+                                                    int is_gravity) {
+  // a, b >= 0 for a true maximum; non-finite logits (and a flat top, a + b = 0) give delta = 0.  The products and sums below are
+  // rounded one at a time, as the fp32 oracle evaluates them (no fma contraction).
+  const float da = l0 - lm, db = l0 - lp, s = da + db;
+  float delta = (isfinite(da) && isfinite(db) && s > 0.0f) ? __fdiv_rn(da - db, 2.0f * s) : 0.0f;
+  if (!is_gravity && (bi == 0 || bi == NC - 1)) delta = 0.0f;
+  const float p = (float)bi + delta;
+  if (is_gravity) {
+    float* o = field + (long long)b * 2 * HW + r;
+    if (bi == NC - 1) { o[0] = 0.f; o[HW] = 0.f; }
+    else {
+      const float ang = __fmul_rn(__fdiv_rn(__fsub_rn(__fmul_rn(p, gravity_bin_deg(NC)), 180.0f), 180.0f), 3.14159265358979323846f);
+      o[0] = cosf(ang); o[HW] = sinf(ang);
+    }
+  } else {
+    const float bin = latitude_bin_deg(NC);
+    field[(long long)b * HW + r] = __fadd_rn(__fadd_rn(-90.0f, __fmul_rn(p, bin)), bin * 0.5f);
+  }
+}
+
 // Classification variant: argmax over channels + bin decode (gravity_head.py:243-244 + utils.py:114-130;
 // latitude_head.py:205-208 + utils.py:148-162).  logits NCHW [B, NC, HW] -> field [B, 2 or 1, HW].
 // torch.argmax returns the FIRST maximal index; strict '>' reproduces that.
+// kRefine: the sub-bin decode instead, reading the winner's two neighbour planes after the pass.
+template <bool kRefine>
 __global__ void __launch_bounds__(256) argmax_decode_kernel(const float* __restrict__ logits, float* __restrict__ field, int B, int HW, int NC, int is_gravity) {
   const long long pix = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (pix >= (long long)B * HW) return;
@@ -705,7 +738,12 @@ __global__ void __launch_bounds__(256) argmax_decode_kernel(const float* __restr
     const float v = __ldg(lp + (long long)c * HW);
     if (v > best) { best = v; bi = c; }
   }
-  decode_bin_store(field, b, r, HW, NC, bi, is_gravity);
+  if constexpr (kRefine) {
+    const int2 nb = subbin_neighbours(NC, bi, is_gravity);
+    subbin_decode_store(field, b, r, HW, NC, bi, best, __ldg(lp + (long long)nb.x * HW), __ldg(lp + (long long)nb.y * HW), is_gravity);
+  } else {
+    decode_bin_store(field, b, r, HW, NC, bi, is_gravity);
+  }
 }
 
 // Head confidence (DESIGN.md section 1): conf = max_c softmax(l)_c = 1 / sum_c exp(l_c - l_max) in fp32 over all NC classes.
@@ -715,6 +753,8 @@ __device__ __forceinline__ void conf_update(float v, float& m, float& s) {
   else s += expf(v - m);
 }
 // argmax_decode_kernel plus the confidence, in one pass over the logits (the logits are read once).  conf: [B, HW].
+// kRefine: as argmax_decode_kernel's; conf does not depend on it.
+template <bool kRefine>
 __global__ void __launch_bounds__(256) argmax_conf_decode_kernel(const float* __restrict__ logits, float* __restrict__ field, float* __restrict__ conf,
                                                                  int B, int HW, int NC, int is_gravity) {
   const long long pix = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -729,7 +769,12 @@ __global__ void __launch_bounds__(256) argmax_conf_decode_kernel(const float* __
     else s += expf(v - best);
   }
   conf[pix] = 1.0f / s;
-  decode_bin_store(field, b, r, HW, NC, bi, is_gravity);
+  if constexpr (kRefine) {
+    const int2 nb = subbin_neighbours(NC, bi, is_gravity);
+    subbin_decode_store(field, b, r, HW, NC, bi, best, __ldg(lp + (long long)nb.x * HW), __ldg(lp + (long long)nb.y * HW), is_gravity);
+  } else {
+    decode_bin_store(field, b, r, HW, NC, bi, is_gravity);
+  }
 }
 
 // Classification heads WITHOUT the logits (SURVEY.md 8f-3, option "decode_only"): 1x1 prediction conv 32 -> NC
@@ -742,7 +787,10 @@ __global__ void __launch_bounds__(256) argmax_conf_decode_kernel(const float* __
 // (the four lanes of a quad read four different rows with 16-byte loads: no bank conflict).
 // kConf: also the head confidence into conf [B, HW]: each lane keeps a running (max, sum) over its classes (conf_update), and the
 // quad merges the pairs with the same two shuffles, s = s1 exp(m1 - m) + s2 exp(m2 - m).  kConf = false does not read conf.
-template <bool kConf>
+// kRefine: the sub-bin decode.  The two neighbour logits are recomputed from f[] with the same fma chain (bit-identical to the
+// logits the separate path reads): lanes q = 0, 2 evaluate the lower neighbour, q = 1, 3 the upper one, and lane 0, which stores,
+// takes the upper one from lane 1.  The winner is lane 0's, broadcast to the quad (with NaN logits the lanes' winners can differ).
+template <bool kConf, bool kRefine>
 __global__ void __launch_bounds__(256) pred_argmax_decode_kernel(const float* __restrict__ in, int ldi, int icoff, const float* __restrict__ w,
                                                                  const float* __restrict__ bias, float* __restrict__ field, int B, int HW, int NC,
                                                                  int is_gravity, float* __restrict__ conf) {
@@ -792,8 +840,22 @@ __global__ void __launch_bounds__(256) pred_argmax_decode_kernel(const float* __
         cm = m;
       }
     }
+    float lm = 0.0f, lp = 0.0f;
+    if constexpr (kRefine) {
+      const int2 nb = subbin_neighbours(NC, __shfl_sync(0xffffffffu, bi, 0, 4), is_gravity);
+      const float4* wr = reinterpret_cast<const float4*>(s_pw + ((q & 1) ? nb.y : nb.x) * 36);
+      float v = s_b[(q & 1) ? nb.y : nb.x];
+#pragma unroll
+      for (int d4 = 0; d4 < 8; ++d4) {
+        const float4 ww = wr[d4];
+        v = fmaf(f[4 * d4], ww.x, v); v = fmaf(f[4 * d4 + 1], ww.y, v); v = fmaf(f[4 * d4 + 2], ww.z, v); v = fmaf(f[4 * d4 + 3], ww.w, v);
+      }
+      lm = v;
+      lp = __shfl_xor_sync(0xffffffffu, v, 1);
+    }
     if (live && q == 0) {
-      decode_bin_store(field, (int)(pix / HW), (int)(pix % HW), HW, NC, bi, is_gravity);
+      if constexpr (kRefine) subbin_decode_store(field, (int)(pix / HW), (int)(pix % HW), HW, NC, bi, best, lm, lp, is_gravity);
+      else decode_bin_store(field, (int)(pix / HW), (int)(pix % HW), HW, NC, bi, is_gravity);
       if constexpr (kConf) conf[pix] = 1.0f / cs;
     }
   }

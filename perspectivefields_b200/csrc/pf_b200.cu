@@ -384,6 +384,7 @@ static int launch_postprocess(const float* vec, const float* lat, int n, int SH,
 // prediction 1x1 convs (+ normalise / clamp) -> NCHW outputs, then argmax decode (classification) and resample to the
 // original resolutions.  conv1_out: [n,NH,NW,64] fp32 (gravity head channels 0-31, latitude head 32-63).  cf (classification
 // heads only, else NULL): the decode kernels also write the head confidence, resampled to the original sizes after the fields.
+// Option "subbin" selects the decode kernels' sub-bin instantiations; nothing else changes.
 static int fwd_tails_post(Fwd& F, const pf_batch* bt, const pf_confidence* cf, const float* conv1_out, PostImage* d_post, bool pred_done = false) {
   pf_engine* e = F.e;
   const pf_model_desc& D = e->desc;
@@ -410,17 +411,12 @@ static int fwd_tails_post(Fwd& F, const pf_batch* bt, const pf_confidence* cf, c
     // option "decode_only": 1x1 conv + argmax + bin decode in one kernel; pred_gravity / pred_latitude hold the decoded fields
     if (!dry) {
       const unsigned grid = ew_grid((long long)n * HW * 4);
-      if (cf) {
-        LAUNCHED((pred_argmax_decode_kernel<true><<<grid, 256, D.gravity_classes * 37 * 4, st>>>(conv1_out, 64, 0, e->pred_g_w, e->pred_g_b, bt->pred_gravity,
-                                                                                              n, HW, D.gravity_classes, 1, cf->gravity), cudaGetLastError()));
-        LAUNCHED((pred_argmax_decode_kernel<true><<<grid, 256, D.latitude_classes * 37 * 4, st>>>(conv1_out, 64, 32, e->pred_l_w, e->pred_l_b, bt->pred_latitude,
-                                                                                               n, HW, D.latitude_classes, 0, cf->latitude), cudaGetLastError()));
-      } else {
-        LAUNCHED((pred_argmax_decode_kernel<false><<<grid, 256, D.gravity_classes * 37 * 4, st>>>(conv1_out, 64, 0, e->pred_g_w, e->pred_g_b, bt->pred_gravity,
-                                                                                               n, HW, D.gravity_classes, 1, nullptr), cudaGetLastError()));
-        LAUNCHED((pred_argmax_decode_kernel<false><<<grid, 256, D.latitude_classes * 37 * 4, st>>>(conv1_out, 64, 32, e->pred_l_w, e->pred_l_b, bt->pred_latitude,
-                                                                                                n, HW, D.latitude_classes, 0, nullptr), cudaGetLastError()));
-      }
+      const auto kern = cf ? (e->subbin ? pred_argmax_decode_kernel<true, true> : pred_argmax_decode_kernel<true, false>)
+                           : (e->subbin ? pred_argmax_decode_kernel<false, true> : pred_argmax_decode_kernel<false, false>);
+      LAUNCHED((kern<<<grid, 256, D.gravity_classes * 37 * 4, st>>>(conv1_out, 64, 0, e->pred_g_w, e->pred_g_b, bt->pred_gravity, n, HW, D.gravity_classes, 1,
+                                                                   cf ? cf->gravity : nullptr), cudaGetLastError()));
+      LAUNCHED((kern<<<grid, 256, D.latitude_classes * 37 * 4, st>>>(conv1_out, 64, 32, e->pred_l_w, e->pred_l_b, bt->pred_latitude, n, HW, D.latitude_classes,
+                                                                    0, cf ? cf->latitude : nullptr), cudaGetLastError()));
     }
   } else {
     // prediction tails -> NCHW outputs (returned to the caller)
@@ -428,20 +424,20 @@ static int fwd_tails_post(Fwd& F, const pf_batch* bt, const pf_confidence* cf, c
       TRY(F.pred_tail(conv1_out, 64, 0, e->pred_g_w, e->pred_g_b, dry ? nullptr : bt->pred_gravity, HW, D.gravity_classes, D.gravity_classes == 2 ? 1 : 0));
       TRY(F.pred_tail(conv1_out, 64, 32, e->pred_l_w, e->pred_l_b, dry ? nullptr : bt->pred_latitude, HW, D.latitude_classes, D.latitude_classes == 1 ? 2 : 0));
     }
+    const auto dec = e->subbin ? argmax_decode_kernel<true> : argmax_decode_kernel<false>;
+    const auto dec_conf = e->subbin ? argmax_conf_decode_kernel<true> : argmax_conf_decode_kernel<false>;
     if (cls_g) {
       float* dv = ar.f((long long)n * 2 * HW);
       if (!dry && cf)
-        LAUNCHED((argmax_conf_decode_kernel<<<(unsigned)cdivl((long long)n * HW, 256), 256, 0, st>>>(bt->pred_gravity, dv, cf->gravity, n, HW, D.gravity_classes, 1),
-                  cudaGetLastError()));
-      else if (!dry) LAUNCHED((argmax_decode_kernel<<<(unsigned)cdivl((long long)n * HW, 256), 256, 0, st>>>(bt->pred_gravity, dv, n, HW, D.gravity_classes, 1), cudaGetLastError()));
+        LAUNCHED((dec_conf<<<(unsigned)cdivl((long long)n * HW, 256), 256, 0, st>>>(bt->pred_gravity, dv, cf->gravity, n, HW, D.gravity_classes, 1), cudaGetLastError()));
+      else if (!dry) LAUNCHED((dec<<<(unsigned)cdivl((long long)n * HW, 256), 256, 0, st>>>(bt->pred_gravity, dv, n, HW, D.gravity_classes, 1), cudaGetLastError()));
       vec = dv;
     }
     if (cls_l) {
       float* dl = ar.f((long long)n * HW);
       if (!dry && cf)
-        LAUNCHED((argmax_conf_decode_kernel<<<(unsigned)cdivl((long long)n * HW, 256), 256, 0, st>>>(bt->pred_latitude, dl, cf->latitude, n, HW, D.latitude_classes, 0),
-                  cudaGetLastError()));
-      else if (!dry) LAUNCHED((argmax_decode_kernel<<<(unsigned)cdivl((long long)n * HW, 256), 256, 0, st>>>(bt->pred_latitude, dl, n, HW, D.latitude_classes, 0), cudaGetLastError()));
+        LAUNCHED((dec_conf<<<(unsigned)cdivl((long long)n * HW, 256), 256, 0, st>>>(bt->pred_latitude, dl, cf->latitude, n, HW, D.latitude_classes, 0), cudaGetLastError()));
+      else if (!dry) LAUNCHED((dec<<<(unsigned)cdivl((long long)n * HW, 256), 256, 0, st>>>(bt->pred_latitude, dl, n, HW, D.latitude_classes, 0), cudaGetLastError()));
       lat = dl;
     }
   }
@@ -955,6 +951,13 @@ int pf_profile_kernels_read(pf_handle h, char* buf, int cap) {
 int pf_set_option(pf_handle h, const char* name, int value) {
   if (!h || !name) return fail(PF_ERR_ARG, "pf_set_option: null argument");
   if (!strcmp(name, "decode_only")) { h->decode_only = value != 0; return PF_OK; }
+  if (!strcmp(name, "subbin")) {
+    if (value && (h->desc.gravity_classes == 2 || h->desc.latitude_classes == 1))
+      return fail(PF_ERR_ARG, "pf_set_option: \"subbin\" needs classification heads (this model has %d / %d classes)", h->desc.gravity_classes,
+                  h->desc.latitude_classes);
+    h->subbin = value != 0;
+    return PF_OK;
+  }
   if (!strcmp(name, "pdl")) { h->use_pdl = value != 0; return PF_OK; }
   if (!strcmp(name, "bf16")) { h->bf16 = value != 0; return PF_OK; }
   return fail(PF_ERR_ARG, "pf_set_option: unknown option '%s'", name);
@@ -1176,14 +1179,32 @@ int pf_op_resize_f32(const float* img, int H, int W, int C, int new_h, int new_w
 }
 int pf_op_argmax_decode(const float* logits, float* field, int B, int HW, int NC, int is_gravity, void* stream) {
   if (!logits || !field || B < 1 || HW < 1 || NC < 1) return fail(PF_ERR_ARG, "pf_op_argmax_decode: bad argument");
-  LAUNCHED((argmax_decode_kernel<<<(unsigned)cdivl((long long)B * HW, 256), 256, 0, (cudaStream_t)stream>>>(logits, field, B, HW, NC, is_gravity), cudaGetLastError()));
+  LAUNCHED((argmax_decode_kernel<false><<<(unsigned)cdivl((long long)B * HW, 256), 256, 0, (cudaStream_t)stream>>>(logits, field, B, HW, NC, is_gravity), cudaGetLastError()));
   return PF_OK;
 }
 int pf_op_pred_argmax_decode(const float* feat, int ld, int coff, const float* w, const float* bias, float* field, int B, int HW, int NC, int is_gravity,
                              void* stream) {
   if (!feat || !w || !bias || !field || B < 1 || HW < 1 || NC < 1 || NC > 256 || (ld & 3) || (coff & 3)) return fail(PF_ERR_ARG, "pf_op_pred_argmax_decode: bad argument");
-  LAUNCHED((pred_argmax_decode_kernel<false><<<ew_grid((long long)B * HW * 4), 256, NC * 37 * 4, (cudaStream_t)stream>>>(feat, ld, coff, w, bias, field, B, HW, NC,
+  LAUNCHED((pred_argmax_decode_kernel<false, false><<<ew_grid((long long)B * HW * 4), 256, NC * 37 * 4, (cudaStream_t)stream>>>(feat, ld, coff, w, bias, field, B, HW, NC,
                                                                                                                         is_gravity, nullptr),
+            cudaGetLastError()));
+  return PF_OK;
+}
+int pf_op_subbin_decode(const float* logits, float* field, float* conf, int B, int HW, int NC, int is_gravity, void* stream) {
+  if (!logits || !field || B < 1 || HW < 1 || NC < 1 || ((uintptr_t)conf & 3)) return fail(PF_ERR_ARG, "pf_op_subbin_decode: bad argument");
+  const unsigned grid = (unsigned)cdivl((long long)B * HW, 256);
+  if (conf)
+    LAUNCHED((argmax_conf_decode_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(logits, field, conf, B, HW, NC, is_gravity), cudaGetLastError()));
+  else
+    LAUNCHED((argmax_decode_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(logits, field, B, HW, NC, is_gravity), cudaGetLastError()));
+  return PF_OK;
+}
+int pf_op_pred_subbin_decode(const float* feat, int ld, int coff, const float* w, const float* bias, float* field, float* conf, int B, int HW, int NC,
+                             int is_gravity, void* stream) {
+  if (!feat || !w || !bias || !field || B < 1 || HW < 1 || NC < 1 || NC > 256 || (ld & 3) || (coff & 3) || ((uintptr_t)conf & 3))
+    return fail(PF_ERR_ARG, "pf_op_pred_subbin_decode: bad argument");
+  const auto kern = conf ? pred_argmax_decode_kernel<true, true> : pred_argmax_decode_kernel<false, true>;
+  LAUNCHED((kern<<<ew_grid((long long)B * HW * 4), 256, NC * 37 * 4, (cudaStream_t)stream>>>(feat, ld, coff, w, bias, field, B, HW, NC, is_gravity, conf),
             cudaGetLastError()));
   return PF_OK;
 }

@@ -298,7 +298,8 @@ class ResizeTransform:
 
 
 class PerspectiveFields(nn.Module):
-    def __init__(self, version="Paramnet-360Cities-edina-centered", logits=True, precision="fp32", resize=None, confidence=False):
+    def __init__(self, version="Paramnet-360Cities-edina-centered", logits=True, precision="fp32", resize=None, confidence=False,
+                 decode="argmax"):
         """``logits=False`` (classification variant only, SURVEY.md 8f-3; NOT the reference's behaviour): ``pred_gravity`` /
         ``pred_latitude`` hold the decoded fields ([2,320,320] up-vectors, [1,320,320] degrees) instead of the 73 / 180 raw logits,
         which are then never written (engine option "decode_only"); the ``*_original`` entries are unchanged.
@@ -320,7 +321,17 @@ class PerspectiveFields(nn.Module):
         [1/NC, 1]: ``pred_gravity_confidence`` / ``pred_latitude_confidence`` [H, W] at the working size and
         ``pred_gravity_confidence_original`` / ``pred_latitude_confidence_original`` [height, width], resampled as the latitude
         map is.  They follow the other keys, whose values are unchanged.  It combines with ``logits``, ``precision`` and
-        ``resize`` and survives ``.to()`` / ``load_state_dict``; ``calibrate.fit_camera(..., weights="confidence")`` reads it."""
+        ``resize`` and survives ``.to()`` / ``load_state_dict``; ``calibrate.fit_camera(..., weights="confidence")`` reads it.
+
+        ``decode``: how the classification heads' logits become fields.  ``"argmax"`` (default) is the reference's decode: the
+        argmax bin's centre, so up directions snap to 5-degree and latitudes to 1-degree steps.  ``"subbin"`` (classification
+        variant only, ``ValueError`` otherwise; NOT the reference's decode) moves the argmax bin c to c + delta, delta in [-1/2, 1/2]
+        the vertex of the parabola through the logits of c and its two neighbours (DESIGN.md section 1, "Sub-bin decode"; engine
+        option "subbin").  The fields become continuous and are exact for logits quadratic in the bin distance near the peak; how
+        much this helps a trained checkpoint has not been measured.  With ``logits=False``, ``pred_gravity`` / ``pred_latitude``
+        hold the refined fields; with ``logits=True`` only the ``_original`` fields change.  Logits, confidence maps and every other
+        key are unchanged.  It combines with ``logits``, ``precision``, ``resize`` and ``confidence`` and survives ``.to()`` /
+        ``load_state_dict``; ``calibrate.fit_camera`` and ``rectify.level_panoramas`` read the refined fields as they are."""
         super().__init__()
         zoo = model_zoo[version]  # KeyError for unknown versions, like the reference (perspectivefields.py:127)
         self.version = version
@@ -350,6 +361,12 @@ class PerspectiveFields(nn.Module):
         if confidence and self._variant["gravity"] != "classification":
             raise ValueError(f"confidence=True needs classification heads; {version} regresses its fields (PersNet-360Cities has them)")
         self._confidence = bool(confidence)
+        if decode not in ("argmax", "subbin"):
+            raise ValueError(f"decode must be 'argmax' or 'subbin', got {decode!r}")
+        if decode == "subbin":
+            if self._variant["gravity"] != "classification":
+                raise ValueError(f"decode='subbin' needs classification heads; {version} regresses its fields (PersNet-360Cities has them)")
+            self._options["subbin"] = 1
         if precision not in ("fp32", "bf16"):
             raise ValueError(f"precision must be 'fp32' or 'bf16', got {precision!r}")
         if precision == "bf16":

@@ -368,7 +368,8 @@ def level_panoramas(model, panos, views=None, mode="bilinear", weights=None, hub
       vfov 70 degrees, ar 1.  Which view set levels real panoramas best has not been measured, nor has the accuracy of the
       levelling on real tilted panoramas.
     - ``mode``: the sampler of the rotation; ``weights`` ("confidence" needs a model built with ``confidence=True``) and
-      ``huber``: as in ``calibrate.fit_panorama``.
+      ``huber``: as in ``calibrate.fit_panorama``.  A model built with ``decode="subbin"`` works unchanged: the fit reads its
+      refined fields.
 
     Returns a dict: ``im`` (the levelled panoramas, ``rotate_panoramas``' output) and ``fits`` (``fit_panorama``'s dicts).
     The fields the model predicts for a crop are its own: no ground truth is used."""
