@@ -75,6 +75,9 @@ const char* pf_last_error(void);
 
 /* Number of CUDA kernels launched by this library in the calling process so far (all handles). */
 int64_t pf_kernel_launch_count(void);
+/* The engine's Pillow resize-table cache (DESIGN.md section 5): bytes of the 8 MB slab in use and how many times the slab was
+ * full and started over since pf_create.  A reset happens only between batches, before a batch's first table is fetched. */
+int pf_resize_table_stats(pf_handle h, int64_t* bytes_used, int64_t* resets);
 
 /* Engine lifetime.  `device` is the CUDA ordinal; the engine makes it current for its own calls. */
 int pf_create(int device, const pf_model_desc* desc, pf_handle* out);

@@ -197,6 +197,7 @@ def lib():
         "pf_abi_version": (i32, []),
         "pf_last_error": (ctypes.c_char_p, []),
         "pf_kernel_launch_count": (i64, []),
+        "pf_resize_table_stats": (i32, [vp, ctypes.POINTER(i64), ctypes.POINTER(i64)]),
         "pf_create": (i32, [i32, ctypes.POINTER(pf_model_desc), ctypes.POINTER(vp)]),
         "pf_create_sized": (i32, [i32, ctypes.POINTER(pf_model_desc), i32, i32, ctypes.POINTER(vp)]),
         "pf_destroy": (i32, [vp]),
@@ -319,7 +320,7 @@ def lib():
     return L
 
 
-EXPORTS = ["pf_abi_version", "pf_last_error", "pf_kernel_launch_count", "pf_create", "pf_create_sized", "pf_destroy", "pf_set_weight",
+EXPORTS = ["pf_abi_version", "pf_last_error", "pf_kernel_launch_count", "pf_resize_table_stats", "pf_create", "pf_create_sized", "pf_destroy", "pf_set_weight",
            "pf_finalize", "pf_workspace_bytes", "pf_forward", "pf_forward_confidence", "pf_param_workspace_bytes", "pf_param_forward", "pf_param_train_workspace_bytes",
            "pf_param_train_forward", "pf_param_backward", "pf_param_grad_numel", "pf_param_grad_entry", "pf_profile_enable", "pf_profile_read", "pf_profile_kernels_enable",
            "pf_profile_kernels_read", "pf_set_option", "pf_debug_enable", "pf_debug_count", "pf_debug_name", "pf_debug_numel",

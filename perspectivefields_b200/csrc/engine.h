@@ -83,6 +83,7 @@ struct pf_engine {
   char* table_dev = nullptr;
   char* table_host = nullptr;       // pinned
   long long table_off = 0;
+  long long table_resets = 0;       // times the slab was full and started over (pf_resize_table_stats)
   KernelProf kp;                    // pf_profile_kernels_*
   // per-launch profiling of the GEMM engine (bench.py roofline leg): CUDA events on the launch stream
   // tensor maps are pure functions of (pointer, shape, box): cached across calls (the arena hands out the same addresses for the

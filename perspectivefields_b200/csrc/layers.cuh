@@ -752,8 +752,16 @@ __device__ __forceinline__ void conf_update(float v, float& m, float& s) {
   if (v > m) { s = s * expf(m - v) + 1.0f; m = v; }
   else s += expf(v - m);
 }
+// merge another running pair (om, os) into (m, s), the own pair first
+__device__ __forceinline__ void conf_merge(float& m, float& s, float om, float os) {
+  const float mm = fmaxf(m, om);
+  s = s * expf(m - mm) + os * expf(om - mm);
+  m = mm;
+}
 // argmax_decode_kernel plus the confidence, in one pass over the logits (the logits are read once).  conf: [B, HW].
-// kRefine: as argmax_decode_kernel's; conf does not depend on it.
+// kRefine: as argmax_decode_kernel's; conf does not depend on it.  The sum runs in pred_argmax_decode_kernel's order: four
+// running pairs over the classes c = j, j + 4, ... (j = 0..3), merged as its quad shuffles merge them, ((0, 1), (2, 3)), so
+// that both "decode_only" settings return the same confidence bit for bit.
 template <bool kRefine>
 __global__ void __launch_bounds__(256) argmax_conf_decode_kernel(const float* __restrict__ logits, float* __restrict__ field, float* __restrict__ conf,
                                                                  int B, int HW, int NC, int is_gravity) {
@@ -761,14 +769,24 @@ __global__ void __launch_bounds__(256) argmax_conf_decode_kernel(const float* __
   if (pix >= (long long)B * HW) return;
   const int b = (int)(pix / HW), r = (int)(pix % HW);
   const float* lp = logits + (long long)b * NC * HW + r;
-  float best = lp[0], s = 1.0f;
+  float best = lp[0];
   int bi = 0;
-  for (int c = 1; c < NC; ++c) {
-    const float v = __ldg(lp + (long long)c * HW);
-    if (v > best) { s = s * expf(best - v) + 1.0f; best = v; bi = c; }
-    else s += expf(v - best);
+  float cm[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY}, cs[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+  for (int c0 = 0; c0 < NC; c0 += 4) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int c = c0 + j;
+      if (c < NC) {
+        const float v = __ldg(lp + (long long)c * HW);
+        if (v > best) { best = v; bi = c; }
+        conf_update(v, cm[j], cs[j]);
+      }
+    }
   }
-  conf[pix] = 1.0f / s;
+  conf_merge(cm[0], cs[0], cm[1], cs[1]);
+  conf_merge(cm[2], cs[2], cm[3], cs[3]);
+  conf_merge(cm[0], cs[0], cm[2], cs[2]);
+  conf[pix] = 1.0f / cs[0];
   if constexpr (kRefine) {
     const int2 nb = subbin_neighbours(NC, bi, is_gravity);
     subbin_decode_store(field, b, r, HW, NC, bi, best, __ldg(lp + (long long)nb.x * HW), __ldg(lp + (long long)nb.y * HW), is_gravity);
@@ -835,9 +853,7 @@ __global__ void __launch_bounds__(256) pred_argmax_decode_kernel(const float* __
       if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
       if constexpr (kConf) {
         const float om = __shfl_xor_sync(0xffffffffu, cm, o), os = __shfl_xor_sync(0xffffffffu, cs, o);
-        const float m = fmaxf(cm, om);
-        cs = cs * expf(cm - m) + os * expf(om - m);
-        cm = m;
+        conf_merge(cm, cs, om, os);
       }
     }
     float lm = 0.0f, lp = 0.0f;

@@ -5,6 +5,7 @@
 #include <cmath>
 #include <cstring>
 #include <mutex>
+#include <set>
 
 #include "engine.h"
 #include "attention_mma.cuh"
@@ -278,6 +279,20 @@ int Fwd::pred_tail(const float* in, int ldi, int icoff, const float* w, const fl
 
 // ----------------------------------------------------------------------------------------------- the forward graph
 constexpr long long kTableSlabBytes = 8LL << 20;   // ~370 tables of a 2048-pixel axis; reset (after a stream sync) when full
+// slab bytes of one (in_size -> out_size) table: bounds and coefficients, each rounded up to 256 bytes
+static long long table_bytes(int in_size, int out_size) {
+  const long long nb = 2LL * out_size * sizeof(int), nc = (long long)out_size * resample_ksize(in_size, out_size) * sizeof(int);
+  return ((nb + 255) & ~255LL) + ((nc + 255) & ~255LL);
+}
+// slab full: earlier forwards on this stream may still read the old tables and the pinned mirror may still be the source of an
+// in-flight copy -> drain the stream once, then start over
+static int reset_tables(pf_engine* e, cudaStream_t st) {
+  CU(cudaStreamSynchronize(st));
+  e->tables.clear();
+  e->table_off = 0;
+  ++e->table_resets;
+  return PF_OK;
+}
 static int get_table(pf_engine* e, int in_size, int out_size, pf_engine::DevTable* out, cudaStream_t st) {
   auto it = e->tables.find({in_size, out_size});
   if (it == e->tables.end()) {
@@ -285,13 +300,7 @@ static int get_table(pf_engine* e, int in_size, int out_size, pf_engine::DevTabl
     const long long nb = (long long)t.bounds.size() * sizeof(int), nc = (long long)t.coeffs.size() * sizeof(int);
     const long long need = ((nb + 255) & ~255LL) + ((nc + 255) & ~255LL);
     if (need > kTableSlabBytes) return fail(PF_ERR_ARG, "image axis of %d pixels is too long for the resize tables", in_size);
-    if (e->table_off + need > kTableSlabBytes) {
-      // slab full: earlier forwards on this stream may still read the old tables and the pinned mirror may still be the source
-      // of an in-flight copy -> drain the stream once, then start over
-      CU(cudaStreamSynchronize(st));
-      e->tables.clear();
-      e->table_off = 0;
-    }
+    if (e->table_off + need > kTableSlabBytes) TRY(reset_tables(e, st));
     pf_engine::DevTable d{};
     d.ksize = t.ksize;
     const long long o0 = e->table_off, o1 = o0 + ((nb + 255) & ~255LL);
@@ -331,18 +340,39 @@ static int fwd_preprocess(Fwd& F, const pf_batch* bt, float*& x0, PreImage*& d_p
   d_post = (PostImage*)ar.alloc((long long)n * sizeof(PostImage));
   if (!dry) {
     if (bt->images_u8) {
+      // The one launch below reads every image's tables, so all of them must be in the slab at once: a reset while the
+      // descriptors are filled would hand the earlier images tables that the later ones overwrite.  Reset once, before the first
+      // fetch, if this batch's uncached tables do not fit the rest of the slab; a batch whose tables exceed the slab is an error.
+      std::set<std::pair<int, int>> distinct;
+      long long all_bytes = 0, new_bytes = 0;
+      for (int i = 0; i < n; ++i) {
+        const int H = bt->height[i], W = bt->width[i];
+        if (H < 1 || W < 1) return fail(PF_ERR_ARG, "image %d has size %dx%d", i, H, W);
+        if (resample_ksize(H, NH) + 1 > max_rows) return fail(PF_ERR_ARG, "image %d is too tall (%d rows) for the resize kernel", i, H);
+        for (const std::pair<int, int> k : {std::make_pair(W, NW), std::make_pair(H, NH)}) {
+          if (!distinct.insert(k).second) continue;
+          const long long b = table_bytes(k.first, k.second);
+          all_bytes += b;
+          if (!e->tables.count(k)) new_bytes += b;
+        }
+      }
+      if (all_bytes > kTableSlabBytes)
+        return fail(PF_ERR_ARG, "the batch's %d images need %lld bytes of resize tables, more than the %lld-byte cache: split the batch", n, all_bytes,
+                    kTableSlabBytes);
+      if (e->table_off + new_bytes > kTableSlabBytes) TRY(reset_tables(e, st));
+      const long long resets = e->table_resets;
       std::vector<PreImage> pre(n);
       int max_h = 1;
       for (int i = 0; i < n; ++i) {
         const int H = bt->height[i], W = bt->width[i];
-        if (H < 1 || W < 1) return fail(PF_ERR_ARG, "image %d has size %dx%d", i, H, W);
         pf_engine::DevTable tx, ty;
         TRY(get_table(e, W, NW, &tx, st));
         TRY(get_table(e, H, NH, &ty, st));
-        if (ty.ksize + 1 > max_rows) return fail(PF_ERR_ARG, "image %d is too tall (%d rows) for the resize kernel", i, H);
         pre[i] = PreImage{bt->image_offset[i], H, W, tx.ksize, ty.ksize, tx.bounds, tx.coeffs, ty.bounds, ty.coeffs};
         if (H > max_h) max_h = H;
       }
+      if (e->table_resets != resets)
+        return fail(PF_ERR_CUDA, "internal error: the resize-table cache was reset while batch descriptors were filled; nothing was launched");
       CU(cudaMemcpyAsync(d_pre, pre.data(), n * sizeof(PreImage), cudaMemcpyHostToDevice, st));
       int rows = pre_rows_needed(max_h, NH);
       if (rows > max_rows) rows = max_rows;
@@ -709,6 +739,13 @@ extern "C" {
 int pf_abi_version(void) { return PF_ABI_VERSION; }
 const char* pf_last_error(void) { return g_err.c_str(); }
 int64_t pf_kernel_launch_count(void) { return g_launches.load(); }
+
+int pf_resize_table_stats(pf_handle h, int64_t* bytes_used, int64_t* resets) {
+  if (!h || !bytes_used || !resets) return fail(PF_ERR_ARG, "pf_resize_table_stats: null argument");
+  *bytes_used = h->table_off;
+  *resets = h->table_resets;
+  return PF_OK;
+}
 
 // a working size the engine supports: H and W multiples of 32 in [64, 640] (the smallest head level is then at least 2 x 2, which
 // the border-class bias needs) with at most kAmMaxKeys attention keys (H/32) * (W/32)

@@ -22,13 +22,18 @@ struct ResampleTable {  // host-side, for one (in_size -> out_size) axis
   std::vector<int> coeffs;  // [out_size][ksize]
 };
 
+inline int resample_ksize(int in_size, int out_size) {   // coefficients per output pixel (the table's row width)
+  const double scale = (double)in_size / (double)out_size;
+  return (int)ceil(scale < 1.0 ? 1.0 : scale) * 2 + 1;
+}
+
 inline ResampleTable make_resample_table(int in_size, int out_size) {
   ResampleTable t;
   t.in_size = in_size;
   const double scale = (double)in_size / (double)out_size;
   const double filterscale = scale < 1.0 ? 1.0 : scale;
   const double support = 1.0 * filterscale;  // bilinear (triangle) filter support = 1
-  t.ksize = (int)ceil(support) * 2 + 1;
+  t.ksize = resample_ksize(in_size, out_size);
   t.bounds.assign((size_t)out_size * 2, 0);
   t.coeffs.assign((size_t)out_size * t.ksize, 0);
   std::vector<double> k((size_t)t.ksize);
