@@ -177,7 +177,17 @@ int pf_profile_kernels_read(pf_handle h, char* buf, int cap);
  *   GEMMs and 3x3 convolutions, the 7x7 stems and both products of the mma.sync attention core -- is one bf16 MMA of the
  *   operands' hi planes (bf16-rounded operands, fp32 accumulation) instead of the three of the split-precision scheme.  The
  *   CUDA-core kernels (LayerNorm, depthwise convolutions, resampling, softmax, prediction tails, the conv1 border ring, the
- *   ParamNet stem and tail) stay fp32.  Read at every launch: it can be switched between pf_forward calls on one handle. */
+ *   ParamNet stem and tail) stay fp32.  Read at every launch: it can be switched between pf_forward calls on one handle.
+ * "flip_tta" (default 0; NOT the reference's behaviour, DESIGN.md section 1 "Flip test-time augmentation"): the network also
+ *   runs on every image's left-right mirror, taken at the source (uint8: Pillow's resize of x[:, ::-1] with the same tables;
+ *   images_chw: the given image mirrored), as slot n + i of a 2n-slot batch through conv_fuse_conv1.  The two head outputs of
+ *   each image are merged at the working size, b read mirrored back (column W-1-x at x), each merge a sum then a scale:
+ *   regression up normalize(a + M(b) * (-1, 1)), sin-latitude (a + M(b)) * 0.5, classification logits (a + P(M(b))) * 0.5 with
+ *   P the up head's class map c -> (36 - c) mod 72 (bin 72 stays) and the identity for the latitude head.  Decode, confidence,
+ *   post-process and ParamNet then run once on the n merged outputs; every output keeps its shape, and the working-size head
+ *   outputs are exactly mirror-equivariant.  Under "decode_only" no logits of either half are written.  PF_ERR_ARG when set on
+ *   a model with one regression and one classification head.  Read at every call; pf_workspace_bytes returns the need for the
+ *   current value (about twice the need without it). */
 int pf_set_option(pf_handle h, const char* name, int value);
 
 /* Debug taps (tests only): when enabled, intermediates of the next pf_forward (or pf_param_forward) are kept (never recycled) and can be
@@ -626,6 +636,18 @@ int pf_op_pred_argmax_decode(const float* feat, int ld, int coff, const float* w
 int pf_op_subbin_decode(const float* logits, float* field, float* conf, int B, int HW, int NC, int is_gravity, void* stream);
 int pf_op_pred_subbin_decode(const float* feat, int ld, int coff, const float* w, const float* bias, float* field, float* conf, int B, int HW, int NC,
                              int is_gravity, void* stream);
+/* The merges of option "flip_tta" (DESIGN.md section 1, "Flip test-time augmentation"), through the helpers pf_forward launches
+ * them with.  Slot i of the 2n input slots is image i, slot n + i its mirror; outputs hold the n merged images at H x W.
+ * pf_op_flip_merge_reg: regression heads, g2 [2n,2,H*W] unit up vectors and l2 [2n,1,H*W] sin-latitudes -> gravity [n,2,H*W],
+ *   latitude [n,1,H*W].
+ * pf_op_flip_pred: a classification head from conv1 features feat [2n*H*W, ld] (channels coff..coff+31; 16-byte aligned), weights
+ *   [NC][32], bias [NC]: the 1x1 convs of both slots (the fma chain of pf_op_pred_tail) and the merged logits.  decode = 0: logits
+ *   [n,NC,H*W] to out (conf NULL, subbin 0); decode = 1: the argmax (subbin = 1: sub-bin) decode of the merged logits to out
+ *   ([n,2,H*W] when is_gravity, else [n,1,H*W] degrees) and, when conf is not NULL, their confidence [n,H*W]; no logits are written.
+ * Every argument is checked before anything is launched (PF_ERR_ARG). */
+int pf_op_flip_merge_reg(const float* g2, const float* l2, float* gravity, float* latitude, int n, int H, int W, void* stream);
+int pf_op_flip_pred(const float* feat, int ld, int coff, const float* w, const float* bias, float* out, float* conf, int n, int H, int W, int NC,
+                    int is_gravity, int decode, int subbin, void* stream);
 /* resample of decoded fields to the original sizes (gravity_head.py:246-256, latitude_head.py:209-219, utils/utils.py:483-507):
  * vec [n,2,320,320], lat [n,1,320,320] -> blobs as in pf_batch; lat_is_sin: lat holds sin(latitude) (regression head). */
 int pf_op_postprocess(const float* vec, const float* lat, int n, const int32_t* height, const int32_t* width,

@@ -292,6 +292,8 @@ def lib():
         "pf_op_pred_argmax_decode": (i32, [vp, i32, i32, vp, vp, vp, i32, i32, i32, i32, vp]),
         "pf_op_subbin_decode": (i32, [vp, vp, vp, i32, i32, i32, i32, vp]),
         "pf_op_pred_subbin_decode": (i32, [vp, i32, i32, vp, vp, vp, vp, i32, i32, i32, i32, vp]),
+        "pf_op_flip_merge_reg": (i32, [vp, vp, vp, vp, i32, i32, i32, vp]),
+        "pf_op_flip_pred": (i32, [vp, i32, i32, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp]),
         "pf_op_postprocess": (i32, [vp, vp, i32, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32), vp, ctypes.POINTER(i64), vp,
                                     ctypes.POINTER(i64), i32, vp]),
         "pf_op_postprocess_sized": (i32, [vp, vp, i32, i32, i32, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32), vp,
@@ -335,7 +337,7 @@ EXPORTS = ["pf_abi_version", "pf_last_error", "pf_kernel_launch_count", "pf_resi
            "pf_op_attention_tc", "pf_op_attention_tc_bf16", "pf_op_attention_tc_keys", "pf_op_dwconv3x3_gelu",
            "pf_op_dwconv7x7", "pf_op_upsample2x", "pf_op_preprocess", "pf_op_preprocess_sized", "pf_op_fill_stream", "pf_op_resize_u8",
            "pf_op_resize_f32", "pf_op_argmax_decode", "pf_op_pred_argmax_decode", "pf_op_subbin_decode", "pf_op_pred_subbin_decode",
-           "pf_op_postprocess", "pf_op_postprocess_sized",
+           "pf_op_flip_merge_reg", "pf_op_flip_pred", "pf_op_postprocess", "pf_op_postprocess_sized",
            "pf_op_pn_wgrad", "pf_op_pn_colsum", "pf_op_pn_ln_bwd", "pf_op_pn_dw7_bwd", "pf_op_pn_stem_bwd", "pf_op_pn_fields_grad",
            "pf_op_pn_tail_bwd", "pf_op_pn_pw2_grads", "pf_op_pn_gelu_bwd", "pf_op_pn_scale_split", "pf_op_pn_col2im2",
            "pf_op_layernorm_ex", "pf_op_dwconv3x3_gelu_ex", "pf_op_upsample2x_ex", "pf_op_stem_gather", "pf_op_pn_stem",

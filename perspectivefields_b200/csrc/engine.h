@@ -66,6 +66,7 @@ struct pf_engine {
   bool use_pdl = true;                // option "pdl": programmatic dependent launch of the graph's kernels (common.cuh)
   bool decode_only = false;           // option "decode_only": classification heads return decoded fields, logits are never written
   bool subbin = false;                // option "subbin": classification heads decode their argmax bin to a sub-bin position
+  bool flip_tta = false;              // option "flip_tta": the network also runs on every image's mirror; the heads' outputs are merged
   const float *pred_g_w, *pred_g_b, *pred_l_w, *pred_l_b;
   const float *pn_stem_w, *pn_stem_b;
   LnW pn_stem_ln, pn_ds_ln[4], pn_norm;
@@ -309,6 +310,14 @@ struct Fwd {
   int param_tail(const float* feat, int HW, const LnW& norm, const float* hw, const float* hb, int kind, float* params, float* raw);
   // 1x1 conv 32 -> NC on channels icoff .. icoff + 31 of [n * HW, ldi] -> NCHW out; mode 0 raw, 1 normalise (NC 2), 2 clamp
   int pred_tail(const float* in, int ldi, int icoff, const float* w, const float* b, float* out, int HW, int NC, int mode);
+  // option "flip_tta": the n merged outputs of the 2n slots (image i in slot i, its mirror in slot n + i) at the working size H x W.
+  // Regression heads: g2 [2n, 2, HW] / l2 [2n, 1, HW] head outputs -> g [n, 2, HW] / l [n, 1, HW]
+  int flip_merge_reg(const float* g2, const float* l2, float* g, float* l, int H, int W);
+  // classification head of NC classes from channels icoff .. icoff + 31 of conv1 features [2n * HW, ldi]: decode = false writes the
+  // merged logits [n, NC, HW] to out; decode = true the decoded field (argmax, or sub-bin with refine) to out and, when conf is not
+  // NULL, the confidence [n, HW]
+  int flip_pred(const float* in, int ldi, int icoff, const float* w, const float* b, float* out, float* conf, int H, int W, int NC, int is_gravity,
+                bool decode, bool refine);
 };
 
 

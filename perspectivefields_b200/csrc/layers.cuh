@@ -878,6 +878,130 @@ __global__ void __launch_bounds__(256) pred_argmax_decode_kernel(const float* __
 }
 
 // =====================================================================================================
+// Flip test-time augmentation (DESIGN.md section 1, "Flip test-time augmentation"; option "flip_tta").  The network ran on 2n
+// slots: slot i is image i, slot n + i its mirror x[:, ::-1].  The merges below write n outputs at the working size H x W; b is
+// read at column W - 1 - x for output column x (M(b)).  Every merge is a sum, then a scale, rounded one at a time (no fma
+// contraction), and the up vector's x component enters as an exact negation: merge(mirror) is the mirror of merge bit for bit.
+
+// Regression heads: g2 [2n, 2, HW] (normalised up vectors), l2 [2n, 1, HW] (clamped sin-latitude) -> g [n, 2, HW], l [n, 1, HW]:
+//   g = normalize(a + M(b) * (-1, 1)) with F.normalize's rule v / max(|v|, 1e-12);  l = (a + M(b)) * 0.5.
+__global__ void __launch_bounds__(256) flip_merge_reg_kernel(const float* __restrict__ g2, const float* __restrict__ l2, float* __restrict__ g,
+                                                             float* __restrict__ l, int n, int H, int W) {
+  const int HW = H * W;
+  const int pix = blockIdx.x * blockDim.x + threadIdx.x;
+  if (pix >= n * HW) return;
+  const int i = pix / HW, r = pix - i * HW, y = r / W, x = r - y * W;
+  const int rb = y * W + (W - 1 - x);
+  const float* ga = g2 + (size_t)i * 2 * HW + r;
+  const float* gb = g2 + (size_t)(n + i) * 2 * HW + rb;
+  const float vx = __fsub_rn(__ldg(ga), __ldg(gb)), vy = __fadd_rn(__ldg(ga + HW), __ldg(gb + HW));
+  const float nrm = fmaxf(__fsqrt_rn(__fadd_rn(__fmul_rn(vx, vx), __fmul_rn(vy, vy))), 1e-12f);
+  float* go = g + (size_t)i * 2 * HW + r;
+  go[0] = __fdiv_rn(vx, nrm);
+  go[HW] = __fdiv_rn(vy, nrm);
+  l[pix] = __fmul_rn(__fadd_rn(__ldg(l2 + (size_t)i * HW + r), __ldg(l2 + (size_t)(n + i) * HW + rb)), 0.5f);
+}
+
+// Class of the mirrored direction: up-direction bin c (angle 5c - 180 degrees for NC = 73) becomes 180 degrees minus that
+// angle, bin (3 (NC - 1) / 2 - c) mod (NC - 1) = (36 - c) mod 72; the no-direction bin NC - 1 and every latitude class stay.
+__host__ __device__ inline int flip_class(int c, int NC, int is_gravity) {
+  if (!is_gravity || c >= NC - 1) return c;
+  const int m = NC - 1;
+  return (m + m / 2 - c) % m;
+}
+// the 1x1 prediction conv of one class on one pixel's 32 features: bias first, then channels 0..31 in order (pred_tail_kernel's
+// fma chain, so the logits equal the unmerged path's bit for bit); wr: the class's weight row (16-byte aligned), b its bias
+__device__ __forceinline__ float pred_logit(const float* f, const float* wr, float b) {
+  const float4* w4 = reinterpret_cast<const float4*>(wr);
+  float v = b;
+#pragma unroll
+  for (int d4 = 0; d4 < 8; ++d4) {
+    const float4 ww = w4[d4];
+    v = fmaf(f[4 * d4], ww.x, v); v = fmaf(f[4 * d4 + 1], ww.y, v); v = fmaf(f[4 * d4 + 2], ww.z, v); v = fmaf(f[4 * d4 + 3], ww.w, v);
+  }
+  return v;
+}
+
+// Classification heads, from the features: per output pixel (i, y, x) the 1x1 prediction conv 32 -> NC of conv1 features
+// (32 channels at icoff of [2n * HW, ldi] NHWC) at slot i, pixel (y, x) (a) and at slot n + i, pixel (y, W - 1 - x) (b), and the
+// merged logits (a_c + b_P(c)) * 0.5, P = flip_class.  The threads, weights and reductions are pred_argmax_decode_kernel's: a quad
+// per pixel, lane q on the classes q, q + 4, ...; weights [NC][36] + bias in shared memory.
+// kDecode = false: the merged logits to out [n, NC, HW] (the decode and confidence kernels then run on them unchanged).
+// kDecode = true ("decode_only"): no logits are written; argmax (first maximal index), kRefine's sub-bin decode and kConf's
+// confidence of the merged logits, in pred_argmax_decode_kernel's order, to out = the field [n, 2 or 1, HW] and conf [n, HW].
+template <bool kDecode, bool kConf, bool kRefine>
+__global__ void __launch_bounds__(256) pred_flip_kernel(const float* __restrict__ in, int ldi, int icoff, const float* __restrict__ w,
+                                                        const float* __restrict__ bias, float* __restrict__ out, float* __restrict__ conf, int n, int H,
+                                                        int W, int NC, int is_gravity) {
+  extern __shared__ __align__(16) float s_pw[];  // [NC][36] then [NC]
+  for (int i = threadIdx.x; i < NC * 32; i += blockDim.x) s_pw[(i >> 5) * 36 + (i & 31)] = __ldg(w + i);
+  float* s_b = s_pw + NC * 36;
+  for (int i = threadIdx.x; i < NC; i += blockDim.x) s_b[i] = __ldg(bias + i);
+  __syncthreads();
+  const int q = threadIdx.x & 3;
+  const int HW = H * W;
+  const long long npix = (long long)n * HW;
+  const long long stride = (long long)gridDim.x * (blockDim.x >> 2);
+  const long long pix_last = npix - 1;
+  const long long iters = (npix + stride - 1) / stride;     // (the same on every lane: the shuffles need the full quad)
+  long long pix = (long long)blockIdx.x * (blockDim.x >> 2) + (threadIdx.x >> 2);
+  for (long long it = 0; it < iters; ++it, pix += stride) {
+    const bool live = pix <= pix_last;
+    const long long pc = live ? pix : pix_last;
+    const int i = (int)(pc / HW), r = (int)(pc - (long long)i * HW), y = r / W, x = r - y * W;
+    const long long pb = (long long)(n + i) * HW + y * W + (W - 1 - x);
+    float fa[32], fb[32];
+#pragma unroll
+    for (int d = 0; d < 32; d += 4) {
+      const float4 t = __ldg(reinterpret_cast<const float4*>(in + pc * ldi + icoff + d));
+      fa[d] = t.x; fa[d + 1] = t.y; fa[d + 2] = t.z; fa[d + 3] = t.w;
+      const float4 u = __ldg(reinterpret_cast<const float4*>(in + pb * ldi + icoff + d));
+      fb[d] = u.x; fb[d + 1] = u.y; fb[d + 2] = u.z; fb[d + 3] = u.w;
+    }
+    auto merged = [&](int c) {
+      const int p = flip_class(c, NC, is_gravity);
+      return __fmul_rn(__fadd_rn(pred_logit(fa, s_pw + c * 36, s_b[c]), pred_logit(fb, s_pw + p * 36, s_b[p])), 0.5f);
+    };
+    if constexpr (!kDecode) {
+      float* o = out + (long long)i * NC * HW + r;
+      for (int c = q; c < NC; c += 4) {
+        const float v = merged(c);
+        if (live) o[(long long)c * HW] = v;
+      }
+    } else {
+      float best = -INFINITY, cm = -INFINITY, cs = 0.0f;
+      int bi = 0x7fffffff;
+      for (int c = q; c < NC; c += 4) {
+        const float v = merged(c);
+        if (v > best || bi == 0x7fffffff) { best = v; bi = c; }
+        if constexpr (kConf) conf_update(v, cm, cs);
+      }
+#pragma unroll
+      for (int o = 1; o < 4; o <<= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
+        if constexpr (kConf) {
+          const float om = __shfl_xor_sync(0xffffffffu, cm, o), os = __shfl_xor_sync(0xffffffffu, cs, o);
+          conf_merge(cm, cs, om, os);
+        }
+      }
+      float lm = 0.0f, lp = 0.0f;
+      if constexpr (kRefine) {
+        const int2 nb = subbin_neighbours(NC, __shfl_sync(0xffffffffu, bi, 0, 4), is_gravity);
+        lm = merged((q & 1) ? nb.y : nb.x);
+        lp = __shfl_xor_sync(0xffffffffu, lm, 1);
+      }
+      if (live && q == 0) {
+        if constexpr (kRefine) subbin_decode_store(out, i, r, HW, NC, bi, best, lm, lp, is_gravity);
+        else decode_bin_store(out, i, r, HW, NC, bi, is_gravity);
+        if constexpr (kConf) conf[pix] = 1.0f / cs;
+      }
+    }
+  }
+}
+
+// =====================================================================================================
 // ParamNet input: cat(pred_gravity, pred_latitude) (param_network.py:47-49 / 194-197), optionally the nearest
 // IH x IW -> OH x OW sub-sample F.interpolate(images, (OH, OW)) (ATen nearest: src = floor(dst * (float)in / out), clamped).
 // NCHW fields at the net size IH x IW -> NHWC [B,OH,OW,4].

@@ -277,6 +277,27 @@ int Fwd::pred_tail(const float* in, int ldi, int icoff, const float* w, const fl
   return PF_OK;
 }
 
+int Fwd::flip_merge_reg(const float* g2, const float* l2, float* g, float* l, int H, int W) {
+  if (n < 1 || H < 1 || W < 1 || !fits31(4LL * n * H * W)) return fail(PF_ERR_ARG, "flip_merge_reg: %d images of %dx%d", n, H, W);
+  if (dry) return PF_OK;
+  LAUNCHED((flip_merge_reg_kernel<<<(unsigned)cdivl((long long)n * H * W, 256), 256, 0, st>>>(g2, l2, g, l, n, H, W), cudaGetLastError()));
+  return PF_OK;
+}
+int Fwd::flip_pred(const float* in, int ldi, int icoff, const float* w, const float* b, float* out, float* conf, int H, int W, int NC, int is_gravity,
+                   bool decode, bool refine) {
+  // (the class map assumes the up head's bins on a circle, an even count of them)
+  if (n < 1 || H < 1 || W < 1 || NC < 2 || NC > 256 || (is_gravity && (NC - 1) % 2) || (ldi | icoff) % 4 || icoff < 0 || icoff + 32 > ldi ||
+      !fits31(2LL * n * H * W) || !fits31((long long)n * NC * H * W) || (!decode && (conf || refine)))
+    return fail(PF_ERR_ARG, "flip_pred: %d images of %dx%d, %d classes, channels %d.. of %d, decode %d / conf %d / refine %d", n, H, W, NC, icoff, ldi,
+                (int)decode, conf != nullptr, (int)refine);
+  if (dry) return PF_OK;
+  const auto kern = !decode ? pred_flip_kernel<false, false, false>
+                            : (conf ? (refine ? pred_flip_kernel<true, true, true> : pred_flip_kernel<true, true, false>)
+                                    : (refine ? pred_flip_kernel<true, false, true> : pred_flip_kernel<true, false, false>));
+  LAUNCHED((kern<<<ew_grid((long long)n * H * W * 4), 256, NC * 37 * 4, st>>>(in, ldi, icoff, w, b, out, conf, n, H, W, NC, is_gravity), cudaGetLastError()));
+  return PF_OK;
+}
+
 // ----------------------------------------------------------------------------------------------- the forward graph
 constexpr long long kTableSlabBytes = 8LL << 20;   // ~370 tables of a 2048-pixel axis; reset (after a stream sync) when full
 // slab bytes of one (in_size -> out_size) table: bounds and coefficients, each rounded up to 256 bytes
@@ -324,18 +345,19 @@ static int pre_rows_needed(int H, int OH) {  // input rows one block of kPreRows
 static int pre_max_smem_rows(int OW) { return kPreSmemBytes / (OW * 3); }   // resampled rows that fit the shared-memory budget
 
 // ----------------------------------------------------------------------------------------------- shared graph sections
-// uint8 HWC (any size) or pre-resized fp32 CHW -> x0 [n,NH,NW,4] fp32 normalised (NH x NW: the engine's working size)
-static int fwd_preprocess(Fwd& F, const pf_batch* bt, float*& x0, PreImage*& d_pre, PostImage*& d_post) {
+// uint8 HWC (any size) or pre-resized fp32 CHW -> x0 [F.n,NH,NW,4] fp32 normalised (NH x NW: the engine's working size).  The
+// batch has n input images; F.n = 2n slots under option "flip_tta" (slot n + i: image i mirrored at the source), else n.
+static int fwd_preprocess(Fwd& F, const pf_batch* bt, int n, float*& x0, PreImage*& d_pre, PostImage*& d_post) {
   pf_engine* e = F.e;
   const pf_model_desc& D = e->desc;
-  const int n = F.n;
+  const int slots = F.n;
   const bool dry = F.dry;
   cudaStream_t st = F.st;
   Arena& ar = F.ar;
   const int NH = e->net_h, NW = e->net_w;
   const int max_rows = pre_max_smem_rows(NW);
   // ---------------- pre-process: uint8 HWC (any size) -> [n,NH,NW,4] fp32 normalised -------------------
-  x0 = ar.f((long long)n * NH * NW * 4);
+  x0 = ar.f((long long)slots * NH * NW * 4);
   d_pre = (PreImage*)ar.alloc((long long)n * sizeof(PreImage));
   d_post = (PostImage*)ar.alloc((long long)n * sizeof(PostImage));
   if (!dry) {
@@ -377,13 +399,13 @@ static int fwd_preprocess(Fwd& F, const pf_batch* bt, float*& x0, PreImage*& d_p
       int rows = pre_rows_needed(max_h, NH);
       if (rows > max_rows) rows = max_rows;
       const int smem = rows * NW * 3;
-      LAUNCHED((preprocess_kernel<<<dim3(NH / kPreRows, n), NW, smem, st>>>(bt->images_u8, d_pre, x0, D.pixel_mean[0], D.pixel_mean[1],
-                                                                           D.pixel_mean[2], D.pixel_std[0], D.pixel_std[1], D.pixel_std[2], rows, NH, NW),
+      LAUNCHED((preprocess_kernel<<<dim3(NH / kPreRows, slots), NW, smem, st>>>(bt->images_u8, d_pre, x0, D.pixel_mean[0], D.pixel_mean[1],
+                                                                               D.pixel_mean[2], D.pixel_std[0], D.pixel_std[1], D.pixel_std[2], rows, NH, NW, n),
                 cudaGetLastError()));
     } else {
-      const long long total = (long long)n * NH * NW;
-      LAUNCHED((normalize_chw_kernel<<<(unsigned)cdivl(total, 256), 256, 0, st>>>(bt->images_chw, x0, n, NH, NW, D.pixel_mean[0], D.pixel_mean[1],
-                                                                                 D.pixel_mean[2], D.pixel_std[0], D.pixel_std[1], D.pixel_std[2]),
+      const long long total = (long long)slots * NH * NW;
+      LAUNCHED((normalize_chw_kernel<<<(unsigned)cdivl(total, 256), 256, 0, st>>>(bt->images_chw, x0, slots, NH, NW, D.pixel_mean[0], D.pixel_mean[1],
+                                                                                 D.pixel_mean[2], D.pixel_std[0], D.pixel_std[1], D.pixel_std[2], n),
                 cudaGetLastError()));
     }
   }
@@ -414,7 +436,9 @@ static int launch_postprocess(const float* vec, const float* lat, int n, int SH,
 // prediction 1x1 convs (+ normalise / clamp) -> NCHW outputs, then argmax decode (classification) and resample to the
 // original resolutions.  conv1_out: [n,NH,NW,64] fp32 (gravity head channels 0-31, latitude head 32-63).  cf (classification
 // heads only, else NULL): the decode kernels also write the head confidence, resampled to the original sizes after the fields.
-// Option "subbin" selects the decode kernels' sub-bin instantiations; nothing else changes.
+// Option "subbin" selects the decode kernels' sub-bin instantiations; nothing else changes.  Option "flip_tta": conv1_out holds
+// 2n slots (F.n = n); the classification heads' 1x1 convs run as the merge kernel (merged logits, or the decode of the merged
+// logits under "decode_only"), everything after them as without the option.
 static int fwd_tails_post(Fwd& F, const pf_batch* bt, const pf_confidence* cf, const float* conv1_out, PostImage* d_post, bool pred_done = false) {
   pf_engine* e = F.e;
   const pf_model_desc& D = e->desc;
@@ -428,16 +452,26 @@ static int fwd_tails_post(Fwd& F, const pf_batch* bt, const pf_confidence* cf, c
   if (e->decode_only && cls_g != cls_l) return fail(PF_ERR_ARG, "decode_only needs both heads to be classification heads");
   const float* vec = dry ? nullptr : bt->pred_gravity;
   const float* lat = dry ? nullptr : bt->pred_latitude;
+  const bool tta = e->flip_tta;
   if (e->debug) {
-    // debug taps: the raw prediction-conv outputs before normalise / clamp (oracle taps g.raw / l.raw)
-    float* rg = ar.f((long long)n * D.gravity_classes * HW);
-    float* rl = ar.f((long long)n * D.latitude_classes * HW);
-    TRY(F.pred_tail(conv1_out, 64, 0, e->pred_g_w, e->pred_g_b, rg, HW, D.gravity_classes, 0));
-    TRY(F.pred_tail(conv1_out, 64, 32, e->pred_l_w, e->pred_l_b, rl, HW, D.latitude_classes, 0));
-    TRY(F.tap("head.raw_g", rg, (long long)n * D.gravity_classes * HW));
-    TRY(F.tap("head.raw_l", rl, (long long)n * D.latitude_classes * HW));
+    // debug taps: the raw prediction-conv outputs before normalise / clamp (oracle taps g.raw / l.raw), of every slot
+    const int slots = tta ? 2 * n : n;
+    float* rg = ar.f((long long)slots * D.gravity_classes * HW);
+    float* rl = ar.f((long long)slots * D.latitude_classes * HW);
+    F.n = slots;
+    const int r1 = F.pred_tail(conv1_out, 64, 0, e->pred_g_w, e->pred_g_b, rg, HW, D.gravity_classes, 0);
+    const int r2 = r1 == PF_OK ? F.pred_tail(conv1_out, 64, 32, e->pred_l_w, e->pred_l_b, rl, HW, D.latitude_classes, 0) : r1;
+    F.n = n;
+    TRY(r2);
+    TRY(F.tap("head.raw_g", rg, (long long)slots * D.gravity_classes * HW));
+    TRY(F.tap("head.raw_l", rl, (long long)slots * D.latitude_classes * HW));
   }
-  if (fused_decode) {
+  if (tta && fused_decode) {
+    TRY(F.flip_pred(conv1_out, 64, 0, e->pred_g_w, e->pred_g_b, dry ? nullptr : bt->pred_gravity, cf ? cf->gravity : nullptr, e->net_h, e->net_w,
+                    D.gravity_classes, 1, true, e->subbin));
+    TRY(F.flip_pred(conv1_out, 64, 32, e->pred_l_w, e->pred_l_b, dry ? nullptr : bt->pred_latitude, cf ? cf->latitude : nullptr, e->net_h, e->net_w,
+                    D.latitude_classes, 0, true, e->subbin));
+  } else if (fused_decode) {
     // option "decode_only": 1x1 conv + argmax + bin decode in one kernel; pred_gravity / pred_latitude hold the decoded fields
     if (!dry) {
       const unsigned grid = ew_grid((long long)n * HW * 4);
@@ -450,7 +484,12 @@ static int fwd_tails_post(Fwd& F, const pf_batch* bt, const pf_confidence* cf, c
     }
   } else {
     // prediction tails -> NCHW outputs (returned to the caller)
-    if (!pred_done) {
+    if (!pred_done && tta) {   // (both heads are classification heads: pf_set_option)
+      TRY(F.flip_pred(conv1_out, 64, 0, e->pred_g_w, e->pred_g_b, dry ? nullptr : bt->pred_gravity, nullptr, e->net_h, e->net_w, D.gravity_classes, 1,
+                      false, false));
+      TRY(F.flip_pred(conv1_out, 64, 32, e->pred_l_w, e->pred_l_b, dry ? nullptr : bt->pred_latitude, nullptr, e->net_h, e->net_w, D.latitude_classes,
+                      0, false, false));
+    } else if (!pred_done) {
       TRY(F.pred_tail(conv1_out, 64, 0, e->pred_g_w, e->pred_g_b, dry ? nullptr : bt->pred_gravity, HW, D.gravity_classes, D.gravity_classes == 2 ? 1 : 0));
       TRY(F.pred_tail(conv1_out, 64, 32, e->pred_l_w, e->pred_l_b, dry ? nullptr : bt->pred_latitude, HW, D.latitude_classes, D.latitude_classes == 1 ? 2 : 0));
     }
@@ -487,9 +526,14 @@ static int fwd_tails_post(Fwd& F, const pf_batch* bt, const pf_confidence* cf, c
 // =============================================================================================== the forward graph
 // The whole network on the TMA -> wgmma engine: every GEMM input is a pre-split bf16 hi/lo tensor written by its producer
 // (LayerNorm, attention, depthwise conv, upsample, stem gather, or the previous GEMM's epilogue).
+// Option "flip_tta": from the pre-process through conv_fuse_conv1 the network runs on n = 2 nimg slots (slot nimg + i: image i
+// mirrored); the heads' outputs are merged into nimg, and the tails, the post-process and ParamNet run on those.
 static int run_forward(Fwd& F, const pf_batch* bt, const pf_confidence* cf = nullptr) {
   pf_engine* e = F.e;
   const pf_model_desc& D = e->desc;
+  const int nimg = F.n;
+  const bool tta = e->flip_tta;
+  F.n = tta ? 2 * nimg : nimg;
   const int n = F.n;
   const bool dry = F.dry;
   cudaStream_t st = F.st;
@@ -505,7 +549,7 @@ static int run_forward(Fwd& F, const pf_batch* bt, const pf_confidence* cf = nul
   float* x0; PreImage* d_pre; PostImage* d_post;
   {
     NvtxRange r_("pf:preprocess");
-    TRY(fwd_preprocess(F, bt, x0, d_pre, d_post));
+    TRY(fwd_preprocess(F, bt, nimg, x0, d_pre, d_post));
   }
   TRY(F.tap("pre", x0, (long long)n * NH * NW * 4));
 
@@ -586,7 +630,12 @@ static int run_forward(Fwd& F, const pf_batch* bt, const pf_confidence* cf = nul
 
   // ---------------- decoder heads (group 0 = gravity, group 1 = latitude, side by side in the channel dimension) ----
   float* conv1_out = ar.f((long long)n * NH * NW * 64);
-  bool fuse_pred = false;
+  const bool fuse_pred = D.gravity_classes == 2 && D.latitude_classes == 1;
+  // option "flip_tta", regression heads: the fused prediction tails write the 2n slots' head outputs here, merged below
+  float* tta_g = tta && fuse_pred ? ar.f((long long)n * 2 * NH * NW) : nullptr;
+  float* tta_l = tta && fuse_pred ? ar.f((long long)n * NH * NW) : nullptr;
+  float* pred_g = dry ? nullptr : (tta ? tta_g : bt->pred_gravity);
+  float* pred_l = dry ? nullptr : (tta ? tta_l : bt->pred_latitude);
   {
     const long long m = ar.mark();
     float* fused = nullptr;       // fp32 top-down feature of the previous level, upsampled to this level's resolution
@@ -635,9 +684,8 @@ static int run_forward(Fwd& F, const pf_batch* bt, const pf_confidence* cf = nul
     // regression heads: the 1x1 prediction conv + normalise / clamp run inside conv_fuse_conv1's epilogue (conv1's own output is
     // then only materialised for the debug taps); classification heads (73 / 180 logits) keep the separate tail kernel
     section("pf:heads.fuse_convs");
-    fuse_pred = D.gravity_classes == 2 && D.latitude_classes == 1;
     const bool keep_conv1 = !fuse_pred || e->debug;   // (not `o.C != nullptr`: the sizing dry run has null pointers)
-    PredTail pt[2] = {{e->pred_g_w, e->pred_g_b, dry ? nullptr : bt->pred_gravity, 2, 1}, {e->pred_l_w, e->pred_l_b, dry ? nullptr : bt->pred_latitude, 1, 2}};
+    PredTail pt[2] = {{e->pred_g_w, e->pred_g_b, pred_g, 2, 1}, {e->pred_l_w, e->pred_l_b, pred_l, 1, 2}};
     // x2 upsample folded into conv1's weights: conv1 runs on the LH x LW grid with N = 4 output phases x 32 (no upsampled
     // tensor); the two outermost output rows / columns, where the identity does not hold, are recomputed by conv1_ring_kernel
     SplitT c0s = F.salloc((long long)n * LH * LW, 128);
@@ -652,13 +700,15 @@ static int run_forward(Fwd& F, const pf_batch* bt, const pf_confidence* cf = nul
     if (!dry) {
       const dim3 grid((unsigned)cdiv(conv1_ring_count(NH, NW), kRingPx), (unsigned)n);
       LAUNCHED((conv1_ring_kernel<<<grid, 256, kRingSmem, st>>>(c0s.hi, c0s.lo, LH, LW, e->conv1f_w, e->conv1f_b, keep_conv1 ? conv1_out : nullptr,
-                                                               fuse_pred ? e->pred_g_w : nullptr, e->pred_g_b, bt->pred_gravity,
-                                                               fuse_pred ? e->pred_l_w : nullptr, e->pred_l_b, bt->pred_latitude), cudaGetLastError()));
+                                                               fuse_pred ? e->pred_g_w : nullptr, e->pred_g_b, pred_g,
+                                                               fuse_pred ? e->pred_l_w : nullptr, e->pred_l_b, pred_l), cudaGetLastError()));
     }
     if (keep_conv1) TRY(F.tap("head.conv1", conv1_out, (long long)n * NH * NW * 64));
     ar.release(m);
   }
   section("pf:tails_postprocess");
+  F.n = nimg;
+  if (tta && fuse_pred) TRY(F.flip_merge_reg(tta_g, tta_l, dry ? nullptr : bt->pred_gravity, dry ? nullptr : bt->pred_latitude, NH, NW));
   TRY(fwd_tails_post(F, bt, cf, conv1_out, d_post, fuse_pred));
 
   // ---------------- ParamNet (ConvNeXt-T on the predicted fields) -------------------------------------------
@@ -995,6 +1045,13 @@ int pf_set_option(pf_handle h, const char* name, int value) {
     h->subbin = value != 0;
     return PF_OK;
   }
+  if (!strcmp(name, "flip_tta")) {
+    if (value && (h->desc.gravity_classes == 2) != (h->desc.latitude_classes == 1))
+      return fail(PF_ERR_ARG, "pf_set_option: \"flip_tta\" needs two regression or two classification heads (this model has %d / %d classes)",
+                  h->desc.gravity_classes, h->desc.latitude_classes);
+    h->flip_tta = value != 0;
+    return PF_OK;
+  }
   if (!strcmp(name, "pdl")) { h->use_pdl = value != 0; return PF_OK; }
   if (!strcmp(name, "bf16")) { h->bf16 = value != 0; return PF_OK; }
   return fail(PF_ERR_ARG, "pf_set_option: unknown option '%s'", name);
@@ -1245,6 +1302,17 @@ int pf_op_pred_subbin_decode(const float* feat, int ld, int coff, const float* w
             cudaGetLastError()));
   return PF_OK;
 }
+int pf_op_flip_merge_reg(const float* g2, const float* l2, float* gravity, float* latitude, int n, int H, int W, void* stream) {
+  if (!g2 || !l2 || !gravity || !latitude) return fail(PF_ERR_ARG, "pf_op_flip_merge_reg: null argument");
+  return op_run("pf_op_flip_merge_reg", n, stream, [&](Fwd& F) { return F.flip_merge_reg(g2, l2, gravity, latitude, H, W); });
+}
+int pf_op_flip_pred(const float* feat, int ld, int coff, const float* w, const float* bias, float* out, float* conf, int n, int H, int W, int NC,
+                    int is_gravity, int decode, int subbin, void* stream) {
+  if (!feat || !w || !bias || !out || ((uintptr_t)conf & 3)) return fail(PF_ERR_ARG, "pf_op_flip_pred: null or unaligned argument");
+  if (!al16(feat) || !al16(w)) return fail(PF_ERR_ARG, "pf_op_flip_pred: unaligned features or weights");
+  return op_run("pf_op_flip_pred", n, stream,
+                [&](Fwd& F) { return F.flip_pred(feat, ld, coff, w, bias, out, conf, H, W, NC, is_gravity ? 1 : 0, decode != 0, subbin != 0); });
+}
 int pf_op_postprocess(const float* vec, const float* lat, int n, const int32_t* height, const int32_t* width, float* gravity_original,
                       const int64_t* gravity_original_offset, float* latitude_original, const int64_t* latitude_original_offset, int lat_is_sin,
                       void* stream) {
@@ -1381,7 +1449,7 @@ int pf_op_preprocess_sized(const uint8_t* img, int H, int W, int net_h, int net_
     TRY(op_upload(F, &pi, 1, &d));
     if (F.dry) return PF_OK;
     LAUNCHED((preprocess_kernel<<<dim3(net_h / kPreRows, 1), net_w, rows * net_w * 3, F.st>>>(img, d, y, mean3[0], mean3[1], mean3[2], std3[0], std3[1], std3[2],
-                                                                                         rows, net_h, net_w),
+                                                                                         rows, net_h, net_w, 1),
               cudaGetLastError()));
     return PF_OK;
   });

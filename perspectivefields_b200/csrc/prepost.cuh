@@ -76,13 +76,18 @@ constexpr int kPreRows = 8;        // output rows per block
 constexpr int kPreMaxW = 640;      // widest working size (block = one thread per output column)
 constexpr int kPreSmemBytes = 200 * 1024;   // budget of the horizontally resampled rows: 213 rows of 320 columns, 106 of 640
 
-// grid = (OH / kPreRows, n_images), block = OW threads (one per output column); OH = net height, OW = net width.
+// grid = (OH / kPreRows, slots), block = OW threads (one per output column); OH = net height, OW = net width.
 // dyn smem = rows_needed * OW * 3 bytes for the horizontally resampled input rows of this tile.
-// out: [n, OH, OW, 4] fp32 NHWC, channels (b, g, r, 0), value = (u8 - mean[c]) / std[c].
+// out: [slots, OH, OW, 4] fp32 NHWC, channels (b, g, r, 0), value = (u8 - mean[c]) / std[c].
+// imgs holds nimg descriptors; slot y >= nimg (option "flip_tta": slots = 2 nimg) is image y - nimg mirrored left-right at the
+// source, i.e. Pillow's resize of x[:, ::-1]: its horizontal pass reads source column W - 1 - j where the plain one reads j, with
+// the same tables (they depend on the sizes only), so the slot equals the plain resize of the flipped image bit for bit.
 __global__ void __launch_bounds__(kPreMaxW) preprocess_kernel(const unsigned char* __restrict__ blob, const PreImage* __restrict__ imgs, float* __restrict__ out,
-                                                              float m0, float m1, float m2, float s0, float s1, float s2, int max_rows, int OH, int OW) {
+                                                              float m0, float m1, float m2, float s0, float s1, float s2, int max_rows, int OH, int OW,
+                                                              int nimg) {
   extern __shared__ unsigned char s_h[];  // [rows][OW][3]
-  const PreImage im = imgs[blockIdx.y];
+  const bool mirror = (int)blockIdx.y >= nimg;
+  const PreImage im = imgs[mirror ? blockIdx.y - nimg : blockIdx.y];
   const int oy0 = blockIdx.x * kPreRows;
   const int x = threadIdx.x;
   const unsigned char* src = blob + im.offset;
@@ -102,12 +107,15 @@ __global__ void __launch_bounds__(kPreMaxW) preprocess_kernel(const unsigned cha
     }
     const int nrows = in_last - in_first;
     // horizontal pass: input rows [in_first, in_last) -> uint8 [nrows][OW][3]
+    // source pixel t of the window: xmin + t, or W - 1 - (xmin + t) mirrored
+    const unsigned char* px0 = src + (long long)in_first * im.W * 3 + (mirror ? im.W - 1 - xmin : xmin) * 3;
+    const int step = mirror ? -3 : 3;
     for (int r = 0; r < nrows; ++r) {
-      const unsigned char* row = src + ((long long)(in_first + r) * im.W + xmin) * 3;
+      const unsigned char* px = px0 + (long long)r * im.W * 3;
       int a0 = 1 << (kPrecisionBits - 1), a1 = a0, a2 = a0;
-      for (int t = 0; t < xn; ++t) {
+      for (int t = 0; t < xn; ++t, px += step) {
         const int k = kx[t];
-        a0 += row[3 * t] * k; a1 += row[3 * t + 1] * k; a2 += row[3 * t + 2] * k;
+        a0 += px[0] * k; a1 += px[1] * k; a2 += px[2] * k;
       }
       unsigned char* d = s_h + (r * OW + x) * 3;
       d[0] = (unsigned char)min(max(a0 >> kPrecisionBits, 0), 255);
@@ -137,13 +145,19 @@ __global__ void __launch_bounds__(kPreMaxW) preprocess_kernel(const unsigned cha
   }
 }
 
-// Lower entry (perspectivefields.py:223-236 called directly): images already resized, fp32 CHW [n,3,H,W] (the net size).
+// Lower entry (perspectivefields.py:223-236 called directly): images already resized, fp32 CHW [nimg,3,H,W] (the net size) ->
+// [n,H,W,4]; slot b >= nimg (option "flip_tta": n = 2 nimg) is image b - nimg mirrored left-right (column W - 1 - x read at x).
 __global__ void __launch_bounds__(256) normalize_chw_kernel(const float* __restrict__ in, float* __restrict__ out, int n, int H, int W,
-                                                            float m0, float m1, float m2, float s0, float s1, float s2) {
+                                                            float m0, float m1, float m2, float s0, float s1, float s2, int nimg) {
   const long long HW = (long long)H * W, total = (long long)n * HW;
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total) return;
-  const long long b = i / HW, p = i % HW;
+  long long b = i / HW, p = i % HW;
+  if (b >= nimg) {
+    const long long y = p / W;
+    b -= nimg;
+    p = y * W + (W - 1 - (p - y * W));
+  }
   const float* s = in + b * 3 * HW + p;
   reinterpret_cast<float4*>(out)[i] = make_float4((s[0] - m0) / s0, (s[HW] - m1) / s1, (s[2 * HW] - m2) / s2, 0.f);
 }

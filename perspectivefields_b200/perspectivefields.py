@@ -299,7 +299,7 @@ class ResizeTransform:
 
 class PerspectiveFields(nn.Module):
     def __init__(self, version="Paramnet-360Cities-edina-centered", logits=True, precision="fp32", resize=None, confidence=False,
-                 decode="argmax"):
+                 decode="argmax", tta=None):
         """``logits=False`` (classification variant only, SURVEY.md 8f-3; NOT the reference's behaviour): ``pred_gravity`` /
         ``pred_latitude`` hold the decoded fields ([2,320,320] up-vectors, [1,320,320] degrees) instead of the 73 / 180 raw logits,
         which are then never written (engine option "decode_only"); the ``*_original`` entries are unchanged.
@@ -331,7 +331,17 @@ class PerspectiveFields(nn.Module):
         much this helps a trained checkpoint has not been measured.  With ``logits=False``, ``pred_gravity`` / ``pred_latitude``
         hold the refined fields; with ``logits=True`` only the ``_original`` fields change.  Logits, confidence maps and every other
         key are unchanged.  It combines with ``logits``, ``precision``, ``resize`` and ``confidence`` and survives ``.to()`` /
-        ``load_state_dict``; ``calibrate.fit_camera`` and ``rectify.level_panoramas`` read the refined fields as they are."""
+        ``load_state_dict``; ``calibrate.fit_camera`` and ``rectify.level_panoramas`` read the refined fields as they are.
+
+        ``tta``: test-time augmentation.  ``None`` (default) runs each image once.  ``"flip"`` (any variant; NOT the reference's
+        behaviour) also runs its left-right mirror, taken before the pre-process, and merges the two heads' outputs at the
+        working size (DESIGN.md section 1, "Flip test-time augmentation"; engine option "flip_tta"): up vectors are summed with
+        the mirror's x component negated and re-normalised, sin-latitudes averaged, classification logits averaged with the up
+        head's classes mirrored.  Decode, confidence, the ``_original`` fields and ParamNet then run on the merged outputs, so
+        every key, shape and order is unchanged, and ``pred_gravity`` / ``pred_latitude`` (logits, or the regression fields)
+        of a mirrored image are the mirror of the image's bit for bit.  The network runs twice per image; how much this helps a
+        trained checkpoint has not been measured.  It combines with ``logits``, ``precision``, ``resize``, ``confidence`` and
+        ``decode`` and survives ``.to()`` / ``load_state_dict``.  Any other value is a ``ValueError``."""
         super().__init__()
         zoo = model_zoo[version]  # KeyError for unknown versions, like the reference (perspectivefields.py:127)
         self.version = version
@@ -371,6 +381,10 @@ class PerspectiveFields(nn.Module):
             raise ValueError(f"precision must be 'fp32' or 'bf16', got {precision!r}")
         if precision == "bf16":
             self._options["bf16"] = 1
+        if not (tta is None or (isinstance(tta, str) and tta == "flip")):
+            raise ValueError(f"tta must be None or 'flip', got {tta!r}")
+        if tta == "flip":
+            self._options["flip_tta"] = 1
         self.training = False
         self._pn_params = None      # param_net_parameters(): trainable ParamNet weights, the source of truth once created
         self._pn_synced = None      # (engine serial, training tensors registered, parameter versions) of the last derivation
