@@ -385,6 +385,21 @@ int pf_fit_camera_groups_weighted(int device, const pf_fit_image* images, int n,
                                   const float* lat_base, const uint8_t* mask_base, const float* weight_base, const int64_t* up_weight_offset,
                                   const int64_t* lat_weight_offset, int principal_point, double huber, int max_iterations, double* params,
                                   double* cost, int32_t* iterations, int32_t* status, void* workspace, int64_t workspace_bytes, void* stream);
+/* Camera tracks (DESIGN.md section 1, "Camera tracks"): each group of pf_fit_camera_groups_weighted is one sequence of evenly
+ * spaced frames, in index order.  The grouped fit's parameters, residuals, weights, start and stop rules, with each frame's cost
+ * divided by its residual count M_t and a random-walk prior on neighbouring frames' roll and pitch:
+ *   C_S = sum_t C_t / M_t + 1/2 sum_t ((r_t+1 - r_t) / sigma_roll_deg)^2 + ((e_t+1 - e_t) / sigma_pitch_deg)^2  (angles in radians).
+ * The roll starts are unwrapped along each sequence.  A frame with M_t = 0 is kept (its angles come from the prior, its cost is
+ * 0).  Status 2 (NaN for every frame of the sequence) when the sequence has fewer than 2 + K residuals (K = 1, or 3 with
+ * principal_point), a zero on the shared diagonal, or (one frame) a zero on its roll / pitch diagonal.  cost[i] = frame i's own
+ * C_t; iterations[i], status[i] = the sequence's.  sigma_roll_deg, sigma_pitch_deg: finite and > 0.  workspace: DEVICE, 256-byte
+ * aligned, pf_fit_camera_sequences_workspace bytes.  Every argument is checked before anything is launched (PF_ERR_ARG). */
+int64_t pf_fit_camera_sequences_workspace(const pf_fit_image* images, int n, const int32_t* group_of, int nseq);
+int pf_fit_camera_sequences(int device, const pf_fit_image* images, int n, const int32_t* group_of, int nseq, const float* up_base,
+                            const float* lat_base, const uint8_t* mask_base, const float* weight_base, const int64_t* up_weight_offset,
+                            const int64_t* lat_weight_offset, int principal_point, double huber, int max_iterations, double sigma_roll_deg,
+                            double sigma_pitch_deg, double* params, double* cost, int32_t* iterations, int32_t* status, void* workspace,
+                            int64_t workspace_bytes, void* stream);
 
 /* ---- panorama levelling (csrc/calib.cuh, csrc/equi.cuh) ------------------------------------------------------------------------
  * pf_fit_panorama: the tilt of each panorama from the fields of views cropped from it (DESIGN.md section 1, "Panorama levelling"):
@@ -433,8 +448,11 @@ typedef struct pf_rectify_image {
   int64_t map_offset;               /* floats of the float32 [out_height, out_width, 2] input positions in map_base, or -1 */
 } pf_rectify_image;
 /* PF_RECTIFY_SAME: f_rel * out_height; PF_RECTIFY_VFOV: out_height / (2 tan(vfov / 2)); PF_RECTIFY_FILL: the smallest focal length
- * >= the SAME one that keeps the four canvas corners inside the input (status 1 and the SAME focal length when none can). */
-enum pf_rectify_focal { PF_RECTIFY_SAME = 0, PF_RECTIFY_VFOV = 1, PF_RECTIFY_FILL = 2 };
+ * >= the SAME one that keeps the four canvas corners inside the input (status 1 and the SAME focal length when none can);
+ * PF_RECTIFY_FILL_COMMON: one zoom for the call, f_o * out_height with f_o the largest FILL focal length / out_height over the
+ * images with usable parameters (status 1 where an image's own FILL is impossible; every status-0 canvas is filled).  3 is not a
+ * mode: earlier versions rejected it, and they still do. */
+enum pf_rectify_focal { PF_RECTIFY_SAME = 0, PF_RECTIFY_VFOV = 1, PF_RECTIFY_FILL = 2, PF_RECTIFY_FILL_COMMON = 4 };
 enum pf_rectify_sampler { PF_RECTIFY_BILINEAR = 0, PF_RECTIFY_NEAREST = 1 };
 /* images: HOST array of n (1 .. 65535) descriptors.  params: DEVICE float64 [n, 5] = roll, pitch, general vfov (degrees),
  * cx_rel, cy_rel per image, read on the device (no synchronisation).  fill: HOST int32 [channels] in 0 .. 255, or NULL for 0.

@@ -78,7 +78,7 @@ class pf_rotate_pano(ctypes.Structure):
                 ("map_offset", ctypes.c_int64)]
 
 
-PF_RECTIFY_SAME, PF_RECTIFY_VFOV, PF_RECTIFY_FILL = 0, 1, 2
+PF_RECTIFY_SAME, PF_RECTIFY_VFOV, PF_RECTIFY_FILL, PF_RECTIFY_FILL_COMMON = 0, 1, 2, 4
 PF_RECTIFY_BILINEAR, PF_RECTIFY_NEAREST = 0, 1
 
 PF_EQUI_U8, PF_EQUI_F32 = 0, 1
@@ -248,6 +248,10 @@ def lib():
                                          ctypes.c_double, i32, vp, vp, vp, vp, vp, i64, vp]),
         "pf_fit_camera_groups_weighted": (i32, [i32, ctypes.POINTER(pf_fit_image), i32, ctypes.POINTER(ctypes.c_int32), i32, vp, vp, vp, vp,
                                                 ctypes.POINTER(i64), ctypes.POINTER(i64), i32, ctypes.c_double, i32, vp, vp, vp, vp, vp, i64, vp]),
+        "pf_fit_camera_sequences_workspace": (i64, [ctypes.POINTER(pf_fit_image), i32, ctypes.POINTER(ctypes.c_int32), i32]),
+        "pf_fit_camera_sequences": (i32, [i32, ctypes.POINTER(pf_fit_image), i32, ctypes.POINTER(ctypes.c_int32), i32, vp, vp, vp, vp,
+                                          ctypes.POINTER(i64), ctypes.POINTER(i64), i32, ctypes.c_double, i32, ctypes.c_double, ctypes.c_double,
+                                          vp, vp, vp, vp, vp, i64, vp]),
         "pf_fit_panorama_workspace": (i64, [ctypes.POINTER(pf_fit_image), i32, ctypes.POINTER(ctypes.c_int32), i32]),
         "pf_fit_panorama": (i32, [i32, ctypes.POINTER(pf_fit_image), ctypes.POINTER(pf_pano_crop), i32, ctypes.POINTER(ctypes.c_int32), i32, vp,
                                   vp, vp, vp, ctypes.POINTER(i64), ctypes.POINTER(i64), ctypes.POINTER(ctypes.c_double), ctypes.c_double, i32,
@@ -329,7 +333,8 @@ EXPORTS = ["pf_abi_version", "pf_last_error", "pf_kernel_launch_count", "pf_resi
            "pf_debug_copy", "pf_camera_fields", "pf_camera_fields_vp", "pf_pano_views", "pf_equi_views", "pf_draw_fields",
            "pf_encode_fields", "pf_head_losses_workspace", "pf_head_losses", "pf_field_errors_workspace", "pf_field_errors",
            "pf_fit_camera_workspace", "pf_fit_camera", "pf_fit_camera_groups_workspace", "pf_fit_camera_groups",
-           "pf_fit_camera_weighted", "pf_fit_camera_groups_weighted", "pf_fit_panorama_workspace", "pf_fit_panorama",
+           "pf_fit_camera_weighted", "pf_fit_camera_groups_weighted", "pf_fit_camera_sequences_workspace", "pf_fit_camera_sequences",
+           "pf_fit_panorama_workspace", "pf_fit_panorama",
            "pf_rotate_panoramas_workspace", "pf_rotate_panoramas",
            "pf_rectify_workspace", "pf_rectify_views", "pf_comm_unique_id", "pf_comm_create", "pf_comm_destroy", "pf_gather",
            "pf_jpeg_create", "pf_jpeg_destroy", "pf_jpeg_info", "pf_jpeg_decode_batch",

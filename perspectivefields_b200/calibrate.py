@@ -58,7 +58,20 @@ def _group_ids(groups, n):
     return (ctypes.c_int32 * n)(*(ids[int(v)] for v in labels)), len(ids)
 
 
-def fit_camera(results, principal_point=False, init="fields", mask=None, huber=None, max_iterations=50, groups=None, weights=None):
+def _smoothness(smoothness, groups):
+    """None, or the prior's (sigma_roll, sigma_pitch) in degrees, each finite and > 0."""
+    if smoothness is None:
+        return None
+    if groups is None:
+        raise ValueError("smoothness needs groups: each group is one sequence of frames")
+    pair = tuple(smoothness) if isinstance(smoothness, (tuple, list)) else (smoothness,) * 2
+    if len(pair) != 2 or any(isinstance(v, (bool, np.bool_)) or not isinstance(v, numbers.Real) or not math.isfinite(v) or v <= 0 for v in pair):
+        raise ValueError(f"smoothness must be None, a finite number > 0 or a pair of them (degrees), got {smoothness!r}")
+    return float(pair[0]), float(pair[1])
+
+
+def fit_camera(results, principal_point=False, init="fields", mask=None, huber=None, max_iterations=50, groups=None, weights=None,
+               smoothness=None):
     """Fit one camera per image to ``results[i]["pred_gravity_original"]`` ([2, H, W] up vectors) and
     ``["pred_latitude_original"]`` ([H, W], degrees), read in place; sizes may differ within one call.  A dict of ground-truth
     fields works too, e.g. ``{"pred_gravity_original": up.permute(2, 0, 1), "pred_latitude_original": lat}``.
@@ -84,6 +97,15 @@ def fit_camera(results, principal_point=False, init="fields", mask=None, huber=N
       section 1, "Camera fit").  All-ones weights give the unweighted fit and 0 / 1 weights the fit
       under the matching ``mask``, bit for bit.  Checked on the host, no synchronisation.
 
+    - ``smoothness``: None, or with ``groups`` the prior of a camera track (DESIGN.md section 1, "Camera tracks"): each group is
+      one sequence of evenly spaced video frames, its members in index order.  Intrinsics stay shared; roll and pitch are fitted
+      jointly along the sequence, each frame's cost divided by its number of residuals, plus a random-walk prior that makes a
+      change of sigma degrees between neighbouring frames cost as much as a frame whose fields disagree with its camera by 1
+      degree on average.  sigma is one number for both angles or a pair (sigma_roll, sigma_pitch), each finite and > 0.  A
+      frame without usable residuals is kept: its angles come from its neighbours, and its ``fit_cost`` is 0.  The roll starts
+      are unwrapped along the sequence.  Status 2 applies to the whole sequence (too few residuals, or a shared parameter no
+      residual constrains).
+
     The fields of a model built with ``decode="subbin"`` (continuous, DESIGN.md section 1 "Sub-bin decode") are read as they are:
     nothing here changes for them.
 
@@ -105,6 +127,7 @@ def fit_camera(results, principal_point=False, init="fields", mask=None, huber=N
     n = len(results)
     if mask is not None and len(mask) != n:
         raise ValueError(f"{n} results but {len(mask)} masks")
+    sigma = _smoothness(smoothness, groups)
     group_of = None if groups is None else _group_ids(groups, n)
     if n == 0:
         return []
@@ -128,6 +151,8 @@ def fit_camera(results, principal_point=False, init="fields", mask=None, huber=N
     with torch.cuda.device(dev):
         if group_of is None:
             ws = _batch.workspace(L.pf_fit_camera_workspace(descs, n), dev)
+        elif sigma is not None:
+            ws = _batch.workspace(L.pf_fit_camera_sequences_workspace(descs, n, group_of[0], group_of[1]), dev)
         else:
             ws = _batch.workspace(L.pf_fit_camera_groups_workspace(descs, n, group_of[0], group_of[1]), dev)
         params = torch.empty((n, 5), dtype=torch.float64, device=dev)
@@ -139,6 +164,8 @@ def fit_camera(results, principal_point=False, init="fields", mask=None, huber=N
                   cost.data_ptr(), its.data_ptr(), status.data_ptr(), ws.data_ptr(), ws.numel(), stream)
         if group_of is None:
             _native.check(L.pf_fit_camera_weighted(dev.index, descs, n, *fields))
+        elif sigma is not None:
+            _native.check(L.pf_fit_camera_sequences(dev.index, descs, n, group_of[0], group_of[1], *fields[:9], *sigma, *fields[9:]))
         else:
             _native.check(L.pf_fit_camera_groups_weighted(dev.index, descs, n, group_of[0], group_of[1], *fields))
         roll, pitch, f, cx, cy = params.t()

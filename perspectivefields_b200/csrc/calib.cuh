@@ -485,7 +485,9 @@ __device__ __forceinline__ void fit_block_sum(double (&v)[N], double* sh) {
 struct FitLocal {
   double r00, l10, r11;
   __device__ __forceinline__ bool factor(const double* A, int P, double lambda) {
-    const double b00 = A[0] + lambda * A[0], b01 = A[1], b11 = A[P] + lambda * A[P];
+    return factor2(A[0] + lambda * A[0], A[1], A[P] + lambda * A[P]);
+  }
+  __device__ __forceinline__ bool factor2(double b00, double b01, double b11) {   // B given by its entries
     if (!(b00 > 0.0)) return false;
     r00 = 1.0 / sqrt(b00);
     l10 = b01 * r00;
@@ -686,6 +688,234 @@ __global__ void __launch_bounds__(kFitGroupThreads, 1) fit_group_step_kernel(Fit
     FitState& s = a.st[i];
     s.evals = evals;
     fit_finish<P>(a, i, s, s.status == 2 ? 2 : status);
+  }
+  if (threadIdx.x == 0) { gs.evals = evals; gs.status = status; }
+}
+
+// ------------------------------------------------------------------------------------------------------ camera tracks
+// Sequences of evenly spaced video frames (DESIGN.md section 1, "Camera tracks"): the grouped fit's parameters and residuals,
+// each frame's cost divided by its residual count M_t (fixed: validity does not depend on theta), plus a random-walk prior
+// 1/2 sum_t ((r_t+1 - r_t) / sr)^2 + ((e_t+1 - e_t) / se)^2 on neighbouring frames (the angles in radians, sr and se the numbers
+// given in degrees).  The start is fit_group_init_kernel's, then fit_seq_init_kernel unwraps the roll starts along each
+// sequence; the pass and fit_reduce_kernel are reused, and fit_seq_step_kernel takes one Levenberg-Marquardt step per sequence.
+// A frame's FitState keeps its own C_t (unscaled), theta, and A / M_t, g / M_t at the accepted point (zero when M_t = 0).
+constexpr int kFitSeqRow = 22;   // per-frame workspace doubles: B (3), E (2 K), g_l (2), the pivot's factor (3), z (2 (K + 1))
+
+struct FitSeqs {
+  FitGroups g;                   // the sequences as groups: members in frame order, state, each frame's sums
+  double* work;                  // [n][kFitSeqRow], row j for the member at position j of g.mem
+  double wr, we;                 // prior weights 1 / sr^2, 1 / se^2
+};
+
+// One thread per sequence: each roll start moved by a multiple of 2 pi to within pi of its (moved) predecessor's
+__global__ void __launch_bounds__(128) fit_seq_init_kernel(FitArgs a, FitSeqs q) {
+  pdl_wait();
+  pdl_launch();
+  const int G = blockIdx.x * blockDim.x + threadIdx.x;
+  if (G >= q.g.ngroups) return;
+  double prev = a.st[q.g.mem[q.g.off[G]]].theta[0];
+  for (int j = q.g.off[G] + 1; j < q.g.off[G + 1]; ++j) {
+    FitState& s = a.st[q.g.mem[j]];
+    const double r = s.theta[0] - 2.0 * kPi * rint((s.theta[0] - prev) / (2.0 * kPi));
+    s.theta[0] = s.cand[0] = r;
+    prev = r;
+  }
+}
+
+// One block per sequence.  Accept or reject the candidate on C_S, then solve (A + lambda diag A) delta = -g: the locals form a
+// block-tridiagonal matrix T (diagonal blocks A_t[ll] / M_t + the prior's W = diag(wr, we) once per neighbour, off-diagonal
+// blocks -W), eliminated from the K shared unknowns by a Schur complement.  The block threads prepare each frame's row (B_t,
+// E_t = A_t[ls] / M_t, g_l,t with the prior's gradient) and the fixed-order block sums D and g_s; thread 0 then runs the block
+// LDL^T recursion along the chain with K + 1 right-hand sides (g_l, E):
+//   P_0 = B_0,  P_t = B_t - W P_t-1^-1 W,  z_t = rhs_t + W P_t-1^-1 z_t-1,  rhs^T T^-1 rhs' = sum_t z_t^T P_t^-1 z'_t,
+// solves S ds = b with S = D_lambda - E^T T^-1 E, b = -g_s + E^T T^-1 g_l, and sweeps back dl_t = P_t^-1 (z'_t + W dl_t+1)
+// with z'_t = -z_g,t - Z_t ds.
+template <int P>
+__global__ void __launch_bounds__(kFitGroupThreads, 1) fit_seq_step_kernel(FitArgs a, FitSeqs q) {
+  constexpr int K = P - 2, NK = K * (K + 1) / 2, NA = P * (P + 1) / 2;
+  constexpr int RB = 0, RE = 3, RG = 3 + 2 * K, RF = 5 + 2 * K, RZ = 8 + 2 * K;   // row offsets
+  static_assert(RZ + 2 * (K + 1) <= kFitSeqRow, "row too short");
+  constexpr int NC = 2 + K, NS = NK + K, NSH = NC > NS ? NC : NS;   // the two block sums' widths, the scratch's
+  __shared__ double shr[kFitGroupThreads / 32 * NSH];
+  __shared__ int sh_status;
+  pdl_wait();
+  pdl_launch();
+  const FitGroups& g = q.g;
+  FitGroupState& gs = g.gs[blockIdx.x];
+  if (gs.status != kFitRunning) return;
+  const int m0 = g.off[blockIdx.x], m1 = g.off[blockIdx.x + 1], m = m1 - m0;
+  const int evals = gs.evals + 1;
+  const double wr = q.wr, we = q.we;
+  double lambda = gs.lambda, C = gs.C, th[K], cs[K];
+#pragma unroll
+  for (int c = 0; c < K; ++c) { th[c] = gs.shared[c]; cs[c] = gs.cand[c]; }
+  auto accept = [&](FitState& s, const double* v) {   // v: the frame's sums
+    const double M = v[1];
+    s.C = 0.5 * v[0];
+#pragma unroll
+    for (int k = 0; k < P; ++k) { s.theta[k] = s.cand[k]; s.g[k] = M > 0.0 ? v[2 + k] / M : 0.0; }
+#pragma unroll
+    for (int k = 0; k < NA; ++k) s.A[k] = M > 0.0 ? v[2 + P + k] / M : 0.0;
+  };
+  const int status = [&]() -> int {
+    // C_S at the candidate: sum C_t / M_t, plus the prior on the pair (t, t + 1) by the thread of t; at the start also the
+    // residual count and D's diagonal
+    double r[NC] = {};
+    for (int j = m0 + (int)threadIdx.x; j < m1; j += blockDim.x) {
+      const double* v = g.sums + (long long)g.mem[j] * kFitQ;
+      const double M = v[1];
+      if (M > 0.0) r[0] += 0.5 * v[0] / M;
+      if (j + 1 < m1) {
+        const double dr = a.st[g.mem[j + 1]].cand[0] - a.st[g.mem[j]].cand[0], de = a.st[g.mem[j + 1]].cand[1] - a.st[g.mem[j]].cand[1];
+        r[0] += 0.5 * (dr * dr * wr + de * de * we);
+      }
+      if (evals == 1) {
+        r[1] += M;
+#pragma unroll
+        for (int c = 0; c < K; ++c) r[2 + c] += M > 0.0 ? v[2 + P + fit_up(P, 2 + c, 2 + c)] / M : 0.0;
+      }
+    }
+    static_assert(NC <= NSH, "scratch too small for the cost sum");
+    fit_block_sum<NC>(r, shr);
+    bool acc = true, done = false;
+    if (evals == 1) {   // the start
+      bool bad = r[1] < 2.0 + K;
+#pragma unroll
+      for (int c = 0; c < K; ++c) bad = bad || r[2 + c] == 0.0;
+      if (m == 1) {
+        const double* v = g.sums + (long long)g.mem[m0] * kFitQ;
+        bad = bad || v[2 + P + fit_up(P, 0, 0)] == 0.0 || v[2 + P + fit_up(P, 1, 1)] == 0.0;
+      }
+      if (bad) return 2;
+      C = r[0];
+    } else if (r[0] < C) {   // accept
+      done = C - r[0] <= kFitCostRtol * C;
+      C = r[0];
+#pragma unroll
+      for (int c = 0; c < K; ++c) th[c] = cs[c];
+      lambda /= 10.0;
+    } else {                 // reject: keep theta, A, g
+      acc = false;
+      lambda *= 10.0;
+      if (lambda > kFitLambdaMax) return 0;
+    }
+    if (acc)
+      for (int j = m0 + (int)threadIdx.x; j < m1; j += blockDim.x) accept(a.st[g.mem[j]], g.sums + (long long)g.mem[j] * kFitQ);
+    if (done) return 0;
+    __syncthreads();   // every frame's accepted theta before the prior's gradient reads its neighbours'
+    // each frame's row, and the sums D (upper triangle) and g_s
+    double r2[NS] = {};
+    for (int j = m0 + (int)threadIdx.x; j < m1; j += blockDim.x) {
+      const FitState& s = a.st[g.mem[j]];
+      double* row = q.work + (long long)j * kFitSeqRow;
+      const double nb = (double)((j > m0) + (j + 1 < m1));
+      double gl0 = s.g[0], gl1 = s.g[1];
+      if (j > m0) { const FitState& o = a.st[g.mem[j - 1]]; gl0 += wr * (s.theta[0] - o.theta[0]); gl1 += we * (s.theta[1] - o.theta[1]); }
+      if (j + 1 < m1) { const FitState& o = a.st[g.mem[j + 1]]; gl0 += wr * (s.theta[0] - o.theta[0]); gl1 += we * (s.theta[1] - o.theta[1]); }
+      row[RB] = s.A[fit_up(P, 0, 0)] + nb * wr; row[RB + 1] = s.A[fit_up(P, 0, 1)]; row[RB + 2] = s.A[fit_up(P, 1, 1)] + nb * we;
+#pragma unroll
+      for (int c = 0; c < K; ++c) { row[RE + c] = s.A[fit_up(P, 0, 2 + c)]; row[RE + K + c] = s.A[fit_up(P, 1, 2 + c)]; }
+      row[RG] = gl0; row[RG + 1] = gl1;
+#pragma unroll
+      for (int c = 0, k = 0; c < K; ++c) {
+        r2[NK + c] += s.g[2 + c];
+#pragma unroll
+        for (int e = c; e < K; ++e, ++k) r2[k] += s.A[fit_up(P, 2 + c, 2 + e)];
+      }
+    }
+    static_assert(NS <= NSH, "scratch too small for the D and g_s sums");
+    fit_block_sum<NS>(r2, shr);   // (its first barrier also orders the rows before thread 0 reads them)
+    if (threadIdx.x == 0) {
+      int st = kFitRunning;
+      double ds[K];
+      bool ok = false;
+      while (lambda <= kFitLambdaMax) {
+        double S[NK], b[K], up[2][K + 1];
+        for (int k = 0; k < NK; ++k) S[k] = 0.0;
+        for (int c = 0; c < K; ++c) b[c] = 0.0;
+        FitLocal Pp{}, Pt{};
+        bool pd = true;
+        for (int t = 0; t < m && pd; ++t) {   // forward: factor P_t, z_t, u_t = P_t^-1 z_t
+          double* row = q.work + (long long)(m0 + t) * kFitSeqRow;
+          double b00 = row[RB] + lambda * row[RB], b01 = row[RB + 1], b11 = row[RB + 2] + lambda * row[RB + 2];
+          double z[2][K + 1];
+          z[0][0] = row[RG]; z[1][0] = row[RG + 1];
+#pragma unroll
+          for (int c = 0; c < K; ++c) { z[0][1 + c] = row[RE + c]; z[1][1 + c] = row[RE + K + c]; }
+          if (t > 0) {
+            double x0, x1, y0, y1;
+            Pp.solve(wr, 0.0, x0, x1);   // P_t-1^-1 W, column by column
+            Pp.solve(0.0, we, y0, y1);
+            b00 -= wr * x0; b01 -= wr * y0; b11 -= we * y1;
+#pragma unroll
+            for (int k = 0; k <= K; ++k) { z[0][k] += wr * up[0][k]; z[1][k] += we * up[1][k]; }
+          }
+          if (!(pd = Pt.factor2(b00, b01, b11))) break;
+#pragma unroll
+          for (int k = 0; k <= K; ++k) Pt.solve(z[0][k], z[1][k], up[0][k], up[1][k]);
+#pragma unroll
+          for (int c = 0, k = 0; c < K; ++c) {
+            b[c] += z[0][1 + c] * up[0][0] + z[1][1 + c] * up[1][0];
+#pragma unroll
+            for (int e = c; e < K; ++e, ++k) S[k] += z[0][1 + c] * up[0][1 + e] + z[1][1 + c] * up[1][1 + e];
+          }
+          row[RF] = Pt.r00; row[RF + 1] = Pt.l10; row[RF + 2] = Pt.r11;
+#pragma unroll
+          for (int k = 0; k <= K; ++k) { row[RZ + k] = z[0][k]; row[RZ + K + 1 + k] = z[1][k]; }
+          Pp = Pt;
+        }
+        if (pd) {
+#pragma unroll
+          for (int c = 0, k = 0; c < K; ++c) {
+            b[c] = -r2[NK + c] + b[c];
+#pragma unroll
+            for (int e = c; e < K; ++e, ++k) S[k] = (e == c ? r2[k] + lambda * r2[k] : r2[k]) - S[k];
+          }
+          if ((ok = cholesky_solve<K>(S, b, ds))) break;
+        }
+        lambda *= 10.0;
+      }
+      if (!ok) {
+        st = 0;
+      } else {
+        bool small = true;
+#pragma unroll
+        for (int c = 0; c < K; ++c) small = small && fabs(ds[c]) <= kFitStepRtol * (1.0 + fabs(th[c]));
+        double n0 = 0.0, n1 = 0.0;   // W dl_t+1
+        for (int t = m - 1; t >= 0; --t) {   // backward: dl_t, the candidate
+          const double* row = q.work + (long long)(m0 + t) * kFitSeqRow;
+          FitLocal Pf;
+          Pf.r00 = row[RF]; Pf.l10 = row[RF + 1]; Pf.r11 = row[RF + 2];
+          double z0 = -row[RZ] + n0, z1 = -row[RZ + K + 1] + n1, x0, x1;
+#pragma unroll
+          for (int c = 0; c < K; ++c) { z0 -= row[RZ + 1 + c] * ds[c]; z1 -= row[RZ + K + 2 + c] * ds[c]; }
+          Pf.solve(z0, z1, x0, x1);
+          FitState& s = a.st[g.mem[m0 + t]];
+          small = small && fabs(x0) <= kFitStepRtol * (1.0 + fabs(s.theta[0])) && fabs(x1) <= kFitStepRtol * (1.0 + fabs(s.theta[1]));
+          s.cand[0] = s.theta[0] + x0; s.cand[1] = s.theta[1] + x1;
+#pragma unroll
+          for (int c = 0; c < K; ++c) s.cand[2 + c] = th[c] + ds[c];
+          n0 = wr * x0; n1 = we * x1;
+        }
+        if (small) st = 0;
+        else if (evals >= a.max_iter) st = 1;
+        else {
+#pragma unroll
+          for (int c = 0; c < K; ++c) { gs.shared[c] = th[c]; gs.cand[c] = th[c] + ds[c]; }
+          gs.C = C; gs.lambda = lambda; gs.evals = evals;
+        }
+      }
+      sh_status = st;
+    }
+    __syncthreads();
+    return sh_status;
+  }();
+  if (status == kFitRunning) return;
+  for (int j = m0 + (int)threadIdx.x; j < m1; j += blockDim.x) {   // finish every frame
+    const int i = g.mem[j];
+    FitState& s = a.st[i];
+    s.evals = evals;
+    fit_finish<P>(a, i, s, status);
   }
   if (threadIdx.x == 0) { gs.evals = evals; gs.status = status; }
 }

@@ -420,17 +420,17 @@ int64_t pf_fit_camera_workspace(const pf_fit_image* images, int n) {
 
 // The groups in CSR form: csr[0 .. ngroups] member offsets, then the members of each group in index order
 static int fit_groups_layout(const pf_fit_image* im, int n, const int32_t* group_of, int ngroups, WsLayout* lay, long long* blocks_out = nullptr,
-                             std::vector<int>* csr = nullptr) {
-  TRY(fit_layout("pf_fit_camera_groups", im, n, lay, blocks_out));
-  if (!group_of || ngroups < 1) return fail(PF_ERR_ARG, "pf_fit_camera_groups: null group_of or ngroups < 1");
+                             std::vector<int>* csr = nullptr, const char* fn = "pf_fit_camera_groups") {
+  TRY(fit_layout(fn, im, n, lay, blocks_out));
+  if (!group_of || ngroups < 1) return fail(PF_ERR_ARG, "%s: null group_of or ngroups < 1", fn);
   std::vector<int> off(ngroups + 1, 0);
   for (int i = 0; i < n; ++i) {
     if (group_of[i] < 0 || group_of[i] >= ngroups)
-      return fail(PF_ERR_ARG, "pf_fit_camera_groups: image %d has group %d outside 0 .. %d", i, group_of[i], ngroups - 1);
+      return fail(PF_ERR_ARG, "%s: image %d has group %d outside 0 .. %d", fn, i, group_of[i], ngroups - 1);
     off[group_of[i] + 1] += 1;
   }
   for (int G = 0; G < ngroups; ++G) {
-    if (off[G + 1] == 0) return fail(PF_ERR_ARG, "pf_fit_camera_groups: group %d has no image", G);
+    if (off[G + 1] == 0) return fail(PF_ERR_ARG, "%s: group %d has no image", fn, G);
     off[G + 1] += off[G];
   }
   lay->add((long long)ngroups * sizeof(FitGroupState)).add((long long)n * kFitQ * 8).add((long long)(ngroups + 1 + n) * 4);
@@ -590,6 +590,71 @@ int pf_fit_camera_groups_weighted(int device, const pf_fit_image* images, int n,
       LAUNCHED(fit_pass_launch(0, weighted, pass_grid, st, a));
       LAUNCHED(launch_pdl(fit_reduce_kernel<3>, reduce_grid, dim3(32 * kFitStepWarps), 0, st, a, g));
       LAUNCHED(launch_pdl(fit_group_step_kernel<3>, group_grid, dim3(kFitGroupThreads), 0, st, a, g));
+    }
+  }
+  return PF_OK;
+}
+
+// ----------------------------------------------------------------------------------------------- camera tracks
+// Workspace layout of pf_fit_camera_sequences: pf_fit_camera_groups' | per-frame rows [n][kFitSeqRow] (float64)
+static int fit_seq_layout(const pf_fit_image* im, int n, const int32_t* group_of, int nseq, WsLayout* lay, long long* blocks_out = nullptr,
+                          std::vector<int>* csr = nullptr) {
+  TRY(fit_groups_layout(im, n, group_of, nseq, lay, blocks_out, csr, "pf_fit_camera_sequences"));
+  lay->add((long long)n * kFitSeqRow * 8);
+  return PF_OK;
+}
+int64_t pf_fit_camera_sequences_workspace(const pf_fit_image* images, int n, const int32_t* group_of, int nseq) {
+  WsLayout lay;
+  TRY(fit_seq_layout(images, n, group_of, nseq, &lay));
+  return lay.total;
+}
+
+int pf_fit_camera_sequences(int device, const pf_fit_image* images, int n, const int32_t* group_of, int nseq, const float* up_base,
+                            const float* lat_base, const uint8_t* mask_base, const float* weight_base, const int64_t* up_weight_offset,
+                            const int64_t* lat_weight_offset, int principal_point, double huber, int max_iterations, double sigma_roll_deg,
+                            double sigma_pitch_deg, double* params, double* cost, int32_t* iterations, int32_t* status, void* workspace,
+                            int64_t workspace_bytes, void* stream) {
+  const char* fn = "pf_fit_camera_sequences";
+  WsLayout lay;
+  long long blocks;
+  std::vector<int> csr;
+  TRY(fit_seq_layout(images, n, group_of, nseq, &lay, &blocks, &csr));
+  if (!(std::isfinite(sigma_roll_deg) && sigma_roll_deg > 0.0 && std::isfinite(sigma_pitch_deg) && sigma_pitch_deg > 0.0))
+    return fail(PF_ERR_ARG, "%s: sigma_roll_deg %g and sigma_pitch_deg %g must be finite and > 0", fn, sigma_roll_deg, sigma_pitch_deg);
+  std::vector<FitImage> d;
+  FitArgs a;
+  bool weighted;
+  TRY(fit_prepare(fn, lay, blocks, images, n, up_base, lat_base, mask_base, weight_base, up_weight_offset, lat_weight_offset,
+                  principal_point, huber, max_iterations, params, cost, iterations, status, workspace, workspace_bytes, &d, &a, &weighted));
+  CU(cudaSetDevice(device));
+  cudaStream_t st = (cudaStream_t)stream;
+  char* ws = (char*)workspace;
+  FitSeqs q{};
+  q.g.gs = (FitGroupState*)(ws + lay.at[3]);
+  q.g.sums = (double*)(ws + lay.at[4]);
+  q.g.off = (const int*)(ws + lay.at[5]);
+  q.g.mem = q.g.off + nseq + 1;
+  q.g.ngroups = nseq;
+  q.work = (double*)(ws + lay.at[6]);
+  q.wr = 1.0 / (sigma_roll_deg * sigma_roll_deg);
+  q.we = 1.0 / (sigma_pitch_deg * sigma_pitch_deg);
+  TRY(upload_descriptors(d.data(), d.size() * sizeof(d[0]), ws, st));
+  CU(cudaMemcpyAsync(ws + lay.at[5], csr.data(), csr.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  const PdlScope pdl(!sync_debug());
+  const dim3 pass_grid((unsigned)blocks), reduce_grid((unsigned)cdiv(n, kFitStepWarps)), seq_grid((unsigned)nseq);
+  const dim3 init_grid((unsigned)cdiv(nseq, 128));
+  LAUNCHED(launch_pdl(fit_init_kernel, dim3(n), dim3(64), 0, st, a, principal_point));
+  LAUNCHED(launch_pdl(fit_group_init_kernel, init_grid, dim3(128), 0, st, a, q.g));
+  LAUNCHED(launch_pdl(fit_seq_init_kernel, init_grid, dim3(128), 0, st, a, q));
+  for (int it = 0; it < max_iterations; ++it) {
+    if (principal_point) {
+      LAUNCHED(fit_pass_launch(1, weighted, pass_grid, st, a));
+      LAUNCHED(launch_pdl(fit_reduce_kernel<5>, reduce_grid, dim3(32 * kFitStepWarps), 0, st, a, q.g));
+      LAUNCHED(launch_pdl(fit_seq_step_kernel<5>, seq_grid, dim3(kFitGroupThreads), 0, st, a, q));
+    } else {
+      LAUNCHED(fit_pass_launch(0, weighted, pass_grid, st, a));
+      LAUNCHED(launch_pdl(fit_reduce_kernel<3>, reduce_grid, dim3(32 * kFitStepWarps), 0, st, a, q.g));
+      LAUNCHED(launch_pdl(fit_seq_step_kernel<3>, seq_grid, dim3(kFitGroupThreads), 0, st, a, q));
     }
   }
   return PF_OK;
@@ -777,7 +842,7 @@ int pf_rectify_views(int device, const pf_rectify_image* images, int n, const ui
     return fail(PF_ERR_ARG, "pf_rectify_views: null input / output / params / camera / status / workspace");
   if (channels != 1 && channels != 3) return fail(PF_ERR_ARG, "pf_rectify_views: %d channels (1 or 3)", channels);
   if (keep_pitch != 0 && keep_pitch != 1) return fail(PF_ERR_ARG, "pf_rectify_views: keep_pitch must be 0 or 1");
-  if (focal_mode != PF_RECTIFY_SAME && focal_mode != PF_RECTIFY_VFOV && focal_mode != PF_RECTIFY_FILL)
+  if (focal_mode != PF_RECTIFY_SAME && focal_mode != PF_RECTIFY_VFOV && focal_mode != PF_RECTIFY_FILL && focal_mode != PF_RECTIFY_FILL_COMMON)
     return fail(PF_ERR_ARG, "pf_rectify_views: unknown focal mode %d", focal_mode);
   if (focal_mode == PF_RECTIFY_VFOV && !(std::isfinite(vfov) && vfov > 0.0 && vfov < 180.0))
     return fail(PF_ERR_ARG, "pf_rectify_views: vfov %g must lie in (0, 180) degrees", vfov);
@@ -810,7 +875,10 @@ int pf_rectify_views(int device, const pf_rectify_image* images, int n, const ui
   for (int c = 0; c < 3; ++c) a.fill[c] = fv[c];
   TRY(upload_descriptors(d.data(), d.size() * sizeof(d[0]), ws, st));
   const PdlScope pdl(!sync_debug());
-  LAUNCHED(launch_pdl(rectify_setup_kernel, dim3((unsigned)cdiv(n, 128)), dim3(128), 0, st, a));
+  if (focal_mode == PF_RECTIFY_FILL_COMMON)
+    LAUNCHED(launch_pdl(rectify_setup_common_kernel, dim3(1), dim3(kRectCommonThreads), 0, st, a));
+  else
+    LAUNCHED(launch_pdl(rectify_setup_kernel, dim3((unsigned)cdiv(n, 128)), dim3(128), 0, st, a));
   const dim3 grid((unsigned)cdivl(max_px, (long long)kRectThreads * kRectPix), (unsigned)n);
   const bool nearest = sampler == PF_RECTIFY_NEAREST;
   if (channels == 3)

@@ -11,7 +11,8 @@
 //
 // Two kernels, chained with programmatic dependent launch and enqueued without synchronisation: rectify_setup_kernel (one thread
 // per image: parameters from device memory -> status, output camera, M) and rectify_warp_kernel (every output pixel of every image,
-// grid.y = image).
+// grid.y = image).  "fill_common" (one zoom for the whole call: the largest "fill" F_o / H_o of the usable images, times each H_o)
+// replaces the setup by rectify_setup_common_kernel, one block that reduces the zoom and then writes every image's setup.
 #pragma once
 #include <math.h>
 #include <stdint.h>
@@ -21,6 +22,7 @@
 namespace pf {
 
 constexpr int kRectFocalSame = 0, kRectFocalVfov = 1, kRectFocalFill = 2;
+constexpr int kRectCommonThreads = 256;
 constexpr int kRectThreads = 256, kRectPix = 4;   // 4 consecutive output pixels (of the image's flat H_o * W_o range) per thread
 constexpr double kRectPi = 3.14159265358979323846;
 
@@ -64,11 +66,10 @@ __device__ __forceinline__ double rect_focal_rel(double cx, double cy, double gv
 }
 
 // ------------------------------------------------------------------------------------------------------------ setup
-__global__ void __launch_bounds__(128) rectify_setup_kernel(RectArgs a) {
-  pdl_wait();      // params may come from the previous kernel on the stream (e.g. the camera fit)
-  pdl_launch();
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= a.n) return;
+// Image i's setup.  kFillZoom: return its "fill" F_o / H_o (0 when its parameters are unusable) and write nothing.  kCommon: write it
+// at F_o = fo_rel H_o, with the status of its own "fill" focal length.  Neither: the focal mode's F_o.
+template <bool kFillZoom = false, bool kCommon = false>
+__device__ __forceinline__ double rect_setup_image(const RectArgs& a, int i, double fo_rel = 0.0) {
   const RectImage d = a.im[i];
   const double* p = a.params + 5LL * i;
   const double roll = p[0], pitch = p[1], gv = p[2], cxr = p[3], cyr = p[4];
@@ -80,11 +81,12 @@ __global__ void __launch_bounds__(128) rectify_setup_kernel(RectArgs a) {
   RectMap& mp = a.map[i];
   double* cam = a.camera + 5LL * i;
   if (!ok) {
+    if constexpr (kFillZoom) return 0.0;
     for (int k = 0; k < 9; ++k) mp.m[k] = NAN;
     mp.ok = 0;
     for (int k = 0; k < 5; ++k) cam[k] = NAN;
     a.status[i] = 2;
-    return;
+    return 0.0;
   }
   const double H = d.H, W = d.W, Ho = d.Ho, Wo = d.Wo;
   const double F = f * H, cx = (cxr + 0.5) * W, cy = (cyr + 0.5) * H;
@@ -99,9 +101,9 @@ __global__ void __launch_bounds__(128) rectify_setup_kernel(RectArgs a) {
   const double Fs = f * Ho;
   double Fo = Fs;
   int status = 0;
-  if (a.focal_mode == kRectFocalVfov) {
+  if (a.focal_mode == kRectFocalVfov && !kFillZoom && !kCommon) {
     Fo = Ho / (2.0 * tan(a.vfov * d2r / 2.0));
-  } else if (a.focal_mode == kRectFocalFill) {
+  } else if (a.focal_mode == kRectFocalFill || kFillZoom || kCommon) {
     // the input rectangle as four half-spaces n_k . c >= 0 of input rays; a canvas corner (a, b) relative to the centre has the
     // ray p + t q with p = R (0, 0, 1), q = R (a, b, 0), t = 1 / F_o
     const double nrm[4][3] = {{F, 0.0, cx}, {-F, 0.0, W - cx}, {0.0, F, cy}, {0.0, -F, H - cy}};
@@ -123,6 +125,8 @@ __global__ void __launch_bounds__(128) rectify_setup_kernel(RectArgs a) {
     if (!inside) status = 1;
     else if (tmax < INFINITY) Fo = fmax(Fs, 1.0 / tmax);
   }
+  if constexpr (kFillZoom) return Fo / Ho;
+  if constexpr (kCommon) Fo = fo_rel * Ho;
   // M = K R K_o^-1 with K = [[F, 0, cx], [0, F, cy], [0, 0, 1]], K_o^-1 = [[1/Fo, 0, -Wo/(2Fo)], [0, 1/Fo, -Ho/(2Fo)], [0, 0, 1]]
   double KR[9];
 #pragma unroll
@@ -145,6 +149,33 @@ __global__ void __launch_bounds__(128) rectify_setup_kernel(RectArgs a) {
   cam[3] = 0.0;
   cam[4] = 0.0;
   a.status[i] = status;
+  return Fo / Ho;
+}
+
+// One thread per image: "same", a vfov, or "fill"
+__global__ void __launch_bounds__(128) rectify_setup_kernel(RectArgs a) {
+  pdl_wait();      // params may come from the previous kernel on the stream (e.g. the camera fit)
+  pdl_launch();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= a.n) return;
+  rect_setup_image(a, i);
+}
+
+// "fill_common", one block for the whole call: f_o = the largest "fill" F_o / H_o of the usable images (a maximum: the same bits
+// in any order), then every image written at F_o = f_o H_o with its own "fill" status.  A larger focal length keeps a filled
+// canvas filled, since every corner constraint has the form t <= bound.
+__global__ void __launch_bounds__(kRectCommonThreads) rectify_setup_common_kernel(RectArgs a) {
+  __shared__ double shm[kRectCommonThreads / 32];
+  pdl_wait();
+  pdl_launch();
+  double fo = 0.0;
+  for (int i = threadIdx.x; i < a.n; i += blockDim.x) fo = fmax(fo, rect_setup_image<true>(a, i));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) fo = fmax(fo, __shfl_xor_sync(0xffffffffu, fo, o));
+  if ((threadIdx.x & 31) == 0) shm[threadIdx.x >> 5] = fo;
+  __syncthreads();
+  for (int w = 0; w < kRectCommonThreads / 32; ++w) fo = fmax(fo, shm[w]);
+  for (int i = threadIdx.x; i < a.n; i += blockDim.x) rect_setup_image<false, true>(a, i, fo);
 }
 
 // ------------------------------------------------------------------------------------------------------------ warp

@@ -145,8 +145,11 @@ def upright(images, cameras, keep_pitch=False, focal="same", size=None, mode="bi
 
     - ``keep_pitch``: False (roll 0 and pitch 0: vertical lines stay vertical) or True (roll 0 only: an in-plane rotation about
       the principal point that levels the horizon).
-    - ``focal``: "same" (f_rel of the input times the output height), a vertical field of view in degrees, or "fill" (the
-      smallest zoom at or above "same" that leaves no fill in the canvas; "same" and status 1 where no zoom can).
+    - ``focal``: "same" (f_rel of the input times the output height), a vertical field of view in degrees, "fill" (the
+      smallest zoom at or above "same" that leaves no fill in the canvas; "same" and status 1 where no zoom can), or
+      "fill_common" (one zoom for the whole call, e.g. the frames of a clip: the largest "fill" f_rel of the images with usable
+      parameters, times each output height; every status-0 canvas is filled, and status 1 marks images whose own "fill" was
+      impossible).  Read from the device cameras without synchronising.
     - ``size``: None (each input's size), one (H, W) for all, or one per image.
     - ``mode``: "bilinear" (rounded to nearest) or "nearest" (for masks and label images).  No antialiasing: a focal length that
       shrinks an image strongly aliases.
@@ -164,12 +167,13 @@ def upright(images, cameras, keep_pitch=False, focal="same", size=None, mode="bi
         raise TypeError(f"keep_pitch must be a bool, got {keep_pitch!r}")
     vfov = 0.0
     if isinstance(focal, str):
-        if focal not in ("same", "fill"):
-            raise ValueError(f"focal must be 'same', 'fill' or a vfov in degrees, got {focal!r}")
-        focal_mode = _native.PF_RECTIFY_SAME if focal == "same" else _native.PF_RECTIFY_FILL
+        modes = {"same": _native.PF_RECTIFY_SAME, "fill": _native.PF_RECTIFY_FILL, "fill_common": _native.PF_RECTIFY_FILL_COMMON}
+        if focal not in modes:
+            raise ValueError(f"focal must be 'same', 'fill', 'fill_common' or a vfov in degrees, got {focal!r}")
+        focal_mode = modes[focal]
     else:
         if not _real_number(focal) or not 0.0 < float(focal) < 180.0:
-            raise ValueError(f"focal must be 'same', 'fill' or a vfov in (0, 180) degrees, got {focal!r}")
+            raise ValueError(f"focal must be 'same', 'fill', 'fill_common' or a vfov in (0, 180) degrees, got {focal!r}")
         focal_mode, vfov = _native.PF_RECTIFY_VFOV, float(focal)
     if mode not in MODES:
         raise ValueError(f"mode must be one of {tuple(MODES)}, got {mode!r}")
