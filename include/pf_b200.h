@@ -310,7 +310,8 @@ int pf_encode_fields(int device, int n, int H, int W, const float* up, const int
  *   classification (>= 3 / >= 2): logits float32 [n, C, H, W] (16-byte aligned, H * W % 4 == 0), labels int64 [n, H, W] ->
  *     losses[2] = loss_gravity, loss_latitude (cross-entropy, mean over the labels that are not the head's ignore value).
  * Every value is multiplied by its head's weight.  A mean over no pixel is NaN, and so is a cross-entropy with a label outside
- * [0, C) that is not the ignore value.  workspace: DEVICE, 256-byte aligned, pf_head_losses_workspace bytes. */
+ * [0, C) that is not the ignore value.  H * W must stay below 2^31.  workspace: DEVICE, 256-byte aligned,
+ * pf_head_losses_workspace bytes. */
 int64_t pf_head_losses_workspace(int n, int H, int W, int gravity_classes, int latitude_classes);
 int pf_head_losses(int device, int n, int H, int W, int gravity_classes, const float* pred_gravity, const void* gt_gravity, int latitude_classes,
                    const float* pred_latitude, const void* gt_latitude, int gravity_ignore, int latitude_ignore, float gravity_weight,

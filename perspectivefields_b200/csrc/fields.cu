@@ -277,7 +277,8 @@ static void loss_blocks(int n, int H, int W, int gc, long long* bg, long long* b
   else { *bg = cdivl(px / kCePix, kMetThreads); *bl = *bg; }
 }
 int64_t pf_head_losses_workspace(int n, int H, int W, int gravity_classes, int latitude_classes) {
-  if (n < 1 || H < 1 || W < 1) return fail(PF_ERR_ARG, "pf_head_losses_workspace: bad batch %d x %d x %d", n, H, W);
+  if (n < 1 || H < 1 || W < 1 || (long long)H * W >= (1LL << 31))
+    return fail(PF_ERR_ARG, "pf_head_losses_workspace: bad batch %d x %d x %d (H * W must stay below 2^31)", n, H, W);
   if (!((gravity_classes == 2 && latitude_classes == 1) || (gravity_classes >= 3 && latitude_classes >= 2)))
     return fail(PF_ERR_ARG, "pf_head_losses_workspace: heads %d / %d: both regression (2 / 1) or both classification", gravity_classes, latitude_classes);
   long long bg, bl;
@@ -302,19 +303,19 @@ int pf_head_losses(int device, int n, int H, int W, int gravity_classes, const f
   long long bg, bl;
   loss_blocks(n, H, W, gravity_classes, &bg, &bl);
   double* psum = (double*)workspace;
-  const int HW = H * W;
+  const long long HW = (long long)H * W;   // < 2^31 (pf_head_losses_workspace)
   if (cls) {
     long long* pcnt = (long long*)((char*)workspace + align256((bg + bl) * 8));
     const CeHead g{pred_gravity, (const long long*)gt_gravity, gravity_classes, gravity_ignore, (int)bg};
     const CeHead l{pred_latitude, (const long long*)gt_latitude, latitude_classes, latitude_ignore, (int)bl};
-    LAUNCHED((cross_entropy_kernel<<<(unsigned)(bg + bl), kMetThreads, 0, st>>>(g, l, n, HW, psum, pcnt), cudaGetLastError()));
+    LAUNCHED((cross_entropy_kernel<<<(unsigned)(bg + bl), kMetThreads, 0, st>>>(g, l, n, (int)HW, psum, pcnt), cudaGetLastError()));
     LAUNCHED((loss_finish_kernel<<<1, kMetThreads, 0, st>>>(0, (int)bg, (int)(bg + bl), psum, pcnt, 0, gravity_weight, latitude_weight, losses),
               cudaGetLastError()));
   } else {
     long long* pcnt = (long long*)((char*)workspace + align256(bg * kRegSums * 8));
     const RegArgs a{pred_gravity, (const float*)gt_gravity, pred_latitude, (const float*)gt_latitude, n, H, W};
     LAUNCHED((regression_loss_kernel<<<(unsigned)bg, kMetThreads, 0, st>>>(a, (int)bg, psum, pcnt), cudaGetLastError()));
-    LAUNCHED((loss_finish_kernel<<<1, kMetThreads, 0, st>>>(1, (int)bg, (int)bg, psum, pcnt, (long long)n * HW, gravity_weight, latitude_weight, losses),
+    LAUNCHED((loss_finish_kernel<<<1, kMetThreads, 0, st>>>(1, (int)bg, (int)bg, psum, pcnt, n * HW, gravity_weight, latitude_weight, losses),
               cudaGetLastError()));
   }
   return PF_OK;

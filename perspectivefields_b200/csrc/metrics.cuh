@@ -97,8 +97,10 @@ __global__ void __launch_bounds__(kMetThreads) encode_fields_kernel(EncodeArgs a
 // ------------------------------------------------------------------------------------------------------ cross-entropy
 // F.cross_entropy(logits, labels, reduction="mean", ignore_index) of both classification heads in one launch.  One thread owns
 // 4 consecutive pixels and walks the C channel planes (stride H*W) with 16-byte streaming loads, keeping an online max and sum
-// of exp in fp32 and picking up the target logit in the same pass: every logit is read from HBM once.  A label that is neither
-// the ignore value nor in [0, C) contributes NaN (never an out-of-bounds read).
+// of exp in fp32 and picking up the target logit in the same pass: every logit is read from HBM once.  A logit of -inf adds
+// nothing (exp(-inf) = 0, also while the running max is still -inf).  The pixel's loss is (max - target) + log(sum): the
+// difference is exact for the argmax target, so a confident pixel keeps log(sum)'s precision whatever the logits' magnitude.
+// A label that is neither the ignore value nor in [0, C) contributes NaN (never an out-of-bounds read).
 constexpr int kCePix = 4, kCeUnroll = 8;
 struct CeHead {
   const float* logits;       // [n, C, HW], 16-byte aligned
@@ -137,7 +139,7 @@ __global__ void __launch_bounds__(kMetThreads) cross_entropy_kernel(CeHead g, Ce
         const float e[kCePix] = {v[j].x, v[j].y, v[j].z, v[j].w};
 #pragma unroll
         for (int k = 0; k < kCePix; ++k) {
-          const float t = __expf(-fabsf(e[k] - m[k]));   // exp(min - max); 0 while m is -inf
+          const float t = e[k] == -INFINITY ? 0.f : __expf(-fabsf(e[k] - m[k]));   // exp(min - max); 0 while m is -inf
           s[k] = e[k] > m[k] ? s[k] * t + 1.f : s[k] + t;
           m[k] = fmaxf(m[k], e[k]);
           if (lab[k] == c0 + j) xt[k] = e[k];
@@ -148,7 +150,7 @@ __global__ void __launch_bounds__(kMetThreads) cross_entropy_kernel(CeHead g, Ce
     for (int k = 0; k < kCePix; ++k) {
       if (lab[k] == h.ignore) continue;
       const bool ok = lab[k] >= 0 && lab[k] < h.C;
-      sum += ok ? (double)(m[k] + logf(s[k]) - xt[k]) : (double)NAN;
+      sum += ok ? (double)((m[k] - xt[k]) + logf(s[k])) : (double)NAN;
       ++cnt;
     }
   }
